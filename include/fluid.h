@@ -205,7 +205,7 @@ int fluid_write(fluid_t* h, int field, const float* host, size_t n_floats);
 int fluid_pressure_solve_host(fluid_t* h, const float* div_host, float* pressure_host_inout,
                               int iters);
 
-/* The consumer on the far side of the path ("next" row of SURVEY §8f, partially built):
+/* The consumer on the far side of the path ("next" row of SURVEY §8f):
  * render(target) of S:1296-1317 with config.BLOOM = config.SUNRAYS = false and TRANSPARENT = false —
  * drawColor(BACK_COLOR) (S:1319-1323) then drawDisplay (S:1331-1348, displayShaderSource S:549-612,
  * SHADING keyword when `shading` != 0) blended ONE / ONE_MINUS_SRC_ALPHA.  Writes width*height RGBA
@@ -236,6 +236,25 @@ typedef struct fluid_postfx {
 int fluid_render_postfx(fluid_t* h, int width, int height, const fluid_postfx* fx, const float* dither_rgb,
                         int dw, int dh, float back_r, float back_g, float back_b, float* host_rgba,
                         size_t n_floats, float* host_bloom, float* host_sunrays);
+
+/* Any of the eight display variants: `keywords` is the set updateKeywords (S:1160-1166) builds from
+ * config.SHADING / BLOOM / SUNRAYS, as FLUID_DISPLAY_* bits.  render() runs applyBloom only with BLOOM and
+ * applySunrays + blur only with SUNRAYS (S:1297-1302), and binds the bloom, dithering and sunrays
+ * textures only for the keywords that are on (S:1339-1346).  The background follows FLUID_BACKGROUND.
+ *  - Without BLOOM and SUNRAYS this is fluid_render(…, keywords & FLUID_DISPLAY_SHADING, …): slab bands
+ *    and half storage work, and fx / dither_rgb may be NULL.
+ *  - With BLOOM or SUNRAYS the handle must be single-GPU with fp32 storage (FLUID_ERR_INVALID
+ *    otherwise), fx is required, and dither_rgb only with BLOOM.  host_bloom / host_sunrays (as for
+ *    fluid_render_postfx, may be NULL) are written only when their keyword is on.
+ * The bloom FBO + pyramid, the sunrays FBOs and the dithering texture live in the handle: made on first
+ * use, made again only when a size changes (FLUID_ERR_NOMEM if that fails; the handle stays usable), and
+ * freed by fluid_destroy.  fluid_render_postfx is this call with all three keywords. */
+#define FLUID_DISPLAY_SHADING 0x1u
+#define FLUID_DISPLAY_BLOOM 0x2u
+#define FLUID_DISPLAY_SUNRAYS 0x4u
+int fluid_render_keywords(fluid_t* h, int width, int height, uint32_t keywords, const fluid_postfx* fx,
+                          const float* dither_rgb, int dw, int dh, float back_r, float back_g, float back_b,
+                          float* host_rgba, size_t n_floats, float* host_bloom, float* host_sunrays);
 
 int fluid_sync(fluid_t* h);
 int fluid_timing_last(fluid_t* h, fluid_timing* out);

@@ -22,7 +22,7 @@ SYMBOLS = [
     "fluid_pass_divergence", "fluid_pass_clear_pressure", "fluid_pass_jacobi",
     "fluid_pass_pressure_solve", "fluid_pass_gradient_subtract", "fluid_pass_advect_velocity",
     "fluid_pass_advect_dye", "fluid_pass_curl_vorticity_divergence", "fluid_field_elems",
-    "fluid_field_dims", "fluid_read", "fluid_write", "fluid_pressure_solve_host", "fluid_render", "fluid_render_band", "fluid_render_postfx", "fluid_sync",
+    "fluid_field_dims", "fluid_read", "fluid_write", "fluid_pressure_solve_host", "fluid_render", "fluid_render_band", "fluid_render_postfx", "fluid_render_keywords", "fluid_sync",
     "fluid_timing_last", "fluid_host_alloc", "fluid_host_free", "fluid_mark", "fluid_elapsed_ms", "fluid_launch_count", "fluid_device_ptr",
     "fluid_last_error",
 ]
@@ -35,6 +35,8 @@ FIELD = {"velocity": 0, "dye": 1, "pressure": 2, "divergence": 3, "curl": 4}
 PARAM = {"DENSITY_DISSIPATION": 0, "VELOCITY_DISSIPATION": 1, "PRESSURE": 2,
          "PRESSURE_ITERATIONS": 3, "CURL": 4, "SPLAT_RADIUS": 5, "ASPECT": 6, "JACOBI_BLOCK": 7, "BACKGROUND": 8}
 FLAG_UNFUSED, FLAG_NO_GRAPH, FLAG_NAIVE_JACOBI, FLAG_TILED_PASSES, FLAG_HALF_STORAGE = 0x1, 0x2, 0x4, 0x8, 0x10
+# display keywords of render() (updateKeywords, S:1160-1166): FLUID_DISPLAY_* of include/fluid.h
+DISPLAY_SHADING, DISPLAY_BLOOM, DISPLAY_SUNRAYS = 0x1, 0x2, 0x4
 STAT = {"launches": 0, "jacobi_launches": 1, "halo_launches": 2, "halo_exchanges": 3,
         "graph_captures": 4, "graph_launches": 5, "halo_transport_p2p": 6}
 
@@ -118,6 +120,7 @@ def lib():
     L.fluid_render.argtypes = [vp, i, i, i, f, f, f, vp, sz]
     L.fluid_render_band.argtypes = [vp, i, C.POINTER(i), C.POINTER(i)]
     L.fluid_render_postfx.argtypes = [vp, i, i, C.POINTER(PostFX), vp, i, i, f, f, f, vp, sz, vp, vp]
+    L.fluid_render_keywords.argtypes = [vp, i, i, C.c_uint32, C.POINTER(PostFX), vp, i, i, f, f, f, vp, sz, vp, vp]
     L.fluid_sync.argtypes = [vp]
     L.fluid_host_alloc.argtypes = [sz]; L.fluid_host_alloc.restype = vp
     L.fluid_host_free.argtypes = [vp]; L.fluid_host_free.restype = None

@@ -120,6 +120,16 @@ struct fluid {
     uint64_t graph_launches = 0, graph_captures = 0;
     float4* frame = nullptr;         // render target of fluid_render (w x h RGBA fp32), grown on demand
     size_t frame_cells = 0;
+    // post-FX targets of render() (initBloomFramebuffers / initSunraysFramebuffers, S:1012-1043): made on
+    // first use, made again only when a size changes, kept across frames like the reference's FBOs
+    struct PostFxTargets {
+        float4* bloom = nullptr;     // the bloom FBO, then its `levels` pyramid levels, in one allocation
+        int bw = 0, bh = 0, levels = 0;
+        float* sun = nullptr;        // sunrays, then sunraysTemp (sw x sh each)
+        int sw = 0, sh = 0;
+        float* dither = nullptr;     // dw x dh RGB dithering texture, uploaded every BLOOM frame
+        int dw = 0, dh = 0;
+    } pfx;
     bool slab() const { return world > 1; }
     int lrows() const { return row1 - row0 + 2 * G; }
     int ldrows() const { return drow1 - drow0 + 2 * Gd; }
@@ -941,6 +951,7 @@ void fluid_destroy(fluid_t* h) {
     cudaFree(h->dt_dev);
     cudaFree(h->scratch);
     cudaFree(h->frame);
+    cudaFree(h->pfx.bloom); cudaFree(h->pfx.sun); cudaFree(h->pfx.dither);
     if (h->comm) { ncdl::api().CommDestroy(h->comm); h->comm = nullptr; }
     for (auto& e : h->mark) if (e) cudaEventDestroy(e);
     for (auto& e : h->tev) if (e) cudaEventDestroy(e);
@@ -1684,6 +1695,16 @@ int fluid_render_band(fluid_t* h, int height, int* y0, int* y1) {
     return FLUID_OK;
 }
 
+// grows the render target to at least `cells` RGBA texels
+static int need_frame(fluid_t* h, size_t cells) {
+    if (cells <= h->frame_cells) return FLUID_OK;
+    CU(cudaStreamSynchronize(h->stream));
+    cudaFree(h->frame); h->frame = nullptr; h->frame_cells = 0;
+    CU(cudaMalloc((void**)&h->frame, cells * sizeof(float4)));
+    h->frame_cells = cells;
+    return FLUID_OK;
+}
+
 // render(target) of S:1296-1317 for config.BLOOM = config.SUNRAYS = false: the background selected by
 // FLUID_BACKGROUND (colour / checkerboard / none), then the display shader (optionally SHADING) blended over it.
 int fluid_render(fluid_t* h, int width, int height, int shading, float back_r, float back_g,
@@ -1694,12 +1715,7 @@ int fluid_render(fluid_t* h, int width, int height, int shading, float back_r, f
     const size_t cells = (size_t)width * (y1 - y0);
     if (n_floats != 4 * cells) return fail(h, FLUID_ERR_INVALID, "render target band has %zu floats, caller passed %zu", 4 * cells, n_floats);
     if (cells == 0) return FLUID_OK;
-    if (cells > h->frame_cells) {
-        CU(cudaStreamSynchronize(h->stream));
-        cudaFree(h->frame); h->frame = nullptr; h->frame_cells = 0;
-        CU(cudaMalloc((void**)&h->frame, cells * sizeof(float4)));
-        h->frame_cells = cells;
-    }
+    if (int rc = need_frame(h, cells)) return rc;
     if (h->slab()) {
         // the band's display + shading taps reach ceil(Hd / height) + 2 dye rows beyond the owned ones:
         // refresh that many ghost rows (the ghost rows of dye.read are stale after advection)
@@ -1730,92 +1746,169 @@ int fluid_render(fluid_t* h, int width, int height, int shading, float back_r, f
 }
 
 
-// render(null) of S:1296-1317 with config.SHADING = BLOOM = SUNRAYS = true (the reference's desktop
-// defaults S:70-84), TRANSPARENT = false: applyBloom (S:1350-1394), applySunrays + blur(…, 1)
-// (S:1396-1419; the mask is drawn into dye.write exactly like S:1300), drawColor, drawDisplay.
+// (Re)allocates one post-FX target once the stream has drained.  Out of memory leaves it empty, so the
+// handle stays usable and the next call tries again.
+static int remake_target(fluid_t* h, void** p, size_t bytes, const char* what) {
+    CU(cudaStreamSynchronize(h->stream));
+    cudaFree(*p); *p = nullptr;
+    if (cudaMalloc(p, bytes) != cudaSuccess) {
+        cudaGetLastError();                      // not sticky: keep it out of the next launch check
+        *p = nullptr;
+        return fail(h, FLUID_ERR_NOMEM, "out of device memory for %s (%zu bytes)", what, bytes);
+    }
+    return FLUID_OK;
+}
+
+// The bloom FBO and its pyramid (initBloomFramebuffers S:1012-1032), cleared like createFBO (S:1059).
+// A pyramid shorter than 2 levels leaves the FBO as cleared (applyBloom returns early, S:1351-1352).
+static int need_bloom_targets(fluid_t* h, int bw, int bh, int levels) {
+    auto& t = h->pfx;
+    if (t.bloom && t.bw == bw && t.bh == bh && t.levels == levels) return FLUID_OK;
+    size_t n = (size_t)bw * bh;
+    for (int i = 0; i < levels; ++i) n += (size_t)(bw >> (i + 1)) * (bh >> (i + 1));
+    t.bw = t.bh = t.levels = 0;
+    if (int rc = remake_target(h, (void**)&t.bloom, n * sizeof(float4), "the bloom FBO and pyramid")) return rc;
+    t.bw = bw; t.bh = bh; t.levels = levels;
+    fill_alpha_kernel<<<(unsigned)((n + 255) / 256), 256, 0, h->stream>>>(t.bloom, n);
+    return check_launch(h, "fill_alpha_kernel");
+}
+
+// sunrays + sunraysTemp (initSunraysFramebuffers S:1034-1043): one-channel FBOs, cleared to 0
+static int need_sunrays_targets(fluid_t* h, int sw, int sh) {
+    auto& t = h->pfx;
+    if (t.sun && t.sw == sw && t.sh == sh) return FLUID_OK;
+    const size_t n = 2 * (size_t)sw * sh;
+    t.sw = t.sh = 0;
+    if (int rc = remake_target(h, (void**)&t.sun, n * sizeof(float), "the sunrays FBOs")) return rc;
+    t.sw = sw; t.sh = sh;
+    CU(cudaMemsetAsync(t.sun, 0, n * sizeof(float), h->stream));
+    return FLUID_OK;
+}
+
+static int need_dither_target(fluid_t* h, int dw, int dh) {
+    auto& t = h->pfx;
+    if (t.dither && t.dw == dw && t.dh == dh) return FLUID_OK;
+    t.dw = t.dh = 0;
+    if (int rc = remake_target(h, (void**)&t.dither, (size_t)dw * dh * 3 * sizeof(float), "the dithering texture")) return rc;
+    t.dw = dw; t.dh = dh;
+    return FLUID_OK;
+}
+
+using DisplayFullKernel = void (*)(const float4*, int, int, const float4*, int, int, const float*, int, int,
+                                   const float*, int, int, float4*, int, int, float, float, float, int, float, float4);
+// indexed by the FLUID_DISPLAY_* mask; the sets without BLOOM or SUNRAYS draw with display_kernel
+static const DisplayFullKernel kDisplayFull[8] = {
+    nullptr, nullptr,
+    display_full_kernel<false, true, false>, display_full_kernel<true, true, false>,
+    display_full_kernel<false, false, true>, display_full_kernel<true, false, true>,
+    display_full_kernel<false, true, true>, display_full_kernel<true, true, true>,
+};
+
+// render(null) of S:1296-1317 for a keyword set with BLOOM or SUNRAYS (single GPU, fp32 storage): applyBloom
+// (S:1350-1394) when BLOOM is on, applySunrays + blur(…, 1) (S:1396-1419; the mask is drawn into dye.write
+// exactly like S:1300) when SUNRAYS is on, then the background and drawDisplay with the chosen keywords.
 // FBO sizes follow initBloomFramebuffers / initSunraysFramebuffers (S:1012-1043).
-int fluid_render_postfx(fluid_t* h, int width, int height, const fluid_postfx* fx, const float* dither_rgb,
-                        int dw, int dh, float back_r, float back_g, float back_b, float* host_rgba,
-                        size_t n_floats, float* host_bloom, float* host_sunrays) {
-    if (!h || !fx || !dither_rgb || !host_rgba || width < 1 || height < 1 || dw < 1 || dh < 1)
+static int render_postfx(fluid_t* h, const char* what, int width, int height, uint32_t keywords,
+                         const fluid_postfx* fx, const float* dither_rgb, int dw, int dh, float back_r,
+                         float back_g, float back_b, float* host_rgba, size_t n_floats, float* host_bloom,
+                         float* host_sunrays) {
+    const bool bloom_on = keywords & FLUID_DISPLAY_BLOOM, sun_on = keywords & FLUID_DISPLAY_SUNRAYS;
+    if (!h || !fx || !host_rgba || width < 1 || height < 1 || (bloom_on && (!dither_rgb || dw < 1 || dh < 1)))
         return fail(h, FLUID_ERR_INVALID, "bad argument");
-    if (h->slab()) return not_on_slab(h, "fluid_render_postfx");
-    if (h->half) return fail(h, FLUID_ERR_INVALID, "fluid_render_postfx is not built for FLUID_FLAG_HALF_STORAGE (the reference's bloom / sunrays FBOs are fp16 too)");
+    if (h->slab()) return not_on_slab(h, what);
+    if (h->half) return fail(h, FLUID_ERR_INVALID, "%s is not built for FLUID_FLAG_HALF_STORAGE (the reference's bloom / sunrays FBOs are fp16 too)", what);
     const size_t cells = (size_t)width * height;
     if (n_floats != 4 * cells) return fail(h, FLUID_ERR_INVALID, "render target has %zu floats, caller passed %zu", 4 * cells, n_floats);
-    int bw, bh, sw, sh;
-    fluid_get_resolution(fx->bloom_resolution, width, height, &bw, &bh);
-    fluid_get_resolution(fx->sunrays_resolution, width, height, &sw, &sh);
+    int bw = 1, bh = 1, sw = 1, sh = 1, levels = 0;
+    if (bloom_on) fluid_get_resolution(fx->bloom_resolution, width, height, &bw, &bh);
+    if (sun_on) fluid_get_resolution(fx->sunrays_resolution, width, height, &sw, &sh);
     if (bw < 1 || bh < 1 || sw < 1 || sh < 1) return fail(h, FLUID_ERR_INVALID, "bad post-FX resolution");
-    std::vector<void*> tmp;
-    auto dalloc = [&](size_t bytes) -> void* { void* p = nullptr; if (cudaMalloc(&p, bytes) != cudaSuccess) return nullptr; tmp.push_back(p); return p; };
-    auto cleanup = [&]() { cudaStreamSynchronize(h->stream); for (void* p : tmp) cudaFree(p); };
-    int rc = FLUID_OK;
-    auto body = [&]() -> int {
-        if (cells > h->frame_cells) {
-            CU(cudaStreamSynchronize(h->stream));
-            cudaFree(h->frame); h->frame = nullptr; h->frame_cells = 0;
-            CU(cudaMalloc((void**)&h->frame, cells * sizeof(float4)));
-            h->frame_cells = cells;
-        }
-        const int Wd = h->cfg.dye_w, Hd = h->cfg.dye_h;
-        dim3 b(32, 8);
-        float4* bloom = (float4*)dalloc((size_t)bw * bh * sizeof(float4));
-        float* sun = (float*)dalloc((size_t)sw * sh * sizeof(float));
-        float* sun2 = (float*)dalloc((size_t)sw * sh * sizeof(float));
-        float* dith = (float*)dalloc((size_t)dw * dh * 3 * sizeof(float));
-        if (!bloom || !sun || !sun2 || !dith) return fail(h, FLUID_ERR_NOMEM, "out of device memory for the post-FX targets");
-        CU(cudaMemcpyAsync(dith, dither_rgb, (size_t)dw * dh * 3 * sizeof(float), cudaMemcpyHostToDevice, h->stream));
-        fill_alpha_kernel<<<(unsigned)(((size_t)bw * bh + 255) / 256), 256, 0, h->stream>>>(bloom, (size_t)bw * bh);   // createFBO clear
-        // ---- applyBloom(dye.read, bloom) ----------------------------------------------------------
+    if (bloom_on)
+        while (levels < fx->bloom_iterations && (bw >> (levels + 1)) >= 2 && (bh >> (levels + 1)) >= 2) ++levels;
+    int rc = need_frame(h, cells); if (rc) return rc;
+    if (bloom_on) {
+        if ((rc = need_bloom_targets(h, bw, bh, levels)) || (rc = need_dither_target(h, dw, dh))) return rc;
+        CU(cudaMemcpyAsync(h->pfx.dither, dither_rgb, (size_t)dw * dh * 3 * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+    }
+    if (sun_on && (rc = need_sunrays_targets(h, sw, sh))) return rc;
+    const int Wd = h->cfg.dye_w, Hd = h->cfg.dye_h;
+    float4* bloom = h->pfx.bloom;
+    float *sun = h->pfx.sun, *sun2 = sun ? sun + (size_t)sw * sh : nullptr;
+    dim3 b(32, 8);
+    int nk = 0;
+    // ---- applyBloom(dye.read, bloom) ----------------------------------------------------------------
+    if (bloom_on && levels >= 2) {
         struct Lv { float4* p; int w, h; };
         std::vector<Lv> pyr;
-        for (int i = 0; i < fx->bloom_iterations; ++i) {
+        float4* p = bloom + (size_t)bw * bh;
+        for (int i = 0; i < levels; ++i) {
             const int pw = bw >> (i + 1), ph = bh >> (i + 1);
-            if (pw < 2 || ph < 2) break;
-            float4* p = (float4*)dalloc((size_t)pw * ph * sizeof(float4));
-            if (!p) return fail(h, FLUID_ERR_NOMEM, "out of device memory for the bloom pyramid");
             pyr.push_back({p, pw, ph});
+            p += (size_t)pw * ph;
         }
-        int nk = 1;
-        if (pyr.size() >= 2) {
-            const double knee = fx->bloom_threshold * fx->bloom_soft_knee + 0.0001;
-            bloom_prefilter_kernel<<<grid2d(bw, bh, b), b, 0, h->stream>>>(
-                (const float4*)h->dye.read, Wd, Hd, bloom, bw, bh, (float)(fx->bloom_threshold - knee),
-                (float)(knee * 2), (float)(0.25 / knee), (float)fx->bloom_threshold);
-            ++nk;
-            Lv last{bloom, bw, bh};
-            for (auto& d : pyr) {
-                box4_kernel<<<grid2d(d.w, d.h, b), b, 0, h->stream>>>(last.p, last.w, last.h, d.p, d.w, d.h, 1.0f, 0);
-                last = d; ++nk;
-            }
-            for (int i = (int)pyr.size() - 2; i >= 0; --i) {
-                box4_kernel<<<grid2d(pyr[i].w, pyr[i].h, b), b, 0, h->stream>>>(last.p, last.w, last.h, pyr[i].p, pyr[i].w, pyr[i].h, 1.0f, 1);
-                last = pyr[i]; ++nk;
-            }
-            box4_kernel<<<grid2d(bw, bh, b), b, 0, h->stream>>>(last.p, last.w, last.h, bloom, bw, bh, (float)fx->bloom_intensity, 0);
-            ++nk;
+        const double knee = fx->bloom_threshold * fx->bloom_soft_knee + 0.0001;
+        bloom_prefilter_kernel<<<grid2d(bw, bh, b), b, 0, h->stream>>>(
+            (const float4*)h->dye.read, Wd, Hd, bloom, bw, bh, (float)(fx->bloom_threshold - knee),
+            (float)(knee * 2), (float)(0.25 / knee), (float)fx->bloom_threshold);
+        ++nk;
+        Lv last{bloom, bw, bh};
+        for (auto& d : pyr) {
+            box4_kernel<<<grid2d(d.w, d.h, b), b, 0, h->stream>>>(last.p, last.w, last.h, d.p, d.w, d.h, 1.0f, 0);
+            last = d; ++nk;
         }
-        // ---- applySunrays(dye.read, dye.write, sunrays); blur(sunrays, sunraysTemp, 1) ---------------
+        for (int i = (int)pyr.size() - 2; i >= 0; --i) {
+            box4_kernel<<<grid2d(pyr[i].w, pyr[i].h, b), b, 0, h->stream>>>(last.p, last.w, last.h, pyr[i].p, pyr[i].w, pyr[i].h, 1.0f, 1);
+            last = pyr[i]; ++nk;
+        }
+        box4_kernel<<<grid2d(bw, bh, b), b, 0, h->stream>>>(last.p, last.w, last.h, bloom, bw, bh, (float)fx->bloom_intensity, 0);
+        ++nk;
+    }
+    // ---- applySunrays(dye.read, dye.write, sunrays); blur(sunrays, sunraysTemp, 1) -------------------
+    if (sun_on) {
         sunrays_mask_kernel<<<grid2d(Wd, Hd, b), b, 0, h->stream>>>((const float4*)h->dye.read, (float4*)h->dye.write, Wd, Hd);
         sunrays_kernel<<<grid2d(sw, sh, b), b, 0, h->stream>>>((const float4*)h->dye.write, Wd, Hd, sun, sw, sh, (float)fx->sunrays_weight);
         blur3_kernel<<<grid2d(sw, sh, b), b, 0, h->stream>>>(sun, sun2, sw, sh, (float)(1.0 / (double)sw), 0.0f);
         blur3_kernel<<<grid2d(sw, sh, b), b, 0, h->stream>>>(sun2, sun, sw, sh, 0.0f, (float)(1.0 / (double)sh));
-        // ---- drawColor + drawDisplay ---------------------------------------------------------------------
-        display_full_kernel<<<grid2d(width, height, b), b, 0, h->stream>>>(
-            (const float4*)h->dye.read, Wd, Hd, bloom, bw, bh, sun, sw, sh, dith, dw, dh, h->frame, width, height,
-            back_r, back_g, back_b, h->background, h->cfg.aspect,
-            make_float4((float)(1.0 / (double)width), (float)(1.0 / (double)height), (float)((double)width / (double)dw), (float)((double)height / (double)dh)));
-        int r = check_launch(h, "post-FX kernels", nk + 5); if (r) return r;
-        CU(cudaMemcpyAsync(host_rgba, h->frame, cells * sizeof(float4), cudaMemcpyDeviceToHost, h->stream));
-        if (host_bloom) CU(cudaMemcpyAsync(host_bloom, bloom, (size_t)bw * bh * sizeof(float4), cudaMemcpyDeviceToHost, h->stream));
-        if (host_sunrays) CU(cudaMemcpyAsync(host_sunrays, sun, (size_t)sw * sh * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-        CU(cudaStreamSynchronize(h->stream));
-        return FLUID_OK;
-    };
-    rc = body();
-    cleanup();
-    return rc;
+        nk += 4;
+    }
+    // ---- background + drawDisplay -----------------------------------------------------------------------
+    kDisplayFull[keywords]<<<grid2d(width, height, b), b, 0, h->stream>>>(
+        (const float4*)h->dye.read, Wd, Hd, bloom_on ? bloom : nullptr, bw, bh, sun_on ? sun : nullptr, sw, sh,
+        bloom_on ? h->pfx.dither : nullptr, dw, dh, h->frame, width, height, back_r, back_g, back_b, h->background,
+        h->cfg.aspect,
+        make_float4((float)(1.0 / (double)width), (float)(1.0 / (double)height),
+                    bloom_on ? (float)((double)width / (double)dw) : 0.0f, bloom_on ? (float)((double)height / (double)dh) : 0.0f));
+    ++nk;
+    if ((rc = check_launch(h, "post-FX kernels", nk))) return rc;
+    CU(cudaMemcpyAsync(host_rgba, h->frame, cells * sizeof(float4), cudaMemcpyDeviceToHost, h->stream));
+    if (bloom_on && host_bloom) CU(cudaMemcpyAsync(host_bloom, bloom, (size_t)bw * bh * sizeof(float4), cudaMemcpyDeviceToHost, h->stream));
+    if (sun_on && host_sunrays) CU(cudaMemcpyAsync(host_sunrays, sun, (size_t)sw * sh * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+    CU(cudaStreamSynchronize(h->stream));
+    return FLUID_OK;
+}
+
+// render() with the display keywords of updateKeywords (S:1160-1166): without BLOOM and SUNRAYS this is
+// fluid_render (slab bands, half storage), with either of them render_postfx.
+int fluid_render_keywords(fluid_t* h, int width, int height, uint32_t keywords, const fluid_postfx* fx,
+                          const float* dither_rgb, int dw, int dh, float back_r, float back_g, float back_b,
+                          float* host_rgba, size_t n_floats, float* host_bloom, float* host_sunrays) {
+    if (!h) return FLUID_ERR_INVALID;
+    if (keywords & ~(uint32_t)(FLUID_DISPLAY_SHADING | FLUID_DISPLAY_BLOOM | FLUID_DISPLAY_SUNRAYS))
+        return fail(h, FLUID_ERR_INVALID, "unknown display keyword bits 0x%x", keywords);
+    if (!(keywords & (FLUID_DISPLAY_BLOOM | FLUID_DISPLAY_SUNRAYS)))
+        return fluid_render(h, width, height, (keywords & FLUID_DISPLAY_SHADING) ? 1 : 0, back_r, back_g, back_b,
+                            host_rgba, n_floats);
+    return render_postfx(h, "fluid_render_keywords", width, height, keywords, fx, dither_rgb, dw, dh, back_r,
+                         back_g, back_b, host_rgba, n_floats, host_bloom, host_sunrays);
+}
+
+// render(null) with the reference's desktop defaults SHADING = BLOOM = SUNRAYS = true (S:70-84)
+int fluid_render_postfx(fluid_t* h, int width, int height, const fluid_postfx* fx, const float* dither_rgb,
+                        int dw, int dh, float back_r, float back_g, float back_b, float* host_rgba,
+                        size_t n_floats, float* host_bloom, float* host_sunrays) {
+    return render_postfx(h, "fluid_render_postfx", width, height,
+                         FLUID_DISPLAY_SHADING | FLUID_DISPLAY_BLOOM | FLUID_DISPLAY_SUNRAYS, fx, dither_rgb, dw,
+                         dh, back_r, back_g, back_b, host_rgba, n_floats, host_bloom, host_sunrays);
 }
 
 void* fluid_host_alloc(size_t bytes) {

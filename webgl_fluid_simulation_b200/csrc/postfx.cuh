@@ -1,6 +1,6 @@
 // postfx.cuh — the display-side post-FX of render() (SURVEY §8f rank 1, second half): bloom
 // (applyBloom S:1350-1394; shaders S:614-674) and sunrays (applySunrays + blur S:1396-1419; shaders
-// S:461-494, S:676-724) and the full display shader with SHADING + BLOOM + SUNRAYS (S:549-612).
+// S:461-494, S:676-724) and the display shader for every keyword set with BLOOM or SUNRAYS (S:549-612).
 //
 // Every kernel is one reference blit: one thread per target texel, sources fetched through the
 // GL_LINEAR formula of passes.cuh (linear_fetch4).  Arithmetic order follows the GLSL; with the
@@ -124,7 +124,11 @@ __global__ void __launch_bounds__(256) blur3_kernel(const float* __restrict__ sr
     dst[(size_t)j * w + i] = sum;
 }
 
-// displayShaderSource S:549-612 with SHADING + BLOOM + SUNRAYS over drawColor, premultiplied blend
+// displayShaderSource S:549-612 compiled with the keywords updateKeywords picks (S:1160-1166), over
+// the background of render(), premultiplied blend.  One instantiation per keyword set with BLOOM or
+// SUNRAYS; the sets with neither use display_kernel (passes.cuh).  The inputs of a keyword that is
+// off are never read (pass nullptr).
+template <bool SHADING, bool BLOOM, bool SUNRAYS>
 __global__ void __launch_bounds__(256) display_full_kernel(const float4* __restrict__ dye, int Wd, int Hd,
                                                            const float4* __restrict__ bloom, int bw, int bh,
                                                            const float* __restrict__ sun, int sw, int sh,
@@ -137,26 +141,40 @@ __global__ void __launch_bounds__(256) display_full_kernel(const float4* __restr
     const float dsx = ts.z, dsy = ts.w;
     const float uvx = ((float)i + 0.5f) / (float)w, uvy = ((float)j + 0.5f) / (float)h;
     const float4 c = linear_fetch4(dye, Wd, Hd, uvx, uvy);
-    const float4 lc = linear_fetch4(dye, Wd, Hd, uvx - tsx, uvy), rc = linear_fetch4(dye, Wd, Hd, uvx + tsx, uvy);
-    const float4 tc = linear_fetch4(dye, Wd, Hd, uvx, uvy + tsy), bc = linear_fetch4(dye, Wd, Hd, uvx, uvy - tsy);
-    const float dx = len3(rc) - len3(lc), dy = len3(tc) - len3(bc);
-    const float nz = sqrtf(tsx * tsx + tsy * tsy);
-    const float nl = sqrtf((dx * dx + dy * dy) + nz * nz);
-    const float d = ((dx / nl) * 0.0f + (dy / nl) * 0.0f) + (nz / nl) * 1.0f;
-    const float diffuse = fminf(fmaxf(d + 0.7f, 0.7f), 1.0f);
-    const float4 bl = linear_fetch4(bloom, bw, bh, uvx, uvy);
-    const float s = linear_fetch1(sun, sw, sh, uvx, uvy);
-    const float noise = linear_fetch_rgb_r_repeat(dither, dw, dh, uvx * dsx, uvy * dsy) * 2.0f - 1.0f;
-    const float cin[3] = {c.x, c.y, c.z}, bin[3] = {bl.x, bl.y, bl.z};
-    float cc[3];
+    float cc[3] = {c.x, c.y, c.z};
+    if constexpr (SHADING) {
+        const float4 lc = linear_fetch4(dye, Wd, Hd, uvx - tsx, uvy), rc = linear_fetch4(dye, Wd, Hd, uvx + tsx, uvy);
+        const float4 tc = linear_fetch4(dye, Wd, Hd, uvx, uvy + tsy), bc = linear_fetch4(dye, Wd, Hd, uvx, uvy - tsy);
+        const float dx = len3(rc) - len3(lc), dy = len3(tc) - len3(bc);
+        const float nz = sqrtf(tsx * tsx + tsy * tsy);
+        const float nl = sqrtf((dx * dx + dy * dy) + nz * nz);
+        const float d = ((dx / nl) * 0.0f + (dy / nl) * 0.0f) + (nz / nl) * 1.0f;
+        const float diffuse = fminf(fmaxf(d + 0.7f, 0.7f), 1.0f);
 #pragma unroll
-    for (int k = 0; k < 3; ++k) {
-        const float ck = (cin[k] * diffuse) * s;
-        float bk = bin[k] * s;
-        bk = bk + noise / 255.0f;
-        bk = fmaxf(bk, 0.0f);
-        bk = fmaxf(1.055f * powf(bk, 0.416666667f) - 0.055f, 0.0f);     // linearToGamma S:565-568
-        cc[k] = ck + bk;
+        for (int k = 0; k < 3; ++k) cc[k] = cc[k] * diffuse;
+    }
+    float bl[3] = {0.0f, 0.0f, 0.0f};
+    if constexpr (BLOOM) {
+        const float4 b = linear_fetch4(bloom, bw, bh, uvx, uvy);
+        bl[0] = b.x; bl[1] = b.y; bl[2] = b.z;
+    }
+    if constexpr (SUNRAYS) {
+        const float s = linear_fetch1(sun, sw, sh, uvx, uvy);
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            cc[k] = cc[k] * s;
+            if constexpr (BLOOM) bl[k] = bl[k] * s;
+        }
+    }
+    if constexpr (BLOOM) {
+        const float noise = linear_fetch_rgb_r_repeat(dither, dw, dh, uvx * dsx, uvy * dsy) * 2.0f - 1.0f;
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            float bk = bl[k] + noise / 255.0f;
+            bk = fmaxf(bk, 0.0f);
+            bk = fmaxf(1.055f * powf(bk, 0.416666667f) - 0.055f, 0.0f);     // linearToGamma S:565-568
+            cc[k] = cc[k] + bk;
+        }
     }
     const float a = fmaxf(cc[0], fmaxf(cc[1], cc[2]));
     out[(size_t)j * w + i] = blend_over_background(cc[0], cc[1], cc[2], a, bg_mode, br_, bg_, bb_, aspect, uvx, uvy);

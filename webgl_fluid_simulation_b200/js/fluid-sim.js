@@ -26,8 +26,10 @@ const native = require('../napi/fluid.node');
 const FIELD = { velocity: 0, dye: 1, pressure: 2, divergence: 3, curl: 4 };
 const PARAM = {
     DENSITY_DISSIPATION: 0, VELOCITY_DISSIPATION: 1, PRESSURE: 2, PRESSURE_ITERATIONS: 3,
-    CURL: 4, SPLAT_RADIUS: 5, ASPECT: 6, JACOBI_BLOCK: 7,
+    CURL: 4, SPLAT_RADIUS: 5, ASPECT: 6, JACOBI_BLOCK: 7, BACKGROUND: 8,
 };
+// display keywords of render() (updateKeywords, S:1160-1166): FLUID_DISPLAY_* of include/fluid.h
+const DISPLAY = { SHADING: 0x1, BLOOM: 0x2, SUNRAYS: 0x4 };
 const FLAG = { UNFUSED: 0x1, NO_GRAPH: 0x2, NAIVE_JACOBI: 0x4, TILED_PASSES: 0x8, HALF_STORAGE: 0x10 };
 const STAT = { launches: 0, jacobiLaunches: 1, haloLaunches: 2, haloExchanges: 3, graphCaptures: 4, graphLaunches: 5, haloTransportP2P: 6 };
 
@@ -70,7 +72,7 @@ function wrap (value, min, max) {                               // S:1599-1603
 
 class FluidSimulation {
     constructor (config = {}, canvas = { width: 1024, height: 1024 }, options = {}) {
-        this.config = Object.assign({                           // S:59-69, S:73 (simulation keys)
+        this.config = Object.assign({                           // S:59-85
             SIM_RESOLUTION: 128,
             DYE_RESOLUTION: 1024,
             DENSITY_DISSIPATION: 1,
@@ -85,7 +87,18 @@ class FluidSimulation {
             COLOR_UPDATE_SPEED: 10,
             PAUSED: false,
             BACK_COLOR: { r: 0, g: 0, b: 0 },
+            TRANSPARENT: false,
+            BLOOM: false,           // reference default is true; needs `sim.dithering` (the 64x64 RGB texture), see render()
+            BLOOM_ITERATIONS: 8,
+            BLOOM_RESOLUTION: 256,
+            BLOOM_INTENSITY: 0.8,
+            BLOOM_THRESHOLD: 0.6,
+            BLOOM_SOFT_KNEE: 0.7,
+            SUNRAYS: false,         // reference default is true
+            SUNRAYS_RESOLUTION: 196,
+            SUNRAYS_WEIGHT: 1.0,
         }, config);
+        this.dithering = null;                                  // {width, height, data: Float32Array RGB}, LDR_LLL1_0.png / 255
         this.canvas = canvas;
         this.random = options.random || Math.random;            // injectable for reproducible runs
         this.options = options;
@@ -251,10 +264,25 @@ class FluidSimulation {
         return delta;
     }
 
-    // render(target) of S:1296-1317 with BLOOM = SUNRAYS = false: Float32Array RGBA, row 0 = bottom
-    render (width = this.canvas.width, height = this.canvas.height) {
-        const bc = this.config.BACK_COLOR;                      // normalizeColor, S:1599-1606
-        return native.render(this._h, width, height, !!this.config.SHADING, bc.r / 255, bc.g / 255, bc.b / 255);
+    // render(target) of S:1296-1317: Float32Array RGBA, row 0 = bottom.  config.SHADING / BLOOM / SUNRAYS
+    // pick the display keywords like updateKeywords (S:1160-1166); BLOOM needs this.dithering, BLOOM or
+    // SUNRAYS a single-GPU fp32 handle.  config.TRANSPARENT: the checkerboard under the display on the
+    // screen (target = false, S:1311-1312), the bare display into a capture target (target = true).
+    render (width = this.canvas.width, height = this.canvas.height, target = false) {
+        const c = this.config;
+        const bc = c.BACK_COLOR;                                // normalizeColor, S:1599-1606
+        const bg = !c.TRANSPARENT ? 0 : (target ? 2 : 1);
+        if (this._pushed.BACKGROUND !== bg) {
+            native.setParam(this._h, PARAM.BACKGROUND, bg);
+            this._pushed.BACKGROUND = bg;
+        }
+        this._pushConfig();                                     // the checkerboard uses canvas.width / canvas.height (S:1327)
+        const kw = (c.SHADING ? DISPLAY.SHADING : 0) | (c.BLOOM ? DISPLAY.BLOOM : 0) | (c.SUNRAYS ? DISPLAY.SUNRAYS : 0);
+        const d = this.dithering;
+        if ((kw & DISPLAY.BLOOM) && d == null)
+            throw new Error('BLOOM needs sim.dithering: {width, height, data} of the 64x64 RGB dithering texture (LDR_LLL1_0.png / 255)');
+        return native.renderKeywords(this._h, width, height, kw, c, (kw & DISPLAY.BLOOM) ? d.data : null,
+                                     d ? d.width : 0, d ? d.height : 0, bc.r / 255, bc.g / 255, bc.b / 255);
     }
 
     stat (name) { return native.stat(this._h, STAT[name]); }
@@ -264,4 +292,4 @@ class FluidSimulation {
     sync () { native.sync(this._h); }
 }
 
-module.exports = { FluidSimulation, pointerPrototype, HSVtoRGB, wrap, FIELD, PARAM, FLAG, STAT };
+module.exports = { FluidSimulation, pointerPrototype, HSVtoRGB, wrap, FIELD, PARAM, DISPLAY, FLAG, STAT };

@@ -14,6 +14,8 @@
  *       handle, overwritten by the next read of that field — like rebinding the same texture)
  *   write(h, field, Float32Array)  sync(h)  dims(h, field) -> {width, height, channels, row0}
  *   render(h, width, height, shading, r, g, b) -> Float32Array (RGBA, row 0 = bottom)
+ *   renderKeywords(h, width, height, keywords, config, dither, dw, dh, r, g, b) -> Float32Array (any
+ *       SHADING / BLOOM / SUNRAYS set, FLUID_DISPLAY_* bits)
  *   pressureSolveHost(h, div: Float32Array, p: Float32Array, iters)   stat(h, key)
  *   ncclUniqueId() -> ArrayBuffer(128)  p2pExport(h) -> ArrayBuffer(256)  p2pConnect(h, below, above)
  *   p2pDisable(h)  getResolution(res, cw, ch) -> {width, height}  lastError(h?) -> number-free string
@@ -232,6 +234,42 @@ static napi_value Render(napi_env env, napi_callback_info info) {
     return f32_view(env, dst, n);
 }
 
+/* renderKeywords(h, width, height, keywords, config, dither, dw, dh, r, g, b): fluid_render_keywords with
+ * the BLOOM_* / SUNRAYS_* keys read from `config`; dither is the dw x dh RGB Float32Array (needed with
+ * BLOOM only; pass null otherwise).  Returns the frame (or a slab rank's band of it) like render(). */
+static napi_value RenderKeywords(napi_env env, napi_callback_info info) {
+    ARGS(11)
+    wrap_t* w = wrap_of(env, argv[0]); if (!w) return NULL;
+    int32_t wd = 0, ht = 0, dw = 0, dh = 0; uint32_t kw = 0;
+    napi_get_value_int32(env, argv[1], &wd); napi_get_value_int32(env, argv[2], &ht);
+    napi_get_value_uint32(env, argv[3], &kw);
+    napi_get_value_int32(env, argv[6], &dw); napi_get_value_int32(env, argv[7], &dh);
+    if (wd < 1 || ht < 1) { napi_throw_error(env, NULL, "bad render size"); return NULL; }
+    fluid_postfx fx;
+    fx.bloom_iterations = (int32_t)prop(env, argv[4], "BLOOM_ITERATIONS", 8);        /* S:77-84 defaults */
+    fx.bloom_resolution = (int32_t)prop(env, argv[4], "BLOOM_RESOLUTION", 256);
+    fx.bloom_intensity = prop(env, argv[4], "BLOOM_INTENSITY", 0.8);
+    fx.bloom_threshold = prop(env, argv[4], "BLOOM_THRESHOLD", 0.6);
+    fx.bloom_soft_knee = prop(env, argv[4], "BLOOM_SOFT_KNEE", 0.7);
+    fx.sunrays_resolution = (int32_t)prop(env, argv[4], "SUNRAYS_RESOLUTION", 196);
+    fx.sunrays_weight = prop(env, argv[4], "SUNRAYS_WEIGHT", 1.0);
+    const float* dither = NULL;
+    if (kw & FLUID_DISPLAY_BLOOM) {
+        float* d; size_t len;
+        if (!f32_arg(env, argv[5], &d, &len)) return NULL;
+        if (dw < 1 || dh < 1 || len != (size_t)dw * dh * 3) { napi_throw_error(env, NULL, "dither must hold dw * dh * 3 floats"); return NULL; }
+        dither = d;
+    }
+    int y0 = 0, y1 = ht;                        /* without post-FX a slab rank draws its band only */
+    if (!(kw & (FLUID_DISPLAY_BLOOM | FLUID_DISPLAY_SUNRAYS)) && !check(env, w->h, fluid_render_band(w->h, ht, &y0, &y1))) return NULL;
+    const size_t n = (size_t)wd * (y1 - y0) * 4;
+    float* dst = pinned_for(w, 5, n ? n : 1);
+    if (!dst) { napi_throw_error(env, NULL, "out of pinned host memory"); return NULL; }
+    if (!check(env, w->h, fluid_render_keywords(w->h, wd, ht, kw, &fx, dither, dw, dh, (float)num(env, argv[8]),
+                                                (float)num(env, argv[9]), (float)num(env, argv[10]), dst, n, NULL, NULL))) return NULL;
+    return f32_view(env, dst, n);
+}
+
 static napi_value Sync(napi_env env, napi_callback_info info) {
     ARGS(1)
     wrap_t* w = wrap_of(env, argv[0]); if (!w) return NULL;
@@ -331,6 +369,7 @@ NAPI_MODULE_INIT() {
         {"write", NULL, Write, NULL, NULL, NULL, napi_enumerable, NULL},
         {"pressureSolveHost", NULL, PressureSolveHost, NULL, NULL, NULL, napi_enumerable, NULL},
         {"render", NULL, Render, NULL, NULL, NULL, napi_enumerable, NULL},
+        {"renderKeywords", NULL, RenderKeywords, NULL, NULL, NULL, napi_enumerable, NULL},
         {"sync", NULL, Sync, NULL, NULL, NULL, napi_enumerable, NULL},
         {"stat", NULL, Stat, NULL, NULL, NULL, napi_enumerable, NULL},
         {"dims", NULL, Dims, NULL, NULL, NULL, napi_enumerable, NULL},

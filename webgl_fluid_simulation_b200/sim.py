@@ -27,7 +27,7 @@ import time
 import numpy as np
 
 from . import _lib
-from ._lib import FIELD, PARAM, STAT, Config, FluidError, PostFX, Timing
+from ._lib import DISPLAY_BLOOM, DISPLAY_SHADING, DISPLAY_SUNRAYS, FIELD, PARAM, STAT, Config, FluidError, PostFX, Timing
 
 
 def default_config() -> dict:
@@ -93,6 +93,38 @@ def getResolution(resolution, canvas_w, canvas_h):
     w, h = C.c_int(), C.c_int()
     _lib.lib().fluid_get_resolution(int(resolution), int(canvas_w), int(canvas_h), C.byref(w), C.byref(h))
     return {"width": w.value, "height": h.value}
+
+
+def display_keywords(config) -> int:
+    """updateKeywords, S:1160-1166: the display shader's keyword set as DISPLAY_* bits."""
+    kw = 0
+    if config.get("SHADING"):
+        kw |= DISPLAY_SHADING
+    if config.get("BLOOM"):
+        kw |= DISPLAY_BLOOM
+    if config.get("SUNRAYS"):
+        kw |= DISPLAY_SUNRAYS
+    return kw
+
+
+def postfx_inputs(config, dithering):
+    """What render() hands fluid_render_keywords besides the target: (keywords, PostFX or None without
+    BLOOM and SUNRAYS, the float32 (dh, dw, 3) dithering texture or None without BLOOM).  The dithering
+    texture is drawn only with BLOOM (S:1341-1344), so only then is it required."""
+    kw = display_keywords(config)
+    dith = None
+    if kw & DISPLAY_BLOOM:
+        if dithering is None:
+            raise ValueError("BLOOM needs sim.dithering: the (64, 64, 3) float RGB dithering texture (LDR_LLL1_0.png / 255)")
+        dith = np.ascontiguousarray(dithering, np.float32)
+        if dith.ndim != 3 or dith.shape[2] != 3 or dith.shape[0] < 1 or dith.shape[1] < 1:
+            raise ValueError(f"sim.dithering must be (height, width, 3) RGB, got shape {dith.shape}")
+    if not kw & (DISPLAY_BLOOM | DISPLAY_SUNRAYS):
+        return kw, None, None
+    fx = PostFX(int(config["BLOOM_ITERATIONS"]), int(config["BLOOM_RESOLUTION"]), float(config["BLOOM_INTENSITY"]),
+                float(config["BLOOM_THRESHOLD"]), float(config["BLOOM_SOFT_KNEE"]), int(config["SUNRAYS_RESOLUTION"]),
+                float(config["SUNRAYS_WEIGHT"]))
+    return kw, fx, dith
 
 
 class _Field:
@@ -353,7 +385,10 @@ class FluidSimulation:
         """render(target), S:1296-1317: (height, width, 4) float32 RGBA, row 0 = bottom.  Defaults
         to the canvas size (target == null branch, S:1332-1333).  config.TRANSPARENT: the display is
         drawn over the checkerboard on the screen (target=False, S:1311-1312) and bare, un-blended,
-        into a capture target (target=True: what captureScreenshot renders into, S:287-299)."""
+        into a capture target (target=True: what captureScreenshot renders into, S:287-299).
+        config.SHADING / BLOOM / SUNRAYS pick the display keywords like updateKeywords (S:1160-1166);
+        BLOOM needs `sim.dithering`.  BLOOM or SUNRAYS need a single-GPU fp32 handle.  last_bloom /
+        last_sunrays hold the bloom FBO / sunrays texture of the frame, or None when that keyword is off."""
         w = int(width or self.canvas["width"]); h = int(height or self.canvas["height"])
         bc = self.config["BACK_COLOR"]                       # normalizeColor, S:1599-1606
         out = np.empty((h, w, 4), np.float32)
@@ -363,32 +398,24 @@ class FluidSimulation:
             self._check(self._L.fluid_set_param(self._h, PARAM["BACKGROUND"], float(bg)))
             self._pushed["BACKGROUND"] = bg
         self._push_config()                                  # the checkerboard uses canvas.width / canvas.height (S:1327)
-        if cfg.get("BLOOM") or cfg.get("SUNRAYS"):
-            # built for the reference's default keyword set only: SHADING + BLOOM + SUNRAYS
-            if not (cfg.get("BLOOM") and cfg.get("SUNRAYS") and cfg.get("SHADING")):
-                raise NotImplementedError("post-FX are built for SHADING + BLOOM + SUNRAYS together (the reference defaults)")
-            dith = getattr(self, "dithering", None)
-            if dith is None:
-                raise ValueError("set sim.dithering to the (64, 64, 3) float RGB dithering texture (LDR_LLL1_0.png / 255)")
-            dith = np.ascontiguousarray(dith, np.float32)
-            fx = PostFX(int(cfg["BLOOM_ITERATIONS"]), int(cfg["BLOOM_RESOLUTION"]), float(cfg["BLOOM_INTENSITY"]),
-                        float(cfg["BLOOM_THRESHOLD"]), float(cfg["BLOOM_SOFT_KNEE"]), int(cfg["SUNRAYS_RESOLUTION"]),
-                        float(cfg["SUNRAYS_WEIGHT"]))
-            b = getResolution(cfg["BLOOM_RESOLUTION"], w, h); sr = getResolution(cfg["SUNRAYS_RESOLUTION"], w, h)
+        kw, fx, dith = postfx_inputs(cfg, getattr(self, "dithering", None))
+        self.last_bloom = self.last_sunrays = None           # the bloom FBO / sunrays texture of this frame, if drawn
+        if kw & DISPLAY_BLOOM:
+            b = getResolution(cfg["BLOOM_RESOLUTION"], w, h)
             self.last_bloom = np.empty((b["height"], b["width"], 4), np.float32)
+        if kw & DISPLAY_SUNRAYS:
+            sr = getResolution(cfg["SUNRAYS_RESOLUTION"], w, h)
             self.last_sunrays = np.empty((sr["height"], sr["width"]), np.float32)
-            self._check(self._L.fluid_render_postfx(
-                self._h, w, h, C.byref(fx), dith.ctypes.data_as(C.c_void_p), dith.shape[1], dith.shape[0],
-                bc["r"] / 255, bc["g"] / 255, bc["b"] / 255, out.ctypes.data_as(C.c_void_p), out.size,
-                self.last_bloom.ctypes.data_as(C.c_void_p), self.last_sunrays.ctypes.data_as(C.c_void_p)))
-            return out
-        y0, y1 = C.c_int(), C.c_int()                        # a slab rank draws its band of the target only
-        self._check(self._L.fluid_render_band(self._h, h, C.byref(y0), C.byref(y1)))
-        out = out[: y1.value - y0.value]
-        self.render_band = (y0.value, y1.value)
-        self._check(self._L.fluid_render(self._h, w, h, 1 if self.config["SHADING"] else 0,
-                                         bc["r"] / 255, bc["g"] / 255, bc["b"] / 255,
-                                         out.ctypes.data_as(C.c_void_p), out.size))
+        if fx is None:                                       # a slab rank draws its band of the target only
+            y0, y1 = C.c_int(), C.c_int()
+            self._check(self._L.fluid_render_band(self._h, h, C.byref(y0), C.byref(y1)))
+            out = out[: y1.value - y0.value]
+            self.render_band = (y0.value, y1.value)
+        ptr = lambda a: None if a is None else a.ctypes.data_as(C.c_void_p)   # noqa: E731
+        self._check(self._L.fluid_render_keywords(
+            self._h, w, h, kw, None if fx is None else C.byref(fx), ptr(dith),
+            0 if dith is None else dith.shape[1], 0 if dith is None else dith.shape[0],
+            bc["r"] / 255, bc["g"] / 255, bc["b"] / 255, ptr(out), out.size, ptr(self.last_bloom), ptr(self.last_sunrays)))
         return out
 
     @staticmethod
