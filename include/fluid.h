@@ -256,6 +256,28 @@ int fluid_render_keywords(fluid_t* h, int width, int height, uint32_t keywords, 
                           const float* dither_rgb, int dw, int dh, float back_r, float back_g, float back_b,
                           float* host_rgba, size_t n_floats, float* host_bloom, float* host_sunrays);
 
+/* captureScreenshot() of S:287-299 up to the bytes toDataURL encodes (normalizeTexture S:309-327):
+ * render(target) with `keywords` into a width x height RGBA half-float target — width x height is
+ * getResolution(CAPTURE_RESOLUTION) of the canvas — returned as 4 * width * height bytes.
+ *  - fp16 target: the background is drawColor(BACK_COLOR) stored in fp16 (back_* = BACK_COLOR / 255,
+ *    rounded to nearest even); the display is blended over it ONE / ONE_MINUS_SRC_ALPHA in fp32 and every
+ *    channel is then rounded to fp16 (nearest even, overflow to +-Inf).  transparent != 0: the display
+ *    is stored bare with blending off (S:1307-1309).  The checkerboard is never drawn and
+ *    FLUID_BACKGROUND is not consulted.
+ *  - Post-FX: the bloom and sunrays FBOs keep the sizes render(null) gives them on a canvas_w x canvas_h
+ *    drawing buffer (S:1012-1043), and share the handle's targets with fluid_render_keywords, so a
+ *    capture on the canvas render() draws does not remake them.  texelSize and ditherScale use
+ *    width x height (S:1332-1344).
+ *  - Bytes: clamp01(v) * 255 truncated to uint8 (NaN gives 0), rows flipped so the TOP row comes
+ *    first.  One device-to-host copy of n_bytes, then a stream sync.
+ * Refused with FLUID_ERR_INVALID, the handle staying usable: unknown keyword bits; n_bytes !=
+ * 4 * width * height; width, height, canvas_w or canvas_h < 1; BLOOM without dither_rgb; fx == NULL with
+ * BLOOM or SUNRAYS; slab handles; half-storage handles with BLOOM or SUNRAYS (without them half storage
+ * works, as in fluid_render). */
+int fluid_capture(fluid_t* h, int width, int height, int canvas_w, int canvas_h, uint32_t keywords,
+                  int transparent, const fluid_postfx* fx, const float* dither_rgb, int dw, int dh,
+                  float back_r, float back_g, float back_b, uint8_t* host_rgba8, size_t n_bytes);
+
 int fluid_sync(fluid_t* h);
 int fluid_timing_last(fluid_t* h, fluid_timing* out);
 

@@ -1705,6 +1705,19 @@ static int need_frame(fluid_t* h, size_t cells) {
     return FLUID_OK;
 }
 
+// The fp32 dye the display kernels sample: dye.read, or in half storage its widened copy in the scratch
+// buffer (the sampler widens fp16 texels exactly; shading is fp32 as in the shader).
+static int display_source(fluid_t* h, const float4** src) {
+    *src = (const float4*)h->dye.read;
+    if (!h->half) return FLUID_OK;
+    const size_t nd = (size_t)h->cfg.dye_w * h->cfg.dye_h * 4;
+    int rc = need_scratch(h, nd); if (rc) return rc;
+    hs::widen_kernel<<<(unsigned)((nd + 255) / 256), 256, 0, h->stream>>>((const hs::h1*)h->dye.read, h->scratch, nd);
+    if ((rc = check_launch(h, "hs::widen_kernel"))) return rc;
+    *src = (const float4*)h->scratch;
+    return FLUID_OK;
+}
+
 // render(target) of S:1296-1317 for config.BLOOM = config.SUNRAYS = false: the background selected by
 // FLUID_BACKGROUND (colour / checkerboard / none), then the display shader (optionally SHADING) blended over it.
 int fluid_render(fluid_t* h, int width, int height, int shading, float back_r, float back_g,
@@ -1726,14 +1739,8 @@ int fluid_render(fluid_t* h, int width, int height, int shading, float back_r, f
             return fail(h, FLUID_ERR_HALO, "render target of %d rows needs %d dye ghost rows, the slab keeps %d", height,
                         (h->cfg.dye_h + height - 1) / height + 2, h->Gd);
     }
-    const float4* dye_src = (const float4*)h->dye.read;
-    if (h->half) {                                   // the sampler widens fp16 texels exactly; shading is fp32 as in the shader
-        const size_t nd = (size_t)h->cfg.dye_w * h->cfg.dye_h * 4;
-        int rc = need_scratch(h, nd); if (rc) return rc;
-        hs::widen_kernel<<<(unsigned)((nd + 255) / 256), 256, 0, h->stream>>>((const hs::h1*)h->dye.read, h->scratch, nd);
-        if ((rc = check_launch(h, "hs::widen_kernel"))) return rc;
-        dye_src = (const float4*)h->scratch;
-    }
+    const float4* dye_src;
+    if (int rc = display_source(h, &dye_src)) return rc;
     dim3 b(32, 8);
     display_kernel<<<grid2d(width, y1 - y0, b), b, 0, h->stream>>>(dye_src, h->cfg.dye_w, h->cfg.dye_h,
                                                                    h->frame, width, height, shading, back_r, back_g, back_b,
@@ -1804,33 +1811,40 @@ static const DisplayFullKernel kDisplayFull[8] = {
     display_full_kernel<false, true, true>, display_full_kernel<true, true, true>,
 };
 
-// render(null) of S:1296-1317 for a keyword set with BLOOM or SUNRAYS (single GPU, fp32 storage): applyBloom
-// (S:1350-1394) when BLOOM is on, applySunrays + blur(…, 1) (S:1396-1419; the mask is drawn into dye.write
-// exactly like S:1300) when SUNRAYS is on, then the background and drawDisplay with the chosen keywords.
-// FBO sizes follow initBloomFramebuffers / initSunraysFramebuffers (S:1012-1043).
-static int render_postfx(fluid_t* h, const char* what, int width, int height, uint32_t keywords,
-                         const fluid_postfx* fx, const float* dither_rgb, int dw, int dh, float back_r,
-                         float back_g, float back_b, float* host_rgba, size_t n_floats, float* host_bloom,
-                         float* host_sunrays) {
+// The 8-bit capture instantiations, indexed the same way
+using CaptureFullKernel = void (*)(const float4*, int, int, const float4*, int, int, const float*, int, int,
+                                   const float*, int, int, uchar4*, int, int, float, float, float, int, float, float4);
+static const CaptureFullKernel kDisplayCapture[8] = {
+    nullptr, nullptr,
+    display_full_kernel<false, true, false, StoreCapture>, display_full_kernel<true, true, false, StoreCapture>,
+    display_full_kernel<false, false, true, StoreCapture>, display_full_kernel<true, false, true, StoreCapture>,
+    display_full_kernel<false, true, true, StoreCapture>, display_full_kernel<true, true, true, StoreCapture>,
+};
+
+// The bloom FBO and the sunrays texture a display kernel samples, as post_fx_chains left them
+struct PostFXOut { int bw, bh, sw, sh; };
+
+// The post-FX chains of render() for the keywords that are on: applyBloom (S:1350-1394) with BLOOM,
+// applySunrays + blur(…, 1) (S:1396-1419; the mask is drawn into dye.write exactly like S:1300) with
+// SUNRAYS.  FBO sizes follow initBloomFramebuffers / initSunraysFramebuffers (S:1012-1043), which size
+// them from the drawing buffer: canvas_w x canvas_h.  Single GPU, fp32 storage, arguments checked by
+// the caller.
+static int post_fx_chains(fluid_t* h, uint32_t keywords, const fluid_postfx* fx, const float* dither_rgb,
+                          int dw, int dh, int canvas_w, int canvas_h, PostFXOut* o) {
     const bool bloom_on = keywords & FLUID_DISPLAY_BLOOM, sun_on = keywords & FLUID_DISPLAY_SUNRAYS;
-    if (!h || !fx || !host_rgba || width < 1 || height < 1 || (bloom_on && (!dither_rgb || dw < 1 || dh < 1)))
-        return fail(h, FLUID_ERR_INVALID, "bad argument");
-    if (h->slab()) return not_on_slab(h, what);
-    if (h->half) return fail(h, FLUID_ERR_INVALID, "%s is not built for FLUID_FLAG_HALF_STORAGE (the reference's bloom / sunrays FBOs are fp16 too)", what);
-    const size_t cells = (size_t)width * height;
-    if (n_floats != 4 * cells) return fail(h, FLUID_ERR_INVALID, "render target has %zu floats, caller passed %zu", 4 * cells, n_floats);
     int bw = 1, bh = 1, sw = 1, sh = 1, levels = 0;
-    if (bloom_on) fluid_get_resolution(fx->bloom_resolution, width, height, &bw, &bh);
-    if (sun_on) fluid_get_resolution(fx->sunrays_resolution, width, height, &sw, &sh);
+    if (bloom_on) fluid_get_resolution(fx->bloom_resolution, canvas_w, canvas_h, &bw, &bh);
+    if (sun_on) fluid_get_resolution(fx->sunrays_resolution, canvas_w, canvas_h, &sw, &sh);
     if (bw < 1 || bh < 1 || sw < 1 || sh < 1) return fail(h, FLUID_ERR_INVALID, "bad post-FX resolution");
     if (bloom_on)
         while (levels < fx->bloom_iterations && (bw >> (levels + 1)) >= 2 && (bh >> (levels + 1)) >= 2) ++levels;
-    int rc = need_frame(h, cells); if (rc) return rc;
+    int rc;
     if (bloom_on) {
         if ((rc = need_bloom_targets(h, bw, bh, levels)) || (rc = need_dither_target(h, dw, dh))) return rc;
         CU(cudaMemcpyAsync(h->pfx.dither, dither_rgb, (size_t)dw * dh * 3 * sizeof(float), cudaMemcpyHostToDevice, h->stream));
     }
     if (sun_on && (rc = need_sunrays_targets(h, sw, sh))) return rc;
+    *o = {bw, bh, sw, sh};
     const int Wd = h->cfg.dye_w, Hd = h->cfg.dye_h;
     float4* bloom = h->pfx.bloom;
     float *sun = h->pfx.sun, *sun2 = sun ? sun + (size_t)sw * sh : nullptr;
@@ -1871,18 +1885,43 @@ static int render_postfx(fluid_t* h, const char* what, int width, int height, ui
         blur3_kernel<<<grid2d(sw, sh, b), b, 0, h->stream>>>(sun2, sun, sw, sh, 0.0f, (float)(1.0 / (double)sh));
         nk += 4;
     }
+    return check_launch(h, "post-FX kernels", nk);
+}
+
+// The `ts` argument of display_full_kernel for a width x height target: texelSize = 1 / width, 1 / height
+// (S:1337) and getTextureScale (S:1626-1631) are JS doubles, narrowed here.
+static float4 display_scales(uint32_t keywords, int width, int height, int dw, int dh) {
+    const bool bloom_on = keywords & FLUID_DISPLAY_BLOOM;
+    return make_float4((float)(1.0 / (double)width), (float)(1.0 / (double)height),
+                       bloom_on ? (float)((double)width / (double)dw) : 0.0f, bloom_on ? (float)((double)height / (double)dh) : 0.0f);
+}
+
+// render(null) of S:1296-1317 for a keyword set with BLOOM or SUNRAYS (single GPU, fp32 storage): the
+// post-FX chains on width x height FBOs, then the background and drawDisplay with the chosen keywords.
+static int render_postfx(fluid_t* h, const char* what, int width, int height, uint32_t keywords,
+                         const fluid_postfx* fx, const float* dither_rgb, int dw, int dh, float back_r,
+                         float back_g, float back_b, float* host_rgba, size_t n_floats, float* host_bloom,
+                         float* host_sunrays) {
+    const bool bloom_on = keywords & FLUID_DISPLAY_BLOOM, sun_on = keywords & FLUID_DISPLAY_SUNRAYS;
+    if (!h || !fx || !host_rgba || width < 1 || height < 1 || (bloom_on && (!dither_rgb || dw < 1 || dh < 1)))
+        return fail(h, FLUID_ERR_INVALID, "bad argument");
+    if (h->slab()) return not_on_slab(h, what);
+    if (h->half) return fail(h, FLUID_ERR_INVALID, "%s is not built for FLUID_FLAG_HALF_STORAGE (the reference's bloom / sunrays FBOs are fp16 too)", what);
+    const size_t cells = (size_t)width * height;
+    if (n_floats != 4 * cells) return fail(h, FLUID_ERR_INVALID, "render target has %zu floats, caller passed %zu", 4 * cells, n_floats);
+    int rc = need_frame(h, cells); if (rc) return rc;
+    PostFXOut o;
+    if ((rc = post_fx_chains(h, keywords, fx, dither_rgb, dw, dh, width, height, &o))) return rc;
     // ---- background + drawDisplay -----------------------------------------------------------------------
+    dim3 b(32, 8);
     kDisplayFull[keywords]<<<grid2d(width, height, b), b, 0, h->stream>>>(
-        (const float4*)h->dye.read, Wd, Hd, bloom_on ? bloom : nullptr, bw, bh, sun_on ? sun : nullptr, sw, sh,
-        bloom_on ? h->pfx.dither : nullptr, dw, dh, h->frame, width, height, back_r, back_g, back_b, h->background,
-        h->cfg.aspect,
-        make_float4((float)(1.0 / (double)width), (float)(1.0 / (double)height),
-                    bloom_on ? (float)((double)width / (double)dw) : 0.0f, bloom_on ? (float)((double)height / (double)dh) : 0.0f));
-    ++nk;
-    if ((rc = check_launch(h, "post-FX kernels", nk))) return rc;
+        (const float4*)h->dye.read, h->cfg.dye_w, h->cfg.dye_h, bloom_on ? h->pfx.bloom : nullptr, o.bw, o.bh,
+        sun_on ? h->pfx.sun : nullptr, o.sw, o.sh, bloom_on ? h->pfx.dither : nullptr, dw, dh, h->frame, width,
+        height, back_r, back_g, back_b, h->background, h->cfg.aspect, display_scales(keywords, width, height, dw, dh));
+    if ((rc = check_launch(h, "display_full_kernel"))) return rc;
     CU(cudaMemcpyAsync(host_rgba, h->frame, cells * sizeof(float4), cudaMemcpyDeviceToHost, h->stream));
-    if (bloom_on && host_bloom) CU(cudaMemcpyAsync(host_bloom, bloom, (size_t)bw * bh * sizeof(float4), cudaMemcpyDeviceToHost, h->stream));
-    if (sun_on && host_sunrays) CU(cudaMemcpyAsync(host_sunrays, sun, (size_t)sw * sh * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+    if (bloom_on && host_bloom) CU(cudaMemcpyAsync(host_bloom, h->pfx.bloom, (size_t)o.bw * o.bh * sizeof(float4), cudaMemcpyDeviceToHost, h->stream));
+    if (sun_on && host_sunrays) CU(cudaMemcpyAsync(host_sunrays, h->pfx.sun, (size_t)o.sw * o.sh * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
     CU(cudaStreamSynchronize(h->stream));
     return FLUID_OK;
 }
@@ -1909,6 +1948,55 @@ int fluid_render_postfx(fluid_t* h, int width, int height, const fluid_postfx* f
     return render_postfx(h, "fluid_render_postfx", width, height,
                          FLUID_DISPLAY_SHADING | FLUID_DISPLAY_BLOOM | FLUID_DISPLAY_SUNRAYS, fx, dither_rgb, dw,
                          dh, back_r, back_g, back_b, host_rgba, n_floats, host_bloom, host_sunrays);
+}
+
+// captureScreenshot (S:287-299) up to normalizeTexture (S:309-327): render(target) into a width x height
+// RGBA half-float target.  The post-FX chains run on the canvas-sized FBOs of render(null); the display
+// draws at the target's size over drawColor(BACK_COLOR) stored in fp16 (not TRANSPARENT) or bare with
+// blending off (TRANSPARENT), never over the checkerboard (S:1303-1314).  The display kernel's epilogue
+// does the fp16 store, the 8-bit truncation and the flip; the fp32 frame never reaches memory.
+int fluid_capture(fluid_t* h, int width, int height, int canvas_w, int canvas_h, uint32_t keywords,
+                  int transparent, const fluid_postfx* fx, const float* dither_rgb, int dw, int dh,
+                  float back_r, float back_g, float back_b, uint8_t* host_rgba8, size_t n_bytes) {
+    if (!h) return FLUID_ERR_INVALID;
+    if (keywords & ~(uint32_t)(FLUID_DISPLAY_SHADING | FLUID_DISPLAY_BLOOM | FLUID_DISPLAY_SUNRAYS))
+        return fail(h, FLUID_ERR_INVALID, "unknown display keyword bits 0x%x", keywords);
+    const bool bloom_on = keywords & FLUID_DISPLAY_BLOOM, sun_on = keywords & FLUID_DISPLAY_SUNRAYS;
+    const bool postfx = bloom_on || sun_on;
+    if (!host_rgba8 || width < 1 || height < 1 || canvas_w < 1 || canvas_h < 1 || (postfx && !fx) ||
+        (bloom_on && (!dither_rgb || dw < 1 || dh < 1)))
+        return fail(h, FLUID_ERR_INVALID, "bad argument");
+    const size_t cells = (size_t)width * height;
+    if (n_bytes != 4 * cells) return fail(h, FLUID_ERR_INVALID, "capture image has %zu bytes, caller passed %zu", 4 * cells, n_bytes);
+    if (h->slab()) return not_on_slab(h, "fluid_capture");
+    if (h->half && postfx)
+        return fail(h, FLUID_ERR_INVALID, "fluid_capture with BLOOM or SUNRAYS is not built for FLUID_FLAG_HALF_STORAGE");
+    // drawColor's store of normalizeColor(BACK_COLOR) into the half-float target
+    const float b16[3] = {__half2float(__float2half_rn(back_r)), __half2float(__float2half_rn(back_g)),
+                          __half2float(__float2half_rn(back_b))};
+    const int bg_mode = transparent ? 2 : 0;
+    int rc = need_frame(h, (cells + 3) / 4); if (rc) return rc;      // the frame's storage holds the uchar4 image
+    uchar4* img = (uchar4*)h->frame;
+    dim3 b(32, 8);
+    if (!postfx) {
+        const float4* dye_src;
+        if ((rc = display_source(h, &dye_src))) return rc;
+        display_kernel<StoreCapture><<<grid2d(width, height, b), b, 0, h->stream>>>(
+            dye_src, h->cfg.dye_w, h->cfg.dye_h, img, width, height, (keywords & FLUID_DISPLAY_SHADING) ? 1 : 0,
+            b16[0], b16[1], b16[2], make_float2((float)(1.0 / (double)width), (float)(1.0 / (double)height)), bg_mode,
+            h->cfg.aspect, 0, 0, height);
+    } else {
+        PostFXOut o;
+        if ((rc = post_fx_chains(h, keywords, fx, dither_rgb, dw, dh, canvas_w, canvas_h, &o))) return rc;
+        kDisplayCapture[keywords]<<<grid2d(width, height, b), b, 0, h->stream>>>(
+            (const float4*)h->dye.read, h->cfg.dye_w, h->cfg.dye_h, bloom_on ? h->pfx.bloom : nullptr, o.bw, o.bh,
+            sun_on ? h->pfx.sun : nullptr, o.sw, o.sh, bloom_on ? h->pfx.dither : nullptr, dw, dh, img, width,
+            height, b16[0], b16[1], b16[2], bg_mode, h->cfg.aspect, display_scales(keywords, width, height, dw, dh));
+    }
+    if ((rc = check_launch(h, "capture display kernel"))) return rc;
+    CU(cudaMemcpyAsync(host_rgba8, img, n_bytes, cudaMemcpyDeviceToHost, h->stream));
+    CU(cudaStreamSynchronize(h->stream));
+    return FLUID_OK;
 }
 
 void* fluid_host_alloc(size_t bytes) {

@@ -127,13 +127,14 @@ __global__ void __launch_bounds__(256) blur3_kernel(const float* __restrict__ sr
 // displayShaderSource S:549-612 compiled with the keywords updateKeywords picks (S:1160-1166), over
 // the background of render(), premultiplied blend.  One instantiation per keyword set with BLOOM or
 // SUNRAYS; the sets with neither use display_kernel (passes.cuh).  The inputs of a keyword that is
-// off are never read (pass nullptr).
-template <bool SHADING, bool BLOOM, bool SUNRAYS>
+// off are never read (pass nullptr).  Out: the output policy (passes.cuh), the fp32 frame of render()
+// or the 8-bit image of captureScreenshot.
+template <bool SHADING, bool BLOOM, bool SUNRAYS, class Out = StoreFrame>
 __global__ void __launch_bounds__(256) display_full_kernel(const float4* __restrict__ dye, int Wd, int Hd,
                                                            const float4* __restrict__ bloom, int bw, int bh,
                                                            const float* __restrict__ sun, int sw, int sh,
                                                            const float* __restrict__ dither, int dw, int dh,
-                                                           float4* __restrict__ out, int w, int h, float br_, float bg_,
+                                                           typename Out::T* __restrict__ out, int w, int h, float br_, float bg_,
                                                            float bb_, int bg_mode, float aspect, float4 ts) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y * blockDim.y + threadIdx.y;
     if (i >= w || j >= h) return;
@@ -177,7 +178,8 @@ __global__ void __launch_bounds__(256) display_full_kernel(const float4* __restr
         }
     }
     const float a = fmaxf(cc[0], fmaxf(cc[1], cc[2]));
-    out[(size_t)j * w + i] = blend_over_background(cc[0], cc[1], cc[2], a, bg_mode, br_, bg_, bb_, aspect, uvx, uvy);
+    out[(size_t)Out::row(j, h) * w + i] =
+        Out::pack(blend_over_background(cc[0], cc[1], cc[2], a, bg_mode, br_, bg_, bb_, aspect, uvx, uvy));
 }
 
 }  // namespace fk

@@ -75,6 +75,7 @@ class FluidSimulation {
         this.config = Object.assign({                           // S:59-85
             SIM_RESOLUTION: 128,
             DYE_RESOLUTION: 1024,
+            CAPTURE_RESOLUTION: 512,    // S:62
             DENSITY_DISSIPATION: 1,
             VELOCITY_DISSIPATION: 0.2,
             PRESSURE: 0.8,
@@ -277,12 +278,36 @@ class FluidSimulation {
             this._pushed.BACKGROUND = bg;
         }
         this._pushConfig();                                     // the checkerboard uses canvas.width / canvas.height (S:1327)
-        const kw = (c.SHADING ? DISPLAY.SHADING : 0) | (c.BLOOM ? DISPLAY.BLOOM : 0) | (c.SUNRAYS ? DISPLAY.SUNRAYS : 0);
+        const kw = this._keywords();
         const d = this.dithering;
-        if ((kw & DISPLAY.BLOOM) && d == null)
-            throw new Error('BLOOM needs sim.dithering: {width, height, data} of the 64x64 RGB dithering texture (LDR_LLL1_0.png / 255)');
         return native.renderKeywords(this._h, width, height, kw, c, (kw & DISPLAY.BLOOM) ? d.data : null,
                                      d ? d.width : 0, d ? d.height : 0, bc.r / 255, bc.g / 255, bc.b / 255);
+    }
+
+    // updateKeywords (S:1160-1166) as DISPLAY bits; BLOOM needs this.dithering
+    _keywords () {
+        const c = this.config;
+        const kw = (c.SHADING ? DISPLAY.SHADING : 0) | (c.BLOOM ? DISPLAY.BLOOM : 0) | (c.SUNRAYS ? DISPLAY.SUNRAYS : 0);
+        if ((kw & DISPLAY.BLOOM) && this.dithering == null)
+            throw new Error('BLOOM needs sim.dithering: {width, height, data} of the 64x64 RGB dithering texture (LDR_LLL1_0.png / 255)');
+        return kw;
+    }
+
+    // captureScreenshot() of S:287-299 up to normalizeTexture (S:309-327): render() into an RGBA half-float
+    // target of getResolution(CAPTURE_RESOLUTION), quantised to 8 bits on the GPU.  The bloom and sunrays
+    // FBOs keep the canvas sizes; TRANSPARENT stores the display bare.  Returns {width, height, data:
+    // Uint8Array RGBA, top row first}: what textureToCanvas puts on the capture canvas.  toDataURL and the
+    // download (S:296-298) stay in the page.
+    captureScreenshot () {
+        const c = this.config;
+        const bc = c.BACK_COLOR;                                // normalizeColor, S:1599-1606
+        const res = native.getResolution(c.CAPTURE_RESOLUTION, this.canvas.width, this.canvas.height);
+        const kw = this._keywords();
+        const d = this.dithering;
+        const data = native.capture(this._h, res.width, res.height, this.canvas.width, this.canvas.height, kw,
+                                    !!c.TRANSPARENT, c, (kw & DISPLAY.BLOOM) ? d.data : null, d ? d.width : 0,
+                                    d ? d.height : 0, bc.r / 255, bc.g / 255, bc.b / 255);
+        return { width: res.width, height: res.height, data };
     }
 
     stat (name) { return native.stat(this._h, STAT[name]); }

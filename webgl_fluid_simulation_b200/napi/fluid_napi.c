@@ -16,6 +16,8 @@
  *   render(h, width, height, shading, r, g, b) -> Float32Array (RGBA, row 0 = bottom)
  *   renderKeywords(h, width, height, keywords, config, dither, dw, dh, r, g, b) -> Float32Array (any
  *       SHADING / BLOOM / SUNRAYS set, FLUID_DISPLAY_* bits)
+ *   capture(h, width, height, canvasWidth, canvasHeight, keywords, transparent, config, dither, dw, dh,
+ *       r, g, b) -> Uint8Array (captureScreenshot's RGBA8 image, top row first)
  *   pressureSolveHost(h, div: Float32Array, p: Float32Array, iters)   stat(h, key)
  *   ncclUniqueId() -> ArrayBuffer(128)  p2pExport(h) -> ArrayBuffer(256)  p2pConnect(h, below, above)
  *   p2pDisable(h)  getResolution(res, cw, ch) -> {width, height}  lastError(h?) -> number-free string
@@ -234,6 +236,29 @@ static napi_value Render(napi_env env, napi_callback_info info) {
     return f32_view(env, dst, n);
 }
 
+/* The BLOOM_* / SUNRAYS_* keys of `config` (S:77-84 defaults) */
+static void postfx_from(napi_env env, napi_value o, fluid_postfx* fx) {
+    fx->bloom_iterations = (int32_t)prop(env, o, "BLOOM_ITERATIONS", 8);
+    fx->bloom_resolution = (int32_t)prop(env, o, "BLOOM_RESOLUTION", 256);
+    fx->bloom_intensity = prop(env, o, "BLOOM_INTENSITY", 0.8);
+    fx->bloom_threshold = prop(env, o, "BLOOM_THRESHOLD", 0.6);
+    fx->bloom_soft_knee = prop(env, o, "BLOOM_SOFT_KNEE", 0.7);
+    fx->sunrays_resolution = (int32_t)prop(env, o, "SUNRAYS_RESOLUTION", 196);
+    fx->sunrays_weight = prop(env, o, "SUNRAYS_WEIGHT", 1.0);
+}
+
+/* The dw x dh RGB dithering texture: a Float32Array with BLOOM, ignored (NULL) without it.  0 with a JS
+ * exception pending if it is missing or the wrong size. */
+static int dither_from(napi_env env, uint32_t kw, napi_value v, int32_t dw, int32_t dh, const float** dither) {
+    *dither = NULL;
+    if (!(kw & FLUID_DISPLAY_BLOOM)) return 1;
+    float* d; size_t len;
+    if (!f32_arg(env, v, &d, &len)) return 0;
+    if (dw < 1 || dh < 1 || len != (size_t)dw * dh * 3) { napi_throw_error(env, NULL, "dither must hold dw * dh * 3 floats"); return 0; }
+    *dither = d;
+    return 1;
+}
+
 /* renderKeywords(h, width, height, keywords, config, dither, dw, dh, r, g, b): fluid_render_keywords with
  * the BLOOM_* / SUNRAYS_* keys read from `config`; dither is the dw x dh RGB Float32Array (needed with
  * BLOOM only; pass null otherwise).  Returns the frame (or a slab rank's band of it) like render(). */
@@ -246,20 +271,9 @@ static napi_value RenderKeywords(napi_env env, napi_callback_info info) {
     napi_get_value_int32(env, argv[6], &dw); napi_get_value_int32(env, argv[7], &dh);
     if (wd < 1 || ht < 1) { napi_throw_error(env, NULL, "bad render size"); return NULL; }
     fluid_postfx fx;
-    fx.bloom_iterations = (int32_t)prop(env, argv[4], "BLOOM_ITERATIONS", 8);        /* S:77-84 defaults */
-    fx.bloom_resolution = (int32_t)prop(env, argv[4], "BLOOM_RESOLUTION", 256);
-    fx.bloom_intensity = prop(env, argv[4], "BLOOM_INTENSITY", 0.8);
-    fx.bloom_threshold = prop(env, argv[4], "BLOOM_THRESHOLD", 0.6);
-    fx.bloom_soft_knee = prop(env, argv[4], "BLOOM_SOFT_KNEE", 0.7);
-    fx.sunrays_resolution = (int32_t)prop(env, argv[4], "SUNRAYS_RESOLUTION", 196);
-    fx.sunrays_weight = prop(env, argv[4], "SUNRAYS_WEIGHT", 1.0);
-    const float* dither = NULL;
-    if (kw & FLUID_DISPLAY_BLOOM) {
-        float* d; size_t len;
-        if (!f32_arg(env, argv[5], &d, &len)) return NULL;
-        if (dw < 1 || dh < 1 || len != (size_t)dw * dh * 3) { napi_throw_error(env, NULL, "dither must hold dw * dh * 3 floats"); return NULL; }
-        dither = d;
-    }
+    postfx_from(env, argv[4], &fx);
+    const float* dither;
+    if (!dither_from(env, kw, argv[5], dw, dh, &dither)) return NULL;
     int y0 = 0, y1 = ht;                        /* without post-FX a slab rank draws its band only */
     if (!(kw & (FLUID_DISPLAY_BLOOM | FLUID_DISPLAY_SUNRAYS)) && !check(env, w->h, fluid_render_band(w->h, ht, &y0, &y1))) return NULL;
     const size_t n = (size_t)wd * (y1 - y0) * 4;
@@ -268,6 +282,32 @@ static napi_value RenderKeywords(napi_env env, napi_callback_info info) {
     if (!check(env, w->h, fluid_render_keywords(w->h, wd, ht, kw, &fx, dither, dw, dh, (float)num(env, argv[8]),
                                                 (float)num(env, argv[9]), (float)num(env, argv[10]), dst, n, NULL, NULL))) return NULL;
     return f32_view(env, dst, n);
+}
+
+/* capture(h, width, height, canvasWidth, canvasHeight, keywords, transparent, config, dither, dw, dh, r, g, b):
+ * fluid_capture, arguments as for renderKeywords.  Returns a new Uint8Array of width * height * 4 bytes, top
+ * row first: what normalizeTexture (S:309-327) hands textureToCanvas. */
+static napi_value Capture(napi_env env, napi_callback_info info) {
+    ARGS(14)
+    wrap_t* w = wrap_of(env, argv[0]); if (!w) return NULL;
+    int32_t wd = 0, ht = 0, cw = 0, ch = 0, dw = 0, dh = 0; uint32_t kw = 0; bool transparent = false;
+    napi_get_value_int32(env, argv[1], &wd); napi_get_value_int32(env, argv[2], &ht);
+    napi_get_value_int32(env, argv[3], &cw); napi_get_value_int32(env, argv[4], &ch);
+    napi_get_value_uint32(env, argv[5], &kw); napi_get_value_bool(env, argv[6], &transparent);
+    napi_get_value_int32(env, argv[9], &dw); napi_get_value_int32(env, argv[10], &dh);
+    if (wd < 1 || ht < 1) { napi_throw_error(env, NULL, "bad capture size"); return NULL; }
+    fluid_postfx fx;
+    postfx_from(env, argv[7], &fx);
+    const float* dither;
+    if (!dither_from(env, kw, argv[8], dw, dh, &dither)) return NULL;
+    const size_t n = (size_t)wd * ht * 4;
+    void* data = NULL; napi_value ab, ta;
+    if (napi_create_arraybuffer(env, n, &data, &ab) != napi_ok) return NULL;
+    if (!check(env, w->h, fluid_capture(w->h, wd, ht, cw, ch, kw, transparent ? 1 : 0, &fx, dither, dw, dh,
+                                        (float)num(env, argv[11]), (float)num(env, argv[12]), (float)num(env, argv[13]),
+                                        (uint8_t*)data, n))) return NULL;
+    if (napi_create_typedarray(env, napi_uint8_array, n, ab, 0, &ta) != napi_ok) return NULL;
+    return ta;
 }
 
 static napi_value Sync(napi_env env, napi_callback_info info) {
@@ -370,6 +410,7 @@ NAPI_MODULE_INIT() {
         {"pressureSolveHost", NULL, PressureSolveHost, NULL, NULL, NULL, napi_enumerable, NULL},
         {"render", NULL, Render, NULL, NULL, NULL, napi_enumerable, NULL},
         {"renderKeywords", NULL, RenderKeywords, NULL, NULL, NULL, napi_enumerable, NULL},
+        {"capture", NULL, Capture, NULL, NULL, NULL, napi_enumerable, NULL},
         {"sync", NULL, Sync, NULL, NULL, NULL, napi_enumerable, NULL},
         {"stat", NULL, Stat, NULL, NULL, NULL, napi_enumerable, NULL},
         {"dims", NULL, Dims, NULL, NULL, NULL, napi_enumerable, NULL},

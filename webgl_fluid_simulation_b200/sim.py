@@ -22,7 +22,9 @@ from __future__ import annotations
 import ctypes as C
 import math
 import random as _random
+import struct
 import time
+import zlib
 
 import numpy as np
 
@@ -36,6 +38,7 @@ def default_config() -> dict:
     return {
         "SIM_RESOLUTION": 128,
         "DYE_RESOLUTION": 1024,
+        "CAPTURE_RESOLUTION": 512,   # S:62, captureScreenshot's target (S:288)
         "DENSITY_DISSIPATION": 1,
         "VELOCITY_DISSIPATION": 0.2,
         "PRESSURE": 0.8,
@@ -125,6 +128,38 @@ def postfx_inputs(config, dithering):
                 float(config["BLOOM_THRESHOLD"]), float(config["BLOOM_SOFT_KNEE"]), int(config["SUNRAYS_RESOLUTION"]),
                 float(config["SUNRAYS_WEIGHT"]))
     return kw, fx, dith
+
+
+def capture_inputs(config, canvas_w, canvas_h, dithering):
+    """What captureScreenshot (S:287-299) hands fluid_capture: the target size getResolution(CAPTURE_RESOLUTION)
+    of the canvas, the display keywords, config.TRANSPARENT, and the PostFX / dithering texture of
+    postfx_inputs (the dithering texture is required only with BLOOM)."""
+    res = getResolution(config["CAPTURE_RESOLUTION"], canvas_w, canvas_h)
+    kw, fx, dith = postfx_inputs(config, dithering)
+    return dict(width=res["width"], height=res["height"], keywords=kw, transparent=bool(config.get("TRANSPARENT")),
+                fx=fx, dither=dith)
+
+
+def write_png(path, rgba8) -> None:
+    """Writes an (h, w, 4) uint8 image, top row first, as an 8-bit RGBA PNG: signature, IHDR (colour type
+    6), one zlib IDAT with filter 0 on every row, IEND.  It stands in for toDataURL + downloadURI
+    (S:296-297).  The bytes are written as they are: browsers that keep 2-D canvases premultiplied change
+    RGB wherever alpha < 255 on the way through putImageData / toDataURL, which is browser-defined and
+    not emulated."""
+    img = np.ascontiguousarray(rgba8)
+    if img.dtype != np.uint8 or img.ndim != 3 or img.shape[2] != 4:
+        raise ValueError(f"write_png needs an (h, w, 4) uint8 image, got {img.dtype} {img.shape}")
+    h, w = img.shape[:2]
+
+    def chunk(tag, data):
+        return struct.pack(">I", len(data)) + tag + data + struct.pack(">I", zlib.crc32(tag + data) & 0xFFFFFFFF)
+
+    raw = np.concatenate([np.zeros((h, 1), np.uint8), img.reshape(h, 4 * w)], axis=1).tobytes()
+    with open(path, "wb") as f:
+        f.write(b"\x89PNG\r\n\x1a\n")
+        f.write(chunk(b"IHDR", struct.pack(">IIBBBBB", w, h, 8, 6, 0, 0, 0)))
+        f.write(chunk(b"IDAT", zlib.compress(raw, 6)))
+        f.write(chunk(b"IEND", b""))
 
 
 class _Field:
@@ -416,6 +451,27 @@ class FluidSimulation:
             self._h, w, h, kw, None if fx is None else C.byref(fx), ptr(dith),
             0 if dith is None else dith.shape[1], 0 if dith is None else dith.shape[0],
             bc["r"] / 255, bc["g"] / 255, bc["b"] / 255, ptr(out), out.size, ptr(self.last_bloom), ptr(self.last_sunrays)))
+        return out
+
+    def captureScreenshot(self, path=None) -> np.ndarray:
+        """captureScreenshot(), S:287-299: render() into an RGBA half-float target of
+        getResolution(CAPTURE_RESOLUTION) and normalizeTexture (S:309-327), all on the GPU.  Returns the
+        (h, w, 4) uint8 image, TOP row first.  The bloom and sunrays FBOs keep the canvas sizes, as in the
+        reference; config.TRANSPARENT stores the display bare (no checkerboard); BLOOM needs `sim.dithering`.
+        With `path`, also writes the image as a PNG (write_png: the bytes unchanged)."""
+        cfg = self.config
+        cw, ch = self.canvas["width"], self.canvas["height"]
+        a = capture_inputs(cfg, cw, ch, getattr(self, "dithering", None))
+        w, h, fx, dith = a["width"], a["height"], a["fx"], a["dither"]
+        bc = cfg["BACK_COLOR"]                               # normalizeColor, S:1599-1606
+        out = np.empty((h, w, 4), np.uint8)
+        ptr = lambda x: None if x is None else x.ctypes.data_as(C.c_void_p)   # noqa: E731
+        self._check(self._L.fluid_capture(
+            self._h, w, h, cw, ch, a["keywords"], 1 if a["transparent"] else 0, None if fx is None else C.byref(fx),
+            ptr(dith), 0 if dith is None else dith.shape[1], 0 if dith is None else dith.shape[0],
+            bc["r"] / 255, bc["g"] / 255, bc["b"] / 255, ptr(out), out.size))
+        if path is not None:
+            write_png(path, out)
         return out
 
     @staticmethod
