@@ -41,9 +41,6 @@ struct fluid {
     int device = 0;
     int sm_count = 132;
     cudaStream_t stream = nullptr;
-    cudaStream_t stream2 = nullptr;  // slab mode: halo exchange + boundary strips, overlapped with the interior launch
-    cudaStream_t active = nullptr;   // where halo / Jacobi launches go right now (== stream except inside that overlap)
-    cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
     cudaEvent_t mark[2] = {nullptr, nullptr};
     cudaEvent_t tev[8] = {};
     Pair velocity, dye, pressure;    // float2 / float4 / float
@@ -96,11 +93,6 @@ struct fluid {
     } peer[2];                       // [0] = rank-1 (below), [1] = rank+1 (above)
     bool p2p = false;
     uint32_t p2p_seq = 0;
-    // pressure ghost rows stored by the neighbours' last Jacobi launch (jacobi.cuh, TbSync): sequence number of
-    // the last mirrored solve, whether pressure.read's ghost rows still hold it, and how many rows deep
-    uint32_t mir_seq = 0;
-    bool p_mirror_valid = false;
-    int p_mirror_rows = 0;
     // fluid_pressure_solve_host pipelined over row bands (single GPU): copy streams, per-band events and the
     // band-private ping-pong rows of the intermediate launches
     struct HostPipe {
@@ -109,8 +101,6 @@ struct fluid {
         float* s[2] = {nullptr, nullptr};
         size_t s_floats = 0;
     } hp;
-    fk::TbSync tb_sync{};                      // hand-offs of the NEXT blocked launch (launch_tb: SYNC instantiation when tb_sync_on)
-    bool tb_sync_on = false;
     // divergence ghost rows of the exchange about to be issued: the peer-memory wait kernel scans them (halo.cuh)
     struct { const float* div; unsigned char* map; int W, row_off, lo0, hi0, lo1, hi1; } scan{};
     bool scan_pending = false;
@@ -238,7 +228,7 @@ int clear_tiny_map(fluid_t* h) {
 int scan_tiny(fluid_t* h, int j_lo, int j_hi) {
     if (j_hi <= j_lo) return FLUID_OK;
     dim3 b(256), g((h->cfg.sim_w + 255) / 256, j_hi - j_lo);
-    tiny_scan_kernel<<<g, b, 0, h->active>>>(h->divergence, h->tiny_map, h->cfg.sim_w, h->roff, j_lo, j_hi);
+    tiny_scan_kernel<<<g, b, 0, h->stream>>>(h->divergence, h->tiny_map, h->cfg.sim_w, h->roff, j_lo, j_hi);
     return check_launch(h, "tiny_scan_kernel");
 }
 
@@ -289,8 +279,7 @@ void build_tmaps(fluid_t* h) {
 // cp.async (LDGSTS) ring on an H100 SXM (700 W power limit) at 4096^2 x 50, K = 10 (0.446 vs 0.464 ms
 // per solve).  FLUID_TB_STAGE=ldgsts selects the ring (bit-identical results).  Row slabs (N > 1) keep
 // the ring unless FLUID_TB_STAGE=tma asks for the boxes.  Launches whose buffers the tensor maps do not
-// describe (the band-private rows of fluid_pressure_solve_host) and launches with slab hand-offs (the
-// SYNC instantiation) always use the ring: see launch_tb.
+// describe (the band-private rows of fluid_pressure_solve_host) always use the ring: see launch_tb.
 const char* tb_stage_env() {
     static const char* e = getenv("FLUID_TB_STAGE");
     return e ? e : "";
@@ -300,50 +289,33 @@ bool tb_use_tma(const fluid_t* h) {
     if (h->slab()) return !strcmp(tb_stage_env(), "tma");
     return strcmp(tb_stage_env(), "ldgsts") != 0;
 }
-// FLUID_HALO_MIRROR=1: the mirrored-halo schedule of run_jacobi (peer-memory transport, ring staging)
-bool halo_mirror_requested() {
-    static const bool on = getenv("FLUID_HALO_MIRROR") && !strcmp(getenv("FLUID_HALO_MIRROR"), "1");
-    return on;
-}
 
 template <int K, bool SCALE>
 int launch_tb(fluid_t* h, const JacobiArgs& a) {
     using T = TB<K>;
     const int nxw = (a.W + T::VALID - 1) / T::VALID;
-    int nch = (a.out_hi - a.out_lo + a.rows_per_chunk - 1) / a.rows_per_chunk;
-    if (a.nch1 > 0) nch = a.nch1 + (a.seg2_hi - a.seg2_lo + a.rows_per_chunk - 1) / a.rows_per_chunk;
+    const int nch = (a.out_hi - a.out_lo + a.rows_per_chunk - 1) / a.rows_per_chunk;
     TmapPair maps;
     memset(&maps, 0, sizeof maps);
     // chained to the previous launch of the same solve by programmatic dependent launch (jacobi.cuh);
-    // not while a graph is being captured, FLUID_PDL=0 turns it off
-    static const bool pdl_off = getenv("FLUID_PDL") && !strcmp(getenv("FLUID_PDL"), "0");
-    // tuning: run the SYNC instantiation everywhere (all hand-offs null) to time it against the plain one
-    static const bool force_sync = getenv("FLUID_TB_FORCE_SYNC") && !strcmp(getenv("FLUID_TB_FORCE_SYNC"), "1");
+    // not while a graph is being captured
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cudaLaunchConfig_t lc{};
-    lc.gridDim = dim3(nxw * nch); lc.blockDim = dim3(32); lc.stream = h->active;
-    // FLUID_PDL_GRAPH=1: also while a step graph is captured (the launch becomes a programmatic edge)
-    static const bool pdl_graph = getenv("FLUID_PDL_GRAPH") && !strcmp(getenv("FLUID_PDL_GRAPH"), "1");
-    lc.attrs = attr; lc.numAttrs = (h->pdl_chain && !pdl_off && (!h->capturing || pdl_graph)) ? 1 : 0;
+    lc.gridDim = dim3(nxw * nch); lc.blockDim = dim3(32); lc.stream = h->stream;   // one warp per CTA
+    lc.attrs = attr; lc.numAttrs = (h->pdl_chain && !h->capturing) ? 1 : 0;
     // the tensor maps address rows from the base of the mapped buffers, the kernel from a.pin / a.div
-    const bool tma = tb_use_tma(h) && !h->tb_sync_on && !force_sync && a.div == h->divergence &&
-                     (a.pin == h->tmaps.p_ptr[0] || a.pin == h->tmaps.p_ptr[1]);
+    const bool tma = tb_use_tma(h) && a.div == h->divergence && (a.pin == h->tmaps.p_ptr[0] || a.pin == h->tmaps.p_ptr[1]);
     if (tma) {
         const int k = (a.pin == h->tmaps.p_ptr[0]) ? 0 : 1;
         memcpy(maps.p, &h->tmaps.p[k], sizeof(CUtensorMap));
         memcpy(maps.d, &h->tmaps.d, sizeof(CUtensorMap));
         lc.dynamicSmemBytes = T::SMEM_TMA;
-        { TbArgs<false> ta; static_cast<JacobiArgs&>(ta) = a; cudaLaunchKernelEx(&lc, jacobi_tb_kernel<K, SCALE, true, false>, ta, maps); }   // one warp per CTA
-    } else if (h->tb_sync_on || force_sync) {         // slab launch with hand-offs (run_jacobi fills h->tb_sync)
-        lc.dynamicSmemBytes = T::SMEM_LDGSTS;
-        TbArgs<true> ta; static_cast<JacobiArgs&>(ta) = a; ta.sy = h->tb_sync;
-        cudaLaunchKernelEx(&lc, jacobi_tb_kernel<K, SCALE, false, true>, ta, maps);
+        cudaLaunchKernelEx(&lc, jacobi_tb_kernel<K, SCALE, true>, a, maps);
     } else {
         lc.dynamicSmemBytes = T::SMEM_LDGSTS;
-        TbArgs<false> ta; static_cast<JacobiArgs&>(ta) = a;
-        cudaLaunchKernelEx(&lc, jacobi_tb_kernel<K, SCALE, false, false>, ta, maps);
+        cudaLaunchKernelEx(&lc, jacobi_tb_kernel<K, SCALE, false>, a, maps);
     }
     ++h->jacobi_kernel_launches;
     return check_launch(h, "jacobi_tb_kernel");
@@ -357,16 +329,16 @@ int launch_tb_k(fluid_t* h, const JacobiArgs& a, bool scale) {
 // rows per warp stream: enough chunks that every SM holds its full complement of resident warps
 // (single wave), rounded so that a stream's step count R + 2K is a multiple of the unroll U.
 template <int K>
-int tb_rows(const fluid_t* h, int W, int rows, int reserve = 0) {
+int tb_rows(const fluid_t* h, int W, int rows) {
     if (h->jacobi_rows_override > 0) return h->jacobi_rows_override;
     using T = TB<K>;
     const int nxw = (W + T::VALID - 1) / T::VALID;
     int occ = 0;
-    if (tb_use_tma(h)) cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, jacobi_tb_kernel<K, false, true, false>, 32, T::SMEM_TMA);
-    else cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, jacobi_tb_kernel<K, false, false, false>, 32, T::SMEM_LDGSTS);
+    if (tb_use_tma(h)) cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, jacobi_tb_kernel<K, false, true>, 32, T::SMEM_TMA);
+    else cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, jacobi_tb_kernel<K, false, false>, 32, T::SMEM_LDGSTS);
     if (occ < 1) occ = 1;
     if (h->jacobi_warps_per_sm > 0) occ = std::min(occ, h->jacobi_warps_per_sm);
-    const int resident_warps = std::max(nxw, h->sm_count * occ - reserve);
+    const int resident_warps = std::max(nxw, h->sm_count * occ);
     const int nch = std::max(1, resident_warps / nxw);
     int r = (rows + nch - 1) / nch;
     r = std::max(r, 4 * K);                 // keep the 2K warm-up rows a bounded fraction
@@ -376,12 +348,10 @@ int tb_rows(const fluid_t* h, int W, int rows, int reserve = 0) {
     return std::min(r, rows);
 }
 
-// rows_fixed > 0: use that chunk height (the boundary strips of a slab are one chunk each);
-// reserve: resident streams to leave free on the chip (for a launch that runs beside this one)
-int launch_tb_dyn(fluid_t* h, int K, JacobiArgs a, bool scale, int rows_fixed = 0, int reserve = 0) {
+int launch_tb_dyn(fluid_t* h, int K, JacobiArgs a, bool scale) {
     const int rows = a.out_hi - a.out_lo;
     switch (K) {
-#define CASE(KK) case KK: a.rows_per_chunk = rows_fixed > 0 ? rows_fixed : tb_rows<KK>(h, a.W, rows, reserve); return launch_tb_k<KK>(h, a, scale);
+#define CASE(KK) case KK: a.rows_per_chunk = tb_rows<KK>(h, a.W, rows); return launch_tb_k<KK>(h, a, scale);
         CASE(1) CASE(2) CASE(3) CASE(4) CASE(5) CASE(6) CASE(7) CASE(8) CASE(9) CASE(10) CASE(11) CASE(12)
 #undef CASE
     }
@@ -399,8 +369,6 @@ bool tb_eligible(const fluid_t* h) {
 // message of its own); divergence ghosts are exchanged once per solve (it is constant in the loop).
 int run_jacobi(fluid_t* h, int iters, bool scale_first, int* launches_out) {
     int nl = 0;
-    const bool p_ghosts_mirrored = h->p_mirror_valid;    // every path below rewrites pressure
-    h->p_mirror_valid = false;
     const int W = h->cfg.sim_w, H = h->cfg.sim_h;
     JacobiArgs a{};
     a.div = h->divergence; a.W = W; a.H = H; a.row_off = h->roff; a.out_lo = h->row0; a.out_hi = h->row1;
@@ -454,54 +422,29 @@ int run_jacobi(fluid_t* h, int iters, bool scale_first, int* launches_out) {
     // one latency-bound message per launch).  If the ghost zone is too thin for that (iterations
     // raised after creation) fall back to one K-row message per launch.
     const bool deep = h->slab() && (iters + 1 <= h->G) && (iters + 1 <= h->row1 - h->row0);
-    // Optional overlap (deep + blocked, either transport): the exchange and the two boundary strips of
-    // launch 1 — the only rows of it that read ghost rows — go to a second stream, the interior rows
-    // [row0+K1, row1-K1) of launch 1 run meanwhile on the compute stream.
-    // Default OFF (the split adds a second stream, an event pair and a second launch to every solve);
-    // FLUID_HALO_OVERLAP=1 enables it.
-    static const bool overlap_off = !(getenv("FLUID_HALO_OVERLAP") && !strcmp(getenv("FLUID_HALO_OVERLAP"), "1"));
-    const int K1 = base + (extra ? 1 : 0);
-    const bool overlap = deep && blocked && !overlap_off && h->stream2 && (h->row1 - h->row0) >= 2 * K1 + 4 * K1;
-    // Peer-memory transport, two or more blocked launches: the last launch of this solve stores the pressure
-    // rows the neighbours need next time into their ghost rows itself (TbSync in jacobi.cuh), and if the
-    // previous solve did so — nothing wrote pressure since — this solve starts without a pressure message.
-    // FLUID_HALO_MIRROR=1 enables it (default: the explicit exchange); fluid_create_slab refuses it together
-    // with FLUID_TB_STAGE=tma, whose launches cannot carry the hand-offs.
-    const bool mirror = deep && blocked && h->p2p && nlaunch >= 2 && halo_mirror_requested() && !overlap && !tb_use_tma(h);
-    const bool p_in_place = mirror && p_ghosts_mirrored && h->p_mirror_rows >= iters + 1;
-    unsigned* const my_flags = h->slab() ? (unsigned*)(h->arena + h->off_flags) : nullptr;
-    auto peer_flags = [&](int side) { return (unsigned*)(h->peer[side].base + h->peer[side].off_flags); };
     if (h->slab()) {
-        if (overlap) {
-            CU(cudaEventRecord(h->ev_fork, h->stream));
-            CU(cudaStreamWaitEvent(h->stream2, h->ev_fork, 0));
-            h->active = h->stream2;
-        }
         if (deep) {
-            const HaloItem itp = {h->pressure.read, (size_t)W * sizeof(float), h->roff, h->row0, h->row1, iters + 1, HB_PRESSURE};
-            const HaloItem itd = {h->divergence, (size_t)W * sizeof(float), h->roff, h->row0, h->row1, iters, HB_DIVERGENCE};
             // divergence is constant during a solve and often across solves (a host that iterates the solve on
             // one right-hand side, bench.py's loop): its ghost rows — and their tiny-value flags — are still in
             // place unless some pass rewrote divergence since they were last received (SPMD-identical decision)
             const bool send_div = h->div_sent_epoch != h->div_epoch || h->div_sent_rows < iters;
-            HaloItem it[2];
-            int nitems = 0;
-            if (!p_in_place) it[nitems++] = itp;
-            if (send_div) it[nitems++] = itd;
+            const HaloItem it[2] = {
+                {h->pressure.read, (size_t)W * sizeof(float), h->roff, h->row0, h->row1, iters + 1, HB_PRESSURE},
+                {h->divergence, (size_t)W * sizeof(float), h->roff, h->row0, h->row1, iters, HB_DIVERGENCE}};
             // the neighbours' divergence rows get their tiny values flagged like the local producers do:
             // inside the wait kernel on the peer-memory path, by a scan kernel after the NCCL group
             h->scan.div = h->divergence; h->scan.map = h->tiny_map; h->scan.W = W; h->scan.row_off = h->roff;
             h->scan.lo0 = std::max(h->row0 - iters, 0); h->scan.hi0 = h->row0;
             h->scan.lo1 = h->row1; h->scan.hi1 = std::min(h->row1 + iters, H);
             h->scan_pending = h->p2p && send_div;
-            int rc = nitems ? exchange_many(h, it, nitems) : FLUID_OK;
+            int rc = exchange_many(h, it, send_div ? 2 : 1);
             if (send_div) { h->div_sent_epoch = h->div_epoch; h->div_sent_rows = iters; }
             if (!rc && !h->p2p && send_div) {
                 rc = scan_tiny(h, h->scan.lo0, h->scan.hi0);
                 if (!rc) rc = scan_tiny(h, h->scan.lo1, h->scan.hi1);
             }
             h->scan_pending = false;
-            if (rc) { h->active = h->stream; return rc; }
+            if (rc) return rc;
         } else {
             const int kmax = base + (extra ? 1 : 0);
             int rc = exchange_rows(h, HB_DIVERGENCE, h->divergence, (size_t)W * sizeof(float), h->roff, h->row0, h->row1, kmax);
@@ -528,65 +471,15 @@ int run_jacobi(fluid_t* h, int iters, bool scale_first, int* launches_out) {
             }
             a.out_lo = std::max(h->row0 - ext, 0); a.out_hi = std::min(h->row1 + ext, H);
         }
-        h->tb_sync = TbSync{}; h->tb_sync_on = false;
-        if (mirror) {
-            const unsigned seq = h->mir_seq + 1;
-            h->tb_sync_on = (k == 0 && p_in_place) || k == nlaunch - 2 || last;
-            static const bool dbg = getenv("FLUID_DEBUG_HALO_TIMING") != nullptr;
-            if (dbg) h->tb_sync.dbg = (unsigned long long*)(h->arena + h->off_flags + 512);
-            h->tb_sync.own_lo = h->row0; h->tb_sync.own_hi = h->row1;
-            if (k == 0 && p_in_place) {                          // wait for the previous solve's mirrored rows
-                for (int s = 0; s < 2; ++s)
-                    if (h->peer[s].present) h->tb_sync.pre_wait[s] = my_flags + 66 + s;
-                h->tb_sync.pre_seq = h->mir_seq;
-            }
-            if (k == nlaunch - 2) {                              // last reader of the ghost rows the neighbours will overwrite
-                h->tb_sync.ticket = my_flags + 72;
-                for (int s = 0; s < 2; ++s)
-                    if (h->peer[s].present) h->tb_sync.done_flag[s] = peer_flags(s) + (s == 0 ? 65 : 64);
-                h->tb_sync.done_seq = seq;
-            }
-            if (last) {
-                const int pidx = ((char*)h->pressure.write == h->arena + h->off_p[0]) ? 0 : 1;
-                for (int s = 0; s < 2; ++s) {
-                    const fluid::Peer& P = h->peer[s];
-                    if (!P.present) continue;
-                    h->tb_sync.mirror[s] = (float*)(P.base + P.off_p[pidx]) - (ptrdiff_t)P.roff * W;
-                    h->tb_sync.mir_lo[s] = s == 0 ? h->row0 : h->row1 - (iters + 1);
-                    h->tb_sync.mir_hi[s] = s == 0 ? h->row0 + (iters + 1) : h->row1;
-                    h->tb_sync.mir_wait[s] = my_flags + 64 + s;
-                    h->tb_sync.done_flag[s] = peer_flags(s) + (s == 0 ? 67 : 66);
-                }
-                h->tb_sync.mir_seq = seq; h->tb_sync.ticket = my_flags + 73; h->tb_sync.done_seq = seq;
-            }
-        }
         const bool sc = scale_first && k == 0;
         int rc;
-        if (blocked && overlap && k == 0) {
-            // boundary strips [out_lo, row0+K) and [row1-K, out_hi) behind the exchange on stream2 ...
-            const int nxw = (W + 127) / 128 + 8;             // upper bound of the strips' stream count (any K)
-            JacobiArgs bnd = a;
-            bnd.out_lo = a.out_lo; bnd.out_hi = std::min(h->row0 + K, a.out_hi);
-            bnd.seg2_lo = std::max(h->row1 - K, bnd.out_hi); bnd.seg2_hi = a.out_hi;
-            const int strip = std::max(bnd.out_hi - bnd.out_lo, bnd.seg2_hi - bnd.seg2_lo);
-            bnd.nch1 = 1;
-            rc = launch_tb_dyn(h, K, bnd, sc, strip);        // h->active == stream2
-            h->active = h->stream;
-            if (rc) return rc;
-            CU(cudaEventRecord(h->ev_join, h->stream2));
-            // ... the interior meanwhile on the compute stream, sized to leave the strips' slots free
-            JacobiArgs in = a;
-            in.out_lo = bnd.out_hi; in.out_hi = bnd.seg2_lo;
-            rc = launch_tb_dyn(h, K, in, sc, 0, 2 * nxw);
-            if (rc) return rc;
-            CU(cudaStreamWaitEvent(h->stream, h->ev_join, 0));
-        } else if (blocked) {
+        if (blocked) {
             // programmatic dependent launch: behind another blocked launch of this solve, and — first launch —
             // behind whatever kernel precedes it on the stream (the previous solve's last launch in a host loop
             // of solves; a kernel without griddepcontrol.launch_dependents simply triggers at its end)
-            h->pdl_chain = !(overlap && k <= 1);
+            h->pdl_chain = true;
             rc = launch_tb_dyn(h, K, a, sc);
-            h->pdl_chain = false; h->tb_sync_on = false;
+            h->pdl_chain = false;
         } else if (tb_eligible(h)) {
             dim3 b(32, 8);
             dim3 g((W / 4 + b.x - 1) / b.x, (a.out_hi - a.out_lo + b.y - 1) / b.y);
@@ -603,7 +496,6 @@ int run_jacobi(fluid_t* h, int iters, bool scale_first, int* launches_out) {
         if (rc) return rc;
         swap_p(h); ++nl;
     }
-    if (mirror) { ++h->mir_seq; h->p_mirror_valid = true; h->p_mirror_rows = iters + 1; }
     if (launches_out) *launches_out = nl;
     return FLUID_OK;
 }
@@ -771,10 +663,6 @@ int create_common(const fluid_config* cfg, int rank, int world, const void* uid,
         int rc = fail(nullptr, FLUID_ERR_INVALID, "FLUID_FLAG_HALF_STORAGE is a single-GPU mode");
         delete h; return rc;
     }
-    if (world > 1 && halo_mirror_requested() && !strcmp(tb_stage_env(), "tma")) {
-        int rc = fail(nullptr, FLUID_ERR_INVALID, "FLUID_HALO_MIRROR=1 needs the cp.async staging: unset FLUID_TB_STAGE=tma");
-        delete h; return rc;
-    }
     if (!slab_geometry(h, cfg->sim_h, cfg->dye_h, cfg->pressure_iterations)) {
         int rc = fail(nullptr, FLUID_ERR_INVALID, "slabs of %d rows are too short for a 14-row halo: use fewer GPUs", cfg->sim_h / world);
         delete h; return rc;
@@ -783,12 +671,6 @@ int create_common(const fluid_config* cfg, int rank, int world, const void* uid,
     if (const char* e = getenv("FLUID_JACOBI_WARPS")) h->jacobi_warps_per_sm = atoi(e);
     auto body = [&]() -> int {
         CU(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
-        h->active = h->stream;
-        if (world > 1) {
-            CU(cudaStreamCreateWithFlags(&h->stream2, cudaStreamNonBlocking));
-            CU(cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming));
-            CU(cudaEventCreateWithFlags(&h->ev_join, cudaEventDisableTiming));
-        }
         for (auto& e : h->mark) CU(cudaEventCreate(&e));
         for (auto& e : h->tev) CU(cudaEventCreate(&e));
         CU(cudaMalloc((void**)&h->halo_flag, sizeof(int)));
@@ -924,7 +806,7 @@ int fluid_p2p_disable(fluid_t* h) {
     if (!h) return FLUID_ERR_INVALID;
     if (h->stream) CU(cudaStreamSynchronize(h->stream));
     for (auto& p : h->peer) if (p.present && p.base) { cudaIpcCloseMemHandle(p.base); p.base = nullptr; p.present = false; }
-    h->p2p = false; h->p_mirror_valid = false;
+    h->p2p = false;
     return FLUID_OK;
 }
 
@@ -933,19 +815,6 @@ void fluid_destroy(fluid_t* h) {
     cudaSetDevice(h->device);
     if (h->stream) cudaStreamSynchronize(h->stream);
     drop_graphs(h);
-    if (h->p2p && getenv("FLUID_DEBUG_HALO_TIMING")) {
-        unsigned long long d[5] = {};
-        cudaMemcpy(d, h->arena + h->off_flags + 128, sizeof d, cudaMemcpyDeviceToHost);
-        unsigned long long m[9] = {};
-        cudaMemcpy(m, h->arena + h->off_flags + 512, sizeof m, cudaMemcpyDeviceToHost);
-        if (m[6] || m[8])
-            fprintf(stderr, "[mirror rank %d] streams that waited for mirror-ready: %llu, avg %.1f us; mirroring warps: %llu, waited %.1f us for done-reading, "
-                            "copied for %.1f us; stream life (hand-off launches): %.1f us touching ghost rows (%llu), %.1f us others (%llu)\n",
-                    h->rank, m[1], m[1] ? m[0] / 1e3 / m[1] : 0.0, m[4], m[4] ? m[2] / 1e3 / m[4] : 0.0, m[4] ? m[3] / 1e3 / m[4] : 0.0,
-                    m[6] ? m[5] / 1e3 / m[6] : 0.0, m[6], m[8] ? m[7] / 1e3 / m[8] : 0.0, m[8]);
-        if (d[3]) fprintf(stderr, "[halo rank %d] exchanges %llu: wait-free %.1f us, push (start->published) %.1f us, wait-ready %.1f us\n",
-                          h->rank, d[3], d[0] / 1e3 / d[3], d[1] / 1e3 / d[3], d[2] / 1e3 / d[3]);
-    }
     free_fields(h);
     cudaFree(h->halo_flag);
     cudaFree(h->dt_dev);
@@ -961,9 +830,6 @@ void fluid_destroy(fluid_t* h) {
     for (auto& e : h->hp.ev_up) if (e) cudaEventDestroy(e);
     for (auto& e : h->hp.ev_done) if (e) cudaEventDestroy(e);
     cudaFree(h->hp.s[0]); cudaFree(h->hp.s[1]);
-    if (h->ev_fork) cudaEventDestroy(h->ev_fork);
-    if (h->ev_join) cudaEventDestroy(h->ev_join);
-    if (h->stream2) { cudaStreamSynchronize(h->stream2); cudaStreamDestroy(h->stream2); }
     if (h->stream) cudaStreamDestroy(h->stream);
     delete h;
 }
@@ -1417,7 +1283,7 @@ int fluid_resize(fluid_t* h, int sim_w, int sim_h, int dye_w, int dye_h) {
         char* old_arena = h->arena; const float2* old_v = (const float2*)h->velocity.read; const float4* old_d = (const float4*)h->dye.read;
         const int old_roff = h->roff, old_droff = h->droff;
         for (auto& p : h->peer) if (p.present && p.base) { cudaIpcCloseMemHandle(p.base); p.base = nullptr; p.present = false; }
-        h->p2p = false; h->p_mirror_valid = false;
+        h->p2p = false;
         h->arena = nullptr;
         h->cfg.sim_w = sim_w; h->cfg.sim_h = sim_h; h->cfg.dye_w = dye_w; h->cfg.dye_h = dye_h;
         if (!slab_geometry(h, sim_h, dye_h, h->cfg.pressure_iterations)) {
@@ -1568,7 +1434,6 @@ int fluid_write(fluid_t* h, int field, const float* host, size_t n_floats) {
     CU(cudaMemcpyAsync(p, host, n * sizeof(float), cudaMemcpyHostToDevice, h->stream));
     CU(cudaStreamSynchronize(h->stream));
     if (field == FLUID_FIELD_VELOCITY) h->v_ghost_valid = false;   // ghosts rebuilt by the next step
-    if (field == FLUID_FIELD_PRESSURE) h->p_mirror_valid = false;  // the neighbours' ghost copies are stale now
     if (field == FLUID_FIELD_DIVERGENCE) {                          // host-provided divergence: rebuild the map
         int rc = clear_tiny_map(h); if (rc) return rc;
         if ((rc = scan_tiny(h, h->row0, h->row1))) return rc;
@@ -1608,7 +1473,6 @@ int solve_host_banded(fluid_t* h, const float* div_host, float* p_host, int iter
     }
     float* const p_in = (float*)h->pressure.read;
     float* const result = (float*)h->pressure.write;
-    h->p_mirror_valid = false;
     int rc = clear_tiny_map(h); if (rc) return rc;
     CU(cudaEventRecord(hp.ev_start, h->stream));          // the copies overwrite fields earlier work on the stream may still read
     CU(cudaStreamWaitEvent(hp.up, hp.ev_start, 0));
@@ -1677,7 +1541,6 @@ int fluid_pressure_solve_host(fluid_t* h, const float* div_host, float* p_host, 
     // make the copies asynchronous DMA.  Either way all three copies are inside this call.
     CU(cudaMemcpyAsync(h->divergence + go, div_host, n * sizeof(float), cudaMemcpyHostToDevice, h->stream));
     CU(cudaMemcpyAsync((float*)h->pressure.read + go, p_host, n * sizeof(float), cudaMemcpyHostToDevice, h->stream));
-    h->p_mirror_valid = false;
     int rc = clear_tiny_map(h); if (rc) return rc;
     if ((rc = scan_tiny(h, h->row0, h->row1))) return rc;
     rc = run_jacobi(h, iters, true, nullptr); if (rc) return rc;

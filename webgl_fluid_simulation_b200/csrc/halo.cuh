@@ -25,11 +25,26 @@ struct PushArgs {
     int present[2];
     unsigned* counter;         // block-completion counter (local)
     int* err;                  // set when a bounded spin times out (reported as FLUID_ERR_HALO)
-    unsigned long long* dbg;   // FLUID_DEBUG_HALO_TIMING: [0] sum wait-free ns [1] sum push ns [2] sum wait-ready ns [3] count [4] t_start
     ScanArgs scan;             // divergence ghost strips to scan for tiny values once they have arrived (W == 0: none)
 };
 
-using fk::ld_acquire_sys; using fk::st_release_sys; using fk::global_ns; using fk::spin_until;   // jacobi.cuh
+__device__ __forceinline__ unsigned ld_acquire_sys(const unsigned* p) {
+    unsigned v; asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return v;
+}
+__device__ __forceinline__ void st_release_sys(unsigned* p, unsigned v) {
+    asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+__device__ __forceinline__ unsigned long long global_ns() {
+    unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); return t;
+}
+// bounded spin: a neighbour that never arrives costs 4 s and an error flag, never a hung GPU
+__device__ __forceinline__ void spin_until(const unsigned* flag, unsigned seq, int* err) {
+    const unsigned long long t0 = global_ns();
+    while ((int)(ld_acquire_sys(flag) - seq) < 0) {
+        if (global_ns() - t0 > 4000000000ull) { *err = 2; break; }
+        __nanosleep(100);
+    }
+}
 
 // One halo exchange in ONE kernel, producer and consumer side:
 //   (a) tell the neighbours my ghost rows may be overwritten (this kernel is stream-ordered after
@@ -39,15 +54,12 @@ using fk::ld_acquire_sys; using fk::st_release_sys; using fk::global_ns; using f
 //       done, release-store "ready = seq" into the neighbours' flag words.
 __global__ void __launch_bounds__(256) halo_push_kernel(PushArgs a) {
     if (threadIdx.x == 0) {
-        unsigned long long t0 = 0;
         if (blockIdx.x == 0) {
-            if (a.dbg) { t0 = global_ns(); a.dbg[4] = t0; }
             for (int side = 0; side < 2; ++side)
                 if (a.present[side]) st_release_sys(a.peer_flags[side] + (side == 0 ? 3 : 2), a.seq);
         }
         for (int side = 0; side < 2; ++side)
             if (a.present[side]) spin_until(a.my_flags + (side == 0 ? 2 : 3), a.seq, a.err);
-        if (blockIdx.x == 0 && a.dbg) atomicAdd(a.dbg + 0, global_ns() - t0);
     }
     __syncthreads();
     for (int k = 0; k < a.count; ++k) {
@@ -67,16 +79,13 @@ __global__ void __launch_bounds__(256) halo_push_kernel(PushArgs a) {
             __threadfence_system();
             for (int side = 0; side < 2; ++side)
                 if (a.present[side]) st_release_sys(a.peer_flags[side] + (side == 0 ? 1 : 0), a.seq);
-            if (a.dbg) { atomicAdd(a.dbg + 1, global_ns() - a.dbg[4]); atomicAdd(a.dbg + 3, 1ull); }
         }
     }
     // (e) consumer side in the SAME kernel (every block is resident: the grid is at most 2 blocks per SM):
     // acquire the neighbours' "ready" words, then (f) flag tiny values in the divergence strips that arrived.
     if (threadIdx.x == 0) {
-        const unsigned long long t0 = (a.dbg && blockIdx.x == 0) ? global_ns() : 0;
         if (a.present[0]) spin_until(a.my_flags + 0, a.seq, a.err);
         if (a.present[1]) spin_until(a.my_flags + 1, a.seq, a.err);
-        if (a.dbg && blockIdx.x == 0) atomicAdd(a.dbg + 2, global_ns() - t0);
     }
     __syncthreads();
     if (a.scan.W > 0) {
@@ -97,8 +106,6 @@ int exchange_p2p(fluid_t* h, const HaloItem* it, int count) {
     pa.my_flags = (unsigned*)(h->arena + h->off_flags);
     pa.counter = pa.my_flags + 8;
     pa.err = h->halo_flag;
-    static const bool dbg = getenv("FLUID_DEBUG_HALO_TIMING") != nullptr;
-    pa.dbg = dbg ? (unsigned long long*)(h->arena + h->off_flags + 128) : nullptr;
     unsigned long long total4 = 0;
     for (int side = 0; side < 2; ++side) {
         pa.present[side] = h->peer[side].present ? 1 : 0;
@@ -131,7 +138,7 @@ int exchange_p2p(fluid_t* h, const HaloItem* it, int count) {
         pa.scan = ScanArgs{h->scan.div, h->scan.map, h->scan.W, h->scan.row_off, h->scan.lo0, h->scan.hi0, h->scan.lo1, h->scan.hi1};
         h->scan_pending = false;
     }
-    halo_push_kernel<<<blocks, 256, 0, h->active>>>(pa);     // push + handshake + wait + scan: one launch per exchange
+    halo_push_kernel<<<blocks, 256, 0, h->stream>>>(pa);     // push + handshake + wait + scan: one launch per exchange
     int rc = check_launch(h, "halo_push_kernel"); if (rc) return rc;
     h->halo_kernel_launches += 1;
     ++h->halo_groups;
@@ -144,8 +151,6 @@ int exchange_many(fluid_t* h, const HaloItem* it, int count) {
         if (it[k].n > it[k].r1 - it[k].r0)
             return fail(h, FLUID_ERR_HALO, "halo of %d rows exceeds the slab height %d (use fewer GPUs or a taller grid)",
                         it[k].n, it[k].r1 - it[k].r0);
-    static const bool skip = getenv("FLUID_DEBUG_SKIP_HALO") != nullptr;   // TIMING EXPERIMENTS ONLY: wrong results
-    if (skip) return FLUID_OK;
     if (h->p2p) return exchange_p2p(h, it, count);
     ncdl::Api& N = ncdl::api();
     int rc = N.GroupStart();
@@ -156,12 +161,12 @@ int exchange_many(fluid_t* h, const HaloItem* it, int count) {
         auto at = [&](int grow) { return b + (size_t)(grow - q.off) * q.row_bytes; };
         const size_t bytes = (size_t)q.n * q.row_bytes;
         if (h->rank + 1 < h->world) {
-            if (!rc) rc = N.Send(at(q.r1 - q.n), bytes, ncdl::ncclInt8, h->rank + 1, h->comm, h->active);
-            if (!rc) rc = N.Recv(at(q.r1), bytes, ncdl::ncclInt8, h->rank + 1, h->comm, h->active);
+            if (!rc) rc = N.Send(at(q.r1 - q.n), bytes, ncdl::ncclInt8, h->rank + 1, h->comm, h->stream);
+            if (!rc) rc = N.Recv(at(q.r1), bytes, ncdl::ncclInt8, h->rank + 1, h->comm, h->stream);
         }
         if (h->rank > 0) {
-            if (!rc) rc = N.Send(at(q.r0), bytes, ncdl::ncclInt8, h->rank - 1, h->comm, h->active);
-            if (!rc) rc = N.Recv(at(q.r0 - q.n), bytes, ncdl::ncclInt8, h->rank - 1, h->comm, h->active);
+            if (!rc) rc = N.Send(at(q.r0), bytes, ncdl::ncclInt8, h->rank - 1, h->comm, h->stream);
+            if (!rc) rc = N.Recv(at(q.r0 - q.n), bytes, ncdl::ncclInt8, h->rank - 1, h->comm, h->stream);
         }
     }
     const int rc2 = N.GroupEnd();

@@ -33,71 +33,6 @@
 
 namespace fk {
 
-// ---- cross-GPU hand-offs of a slab solve (peer-memory transport; everything null on one GPU) ------
-__device__ __forceinline__ unsigned ld_acquire_sys(const unsigned* p) {
-    unsigned v; asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return v;
-}
-__device__ __forceinline__ void st_release_sys(unsigned* p, unsigned v) {
-    asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-__device__ __forceinline__ unsigned long long global_ns() {
-    unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); return t;
-}
-// bounded spin: a neighbour that never arrives costs 4 s and an error flag, never a hung GPU
-__device__ __forceinline__ void spin_until(const unsigned* flag, unsigned seq, int* err) {
-    const unsigned long long t0 = global_ns();
-    while ((int)(ld_acquire_sys(flag) - seq) < 0) {
-        if (global_ns() - t0 > 4000000000ull) { *err = 2; break; }
-        __nanosleep(100);
-    }
-}
-
-// The LAST blocked launch of a solve stores the rows its neighbours will need as ghost rows of the
-// NEXT solve straight into their arenas (NVLink stores from the compute kernel: no separate message,
-// no exchange kernel between two solves), guarded by two flag hand-offs:
-//   * "done reading": the neighbour's PENULTIMATE launch was the last reader of the ghost rows about
-//     to be overwritten (same ping-pong buffer); its last CTA to finish release-stores the solve's
-//     sequence number into my flag word, and my mirroring warps acquire it first;
-//   * "mirror ready": my last CTA to finish release-stores the sequence number into the neighbour's
-//     flag word; the streams of its next first launch that read ghost rows acquire it first.
-// The same wait for a whole (converged, one-warp-CTA) warp: lane 0 polls, a vote carries the outcome — one
-// request per poll instead of 32, and no lane-dependent branch (see tb_mirror for why that matters here).
-// Each lane then performs its own acquire load of the flag before it touches what the flag guards.
-__device__ __forceinline__ void warp_spin_until(const unsigned* flag, unsigned seq, int* err) {
-    const unsigned long long t0 = global_ns();
-    const unsigned l0 = (threadIdx.x == 0) ? 1u : 0u;
-    for (;;) {
-        unsigned v = seq;
-        asm volatile("{ .reg .pred q; setp.ne.u32 q, %2, 0; @q ld.acquire.sys.global.u32 %0, [%1]; }" : "+r"(v) : "l"(flag), "r"(l0) : "memory");
-        if (!__any_sync(0xffffffffu, (int)(v - seq) < 0)) break;
-        if (global_ns() - t0 > 4000000000ull) { *err = 2; break; }      // all lanes agree within a poll or two; the store is idempotent
-        __nanosleep(200);
-    }
-    // every lane's own acquire of the (now satisfied) flag — not a fence: MEMBAR.SYS would first drain the rows
-    // this warp has just stored
-    (void)ld_acquire_sys(flag);
-}
-
-struct TbSync {
-    const unsigned* pre_wait[2];   // [0] below, [1] above: streams reading rows outside [own_lo, own_hi) wait for *flag >= pre_seq
-    unsigned pre_seq;
-    int own_lo, own_hi;
-    float* mirror[2];              // neighbour's copy of pout, offset so that GLOBAL row j starts at mirror + j*W
-    int mir_lo[2], mir_hi[2];      // global rows [lo, hi) of mine the neighbour on that side keeps as ghost rows
-    const unsigned* mir_wait[2];   // "done reading" words (local), value mir_seq
-    unsigned mir_seq;
-    unsigned* ticket;              // CTA completion counter (local); null: this launch signals nothing
-    unsigned* done_flag[2];        // words in the neighbours' arenas that receive done_seq when the whole grid is done
-    unsigned done_seq;
-    // FLUID_DEBUG_HALO_TIMING: u64 sums — [0] ns streams waited for "mirror ready", [1] such streams, [2] ns mirroring
-    // warps waited for "done reading", [3] ns they spent copying, [4] such warps, [5] / [6] ns and count of streams
-    // touching ghost rows (whole life), [7] / [8] of the other streams
-    unsigned long long* dbg;
-};
-__device__ __forceinline__ void dbg_add(unsigned long long* p, unsigned long long v, bool on) {   // predicated, no branch (see tb_mirror)
-    asm volatile("{ .reg .pred q; setp.ne.u32 q, %2, 0; @q red.global.add.u64 [%0], %1; }" ::"l"(p), "l"(v), "r"((unsigned)on) : "memory");
-}
-
 struct JacobiArgs {
     const float* pin;    // local row 0 of the source pressure buffer
     const float* div;    // local row 0 of divergence
@@ -109,18 +44,7 @@ struct JacobiArgs {
     float scale;         // SCALE: value of config.PRESSURE
     int* err;            // device error word (3 = a bounded mbarrier wait gave up)
     const unsigned char* tiny_map;   // tb kernel: where divergence defeats the fma contraction (may be null)
-    // tb kernel, optional SECOND row range of the same launch (the two boundary strips of a slab, which
-    // wait for the halo while the interior runs): chunks 0..nch1-1 tile [out_lo, out_hi), the rest
-    // tile [seg2_lo, seg2_hi).  nch1 <= 0: single range.
-    int nch1, seg2_lo, seg2_hi;
 };
-// kernel argument block: the hand-offs exist only in the SYNC instantiation.  The single-GPU kernel must
-// not pay for slab plumbing: with TbSync inside JacobiArgs and the null checks compiled into the one
-// kernel, the single-GPU kernel grows and its hot loop moves.  (A derived struct, not a
-// separate kernel parameter: with the latter ptxas gave up the converged-warp assumption of the hot
-// loops — shuffles with BRA.DIV scaffolding, a fifth copy of the block body.)
-template <bool SYNC> struct TbArgs : JacobiArgs {};
-template <> struct TbArgs<true> : JacobiArgs { TbSync sy; };
 
 // the two tensor maps a temporally blocked launch reads through (TMA staging); 64-byte aligned
 // CUtensorMap images, passed by value as a __grid_constant__ kernel parameter
@@ -206,7 +130,8 @@ __global__ void __launch_bounds__(256) jacobi_sweep_kernel(JacobiArgs a) {
 //     mbarrier and fetches a 128-column x 3-row box of p and of div per pipeline block; columns
 //     outside the grid and rows outside the buffer are zero-filled by the hardware (never used
 //     by a valid output); or
-//   * LDGSTS: by per-lane 16-byte cp.async (the generation-5 path, kept selectable).
+//   * LDGSTS: by per-lane 16-byte cp.async (the generation-5 path): the default of row slabs, and
+//     the only staging of launches whose buffers the tensor maps do not describe.
 template <int K>
 struct TB {
     static constexpr int HX = (K + 3) / 4 * 4;       // x halo (columns) on each side of a window
@@ -555,73 +480,6 @@ __device__ FLUID_TB_EXACT_ATTR void tb_stream_exact(const JacobiArgs& a, const v
     else tb_stream<K, SCALE, false, true, TMA>(a, tm_p, tm_d, smem4, lane, x0, lc, gx, rev, lane_out, y0, y1, ys, ye);
 }
 
-// Slab epilogue of a stream (last launch of a solve): copy the rows this warp just produced that lie in
-// a neighbour's ghost zone into the neighbour's buffer.  The warp re-reads its own stores (same
-// thread, same address: program order), waits for the neighbour's "done reading" first.
-// Written WITHOUT lane-dependent control flow (predicated PTX instead of if (lane ...)): code that may
-// diverge after the stream makes the compiler drop its "this one-warp CTA is always converged"
-// assumption for the whole kernel, and the shuffles of the hot loops get divergence scaffolding.
-__device__ __forceinline__ void st_v4_if(float4* p, const float4 v, const bool on) {
-    asm volatile("{ .reg .pred q; setp.ne.u32 q, %5, 0; @q st.global.v4.f32 [%0], {%1, %2, %3, %4}; }"
-                 ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w), "r"((unsigned)on) : "memory");
-}
-__device__ __forceinline__ void tb_mirror(const JacobiArgs& a, const TbSync& sy, const int gx, const bool lane_out, const int y0, const int y1) {
-    const int W4 = a.W >> 2;
-    const int col = lane_out ? (gx >> 2) : 0;
-    const float4* own = reinterpret_cast<const float4*>(a.pout) - (ptrdiff_t)a.row_off * W4 + col;
-#pragma unroll 1
-    for (int s = 0; s < 2; ++s) {
-        if (sy.mirror[s] == nullptr) continue;
-        const int lo = max(y0, sy.mir_lo[s]), hi = min(y1, sy.mir_hi[s]);
-        if (lo >= hi) continue;
-        const unsigned long long t1 = sy.dbg ? global_ns() : 0ull;
-        warp_spin_until(sy.mir_wait[s], sy.mir_seq, a.err);
-        const unsigned long long t2 = sy.dbg ? global_ns() : 0ull;
-        float4* dst = reinterpret_cast<float4*>(sy.mirror[s]) + col;
-        // 16 rows at a time: all the loads first (the stores are volatile asm, nothing moves across them —
-        // one load -> store pair per row would be a chain of serial L2 round trips)
-#pragma unroll 1
-        for (int r = lo; r < hi; r += 16) {
-            float4 v[16];
-#pragma unroll
-            for (int q = 0; q < 16; ++q) v[q] = own[(ptrdiff_t)min(r + q, hi - 1) * W4];
-#pragma unroll
-            for (int q = 0; q < 16; ++q) st_v4_if(dst + (ptrdiff_t)min(r + q, hi - 1) * W4, v[q], lane_out);   // the last row may be stored twice
-        }
-        // this lane's stores are performed at the neighbour before the lane goes on to the completion ticket.
-        // (fence.acq_rel, not __threadfence_system(): that one is fence.sc — MEMBAR.SC.SYS, totally ordered
-        // among ALL the grid's warps, far more than this lane's stores need)
-        asm volatile("fence.acq_rel.sys;" ::: "memory");
-        if (sy.dbg) {
-            const unsigned long long t3 = global_ns();
-            const bool l0 = (threadIdx.x == 0);
-            dbg_add(sy.dbg + 2, t2 - t1, l0); dbg_add(sy.dbg + 3, t3 - t2, l0); dbg_add(sy.dbg + 4, 1ull, l0);
-        }
-    }
-}
-
-// Grid-completion signal: the last CTA to get here release-stores done_seq into the neighbours' words.
-__device__ __forceinline__ void tb_signal_done(const TbSync& sy, const int lane) {
-    // every lane is past its stores (and, in tb_mirror, its fence) before lane 0 takes the ticket — a vote,
-    // not __syncwarp: see above.  The ticket is a release at GPU scope; the last CTA's fence + release-store
-    // at system scope then publishes everything that happened before any ticket.
-    const unsigned first = (__all_sync(0xffffffffu, 1) && lane == 0) ? 1u : 0u;
-    unsigned t;
-    asm volatile("{ .reg .pred q; setp.ne.u32 q, %1, 0; mov.u32 %0, 0xffffffff; @q atom.acq_rel.gpu.global.add.u32 %0, [%2], 1; }"
-                 : "=r"(t) : "r"(first), "l"(sy.ticket) : "memory");
-    const unsigned last = (t == gridDim.x - 1) ? 1u : 0u;              // lane 0 of the last CTA only
-    if (__any_sync(0xffffffffu, last)) {                               // warp-uniform branch: one CTA of the grid enters
-        asm volatile("{ .reg .pred q; setp.ne.u32 q, %0, 0; @q st.global.u32 [%1], 0; @q fence.acq_rel.sys; }"
-                     ::"r"(last), "l"(sy.ticket) : "memory");
-#pragma unroll
-        for (int s = 0; s < 2; ++s) {
-            if (sy.done_flag[s] == nullptr) continue;
-            asm volatile("{ .reg .pred q; setp.ne.u32 q, %0, 0; @q st.release.sys.global.u32 [%1], %2; }"
-                         ::"r"(last), "l"(sy.done_flag[s]), "r"(sy.done_seq) : "memory");
-        }
-    }
-}
-
 // One warp per CTA: every quantity that steers control flow derives from blockIdx and kernel
 // arguments only, so the compiler can prove the warp converged at each shuffle (no WARPSYNC /
 // BSSY scaffolding) and keeps loop state in uniform registers.
@@ -633,8 +491,8 @@ __device__ __forceinline__ void tb_signal_done(const TbSync& sy, const int lane)
 #else
 #define FLUID_TB_BOUNDS __launch_bounds__(32, FLUID_TB_MINBLOCKS)
 #endif
-template <int K, bool SCALE, bool TMA, bool SYNC>
-__global__ void FLUID_TB_BOUNDS jacobi_tb_kernel(TbArgs<SYNC> a, const __grid_constant__ TmapPair maps) {
+template <int K, bool SCALE, bool TMA>
+__global__ void FLUID_TB_BOUNDS jacobi_tb_kernel(JacobiArgs a, const __grid_constant__ TmapPair maps) {
     using T = TB<K>;
     extern __shared__ __align__(128) float4 smem4[];
     // Programmatic dependent launch: back-to-back blocked launches of one solve are chained with
@@ -647,8 +505,7 @@ __global__ void FLUID_TB_BOUNDS jacobi_tb_kernel(TbArgs<SYNC> a, const __grid_co
     const int nxw = (a.W + T::VALID - 1) / T::VALID;
     const int wid = blockIdx.x;
     const int wx = wid % nxw;
-    int cy = wid / nxw, seg_lo = a.out_lo, seg_hi = a.out_hi;
-    if (a.nch1 > 0 && cy >= a.nch1) { cy -= a.nch1; seg_lo = a.seg2_lo; seg_hi = a.seg2_hi; }
+    const int cy = wid / nxw;
 
     // ---- x geometry of this lane: mirrored / clamped float4 column group ------------------------
     const int W = a.W, H = a.H;
@@ -663,25 +520,12 @@ __global__ void FLUID_TB_BOUNDS jacobi_tb_kernel(TbArgs<SYNC> a, const __grid_co
     const int x0 = wx * T::VALID - T::HX;
 
     // ---- y geometry of this warp's stream ----------------------------------------------------------
-    const int y0 = seg_lo + cy * a.rows_per_chunk;
-    const int y1 = min(y0 + a.rows_per_chunk, seg_hi);
+    const int y0 = a.out_lo + cy * a.rows_per_chunk;
+    const int y1 = min(y0 + a.rows_per_chunk, a.out_hi);
     const int ys = max(y0 - K, 0);                    // first input row
     const int ye = min(y1 - 1 + K, H - 1);            // last input row
 
     asm volatile("griddepcontrol.wait;" ::: "memory");      // everything below reads what the previous launch wrote
-
-    // slab, first launch of a solve whose pressure ghost rows were stored by the neighbours' previous
-    // last launch: the streams that read those rows acquire "mirror ready" first
-    // (every lane polls the same word — warp-uniform control flow, see tb_mirror)
-    unsigned long long t_start = 0;
-    if constexpr (SYNC) {
-        const TbSync& sy = a.sy;
-        if (sy.dbg) t_start = global_ns();
-        const bool w0 = sy.pre_wait[0] != nullptr && ys < sy.own_lo, w1 = sy.pre_wait[1] != nullptr && ye >= sy.own_hi;
-        if (w0) warp_spin_until(sy.pre_wait[0], sy.pre_seq, a.err);
-        if (w1) warp_spin_until(sy.pre_wait[1], sy.pre_seq, a.err);
-        if (sy.dbg && (w0 || w1)) { dbg_add(sy.dbg + 0, global_ns() - t_start, lane == 0); dbg_add(sy.dbg + 1, 1ull, lane == 0); }
-    }
 
     // ---- does the divergence this stream reads hold a value that defeats the fma contraction? ----
     bool exact = false;
@@ -706,15 +550,6 @@ __global__ void FLUID_TB_BOUNDS jacobi_tb_kernel(TbArgs<SYNC> a, const __grid_co
         else tb_stream<K, SCALE, true, false, TMA>(a, tp, td, smem4, lane, x0, lc, gx, rev, lane_out, y0, y1, ys, ye);
     } else {
         tb_stream_exact<K, SCALE, TMA>(a, tp, td, smem4, lane, x0, lc, gx, rev, lane_out, y0, y1, ys, ye, any_rev);
-    }
-    if constexpr (SYNC) {
-        const TbSync& sy = a.sy;
-        if (sy.dbg) {
-            const bool edge = (ys < sy.own_lo) || (ye >= sy.own_hi);
-            dbg_add(sy.dbg + (edge ? 5 : 7), global_ns() - t_start, lane == 0); dbg_add(sy.dbg + (edge ? 6 : 8), 1ull, lane == 0);
-        }
-        if (sy.mirror[0] != nullptr || sy.mirror[1] != nullptr) tb_mirror(a, sy, gx, lane_out, y0, y1);
-        if (sy.ticket != nullptr) tb_signal_done(sy, lane);
     }
 }
 
