@@ -161,6 +161,14 @@ int fluid_step(fluid_t* h, float dt);
  * dye.rgb += exp(..)*(r,g,b), dye.a = 1; radius = correctRadius(SPLAT_RADIUS/100) (S:1457-1462). */
 int fluid_splat(fluid_t* h, float x, float y, float dx, float dy, float r, float g, float b);
 
+/* n calls of fluid_splat(h, s[7k+0], ..., s[7k+6]), k = 0..n-1, in that order, with the same bits, in
+ * ceil(n/128) launches (fluid_splat itself is one): records are (x, y, dx, dy, r, g, b); radius and
+ * aspect come from the handle's config, read once.  A frame that produces several splats (a burst of
+ * multipleSplats, one per moved pointer) should hand them over in one call.  The array is copied
+ * before the call returns.  n == 0 does nothing (dye alpha included); n < 0, or splats == NULL with
+ * n > 0, is FLUID_ERR_INVALID and leaves the fields untouched. */
+int fluid_splats(fluid_t* h, const float* splats, int n);
+
 /* config.<KEY> = value (S:59-69).  PRESSURE_ITERATIONS / JACOBI_BLOCK are rounded to int. */
 int fluid_set_param(fluid_t* h, int key, float value);
 int fluid_get_param(fluid_t* h, int key, float* value);

@@ -29,7 +29,7 @@ def main():
     out = ["# SASS instruction-class counts per kernel of libfluid_b200.so (static, whole kernel body)", "",
            "cubins in the library: " + ", ".join(sorted(set(re.findall(r"sm_\d+a?", arch)))) + " (sm_90a only)", "",
            "| kernel | total | " + " | ".join(CLASSES) + " |", "|---|---|" + "---|" * len(CLASSES)]
-    show = [k for k in kernels if re.search(r"tb_kernelILi10|cvd_stream|gradient_stream|advect_\w+4|splat_|display|jacobi_sweep|jacobi8|halo_push|tiny_scan|curl_vorticity_div", k)]
+    show = [k for k in kernels if re.search(r"tb_kernelILi10|cvd_stream|gradient_stream|advect_\w+4|splats_kernel|display|jacobi_sweep|jacobi8|halo_push|tiny_scan|curl_vorticity_div", k)]
     for k in show:
         c = kernels[k]
         name = re.sub(r"\(.*", "", demangle(k)).replace("fk::", "")

@@ -24,13 +24,15 @@ FAST = float(os.environ.get("SLAB_FAST", 0))     # texels/s of an extra splat pl
 def drive(sim, seed=5):
     rs = np.random.RandomState(seed)
     sim.random = lambda: float(rs.random_sample())
-    sim.multipleSplats(6)
+    sim.multipleSplats(6)                                # one splat() per record ...
     if FAST:   # the fastest thing a pointer flick produces, right on the boundary between two slabs, aimed across it
-        sim.splat(0.5, 0.5, 0.3 * FAST, FAST, (0.9, 0.2, 0.1)); sim.splat(0.25, 0.5, 0.0, -FAST, (0.1, 0.8, 0.3))
+        sim.splats([(0.5, 0.5, 0.3 * FAST, FAST, 0.9, 0.2, 0.1), (0.25, 0.5, 0.0, -FAST, 0.1, 0.8, 0.3)])
     for k in range(STEPS):
         sim.step(0.016666)
-        if k == 1:
-            sim.multipleSplats(2)
+        if k == 1:                                       # ... and a burst in one splats() call
+            sim.splats([(rs.random_sample(), rs.random_sample(), 1000 * (rs.random_sample() - 0.5),
+                         1000 * (rs.random_sample() - 0.5), 1.5 * rs.random_sample(), 0.0, 1.5 * rs.random_sample())
+                        for _ in range(6)])
     out = {n: sim.readField(n) for n in ("velocity", "dye", "pressure", "divergence")}
     out["frame_"] = sim.render(256, 192)                 # a slab rank returns its band of the 256 x 192 target
     if RESIZE:                                           # resizeDoubleFBO on a live simulation (S:1116-1126), slab or not

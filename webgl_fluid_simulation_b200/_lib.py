@@ -18,7 +18,7 @@ CSRC = os.path.join(_HERE, "csrc")
 SYMBOLS = [
     "fluid_abi_version", "fluid_config_default", "fluid_get_resolution", "fluid_create",
     "fluid_create_slab", "fluid_nccl_unique_id", "fluid_p2p_export", "fluid_p2p_connect", "fluid_p2p_disable", "fluid_destroy", "fluid_resize", "fluid_step",
-    "fluid_splat", "fluid_set_param", "fluid_set_param_f64", "fluid_get_param", "fluid_stat", "fluid_pass_curl", "fluid_pass_vorticity",
+    "fluid_splat", "fluid_splats", "fluid_set_param", "fluid_set_param_f64", "fluid_get_param", "fluid_stat", "fluid_pass_curl", "fluid_pass_vorticity",
     "fluid_pass_divergence", "fluid_pass_clear_pressure", "fluid_pass_jacobi",
     "fluid_pass_pressure_solve", "fluid_pass_gradient_subtract", "fluid_pass_advect_velocity",
     "fluid_pass_advect_dye", "fluid_pass_curl_vorticity_divergence", "fluid_field_elems",
@@ -103,6 +103,7 @@ def lib():
     L.fluid_resize.argtypes = [vp, i, i, i, i]
     L.fluid_step.argtypes = [vp, f]
     L.fluid_splat.argtypes = [vp] + [f] * 7
+    L.fluid_splats.argtypes = [vp, fp, i]
     L.fluid_set_param.argtypes = [vp, i, f]
     L.fluid_set_param_f64.argtypes = [vp, i, C.c_double]
     L.fluid_get_param.argtypes = [vp, i, fp]

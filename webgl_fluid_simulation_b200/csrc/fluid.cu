@@ -1222,43 +1222,56 @@ int fluid_step(fluid_t* h, float dt) {
     return FLUID_OK;
 }
 
-// splat(x,y,dx,dy,color), S:1441-1455
-int fluid_splat(fluid_t* h, float x, float y, float dx, float dy, float r, float g, float b) {
+static SplatPlane splat_plane(const Grid& g) {
+    SplatPlane p{};
+    p.g = g; p.pow2 = is_pow2(g.W) && is_pow2(g.H);
+    p.tsx = (float)(1.0 / (double)g.W); p.tsy = (float)(1.0 / (double)g.H);
+    p.bx = (g.W + SPL_BW - 1) / SPL_BW;
+    return p;
+}
+static int splat_blocks(const SplatPlane& p) { return p.bx * ((p.g.j_hi - p.g.j_lo + SPL_BH - 1) / SPL_BH); }
+
+// n x splat(x,y,dx,dy,color) of S:1441-1455, in order, SPLATS_PER_LAUNCH records per launch
+int fluid_splats(fluid_t* h, const float* splats, int n) {
     if (!h) return FLUID_ERR_INVALID;
+    if (n < 0 || (n > 0 && !splats)) return fail(h, FLUID_ERR_INVALID, "fluid_splats: bad record block (%d records at %p)", n, (const void*)splats);
+    if (n == 0) return FLUID_OK;
+    static_assert(sizeof(SplatRec) == 7 * sizeof(float), "records are 7 packed floats");
+    static_assert(sizeof(SplatsArgs) <= 4096, "the records travel in the 4 KB kernel parameter block");
+    SplatsArgs a{};
     // correctRadius(config.SPLAT_RADIUS / 100.0): JS double arithmetic, narrowed by gl.uniform1f
     double rad = h->splat_radius_d / 100.0;
     if (h->aspect_d > 1.0) rad *= h->aspect_d;
-    const float radius = (float)rad;
-    if (h->half) {
-        const int W = h->cfg.sim_w, H = h->cfg.sim_h, Wd = h->cfg.dye_w, Hd = h->cfg.dye_h;
-        hs::splat_velocity_kernel<<<hs_grid(W, H), HS_BLOCK, 0, h->stream>>>((const hs::h2*)h->velocity.read, (hs::h2*)h->velocity.write, W, H,
-                                                                             h->cfg.aspect, x, y, dx, dy, radius);
-        int rc = check_launch(h, "hs::splat_velocity_kernel"); if (rc) return rc;
-        swap_v(h);
-        hs::splat_dye_kernel<<<hs_grid(Wd, Hd), HS_BLOCK, 0, h->stream>>>((const hs::h4*)h->dye.read, (hs::h4*)h->dye.write, Wd, Hd,
-                                                                          h->cfg.aspect, x, y, r, g, b, radius);
-        rc = check_launch(h, "hs::splat_dye_kernel"); if (rc) return rc;
-        swap_dye(h);
-        return FLUID_OK;
+    a.radius = (float)rad;
+    a.aspect = h->cfg.aspect;
+    // a splat is point-wise, so the +-3 velocity ghost rows of a slab are simply splatted as well
+    a.v = splat_plane(sim_grid_ext(h, h->slab() ? 3 : 0));
+    a.d = splat_plane(dye_grid(h));
+    a.blocks_v = splat_blocks(a.v);
+    const int blocks = a.blocks_v + splat_blocks(a.d);
+    for (int k0 = 0; k0 < n; k0 += SPLATS_PER_LAUNCH) {
+        a.n = std::min(n - k0, SPLATS_PER_LAUNCH);
+        memcpy(a.rec, splats + 7 * (size_t)k0, (size_t)a.n * sizeof(SplatRec));
+        // the first launch reads .read; the next ones continue in place on .write
+        const void* vin = k0 ? h->velocity.write : h->velocity.read;
+        const void* din = k0 ? h->dye.write : h->dye.read;
+        if (h->half)
+            splats_kernel<hs::SplatHalf><<<blocks, 256, 0, h->stream>>>((const hs::h2*)vin, (hs::h2*)h->velocity.write,
+                                                                         (const hs::h4*)din, (hs::h4*)h->dye.write, a);
+        else
+            splats_kernel<SplatF32><<<blocks, 256, 0, h->stream>>>((const float2*)vin, (float2*)h->velocity.write,
+                                                                    (const float4*)din, (float4*)h->dye.write, a);
+        int rc = check_launch(h, "splats_kernel"); if (rc) return rc;
     }
-    dim3 bl(64, 4);
-    // a splat is point-wise, so the +-3 velocity ghost rows are simply splatted as well
-    Grid gs = sim_grid_ext(h, h->slab() ? 3 : 0), gd = dye_grid(h);
-    SplatArgs sa{};
-    sa.aspect = h->cfg.aspect; sa.px = x; sa.py = y; sa.radius = radius;
-    sa.g = gs; sa.pow2 = is_pow2(gs.W) && is_pow2(gs.H);
-    sa.tsx = (float)(1.0 / (double)gs.W); sa.tsy = (float)(1.0 / (double)gs.H);
-    splat_velocity_kernel<<<grid2d(gs.W, gs.j_hi - gs.j_lo, bl), bl, 0, h->stream>>>(
-        (const float2*)h->velocity.read, (float2*)h->velocity.write, sa, dx, dy);
-    int rc = check_launch(h, "splat_velocity_kernel"); if (rc) return rc;
     swap_v(h);                                   // S:1449
-    sa.g = gd; sa.pow2 = is_pow2(gd.W) && is_pow2(gd.H);
-    sa.tsx = (float)(1.0 / (double)gd.W); sa.tsy = (float)(1.0 / (double)gd.H);
-    splat_dye_kernel<<<grid2d(gd.W, gd.j_hi - gd.j_lo, bl), bl, 0, h->stream>>>(
-        (const float4*)h->dye.read, (float4*)h->dye.write, sa, r, g, b);
-    rc = check_launch(h, "splat_dye_kernel"); if (rc) return rc;
-    swap_dye(h);                                        // S:1454
+    swap_dye(h);                                 // S:1454
     return FLUID_OK;
+}
+
+// splat(x,y,dx,dy,color), S:1441-1455
+int fluid_splat(fluid_t* h, float x, float y, float dx, float dy, float r, float g, float b) {
+    const float rec[7] = {x, y, dx, dy, r, g, b};
+    return fluid_splats(h, rec, 1);
 }
 
 // initFramebuffers() on a live simulation: S:982-1010 + resizeDoubleFBO S:1116-1126

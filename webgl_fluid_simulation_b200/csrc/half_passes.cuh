@@ -161,32 +161,33 @@ __global__ void __launch_bounds__(256) advect_kernel(const h2* __restrict__ vel,
     st(out, j * W + i, o);
 }
 
-// splatShader S:726-744
-__device__ __forceinline__ float splat_w(int i, int j, int W, int H, float aspect, float px, float py, float radius) {
-    const float uvx = ((float)i + 0.5f) / (float)W, uvy = ((float)j + 0.5f) / (float)H;
-    float dx = uvx - px;
-    const float dy = uvy - py;
-    dx = dx * aspect;
-    return expf(-(dx * dx + dy * dy) / radius);
-}
-__global__ void __launch_bounds__(256) splat_velocity_kernel(const h2* __restrict__ base, h2* __restrict__ out, int W, int H,
-                                                             float aspect, float px, float py, float cx, float cy, float radius) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y * blockDim.y + threadIdx.y;
-    if (i >= W || j >= H) return;
-    const float e = splat_w(i, j, W, H, aspect, px, py, radius);
-    float2 b = ld(base, j * W + i);
-    b.x = b.x + e * cx; b.y = b.y + e * cy;
-    st(out, j * W + i, b);
-}
-__global__ void __launch_bounds__(256) splat_dye_kernel(const h4* __restrict__ base, h4* __restrict__ out, int W, int H,
-                                                        float aspect, float px, float py, float cr, float cg, float cb, float radius) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y * blockDim.y + threadIdx.y;
-    if (i >= W || j >= H) return;
-    const float e = splat_w(i, j, W, H, aspect, px, py, radius);
-    float4 b = ld(base, j * W + i);
-    b.x = b.x + e * cr; b.y = b.y + e * cg; b.z = b.z + e * cb; b.w = 1.0f;
-    st(out, j * W + i, b);
-}
+// storage policy of splats_kernel (passes.cuh): round() is the st() + ld() pair above, the RN-even
+// store of one splat() call and the exact widening read of the next.  Plain loads: launches after a
+// block's first run in place.
+struct SplatHalf {
+    typedef h2 V;
+    typedef h4 D;
+    template <int C> static __device__ __forceinline__ void load(const void* p, size_t o, float* v) {
+        if (C == 2) {
+            const float2 t = __half22float2(static_cast<const h2*>(p)[o]); v[0] = t.x; v[1] = t.y;
+        } else {
+            const h4 t = static_cast<const h4*>(p)[o];
+            const float2 a = __half22float2(t.a), b = __half22float2(t.b);
+            v[0] = a.x; v[1] = a.y; v[2] = b.x; v[3] = b.y;
+        }
+    }
+    template <int C> static __device__ __forceinline__ void store(void* p, size_t o, const float* v) {
+        if (C == 2) static_cast<h2*>(p)[o] = __floats2half2_rn(v[0], v[1]);
+        else { h4 t; t.a = __floats2half2_rn(v[0], v[1]); t.b = __floats2half2_rn(v[2], v[3]); static_cast<h4*>(p)[o] = t; }
+    }
+    template <int C> static __device__ __forceinline__ void round(float* v) {
+#pragma unroll
+        for (int q = 0; q < C; q += 2) {
+            const float2 t = __half22float2(__floats2half2_rn(v[q], v[q + 1]));
+            v[q] = t.x; v[q + 1] = t.y;
+        }
+    }
+};
 
 // host <-> device conversions of fluid_read / fluid_write (the ABI speaks fp32)
 __global__ void __launch_bounds__(256) widen_kernel(const h1* __restrict__ in, float* __restrict__ out, size_t n) {

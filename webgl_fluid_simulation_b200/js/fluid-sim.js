@@ -164,6 +164,15 @@ class FluidSimulation {
         native.splat(this._h, x, y, dx, dy, color.r, color.g, color.b);
     }
 
+    // len/7 splat() calls in one: records is a Float32Array of (x, y, dx, dy, r, g, b) records,
+    // applied in order with the same result as one splat() per record, in ceil(n/128) launches
+    splats (records) {
+        if (!(records instanceof Float32Array) || records.length % 7 !== 0)
+            throw new TypeError('splats() takes a Float32Array of 7-float records (x, y, dx, dy, r, g, b)');
+        this._pushConfig();
+        native.splats(this._h, records);
+    }
+
     splatPointer (pointer) {                                    // S:1421-1425
         const dx = pointer.deltaX * this.config.SPLAT_FORCE;
         const dy = pointer.deltaY * this.config.SPLAT_FORCE;

@@ -10,6 +10,7 @@
  * Exports (all take the handle first):
  *   create(cfg) / createSlab(cfg, rank, world, uid) -> handle        destroy(h)
  *   step(h, dt)  splat(h, x, y, dx, dy, r, g, b)  setParam(h, key, value)  resize(h, sw, sh, dw, dh)
+ *   splats(h, Float32Array of n * 7 floats: n splat() records (x, y, dx, dy, r, g, b), in order)
  *   read(h, field) -> Float32Array over PINNED host memory (one buffer per field, owned by the
  *       handle, overwritten by the next read of that field — like rebinding the same texture)
  *   write(h, field, Float32Array)  sync(h)  dims(h, field) -> {width, height, channels, row0}
@@ -211,6 +212,17 @@ static napi_value Write(napi_env env, napi_callback_info info) {
     return undefined(env);
 }
 
+/* splats(h, Float32Array of n * 7 floats): n splat() records (x, y, dx, dy, r, g, b) in one call */
+static napi_value Splats(napi_env env, napi_callback_info info) {
+    ARGS(2)
+    wrap_t* w = wrap_of(env, argv[0]); if (!w) return NULL;
+    float* data; size_t len;
+    if (!f32_arg(env, argv[1], &data, &len)) return NULL;
+    if (len % 7 != 0 || len / 7 > 0x7fffffff) { napi_throw_error(env, NULL, "splats needs a whole number of 7-float records"); return NULL; }
+    check(env, w->h, fluid_splats(w->h, data, (int)(len / 7)));
+    return undefined(env);
+}
+
 static napi_value PressureSolveHost(napi_env env, napi_callback_info info) {
     ARGS(4)
     wrap_t* w = wrap_of(env, argv[0]); if (!w) return NULL;
@@ -403,6 +415,7 @@ NAPI_MODULE_INIT() {
         {"destroy", NULL, Destroy, NULL, NULL, NULL, napi_enumerable, NULL},
         {"step", NULL, Step, NULL, NULL, NULL, napi_enumerable, NULL},
         {"splat", NULL, Splat, NULL, NULL, NULL, napi_enumerable, NULL},
+        {"splats", NULL, Splats, NULL, NULL, NULL, napi_enumerable, NULL},
         {"setParam", NULL, SetParam, NULL, NULL, NULL, napi_enumerable, NULL},
         {"resize", NULL, Resize, NULL, NULL, NULL, napi_enumerable, NULL},
         {"read", NULL, Read, NULL, NULL, NULL, napi_enumerable, NULL},

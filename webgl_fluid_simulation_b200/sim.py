@@ -303,6 +303,16 @@ class FluidSimulation:
         self._check(self._L.fluid_splat(self._h, float(x), float(y), float(dx), float(dy),
                                         float(r), float(g), float(b)))
 
+    def splats(self, records):
+        """len(records) splat() calls in one: records is (n, 7) of (x, y, dx, dy, r, g, b), applied in
+        order with the same bits as one splat() per row, in ceil(n/128) launches."""
+        a = np.asarray(records)
+        if a.ndim != 2 or a.shape[1] != 7:
+            raise ValueError(f"splats() takes an (n, 7) array of (x, y, dx, dy, r, g, b), got shape {a.shape}")
+        a = np.ascontiguousarray(a, np.float32)        # round to nearest, as c_float does per argument
+        self._push_config()
+        self._check(self._L.fluid_splats(self._h, a.ctypes.data_as(C.POINTER(C.c_float)), a.shape[0]))
+
     def splatPointer(self, pointer):
         """S:1421-1425."""
         dx = pointer.deltaX * self.config["SPLAT_FORCE"]
