@@ -312,7 +312,9 @@ typedef enum fluid_stat_key {
     FLUID_STAT_HALO_EXCHANGES = 3,   /* halo exchanges issued (either transport)                      */
     FLUID_STAT_GRAPH_CAPTURES = 4,   /* step() graphs captured + instantiated                         */
     FLUID_STAT_GRAPH_LAUNCHES = 5,   /* step() graphs replayed                                        */
-    FLUID_STAT_HALO_TRANSPORT_P2P = 6 /* 1 when the peer-memory halo path is active                    */
+    FLUID_STAT_HALO_TRANSPORT_P2P = 6, /* 1 when the peer-memory halo path is active                   */
+    FLUID_STAT_CVD_STREAM_LAUNCHES = 7,      /* row-streaming curl-vorticity-divergence kernels executed */
+    FLUID_STAT_GRADIENT_STREAM_LAUNCHES = 8  /* row-streaming gradientSubtract kernels executed          */
 } fluid_stat_key;
 uint64_t fluid_stat(fluid_t* h, int key);
 

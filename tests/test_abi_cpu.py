@@ -30,6 +30,23 @@ def test_header_and_library_agree(L):
     assert L.fluid_abi_version() == 2
 
 
+def test_stat_tables_match_the_header_enum():
+    """fluid_stat keys: the Python STAT table and the JS one name every FLUID_STAT_* of the header,
+    with the same value (the JS keys are the camelCase form of the same names)."""
+    hdr = open(os.path.join(ROOT, "include", "fluid.h")).read()
+    hdr = re.sub(r"/\*.*?\*/", "", hdr, flags=re.S)
+    body = re.search(r"typedef enum fluid_stat_key \{(.*?)\} fluid_stat_key;", hdr, re.S).group(1)
+    enum = {k.lower(): int(v) for k, v in re.findall(r"FLUID_STAT_([A-Z0-9_]+)\s*=\s*(\d+)", body)}
+    assert len(enum) == body.count("=") and len(set(enum.values())) == len(enum), body
+    assert {"cvd_stream_launches": 7, "gradient_stream_launches": 8}.items() <= enum.items()
+    assert _lib.STAT == enum
+    js = open(os.path.join(ROOT, "webgl_fluid_simulation_b200", "js", "fluid-sim.js")).read()
+    table = re.search(r"const STAT = \{(.*?)\};", js, re.S).group(1)
+    js_stat = {k: int(v) for k, v in re.findall(r"(\w+)\s*:\s*(\d+)", table)}
+    camel = {re.sub(r"_([a-z0-9])", lambda m: m.group(1).upper(), k).replace("P2p", "P2P"): v for k, v in enum.items()}
+    assert js_stat == camel
+
+
 def test_no_torch_types_in_the_abi():
     hdr = open(os.path.join(ROOT, "include", "fluid.h")).read()
     hdr = re.sub(r"/\*.*?\*/", "", hdr, flags=re.S)      # signatures only, not the prose

@@ -92,18 +92,65 @@ def test_passes_vs_golden_reference_shader_outputs(pkg, name):
     s.close()
 
 
-@pytest.mark.parametrize("W,H", [(64, 40), (128, 128), (256, 96), (16, 2), (132, 77), (520, 33)])
+# Grids too small to give every SM a warp stream run the tiled kernels of passes.cuh; these run
+# curl_vorticity_divergence_kernel and gradient_subtract_kernel (and (16, 2) at 16 columns too).
+TILED_SHAPES = [(64, 40), (128, 128), (256, 96), (16, 2), (132, 77), (520, 33)]
+# Grids that select the row-streaming kernels of stream_passes.cuh (cvd: 120 output columns per
+# warp, lanes 1..30; gradient: 128 columns, lanes 0..31).  Warp counts from stream_args, for 132 SMs:
+#   8x4096    one window; both x walls inside one warp, only lanes 1 and 2 produce output
+#   12x4093   W/4 odd; the last 16-row chunk is partial (4093 = 255*16 + 13)
+#   124x2050  the second cvd window has one output lane; W % 128 = 124 for gradient
+#   964x600   964 = 8*120 + 4: the last cvd window produces only its wall lane
+#   132x2051  gradient: the last 128-column window has one live lane; H % 4 = 3, so the GS_U tail re-reads
+#   16900xH   141 cvd / 133 gradient windows fill the SMs in one chunk; H = 1 puts both y walls on one
+#             row; gradient's last window is a single wall lane
+#   1024x512  an ordinary power-of-two grid
+STREAM_SHAPES = [(8, 4096), (12, 4093), (124, 2050), (964, 600), (132, 2051), (16900, 1), (16900, 2),
+                 (16900, 3), (1024, 512)]
+
+
+@pytest.mark.parametrize("W,H", TILED_SHAPES + STREAM_SHAPES)
 def test_fused_curl_vorticity_divergence_equals_three_passes(pkg, oracle, W, H):
+    """fluid_pass_curl_vorticity_divergence == curl, vorticity, divergence of the oracle, bitwise, and
+    == the tiled kernel (FLAG_TILED_PASSES).  STREAM_SHAPES must run cvd_stream_kernel, TILED_SHAPES
+    curl_vorticity_divergence_kernel: the launch counter says which one ran."""
     O = oracle
     v, _, _ = rand_fields(W, H, W, H, 11)
-    s = make(pkg, W, H, W, H)
-    s.writeField("velocity", v)
-    s.pass_("curl_vorticity_divergence", DT)
-    c = O.curl(v); v2 = O.vorticity(v, c, 30.0, DT)
-    assert bits_equal(s.readField("curl"), c)
-    assert bits_equal(s.readField("velocity"), v2)
-    assert bits_equal(s.readField("divergence"), O.divergence(v2))
-    s.close()
+    c = O.curl(v); v2 = O.vorticity(v, c, 30.0, DT); d = O.divergence(v2)
+    outs = []
+    for flags in (0, pkg.FLAG_TILED_PASSES):
+        s = make(pkg, W, H, W, H, flags=flags)
+        s.writeField("velocity", v)
+        n0 = s.stat("cvd_stream_launches")
+        s.pass_("curl_vorticity_divergence", DT)
+        streamed = s.stat("cvd_stream_launches") - n0
+        assert streamed == (1 if flags == 0 and (W, H) in STREAM_SHAPES else 0), streamed
+        outs.append([s.readField(n) for n in ("curl", "velocity", "divergence")])
+        s.close()
+    for got, tiled, want in zip(outs[0], outs[1], (c, v2, d)):
+        assert bits_equal(got, want)
+        assert bits_equal(got, tiled)
+
+
+@pytest.mark.parametrize("W,H", TILED_SHAPES + STREAM_SHAPES)
+def test_gradient_subtract_streaming_and_tiled_vs_oracle(pkg, oracle, W, H):
+    """fluid_pass_gradient_subtract == the oracle bitwise and == the tiled kernel; STREAM_SHAPES run
+    gradient_stream_kernel, TILED_SHAPES gradient_subtract_kernel."""
+    O = oracle
+    v, _, p = rand_fields(W, H, W, H, 12)
+    want = O.gradient_subtract(p, v)
+    outs = []
+    for flags in (0, pkg.FLAG_TILED_PASSES):
+        s = make(pkg, W, H, W, H, flags=flags)
+        s.writeField("velocity", v); s.writeField("pressure", p)
+        n0 = s.stat("gradient_stream_launches")
+        s.pass_("gradient_subtract")
+        streamed = s.stat("gradient_stream_launches") - n0
+        assert streamed == (1 if flags == 0 and (W, H) in STREAM_SHAPES else 0), streamed
+        outs.append(s.readField("velocity"))
+        s.close()
+    assert bits_equal(outs[0], want)
+    assert bits_equal(outs[0], outs[1])
 
 
 @pytest.mark.parametrize("W,H,iters,jb", [(128, 64, 20, 8), (256, 200, 50, 8), (512, 96, 30, 10),
@@ -531,12 +578,8 @@ def test_render_postfx_vs_oracle_and_executed_shaders(pkg, oracle, name):
     s.close()
 
 
-def test_half_storage_every_pass_and_whole_steps_bitwise_vs_oracle(pkg, oracle):
-    """FLUID_FLAG_HALF_STORAGE: the reference's own storage format (half-float textures, S:138-147,
-    S:986-1006): fp32 arithmetic, fp16 round-to-nearest-even on every pass write.  Per pass and for
-    whole steps bit-identical to the oracle's half_storage mode (oracle_round_half after every blit)."""
-    O = oracle
-    W, H, Wd, Hd = 64, 48, 128, 96
+def half_every_pass(pkg, O, W, H, Wd, Hd):
+    """Each pass of a half-storage handle against the oracle, rounded to fp16 after every blit."""
     v, dye, p = rand_fields(W, H, Wd, Hd, 77)
     v, dye, p = O.round_half(v), O.round_half(dye), O.round_half(p)
     s = make(pkg, W, H, Wd, Hd, flags=pkg.FLAG_HALF_STORAGE)
@@ -555,8 +598,12 @@ def test_half_storage_every_pass_and_whole_steps_bitwise_vs_oracle(pkg, oracle):
     s.pass_("advect_velocity", DT); v4 = s.readField("velocity"); assert bits_equal(v4, R(O.advect(v3, v3, DT, 0.2)))
     s.pass_("advect_dye", DT); assert bits_equal(s.readField("dye"), R(O.advect(v4, dye, DT, 1.0)))
     s.close()
-    # whole steps (graph replay), 128^2 / 256^2, 20 iterations: every field, three steps
-    W = H = 128; Wd = Hd = 256
+
+
+def half_whole_steps(pkg, O, W, H, Wd, Hd):
+    """Three whole steps (graph replay, 20 iterations) of a half-storage handle against the oracle's
+    half mode, every field, then render() of the fp16 dye through the fp32 display shader."""
+    R = O.round_half
     v, dye, p = rand_fields(W, H, Wd, Hd, 78)
     v, dye, p = R(v), R(dye), R(p)
     s = make(pkg, W, H, Wd, Hd, flags=pkg.FLAG_HALF_STORAGE)
@@ -567,8 +614,51 @@ def test_half_storage_every_pass_and_whole_steps_bitwise_vs_oracle(pkg, oracle):
         s.step(DT); ref.step(DT)
     for n in ("velocity", "dye", "pressure", "divergence", "curl"):
         assert bits_equal(s.readField(n), getattr(ref, n)), n
-    # render() reads the fp16 dye through the fp32 display shader
     assert bits_equal(s.render(64, 64), O.display(ref.dye, 64, 64, True, (0.0, 0.0, 0.0)))
+    s.close()
+
+
+def test_half_storage_every_pass_and_whole_steps_bitwise_vs_oracle(pkg, oracle):
+    """FLUID_FLAG_HALF_STORAGE: the reference's own storage format (half-float textures, S:138-147,
+    S:986-1006): fp32 arithmetic, fp16 round-to-nearest-even on every pass write.  Per pass and for
+    whole steps bit-identical to the oracle's half_storage mode (oracle_round_half after every blit)."""
+    half_every_pass(pkg, oracle, 64, 48, 128, 96)
+    half_whole_steps(pkg, oracle, 128, 128, 256, 256)
+
+
+# half storage at every parity size and where the kernel choice changes: hs::jacobi8_kernel
+# (W % 8 == 0, W >= 64) fetches across warps only when W/8 > 32; 264 has one live lane in the second
+# warp, 520 several full warps and a partial one, 1024 four warps per row (the roofline_half_storage
+# size); W = 100 (W % 8 = 4) runs the one-cell hs::jacobi_kernel
+HALF_SIZES = SIZES + [(264, 40, 528, 80), (520, 33, 780, 50), (100, 60, 150, 90), (1024, 1024, 1024, 1024)]
+
+
+@pytest.mark.parametrize("W,H,Wd,Hd", HALF_SIZES)
+def test_half_storage_passes_and_steps_at_every_jacobi_width(pkg, oracle, W, H, Wd, Hd):
+    """The same two checks as above at shapes that select each half-storage Jacobi path and reach
+    hs::jacobi8_kernel's cross-warp fetches."""
+    half_every_pass(pkg, oracle, W, H, Wd, Hd)
+    half_whole_steps(pkg, oracle, W, H, Wd, Hd)
+
+
+@pytest.mark.parametrize("src,dst", [((64, 48, 128, 96), (100, 75, 150, 113)),
+                                     ((36, 20, 54, 30), (23, 41, 97, 31))])
+def test_half_storage_resize_carries_state_like_resizeDoubleFBO(pkg, oracle, src, dst):
+    """initFramebuffers() on a half-storage handle (fluid_resize): velocity and dye resampled with the
+    LINEAR copy, then rounded to fp16 like the reference's half-float target; pressure, divergence
+    and curl start over at zero.  Ragged sizes, up and down."""
+    O = oracle
+    R = O.round_half
+    v, dye, p = (R(a) for a in rand_fields(*src, 41))
+    s = make(pkg, *src, flags=pkg.FLAG_HALF_STORAGE)
+    s.writeField("velocity", v); s.writeField("dye", dye); s.writeField("pressure", p)
+    s._sizes = dst; s.initFramebuffers()
+    W, H, Wd, Hd = dst
+    assert s._dims("velocity")[:2] == (W, H) and s._dims("dye")[:2] == (Wd, Hd)
+    assert bits_equal(s.readField("velocity"), R(O.resample(v, W, H)))
+    assert bits_equal(s.readField("dye"), R(O.resample(dye, Wd, Hd)))
+    for n in ("pressure", "divergence", "curl"):
+        assert not s.readField(n).any(), n
     s.close()
 
 

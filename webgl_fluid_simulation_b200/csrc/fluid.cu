@@ -50,6 +50,8 @@ struct fluid {
     uint64_t launches = 0;
     uint64_t jacobi_kernel_launches = 0;   // Jacobi kernels only (fluid_stat FLUID_STAT_JACOBI_LAUNCHES)
     uint64_t halo_kernel_launches = 0;     // halo_push / halo_wait kernels of the peer-memory transport
+    uint64_t cvd_stream_launches = 0;      // cvd_stream_kernel / gradient_stream_kernel (FLUID_STAT_*_STREAM_LAUNCHES):
+    uint64_t gradient_stream_launches = 0; // which of a pass's kernels the grid size picked
     uint64_t div_epoch = 1, div_sent_epoch = 0;   // slab: the divergence ghost rows are re-sent only after divergence was rewritten
     int div_sent_rows = 0;
     bool pdl_chain = false;                // the next blocked Jacobi launch directly follows another one of the same solve
@@ -105,7 +107,10 @@ struct fluid {
     struct { const float* div; unsigned char* map; int W, row_off, lo0, hi0, lo1, hi1; } scan{};
     bool scan_pending = false;
     // ---- step() as a CUDA graph (single GPU): one instantiated graph per (dt, config scalars, parity)
-    struct StepGraph { cudaGraphExec_t exec = nullptr; int flip_v = 0, flip_p = 0, flip_dye = 0, kernels = 0, jacobi_launches = 0; };
+    struct StepGraph {
+        cudaGraphExec_t exec = nullptr;
+        int flip_v = 0, flip_p = 0, flip_dye = 0, kernels = 0, jacobi_launches = 0, cvd_stream = 0, gradient_stream = 0;
+    };
     std::map<std::string, StepGraph> graphs;
     uint64_t graph_launches = 0, graph_captures = 0;
     float4* frame = nullptr;         // render target of fluid_render (w x h RGBA fp32), grown on demand
@@ -963,6 +968,7 @@ static int do_cvd(fluid_t* h, Grid g) {
             (const float2*)h->velocity.read, h->curl, (float2*)h->velocity.write, h->divergence, a, h->cfg.curl,
             h->dt_dev, h->tiny_map);
         int rc = check_launch(h, "cvd_stream_kernel"); if (rc) return rc;
+        ++h->cvd_stream_launches;
         swap_v(h);
         return FLUID_OK;
     }
@@ -989,6 +995,7 @@ static int do_gradient(fluid_t* h, Grid g) {
         gradient_stream_kernel<<<(nwarps + GS_WARPS - 1) / GS_WARPS, 32 * GS_WARPS, 0, h->stream>>>(
             (const float*)h->pressure.read, (const float2*)h->velocity.read, (float2*)h->velocity.write, a);
         int rc = check_launch(h, "gradient_stream_kernel"); if (rc) return rc;
+        ++h->gradient_stream_launches;
         swap_v(h);                                   // S:1273
         return FLUID_OK;
     }
@@ -1188,6 +1195,7 @@ int fluid_step(fluid_t* h, float dt) {
         if (h->graphs.size() > 64) drop_graphs(h);          // config sliders dragged for a long time: stay bounded
         const int pv = h->par_v, pp = h->par_p, pd = h->par_dye;
         const uint64_t l0 = h->launches, j0 = h->jacobi_kernel_launches;
+        const uint64_t cs0 = h->cvd_stream_launches, gs0 = h->gradient_stream_launches;
         cudaGraph_t g = nullptr;
         CU(cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeThreadLocal));
         h->capturing = true;
@@ -1202,7 +1210,9 @@ int fluid_step(fluid_t* h, float dt) {
         if (e != cudaSuccess) return fail(h, FLUID_ERR_CUDA, "cudaGraphInstantiate failed: %s", cudaGetErrorString(e));
         sg.flip_v = pv ^ h->par_v; sg.flip_p = pp ^ h->par_p; sg.flip_dye = pd ^ h->par_dye;
         sg.kernels = (int)(h->launches - l0); sg.jacobi_launches = (int)(h->jacobi_kernel_launches - j0);
+        sg.cvd_stream = (int)(h->cvd_stream_launches - cs0); sg.gradient_stream = (int)(h->gradient_stream_launches - gs0);
         h->launches = l0; h->jacobi_kernel_launches = j0;    // captured, not yet executed
+        h->cvd_stream_launches = cs0; h->gradient_stream_launches = gs0;
         ++h->graph_captures;
         it = h->graphs.emplace(key, sg).first;
         // the capture already performed the host-side swaps of this step
@@ -1215,6 +1225,8 @@ int fluid_step(fluid_t* h, float dt) {
     CU(cudaGraphLaunch(it->second.exec, h->stream));
     h->launches += it->second.kernels;
     h->jacobi_kernel_launches += it->second.jacobi_launches;
+    h->cvd_stream_launches += it->second.cvd_stream;
+    h->gradient_stream_launches += it->second.gradient_stream;
     h->timing.jacobi_launches = it->second.jacobi_launches;
     h->timing.total_launches = it->second.kernels;
     h->have_timing = false;
@@ -1926,6 +1938,8 @@ uint64_t fluid_stat(fluid_t* h, int key) {
         case FLUID_STAT_GRAPH_CAPTURES: return h->graph_captures;
         case FLUID_STAT_GRAPH_LAUNCHES: return h->graph_launches;
         case FLUID_STAT_HALO_TRANSPORT_P2P: return h->p2p ? 1 : 0;
+        case FLUID_STAT_CVD_STREAM_LAUNCHES: return h->cvd_stream_launches;
+        case FLUID_STAT_GRADIENT_STREAM_LAUNCHES: return h->gradient_stream_launches;
     }
     return 0;
 }

@@ -525,7 +525,9 @@ class FluidSimulation:
 
     def stat(self, name) -> int:
         """Library counters (fluid_stat): launches, jacobi_launches, halo_launches, halo_exchanges,
-        graph_captures, graph_launches, halo_transport_p2p."""
+        graph_captures, graph_launches, halo_transport_p2p, cvd_stream_launches and
+        gradient_stream_launches (how many curl-vorticity-divergence / gradientSubtract passes ran
+        the row-streaming kernel rather than the tiled one; graph replays included)."""
         return int(self._L.fluid_stat(self._h, STAT[name]))
 
     def device_ptr(self, name) -> int:
