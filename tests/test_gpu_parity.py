@@ -629,7 +629,7 @@ def test_half_storage_every_pass_and_whole_steps_bitwise_vs_oracle(pkg, oracle):
 # half storage at every parity size and where the kernel choice changes: hs::jacobi8_kernel
 # (W % 8 == 0, W >= 64) fetches across warps only when W/8 > 32; 264 has one live lane in the second
 # warp, 520 several full warps and a partial one, 1024 four warps per row (the roofline_half_storage
-# size); W = 100 (W % 8 = 4) runs the one-cell hs::jacobi_kernel
+# size); W = 100 (W % 8 = 4) runs the one-cell jacobi_scalar_kernel<hs::StoreHalf>
 HALF_SIZES = SIZES + [(264, 40, 528, 80), (520, 33, 780, 50), (100, 60, 150, 90), (1024, 1024, 1024, 1024)]
 
 

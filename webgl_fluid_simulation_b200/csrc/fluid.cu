@@ -212,8 +212,11 @@ int need_scratch(fluid_t* h, size_t floats) {
     h->scratch_floats = floats;
     return FLUID_OK;
 }
-inline dim3 hs_grid(int W, int H) { return dim3((W + 63) / 64, (H + 3) / 4); }
-const dim3 HS_BLOCK(64, 4);
+// f(StoreF32{}) or f(hs::StoreHalf{}): a launch written once, instantiated for the handle's storage format
+template <class F>
+auto with_storage(const fluid_t* h, F&& f) {
+    return h->half ? f(hs::StoreHalf{}) : f(StoreF32{});
+}
 
 // ---- the tiny-divergence map (jacobi.cuh): one byte per 128 x 32 cells of the GLOBAL grid -------------
 int alloc_tiny_map(fluid_t* h) {
@@ -386,35 +389,21 @@ int run_jacobi(fluid_t* h, int iters, bool scale_first, int* launches_out) {
     kb = std::min(kb, KMAX);
     if (h->slab()) kb = std::max(1, std::min(kb, h->G - 1));
     const bool naive = (h->cfg.flags & FLUID_FLAG_NAIVE_JACOBI) || kb == 1;
-    if (h->half) {                                   // fp16 storage: the literal loop, every sweep rounds to fp16 (S:1253-1266)
-        const int n = W * H;
-        if (scale_first) {
-            hs::scale_kernel<<<(n + 255) / 256, 256, 0, h->stream>>>((const hs::h1*)h->pressure.read, (hs::h1*)h->pressure.write, n, h->cfg.pressure);
-            int rc = check_launch(h, "hs::scale_kernel"); if (rc) return rc;
-            swap_p(h); ++nl;
-        }
-        for (int k = 0; k < iters; ++k) {
-            if (W % 8 == 0 && W >= 64) {
-                dim3 b(32, 8), g((W / 8 + 31) / 32, (H + 7) / 8);
-                hs::jacobi8_kernel<<<g, b, 0, h->stream>>>((const hs::h1*)h->pressure.read, (const hs::h1*)h->divergence, (hs::h1*)h->pressure.write, W, H);
-            } else {
-                hs::jacobi_kernel<<<hs_grid(W, H), HS_BLOCK, 0, h->stream>>>((const hs::h1*)h->pressure.read, (const hs::h1*)h->divergence, (hs::h1*)h->pressure.write, W, H);
-            }
-            ++h->jacobi_kernel_launches;
-            int rc = check_launch(h, "hs::jacobi_kernel"); if (rc) return rc;
-            swap_p(h); ++nl;
-        }
-        if (launches_out) *launches_out = nl;
-        return FLUID_OK;
+    // clear pass alone (owned + ghost rows; ghosts are refreshed before use anyway).  Half storage always
+    // clears in a launch of its own: the reference rounds the cleared field to fp16 before the first sweep.
+    if (scale_first && (iters <= 0 || h->half)) {
+        const size_t n = sim_cells(h);
+        int rc = with_storage(h, [&](auto s) {
+            using S = decltype(s);
+            scale_kernel<S><<<(unsigned)((n + 255) / 256), 256, 0, h->stream>>>(
+                (const typename S::T1*)h->pressure.read, (typename S::T1*)h->pressure.write, n, h->cfg.pressure);
+            return check_launch(h, "scale_kernel");
+        });
+        if (rc) return rc;
+        swap_p(h); ++nl;
+        scale_first = false;
     }
     if (iters <= 0) {
-        if (scale_first) {   // clear pass alone (owned + ghost rows; ghosts are refreshed before use anyway)
-            const size_t n = sim_cells(h);
-            scale_kernel<<<(unsigned)((n + 255) / 256), 256, 0, h->stream>>>(
-                (const float*)h->pressure.read, (float*)h->pressure.write, n, h->cfg.pressure);
-            int rc = check_launch(h, "scale_kernel"); if (rc) return rc;
-            swap_p(h); ++nl;
-        }
         if (launches_out) *launches_out = nl;
         return FLUID_OK;
     }
@@ -492,9 +481,16 @@ int run_jacobi(fluid_t* h, int iters, bool scale_first, int* launches_out) {
             else jacobi_sweep_kernel<false><<<g, b, 0, h->stream>>>(a);
             ++h->jacobi_kernel_launches;
             rc = check_launch(h, "jacobi_sweep_kernel");
+        } else if (h->half && W % 8 == 0 && W >= 64) {
+            dim3 b(32, 8), g((W / 8 + 31) / 32, (H + 7) / 8);
+            hs::jacobi8_kernel<<<g, b, 0, h->stream>>>((const hs::h1*)a.pin, (const hs::h1*)a.div, (hs::h1*)a.pout, W, H);
+            ++h->jacobi_kernel_launches;
+            rc = check_launch(h, "hs::jacobi8_kernel");
         } else {
             dim3 b(64, 4);
-            jacobi_scalar_kernel<<<grid2d(W, a.out_hi - a.out_lo, b), b, 0, h->stream>>>(a, sc);
+            with_storage(h, [&](auto s) {
+                jacobi_scalar_kernel<decltype(s)><<<grid2d(W, a.out_hi - a.out_lo, b), b, 0, h->stream>>>(a, sc);
+            });
             ++h->jacobi_kernel_launches;
             rc = check_launch(h, "jacobi_scalar_kernel");
         }
@@ -502,6 +498,18 @@ int run_jacobi(fluid_t* h, int iters, bool scale_first, int* launches_out) {
         swap_p(h); ++nl;
     }
     if (launches_out) *launches_out = nl;
+    return FLUID_OK;
+}
+
+// pressure, divergence and curl of a single-GPU handle, zeroed (createFBO / createDoubleFBO, S:1004-1006)
+int alloc_scalar_fields(fluid_t* h) {
+    cudaFree(h->pressure.read); cudaFree(h->pressure.write); cudaFree(h->divergence); cudaFree(h->curl);
+    h->pressure = Pair{}; h->divergence = h->curl = nullptr;
+    const size_t bytes = sim_cells(h) * sbytes(h);
+    for (void** p : {&h->pressure.read, &h->pressure.write, (void**)&h->divergence, (void**)&h->curl}) {
+        CU(cudaMalloc(p, bytes));
+        CU(cudaMemsetAsync(*p, 0, bytes, h->stream));
+    }
     return FLUID_OK;
 }
 
@@ -530,28 +538,19 @@ int alloc_fields(fluid_t* h) {
         CU(cudaMalloc(&h->velocity.write, n * vbytes(h)));
         CU(cudaMalloc(&h->dye.read, nd * dbytes(h)));
         CU(cudaMalloc(&h->dye.write, nd * dbytes(h)));
-        CU(cudaMalloc(&h->pressure.read, n * sbytes(h)));
-        CU(cudaMalloc(&h->pressure.write, n * sbytes(h)));
-        CU(cudaMalloc((void**)&h->divergence, n * sbytes(h)));
-        CU(cudaMalloc((void**)&h->curl, n * sbytes(h)));
         CU(cudaMemsetAsync(h->velocity.read, 0, n * vbytes(h), h->stream));
         CU(cudaMemsetAsync(h->velocity.write, 0, n * vbytes(h), h->stream));
-        CU(cudaMemsetAsync(h->pressure.read, 0, n * sbytes(h), h->stream));
-        CU(cudaMemsetAsync(h->pressure.write, 0, n * sbytes(h), h->stream));
-        CU(cudaMemsetAsync(h->divergence, 0, n * sbytes(h), h->stream));
-        CU(cudaMemsetAsync(h->curl, 0, n * sbytes(h), h->stream));
+        int rc = alloc_scalar_fields(h); if (rc) return rc;
     }
     { int rc = alloc_tiny_map(h); if (rc) return rc; }
     build_tmaps(h);
     h->div_sent_epoch = 0;                               // fresh buffers: no divergence ghost rows in place yet
-    if (h->half) {
-        hs::fill_alpha_kernel<<<(unsigned)((nd + 255) / 256), 256, 0, h->stream>>>((hs::h4*)h->dye.read, nd);
-        hs::fill_alpha_kernel<<<(unsigned)((nd + 255) / 256), 256, 0, h->stream>>>((hs::h4*)h->dye.write, nd);
-    } else {
-        fill_alpha_kernel<<<(unsigned)((nd + 255) / 256), 256, 0, h->stream>>>((float4*)h->dye.read, nd);
-        fill_alpha_kernel<<<(unsigned)((nd + 255) / 256), 256, 0, h->stream>>>((float4*)h->dye.write, nd);
-    }
-    return check_launch(h, "fill_alpha_kernel", 2);
+    return with_storage(h, [&](auto s) {
+        using S = decltype(s);
+        for (void* d : {h->dye.read, h->dye.write})
+            fill_alpha_kernel<S><<<(unsigned)((nd + 255) / 256), 256, 0, h->stream>>>((typename S::T4*)d, nd);
+        return check_launch(h, "fill_alpha_kernel", 2);
+    });
 }
 
 void free_fields(fluid_t* h) {
@@ -890,39 +889,37 @@ int fluid_get_param(fluid_t* h, int key, float* v) {
 // slab); the public fluid_pass_* wrappers are the single-GPU, one-blit-per-call test surface.
 
 static int do_curl(fluid_t* h, Grid g) {
-    if (h->half) {
-        hs::curl_kernel<<<hs_grid(g.W, g.H), HS_BLOCK, 0, h->stream>>>((const hs::h2*)h->velocity.read, (hs::h1*)h->curl, g.W, g.H);
-        return check_launch(h, "hs::curl_kernel");
-    }
-    dim3 b(64, 4);
-    curl_kernel<<<grid2d(g.W, g.j_hi - g.j_lo, b), b, 0, h->stream>>>((const float2*)h->velocity.read, h->curl, g);
-    return check_launch(h, "curl_kernel");
+    return with_storage(h, [&](auto s) {
+        using S = decltype(s);
+        dim3 b(64, 4);
+        curl_kernel<S><<<grid2d(g.W, g.j_hi - g.j_lo, b), b, 0, h->stream>>>(
+            (const typename S::T2*)h->velocity.read, (typename S::T1*)h->curl, g);
+        return check_launch(h, "curl_kernel");
+    });
 }
 static int do_vorticity(fluid_t* h, Grid g) {
-    if (h->half) {
-        hs::vorticity_kernel<<<hs_grid(g.W, g.H), HS_BLOCK, 0, h->stream>>>((const hs::h2*)h->velocity.read, (const hs::h1*)h->curl,
-                                                                            (hs::h2*)h->velocity.write, g.W, g.H, h->cfg.curl, h->dt_dev);
-        int rc = check_launch(h, "hs::vorticity_kernel"); if (rc) return rc;
-        swap_v(h);
-        return FLUID_OK;
-    }
-    dim3 b(64, 4);
-    vorticity_kernel<<<grid2d(g.W, g.j_hi - g.j_lo, b), b, 0, h->stream>>>(
-        (const float2*)h->velocity.read, h->curl, (float2*)h->velocity.write, g, h->cfg.curl, h->dt_dev);
-    int rc = check_launch(h, "vorticity_kernel"); if (rc) return rc;
+    int rc = with_storage(h, [&](auto s) {
+        using S = decltype(s);
+        dim3 b(64, 4);
+        vorticity_kernel<S><<<grid2d(g.W, g.j_hi - g.j_lo, b), b, 0, h->stream>>>(
+            (const typename S::T2*)h->velocity.read, (const typename S::T1*)h->curl, (typename S::T2*)h->velocity.write, g,
+            h->cfg.curl, h->dt_dev);
+        return check_launch(h, "vorticity_kernel");
+    });
+    if (rc) return rc;
     swap_v(h);                                   // S:1246
     return FLUID_OK;
 }
 static int do_divergence(fluid_t* h, Grid g) {
-    if (h->half) {
-        hs::divergence_kernel<<<hs_grid(g.W, g.H), HS_BLOCK, 0, h->stream>>>((const hs::h2*)h->velocity.read, (hs::h1*)h->divergence, g.W, g.H);
-        return check_launch(h, "hs::divergence_kernel");
-    }
-    dim3 b(64, 4);
-    { int rc = clear_tiny_map(h); if (rc) return rc; }
-    divergence_kernel<<<grid2d(g.W, g.j_hi - g.j_lo, b), b, 0, h->stream>>>(
-        (const float2*)h->velocity.read, h->divergence, g, h->tiny_map);
-    return check_launch(h, "divergence_kernel");
+    // half storage never runs the contracted Jacobi tail, so it keeps no tiny-divergence map
+    if (!h->half) { int rc = clear_tiny_map(h); if (rc) return rc; }
+    return with_storage(h, [&](auto s) {
+        using S = decltype(s);
+        dim3 b(64, 4);
+        divergence_kernel<S><<<grid2d(g.W, g.j_hi - g.j_lo, b), b, 0, h->stream>>>(
+            (const typename S::T2*)h->velocity.read, (typename S::T1*)h->divergence, g, h->half ? nullptr : h->tiny_map);
+        return check_launch(h, "divergence_kernel");
+    });
 }
 // rows per warp stream of the row-streaming kernels: one full wave of resident warps (`warps_per_sm`
 // from the occupancy calculator), at least `rmin` rows each so that the halo rows a stream re-reads
@@ -942,7 +939,7 @@ static int stream_warps(const StreamArgs& a) {
     return a.nxw * ((a.g.j_hi - a.g.j_lo + a.rows_per_chunk - 1) / a.rows_per_chunk);
 }
 static bool streaming_ok(const fluid_t* h) {
-    return h->cfg.sim_w % 4 == 0 && h->cfg.sim_w >= 8 && !(h->cfg.flags & FLUID_FLAG_TILED_PASSES);
+    return !h->half && h->cfg.sim_w % 4 == 0 && h->cfg.sim_w >= 8 && !(h->cfg.flags & FLUID_FLAG_TILED_PASSES);
 }
 
 static int do_curl(fluid_t* h, Grid g);
@@ -982,13 +979,6 @@ static int do_cvd(fluid_t* h, Grid g) {
     return FLUID_OK;
 }
 static int do_gradient(fluid_t* h, Grid g) {
-    if (h->half) {
-        hs::gradient_kernel<<<hs_grid(g.W, g.H), HS_BLOCK, 0, h->stream>>>((const hs::h1*)h->pressure.read, (const hs::h2*)h->velocity.read,
-                                                                           (hs::h2*)h->velocity.write, g.W, g.H);
-        int rc = check_launch(h, "hs::gradient_kernel"); if (rc) return rc;
-        swap_v(h);
-        return FLUID_OK;
-    }
     const StreamArgs a = stream_args(h, g, 128, 8, 32, GS_U);
     const int nwarps = stream_warps(a);
     if (streaming_ok(h) && nwarps >= h->sm_count) {
@@ -999,10 +989,14 @@ static int do_gradient(fluid_t* h, Grid g) {
         swap_v(h);                                   // S:1273
         return FLUID_OK;
     }
-    dim3 b(64, 4);
-    gradient_subtract_kernel<<<grid2d(g.W, g.j_hi - g.j_lo, b), b, 0, h->stream>>>(
-        (const float*)h->pressure.read, (const float2*)h->velocity.read, (float2*)h->velocity.write, g);
-    int rc = check_launch(h, "gradient_subtract_kernel"); if (rc) return rc;
+    int rc = with_storage(h, [&](auto s) {
+        using S = decltype(s);
+        dim3 b(64, 4);
+        gradient_subtract_kernel<S><<<grid2d(g.W, g.j_hi - g.j_lo, b), b, 0, h->stream>>>(
+            (const typename S::T1*)h->pressure.read, (const typename S::T2*)h->velocity.read, (typename S::T2*)h->velocity.write, g);
+        return check_launch(h, "gradient_subtract_kernel");
+    });
+    if (rc) return rc;
     swap_v(h);                                   // S:1273
     return FLUID_OK;
 }
@@ -1011,15 +1005,6 @@ static void valid_rows(int r0, int r1, int g, int H, int* lo, int* hi) {
     *lo = std::max(r0 - g, 0); *hi = std::min(r1 + g, H);
 }
 static int do_advect_velocity(fluid_t* h, Grid out) {
-    if (h->half) {
-        hs::advect_kernel<hs::h2, float2><<<hs_grid(out.W, out.H), HS_BLOCK, 0, h->stream>>>(
-            (const hs::h2*)h->velocity.read, out.W, out.H, (const hs::h2*)h->velocity.read, (hs::h2*)h->velocity.write, out.W, out.H,
-            h->dt_dev, h->cfg.velocity_dissipation, (float)(1.0 / (double)out.W), (float)(1.0 / (double)out.H),
-            (float)(1.0 / (double)out.W), (float)(1.0 / (double)out.H));
-        int rc = check_launch(h, "hs::advect_kernel"); if (rc) return rc;
-        swap_v(h);
-        return FLUID_OK;
-    }
     dim3 b(64, 4);
     AdvectArgs a{};
     a.vel = sim_grid(h); a.src = out;
@@ -1027,29 +1012,24 @@ static int do_advect_velocity(fluid_t* h, Grid out) {
     a.src_lo = a.vel_lo; a.src_hi = a.vel_hi;
     a.dtp = h->dt_dev; a.dissipation = h->cfg.velocity_dissipation; a.halo_violation = h->halo_flag;
     a.tsx = a.dsx = (float)(1.0 / (double)h->cfg.sim_w); a.tsy = a.dsy = (float)(1.0 / (double)h->cfg.sim_h);
-    const bool p2 = is_pow2(h->cfg.sim_w) && is_pow2(h->cfg.sim_h);
+    // half storage: the !POW2 kernel, which bilerps the own-texel velocity like the reference (passes.cuh)
+    const bool p2 = !h->half && is_pow2(h->cfg.sim_w) && is_pow2(h->cfg.sim_h);
     if (p2 && h->cfg.sim_w >= 128 && !(h->cfg.flags & FLUID_FLAG_TILED_PASSES)) {    // 4 cells per thread, 32 apart
         dim3 b4(32, 8), g4(out.W / 128, (out.j_hi - out.j_lo + 7) / 8);
         if (h->slab()) advect_velocity4_kernel<true><<<g4, b4, 0, h->stream>>>((const float2*)h->velocity.read, (float2*)h->velocity.write, a);
         else advect_velocity4_kernel<false><<<g4, b4, 0, h->stream>>>((const float2*)h->velocity.read, (float2*)h->velocity.write, a);
-    } else if (p2) advect_velocity_kernel<true><<<grid2d(out.W, out.j_hi - out.j_lo, b), b, 0, h->stream>>>(
+    } else if (p2) advect_velocity_kernel<StoreF32, true><<<grid2d(out.W, out.j_hi - out.j_lo, b), b, 0, h->stream>>>(
         (const float2*)h->velocity.read, (float2*)h->velocity.write, a);
-    else advect_velocity_kernel<false><<<grid2d(out.W, out.j_hi - out.j_lo, b), b, 0, h->stream>>>(
-        (const float2*)h->velocity.read, (float2*)h->velocity.write, a);
+    else with_storage(h, [&](auto s) {
+        using S = decltype(s);
+        advect_velocity_kernel<S, false><<<grid2d(out.W, out.j_hi - out.j_lo, b), b, 0, h->stream>>>(
+            (const typename S::T2*)h->velocity.read, (typename S::T2*)h->velocity.write, a);
+    });
     int rc = check_launch(h, "advect_velocity_kernel"); if (rc) return rc;
     swap_v(h);                                   // S:1285
     return FLUID_OK;
 }
 static int do_advect_dye(fluid_t* h) {
-    if (h->half) {
-        hs::advect_kernel<hs::h4, float4><<<hs_grid(h->cfg.dye_w, h->cfg.dye_h), HS_BLOCK, 0, h->stream>>>(
-            (const hs::h2*)h->velocity.read, h->cfg.sim_w, h->cfg.sim_h, (const hs::h4*)h->dye.read, (hs::h4*)h->dye.write,
-            h->cfg.dye_w, h->cfg.dye_h, h->dt_dev, h->cfg.density_dissipation, (float)(1.0 / (double)h->cfg.sim_w),
-            (float)(1.0 / (double)h->cfg.sim_h), (float)(1.0 / (double)h->cfg.dye_w), (float)(1.0 / (double)h->cfg.dye_h));
-        int rc = check_launch(h, "hs::advect_kernel"); if (rc) return rc;
-        swap_dye(h);
-        return FLUID_OK;
-    }
     dim3 b(64, 4);
     AdvectArgs a{};
     a.vel = sim_grid(h); a.src = dye_grid(h);
@@ -1059,7 +1039,7 @@ static int do_advect_dye(fluid_t* h) {
     a.dtp = h->dt_dev; a.dissipation = h->cfg.density_dissipation; a.halo_violation = h->halo_flag;
     a.tsx = (float)(1.0 / (double)h->cfg.sim_w); a.tsy = (float)(1.0 / (double)h->cfg.sim_h);
     a.dsx = (float)(1.0 / (double)h->cfg.dye_w); a.dsy = (float)(1.0 / (double)h->cfg.dye_h);
-    const bool p2 = is_pow2(h->cfg.sim_w) && is_pow2(h->cfg.sim_h) && is_pow2(h->cfg.dye_w) && is_pow2(h->cfg.dye_h);
+    const bool p2 = !h->half && is_pow2(h->cfg.sim_w) && is_pow2(h->cfg.sim_h) && is_pow2(h->cfg.dye_w) && is_pow2(h->cfg.dye_h);
     const bool same = h->cfg.sim_w == h->cfg.dye_w && h->cfg.sim_h == h->cfg.dye_h;
     const dim3 gr = grid2d(a.src.W, a.src.j_hi - a.src.j_lo, b);
     const float2* V = (const float2*)h->velocity.read; const float4* Dr = (const float4*)h->dye.read; float4* Dw = (float4*)h->dye.write;
@@ -1069,9 +1049,13 @@ static int do_advect_dye(fluid_t* h) {
         else if (same) advect_dye4_kernel<true, false><<<g4, b4, 0, h->stream>>>(V, Dr, Dw, a);
         else if (h->slab()) advect_dye4_kernel<false, true><<<g4, b4, 0, h->stream>>>(V, Dr, Dw, a);
         else advect_dye4_kernel<false, false><<<g4, b4, 0, h->stream>>>(V, Dr, Dw, a);
-    } else if (p2 && same) advect_dye_kernel<true, true><<<gr, b, 0, h->stream>>>(V, Dr, Dw, a);
-    else if (p2) advect_dye_kernel<true, false><<<gr, b, 0, h->stream>>>(V, Dr, Dw, a);
-    else advect_dye_kernel<false, false><<<gr, b, 0, h->stream>>>(V, Dr, Dw, a);
+    } else if (p2 && same) advect_dye_kernel<StoreF32, true, true><<<gr, b, 0, h->stream>>>(V, Dr, Dw, a);
+    else if (p2) advect_dye_kernel<StoreF32, true, false><<<gr, b, 0, h->stream>>>(V, Dr, Dw, a);
+    else with_storage(h, [&](auto s) {
+        using S = decltype(s);
+        advect_dye_kernel<S, false, false><<<gr, b, 0, h->stream>>>(
+            (const typename S::T2*)h->velocity.read, (const typename S::T4*)h->dye.read, (typename S::T4*)h->dye.write, a);
+    });
     int rc = check_launch(h, "advect_dye_kernel"); if (rc) return rc;
     swap_dye(h);                                        // S:1293
     return FLUID_OK;
@@ -1267,13 +1251,13 @@ int fluid_splats(fluid_t* h, const float* splats, int n) {
         // the first launch reads .read; the next ones continue in place on .write
         const void* vin = k0 ? h->velocity.write : h->velocity.read;
         const void* din = k0 ? h->dye.write : h->dye.read;
-        if (h->half)
-            splats_kernel<hs::SplatHalf><<<blocks, 256, 0, h->stream>>>((const hs::h2*)vin, (hs::h2*)h->velocity.write,
-                                                                         (const hs::h4*)din, (hs::h4*)h->dye.write, a);
-        else
-            splats_kernel<SplatF32><<<blocks, 256, 0, h->stream>>>((const float2*)vin, (float2*)h->velocity.write,
-                                                                    (const float4*)din, (float4*)h->dye.write, a);
-        int rc = check_launch(h, "splats_kernel"); if (rc) return rc;
+        int rc = with_storage(h, [&](auto s) {
+            using S = decltype(s);
+            splats_kernel<S><<<blocks, 256, 0, h->stream>>>((const typename S::T2*)vin, (typename S::T2*)h->velocity.write,
+                                                            (const typename S::T4*)din, (typename S::T4*)h->dye.write, a);
+            return check_launch(h, "splats_kernel");
+        });
+        if (rc) return rc;
     }
     swap_v(h);                                   // S:1449
     swap_dye(h);                                 // S:1454
@@ -1330,83 +1314,44 @@ int fluid_resize(fluid_t* h, int sim_w, int sim_h, int dye_w, int dye_h) {
     }
     CU(cudaStreamSynchronize(h->stream));
     drop_graphs(h);                                          // graphs hold the old buffers' addresses
-    if (h->half) {
-        // fp16 storage: widen the old texture, draw the copy through the LINEAR sampler in fp32, round the
-        // new texture to fp16 (what the reference's blit into an RGBA16F / RG16F target does)
-        auto redo = [&](Pair& f, int ow_, int oh_, int nw_, int nh_, int ch, bool alpha) -> int {
-            const size_t on = (size_t)ow_ * oh_ * ch, nn = (size_t)nw_ * nh_ * ch;
-            float *wide = nullptr, *res = nullptr; void *nr = nullptr, *nwp = nullptr;
-            CU(cudaMalloc((void**)&wide, on * 4)); CU(cudaMalloc((void**)&res, nn * 4));
-            CU(cudaMalloc(&nr, nn * 2)); CU(cudaMalloc(&nwp, nn * 2));
-            hs::widen_kernel<<<(unsigned)((on + 255) / 256), 256, 0, h->stream>>>((const hs::h1*)f.read, wide, on);
-            dim3 b(64, 4);
-            if (ch == 4) resample_kernel<float4><<<grid2d(nw_, nh_, b), b, 0, h->stream>>>((const float4*)wide, ow_, oh_, (float4*)res, nw_, nh_);
-            else resample_kernel<float2><<<grid2d(nw_, nh_, b), b, 0, h->stream>>>((const float2*)wide, ow_, oh_, (float2*)res, nw_, nh_);
-            hs::narrow_kernel<<<(unsigned)((nn + 255) / 256), 256, 0, h->stream>>>(res, (hs::h1*)nr, nn);
-            if (alpha) hs::fill_alpha_kernel<<<(unsigned)((nn / 4 + 255) / 256), 256, 0, h->stream>>>((hs::h4*)nwp, nn / 4);
-            else CU(cudaMemsetAsync(nwp, 0, nn * 2, h->stream));
-            int rc = check_launch(h, "half resize", 3); if (rc) return rc;
-            CU(cudaStreamSynchronize(h->stream));
-            cudaFree(wide); cudaFree(res); cudaFree(f.read); cudaFree(f.write);
-            f.read = nr; f.write = nwp;
-            return FLUID_OK;
-        };
-        const int ow = h->cfg.sim_w, oh = h->cfg.sim_h, odw = h->cfg.dye_w, odh = h->cfg.dye_h;
-        int rc;
-        if ((dye_w != odw || dye_h != odh) && (rc = redo(h->dye, odw, odh, dye_w, dye_h, 4, true))) return rc;
-        if ((sim_w != ow || sim_h != oh) && (rc = redo(h->velocity, ow, oh, sim_w, sim_h, 2, false))) return rc;
-        const size_t n = (size_t)sim_w * sim_h;
-        cudaFree(h->pressure.read); cudaFree(h->pressure.write); cudaFree(h->divergence); cudaFree(h->curl);
-        h->pressure = Pair{}; h->divergence = h->curl = nullptr;
-        CU(cudaMalloc(&h->pressure.read, n * 2)); CU(cudaMalloc(&h->pressure.write, n * 2));
-        CU(cudaMalloc((void**)&h->divergence, n * 2)); CU(cudaMalloc((void**)&h->curl, n * 2));
-        CU(cudaMemsetAsync(h->pressure.read, 0, n * 2, h->stream)); CU(cudaMemsetAsync(h->pressure.write, 0, n * 2, h->stream));
-        CU(cudaMemsetAsync(h->divergence, 0, n * 2, h->stream)); CU(cudaMemsetAsync(h->curl, 0, n * 2, h->stream));
-        h->cfg.sim_w = sim_w; h->cfg.sim_h = sim_h; h->cfg.dye_w = dye_w; h->cfg.dye_h = dye_h;
-        h->row0 = 0; h->row1 = sim_h; h->drow0 = 0; h->drow1 = dye_h;
-        return alloc_tiny_map(h);
-    }
+    // velocity and dye: the LINEAR copy of the old texture, written to the new one in the storage format
+    // (in half storage the reference's blit into an RG16F / RGBA16F target rounds to fp16)
     const int ow = h->cfg.sim_w, oh = h->cfg.sim_h, odw = h->cfg.dye_w, odh = h->cfg.dye_h;
-    dim3 b(64, 4);
     const size_t n = (size_t)sim_w * sim_h, nd = (size_t)dye_w * dye_h;
-    if (dye_w != odw || dye_h != odh) {
-        float4 *nr = nullptr, *nw = nullptr;
-        CU(cudaMalloc((void**)&nr, nd * sizeof(float4)));
-        CU(cudaMalloc((void**)&nw, nd * sizeof(float4)));
-        resample_kernel<float4><<<grid2d(dye_w, dye_h, b), b, 0, h->stream>>>(
-            (const float4*)h->dye.read, odw, odh, nr, dye_w, dye_h);
-        fill_alpha_kernel<<<(unsigned)((nd + 255) / 256), 256, 0, h->stream>>>(nw, nd);
-        int rc = check_launch(h, "resample_kernel", 2); if (rc) return rc;
-        CU(cudaStreamSynchronize(h->stream));
-        cudaFree(h->dye.read); cudaFree(h->dye.write);
-        h->dye.read = nr; h->dye.write = nw;
-    }
-    if (sim_w != ow || sim_h != oh) {
-        float2 *nr = nullptr, *nw = nullptr;
-        CU(cudaMalloc((void**)&nr, n * sizeof(float2)));
-        CU(cudaMalloc((void**)&nw, n * sizeof(float2)));
-        resample_kernel<float2><<<grid2d(sim_w, sim_h, b), b, 0, h->stream>>>(
-            (const float2*)h->velocity.read, ow, oh, nr, sim_w, sim_h);
-        int rc = check_launch(h, "resample_kernel"); if (rc) return rc;
-        CU(cudaMemsetAsync(nw, 0, n * sizeof(float2), h->stream));
-        CU(cudaStreamSynchronize(h->stream));
-        cudaFree(h->velocity.read); cudaFree(h->velocity.write);
-        h->velocity.read = nr; h->velocity.write = nw;
-    }
-    // divergence, curl, pressure are always re-created (createFBO / createDoubleFBO, S:1004-1006)
-    cudaFree(h->pressure.read); cudaFree(h->pressure.write); cudaFree(h->divergence); cudaFree(h->curl);
-    h->pressure = Pair{}; h->divergence = h->curl = nullptr;
-    CU(cudaMalloc(&h->pressure.read, n * sizeof(float)));
-    CU(cudaMalloc(&h->pressure.write, n * sizeof(float)));
-    CU(cudaMalloc((void**)&h->divergence, n * sizeof(float)));
-    CU(cudaMalloc((void**)&h->curl, n * sizeof(float)));
-    CU(cudaMemsetAsync(h->pressure.read, 0, n * sizeof(float), h->stream));
-    CU(cudaMemsetAsync(h->pressure.write, 0, n * sizeof(float), h->stream));
-    CU(cudaMemsetAsync(h->divergence, 0, n * sizeof(float), h->stream));
-    CU(cudaMemsetAsync(h->curl, 0, n * sizeof(float), h->stream));
+    int rc = with_storage(h, [&](auto s) -> int {
+        using S = decltype(s);
+        typedef typename S::T2 V;
+        typedef typename S::T4 D;
+        dim3 b(64, 4);
+        if (dye_w != odw || dye_h != odh) {
+            void *nr = nullptr, *nw = nullptr;
+            CU(cudaMalloc(&nr, nd * dbytes(h)));
+            CU(cudaMalloc(&nw, nd * dbytes(h)));
+            resample_kernel<S><<<grid2d(dye_w, dye_h, b), b, 0, h->stream>>>((const D*)h->dye.read, odw, odh, (D*)nr, dye_w, dye_h);
+            fill_alpha_kernel<S><<<(unsigned)((nd + 255) / 256), 256, 0, h->stream>>>((D*)nw, nd);
+            int rc = check_launch(h, "resample_kernel", 2); if (rc) return rc;
+            CU(cudaStreamSynchronize(h->stream));
+            cudaFree(h->dye.read); cudaFree(h->dye.write);
+            h->dye.read = nr; h->dye.write = nw;
+        }
+        if (sim_w != ow || sim_h != oh) {
+            void *nr = nullptr, *nw = nullptr;
+            CU(cudaMalloc(&nr, n * vbytes(h)));
+            CU(cudaMalloc(&nw, n * vbytes(h)));
+            resample_kernel<S><<<grid2d(sim_w, sim_h, b), b, 0, h->stream>>>((const V*)h->velocity.read, ow, oh, (V*)nr, sim_w, sim_h);
+            int rc = check_launch(h, "resample_kernel"); if (rc) return rc;
+            CU(cudaMemsetAsync(nw, 0, n * vbytes(h), h->stream));
+            CU(cudaStreamSynchronize(h->stream));
+            cudaFree(h->velocity.read); cudaFree(h->velocity.write);
+            h->velocity.read = nr; h->velocity.write = nw;
+        }
+        return FLUID_OK;
+    });
+    if (rc) return rc;
     h->cfg.sim_w = sim_w; h->cfg.sim_h = sim_h; h->cfg.dye_w = dye_w; h->cfg.dye_h = dye_h;
     h->row0 = 0; h->row1 = sim_h; h->drow0 = 0; h->drow1 = dye_h; h->roff = 0; h->droff = 0;
-    { int rc = alloc_tiny_map(h); if (rc) return rc; }
+    if ((rc = alloc_scalar_fields(h))) return rc;
+    if ((rc = alloc_tiny_map(h))) return rc;
     build_tmaps(h);
     return FLUID_OK;
 }

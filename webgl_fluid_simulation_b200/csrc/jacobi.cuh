@@ -54,6 +54,9 @@ struct __align__(64) TmapPair {
 };
 
 // ------------------------------------------------------------------------------------------------
+// S: storage policy (passes.cuh).  The pointers of JacobiArgs address S::T1 elements: fp16 ones in
+// half storage, where do_scale is false (the clear pass is a launch of its own there).
+template <class S>
 __global__ void __launch_bounds__(256) jacobi_scalar_kernel(JacobiArgs a, bool do_scale) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     const int j = a.out_lo + blockIdx.y * blockDim.y + threadIdx.y;
@@ -61,11 +64,14 @@ __global__ void __launch_bounds__(256) jacobi_scalar_kernel(JacobiArgs a, bool d
     const int il = max(i - 1, 0), ir = min(i + 1, a.W - 1);
     const int jb = max(j - 1, 0) - a.row_off, jt = min(j + 1, a.H - 1) - a.row_off;
     const int jl = j - a.row_off;
+    const auto* pin = reinterpret_cast<const typename S::T1*>(a.pin);
+    const auto* div = reinterpret_cast<const typename S::T1*>(a.div);
     const float s = do_scale ? a.scale : 1.0f;
-    float L = a.pin[(size_t)jl * a.W + il], R = a.pin[(size_t)jl * a.W + ir];
-    float B = a.pin[(size_t)jb * a.W + i], T = a.pin[(size_t)jt * a.W + i];
+    float L = S::ld(pin, (size_t)jl * a.W + il), R = S::ld(pin, (size_t)jl * a.W + ir);
+    float B = S::ld(pin, (size_t)jb * a.W + i), T = S::ld(pin, (size_t)jt * a.W + i);
     if (do_scale) { L = s * L; R = s * R; B = s * B; T = s * T; }
-    a.pout[(size_t)jl * a.W + i] = ((((L + R) + B) + T) - a.div[(size_t)jl * a.W + i]) * 0.25f;
+    S::st(reinterpret_cast<typename S::T1*>(a.pout), (size_t)jl * a.W + i,
+          ((((L + R) + B) + T) - S::ld(div, (size_t)jl * a.W + i)) * 0.25f);
 }
 
 // ------------------------------------------------------------------------------------------------
