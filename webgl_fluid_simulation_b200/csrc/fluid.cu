@@ -242,7 +242,12 @@ int scan_tiny(fluid_t* h, int j_lo, int j_hi) {
 
 // ---- Jacobi dispatch -----------------------------------------------------------------------------
 
+// Temporal-block depths: default 10, at most KMAX (slab.py mirrors both).  A single-GPU solve staged
+// by TMA goes one deeper, KMAX_TMA (measurements at run_jacobi): its instantiation fits 255 registers
+// without spills, while the cp.async-staged one spills at that depth and is never instantiated.
 constexpr int KMAX = 12;
+constexpr int K_DEFAULT = 10;
+constexpr int KMAX_TMA = 13;
 
 // cuTensorMapEncodeTiled through the runtime (no link-time dependency on libcuda)
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -321,9 +326,11 @@ int launch_tb(fluid_t* h, const JacobiArgs& a) {
         memcpy(maps.d, &h->tmaps.d, sizeof(CUtensorMap));
         lc.dynamicSmemBytes = T::SMEM_TMA;
         cudaLaunchKernelEx(&lc, jacobi_tb_kernel<K, SCALE, true>, a, maps);
-    } else {
+    } else if constexpr (K <= KMAX) {
         lc.dynamicSmemBytes = T::SMEM_LDGSTS;
         cudaLaunchKernelEx(&lc, jacobi_tb_kernel<K, SCALE, false>, a, maps);
+    } else {
+        return fail(h, FLUID_ERR_INVALID, "temporal block depth %d needs TMA staging", K);
     }
     ++h->jacobi_kernel_launches;
     return check_launch(h, "jacobi_tb_kernel");
@@ -342,7 +349,8 @@ int tb_rows(const fluid_t* h, int W, int rows) {
     using T = TB<K>;
     const int nxw = (W + T::VALID - 1) / T::VALID;
     int occ = 0;
-    if (tb_use_tma(h)) cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, jacobi_tb_kernel<K, false, true>, 32, T::SMEM_TMA);
+    if constexpr (K > KMAX) cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, jacobi_tb_kernel<K, false, true>, 32, T::SMEM_TMA);
+    else if (tb_use_tma(h)) cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, jacobi_tb_kernel<K, false, true>, 32, T::SMEM_TMA);
     else cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, jacobi_tb_kernel<K, false, false>, 32, T::SMEM_LDGSTS);
     if (occ < 1) occ = 1;
     if (h->jacobi_warps_per_sm > 0) occ = std::min(occ, h->jacobi_warps_per_sm);
@@ -361,6 +369,7 @@ int launch_tb_dyn(fluid_t* h, int K, JacobiArgs a, bool scale) {
     switch (K) {
 #define CASE(KK) case KK: a.rows_per_chunk = tb_rows<KK>(h, a.W, rows); return launch_tb_k<KK>(h, a, scale);
         CASE(1) CASE(2) CASE(3) CASE(4) CASE(5) CASE(6) CASE(7) CASE(8) CASE(9) CASE(10) CASE(11) CASE(12)
+        CASE(13)
 #undef CASE
     }
     return fail(h, FLUID_ERR_INVALID, "temporal block depth %d out of range", K);
@@ -383,10 +392,12 @@ int run_jacobi(fluid_t* h, int iters, bool scale_first, int* launches_out) {
     a.scale = h->cfg.pressure;
     a.err = h->halo_flag;
     a.tiny_map = h->tiny_map;
-    // default depth: on an H100 SXM at 4096^2 x 50 the solve time falls with K up to 10 (TMA staging: 0.605 ms
-    // at K = 8, 0.515 at 9, 0.446 at 10) and is flat beyond it (0.446 at 11 and 12)
-    int kb = h->cfg.jacobi_block > 0 ? h->cfg.jacobi_block : 10;
-    kb = std::min(kb, KMAX);
+    // default depth: on an H100 at 4096^2 x 50 (TMA staging) 4 launches of 13 / 12 sweeps take 0.500 ms per
+    // solve and 5 launches of 10 take 0.524 (80 GB HBM3 card, 400 W power limit; DESIGN §5).  Iteration
+    // counts that split into the same number of launches either way (20, 30, 40) keep depth 10 launches.
+    const bool tma13 = !h->slab() && tb_use_tma(h);
+    int kb = h->cfg.jacobi_block > 0 ? h->cfg.jacobi_block : (tma13 ? KMAX_TMA : K_DEFAULT);
+    kb = std::min(kb, tma13 ? KMAX_TMA : KMAX);
     if (h->slab()) kb = std::max(1, std::min(kb, h->G - 1));
     const bool naive = (h->cfg.flags & FLUID_FLAG_NAIVE_JACOBI) || kb == 1;
     // clear pass alone (owned + ghost rows; ghosts are refreshed before use anyway).  Half storage always
@@ -1429,7 +1440,7 @@ int solve_host_banded(fluid_t* h, const float* div_host, float* p_host, int iter
         for (auto& e : hp.ev_up) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
         for (auto& e : hp.ev_done) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
     }
-    int kb = h->cfg.jacobi_block > 0 ? h->cfg.jacobi_block : 10;
+    int kb = h->cfg.jacobi_block > 0 ? h->cfg.jacobi_block : K_DEFAULT;
     kb = std::min(kb, KMAX);
     const int nlaunch = (iters + kb - 1) / kb;
     const int base = iters / nlaunch, extra = iters % nlaunch;
