@@ -550,10 +550,12 @@ __global__ void FLUID_TB_BOUNDS jacobi_tb_kernel(JacobiArgs a, const __grid_cons
     const void* td = &maps.d;
     // The common case first, so that it is laid out first: code placement matters to this kernel (it
     // runs one or two warps per scheduler, straight out of the instruction caches).  The un-contracted
-    // instantiations are kept out of line for the same reason.
+    // instantiations are kept out of line for the same reason.  Every contracted stream, mirrored
+    // window or not, runs ONE instantiation (REV: 8 selects per step, the identity where rev is false):
+    // an SM whose resident warps ran two separate steady-state loops would keep two loop bodies in its
+    // instruction cache, and a loop body twice as large measured 11 % slower (DESIGN §5.8).
     if (!exact) {
-        if (!any_rev) tb_stream<K, SCALE, false, false, TMA>(a, tp, td, smem4, lane, x0, lc, gx, rev, lane_out, y0, y1, ys, ye);
-        else tb_stream<K, SCALE, true, false, TMA>(a, tp, td, smem4, lane, x0, lc, gx, rev, lane_out, y0, y1, ys, ye);
+        tb_stream<K, SCALE, true, false, TMA>(a, tp, td, smem4, lane, x0, lc, gx, rev, lane_out, y0, y1, ys, ye);
     } else {
         tb_stream_exact<K, SCALE, TMA>(a, tp, td, smem4, lane, x0, lc, gx, rev, lane_out, y0, y1, ys, ye, any_rev);
     }
