@@ -574,9 +574,11 @@ void oracle_sim_step(oracle_sim* s, float dt) {
 /* splat(x,y,dx,dy,color), S:1441-1455, radius = correctRadius(SPLAT_RADIUS/100), S:1457-1462 */
 void oracle_sim_splat(oracle_sim* s, float x, float y, float dx, float dy, float r, float g,
                       float b) {
-    /* JS evaluates correctRadius() in double and gl.uniform1f narrows it to fp32 */
+    /* JS evaluates correctRadius() in double and gl.uniform1f narrows it to fp32.  The aspect is
+     * the double canvas ratio: widening the fp32 s->aspect can move the radius by an ulp (142x100). */
     double rad = (double)s->splat_radius / 100.0;
-    if (s->aspect > 1.0f) rad *= (double)s->aspect;
+    const double aspect = (double)s->W / (double)s->H;
+    if (aspect > 1.0) rad *= aspect;
     const float radius = (float)rad;
     const float cv[3] = {dx, dy, 0.0f};
     oracle_splat(s->v, s->v2, s->W, s->H, 2, s->aspect, x, y, cv, radius);

@@ -3,6 +3,7 @@ vectors.  Bitwise for every pass whose arithmetic is IEEE-exact (all but splat's
 import numpy as np
 import pytest
 
+import splat_model as M
 from conftest import bits_equal, golden, max_rel
 
 pytestmark = pytest.mark.gpu
@@ -59,11 +60,13 @@ def test_every_pass_bitwise_vs_oracle(pkg, oracle, W, H, Wd, Hd):
     s.pass_("advect_dye", DT); d2 = s.readField("dye")
     assert bits_equal(d2, O.advect(v4, dye, DT, 1.0))
     s.splat(0.3, 0.6, 123.0, -456.0, (0.5, 0.2, 0.9))
-    rad = O.correct_radius(0.25, W / H)
-    assert max_rel(s.readField("velocity"), O.splat(v4, W / H, 0.3, 0.6, (123.0, -456.0, 0), rad)) < SPLAT_TOL
-    sd = s.readField("dye")
-    assert max_rel(sd, O.splat(d2, W / H, 0.3, 0.6, (0.5, 0.2, 0.9), rad)) < SPLAT_TOL
-    assert np.all(sd[..., 3] == 1.0)
+    # splat: every texel within the fp32 shader arithmetic with an expf inside EXPF_ULP (splat_model)
+    rec = np.array([[0.3, 0.6, 123.0, -456.0, 0.5, 0.2, 0.9]], np.float32)
+    aspect, rad = M.aspect_of(W, H), M.radius_of(0.25, W, H)
+    for name, base in (("velocity", v4), ("dye", d2)):
+        n, bad = M.check_splat(s.readField(name), *M.splat_interval(base, rec, aspect, rad))
+        assert n == 0, (name, n, bad)
+    assert np.all(s.readField("dye")[..., 3] == 1.0)
     s.close()
 
 

@@ -83,6 +83,19 @@ def test_c_step_equals_python_orchestration(oracle):
     b.close()
 
 
+def test_c_splat_equals_python_splat_when_the_radius_depends_on_the_aspect_narrowing(oracle):
+    """oracle_sim_splat == OracleSim.splat, bitwise, on a 142x100 grid: correctRadius multiplies by the
+    aspect in double, and float32(142 / 100) widened back to double gives a radius one ulp lower."""
+    O = oracle
+    a = O.OracleSim(142, 100, 142, 100)
+    b = O.OracleSimC(142, 100, 142, 100)
+    for rec in ((0.3, 0.6, 123.0, -456.0, 0.5, 0.2, 0.9), (0.71, 0.2, -40.0, 7.0, 1.2, -0.3, 0.05)):
+        a.splat(*rec); b.splat(*rec)
+    for n in ("velocity", "dye"):
+        assert bits_equal(getattr(a, n), b.field(n)), n
+    b.close()
+
+
 def test_p4_report_distance_to_desktop_webgl(oracle, capsys):
     """REPORT ONLY (never gates): distance from the fp32 oracle to the reference as a desktop
     browser runs it (LINEAR samplers, half-float textures).  Bounds are loose sanity rails."""
