@@ -1,5 +1,5 @@
 """Lane-level numpy model of csrc/jacobi.cuh::jacobi_tb_kernel — same window geometry, mirrored
-loads, D-deep staging ring, 3-slot rotating windows, shifted K+3-slot div register ring, wall selects,
+loads, staged 128-column boxes, 3-slot rotating windows, shifted K+3-slot div register ring, wall selects,
 chunking and store predicate, statement for statement.  It exists so the kernel's index logic can be checked against the oracle
 on a machine without a GPU (tests/test_jacobi_tb_model.py); it is not used by the product."""
 import numpy as np
@@ -32,7 +32,7 @@ def jacobi_tb_model(pin, div, K, rows_per_chunk, scale=None, row_off=0, out_lo=N
     H = rows_local if H is None else H
     out_lo = 0 if out_lo is None else out_lo
     out_hi = H if out_hi is None else out_hi
-    HX = (K + 3) // 4 * 4; VALID = 128 - 2 * HX; RD = K + 3; U = 3; D = 8
+    HX = (K + 3) // 4 * 4; VALID = 128 - 2 * HX; RD = K + 3; U = 3
     assert W % 4 == 0 and W >= 16
     if pout is None:
         pout = np.full_like(pin, np.nan)
@@ -49,34 +49,28 @@ def jacobi_tb_model(pin, div, K, rows_per_chunk, scale=None, row_off=0, out_lo=N
         lane_out = (lane >= HX // 4) & (lane < 32 - HX // 4) & (gx >= 0) & (gx < W)
         y0 = out_lo + cy * rows_per_chunk
         y1 = min(y0 + rows_per_chunk, out_hi)
-        ys = max(y0 - K, 0); ye = min(y1 - 1 + K, H - 1)
+        ys = max(y0 - K, 0)
         nsteps = y1 - ys + K
-        cols = lc[:, None] + np.arange(4)[None, :]
+        # TMA staging: step s takes row ys + s of the 128-column box from column x0, zero outside the
+        # buffer's rows and the grid's columns; a lane reads its column group clamped into the box
+        x0 = wx * VALID - HX
+        cols = np.minimum(np.maximum(lc, x0), x0 + 124)[:, None] + np.arange(4)[None, :]
+        inside = (cols >= 0) & (cols < W)
 
         def load(buf, r):
-            v = buf[r - row_off][cols]
+            v = np.zeros((32, 4), F)
+            if 0 <= r - row_off < buf.shape[0]:
+                v[inside] = buf[r - row_off][cols[inside]]
             v[rev] = v[rev][:, ::-1]
-            return v.astype(F)
+            return v
 
         w = np.zeros((K, 3, 32, 4), F)
         dr = np.full((RD, 32, 4), np.nan, F)
-        # staging ring: rows ys .. ys+D-1 (clamped to ye)
-        rload = ys
-        stage_p, stage_d = [None] * D, [None] * D
-        for q in range(D):
-            stage_p[q] = load(pin, rload); stage_d[q] = load(div, rload)
-            if rload < ye:
-                rload += 1
-        slot = 0
         rout = ys - K
         for s0 in range(0, nsteps, U):
             edge = (ys + s0 - K <= 0) or (ys + s0 + 2 >= H - 1)
             for ph in range(U):
-                inn = stage_p[slot].copy(); dv = stage_d[slot].copy()
-                stage_p[slot] = load(pin, rload); stage_d[slot] = load(div, rload)
-                if rload < ye:
-                    rload += 1
-                slot = 0 if slot + 1 == D else slot + 1
+                inn = load(pin, ys + s0 + ph); dv = load(div, ys + s0 + ph)
                 if scale is not None:
                     inn = F(scale) * inn
                 w[0, (ph + 2) % 3] = inn

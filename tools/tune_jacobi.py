@@ -1,6 +1,5 @@
 """Sweeps the temporal-block depth and the rows-per-warp-stream of jacobi_tb_kernel on an H100.
-usage: python tools/tune_jacobi.py [W] [iters] > tune.txt   (FLUID_TB_STAGE=ldgsts: the cp.async ring
-instead of the default TMA staging)"""
+usage: python tools/tune_jacobi.py [W] [iters] > tune.txt"""
 import os
 import sys
 

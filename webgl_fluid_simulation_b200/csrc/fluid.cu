@@ -62,8 +62,8 @@ struct fluid {
     float* dt_dev = nullptr;               // step()'s dt lives in device memory: one graph serves every dt
     unsigned char* tiny_map = nullptr;     // where divergence has 0 < |d| < 2^-123 (jacobi.cuh): 1 byte per 128x32 cells, GLOBAL rows
     size_t tiny_map_bytes = 0;
-    // 2-D tensor maps (TMA staging of the blocked Jacobi kernel) of the two pressure buffers and divergence
-    struct Tmaps { CUtensorMap p[2]; void* p_ptr[2] = {nullptr, nullptr}; CUtensorMap d; bool ok = false; } tmaps;
+    // 2-D tensor maps the blocked Jacobi kernel stages through: m[k] maps pressure buffer p[k] and divergence
+    struct Tmaps { fk::TmapPair m[2]; const void* p[2] = {nullptr, nullptr}; } tmaps;
     double splat_radius_d = 0.25;          // config.SPLAT_RADIUS and the canvas aspect as the JS doubles they are
     double aspect_d = 1.0;                 // (correctRadius S:1457-1462 is double arithmetic, narrowed once)
     int background = 0;                    // FLUID_BACKGROUND: what render() draws the display over (0 colour, 1 checkerboard, 2 none)
@@ -242,12 +242,15 @@ int scan_tiny(fluid_t* h, int j_lo, int j_hi) {
 
 // ---- Jacobi dispatch -----------------------------------------------------------------------------
 
-// Temporal-block depths: default 10, at most KMAX (slab.py mirrors both).  A single-GPU solve staged
-// by TMA goes one deeper, KMAX_TMA (measurements at run_jacobi): its instantiation fits 255 registers
-// without spills, while the cp.async-staged one spills at that depth and is never instantiated.
-constexpr int KMAX = 12;
+// Temporal-block depths, at most KMAX (slab.py mirrors both): the depth-13 instantiation fits 255
+// registers without spills.  A single-GPU in-place solve defaults to KMAX (measurements at run_jacobi);
+// row slabs and the banded host solve default to K_DEFAULT, the depth they have been run at.
+constexpr int KMAX = 13;
 constexpr int K_DEFAULT = 10;
-constexpr int KMAX_TMA = 13;
+
+bool tb_eligible(const fluid_t* h) {
+    return !h->half && (h->cfg.sim_w % 4 == 0) && h->cfg.sim_w >= 16 && h->cfg.sim_h >= 2;
+}
 
 // cuTensorMapEncodeTiled through the runtime (no link-time dependency on libcuda)
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -264,52 +267,44 @@ EncodeTiledFn encode_tiled_fn() {
     return fn;
 }
 
-// fp32 field of `rows` x W as a 2-D tensor; box = 128 columns x 3 rows, no swizzle, out-of-range
-// elements read as zero (the blocked kernel never lets them reach a valid output)
-bool encode_rows_map(CUtensorMap* tm, void* base, int W, int rows) {
+// fp32 field of `rows` x W from `base` as a 2-D tensor map (`tm`: TmapPair::p or ::d); box = 128 columns
+// x 3 rows, no swizzle, out-of-range elements read as zero (the blocked kernel never lets them reach a
+// valid output)
+int encode_rows_map(fluid_t* h, unsigned char (&tm)[128], const void* base, int W, int rows) {
+    static_assert(sizeof(CUtensorMap) == sizeof(tm), "TmapPair holds CUtensorMap images");
     EncodeTiledFn enc = encode_tiled_fn();
-    if (!enc || W % 4 != 0) return false;
     const cuuint64_t dims[2] = {(cuuint64_t)W, (cuuint64_t)rows};
     const cuuint64_t strides[1] = {(cuuint64_t)W * sizeof(float)};
     const cuuint32_t box[2] = {128, 3};
     const cuuint32_t estr[2] = {1, 1};
-    return enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-               CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+    if (!enc || enc(reinterpret_cast<CUtensorMap*>(tm), CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(base), dims,
+                    strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
+                    CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
+        return fail(h, FLUID_ERR_CUDA, "cuTensorMapEncodeTiled of a %d x %d fp32 field failed", W, rows);
+    return FLUID_OK;
 }
 
-// (re)build the tensor maps after the pressure / divergence buffers were allocated
-void build_tmaps(fluid_t* h) {
-    h->tmaps.ok = false;
-    if (h->half || h->cfg.sim_w % 4 != 0 || h->cfg.sim_w < 16) return;
-    const int rows = h->lrows();
-    h->tmaps.p_ptr[0] = h->pressure.read; h->tmaps.p_ptr[1] = h->pressure.write;
-    h->tmaps.ok = encode_rows_map(&h->tmaps.p[0], h->pressure.read, h->cfg.sim_w, rows) &&
-                  encode_rows_map(&h->tmaps.p[1], h->pressure.write, h->cfg.sim_w, rows) &&
-                  encode_rows_map(&h->tmaps.d, h->divergence, h->cfg.sim_w, rows);
+// (re)build the tensor maps after the pressure / divergence buffers were allocated.  The blocked kernel
+// stages only through them, so a handle that runs it cannot do without.
+int build_tmaps(fluid_t* h) {
+    h->tmaps = {};
+    if (!tb_eligible(h)) return FLUID_OK;
+    const void* p[2] = {h->pressure.read, h->pressure.write};
+    for (int k = 0; k < 2; ++k) {
+        int rc = encode_rows_map(h, h->tmaps.m[k].p, p[k], h->cfg.sim_w, h->lrows());
+        if (!rc) rc = encode_rows_map(h, h->tmaps.m[k].d, h->divergence, h->cfg.sim_w, h->lrows());
+        if (rc) return rc;
+        h->tmaps.p[k] = p[k];
+    }
+    return FLUID_OK;
 }
 
-// staging of the blocked kernel.  Default: the 2-D TMA boxes — measured 4 % faster than the per-lane
-// cp.async (LDGSTS) ring on an H100 SXM (700 W power limit) at 4096^2 x 50, K = 10 (0.446 vs 0.464 ms
-// per solve).  FLUID_TB_STAGE=ldgsts selects the ring (bit-identical results).  Row slabs (N > 1) keep
-// the ring unless FLUID_TB_STAGE=tma asks for the boxes.  Launches whose buffers the tensor maps do not
-// describe (the band-private rows of fluid_pressure_solve_host) always use the ring: see launch_tb.
-const char* tb_stage_env() {
-    static const char* e = getenv("FLUID_TB_STAGE");
-    return e ? e : "";
-}
-bool tb_use_tma(const fluid_t* h) {
-    if (!h->tmaps.ok) return false;
-    if (h->slab()) return !strcmp(tb_stage_env(), "tma");
-    return strcmp(tb_stage_env(), "ldgsts") != 0;
-}
-
+// `maps` describe a.pin and a.div from their local row 0
 template <int K, bool SCALE>
-int launch_tb(fluid_t* h, const JacobiArgs& a) {
+int launch_tb(fluid_t* h, const JacobiArgs& a, const TmapPair& maps) {
     using T = TB<K>;
     const int nxw = (a.W + T::VALID - 1) / T::VALID;
     const int nch = (a.out_hi - a.out_lo + a.rows_per_chunk - 1) / a.rows_per_chunk;
-    TmapPair maps;
-    memset(&maps, 0, sizeof maps);
     // chained to the previous launch of the same solve by programmatic dependent launch (jacobi.cuh);
     // not while a graph is being captured
     cudaLaunchAttribute attr[1];
@@ -318,27 +313,15 @@ int launch_tb(fluid_t* h, const JacobiArgs& a) {
     cudaLaunchConfig_t lc{};
     lc.gridDim = dim3(nxw * nch); lc.blockDim = dim3(32); lc.stream = h->stream;   // one warp per CTA
     lc.attrs = attr; lc.numAttrs = (h->pdl_chain && !h->capturing) ? 1 : 0;
-    // the tensor maps address rows from the base of the mapped buffers, the kernel from a.pin / a.div
-    const bool tma = tb_use_tma(h) && a.div == h->divergence && (a.pin == h->tmaps.p_ptr[0] || a.pin == h->tmaps.p_ptr[1]);
-    if (tma) {
-        const int k = (a.pin == h->tmaps.p_ptr[0]) ? 0 : 1;
-        memcpy(maps.p, &h->tmaps.p[k], sizeof(CUtensorMap));
-        memcpy(maps.d, &h->tmaps.d, sizeof(CUtensorMap));
-        lc.dynamicSmemBytes = T::SMEM_TMA;
-        cudaLaunchKernelEx(&lc, jacobi_tb_kernel<K, SCALE, true>, a, maps);
-    } else if constexpr (K <= KMAX) {
-        lc.dynamicSmemBytes = T::SMEM_LDGSTS;
-        cudaLaunchKernelEx(&lc, jacobi_tb_kernel<K, SCALE, false>, a, maps);
-    } else {
-        return fail(h, FLUID_ERR_INVALID, "temporal block depth %d needs TMA staging", K);
-    }
+    lc.dynamicSmemBytes = T::SMEM;
+    cudaLaunchKernelEx(&lc, jacobi_tb_kernel<K, SCALE>, a, maps);
     ++h->jacobi_kernel_launches;
     return check_launch(h, "jacobi_tb_kernel");
 }
 
 template <int K>
-int launch_tb_k(fluid_t* h, const JacobiArgs& a, bool scale) {
-    return scale ? launch_tb<K, true>(h, a) : launch_tb<K, false>(h, a);
+int launch_tb_k(fluid_t* h, const JacobiArgs& a, const TmapPair& maps, bool scale) {
+    return scale ? launch_tb<K, true>(h, a, maps) : launch_tb<K, false>(h, a, maps);
 }
 
 // rows per warp stream: enough chunks that every SM holds its full complement of resident warps
@@ -349,9 +332,7 @@ int tb_rows(const fluid_t* h, int W, int rows) {
     using T = TB<K>;
     const int nxw = (W + T::VALID - 1) / T::VALID;
     int occ = 0;
-    if constexpr (K > KMAX) cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, jacobi_tb_kernel<K, false, true>, 32, T::SMEM_TMA);
-    else if (tb_use_tma(h)) cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, jacobi_tb_kernel<K, false, true>, 32, T::SMEM_TMA);
-    else cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, jacobi_tb_kernel<K, false, false>, 32, T::SMEM_LDGSTS);
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, jacobi_tb_kernel<K, false>, 32, T::SMEM);
     if (occ < 1) occ = 1;
     if (h->jacobi_warps_per_sm > 0) occ = std::min(occ, h->jacobi_warps_per_sm);
     const int resident_warps = std::max(nxw, h->sm_count * occ);
@@ -364,19 +345,15 @@ int tb_rows(const fluid_t* h, int W, int rows) {
     return std::min(r, rows);
 }
 
-int launch_tb_dyn(fluid_t* h, int K, JacobiArgs a, bool scale) {
+int launch_tb_dyn(fluid_t* h, int K, JacobiArgs a, const TmapPair& maps, bool scale) {
     const int rows = a.out_hi - a.out_lo;
     switch (K) {
-#define CASE(KK) case KK: a.rows_per_chunk = tb_rows<KK>(h, a.W, rows); return launch_tb_k<KK>(h, a, scale);
+#define CASE(KK) case KK: a.rows_per_chunk = tb_rows<KK>(h, a.W, rows); return launch_tb_k<KK>(h, a, maps, scale);
         CASE(1) CASE(2) CASE(3) CASE(4) CASE(5) CASE(6) CASE(7) CASE(8) CASE(9) CASE(10) CASE(11) CASE(12)
         CASE(13)
 #undef CASE
     }
     return fail(h, FLUID_ERR_INVALID, "temporal block depth %d out of range", K);
-}
-
-bool tb_eligible(const fluid_t* h) {
-    return !h->half && (h->cfg.sim_w % 4 == 0) && h->cfg.sim_w >= 16 && h->cfg.sim_h >= 2;
 }
 
 // `iters` sweeps reading pressure.read, result in pressure.read (swaps like S:1265).
@@ -392,12 +369,11 @@ int run_jacobi(fluid_t* h, int iters, bool scale_first, int* launches_out) {
     a.scale = h->cfg.pressure;
     a.err = h->halo_flag;
     a.tiny_map = h->tiny_map;
-    // default depth: on an H100 at 4096^2 x 50 (TMA staging) 4 launches of 13 / 12 sweeps take 0.500 ms per
-    // solve and 5 launches of 10 take 0.524 (80 GB HBM3 card, 400 W power limit; DESIGN §5).  Iteration
-    // counts that split into the same number of launches either way (20, 30, 40) keep depth 10 launches.
-    const bool tma13 = !h->slab() && tb_use_tma(h);
-    int kb = h->cfg.jacobi_block > 0 ? h->cfg.jacobi_block : (tma13 ? KMAX_TMA : K_DEFAULT);
-    kb = std::min(kb, tma13 ? KMAX_TMA : KMAX);
+    // default depth: on an H100 at 4096^2 x 50 4 launches of 13 / 12 sweeps take 0.500 ms per solve and 5
+    // launches of 10 take 0.524 (80 GB HBM3 card, 400 W power limit; DESIGN §5).  Iteration counts that
+    // split into the same number of launches either way (20, 30, 40) keep depth 10 launches.
+    int kb = h->cfg.jacobi_block > 0 ? h->cfg.jacobi_block : (h->slab() ? K_DEFAULT : KMAX);
+    kb = std::min(kb, KMAX);
     if (h->slab()) kb = std::max(1, std::min(kb, h->G - 1));
     const bool naive = (h->cfg.flags & FLUID_FLAG_NAIVE_JACOBI) || kb == 1;
     // clear pass alone (owned + ghost rows; ghosts are refreshed before use anyway).  Half storage always
@@ -479,11 +455,15 @@ int run_jacobi(fluid_t* h, int iters, bool scale_first, int* launches_out) {
         const bool sc = scale_first && k == 0;
         int rc;
         if (blocked) {
+            // the maps of the buffer this launch reads, found by its address (a resize re-allocates pressure
+            // and leaves par_p as it was)
+            const int m = (a.pin == h->tmaps.p[0]) ? 0 : (a.pin == h->tmaps.p[1]) ? 1 : -1;
+            if (m < 0) return fail(h, FLUID_ERR_CUDA, "jacobi_tb_kernel: the pressure buffer has no tensor map");
             // programmatic dependent launch: behind another blocked launch of this solve, and — first launch —
             // behind whatever kernel precedes it on the stream (the previous solve's last launch in a host loop
             // of solves; a kernel without griddepcontrol.launch_dependents simply triggers at its end)
             h->pdl_chain = true;
-            rc = launch_tb_dyn(h, K, a, sc);
+            rc = launch_tb_dyn(h, K, a, h->tmaps.m[m], sc);
             h->pdl_chain = false;
         } else if (tb_eligible(h)) {
             dim3 b(32, 8);
@@ -554,7 +534,7 @@ int alloc_fields(fluid_t* h) {
         int rc = alloc_scalar_fields(h); if (rc) return rc;
     }
     { int rc = alloc_tiny_map(h); if (rc) return rc; }
-    build_tmaps(h);
+    { int rc = build_tmaps(h); if (rc) return rc; }
     h->div_sent_epoch = 0;                               // fresh buffers: no divergence ghost rows in place yet
     return with_storage(h, [&](auto s) {
         using S = decltype(s);
@@ -577,7 +557,7 @@ void free_fields(fluid_t* h) {
     h->velocity = Pair{}; h->dye = Pair{}; h->pressure = Pair{};
     h->divergence = h->curl = nullptr;
     cudaFree(h->tiny_map); h->tiny_map = nullptr;
-    h->tmaps.ok = false;
+    h->tmaps = {};
 }
 
 // pointer to the first OWNED row of a field's .read buffer, plus its owned extent
@@ -1363,8 +1343,7 @@ int fluid_resize(fluid_t* h, int sim_w, int sim_h, int dye_w, int dye_h) {
     h->row0 = 0; h->row1 = sim_h; h->drow0 = 0; h->drow1 = dye_h; h->roff = 0; h->droff = 0;
     if ((rc = alloc_scalar_fields(h))) return rc;
     if ((rc = alloc_tiny_map(h))) return rc;
-    build_tmaps(h);
-    return FLUID_OK;
+    return build_tmaps(h);
 }
 
 // ---- data in / out --------------------------------------------------------------------------------
@@ -1445,6 +1424,9 @@ int solve_host_banded(fluid_t* h, const float* div_host, float* p_host, int iter
     const int nlaunch = (iters + kb - 1) / kb;
     const int base = iters / nlaunch, extra = iters % nlaunch;
     const int band = (H + nb - 1) / nb, halo = iters;
+    // band-private rows [loc, loc + band + 2*halo): every row a launch of band [b_lo, b_hi) reads or writes lies
+    // in [max(b_lo - halo, 0), b_hi + halo).  Boxes staged beyond a map's rows read as zero, and rows past what
+    // a launch wrote never reach a valid output, as on the whole grid.
     const size_t need = (size_t)(band + 2 * halo) * W;
     if (hp.s_floats < need) {
         cudaFree(hp.s[0]); cudaFree(hp.s[1]); hp.s[0] = hp.s[1] = nullptr; hp.s_floats = 0;
@@ -1454,7 +1436,14 @@ int solve_host_banded(fluid_t* h, const float* div_host, float* p_host, int iter
     }
     float* const p_in = (float*)h->pressure.read;
     float* const result = (float*)h->pressure.write;
-    int rc = clear_tiny_map(h); if (rc) return rc;
+    // tensor maps of what the launches of a band read, all from the band's local row 0: launch 0 reads the
+    // uploaded field (m[0]), launch k > 0 the band-private rows s[(k-1)&1] (m[1 + ((k-1)&1)]); the band's
+    // divergence maps are filled in per band
+    TmapPair m[3];
+    int rc = FLUID_OK;
+    for (int k = 0; k < 2 && !rc; ++k) rc = encode_rows_map(h, m[1 + k].p, hp.s[k], W, band + 2 * halo);
+    if (rc) return rc;
+    if ((rc = clear_tiny_map(h))) return rc;
     CU(cudaEventRecord(hp.ev_start, h->stream));          // the copies overwrite fields earlier work on the stream may still read
     CU(cudaStreamWaitEvent(hp.up, hp.ev_start, 0));
     for (int b = 0; b < nb; ++b) {
@@ -1470,7 +1459,13 @@ int solve_host_banded(fluid_t* h, const float* div_host, float* p_host, int iter
         CU(cudaEventRecord(hp.ev_up[b], hp.up));
         CU(cudaStreamWaitEvent(h->stream, hp.ev_up[b], 0));
         if ((rc = scan_tiny(h, up_lo, up_hi))) return rc;
-        const int loc = b_lo - halo;                      // global row of local row 0 of the band-private rows (may be < 0)
+        // global row of local row 0 of the band-private rows.  No launch of the band reads a row below
+        // b_lo - halo, or below row 0, so every field is passed from a row inside its allocation.
+        const int loc = std::max(b_lo - halo, 0);
+        if ((rc = encode_rows_map(h, m[0].p, p_in + (ptrdiff_t)loc * W, W, H - loc))) return rc;
+        if ((rc = encode_rows_map(h, m[0].d, h->divergence + (ptrdiff_t)loc * W, W, H - loc))) return rc;
+        memcpy(m[1].d, m[0].d, sizeof m[0].d);
+        memcpy(m[2].d, m[0].d, sizeof m[0].d);
         int remaining = iters;
         for (int k = 0; k < nlaunch; ++k) {
             const int K = base + (k < extra ? 1 : 0);
@@ -1480,13 +1475,13 @@ int solve_host_banded(fluid_t* h, const float* div_host, float* p_host, int iter
             a.W = W; a.H = H; a.scale = h->cfg.pressure; a.err = h->halo_flag; a.tiny_map = h->tiny_map;
             a.out_lo = std::max(b_lo - remaining, 0); a.out_hi = std::min(b_hi + remaining, H);
             // the kernel addresses all three fields as "local row 0 + (row - row_off)": a whole-grid field G is
-            // passed as G + loc*W (only rows inside the grid are ever dereferenced)
+            // passed as G + loc*W
             a.row_off = loc;
             a.div = h->divergence + (ptrdiff_t)loc * W;
             a.pin = (k == 0) ? p_in + (ptrdiff_t)loc * W : hp.s[(k - 1) & 1];
             a.pout = last ? result + (ptrdiff_t)loc * W : hp.s[k & 1];
             h->pdl_chain = (k > 0);
-            rc = launch_tb_dyn(h, K, a, k == 0);
+            rc = launch_tb_dyn(h, K, a, m[k == 0 ? 0 : 1 + ((k - 1) & 1)], k == 0);
             h->pdl_chain = false;
             if (rc) return rc;
         }

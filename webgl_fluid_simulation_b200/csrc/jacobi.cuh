@@ -21,10 +21,9 @@
 //       explicitly (EDGE instantiation, only on the few steps that touch those rows);
 //     * div[r] is needed by level t when it produces row r, i.e. K times at K different steps:
 //       each lane keeps its float4 of the last K+3 rows in a register ring (see tb_block);
-//     * p / div rows are staged D rows ahead into a per-warp shared-memory ring, so the few
-//       resident warps still keep enough bytes in flight for HBM.  Two interchangeable fills:
-//       TMA — one elected lane issues cp.async.bulk (UBLKCP) of the window's 512 B row segment
-//       with mbarrier complete_tx; or LDGSTS — every lane cp.asyncs its own 16 B.
+//     * p / div rows are staged ahead into a per-warp shared-memory ring, so the few resident
+//       warps still keep enough bytes in flight for HBM: one lane issues 2-D tensor-map TMA boxes
+//       (cp.async.bulk.tensor, SASS UTMALDG) of the window's rows with mbarrier complete_tx.
 //   The optional SCALE template fuses the clear pass (S:1253-1257, p <- PRESSURE*p) into the
 //   level-0 load of the first launch: one fp32 multiply, same rounding as the separate blit.
 #pragma once
@@ -46,7 +45,8 @@ struct JacobiArgs {
     const unsigned char* tiny_map;   // tb kernel: where divergence defeats the fma contraction (may be null)
 };
 
-// the two tensor maps a temporally blocked launch reads through (TMA staging); 64-byte aligned
+// the two tensor maps a temporally blocked launch reads through: p describes the buffer passed as
+// JacobiArgs::pin, d the one passed as div, both from their local row 0.  64-byte aligned
 // CUtensorMap images, passed by value as a __grid_constant__ kernel parameter
 struct __align__(64) TmapPair {
     unsigned char p[128];
@@ -131,26 +131,20 @@ __global__ void __launch_bounds__(256) jacobi_sweep_kernel(JacobiArgs a) {
 // touches a flagged cell runs the EXACT instantiation (subtract, then multiply).  4 lane-ops per
 // update instead of 5 everywhere else.
 //
-// Staging.  p / div rows reach a warp through a shared-memory ring, filled either
-//   * TMA: by 2-D tensor-map TMA (cp.async.bulk.tensor.2d, SASS UTMALDG): one elected lane arms an
-//     mbarrier and fetches a 128-column x 3-row box of p and of div per pipeline block; columns
-//     outside the grid and rows outside the buffer are zero-filled by the hardware (never used
-//     by a valid output); or
-//   * LDGSTS: by per-lane 16-byte cp.async (the generation-5 path): the default of row slabs, and
-//     the only staging of launches whose buffers the tensor maps do not describe.
+// Staging.  p / div rows reach a warp through a shared-memory ring filled by 2-D tensor-map TMA
+// (cp.async.bulk.tensor.2d, SASS UTMALDG): one elected lane arms an mbarrier and fetches a
+// 128-column x 3-row box of p and of div per pipeline block; columns outside the grid and rows
+// outside the mapped buffer are zero-filled by the hardware (never used by a valid output).
 template <int K>
 struct TB {
     static constexpr int HX = (K + 3) / 4 * 4;       // x halo (columns) on each side of a window
     static constexpr int VALID = 128 - 2 * HX;       // columns a window produces
     static constexpr int RD = K + 3;                 // div register-ring slots
     static constexpr int U = 3;                      // pipeline steps per unrolled block
-    // LDGSTS ring: D rows of p + D rows of div, one float4 per lane per row
-    static constexpr int D = 8;
-    static constexpr int SMEM_LDGSTS = D * 2 * 32 * (int)sizeof(float4);
-    // TMA ring: NS stages, each a 3-row box of p followed by a 3-row box of div (row = 512 B)
+    // NS stages, each a 3-row box of p followed by a 3-row box of div (row = 512 B), then NS mbarriers
     static constexpr int NS = 4;
     static constexpr int STAGE4 = 2 * U * 32;        // float4 per stage
-    static constexpr int SMEM_TMA = NS * STAGE4 * (int)sizeof(float4) + NS * 8;
+    static constexpr int SMEM = NS * STAGE4 * (int)sizeof(float4) + NS * 8;
 };
 
 // coarse map of "divergence has a value with 0 < |d| < 2^-123 here": one byte per cell
@@ -159,17 +153,6 @@ constexpr float TINY_DIV = 9.4039548e-38f;           // 2^-123
 __host__ __device__ inline int tiny_map_w(int W) { return (W + TINY_CW - 1) / TINY_CW; }
 __host__ __device__ inline int tiny_map_h(int H) { return (H + TINY_CH - 1) / TINY_CH; }
 __device__ __forceinline__ bool is_tiny_div(float d) { return d != 0.0f && fabsf(d) < TINY_DIV; }
-
-// ---- cp.async (LDGSTS) staging: global -> shared without passing through registers ------------
-// Each lane copies, and later reads back, ONLY its own 16 bytes of a row, so the per-thread
-// completion wait (cp.async.wait_group) is all the synchronisation the ring needs.
-__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src) {
-    const unsigned d = (unsigned)__cvta_generic_to_shared(smem_dst);
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(gmem_src) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
 // ---- TMA (2-D tensor map) + mbarrier ----------------------------------------------------------------
 // Waits are bounded: a mis-armed barrier costs an error word, never a hung kernel.
@@ -243,14 +226,9 @@ __device__ __forceinline__ float4 jacobi4(const float4 below, const float4 c, co
 struct TBStream {
     float4* op;          // where level K's row of THIS step goes (advances one row per step)
     int rout;            // global row index op points at  (= ys + s - K)
-    // LDGSTS variant
-    const float4* pl;    // next p row to stage (this lane's float4 column group)
-    const float4* dl;    // next div row to stage
-    const float4* stage; // this lane's cell of the staging slot consumed at this step
-    int rload;           // global row index pl/dl point at
-    int slot;            // staging slot consumed at this step (0..D-1)
-    // TMA variant
-    int stg;             // stage consumed by this block (0..NS-1)
+    // alignas: rout alone in its 8 bytes, the layout this kernel has been measured with.  Packing stg
+    // next to rout renumbers the PTX registers, and ptxas then schedules the whole kernel differently.
+    alignas(8) int stg;  // stage consumed by this block (0..NS-1)
     unsigned phase;      // mbarrier parity of that stage
     int yfill;           // local row coordinate of the next box to fetch
 };
@@ -274,52 +252,25 @@ struct TBTma {           // warp-uniform TMA bookkeeping
 //     the ALU pipe, beside the fp32 pipe that bounds the kernel);
 //   * EDGE instantiates the wall selects in y, REV the mirrored-lane reversal in x, EXACT the
 //     un-contracted tail; all are chosen by warp-uniform branches OUTSIDE the steady-state loop.
-template <int K, bool SCALE, bool EDGE, bool REV, bool EXACT, bool TMA>
+template <int K, bool SCALE, bool EDGE, bool REV, bool EXACT>
 __device__ __forceinline__ void tb_block(float4 (&w)[K][3], float4 (&dr)[TB<K>::RD], TBStream& st,
                                          const float4* __restrict__ ring, const TBTma& tm, const int W4,
-                                         const int ye, const int y0, const int y1, const int H,
+                                         const int y0, const int y1, const int H,
                                          const bool rev, const bool lane_out, const float scale) {
     using T = TB<K>;
-    const float4* srow = ring;
-    if (TMA) {
-        mbar_wait(tm.bars + st.stg, st.phase, tm.err);
-        srow = ring + st.stg * T::STAGE4;
-    }
+    mbar_wait(tm.bars + st.stg, st.phase, tm.err);
+    const float4* srow = ring + st.stg * T::STAGE4;
     // The K levels x 3 steps of a block form a dependency lattice: node (ph, t) needs node
     // (ph, t-1) of the same step (the fresh row above) and rows of level t-1 from the two previous
-    // steps.  Source order is step by step; ptxas interleaves the chains itself.  (FLUID_TB_DIAG,
-    // a tuning build, emits the lattice anti-diagonal by anti-diagonal instead — legal because ph
-    // ascends inside a diagonal.)
-#ifdef FLUID_TB_DIAG
-#pragma unroll
-    for (int dg = 0; dg < K + 3; ++dg) {
-#pragma unroll
-        for (int ph = 0; ph < 3; ++ph) {
-            const int t = dg - ph;
-            if (t < 0 || t > K) continue;
-#else
+    // steps.  Source order is step by step; ptxas interleaves the chains itself.
 #pragma unroll
     for (int ph = 0; ph < 3; ++ph) {
 #pragma unroll
         for (int t = 0; t <= K; ++t) {
-#endif
             if (t == 0) {
                 // ---- level 0: the oldest staged row ---------------------------------------------------
-                float4 in, dv;
-                if (TMA) {
-                    in = lds128(srow + ph * 32);
-                    dv = lds128(srow + (3 + ph) * 32);
-                } else {
-                    cp_async_wait<T::D - 1>();
-                    in = lds128(st.stage);
-                    dv = lds128(st.stage + T::D * 32);
-                    cp_async16(const_cast<float4*>(st.stage), st.pl);
-                    cp_async16(const_cast<float4*>(st.stage) + T::D * 32, st.dl);
-                    cp_async_commit();
-                    if (st.rload < ye) { ++st.rload; st.pl += W4; st.dl += W4; }   // loads clamp to row ye
-                    st.slot = (st.slot + 1 == T::D) ? 0 : st.slot + 1;
-                    st.stage = ring + st.slot * 32;
-                }
+                float4 in = lds128(srow + ph * 32);
+                float4 dv = lds128(srow + (3 + ph) * 32);
                 if (REV) { in = rev4(in, rev); dv = rev4(dv, rev); }
                 if (SCALE) {
                     in.x = scale * in.x; in.y = scale * in.y; in.z = scale * in.z; in.w = scale * in.w;
@@ -354,28 +305,26 @@ __device__ __forceinline__ void tb_block(float4 (&w)[K][3], float4 (&dr)[TB<K>::
     st.op += 3 * W4;
 #pragma unroll
     for (int j = 0; j < K; ++j) dr[j] = dr[j + 3];
-    if (TMA) {
-        // Refill the stage consumed ONE BLOCK AGO with the box NS-1 blocks ahead: every value read
-        // from it has been used by now, so all lanes' reads of it have completed.
-        __syncwarp();
-        if (tm.lane == 0) {
-            const int q = (st.stg == 0) ? T::NS - 1 : st.stg - 1;
-            float4* dst = tm.slots + q * T::STAGE4;
-            mbar_expect_tx(tm.bars + q, 2u * 3u * 512u);
-            tma_load_2d(dst, tm.tm_p, tm.x0, st.yfill, tm.bars + q);
-            tma_load_2d(dst + 3 * 32, tm.tm_d, tm.x0, st.yfill, tm.bars + q);
-        }
-        st.yfill += 3;
-        if (st.stg + 1 == T::NS) { st.stg = 0; st.phase ^= 1u; } else { ++st.stg; }
+    // Refill the stage consumed ONE BLOCK AGO with the box NS-1 blocks ahead: every value read
+    // from it has been used by now, so all lanes' reads of it have completed.
+    __syncwarp();
+    if (tm.lane == 0) {
+        const int q = (st.stg == 0) ? T::NS - 1 : st.stg - 1;
+        float4* dst = tm.slots + q * T::STAGE4;
+        mbar_expect_tx(tm.bars + q, 2u * 3u * 512u);
+        tma_load_2d(dst, tm.tm_p, tm.x0, st.yfill, tm.bars + q);
+        tma_load_2d(dst + 3 * 32, tm.tm_d, tm.x0, st.yfill, tm.bars + q);
     }
+    st.yfill += 3;
+    if (st.stg + 1 == T::NS) { st.stg = 0; st.phase ^= 1u; } else { ++st.stg; }
 }
 
-template <int K, bool SCALE, bool REV, bool EXACT, bool TMA>
+template <int K, bool SCALE, bool REV, bool EXACT>
 __device__ __forceinline__ void tb_stream(const JacobiArgs& a, const void* tm_p, const void* tm_d,
                                           float4* __restrict__ smem4, const int lane, const int x0,
                                           const int lc, const int gx, const bool rev,
                                           const bool lane_out, const int y0, const int y1,
-                                          const int ys, const int ye) {
+                                          const int ys) {
     using T = TB<K>;
     const int W = a.W, H = a.H, W4 = W >> 2;
     const int nsteps = y1 - ys + K;                   // level K emits row ys+s-K at step s
@@ -395,52 +344,33 @@ __device__ __forceinline__ void tb_stream(const JacobiArgs& a, const void* tm_p,
 
     TBStream st{};
     TBTma tm{};
-    const float4* ring;
-    if (TMA) {
-        // every lane reads its (mirrored / clamped) column group out of the staged 128-column box.  In the
-        // last window the mirror image of the outermost lanes lies left of the box (x0 > lc); those lanes
-        // feed no output (beyond lane_out and the shuffle cone), so they read the box's first column
-        // instead of shared memory below it.
-        ring = smem4 + ((min(max(lc, x0), x0 + 124) - x0) >> 2);
-        tm.tm_p = tm_p; tm.tm_d = tm_d;
-        tm.bars = reinterpret_cast<unsigned long long*>(smem4 + T::NS * T::STAGE4);
-        tm.slots = smem4;
-        tm.x0 = x0; tm.lane = lane; tm.err = a.err;
-        st.stg = 0; st.phase = 0;
-        st.yfill = ys - a.row_off;
+    // every lane reads its (mirrored / clamped) column group out of the staged 128-column box.  In the
+    // last window the mirror image of the outermost lanes lies left of the box (x0 > lc); those lanes
+    // feed no output (beyond lane_out and the shuffle cone), so they read the box's first column
+    // instead of shared memory below it.
+    const float4* ring = smem4 + ((min(max(lc, x0), x0 + 124) - x0) >> 2);
+    tm.tm_p = tm_p; tm.tm_d = tm_d;
+    tm.bars = reinterpret_cast<unsigned long long*>(smem4 + T::NS * T::STAGE4);
+    tm.slots = smem4;
+    tm.x0 = x0; tm.lane = lane; tm.err = a.err;
+    st.stg = 0; st.phase = 0;
+    st.yfill = ys - a.row_off;
+    if (lane == 0) {
+#pragma unroll
+        for (int q = 0; q < T::NS; ++q) mbar_init(tm.bars + q, 1);
+        mbar_fence_init();
+    }
+    __syncwarp();
+    // boxes of blocks 0 .. NS-2 into stages 0 .. NS-2; stage NS-1 is filled at the end of block 0
+#pragma unroll
+    for (int q = 0; q < T::NS - 1; ++q) {
         if (lane == 0) {
-#pragma unroll
-            for (int q = 0; q < T::NS; ++q) mbar_init(tm.bars + q, 1);
-            mbar_fence_init();
+            float4* dst = tm.slots + q * T::STAGE4;
+            mbar_expect_tx(tm.bars + q, 2u * 3u * 512u);
+            tma_load_2d(dst, tm_p, x0, st.yfill, tm.bars + q);
+            tma_load_2d(dst + 3 * 32, tm_d, x0, st.yfill, tm.bars + q);
         }
-        __syncwarp();
-        // boxes of blocks 0 .. NS-2 into stages 0 .. NS-2; stage NS-1 is filled at the end of block 0
-#pragma unroll
-        for (int q = 0; q < T::NS - 1; ++q) {
-            if (lane == 0) {
-                float4* dst = tm.slots + q * T::STAGE4;
-                mbar_expect_tx(tm.bars + q, 2u * 3u * 512u);
-                tma_load_2d(dst, tm_p, x0, st.yfill, tm.bars + q);
-                tma_load_2d(dst + 3 * 32, tm_d, x0, st.yfill, tm.bars + q);
-            }
-            st.yfill += 3;
-        }
-    } else {
-        ring = smem4 + lane;                          // p slot q at ring[q*32], div at ring[(D+q)*32]
-        const float4* Pg = reinterpret_cast<const float4*>(a.pin) + base + (lc >> 2);
-        const float4* Dg = reinterpret_cast<const float4*>(a.div) + base + (lc >> 2);
-        st.pl = Pg + (ptrdiff_t)ys * W4;
-        st.dl = Dg + (ptrdiff_t)ys * W4;
-        st.rload = ys; st.slot = 0;
-        // fill the staging ring: rows ys .. ys+D-1 (clamped to ye), one cp.async group per row
-#pragma unroll
-        for (int q = 0; q < T::D; ++q) {
-            cp_async16(smem4 + lane + q * 32, st.pl);
-            cp_async16(smem4 + lane + (T::D + q) * 32, st.dl);
-            cp_async_commit();
-            if (st.rload < ye) { ++st.rload; st.pl += W4; st.dl += W4; }
-        }
-        st.stage = ring;
+        st.yfill += 3;
     }
     st.rout = ys - K;
     st.op = Og + (ptrdiff_t)st.rout * W4;             // only dereferenced for rows in [y0, y1)
@@ -454,36 +384,26 @@ __device__ __forceinline__ void tb_stream(const JacobiArgs& a, const void* tm_p,
     for (int part = 0; part < 2; ++part) {
 #pragma unroll 1
         for (; s0 < nsteps && ((ys + s0 - K <= 0) || (ys + s0 + 2 >= H - 1)); s0 += 3)
-            tb_block<K, SCALE, true, REV, EXACT, TMA>(w, dr, st, ring, tm, W4, ye, y0, y1, H, rev, lane_out, a.scale);
+            tb_block<K, SCALE, true, REV, EXACT>(w, dr, st, ring, tm, W4, y0, y1, H, rev, lane_out, a.scale);
 #pragma unroll 1
         for (; s0 < nsteps && !((ys + s0 - K <= 0) || (ys + s0 + 2 >= H - 1)); s0 += 3)
-            tb_block<K, SCALE, false, REV, EXACT, TMA>(w, dr, st, ring, tm, W4, ye, y0, y1, H, rev, lane_out, a.scale);
+            tb_block<K, SCALE, false, REV, EXACT>(w, dr, st, ring, tm, W4, y0, y1, H, rev, lane_out, a.scale);
     }
     // drain the over-fetched tail before the CTA (and its shared memory) goes away
-    if (TMA) {
 #pragma unroll 1
-        for (int q = 0; q < T::NS - 1; ++q) {
-            mbar_wait(tm.bars + st.stg, st.phase, tm.err);
-            if (st.stg + 1 == T::NS) { st.stg = 0; st.phase ^= 1u; } else { ++st.stg; }
-        }
-    } else {
-        cp_async_wait<0>();
+    for (int q = 0; q < T::NS - 1; ++q) {
+        mbar_wait(tm.bars + st.stg, st.phase, tm.err);
+        if (st.stg + 1 == T::NS) { st.stg = 0; st.phase ^= 1u; } else { ++st.stg; }
     }
 }
 
-#ifdef FLUID_TB_EXACT_INLINE
-#define FLUID_TB_EXACT_ATTR __forceinline__
-#else
-#define FLUID_TB_EXACT_ATTR __noinline__
-#endif
-template <int K, bool SCALE, bool TMA>
-__device__ FLUID_TB_EXACT_ATTR void tb_stream_exact(const JacobiArgs& a, const void* tm_p, const void* tm_d,
+template <int K, bool SCALE>
+__device__ __noinline__ void tb_stream_exact(const JacobiArgs& a, const void* tm_p, const void* tm_d,
                                              float4* __restrict__ smem4, const int lane, const int x0,
                                              const int lc, const int gx, const bool rev, const bool lane_out,
-                                             const int y0, const int y1, const int ys, const int ye,
-                                             const bool any_rev) {
-    if (any_rev) tb_stream<K, SCALE, true, true, TMA>(a, tm_p, tm_d, smem4, lane, x0, lc, gx, rev, lane_out, y0, y1, ys, ye);
-    else tb_stream<K, SCALE, false, true, TMA>(a, tm_p, tm_d, smem4, lane, x0, lc, gx, rev, lane_out, y0, y1, ys, ye);
+                                             const int y0, const int y1, const int ys, const bool any_rev) {
+    if (any_rev) tb_stream<K, SCALE, true, true>(a, tm_p, tm_d, smem4, lane, x0, lc, gx, rev, lane_out, y0, y1, ys);
+    else tb_stream<K, SCALE, false, true>(a, tm_p, tm_d, smem4, lane, x0, lc, gx, rev, lane_out, y0, y1, ys);
 }
 
 // One warp per CTA: every quantity that steers control flow derives from blockIdx and kernel
@@ -497,7 +417,7 @@ __device__ FLUID_TB_EXACT_ATTR void tb_stream_exact(const JacobiArgs& a, const v
 #else
 #define FLUID_TB_BOUNDS __launch_bounds__(32, FLUID_TB_MINBLOCKS)
 #endif
-template <int K, bool SCALE, bool TMA>
+template <int K, bool SCALE>
 __global__ void FLUID_TB_BOUNDS jacobi_tb_kernel(JacobiArgs a, const __grid_constant__ TmapPair maps) {
     using T = TB<K>;
     extern __shared__ __align__(128) float4 smem4[];
@@ -535,7 +455,6 @@ __global__ void FLUID_TB_BOUNDS jacobi_tb_kernel(JacobiArgs a, const __grid_cons
 
     // ---- does the divergence this stream reads hold a value that defeats the fma contraction? ----
     bool exact = false;
-#ifndef FLUID_TB_NO_EXACT          // tuning builds only: measures what the second instantiation costs in code size
     if (a.tiny_map) {
         const int mw = tiny_map_w(W);
         const int cx0 = max(x0, 0) / TINY_CW, cx1 = min(x0 + 127, W - 1) / TINY_CW;
@@ -545,7 +464,6 @@ __global__ void FLUID_TB_BOUNDS jacobi_tb_kernel(JacobiArgs a, const __grid_cons
         for (int k = lane; k < n; k += 32) f |= a.tiny_map[(cy0 + k / ncx) * mw + cx0 + k % ncx];
         exact = __any_sync(0xffffffffu, f != 0);
     }
-#endif
     const void* tp = &maps.p;
     const void* td = &maps.d;
     // The common case first, so that it is laid out first: code placement matters to this kernel (it
@@ -555,9 +473,9 @@ __global__ void FLUID_TB_BOUNDS jacobi_tb_kernel(JacobiArgs a, const __grid_cons
     // an SM whose resident warps ran two separate steady-state loops would keep two loop bodies in its
     // instruction cache, and a loop body twice as large measured 11 % slower (DESIGN §5.8).
     if (!exact) {
-        tb_stream<K, SCALE, true, false, TMA>(a, tp, td, smem4, lane, x0, lc, gx, rev, lane_out, y0, y1, ys, ye);
+        tb_stream<K, SCALE, true, false>(a, tp, td, smem4, lane, x0, lc, gx, rev, lane_out, y0, y1, ys);
     } else {
-        tb_stream_exact<K, SCALE, TMA>(a, tp, td, smem4, lane, x0, lc, gx, rev, lane_out, y0, y1, ys, ye, any_rev);
+        tb_stream_exact<K, SCALE>(a, tp, td, smem4, lane, x0, lc, gx, rev, lane_out, y0, y1, ys, any_rev);
     }
 }
 

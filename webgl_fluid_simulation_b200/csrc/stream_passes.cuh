@@ -115,6 +115,17 @@ constexpr int CVD2_MINBLOCKS = FLUID_CVD_MINBLOCKS;              // register bud
 constexpr int CVD2_RING = FLUID_CVD_RING;                        // rows in flight per warp (1 KB each)
 constexpr int CVD2_SMEM = CVD2_WARPS * CVD2_RING * 64 * (int)sizeof(float4);
 
+// cp.async (LDGSTS): global -> shared without passing through registers.  Each lane copies, and
+// later reads back, ONLY its own 16 bytes of a row, so the per-thread completion wait
+// (cp.async.wait_group) is all the synchronisation the ring needs.
+__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src) {
+    const unsigned d = (unsigned)__cvta_generic_to_shared(smem_dst);
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(gmem_src) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+
 struct Vel4 { float x[4], y[4]; };          // 4 consecutive cells of a velocity row
 
 __device__ __forceinline__ Vel4 unpack_vel(const float4 a, const float4 b) {

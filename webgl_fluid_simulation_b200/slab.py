@@ -17,7 +17,7 @@ from __future__ import annotations
 
 from dataclasses import dataclass
 
-KMAX = 12
+KMAX = 13
 DEFAULT_BLOCK = 10
 DEFAULT_HALO = 64
 VELOCITY_GHOST = 3
