@@ -165,3 +165,40 @@ def test_half_storage_refuses_post_fx_and_draws_shading(pkg, oracle, dither):
     assert s._L.fluid_render_keywords(s._h, 64, 64, 8, None, None, 0, 0, *BACK_RGB, want.ctypes.data_as(C.c_void_p),
                                       want.size, None, None) == -1
     s.close()
+
+
+@pytest.mark.parametrize("entry", ["fluid_render", "fluid_render_keywords", "fluid_render_postfx"])
+def test_refusals_leave_the_handle_usable(pkg, dither, entry):
+    """Every bad argument gets FLUID_ERR_INVALID, and the next good call on the same handle draws the same
+    bits as the first one.  fluid_render has no keywords, fluid_render_postfx no keyword mask."""
+    s = make(pkg, 64, 64, 128, 128)
+    s.writeField("dye", seeded_dye(64, 64, 7))
+    s.dithering = dither
+    all3 = pkg.DISPLAY_SHADING | pkg.DISPLAY_BLOOM | pkg.DISPLAY_SUNRAYS
+    set_keywords(pkg, s, all3)
+    _, fx, dith = pkg.postfx_inputs(s.config, dither)
+    out = np.empty((128, 128, 4), np.float32)
+    ptr = lambda a: a.ctypes.data_as(C.c_void_p)        # noqa: E731
+    L = s._L
+
+    def call(w=128, h=128, kw=all3, fx_=C.byref(fx), d=ptr(dith), dw=dith.shape[1], n=out.size, dst=ptr(out)):
+        if entry == "fluid_render":
+            return L.fluid_render(s._h, w, h, 1, *BACK_RGB, dst, n)
+        if entry == "fluid_render_keywords":
+            return L.fluid_render_keywords(s._h, w, h, kw, fx_, d, dw, dith.shape[0], *BACK_RGB, dst, n, None, None)
+        return L.fluid_render_postfx(s._h, w, h, fx_, d, dw, dith.shape[0], *BACK_RGB, dst, n, None, None)
+
+    assert call() == 0
+    good = out.copy()
+    bad = [dict(n=out.size - 1), dict(n=out.size + 1), dict(w=0), dict(h=0), dict(dst=None)]
+    if entry != "fluid_render":
+        bad += [dict(kw=pkg.DISPLAY_BLOOM, d=None), dict(kw=pkg.DISPLAY_BLOOM, dw=0),
+                dict(kw=pkg.DISPLAY_BLOOM, fx_=None), dict(kw=pkg.DISPLAY_SUNRAYS, fx_=None)]
+    if entry == "fluid_render_keywords":
+        bad += [dict(kw=8), dict(kw=all3 | 0x10)]
+    for b in bad:
+        assert call(**b) == -1, b
+        out[...] = np.nan
+        assert call() == 0, b
+        assert bits_equal(out, good), b
+    s.close()

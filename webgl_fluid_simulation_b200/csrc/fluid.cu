@@ -1293,11 +1293,11 @@ int fluid_resize(fluid_t* h, int sim_w, int sim_h, int dye_w, int dye_h) {
         cudaFree(h->tiny_map); h->tiny_map = nullptr;
         if ((rc = alloc_fields(h))) { cudaFree(old_arena); return rc; }
         dim3 b(64, 4);
-        resample_slab_kernel<<<grid2d(sim_w, h->row1 - h->row0, b), b, 0, h->stream>>>(old_v, ow, oh, old_roff, (float2*)h->velocity.read, sim_w, sim_h,
-                                                                                         h->roff, h->row0, h->row1);
-        resample_slab_kernel<<<grid2d(dye_w, h->drow1 - h->drow0, b), b, 0, h->stream>>>(old_d, odw, odh, old_droff, (float4*)h->dye.read, dye_w, dye_h,
-                                                                                           h->droff, h->drow0, h->drow1);
-        rc = check_launch(h, "resample_slab_kernel", 2);
+        resample_kernel<StoreF32><<<grid2d(sim_w, h->row1 - h->row0, b), b, 0, h->stream>>>(old_v, ow, oh, old_roff, (float2*)h->velocity.read,
+                                                                                             sim_w, sim_h, h->roff, h->row0, h->row1);
+        resample_kernel<StoreF32><<<grid2d(dye_w, h->drow1 - h->drow0, b), b, 0, h->stream>>>(old_d, odw, odh, old_droff, (float4*)h->dye.read,
+                                                                                               dye_w, dye_h, h->droff, h->drow0, h->drow1);
+        rc = check_launch(h, "resample_kernel", 2);
         CU(cudaStreamSynchronize(h->stream));
         cudaFree(old_arena);
         h->v_ghost_valid = false;                            // the +-3 velocity ghost rows are rebuilt by the next step
@@ -1318,7 +1318,7 @@ int fluid_resize(fluid_t* h, int sim_w, int sim_h, int dye_w, int dye_h) {
             void *nr = nullptr, *nw = nullptr;
             CU(cudaMalloc(&nr, nd * dbytes(h)));
             CU(cudaMalloc(&nw, nd * dbytes(h)));
-            resample_kernel<S><<<grid2d(dye_w, dye_h, b), b, 0, h->stream>>>((const D*)h->dye.read, odw, odh, (D*)nr, dye_w, dye_h);
+            resample_kernel<S><<<grid2d(dye_w, dye_h, b), b, 0, h->stream>>>((const D*)h->dye.read, odw, odh, 0, (D*)nr, dye_w, dye_h, 0, 0, dye_h);
             fill_alpha_kernel<S><<<(unsigned)((nd + 255) / 256), 256, 0, h->stream>>>((D*)nw, nd);
             int rc = check_launch(h, "resample_kernel", 2); if (rc) return rc;
             CU(cudaStreamSynchronize(h->stream));
@@ -1329,7 +1329,7 @@ int fluid_resize(fluid_t* h, int sim_w, int sim_h, int dye_w, int dye_h) {
             void *nr = nullptr, *nw = nullptr;
             CU(cudaMalloc(&nr, n * vbytes(h)));
             CU(cudaMalloc(&nw, n * vbytes(h)));
-            resample_kernel<S><<<grid2d(sim_w, sim_h, b), b, 0, h->stream>>>((const V*)h->velocity.read, ow, oh, (V*)nr, sim_w, sim_h);
+            resample_kernel<S><<<grid2d(sim_w, sim_h, b), b, 0, h->stream>>>((const V*)h->velocity.read, ow, oh, 0, (V*)nr, sim_w, sim_h, 0, 0, sim_h);
             int rc = check_launch(h, "resample_kernel"); if (rc) return rc;
             CU(cudaMemsetAsync(nw, 0, n * vbytes(h), h->stream));
             CU(cudaStreamSynchronize(h->stream));
@@ -1557,41 +1557,6 @@ static int display_source(fluid_t* h, const float4** src) {
     return FLUID_OK;
 }
 
-// render(target) of S:1296-1317 for config.BLOOM = config.SUNRAYS = false: the background selected by
-// FLUID_BACKGROUND (colour / checkerboard / none), then the display shader (optionally SHADING) blended over it.
-int fluid_render(fluid_t* h, int width, int height, int shading, float back_r, float back_g,
-                 float back_b, float* host_rgba, size_t n_floats) {
-    if (!h || !host_rgba || width < 1 || height < 1) return fail(h, FLUID_ERR_INVALID, "bad argument");
-    int y0, y1;
-    fluid_render_band(h, height, &y0, &y1);
-    const size_t cells = (size_t)width * (y1 - y0);
-    if (n_floats != 4 * cells) return fail(h, FLUID_ERR_INVALID, "render target band has %zu floats, caller passed %zu", 4 * cells, n_floats);
-    if (cells == 0) return FLUID_OK;
-    if (int rc = need_frame(h, cells)) return rc;
-    if (h->slab()) {
-        // the band's display + shading taps reach ceil(Hd / height) + 2 dye rows beyond the owned ones:
-        // refresh that many ghost rows (the ghost rows of dye.read are stale after advection)
-        const int need = std::min(h->Gd, (h->cfg.dye_h + height - 1) / height + 2);
-        int rc = exchange_rows(h, HB_DYE, h->dye.read, (size_t)h->cfg.dye_w * sizeof(float4), h->droff, h->drow0, h->drow1, need);
-        if (rc) return rc;
-        if ((h->cfg.dye_h + height - 1) / height + 2 > h->Gd)
-            return fail(h, FLUID_ERR_HALO, "render target of %d rows needs %d dye ghost rows, the slab keeps %d", height,
-                        (h->cfg.dye_h + height - 1) / height + 2, h->Gd);
-    }
-    const float4* dye_src;
-    if (int rc = display_source(h, &dye_src)) return rc;
-    dim3 b(32, 8);
-    display_kernel<<<grid2d(width, y1 - y0, b), b, 0, h->stream>>>(dye_src, h->cfg.dye_w, h->cfg.dye_h,
-                                                                   h->frame, width, height, shading, back_r, back_g, back_b,
-                                                                   make_float2((float)(1.0 / (double)width), (float)(1.0 / (double)height)),
-                                                                   h->background, h->cfg.aspect, h->droff, y0, y1);
-    int rc = check_launch(h, "display_kernel"); if (rc) return rc;
-    CU(cudaMemcpyAsync(host_rgba, h->frame, cells * sizeof(float4), cudaMemcpyDeviceToHost, h->stream));
-    CU(cudaStreamSynchronize(h->stream));
-    return FLUID_OK;
-}
-
-
 // (Re)allocates one post-FX target once the stream has drained.  Out of memory leaves it empty, so the
 // handle stays usable and the next call tries again.
 static int remake_target(fluid_t* h, void** p, size_t bytes, const char* what) {
@@ -1639,26 +1604,6 @@ static int need_dither_target(fluid_t* h, int dw, int dh) {
     t.dw = dw; t.dh = dh;
     return FLUID_OK;
 }
-
-using DisplayFullKernel = void (*)(const float4*, int, int, const float4*, int, int, const float*, int, int,
-                                   const float*, int, int, float4*, int, int, float, float, float, int, float, float4);
-// indexed by the FLUID_DISPLAY_* mask; the sets without BLOOM or SUNRAYS draw with display_kernel
-static const DisplayFullKernel kDisplayFull[8] = {
-    nullptr, nullptr,
-    display_full_kernel<false, true, false>, display_full_kernel<true, true, false>,
-    display_full_kernel<false, false, true>, display_full_kernel<true, false, true>,
-    display_full_kernel<false, true, true>, display_full_kernel<true, true, true>,
-};
-
-// The 8-bit capture instantiations, indexed the same way
-using CaptureFullKernel = void (*)(const float4*, int, int, const float4*, int, int, const float*, int, int,
-                                   const float*, int, int, uchar4*, int, int, float, float, float, int, float, float4);
-static const CaptureFullKernel kDisplayCapture[8] = {
-    nullptr, nullptr,
-    display_full_kernel<false, true, false, StoreCapture>, display_full_kernel<true, true, false, StoreCapture>,
-    display_full_kernel<false, false, true, StoreCapture>, display_full_kernel<true, false, true, StoreCapture>,
-    display_full_kernel<false, true, true, StoreCapture>, display_full_kernel<true, true, true, StoreCapture>,
-};
 
 // The bloom FBO and the sunrays texture a display kernel samples, as post_fx_chains left them
 struct PostFXOut { int bw, bh, sw, sh; };
@@ -1727,66 +1672,119 @@ static int post_fx_chains(fluid_t* h, uint32_t keywords, const fluid_postfx* fx,
     return check_launch(h, "post-FX kernels", nk);
 }
 
-// The `ts` argument of display_full_kernel for a width x height target: texelSize = 1 / width, 1 / height
-// (S:1337) and getTextureScale (S:1626-1631) are JS doubles, narrowed here.
-static float4 display_scales(uint32_t keywords, int width, int height, int dw, int dh) {
-    const bool bloom_on = keywords & FLUID_DISPLAY_BLOOM;
-    return make_float4((float)(1.0 / (double)width), (float)(1.0 / (double)height),
-                       bloom_on ? (float)((double)width / (double)dw) : 0.0f, bloom_on ? (float)((double)height / (double)dh) : 0.0f);
-}
+// display_kernel<SHADING, BLOOM, SUNRAYS, Out>, indexed by [Out == StoreCapture][FLUID_DISPLAY_* mask]
+using DisplayKernel = void (*)(DisplayArgs);
+static const DisplayKernel kDisplay[2][8] = {
+    {display_kernel<false, false, false, StoreFrame>, display_kernel<true, false, false, StoreFrame>,
+     display_kernel<false, true, false, StoreFrame>, display_kernel<true, true, false, StoreFrame>,
+     display_kernel<false, false, true, StoreFrame>, display_kernel<true, false, true, StoreFrame>,
+     display_kernel<false, true, true, StoreFrame>, display_kernel<true, true, true, StoreFrame>},
+    {display_kernel<false, false, false, StoreCapture>, display_kernel<true, false, false, StoreCapture>,
+     display_kernel<false, true, false, StoreCapture>, display_kernel<true, true, false, StoreCapture>,
+     display_kernel<false, false, true, StoreCapture>, display_kernel<true, false, true, StoreCapture>,
+     display_kernel<false, true, true, StoreCapture>, display_kernel<true, true, true, StoreCapture>},
+};
 
-// render(null) of S:1296-1317 for a keyword set with BLOOM or SUNRAYS (single GPU, fp32 storage): the
-// post-FX chains on width x height FBOs, then the background and drawDisplay with the chosen keywords.
-static int render_postfx(fluid_t* h, const char* what, int width, int height, uint32_t keywords,
-                         const fluid_postfx* fx, const float* dither_rgb, int dw, int dh, float back_r,
-                         float back_g, float back_b, float* host_rgba, size_t n_floats, float* host_bloom,
-                         float* host_sunrays) {
-    const bool bloom_on = keywords & FLUID_DISPLAY_BLOOM, sun_on = keywords & FLUID_DISPLAY_SUNRAYS;
-    if (!h || !fx || !host_rgba || width < 1 || height < 1 || (bloom_on && (!dither_rgb || dw < 1 || dh < 1)))
+// One frame of render() or captureScreenshot(), as the entry points below ask for it.
+struct DrawRequest {
+    const char* what;                  // the entry point, for error messages
+    int width, height;                 // the target
+    int canvas_w, canvas_h;            // the drawing buffer the post-FX FBOs are sized from
+    uint32_t keywords;                 // FLUID_DISPLAY_*
+    const fluid_postfx* fx;            // BLOOM or SUNRAYS
+    const float* dither; int dw, dh;   // BLOOM
+    float back[3]; int bg_mode;        // the background (blend_over_background)
+    bool capture;                      // the 8-bit image of captureScreenshot instead of the fp32 frame
+    void* host; size_t n;              // where the image goes: n floats (frame) or n bytes (capture)
+    float* host_bloom;                 // the bloom FBO / sunrays texture, read back when given
+    float* host_sunrays;
+};
+
+// render(target) of S:1296-1317: the post-FX chains of the keywords that are on, then the background and
+// drawDisplay in one display_kernel launch, read back to the host.  Only the fp32 frame without BLOOM and
+// SUNRAYS is drawn on a slab handle, and there only the handle's band of the target (fluid_render_band).
+// Half storage draws from a widened copy of dye and has no post-FX.
+static int draw(fluid_t* h, const DrawRequest& r) {
+    if (!h) return FLUID_ERR_INVALID;
+    if (r.keywords & ~(uint32_t)(FLUID_DISPLAY_SHADING | FLUID_DISPLAY_BLOOM | FLUID_DISPLAY_SUNRAYS))
+        return fail(h, FLUID_ERR_INVALID, "unknown display keyword bits 0x%x", r.keywords);
+    const bool bloom_on = r.keywords & FLUID_DISPLAY_BLOOM, sun_on = r.keywords & FLUID_DISPLAY_SUNRAYS;
+    const bool postfx = bloom_on || sun_on, band = !postfx && !r.capture;
+    if (!r.host || r.width < 1 || r.height < 1 || r.canvas_w < 1 || r.canvas_h < 1 || (postfx && !r.fx) ||
+        (bloom_on && (!r.dither || r.dw < 1 || r.dh < 1)))
         return fail(h, FLUID_ERR_INVALID, "bad argument");
-    if (h->slab()) return not_on_slab(h, what);
-    if (h->half) return fail(h, FLUID_ERR_INVALID, "%s is not built for FLUID_FLAG_HALF_STORAGE (the reference's bloom / sunrays FBOs are fp16 too)", what);
-    const size_t cells = (size_t)width * height;
-    if (n_floats != 4 * cells) return fail(h, FLUID_ERR_INVALID, "render target has %zu floats, caller passed %zu", 4 * cells, n_floats);
-    int rc = need_frame(h, cells); if (rc) return rc;
-    PostFXOut o;
-    if ((rc = post_fx_chains(h, keywords, fx, dither_rgb, dw, dh, width, height, &o))) return rc;
-    // ---- background + drawDisplay -----------------------------------------------------------------------
+    int y0 = 0, y1 = r.height;
+    if (band) fluid_render_band(h, r.height, &y0, &y1);
+    const size_t cells = (size_t)r.width * (y1 - y0);
+    if (r.n != 4 * cells)
+        return fail(h, FLUID_ERR_INVALID, "%s: the target%s has %zu %s, caller passed %zu", r.what, band ? " band" : "",
+                    4 * cells, r.capture ? "bytes" : "floats", r.n);
+    if (cells == 0) return FLUID_OK;
+    if (h->slab() && !band) return not_on_slab(h, r.what);
+    if (h->half && postfx)
+        return fail(h, FLUID_ERR_INVALID, "%s with BLOOM or SUNRAYS is not built for FLUID_FLAG_HALF_STORAGE "
+                    "(the reference's bloom / sunrays FBOs are fp16 too)", r.what);
+    int rc = need_frame(h, r.capture ? (cells + 3) / 4 : cells); if (rc) return rc;   // the capture's uchar4 image lives in the frame
+    if (h->slab()) {
+        // the band's display + shading taps reach ceil(Hd / height) + 2 dye rows beyond the owned ones:
+        // refresh that many ghost rows (the ghost rows of dye.read are stale after advection)
+        const int need = (h->cfg.dye_h + r.height - 1) / r.height + 2;
+        if ((rc = exchange_rows(h, HB_DYE, h->dye.read, (size_t)h->cfg.dye_w * sizeof(float4), h->droff, h->drow0, h->drow1,
+                                std::min(h->Gd, need))))
+            return rc;
+        if (need > h->Gd)
+            return fail(h, FLUID_ERR_HALO, "render target of %d rows needs %d dye ghost rows, the slab keeps %d", r.height, need, h->Gd);
+    }
+    PostFXOut o{};
+    if (postfx && (rc = post_fx_chains(h, r.keywords, r.fx, r.dither, r.dw, r.dh, r.canvas_w, r.canvas_h, &o))) return rc;
+    const float4* dye_src;
+    if ((rc = display_source(h, &dye_src))) return rc;
+    // texelSize = 1 / width, 1 / height (S:1337) and getTextureScale (S:1626-1631) are JS doubles, narrowed here
+    const float4 ts = make_float4((float)(1.0 / (double)r.width), (float)(1.0 / (double)r.height),
+                                  bloom_on ? (float)((double)r.width / (double)r.dw) : 0.0f,
+                                  bloom_on ? (float)((double)r.height / (double)r.dh) : 0.0f);
+    const DisplayArgs a{dye_src, h->cfg.dye_w, h->cfg.dye_h, h->droff, bloom_on ? h->pfx.bloom : nullptr, o.bw, o.bh,
+                        sun_on ? h->pfx.sun : nullptr, o.sw, o.sh, bloom_on ? h->pfx.dither : nullptr, r.dw, r.dh,
+                        h->frame, r.width, r.height, y0, y1, r.back[0], r.back[1], r.back[2], r.bg_mode, h->cfg.aspect, ts};
     dim3 b(32, 8);
-    kDisplayFull[keywords]<<<grid2d(width, height, b), b, 0, h->stream>>>(
-        (const float4*)h->dye.read, h->cfg.dye_w, h->cfg.dye_h, bloom_on ? h->pfx.bloom : nullptr, o.bw, o.bh,
-        sun_on ? h->pfx.sun : nullptr, o.sw, o.sh, bloom_on ? h->pfx.dither : nullptr, dw, dh, h->frame, width,
-        height, back_r, back_g, back_b, h->background, h->cfg.aspect, display_scales(keywords, width, height, dw, dh));
-    if ((rc = check_launch(h, "display_full_kernel"))) return rc;
-    CU(cudaMemcpyAsync(host_rgba, h->frame, cells * sizeof(float4), cudaMemcpyDeviceToHost, h->stream));
-    if (bloom_on && host_bloom) CU(cudaMemcpyAsync(host_bloom, h->pfx.bloom, (size_t)o.bw * o.bh * sizeof(float4), cudaMemcpyDeviceToHost, h->stream));
-    if (sun_on && host_sunrays) CU(cudaMemcpyAsync(host_sunrays, h->pfx.sun, (size_t)o.sw * o.sh * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+    kDisplay[r.capture][r.keywords]<<<grid2d(r.width, y1 - y0, b), b, 0, h->stream>>>(a);
+    if ((rc = check_launch(h, "display_kernel"))) return rc;
+    CU(cudaMemcpyAsync(r.host, h->frame, r.n * (r.capture ? 1 : sizeof(float)), cudaMemcpyDeviceToHost, h->stream));
+    if (bloom_on && r.host_bloom) CU(cudaMemcpyAsync(r.host_bloom, h->pfx.bloom, (size_t)o.bw * o.bh * sizeof(float4), cudaMemcpyDeviceToHost, h->stream));
+    if (sun_on && r.host_sunrays) CU(cudaMemcpyAsync(r.host_sunrays, h->pfx.sun, (size_t)o.sw * o.sh * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
     CU(cudaStreamSynchronize(h->stream));
     return FLUID_OK;
 }
 
-// render() with the display keywords of updateKeywords (S:1160-1166): without BLOOM and SUNRAYS this is
-// fluid_render (slab bands, half storage), with either of them render_postfx.
+// render(target) for config.BLOOM = config.SUNRAYS = false: the background selected by FLUID_BACKGROUND
+// (colour / checkerboard / none), then the display shader (optionally SHADING) blended over it.
+int fluid_render(fluid_t* h, int width, int height, int shading, float back_r, float back_g,
+                 float back_b, float* host_rgba, size_t n_floats) {
+    return draw(h, {.what = "fluid_render", .width = width, .height = height, .canvas_w = width, .canvas_h = height,
+                    .keywords = shading ? (uint32_t)FLUID_DISPLAY_SHADING : 0u, .back = {back_r, back_g, back_b},
+                    .bg_mode = h ? h->background : 0, .host = host_rgba, .n = n_floats});
+}
+
+// render() with the display keywords of updateKeywords (S:1160-1166); the post-FX FBOs are sized from
+// the target.
 int fluid_render_keywords(fluid_t* h, int width, int height, uint32_t keywords, const fluid_postfx* fx,
                           const float* dither_rgb, int dw, int dh, float back_r, float back_g, float back_b,
                           float* host_rgba, size_t n_floats, float* host_bloom, float* host_sunrays) {
-    if (!h) return FLUID_ERR_INVALID;
-    if (keywords & ~(uint32_t)(FLUID_DISPLAY_SHADING | FLUID_DISPLAY_BLOOM | FLUID_DISPLAY_SUNRAYS))
-        return fail(h, FLUID_ERR_INVALID, "unknown display keyword bits 0x%x", keywords);
-    if (!(keywords & (FLUID_DISPLAY_BLOOM | FLUID_DISPLAY_SUNRAYS)))
-        return fluid_render(h, width, height, (keywords & FLUID_DISPLAY_SHADING) ? 1 : 0, back_r, back_g, back_b,
-                            host_rgba, n_floats);
-    return render_postfx(h, "fluid_render_keywords", width, height, keywords, fx, dither_rgb, dw, dh, back_r,
-                         back_g, back_b, host_rgba, n_floats, host_bloom, host_sunrays);
+    return draw(h, {.what = "fluid_render_keywords", .width = width, .height = height, .canvas_w = width,
+                    .canvas_h = height, .keywords = keywords, .fx = fx, .dither = dither_rgb, .dw = dw, .dh = dh,
+                    .back = {back_r, back_g, back_b}, .bg_mode = h ? h->background : 0, .host = host_rgba,
+                    .n = n_floats, .host_bloom = host_bloom, .host_sunrays = host_sunrays});
 }
 
 // render(null) with the reference's desktop defaults SHADING = BLOOM = SUNRAYS = true (S:70-84)
 int fluid_render_postfx(fluid_t* h, int width, int height, const fluid_postfx* fx, const float* dither_rgb,
                         int dw, int dh, float back_r, float back_g, float back_b, float* host_rgba,
                         size_t n_floats, float* host_bloom, float* host_sunrays) {
-    return render_postfx(h, "fluid_render_postfx", width, height,
-                         FLUID_DISPLAY_SHADING | FLUID_DISPLAY_BLOOM | FLUID_DISPLAY_SUNRAYS, fx, dither_rgb, dw,
-                         dh, back_r, back_g, back_b, host_rgba, n_floats, host_bloom, host_sunrays);
+    return draw(h, {.what = "fluid_render_postfx", .width = width, .height = height, .canvas_w = width,
+                    .canvas_h = height, .keywords = FLUID_DISPLAY_SHADING | FLUID_DISPLAY_BLOOM | FLUID_DISPLAY_SUNRAYS,
+                    .fx = fx, .dither = dither_rgb, .dw = dw, .dh = dh, .back = {back_r, back_g, back_b},
+                    .bg_mode = h ? h->background : 0, .host = host_rgba, .n = n_floats, .host_bloom = host_bloom,
+                    .host_sunrays = host_sunrays});
 }
 
 // captureScreenshot (S:287-299) up to normalizeTexture (S:309-327): render(target) into a width x height
@@ -1797,45 +1795,13 @@ int fluid_render_postfx(fluid_t* h, int width, int height, const fluid_postfx* f
 int fluid_capture(fluid_t* h, int width, int height, int canvas_w, int canvas_h, uint32_t keywords,
                   int transparent, const fluid_postfx* fx, const float* dither_rgb, int dw, int dh,
                   float back_r, float back_g, float back_b, uint8_t* host_rgba8, size_t n_bytes) {
-    if (!h) return FLUID_ERR_INVALID;
-    if (keywords & ~(uint32_t)(FLUID_DISPLAY_SHADING | FLUID_DISPLAY_BLOOM | FLUID_DISPLAY_SUNRAYS))
-        return fail(h, FLUID_ERR_INVALID, "unknown display keyword bits 0x%x", keywords);
-    const bool bloom_on = keywords & FLUID_DISPLAY_BLOOM, sun_on = keywords & FLUID_DISPLAY_SUNRAYS;
-    const bool postfx = bloom_on || sun_on;
-    if (!host_rgba8 || width < 1 || height < 1 || canvas_w < 1 || canvas_h < 1 || (postfx && !fx) ||
-        (bloom_on && (!dither_rgb || dw < 1 || dh < 1)))
-        return fail(h, FLUID_ERR_INVALID, "bad argument");
-    const size_t cells = (size_t)width * height;
-    if (n_bytes != 4 * cells) return fail(h, FLUID_ERR_INVALID, "capture image has %zu bytes, caller passed %zu", 4 * cells, n_bytes);
-    if (h->slab()) return not_on_slab(h, "fluid_capture");
-    if (h->half && postfx)
-        return fail(h, FLUID_ERR_INVALID, "fluid_capture with BLOOM or SUNRAYS is not built for FLUID_FLAG_HALF_STORAGE");
     // drawColor's store of normalizeColor(BACK_COLOR) into the half-float target
     const float b16[3] = {__half2float(__float2half_rn(back_r)), __half2float(__float2half_rn(back_g)),
                           __half2float(__float2half_rn(back_b))};
-    const int bg_mode = transparent ? 2 : 0;
-    int rc = need_frame(h, (cells + 3) / 4); if (rc) return rc;      // the frame's storage holds the uchar4 image
-    uchar4* img = (uchar4*)h->frame;
-    dim3 b(32, 8);
-    if (!postfx) {
-        const float4* dye_src;
-        if ((rc = display_source(h, &dye_src))) return rc;
-        display_kernel<StoreCapture><<<grid2d(width, height, b), b, 0, h->stream>>>(
-            dye_src, h->cfg.dye_w, h->cfg.dye_h, img, width, height, (keywords & FLUID_DISPLAY_SHADING) ? 1 : 0,
-            b16[0], b16[1], b16[2], make_float2((float)(1.0 / (double)width), (float)(1.0 / (double)height)), bg_mode,
-            h->cfg.aspect, 0, 0, height);
-    } else {
-        PostFXOut o;
-        if ((rc = post_fx_chains(h, keywords, fx, dither_rgb, dw, dh, canvas_w, canvas_h, &o))) return rc;
-        kDisplayCapture[keywords]<<<grid2d(width, height, b), b, 0, h->stream>>>(
-            (const float4*)h->dye.read, h->cfg.dye_w, h->cfg.dye_h, bloom_on ? h->pfx.bloom : nullptr, o.bw, o.bh,
-            sun_on ? h->pfx.sun : nullptr, o.sw, o.sh, bloom_on ? h->pfx.dither : nullptr, dw, dh, img, width,
-            height, b16[0], b16[1], b16[2], bg_mode, h->cfg.aspect, display_scales(keywords, width, height, dw, dh));
-    }
-    if ((rc = check_launch(h, "capture display kernel"))) return rc;
-    CU(cudaMemcpyAsync(host_rgba8, img, n_bytes, cudaMemcpyDeviceToHost, h->stream));
-    CU(cudaStreamSynchronize(h->stream));
-    return FLUID_OK;
+    return draw(h, {.what = "fluid_capture", .width = width, .height = height, .canvas_w = canvas_w,
+                    .canvas_h = canvas_h, .keywords = keywords, .fx = fx, .dither = dither_rgb, .dw = dw, .dh = dh,
+                    .back = {b16[0], b16[1], b16[2]}, .bg_mode = transparent ? 2 : 0, .capture = true,
+                    .host = host_rgba8, .n = n_bytes});
 }
 
 void* fluid_host_alloc(size_t bytes) {

@@ -1,28 +1,20 @@
-// postfx.cuh — the display-side post-FX of render() (SURVEY §8f rank 1, second half): bloom
-// (applyBloom S:1350-1394; shaders S:614-674) and sunrays (applySunrays + blur S:1396-1419; shaders
-// S:461-494, S:676-724) and the display shader for every keyword set with BLOOM or SUNRAYS (S:549-612).
+// postfx.cuh — the display side of render() and captureScreenshot() (SURVEY §8f rank 1, second half):
+// the post-FX chains of bloom (applyBloom S:1350-1394; shaders S:614-674) and sunrays (applySunrays +
+// blur S:1396-1419; shaders S:461-494, S:676-724), and the display shader (S:549-612) for all eight
+// keyword sets, drawn over the background into the fp32 frame of render() or the 8-bit image of
+// captureScreenshot.
 //
 // Every kernel is one reference blit: one thread per target texel, sources fetched through the
-// GL_LINEAR formula of passes.cuh (linear_fetch4).  Arithmetic order follows the GLSL; with the
+// GL_LINEAR formula of passes.cuh (linear_fetch).  Arithmetic order follows the GLSL; with the
 // library's --fmad=false / IEEE div+sqrt build everything is bit-identical to the CPU oracle except
 // the display's pow() (linearToGamma), which is tolerance-checked like splat's exp().
 #pragma once
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
 #include "passes.cuh"
 
 namespace fk {
-
-__device__ __forceinline__ float linear_fetch1(const float* __restrict__ tex, int W, int H, float uvx, float uvy) {
-    const float u = uvx * (float)W - 0.5f, v = uvy * (float)H - 0.5f;
-    const float fi = floorf(u), fj = floorf(v);
-    const float a = u - fi, b = v - fj;
-    const int i0 = texel_index(fi, W), i1 = texel_index(fi + 1.0f, W);
-    const int j0 = texel_index(fj, H), j1 = texel_index(fj + 1.0f, H);
-    const float w00 = (1.0f - a) * (1.0f - b), w10 = a * (1.0f - b), w01 = (1.0f - a) * b, w11 = a * b;
-    return ((w00 * __ldg(&tex[(size_t)j0 * W + i0]) + w10 * __ldg(&tex[(size_t)j0 * W + i1])) +
-            w01 * __ldg(&tex[(size_t)j1 * W + i0])) + w11 * __ldg(&tex[(size_t)j1 * W + i1]);
-}
 
 // REPEAT-wrapped LINEAR fetch of the first channel of an RGB (3 floats / texel) texture: the
 // dithering texture (createTextureAsync S:1128-1158: LINEAR, REPEAT).
@@ -46,7 +38,7 @@ __global__ void __launch_bounds__(256) bloom_prefilter_kernel(const float4* __re
     const int i = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y * blockDim.y + threadIdx.y;
     if (i >= w || j >= h) return;
     const float uvx = ((float)i + 0.5f) / (float)w, uvy = ((float)j + 0.5f) / (float)h;
-    const float4 c = linear_fetch4(dye, Wd, Hd, uvx, uvy);
+    const float4 c = linear_fetch(dye, Wd, Hd, uvx, uvy);
     const float br = fmaxf(c.x, fmaxf(c.y, c.z));
     float rq = fminf(fmaxf(br - curve0, 0.0f), curve1);
     rq = (curve2 * rq) * rq;
@@ -61,8 +53,8 @@ __global__ void __launch_bounds__(256) box4_kernel(const float4* __restrict__ sr
     if (i >= w || j >= h) return;
     const float tsx = (float)(1.0 / (double)ws), tsy = (float)(1.0 / (double)hs);
     const float uvx = ((float)i + 0.5f) / (float)w, uvy = ((float)j + 0.5f) / (float)h;
-    const float4 L = linear_fetch4(src, ws, hs, uvx - tsx, uvy), R = linear_fetch4(src, ws, hs, uvx + tsx, uvy);
-    const float4 T = linear_fetch4(src, ws, hs, uvx, uvy + tsy), B = linear_fetch4(src, ws, hs, uvx, uvy - tsy);
+    const float4 L = linear_fetch(src, ws, hs, uvx - tsx, uvy), R = linear_fetch(src, ws, hs, uvx + tsx, uvy);
+    const float4 T = linear_fetch(src, ws, hs, uvx, uvy + tsy), B = linear_fetch(src, ws, hs, uvx, uvy - tsy);
     float4 s;
     s.x = ((((0.0f + L.x) + R.x) + T.x) + B.x) * 0.25f * scale;
     s.y = ((((0.0f + L.y) + R.y) + T.y) + B.y) * 0.25f * scale;
@@ -79,7 +71,7 @@ __global__ void __launch_bounds__(256) sunrays_mask_kernel(const float4* __restr
     const int i = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y * blockDim.y + threadIdx.y;
     if (i >= Wd || j >= Hd) return;
     const float uvx = ((float)i + 0.5f) / (float)Wd, uvy = ((float)j + 0.5f) / (float)Hd;
-    float4 c = linear_fetch4(dye, Wd, Hd, uvx, uvy);
+    float4 c = linear_fetch(dye, Wd, Hd, uvx, uvy);
     const float br = fmaxf(c.x, fmaxf(c.y, c.z));
     c.w = 1.0f - fminf(fmaxf(br * 20.0f, 0.0f), 0.8f);
     mask[(size_t)j * Wd + i] = c;
@@ -97,11 +89,11 @@ __global__ void __launch_bounds__(256) sunrays_kernel(const float4* __restrict__
     float dx = uvx - 0.5f, dy = uvy - 0.5f;
     dx = dx * f; dy = dy * f;
     float illum = 1.0f;
-    float color = linear_fetch4(mask, Wm, Hm, uvx, uvy).w;
+    float color = linear_fetch(mask, Wm, Hm, uvx, uvy).w;
 #pragma unroll 1
     for (int k = 0; k < 16; ++k) {
         cx = cx - dx; cy = cy - dy;
-        const float col = linear_fetch4(mask, Wm, Hm, cx, cy).w;
+        const float col = linear_fetch(mask, Wm, Hm, cx, cy).w;
         color = color + (col * illum) * weight;
         illum = illum * Decay;
     }
@@ -115,37 +107,99 @@ __global__ void __launch_bounds__(256) blur3_kernel(const float* __restrict__ sr
     if (i >= w || j >= h) return;
     const float off = 1.33333333f;
     const float uvx = ((float)i + 0.5f) / (float)w, uvy = ((float)j + 0.5f) / (float)h;
-    const float c = linear_fetch1(src, w, h, uvx, uvy);
-    const float l = linear_fetch1(src, w, h, uvx - tsx * off, uvy - tsy * off);
-    const float r = linear_fetch1(src, w, h, uvx + tsx * off, uvy + tsy * off);
+    const float c = linear_fetch(src, w, h, uvx, uvy);
+    const float l = linear_fetch(src, w, h, uvx - tsx * off, uvy - tsy * off);
+    const float r = linear_fetch(src, w, h, uvx + tsx * off, uvy + tsy * off);
     float sum = c * 0.29411764f;
     sum = sum + l * 0.35294117f;
     sum = sum + r * 0.35294117f;
     dst[(size_t)j * w + i] = sum;
 }
 
+__device__ __forceinline__ float len3(float4 v) { return sqrtf((v.x * v.x + v.y * v.y) + v.z * v.z); }
+
+// What drawDisplay is blended over (render(), S:1296-1317) with blendFunc(ONE, ONE_MINUS_SRC_ALPHA)
+// (S:1305): bg_mode 0 = drawColor(BACK_COLOR) (S:1319-1323); 1 = drawCheckerboard — TRANSPARENT on the
+// screen (S:1325-1329, checkerboardShader S:531-547: v = mod(floor(uv.x * 25 * aspect) + floor(uv.y * 25), 2)
+// * 0.1 + 0.8); 2 = nothing, blending disabled — TRANSPARENT into a capture target (S:1307-1308): the
+// display colour goes out as it is.
+__device__ __forceinline__ float4 blend_over_background(float cr, float cg, float cb, float a, int bg_mode, float br,
+                                                        float bg, float bb, float aspect, float uvx, float uvy) {
+    if (bg_mode == 2) return make_float4(cr, cg, cb, a);
+    if (bg_mode == 1) {
+        const float x = floorf((uvx * 25.0f) * aspect), y = floorf((uvy * 25.0f) * 1.0f);
+        const float sxy = x + y;
+        float v = sxy - 2.0f * floorf(sxy / 2.0f);
+        v = v * 0.1f + 0.8f;
+        br = bg = bb = v;
+    }
+    const float k = 1.0f - a;
+    return make_float4(cr + br * k, cg + bg * k, cb + bb * k, a + 1.0f * k);
+}
+
+// normalizeTexture (S:309-327) of one channel of an RGBA half-float capture target (S:289): the value
+// is first stored into the fp16 target (round to nearest even, overflow to +-Inf), then clamp01 * 255
+// goes into a Uint8Array, which truncates.  An fp16 value times 255 is exact in fp32, so this is the
+// JS double result.  fmaxf(NaN, 0) = 0 gives ToUint8(NaN) = 0.
+__device__ __forceinline__ unsigned char capture_byte(float v) {
+    const float s = __half2float(__float2half_rn(v));
+    const float c = fminf(fmaxf(s, 0.0f), 1.0f);
+    return (unsigned char)__float2uint_rz(c * 255.0f);
+}
+
+// Output policies of display_kernel: the element type of `out`, the row of `out` that row r of an
+// n-row band goes to, and what is stored.
+// StoreFrame: the fp32 RGBA frame of render(), row 0 = bottom.
+struct StoreFrame {
+    using T = float4;
+    static __device__ __forceinline__ int row(int r, int) { return r; }
+    static __device__ __forceinline__ float4 pack(float4 v) { return v; }
+};
+// StoreCapture: captureScreenshot (S:287-327) up to the bytes toDataURL encodes: the fp16 store, then
+// normalizeTexture's 8-bit truncation and its flip (top row first).
+struct StoreCapture {
+    using T = uchar4;
+    static __device__ __forceinline__ int row(int r, int n) { return n - 1 - r; }
+    static __device__ __forceinline__ uchar4 pack(float4 v) {
+        return make_uchar4(capture_byte(v.x), capture_byte(v.y), capture_byte(v.z), capture_byte(v.w));
+    }
+};
+
+// The inputs of display_kernel.  Those of a keyword that is off are never read.
+struct DisplayArgs {
+    const float4* dye;                  // fp32 dye; its first row is global row dye_row_off
+    int Wd, Hd, dye_row_off;
+    const float4* bloom; int bw, bh;    // the bloom FBO (BLOOM)
+    const float* sun; int sw, sh;       // the sunrays texture (SUNRAYS)
+    const float* dither; int dw, dh;    // the RGB dithering texture (BLOOM)
+    void* out;                          // Out::T texels of the rows [y0, y1) of the w x h target
+    int w, h, y0, y1;
+    float br, bg, bb;                   // background colour (bg_mode 0)
+    int bg_mode;
+    float aspect;
+    float4 ts;                          // 1/w, 1/h and getTextureScale of the dithering texture (BLOOM)
+};
+
 // displayShaderSource S:549-612 compiled with the keywords updateKeywords picks (S:1160-1166), over
-// the background of render(), premultiplied blend.  One instantiation per keyword set with BLOOM or
-// SUNRAYS; the sets with neither use display_kernel (passes.cuh).  The inputs of a keyword that is
-// off are never read (pass nullptr).  Out: the output policy (passes.cuh), the fp32 frame of render()
-// or the 8-bit image of captureScreenshot.
-template <bool SHADING, bool BLOOM, bool SUNRAYS, class Out = StoreFrame>
-__global__ void __launch_bounds__(256) display_full_kernel(const float4* __restrict__ dye, int Wd, int Hd,
-                                                           const float4* __restrict__ bloom, int bw, int bh,
-                                                           const float* __restrict__ sun, int sw, int sh,
-                                                           const float* __restrict__ dither, int dw, int dh,
-                                                           typename Out::T* __restrict__ out, int w, int h, float br_, float bg_,
-                                                           float bb_, int bg_mode, float aspect, float4 ts) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y * blockDim.y + threadIdx.y;
-    if (i >= w || j >= h) return;
-    const float tsx = ts.x, tsy = ts.y;     // 1/width, 1/height (S:1337) and getTextureScale (S:1626-1631): JS doubles, narrowed on the host
-    const float dsx = ts.z, dsy = ts.w;
-    const float uvx = ((float)i + 0.5f) / (float)w, uvy = ((float)j + 0.5f) / (float)h;
-    const float4 c = linear_fetch4(dye, Wd, Hd, uvx, uvy);
+// the background of render() (blend_over_background).  Out: the output policy.  A slab rank draws the
+// band [y0, y1) of the target from its own dye rows (+ ghost rows); one GPU draws the whole target.
+template <bool SHADING, bool BLOOM, bool SUNRAYS, class Out>
+__global__ void __launch_bounds__(256) display_kernel(DisplayArgs a) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x, j = a.y0 + blockIdx.y * blockDim.y + threadIdx.y;
+    if (i >= a.w || j >= a.y1) return;
+    const float tsx = a.ts.x, tsy = a.ts.y;     // 1/width, 1/height (S:1337) and getTextureScale (S:1626-1631): JS doubles, narrowed on the host
+    const float dsx = a.ts.z, dsy = a.ts.w;
+    // the destination is formed up front: fewer values live across the IEEE div / sqrt slow paths
+    // (the capture instantiation spills otherwise)
+    typename Out::T* const o = static_cast<typename Out::T*>(a.out) + (size_t)Out::row(j - a.y0, a.y1 - a.y0) * a.w + i;
+    const float uvx = ((float)i + 0.5f) / (float)a.w, uvy = ((float)j + 0.5f) / (float)a.h;
+    const float4 c = linear_fetch(a.dye, a.Wd, a.Hd, uvx, uvy, a.dye_row_off);
     float cc[3] = {c.x, c.y, c.z};
     if constexpr (SHADING) {
-        const float4 lc = linear_fetch4(dye, Wd, Hd, uvx - tsx, uvy), rc = linear_fetch4(dye, Wd, Hd, uvx + tsx, uvy);
-        const float4 tc = linear_fetch4(dye, Wd, Hd, uvx, uvy + tsy), bc = linear_fetch4(dye, Wd, Hd, uvx, uvy - tsy);
+        const float4 lc = linear_fetch(a.dye, a.Wd, a.Hd, uvx - tsx, uvy, a.dye_row_off);
+        const float4 rc = linear_fetch(a.dye, a.Wd, a.Hd, uvx + tsx, uvy, a.dye_row_off);
+        const float4 tc = linear_fetch(a.dye, a.Wd, a.Hd, uvx, uvy + tsy, a.dye_row_off);
+        const float4 bc = linear_fetch(a.dye, a.Wd, a.Hd, uvx, uvy - tsy, a.dye_row_off);
         const float dx = len3(rc) - len3(lc), dy = len3(tc) - len3(bc);
         const float nz = sqrtf(tsx * tsx + tsy * tsy);
         const float nl = sqrtf((dx * dx + dy * dy) + nz * nz);
@@ -156,11 +210,11 @@ __global__ void __launch_bounds__(256) display_full_kernel(const float4* __restr
     }
     float bl[3] = {0.0f, 0.0f, 0.0f};
     if constexpr (BLOOM) {
-        const float4 b = linear_fetch4(bloom, bw, bh, uvx, uvy);
+        const float4 b = linear_fetch(a.bloom, a.bw, a.bh, uvx, uvy);
         bl[0] = b.x; bl[1] = b.y; bl[2] = b.z;
     }
     if constexpr (SUNRAYS) {
-        const float s = linear_fetch1(sun, sw, sh, uvx, uvy);
+        const float s = linear_fetch(a.sun, a.sw, a.sh, uvx, uvy);
 #pragma unroll
         for (int k = 0; k < 3; ++k) {
             cc[k] = cc[k] * s;
@@ -168,7 +222,7 @@ __global__ void __launch_bounds__(256) display_full_kernel(const float4* __restr
         }
     }
     if constexpr (BLOOM) {
-        const float noise = linear_fetch_rgb_r_repeat(dither, dw, dh, uvx * dsx, uvy * dsy) * 2.0f - 1.0f;
+        const float noise = linear_fetch_rgb_r_repeat(a.dither, a.dw, a.dh, uvx * dsx, uvy * dsy) * 2.0f - 1.0f;
 #pragma unroll
         for (int k = 0; k < 3; ++k) {
             float bk = bl[k] + noise / 255.0f;
@@ -177,9 +231,8 @@ __global__ void __launch_bounds__(256) display_full_kernel(const float4* __restr
             cc[k] = cc[k] + bk;
         }
     }
-    const float a = fmaxf(cc[0], fmaxf(cc[1], cc[2]));
-    out[(size_t)Out::row(j, h) * w + i] =
-        Out::pack(blend_over_background(cc[0], cc[1], cc[2], a, bg_mode, br_, bg_, bb_, aspect, uvx, uvy));
+    const float alpha = fmaxf(cc[0], fmaxf(cc[1], cc[2]));
+    *o = Out::pack(blend_over_background(cc[0], cc[1], cc[2], alpha, a.bg_mode, a.br, a.bg, a.bb, a.aspect, uvx, uvy));
 }
 
 }  // namespace fk
