@@ -9,7 +9,8 @@ truncated to uint8, and its flip (top row first).
 
 The byte tolerance rule: B(x) = trunc(clamp01(fp16(x)) * 255) is monotone in x, so a byte is accepted
 when it lies in [B(v - d), B(v + d)] with v the model's fp32 pre-store value and d = delta * max(1, |v|),
-delta being the fp32 tolerance of the same comparison in the display keyword tests.
+delta being the fp32 tolerance of the same comparison against the executed shaders.  Against this
+build, captures with BLOOM are checked per texel instead (gamma_model.capture_interval).
 """
 import numpy as np
 

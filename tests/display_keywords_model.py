@@ -42,11 +42,19 @@ def _len3(c):
     return np.sqrt((c[..., 0] * c[..., 0] + c[..., 1] * c[..., 1]) + c[..., 2] * c[..., 2])
 
 
-def _display(dye, w, h, keywords, bloom, sun, dither, back_rgb, background, aspect):
-    """displayShaderSource with `keywords`, then the background of render() (oracle background modes)."""
-    tsx, tsy = F(1.0 / w), F(1.0 / h)
+def uv_grid(w, h):
+    """vUv of every texel of a w x h target: (h, w) fp32 arrays (i + .5) / w and (j + .5) / h."""
     uvx = ((np.arange(w, dtype=F) + F(0.5)) / F(w))[None, :].repeat(h, 0)
     uvy = ((np.arange(h, dtype=F) + F(0.5)) / F(h))[:, None].repeat(w, 1)
+    return uvx, uvy
+
+
+def colour_terms(dye, w, h, keywords, bloom, sun):
+    """displayShaderSource up to the dithering: the dye colour c (LINEAR fetch, SHADING's diffuse, the
+    sunrays multiply) and, with BLOOM, the bloom colour bl (LINEAR fetch, sunrays multiply), else None.
+    Every max / min is C's fmaxf / fminf (np.fmax / np.fmin: a NaN argument is dropped)."""
+    tsx, tsy = F(1.0 / w), F(1.0 / h)
+    uvx, uvy = uv_grid(w, h)
     c = _fetch(dye, uvx, uvy)[..., :3]
     if keywords & SHADING:
         dx = _len3(_fetch(dye, uvx + tsx, uvy)) - _len3(_fetch(dye, uvx - tsx, uvy))
@@ -54,33 +62,72 @@ def _display(dye, w, h, keywords, bloom, sun, dither, back_rgb, background, aspe
         nz = np.sqrt(tsx * tsx + tsy * tsy)
         nl = np.sqrt((dx * dx + dy * dy) + nz * nz)
         d = ((dx / nl) * F(0) + (dy / nl) * F(0)) + (nz / nl) * F(1)
-        diffuse = np.minimum(np.maximum(d + F(0.7), F(0.7)), F(1))
+        diffuse = np.fmin(np.fmax(d + F(0.7), F(0.7)), F(1))
         c = c * diffuse[..., None]
-    if keywords & BLOOM:
-        bl = _fetch(bloom, uvx, uvy)[..., :3]
+    bl = _fetch(bloom, uvx, uvy)[..., :3] if keywords & BLOOM else None
     if keywords & SUNRAYS:
         s = _fetch(sun[..., None], uvx, uvy)
         c = c * s
         if keywords & BLOOM:
             bl = bl * s
-    if keywords & BLOOM:
-        dsx, dsy = F(w / dither.shape[1]), F(h / dither.shape[0])                 # getTextureScale, S:1626-1631
-        noise = _fetch(dither, uvx * dsx, uvy * dsy, repeat=True)[..., :1] * F(2) - F(1)
-        bk = np.maximum(bl + noise / F(255), F(0))
-        bk = np.maximum(F(1.055) * np.power(bk, F(0.416666667)) - F(0.055), F(0))   # linearToGamma S:565-568
-        c = c + bk
-    a = np.maximum(c[..., 0], np.maximum(c[..., 1], c[..., 2]))[..., None]
-    if background == O.BG_NONE:
-        return np.concatenate([c, a], axis=-1).astype(F)
-    if background == O.BG_CHECKERBOARD:                                             # checkerboardShader S:531-547
+    return c, bl
+
+
+def dither_scale(w, h, dither):
+    """getTextureScale (S:1626-1631) of the dithering texture on a w x h target: JS doubles, narrowed once."""
+    return F(w / dither.shape[1]), F(h / dither.shape[0])
+
+
+def gamma_argument(bl, dither, w, h, scale=None):
+    """The argument of linearToGamma's pow: fmaxf(bl + noise / 255, 0), noise = the REPEAT LINEAR fetch of
+    the dithering texture at vUv * getTextureScale, * 2 - 1.  `scale` defaults to the w x h target's."""
+    dsx, dsy = scale if scale is not None else dither_scale(w, h, dither)
+    uvx, uvy = uv_grid(w, h)
+    noise = _fetch(dither, uvx * dsx, uvy * dsy, repeat=True)[..., :1] * F(2) - F(1)
+    return np.fmax(bl + noise / F(255), F(0))
+
+
+GAMMA_EXPONENT = F(0.416666667)
+
+
+def linear_to_gamma(p):
+    """linearToGamma (S:565-568) after its pow: fmaxf(1.055 * p - 0.055, 0), p = pow(bk, 0.416666667)."""
+    return np.fmax(F(1.055) * p - F(0.055), F(0))
+
+
+def background_colour(w, h, back_rgb, background, aspect):
+    """What the display is blended over, (h, w, 3): BACK_COLOR, or checkerboardShader (S:531-547)."""
+    if background == O.BG_CHECKERBOARD:
+        uvx, uvy = uv_grid(w, h)
         x = np.floor((uvx * F(25)) * F(aspect)); y = np.floor((uvy * F(25)) * F(1))
         sxy = x + y
         v = (sxy - F(2) * np.floor(sxy / F(2))) * F(0.1) + F(0.8)
-        bg = np.stack([v, v, v], axis=-1)
-    else:
-        bg = np.broadcast_to(np.asarray(back_rgb, F), c.shape)
+        return np.stack([v, v, v], axis=-1)
+    return np.broadcast_to(np.asarray(back_rgb, F), (h, w, 3))
+
+
+def alpha_of(c):
+    """The display's alpha: fmaxf(c.r, fmaxf(c.g, c.b))."""
+    return np.fmax(c[..., 0], np.fmax(c[..., 1], c[..., 2]))[..., None]
+
+
+def over_background(c, a, back_rgb, background, aspect):
+    """render()'s blend ONE / ONE_MINUS_SRC_ALPHA of (c, a) over the background, or (c, a) bare (BG_NONE)."""
+    if background == O.BG_NONE:
+        return np.concatenate([c, a], axis=-1).astype(F)
+    h, w = c.shape[:2]
+    bg = background_colour(w, h, back_rgb, background, aspect)
     k = F(1) - a
     return np.concatenate([c + bg * k, a + F(1) * k], axis=-1).astype(F)
+
+
+def _display(dye, w, h, keywords, bloom, sun, dither, back_rgb, background, aspect):
+    """displayShaderSource with `keywords`, then the background of render() (oracle background modes)."""
+    c, bl = colour_terms(dye, w, h, keywords, bloom, sun)
+    if keywords & BLOOM:
+        bk = gamma_argument(bl, dither, w, h)
+        c = c + linear_to_gamma(np.power(bk, GAMMA_EXPONENT))      # linearToGamma S:565-568
+    return over_background(c, alpha_of(c), back_rgb, background, aspect)
 
 
 def render_keywords(dye, w, h, dither, cfg=None, back_rgb=(0.0, 0.0, 0.0), background=O.BG_COLOR, aspect=None,

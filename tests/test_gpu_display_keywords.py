@@ -7,13 +7,13 @@ import numpy as np
 import pytest
 
 import display_keywords_model as M
+import gamma_model as G
 from conftest import bits_equal, golden, max_rel
 
 pytestmark = pytest.mark.gpu
 FXCFG = dict(BLOOM_RESOLUTION=64, SUNRAYS_RESOLUTION=48)
 BACK = {"r": 10, "g": 20, "b": 30}
 BACK_RGB = (10 / 255, 20 / 255, 30 / 255)
-POW_TOL = 5e-6          # powf in linearToGamma: CUDA vs glibc last-place differences
 
 
 @pytest.fixture(scope="module")
@@ -46,12 +46,16 @@ def set_keywords(pkg, s, kw):
                     SUNRAYS=bool(kw & pkg.DISPLAY_SUNRAYS))
 
 
-def check_vs_oracle(pkg, s, got, ref, kw):
-    """Sets without BLOOM: frame bitwise.  With BLOOM: frame within the powf tolerance, bloom FBO bitwise.
-    With SUNRAYS: sunrays texture bitwise.  The textures of keywords that are off are not returned."""
+def check_vs_oracle(pkg, s, got, ref, kw, dye, dither, background=M.O.BG_COLOR):
+    """Sets without BLOOM: frame bitwise.  With BLOOM: bloom FBO bitwise, every value of the frame within
+    the per-texel powf interval of gamma_model.py.  With SUNRAYS: sunrays texture bitwise.  The textures
+    of keywords that are off are not returned."""
     if kw & pkg.DISPLAY_BLOOM:
-        assert max_rel(got, ref["target"]) < POW_TOL
         assert bits_equal(s.last_bloom, ref["bloom"])
+        h, w = got.shape[:2]
+        lo, hi = G.display_interval(dye, w, h, kw, s.last_bloom, s.last_sunrays, dither, BACK_RGB, background, w / h)
+        n, bad = G.check_display(got, lo, hi)
+        assert n == 0, (kw, background, n, bad)
     else:
         assert bits_equal(got, ref["target"])
         assert s.last_bloom is None
@@ -76,7 +80,7 @@ def test_every_keyword_set_and_background_vs_oracle(pkg, oracle, dither, Wd, Hd,
             s.config["TRANSPARENT"] = transparent
             got = s.render(w, h, target=target)
             ref = M.render_keywords(dye, w, h, dither, cfg=FXCFG, back_rgb=BACK_RGB, background=bg, keywords=kw)
-            check_vs_oracle(pkg, s, got, ref, kw)
+            check_vs_oracle(pkg, s, got, ref, kw, dye, dither, bg)
             assert bits_equal(s.readField("dye"), dye), (kw, bg)
     s.close()
 
@@ -141,7 +145,7 @@ def test_post_fx_targets_are_reused_and_remade_on_resize(pkg, oracle, dither):
         s.canvas = {"width": w, "height": h}
         got = s.render(w, h)
         ref = M.render_keywords(dye, w, h, dither, cfg=fx, back_rgb=BACK_RGB, keywords=kw)
-        check_vs_oracle(pkg, s, got, ref, kw)
+        check_vs_oracle(pkg, s, got, ref, kw, dye, dither)
     assert np.all(s.last_bloom == np.array([0, 0, 0, 1], np.float32))
     s.close()
 
