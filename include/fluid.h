@@ -314,7 +314,9 @@ typedef enum fluid_stat_key {
     FLUID_STAT_GRAPH_LAUNCHES = 5,   /* step() graphs replayed                                        */
     FLUID_STAT_HALO_TRANSPORT_P2P = 6, /* 1 when the peer-memory halo path is active                   */
     FLUID_STAT_CVD_STREAM_LAUNCHES = 7,      /* row-streaming curl-vorticity-divergence kernels executed */
-    FLUID_STAT_GRADIENT_STREAM_LAUNCHES = 8  /* row-streaming gradientSubtract kernels executed          */
+    FLUID_STAT_GRADIENT_STREAM_LAUNCHES = 8, /* row-streaming gradientSubtract kernels executed          */
+    FLUID_STAT_JACOBI_EXACT_STREAMS = 9      /* blocked Jacobi warps that ran the un-contracted tail:
+                                                tiny divergence, or inputs near FLT_MAX (synchronises)  */
 } fluid_stat_key;
 uint64_t fluid_stat(fluid_t* h, int key);
 

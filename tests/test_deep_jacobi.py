@@ -64,8 +64,9 @@ def test_depth13_bitwise_vs_naive_and_oracle(oracle):
             s = pkg.FluidSimulation({"SIM_RESOLUTION": min(W, H), "DYE_RESOLUTION": 8, "PRESSURE_ITERATIONS": iters},
                                     canvas_width=W, canvas_height=H, flags=flags, jacobi_block=block, sizes=(W, H, 8, 8))
             s.writeField("pressure", p); s.writeField("divergence", d); s.pass_("pressure_solve")
-            got, launches = s.readField("pressure"), s.stat("jacobi_launches")
+            got, launches, exact = s.readField("pressure"), s.stat("jacobi_launches"), s.stat("jacobi_exact_streams")
             s.close()
+            assert (exact > 0) == (tiny and not flags), (W, H, iters, jb, flags, exact)
             assert bits_equal(got, want), (W, H, iters, jb, flags)
             if not flags:
                 assert launches == -(-iters // K_MAX), (W, H, iters, jb)

@@ -23,5 +23,6 @@ def test_mirrored_and_interior_windows_bitwise_every_depth(oracle, W, H):
                                 canvas_width=W, canvas_height=H, jacobi_block=jb, sizes=(W, H, 8, 8))
         s.writeField("pressure", p); s.writeField("divergence", d); s.pass_("pressure_solve")
         got = s.readField("pressure")
+        assert s.stat("jacobi_exact_streams") == 0, (W, H, jb)
         s.close()
         assert bits_equal(got, oracle.jacobi(oracle.clear(p, 0.8), d, 2 * jb + 1)), (W, H, jb)

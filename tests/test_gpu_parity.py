@@ -175,6 +175,7 @@ def test_temporally_blocked_jacobi_bitwise_equals_naive_and_oracle(pkg, oracle, 
         s.writeField("pressure", p); s.writeField("divergence", d)
         s.pass_("pressure_solve")
         outs.append(s.readField("pressure"))
+        assert s.stat("jacobi_exact_streams") == 0          # ordinary data: every stream contracted
         s.close()
     assert bits_equal(outs[0], outs[1])
     if W * H <= 1 << 20:
@@ -232,7 +233,9 @@ def test_properties_at_full_size_4096(pkg):
         # first launch -- exactly the configuration bench.py times
         s = make(pkg, W, H, 64, 64, flags=flags, jb=jb, PRESSURE_ITERATIONS=iters, PRESSURE=pressure)
         s.writeField("pressure", pp); s.writeField("divergence", dd)
-        s.pass_("pressure_solve"); out = s.readField("pressure"); s.close()
+        s.pass_("pressure_solve"); out = s.readField("pressure")
+        assert s.stat("jacobi_exact_streams") == 0
+        s.close()
         return out
     a = solve(p, d)
     assert bits_equal(a, solve(p, d, flags=pkg.FLAG_NAIVE_JACOBI, jb=1))
@@ -342,7 +345,9 @@ def test_blocked_jacobi_bitwise_with_subnormal_and_tiny_values(pkg, oracle, case
         s = make(pkg, W, H, 8, 8, jb=jb, PRESSURE_ITERATIONS=iters)
         s.writeField("pressure", p); s.writeField("divergence", d)
         s.pass_("pressure_solve")
-        got = s.readField("pressure"); s.close()
+        got = s.readField("pressure")
+        assert s.stat("jacobi_exact_streams") > 0, (case, jb)     # the tiny map sent streams to the exact tail
+        s.close()
         assert bits_equal(got, O.jacobi(O.clear(p, 0.8), d, iters)), (case, jb)
 
 

@@ -47,6 +47,7 @@ struct fluid {
     float* divergence = nullptr;
     float* curl = nullptr;
     int* halo_flag = nullptr;        // device flag set by advection when a tap leaves the ghost zone
+    unsigned long long* exact_streams = nullptr;   // device counter: blocked Jacobi warps that ran the exact tail
     uint64_t launches = 0;
     uint64_t jacobi_kernel_launches = 0;   // Jacobi kernels only (fluid_stat FLUID_STAT_JACOBI_LAUNCHES)
     uint64_t halo_kernel_launches = 0;     // halo_push / halo_wait kernels of the peer-memory transport
@@ -369,6 +370,7 @@ int run_jacobi(fluid_t* h, int iters, bool scale_first, int* launches_out) {
     a.scale = h->cfg.pressure;
     a.err = h->halo_flag;
     a.tiny_map = h->tiny_map;
+    a.exact_streams = h->exact_streams;
     // default depth: on an H100 at 4096^2 x 50 4 launches of 13 / 12 sweeps take 0.500 ms per solve and 5
     // launches of 10 take 0.524 (80 GB HBM3 card, 400 W power limit; DESIGN §5).  Iteration counts that
     // split into the same number of launches either way (20, 30, 40) keep depth 10 launches.
@@ -670,6 +672,8 @@ int create_common(const fluid_config* cfg, int rank, int world, const void* uid,
         for (auto& e : h->tev) CU(cudaEventCreate(&e));
         CU(cudaMalloc((void**)&h->halo_flag, sizeof(int)));
         CU(cudaMemsetAsync(h->halo_flag, 0, sizeof(int), h->stream));
+        CU(cudaMalloc((void**)&h->exact_streams, sizeof(unsigned long long)));
+        CU(cudaMemsetAsync(h->exact_streams, 0, sizeof(unsigned long long), h->stream));
         CU(cudaMalloc((void**)&h->dt_dev, sizeof(float)));
         CU(cudaMemsetAsync(h->dt_dev, 0, sizeof(float), h->stream));
         int r = alloc_fields(h); if (r) return r;
@@ -812,6 +816,7 @@ void fluid_destroy(fluid_t* h) {
     drop_graphs(h);
     free_fields(h);
     cudaFree(h->halo_flag);
+    cudaFree(h->exact_streams);
     cudaFree(h->dt_dev);
     cudaFree(h->scratch);
     cudaFree(h->frame);
@@ -1473,6 +1478,7 @@ int solve_host_banded(fluid_t* h, const float* div_host, float* p_host, int iter
             remaining -= K;
             JacobiArgs a{};
             a.W = W; a.H = H; a.scale = h->cfg.pressure; a.err = h->halo_flag; a.tiny_map = h->tiny_map;
+            a.exact_streams = h->exact_streams;
             a.out_lo = std::max(b_lo - remaining, 0); a.out_hi = std::min(b_hi + remaining, H);
             // the kernel addresses all three fields as "local row 0 + (row - row_off)": a whole-grid field G is
             // passed as G + loc*W
@@ -1857,6 +1863,12 @@ uint64_t fluid_stat(fluid_t* h, int key) {
         case FLUID_STAT_HALO_TRANSPORT_P2P: return h->p2p ? 1 : 0;
         case FLUID_STAT_CVD_STREAM_LAUNCHES: return h->cvd_stream_launches;
         case FLUID_STAT_GRADIENT_STREAM_LAUNCHES: return h->gradient_stream_launches;
+        case FLUID_STAT_JACOBI_EXACT_STREAMS: {          // counted on the device: waits for the handle's work
+            unsigned long long n = 0;
+            if (cudaMemcpyAsync(&n, h->exact_streams, sizeof n, cudaMemcpyDeviceToHost, h->stream) != cudaSuccess ||
+                cudaStreamSynchronize(h->stream) != cudaSuccess) return 0;
+            return n;
+        }
     }
     return 0;
 }

@@ -43,6 +43,7 @@ struct JacobiArgs {
     float scale;         // SCALE: value of config.PRESSURE
     int* err;            // device error word (3 = a bounded mbarrier wait gave up)
     const unsigned char* tiny_map;   // tb kernel: where divergence defeats the fma contraction (may be null)
+    unsigned long long* exact_streams;   // tb kernel: warps that ran the un-contracted tail (may be null)
 };
 
 // the two tensor maps a temporally blocked launch reads through: p describes the buffer passed as
@@ -122,14 +123,22 @@ __global__ void __launch_bounds__(256) jacobi_sweep_kernel(JacobiArgs a) {
 // FADD / FMUL / FFMA, 32 lanes per cycle per SM sub-partition).  The reference expression costs 5:
 // ((((L+R)+B)+T)-d)*0.25.  The last two contract into ONE fma with a pre-scaled divergence,
 //        fma(S, 0.25, -0.25*d)  ==  (S - d) * 0.25      bit for bit,
-// whenever d == 0 or |d| >= 2^-123 (and the result does not overflow):  -0.25*d is then exact;
+// whenever d == 0 or |d| >= 2^-123, and rn(S-d) is finite:  -0.25*d is then exact;
 // for |S-d| >= 2^-124 scaling by 2^-2 commutes with the rounding of S-d (normal results); for
 // |S-d| < 2^-124 <= |d|/2 Sterbenz makes S-d exact, so both sides round the same real number once.
-// A divergence value with 0 < |d| < 2^-123 (subnormal-range far fields of a Gaussian splat do
-// produce them) can double-round differently, so the producers of `divergence` keep a coarse map —
-// one byte per 128-column x 32-row cell — of where such values occur, and a warp whose footprint
-// touches a flagged cell runs the EXACT instantiation (subtract, then multiply).  4 lane-ops per
-// update instead of 5 everywhere else.
+// Two ends of the exponent range break it.
+//   * A divergence value with 0 < |d| < 2^-123 (subnormal-range far fields of a Gaussian splat do
+//     produce them) can double-round differently, so the producers of `divergence` keep a coarse map —
+//     one byte per 128-column x 32-row cell — of where such values occur, and a warp whose footprint
+//     touches a flagged cell runs the EXACT instantiation (subtract, then multiply) from the start.
+//   * Finite S and d whose difference rounds to +-inf (|S-d| >= 2^128 - 2^103): the reference gives
+//     inf, the fma the finite S/4 - d/4.  This needs max(|S|, |d|) >= 2^127 - 2^102, which no sweep of
+//     a launch reaches while every level-0 input — PRESSURE*p as loaded, and d — is below BIG_IN = 2^122
+//     (each sweep grows |p| by at most |d|/4: after 12 sweeps |p| < 2^125, so |S| <= 2^127 - 2^103;
+//     proof in tests/test_fma_contraction_cpu.py).  A contracted stream tracks the largest level-0
+//     magnitude it loads (fmaxf: NaN drops out, it meets both tails alike; inf counts) and, if that
+//     reached BIG_IN, runs again through the EXACT instantiation, overwriting the rows it stored.
+// 4 lane-ops per update instead of 5 everywhere else, plus 8 FMNMX per row on the ALU pipe.
 //
 // Staging.  p / div rows reach a warp through a shared-memory ring filled by 2-D tensor-map TMA
 // (cp.async.bulk.tensor.2d, SASS UTMALDG): one elected lane arms an mbarrier and fetches a
@@ -153,6 +162,8 @@ constexpr float TINY_DIV = 9.4039548e-38f;           // 2^-123
 __host__ __device__ inline int tiny_map_w(int W) { return (W + TINY_CW - 1) / TINY_CW; }
 __host__ __device__ inline int tiny_map_h(int H) { return (H + TINY_CH - 1) / TINY_CH; }
 __device__ __forceinline__ bool is_tiny_div(float d) { return d != 0.0f && fabsf(d) < TINY_DIV; }
+// level-0 inputs of a contracted stream at or above this magnitude send it through the EXACT tail
+constexpr float BIG_IN = 5.3169119831396635e36f;     // 2^122
 
 // ---- TMA (2-D tensor map) + mbarrier ----------------------------------------------------------------
 // Waits are bounded: a mis-armed barrier costs an error word, never a hung kernel.
@@ -167,6 +178,9 @@ __device__ __forceinline__ void mbar_expect_tx(void* bar, unsigned bytes) {
 __device__ __forceinline__ void tma_load_2d(void* smem_dst, const void* tmap, int x, int y, void* bar) {
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
                  ::"r"(smem_u32(smem_dst)), "l"(tmap), "r"(x), "r"(y), "r"(smem_u32(bar)) : "memory");
+}
+__device__ __forceinline__ void mbar_inval(void* bar) {
+    asm volatile("mbarrier.inval.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ bool mbar_try_wait(void* bar, unsigned parity) {
     unsigned ok;
@@ -251,9 +265,10 @@ struct TBTma {           // warp-uniform TMA bookkeeping
 //     reads dr[K+ph-t], and the ring is shifted down by 3 at the end of the block (MOVs issue on
 //     the ALU pipe, beside the fp32 pipe that bounds the kernel);
 //   * EDGE instantiates the wall selects in y, REV the mirrored-lane reversal in x, EXACT the
-//     un-contracted tail; all are chosen by warp-uniform branches OUTSIDE the steady-state loop.
+//     un-contracted tail; all are chosen by warp-uniform branches OUTSIDE the steady-state loop;
+//   * a contracted block folds the magnitudes of its level-0 inputs into `big` (BIG_IN above).
 template <int K, bool SCALE, bool EDGE, bool REV, bool EXACT>
-__device__ __forceinline__ void tb_block(float4 (&w)[K][3], float4 (&dr)[TB<K>::RD], TBStream& st,
+__device__ __forceinline__ void tb_block(float4 (&w)[K][3], float4 (&dr)[TB<K>::RD], TBStream& st, float& big,
                                          const float4* __restrict__ ring, const TBTma& tm, const int W4,
                                          const int y0, const int y1, const int H,
                                          const bool rev, const bool lane_out, const float scale) {
@@ -276,6 +291,8 @@ __device__ __forceinline__ void tb_block(float4 (&w)[K][3], float4 (&dr)[TB<K>::
                     in.x = scale * in.x; in.y = scale * in.y; in.z = scale * in.z; in.w = scale * in.w;
                 }
                 if (!EXACT) {                     // d' = -0.25 * d, exact outside the flagged cells
+                    big = fmaxf(big, fmaxf(fmaxf(fmaxf(fabsf(in.x), fabsf(in.y)), fmaxf(fabsf(in.z), fabsf(in.w))),
+                                           fmaxf(fmaxf(fabsf(dv.x), fabsf(dv.y)), fmaxf(fabsf(dv.z), fabsf(dv.w)))));
                     dv.x = __fmul_rn(dv.x, -0.25f); dv.y = __fmul_rn(dv.y, -0.25f);
                     dv.z = __fmul_rn(dv.z, -0.25f); dv.w = __fmul_rn(dv.w, -0.25f);
                 }
@@ -319,8 +336,9 @@ __device__ __forceinline__ void tb_block(float4 (&w)[K][3], float4 (&dr)[TB<K>::
     if (st.stg + 1 == T::NS) { st.stg = 0; st.phase ^= 1u; } else { ++st.stg; }
 }
 
+// returns this lane's largest level-0 magnitude (0 for an EXACT stream)
 template <int K, bool SCALE, bool REV, bool EXACT>
-__device__ __forceinline__ void tb_stream(const JacobiArgs& a, const void* tm_p, const void* tm_d,
+__device__ __forceinline__ float tb_stream(const JacobiArgs& a, const void* tm_p, const void* tm_d,
                                           float4* __restrict__ smem4, const int lane, const int x0,
                                           const int lc, const int gx, const bool rev,
                                           const bool lane_out, const int y0, const int y1,
@@ -380,14 +398,15 @@ __device__ __forceinline__ void tb_stream(const JacobiArgs& a, const void* tm_p,
     // blocks run in SEPARATE loops (not one loop with a branch) so that the steady-state loop
     // has its own register assignment and its window rotation closes without moves.
     int s0 = 0;
+    float big = 0.0f;
 #pragma unroll 1
     for (int part = 0; part < 2; ++part) {
 #pragma unroll 1
         for (; s0 < nsteps && ((ys + s0 - K <= 0) || (ys + s0 + 2 >= H - 1)); s0 += 3)
-            tb_block<K, SCALE, true, REV, EXACT>(w, dr, st, ring, tm, W4, y0, y1, H, rev, lane_out, a.scale);
+            tb_block<K, SCALE, true, REV, EXACT>(w, dr, st, big, ring, tm, W4, y0, y1, H, rev, lane_out, a.scale);
 #pragma unroll 1
         for (; s0 < nsteps && !((ys + s0 - K <= 0) || (ys + s0 + 2 >= H - 1)); s0 += 3)
-            tb_block<K, SCALE, false, REV, EXACT>(w, dr, st, ring, tm, W4, y0, y1, H, rev, lane_out, a.scale);
+            tb_block<K, SCALE, false, REV, EXACT>(w, dr, st, big, ring, tm, W4, y0, y1, H, rev, lane_out, a.scale);
     }
     // drain the over-fetched tail before the CTA (and its shared memory) goes away
 #pragma unroll 1
@@ -395,6 +414,7 @@ __device__ __forceinline__ void tb_stream(const JacobiArgs& a, const void* tm_p,
         mbar_wait(tm.bars + st.stg, st.phase, tm.err);
         if (st.stg + 1 == T::NS) { st.stg = 0; st.phase ^= 1u; } else { ++st.stg; }
     }
+    return big;
 }
 
 template <int K, bool SCALE>
@@ -402,6 +422,7 @@ __device__ __noinline__ void tb_stream_exact(const JacobiArgs& a, const void* tm
                                              float4* __restrict__ smem4, const int lane, const int x0,
                                              const int lc, const int gx, const bool rev, const bool lane_out,
                                              const int y0, const int y1, const int ys, const bool any_rev) {
+    if (lane == 0 && a.exact_streams) atomicAdd(a.exact_streams, 1ull);
     if (any_rev) tb_stream<K, SCALE, true, true>(a, tm_p, tm_d, smem4, lane, x0, lc, gx, rev, lane_out, y0, y1, ys);
     else tb_stream<K, SCALE, false, true>(a, tm_p, tm_d, smem4, lane, x0, lc, gx, rev, lane_out, y0, y1, ys);
 }
@@ -473,10 +494,19 @@ __global__ void FLUID_TB_BOUNDS jacobi_tb_kernel(JacobiArgs a, const __grid_cons
     // an SM whose resident warps ran two separate steady-state loops would keep two loop bodies in its
     // instruction cache, and a loop body twice as large measured 11 % slower (DESIGN §5.8).
     if (!exact) {
-        tb_stream<K, SCALE, true, false>(a, tp, td, smem4, lane, x0, lc, gx, rev, lane_out, y0, y1, ys);
-    } else {
-        tb_stream_exact<K, SCALE>(a, tp, td, smem4, lane, x0, lc, gx, rev, lane_out, y0, y1, ys, any_rev);
+        const float big = tb_stream<K, SCALE, true, false>(a, tp, td, smem4, lane, x0, lc, gx, rev, lane_out, y0, y1, ys);
+        // an input that could make S - d overflow within this launch: solve the stream again with the exact
+        // tail.  It stores the same rows, nobody else reads pout before the grid ends (pin != pout), and its
+        // stages were drained, so the barriers are retired and made afresh
+        exact = __any_sync(0xffffffffu, big >= BIG_IN);
+        if (exact && lane == 0) {
+            unsigned long long* bars = reinterpret_cast<unsigned long long*>(smem4 + T::NS * T::STAGE4);
+            for (int q = 0; q < T::NS; ++q) mbar_inval(bars + q);
+        }
+        __syncwarp();
+        if (!exact) return;
     }
+    tb_stream_exact<K, SCALE>(a, tp, td, smem4, lane, x0, lc, gx, rev, lane_out, y0, y1, ys, any_rev);
 }
 
 // ---- producers of the tiny-divergence map ----------------------------------------------------------

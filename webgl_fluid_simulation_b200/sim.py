@@ -527,7 +527,9 @@ class FluidSimulation:
         """Library counters (fluid_stat): launches, jacobi_launches, halo_launches, halo_exchanges,
         graph_captures, graph_launches, halo_transport_p2p, cvd_stream_launches and
         gradient_stream_launches (how many curl-vorticity-divergence / gradientSubtract passes ran
-        the row-streaming kernel rather than the tiled one; graph replays included)."""
+        the row-streaming kernel rather than the tiled one; graph replays included), and
+        jacobi_exact_streams (warps of the blocked Jacobi kernel that ran the un-contracted tail, for
+        tiny divergence or inputs near FLT_MAX; waits for the handle's queued work)."""
         return int(self._L.fluid_stat(self._h, STAT[name]))
 
     def device_ptr(self, name) -> int:
