@@ -81,6 +81,12 @@ typedef enum fluid_param {
                                          S:986-1006): fp32 arithmetic, round-to-nearest-even on every pass
                                          write, one launch per reference blit; single GPU; the ABI still
                                          speaks fp32 (fluid_read widens, fluid_write narrows)              */
+#define FLUID_FLAG_HALF_POSTFX 0x20u /* the bloom FBO and pyramid, sunrays and sunraysTemp of fluid_render_keywords /
+                                        fluid_capture are fp16 like the reference's RGBA16F / R16F FBOs (S:1012-1043):
+                                        every blit's fp32 result is rounded to nearest even when stored, the additive
+                                        up-pass rounds fragment + widened destination once.  The sunrays mask follows
+                                        the dye's storage.  HALF_STORAGE | HALF_POSTFX is the reference's desktop frame.
+                                        Single GPU; the render() frame stays fp32, host_bloom / host_sunrays widen  */
 #define FLUID_FLAG_TILED_PASSES 0x8u /* generation-1 kernels (one thread per fragment / smem tile) for
                                         curl-vorticity-divergence and gradientSubtract instead of the
                                         row-streaming ones (comparison + fallback path)              */
@@ -251,8 +257,8 @@ int fluid_render_postfx(fluid_t* h, int width, int height, const fluid_postfx* f
  * textures only for the keywords that are on (S:1339-1346).  The background follows FLUID_BACKGROUND.
  *  - Without BLOOM and SUNRAYS this is fluid_render(…, keywords & FLUID_DISPLAY_SHADING, …): slab bands
  *    and half storage work, and fx / dither_rgb may be NULL.
- *  - With BLOOM or SUNRAYS the handle must be single-GPU with fp32 storage (FLUID_ERR_INVALID
- *    otherwise), fx is required, and dither_rgb only with BLOOM.  host_bloom / host_sunrays (as for
+ *  - With BLOOM or SUNRAYS the handle must be single-GPU, with fp32 storage or with
+ *    FLUID_FLAG_HALF_POSTFX (FLUID_ERR_INVALID otherwise), fx is required, and dither_rgb only with BLOOM.  host_bloom / host_sunrays (as for
  *    fluid_render_postfx, may be NULL) are written only when their keyword is on.
  * The bloom FBO + pyramid, the sunrays FBOs and the dithering texture live in the handle: made on first
  * use, made again only when a size changes (FLUID_ERR_NOMEM if that fails; the handle stays usable), and
@@ -280,8 +286,8 @@ int fluid_render_keywords(fluid_t* h, int width, int height, uint32_t keywords, 
  *    first.  One device-to-host copy of n_bytes, then a stream sync.
  * Refused with FLUID_ERR_INVALID, the handle staying usable: unknown keyword bits; n_bytes !=
  * 4 * width * height; width, height, canvas_w or canvas_h < 1; BLOOM without dither_rgb; fx == NULL with
- * BLOOM or SUNRAYS; slab handles; half-storage handles with BLOOM or SUNRAYS (without them half storage
- * works, as in fluid_render). */
+ * BLOOM or SUNRAYS; slab handles; half-storage handles with BLOOM or SUNRAYS unless created with
+ * FLUID_FLAG_HALF_POSTFX (without them half storage works, as in fluid_render). */
 int fluid_capture(fluid_t* h, int width, int height, int canvas_w, int canvas_h, uint32_t keywords,
                   int transparent, const fluid_postfx* fx, const float* dither_rgb, int dw, int dh,
                   float back_r, float back_g, float back_b, uint8_t* host_rgba8, size_t n_bytes);

@@ -58,6 +58,7 @@ struct fluid {
     bool pdl_chain = false;                // the next blocked Jacobi launch directly follows another one of the same solve
     bool capturing = false;                // inside the stream capture of a step graph
     bool half = false;                     // FLUID_FLAG_HALF_STORAGE: fields are fp16 (half_passes.cuh), single GPU only
+    bool half_fx = false;                  // FLUID_FLAG_HALF_POSTFX: the bloom and sunrays targets are fp16, single GPU only
     float* scratch = nullptr;              // half mode: fp32 staging of fluid_read / fluid_write / render
     size_t scratch_floats = 0;
     float* dt_dev = nullptr;               // step()'s dt lives in device memory: one graph serves every dt
@@ -119,9 +120,9 @@ struct fluid {
     // post-FX targets of render() (initBloomFramebuffers / initSunraysFramebuffers, S:1012-1043): made on
     // first use, made again only when a size changes, kept across frames like the reference's FBOs
     struct PostFxTargets {
-        float4* bloom = nullptr;     // the bloom FBO, then its `levels` pyramid levels, in one allocation
+        void* bloom = nullptr;       // the bloom FBO, then its `levels` pyramid levels, in one allocation (T4 texels)
         int bw = 0, bh = 0, levels = 0;
-        float* sun = nullptr;        // sunrays, then sunraysTemp (sw x sh each)
+        void* sun = nullptr;         // sunrays, then sunraysTemp (sw x sh T1 texels each)
         int sw = 0, sh = 0;
         float* dither = nullptr;     // dw x dh RGB dithering texture, uploaded every BLOOM frame
         int dw = 0, dh = 0;
@@ -658,6 +659,11 @@ int create_common(const fluid_config* cfg, int rank, int world, const void* uid,
     h->half = (cfg->flags & FLUID_FLAG_HALF_STORAGE) != 0;
     if (h->half && world > 1) {
         int rc = fail(nullptr, FLUID_ERR_INVALID, "FLUID_FLAG_HALF_STORAGE is a single-GPU mode");
+        delete h; return rc;
+    }
+    h->half_fx = (cfg->flags & FLUID_FLAG_HALF_POSTFX) != 0;
+    if (h->half_fx && world > 1) {
+        int rc = fail(nullptr, FLUID_ERR_INVALID, "FLUID_FLAG_HALF_POSTFX is a single-GPU mode");
         delete h; return rc;
     }
     if (!slab_geometry(h, cfg->sim_h, cfg->dye_h, cfg->pressure_iterations)) {
@@ -1576,6 +1582,11 @@ static int remake_target(fluid_t* h, void** p, size_t bytes, const char* what) {
     return FLUID_OK;
 }
 
+// bytes per texel of the RGBA bloom targets and of the one-channel sunrays targets (fp16 with
+// FLUID_FLAG_HALF_POSTFX, like the reference's RGBA16F / R16F FBOs)
+inline size_t fx4bytes(const fluid_t* h) { return h->half_fx ? 8 : 16; }
+inline size_t fx1bytes(const fluid_t* h) { return h->half_fx ? 2 : 4; }
+
 // The bloom FBO and its pyramid (initBloomFramebuffers S:1012-1032), cleared like createFBO (S:1059).
 // A pyramid shorter than 2 levels leaves the FBO as cleared (applyBloom returns early, S:1351-1352).
 static int need_bloom_targets(fluid_t* h, int bw, int bh, int levels) {
@@ -1584,21 +1595,24 @@ static int need_bloom_targets(fluid_t* h, int bw, int bh, int levels) {
     size_t n = (size_t)bw * bh;
     for (int i = 0; i < levels; ++i) n += (size_t)(bw >> (i + 1)) * (bh >> (i + 1));
     t.bw = t.bh = t.levels = 0;
-    if (int rc = remake_target(h, (void**)&t.bloom, n * sizeof(float4), "the bloom FBO and pyramid")) return rc;
+    if (int rc = remake_target(h, &t.bloom, n * fx4bytes(h), "the bloom FBO and pyramid")) return rc;
     t.bw = bw; t.bh = bh; t.levels = levels;
-    fill_alpha_kernel<<<(unsigned)((n + 255) / 256), 256, 0, h->stream>>>(t.bloom, n);
+    const unsigned blocks = (unsigned)((n + 255) / 256);
+    if (h->half_fx) fill_alpha_kernel<hs::StoreHalf><<<blocks, 256, 0, h->stream>>>((hs::h4*)t.bloom, n);   // (0,0,0,1) is exact in fp16
+    else fill_alpha_kernel<<<blocks, 256, 0, h->stream>>>((float4*)t.bloom, n);
     return check_launch(h, "fill_alpha_kernel");
 }
 
-// sunrays + sunraysTemp (initSunraysFramebuffers S:1034-1043): one-channel FBOs, cleared to 0
+// sunrays + sunraysTemp (initSunraysFramebuffers S:1034-1043): one-channel FBOs, cleared to 0 (all-zero
+// bits in fp32 and fp16 alike)
 static int need_sunrays_targets(fluid_t* h, int sw, int sh) {
     auto& t = h->pfx;
     if (t.sun && t.sw == sw && t.sh == sh) return FLUID_OK;
-    const size_t n = 2 * (size_t)sw * sh;
+    const size_t bytes = 2 * (size_t)sw * sh * fx1bytes(h);
     t.sw = t.sh = 0;
-    if (int rc = remake_target(h, (void**)&t.sun, n * sizeof(float), "the sunrays FBOs")) return rc;
+    if (int rc = remake_target(h, &t.sun, bytes, "the sunrays FBOs")) return rc;
     t.sw = sw; t.sh = sh;
-    CU(cudaMemsetAsync(t.sun, 0, n * sizeof(float), h->stream));
+    CU(cudaMemsetAsync(t.sun, 0, bytes, h->stream));
     return FLUID_OK;
 }
 
@@ -1617,10 +1631,15 @@ struct PostFXOut { int bw, bh, sw, sh; };
 // The post-FX chains of render() for the keywords that are on: applyBloom (S:1350-1394) with BLOOM,
 // applySunrays + blur(…, 1) (S:1396-1419; the mask is drawn into dye.write exactly like S:1300) with
 // SUNRAYS.  FBO sizes follow initBloomFramebuffers / initSunraysFramebuffers (S:1012-1043), which size
-// them from the drawing buffer: canvas_w x canvas_h.  Single GPU, fp32 storage, arguments checked by
-// the caller.
+// them from the drawing buffer: canvas_w x canvas_h.  Sd: the dye's storage policy (the mask is drawn in
+// it), St: the targets' (postfx.cuh).  Single GPU, arguments checked by the caller.
+extern "C++" {
+template <class Sd, class St>
 static int post_fx_chains(fluid_t* h, uint32_t keywords, const fluid_postfx* fx, const float* dither_rgb,
                           int dw, int dh, int canvas_w, int canvas_h, PostFXOut* o) {
+    using D4 = typename Sd::T4;
+    using T4 = typename St::T4;
+    using T1 = typename St::T1;
     const bool bloom_on = keywords & FLUID_DISPLAY_BLOOM, sun_on = keywords & FLUID_DISPLAY_SUNRAYS;
     int bw = 1, bh = 1, sw = 1, sh = 1, levels = 0;
     if (bloom_on) fluid_get_resolution(fx->bloom_resolution, canvas_w, canvas_h, &bw, &bh);
@@ -1636,60 +1655,87 @@ static int post_fx_chains(fluid_t* h, uint32_t keywords, const fluid_postfx* fx,
     if (sun_on && (rc = need_sunrays_targets(h, sw, sh))) return rc;
     *o = {bw, bh, sw, sh};
     const int Wd = h->cfg.dye_w, Hd = h->cfg.dye_h;
-    float4* bloom = h->pfx.bloom;
-    float *sun = h->pfx.sun, *sun2 = sun ? sun + (size_t)sw * sh : nullptr;
+    T4* bloom = static_cast<T4*>(h->pfx.bloom);
+    T1 *sun = static_cast<T1*>(h->pfx.sun), *sun2 = sun ? sun + (size_t)sw * sh : nullptr;
     dim3 b(32, 8);
     int nk = 0;
     // ---- applyBloom(dye.read, bloom) ----------------------------------------------------------------
     if (bloom_on && levels >= 2) {
-        struct Lv { float4* p; int w, h; };
+        struct Lv { T4* p; int w, h; };
         std::vector<Lv> pyr;
-        float4* p = bloom + (size_t)bw * bh;
+        T4* p = bloom + (size_t)bw * bh;
         for (int i = 0; i < levels; ++i) {
             const int pw = bw >> (i + 1), ph = bh >> (i + 1);
             pyr.push_back({p, pw, ph});
             p += (size_t)pw * ph;
         }
         const double knee = fx->bloom_threshold * fx->bloom_soft_knee + 0.0001;
-        bloom_prefilter_kernel<<<grid2d(bw, bh, b), b, 0, h->stream>>>(
-            (const float4*)h->dye.read, Wd, Hd, bloom, bw, bh, (float)(fx->bloom_threshold - knee),
+        bloom_prefilter_kernel<Sd, St><<<grid2d(bw, bh, b), b, 0, h->stream>>>(
+            (const D4*)h->dye.read, Wd, Hd, bloom, bw, bh, (float)(fx->bloom_threshold - knee),
             (float)(knee * 2), (float)(0.25 / knee), (float)fx->bloom_threshold);
         ++nk;
         Lv last{bloom, bw, bh};
         for (auto& d : pyr) {
-            box4_kernel<<<grid2d(d.w, d.h, b), b, 0, h->stream>>>(last.p, last.w, last.h, d.p, d.w, d.h, 1.0f, 0);
+            box4_kernel<St><<<grid2d(d.w, d.h, b), b, 0, h->stream>>>(last.p, last.w, last.h, d.p, d.w, d.h, 1.0f, 0);
             last = d; ++nk;
         }
         for (int i = (int)pyr.size() - 2; i >= 0; --i) {
-            box4_kernel<<<grid2d(pyr[i].w, pyr[i].h, b), b, 0, h->stream>>>(last.p, last.w, last.h, pyr[i].p, pyr[i].w, pyr[i].h, 1.0f, 1);
+            box4_kernel<St><<<grid2d(pyr[i].w, pyr[i].h, b), b, 0, h->stream>>>(last.p, last.w, last.h, pyr[i].p, pyr[i].w, pyr[i].h, 1.0f, 1);
             last = pyr[i]; ++nk;
         }
-        box4_kernel<<<grid2d(bw, bh, b), b, 0, h->stream>>>(last.p, last.w, last.h, bloom, bw, bh, (float)fx->bloom_intensity, 0);
+        box4_kernel<St><<<grid2d(bw, bh, b), b, 0, h->stream>>>(last.p, last.w, last.h, bloom, bw, bh, (float)fx->bloom_intensity, 0);
         ++nk;
     }
     // ---- applySunrays(dye.read, dye.write, sunrays); blur(sunrays, sunraysTemp, 1) -------------------
     if (sun_on) {
-        sunrays_mask_kernel<<<grid2d(Wd, Hd, b), b, 0, h->stream>>>((const float4*)h->dye.read, (float4*)h->dye.write, Wd, Hd);
-        sunrays_kernel<<<grid2d(sw, sh, b), b, 0, h->stream>>>((const float4*)h->dye.write, Wd, Hd, sun, sw, sh, (float)fx->sunrays_weight);
-        blur3_kernel<<<grid2d(sw, sh, b), b, 0, h->stream>>>(sun, sun2, sw, sh, (float)(1.0 / (double)sw), 0.0f);
-        blur3_kernel<<<grid2d(sw, sh, b), b, 0, h->stream>>>(sun2, sun, sw, sh, 0.0f, (float)(1.0 / (double)sh));
+        sunrays_mask_kernel<Sd><<<grid2d(Wd, Hd, b), b, 0, h->stream>>>((const D4*)h->dye.read, (D4*)h->dye.write, Wd, Hd);
+        sunrays_kernel<Sd, St><<<grid2d(sw, sh, b), b, 0, h->stream>>>((const D4*)h->dye.write, Wd, Hd, sun, sw, sh, (float)fx->sunrays_weight);
+        blur3_kernel<St><<<grid2d(sw, sh, b), b, 0, h->stream>>>(sun, sun2, sw, sh, (float)(1.0 / (double)sw), 0.0f);
+        blur3_kernel<St><<<grid2d(sw, sh, b), b, 0, h->stream>>>(sun2, sun, sw, sh, 0.0f, (float)(1.0 / (double)sh));
         nk += 4;
     }
     return check_launch(h, "post-FX kernels", nk);
 }
+}  // extern "C++"
 
-// display_kernel<SHADING, BLOOM, SUNRAYS, Out>, indexed by [Out == StoreCapture][FLUID_DISPLAY_* mask]
+// display_kernel<SHADING, BLOOM, SUNRAYS, Out, Sp>, indexed by [Out == StoreCapture][Sp == hs::StoreHalf]
+// [FLUID_DISPLAY_* mask].  The sets without BLOOM and SUNRAYS read no post-FX target: one instantiation.
 using DisplayKernel = void (*)(DisplayArgs);
-static const DisplayKernel kDisplay[2][8] = {
-    {display_kernel<false, false, false, StoreFrame>, display_kernel<true, false, false, StoreFrame>,
-     display_kernel<false, true, false, StoreFrame>, display_kernel<true, true, false, StoreFrame>,
-     display_kernel<false, false, true, StoreFrame>, display_kernel<true, false, true, StoreFrame>,
-     display_kernel<false, true, true, StoreFrame>, display_kernel<true, true, true, StoreFrame>},
-    {display_kernel<false, false, false, StoreCapture>, display_kernel<true, false, false, StoreCapture>,
-     display_kernel<false, true, false, StoreCapture>, display_kernel<true, true, false, StoreCapture>,
-     display_kernel<false, false, true, StoreCapture>, display_kernel<true, false, true, StoreCapture>,
-     display_kernel<false, true, true, StoreCapture>, display_kernel<true, true, true, StoreCapture>},
+using F32 = StoreF32;
+using F16 = hs::StoreHalf;
+static const DisplayKernel kDisplay[2][2][8] = {
+    {{display_kernel<false, false, false, StoreFrame, F32>, display_kernel<true, false, false, StoreFrame, F32>,
+      display_kernel<false, true, false, StoreFrame, F32>, display_kernel<true, true, false, StoreFrame, F32>,
+      display_kernel<false, false, true, StoreFrame, F32>, display_kernel<true, false, true, StoreFrame, F32>,
+      display_kernel<false, true, true, StoreFrame, F32>, display_kernel<true, true, true, StoreFrame, F32>},
+     {display_kernel<false, false, false, StoreFrame, F32>, display_kernel<true, false, false, StoreFrame, F32>,
+      display_kernel<false, true, false, StoreFrame, F16>, display_kernel<true, true, false, StoreFrame, F16>,
+      display_kernel<false, false, true, StoreFrame, F16>, display_kernel<true, false, true, StoreFrame, F16>,
+      display_kernel<false, true, true, StoreFrame, F16>, display_kernel<true, true, true, StoreFrame, F16>}},
+    {{display_kernel<false, false, false, StoreCapture, F32>, display_kernel<true, false, false, StoreCapture, F32>,
+      display_kernel<false, true, false, StoreCapture, F32>, display_kernel<true, true, false, StoreCapture, F32>,
+      display_kernel<false, false, true, StoreCapture, F32>, display_kernel<true, false, true, StoreCapture, F32>,
+      display_kernel<false, true, true, StoreCapture, F32>, display_kernel<true, true, true, StoreCapture, F32>},
+     {display_kernel<false, false, false, StoreCapture, F32>, display_kernel<true, false, false, StoreCapture, F32>,
+      display_kernel<false, true, false, StoreCapture, F16>, display_kernel<true, true, false, StoreCapture, F16>,
+      display_kernel<false, false, true, StoreCapture, F16>, display_kernel<true, false, true, StoreCapture, F16>,
+      display_kernel<false, true, true, StoreCapture, F16>, display_kernel<true, true, true, StoreCapture, F16>}},
 };
+
+// Queues the copy of n values of a post-FX target into the caller's fp32 array.  An fp16 target goes
+// into `stage` instead, which widen_staged() widens exactly once the stream has synchronised: no launch.
+static int read_target(fluid_t* h, float* host, const void* dev, size_t n, std::vector<__half>& stage) {
+    if (!h->half_fx) {
+        CU(cudaMemcpyAsync(host, dev, n * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+        return FLUID_OK;
+    }
+    stage.resize(n);
+    CU(cudaMemcpyAsync(stage.data(), dev, n * sizeof(__half), cudaMemcpyDeviceToHost, h->stream));
+    return FLUID_OK;
+}
+static void widen_staged(float* host, const std::vector<__half>& stage) {
+    for (size_t k = 0; k < stage.size(); ++k) host[k] = __half2float(stage[k]);
+}
 
 // One frame of render() or captureScreenshot(), as the entry points below ask for it.
 struct DrawRequest {
@@ -1709,7 +1755,8 @@ struct DrawRequest {
 // render(target) of S:1296-1317: the post-FX chains of the keywords that are on, then the background and
 // drawDisplay in one display_kernel launch, read back to the host.  Only the fp32 frame without BLOOM and
 // SUNRAYS is drawn on a slab handle, and there only the handle's band of the target (fluid_render_band).
-// Half storage draws from a widened copy of dye and has no post-FX.
+// Half storage draws from a widened copy of dye; its post-FX needs FLUID_FLAG_HALF_POSTFX, and then the
+// chains read the fp16 dye directly and draw the mask into the fp16 dye.write.
 static int draw(fluid_t* h, const DrawRequest& r) {
     if (!h) return FLUID_ERR_INVALID;
     if (r.keywords & ~(uint32_t)(FLUID_DISPLAY_SHADING | FLUID_DISPLAY_BLOOM | FLUID_DISPLAY_SUNRAYS))
@@ -1727,9 +1774,9 @@ static int draw(fluid_t* h, const DrawRequest& r) {
                     4 * cells, r.capture ? "bytes" : "floats", r.n);
     if (cells == 0) return FLUID_OK;
     if (h->slab() && !band) return not_on_slab(h, r.what);
-    if (h->half && postfx)
+    if (h->half && !h->half_fx && postfx)
         return fail(h, FLUID_ERR_INVALID, "%s with BLOOM or SUNRAYS is not built for FLUID_FLAG_HALF_STORAGE "
-                    "(the reference's bloom / sunrays FBOs are fp16 too)", r.what);
+                    "(the reference's bloom / sunrays FBOs are fp16 too: add FLUID_FLAG_HALF_POSTFX)", r.what);
     int rc = need_frame(h, r.capture ? (cells + 3) / 4 : cells); if (rc) return rc;   // the capture's uchar4 image lives in the frame
     if (h->slab()) {
         // the band's display + shading taps reach ceil(Hd / height) + 2 dye rows beyond the owned ones:
@@ -1742,7 +1789,12 @@ static int draw(fluid_t* h, const DrawRequest& r) {
             return fail(h, FLUID_ERR_HALO, "render target of %d rows needs %d dye ghost rows, the slab keeps %d", r.height, need, h->Gd);
     }
     PostFXOut o{};
-    if (postfx && (rc = post_fx_chains(h, r.keywords, r.fx, r.dither, r.dw, r.dh, r.canvas_w, r.canvas_h, &o))) return rc;
+    if (postfx) {
+        const auto chains = !h->half_fx ? post_fx_chains<StoreF32, StoreF32>
+                          : !h->half    ? post_fx_chains<StoreF32, hs::StoreHalf>
+                                        : post_fx_chains<hs::StoreHalf, hs::StoreHalf>;
+        if ((rc = chains(h, r.keywords, r.fx, r.dither, r.dw, r.dh, r.canvas_w, r.canvas_h, &o))) return rc;
+    }
     const float4* dye_src;
     if ((rc = display_source(h, &dye_src))) return rc;
     // texelSize = 1 / width, 1 / height (S:1337) and getTextureScale (S:1626-1631) are JS doubles, narrowed here
@@ -1753,12 +1805,15 @@ static int draw(fluid_t* h, const DrawRequest& r) {
                         sun_on ? h->pfx.sun : nullptr, o.sw, o.sh, bloom_on ? h->pfx.dither : nullptr, r.dw, r.dh,
                         h->frame, r.width, r.height, y0, y1, r.back[0], r.back[1], r.back[2], r.bg_mode, h->cfg.aspect, ts};
     dim3 b(32, 8);
-    kDisplay[r.capture][r.keywords]<<<grid2d(r.width, y1 - y0, b), b, 0, h->stream>>>(a);
+    kDisplay[r.capture][h->half_fx][r.keywords]<<<grid2d(r.width, y1 - y0, b), b, 0, h->stream>>>(a);
     if ((rc = check_launch(h, "display_kernel"))) return rc;
     CU(cudaMemcpyAsync(r.host, h->frame, r.n * (r.capture ? 1 : sizeof(float)), cudaMemcpyDeviceToHost, h->stream));
-    if (bloom_on && r.host_bloom) CU(cudaMemcpyAsync(r.host_bloom, h->pfx.bloom, (size_t)o.bw * o.bh * sizeof(float4), cudaMemcpyDeviceToHost, h->stream));
-    if (sun_on && r.host_sunrays) CU(cudaMemcpyAsync(r.host_sunrays, h->pfx.sun, (size_t)o.sw * o.sh * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+    std::vector<__half> bloom16, sun16;
+    if (bloom_on && r.host_bloom && (rc = read_target(h, r.host_bloom, h->pfx.bloom, (size_t)o.bw * o.bh * 4, bloom16))) return rc;
+    if (sun_on && r.host_sunrays && (rc = read_target(h, r.host_sunrays, h->pfx.sun, (size_t)o.sw * o.sh, sun16))) return rc;
     CU(cudaStreamSynchronize(h->stream));
+    widen_staged(r.host_bloom, bloom16);
+    widen_staged(r.host_sunrays, sun16);
     return FLUID_OK;
 }
 

@@ -12,6 +12,7 @@
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
+#include "half_passes.cuh"
 #include "passes.cuh"
 
 namespace fk {
@@ -31,55 +32,66 @@ __device__ __forceinline__ float linear_fetch_rgb_r_repeat(const float* __restri
             w01 * __ldg(&tex[((size_t)j1 * W + i0) * 3])) + w11 * __ldg(&tex[((size_t)j1 * W + i1) * 3]);
 }
 
+// The chain kernels are templates on storage policies (passes.cuh StoreF32, half_passes.cuh
+// hs::StoreHalf): Sd is the dye's, which the sunrays mask shares because it is drawn into dye.write;
+// St is the bloom FBO's, the pyramid's and the sunrays FBOs' (FLUID_FLAG_HALF_POSTFX: fp16, every
+// blit's fp32 result rounded to nearest even when it is stored, like the reference's RGBA16F / R16F
+// targets).  Fetches widen the stored texels exactly and run the same fp32 LINEAR arithmetic.
+
 // bloomPrefilterShader S:614-631
-__global__ void __launch_bounds__(256) bloom_prefilter_kernel(const float4* __restrict__ dye, int Wd, int Hd,
-                                                              float4* __restrict__ out, int w, int h, float curve0,
+template <class Sd, class St>
+__global__ void __launch_bounds__(256) bloom_prefilter_kernel(const typename Sd::T4* __restrict__ dye, int Wd, int Hd,
+                                                              typename St::T4* __restrict__ out, int w, int h, float curve0,
                                                               float curve1, float curve2, float threshold) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y * blockDim.y + threadIdx.y;
     if (i >= w || j >= h) return;
     const float uvx = ((float)i + 0.5f) / (float)w, uvy = ((float)j + 0.5f) / (float)h;
-    const float4 c = linear_fetch(dye, Wd, Hd, uvx, uvy);
+    const float4 c = linear_fetch<Sd>(dye, Wd, Hd, uvx, uvy);
     const float br = fmaxf(c.x, fmaxf(c.y, c.z));
     float rq = fminf(fmaxf(br - curve0, 0.0f), curve1);
     rq = (curve2 * rq) * rq;
     const float f = fmaxf(rq, br - threshold) / fmaxf(br, 0.0001f);
-    out[(size_t)j * w + i] = make_float4(c.x * f, c.y * f, c.z * f, 0.0f);
+    St::st(out, (size_t)j * w + i, make_float4(c.x * f, c.y * f, c.z * f, 0.0f));
 }
 
-// bloomBlurShader S:633-651 / bloomFinalShader S:653-674; add = blendFunc(ONE, ONE) (S:1374-1375)
-__global__ void __launch_bounds__(256) box4_kernel(const float4* __restrict__ src, int ws, int hs,
-                                                   float4* __restrict__ dst, int w, int h, float scale, int add) {
+// bloomBlurShader S:633-651 / bloomFinalShader S:653-674; add = blendFunc(ONE, ONE) (S:1374-1375): the
+// fragment plus the widened destination texel, rounded once by the store
+template <class St>
+__global__ void __launch_bounds__(256) box4_kernel(const typename St::T4* __restrict__ src, int ws, int hs,
+                                                   typename St::T4* __restrict__ dst, int w, int h, float scale, int add) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y * blockDim.y + threadIdx.y;
     if (i >= w || j >= h) return;
     const float tsx = (float)(1.0 / (double)ws), tsy = (float)(1.0 / (double)hs);
     const float uvx = ((float)i + 0.5f) / (float)w, uvy = ((float)j + 0.5f) / (float)h;
-    const float4 L = linear_fetch(src, ws, hs, uvx - tsx, uvy), R = linear_fetch(src, ws, hs, uvx + tsx, uvy);
-    const float4 T = linear_fetch(src, ws, hs, uvx, uvy + tsy), B = linear_fetch(src, ws, hs, uvx, uvy - tsy);
+    const float4 L = linear_fetch<St>(src, ws, hs, uvx - tsx, uvy), R = linear_fetch<St>(src, ws, hs, uvx + tsx, uvy);
+    const float4 T = linear_fetch<St>(src, ws, hs, uvx, uvy + tsy), B = linear_fetch<St>(src, ws, hs, uvx, uvy - tsy);
     float4 s;
     s.x = ((((0.0f + L.x) + R.x) + T.x) + B.x) * 0.25f * scale;
     s.y = ((((0.0f + L.y) + R.y) + T.y) + B.y) * 0.25f * scale;
     s.z = ((((0.0f + L.z) + R.z) + T.z) + B.z) * 0.25f * scale;
     s.w = ((((0.0f + L.w) + R.w) + T.w) + B.w) * 0.25f * scale;
-    float4* o = dst + (size_t)j * w + i;
-    if (add) { const float4 d = *o; s.x = s.x + d.x; s.y = s.y + d.y; s.z = s.z + d.z; s.w = s.w + d.w; }
-    *o = s;
+    const size_t o = (size_t)j * w + i;
+    if (add) { const float4 d = St::ld(dst, o); s.x = s.x + d.x; s.y = s.y + d.y; s.z = s.z + d.z; s.w = s.w + d.w; }
+    St::st(dst, o, s);
 }
 
-// sunraysMaskShader S:676-691 (target = dye.write, like the reference: S:1300)
-__global__ void __launch_bounds__(256) sunrays_mask_kernel(const float4* __restrict__ dye, float4* __restrict__ mask,
-                                                           int Wd, int Hd) {
+// sunraysMaskShader S:676-691 (target = dye.write, like the reference: S:1300, so stored as the dye is)
+template <class Sd>
+__global__ void __launch_bounds__(256) sunrays_mask_kernel(const typename Sd::T4* __restrict__ dye,
+                                                           typename Sd::T4* __restrict__ mask, int Wd, int Hd) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y * blockDim.y + threadIdx.y;
     if (i >= Wd || j >= Hd) return;
     const float uvx = ((float)i + 0.5f) / (float)Wd, uvy = ((float)j + 0.5f) / (float)Hd;
-    float4 c = linear_fetch(dye, Wd, Hd, uvx, uvy);
+    float4 c = linear_fetch<Sd>(dye, Wd, Hd, uvx, uvy);
     const float br = fmaxf(c.x, fmaxf(c.y, c.z));
     c.w = 1.0f - fminf(fmaxf(br * 20.0f, 0.0f), 0.8f);
-    mask[(size_t)j * Wd + i] = c;
+    Sd::st(mask, (size_t)j * Wd + i, c);
 }
 
 // sunraysShader S:693-724
-__global__ void __launch_bounds__(256) sunrays_kernel(const float4* __restrict__ mask, int Wm, int Hm,
-                                                      float* __restrict__ out, int w, int h, float weight) {
+template <class Sd, class St>
+__global__ void __launch_bounds__(256) sunrays_kernel(const typename Sd::T4* __restrict__ mask, int Wm, int Hm,
+                                                      typename St::T1* __restrict__ out, int w, int h, float weight) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y * blockDim.y + threadIdx.y;
     if (i >= w || j >= h) return;
     const float Density = 0.3f, Decay = 0.95f, Exposure = 0.7f;
@@ -89,31 +101,32 @@ __global__ void __launch_bounds__(256) sunrays_kernel(const float4* __restrict__
     float dx = uvx - 0.5f, dy = uvy - 0.5f;
     dx = dx * f; dy = dy * f;
     float illum = 1.0f;
-    float color = linear_fetch(mask, Wm, Hm, uvx, uvy).w;
+    float color = linear_fetch<Sd>(mask, Wm, Hm, uvx, uvy).w;
 #pragma unroll 1
     for (int k = 0; k < 16; ++k) {
         cx = cx - dx; cy = cy - dy;
-        const float col = linear_fetch(mask, Wm, Hm, cx, cy).w;
+        const float col = linear_fetch<Sd>(mask, Wm, Hm, cx, cy).w;
         color = color + (col * illum) * weight;
         illum = illum * Decay;
     }
-    out[(size_t)j * w + i] = color * Exposure;
+    St::st(out, (size_t)j * w + i, color * Exposure);
 }
 
 // blurShader S:478-494 + blurVertexShader S:461-476 on the one-channel sunrays texture
-__global__ void __launch_bounds__(256) blur3_kernel(const float* __restrict__ src, float* __restrict__ dst, int w, int h,
-                                                    float tsx, float tsy) {
+template <class St>
+__global__ void __launch_bounds__(256) blur3_kernel(const typename St::T1* __restrict__ src, typename St::T1* __restrict__ dst,
+                                                    int w, int h, float tsx, float tsy) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y * blockDim.y + threadIdx.y;
     if (i >= w || j >= h) return;
     const float off = 1.33333333f;
     const float uvx = ((float)i + 0.5f) / (float)w, uvy = ((float)j + 0.5f) / (float)h;
-    const float c = linear_fetch(src, w, h, uvx, uvy);
-    const float l = linear_fetch(src, w, h, uvx - tsx * off, uvy - tsy * off);
-    const float r = linear_fetch(src, w, h, uvx + tsx * off, uvy + tsy * off);
+    const float c = linear_fetch<St>(src, w, h, uvx, uvy);
+    const float l = linear_fetch<St>(src, w, h, uvx - tsx * off, uvy - tsy * off);
+    const float r = linear_fetch<St>(src, w, h, uvx + tsx * off, uvy + tsy * off);
     float sum = c * 0.29411764f;
     sum = sum + l * 0.35294117f;
     sum = sum + r * 0.35294117f;
-    dst[(size_t)j * w + i] = sum;
+    St::st(dst, (size_t)j * w + i, sum);
 }
 
 __device__ __forceinline__ float len3(float4 v) { return sqrtf((v.x * v.x + v.y * v.y) + v.z * v.z); }
@@ -169,8 +182,8 @@ struct StoreCapture {
 struct DisplayArgs {
     const float4* dye;                  // fp32 dye; its first row is global row dye_row_off
     int Wd, Hd, dye_row_off;
-    const float4* bloom; int bw, bh;    // the bloom FBO (BLOOM)
-    const float* sun; int sw, sh;       // the sunrays texture (SUNRAYS)
+    const void* bloom; int bw, bh;      // the bloom FBO (BLOOM): Sp::T4 texels
+    const void* sun; int sw, sh;        // the sunrays texture (SUNRAYS): Sp::T1 texels
     const float* dither; int dw, dh;    // the RGB dithering texture (BLOOM)
     void* out;                          // Out::T texels of the rows [y0, y1) of the w x h target
     int w, h, y0, y1;
@@ -181,9 +194,10 @@ struct DisplayArgs {
 };
 
 // displayShaderSource S:549-612 compiled with the keywords updateKeywords picks (S:1160-1166), over
-// the background of render() (blend_over_background).  Out: the output policy.  A slab rank draws the
-// band [y0, y1) of the target from its own dye rows (+ ghost rows); one GPU draws the whole target.
-template <bool SHADING, bool BLOOM, bool SUNRAYS, class Out>
+// the background of render() (blend_over_background).  Out: the output policy; Sp: the storage policy
+// of the bloom and sunrays targets (post_fx_chains' St).  A slab rank draws the band [y0, y1) of the
+// target from its own dye rows (+ ghost rows); one GPU draws the whole target.
+template <bool SHADING, bool BLOOM, bool SUNRAYS, class Out, class Sp>
 __global__ void __launch_bounds__(256) display_kernel(DisplayArgs a) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x, j = a.y0 + blockIdx.y * blockDim.y + threadIdx.y;
     if (i >= a.w || j >= a.y1) return;
@@ -210,11 +224,11 @@ __global__ void __launch_bounds__(256) display_kernel(DisplayArgs a) {
     }
     float bl[3] = {0.0f, 0.0f, 0.0f};
     if constexpr (BLOOM) {
-        const float4 b = linear_fetch(a.bloom, a.bw, a.bh, uvx, uvy);
+        const float4 b = linear_fetch<Sp>(static_cast<const typename Sp::T4*>(a.bloom), a.bw, a.bh, uvx, uvy);
         bl[0] = b.x; bl[1] = b.y; bl[2] = b.z;
     }
     if constexpr (SUNRAYS) {
-        const float s = linear_fetch(a.sun, a.sw, a.sh, uvx, uvy);
+        const float s = linear_fetch<Sp>(static_cast<const typename Sp::T1*>(a.sun), a.sw, a.sh, uvx, uvy);
 #pragma unroll
         for (int k = 0; k < 3; ++k) {
             cc[k] = cc[k] * s;

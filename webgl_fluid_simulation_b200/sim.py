@@ -432,8 +432,11 @@ class FluidSimulation:
         drawn over the checkerboard on the screen (target=False, S:1311-1312) and bare, un-blended,
         into a capture target (target=True: what captureScreenshot renders into, S:287-299).
         config.SHADING / BLOOM / SUNRAYS pick the display keywords like updateKeywords (S:1160-1166);
-        BLOOM needs `sim.dithering`.  BLOOM or SUNRAYS need a single-GPU fp32 handle.  last_bloom /
-        last_sunrays hold the bloom FBO / sunrays texture of the frame, or None when that keyword is off."""
+        BLOOM needs `sim.dithering`.  BLOOM or SUNRAYS need a single-GPU handle, fp32 or created with
+        FLAG_HALF_POSTFX (then the bloom and sunrays targets are fp16, as are the reference's; with
+        FLAG_HALF_STORAGE | FLAG_HALF_POSTFX this is the reference's desktop frame).  last_bloom /
+        last_sunrays hold the bloom FBO / sunrays texture of the frame (widened to float32), or None when
+        that keyword is off."""
         w = int(width or self.canvas["width"]); h = int(height or self.canvas["height"])
         bc = self.config["BACK_COLOR"]                       # normalizeColor, S:1599-1606
         out = np.empty((h, w, 4), np.float32)
@@ -468,6 +471,7 @@ class FluidSimulation:
         getResolution(CAPTURE_RESOLUTION) and normalizeTexture (S:309-327), all on the GPU.  Returns the
         (h, w, 4) uint8 image, TOP row first.  The bloom and sunrays FBOs keep the canvas sizes, as in the
         reference; config.TRANSPARENT stores the display bare (no checkerboard); BLOOM needs `sim.dithering`.
+        BLOOM or SUNRAYS need the same handles as render().
         With `path`, also writes the image as a PNG (write_png: the bytes unchanged)."""
         cfg = self.config
         cw, ch = self.canvas["width"], self.canvas["height"]
