@@ -212,10 +212,10 @@ int fluid_write(fluid_t* h, int field, const float* host, size_t n_floats);
 /* End-to-end form of the pressure solve for callers that keep fields in HOST memory: uploads
  * divergence and pressure, runs clear + `iters` Jacobi sweeps, downloads pressure.  All three
  * copies are inside the call (this is what bench.py's `e2e` times).  On a single-GPU handle the grid
- * is cut into row bands that are solved and downloaded while later bands still upload (same bits as
- * the one-piece solve; FLUID_E2E_BANDS=1 disables it); pass pinned buffers (fluid_host_alloc) for the
- * copies to overlap.  The divergence and pressure fields of the handle hold the uploaded divergence
- * and the result afterwards. */
+ * is cut into up to 16 row bands that are solved and downloaded while later bands still upload (same
+ * bits as the one-piece solve, which grids too short for two bands take); pass pinned buffers
+ * (fluid_host_alloc) for the copies to overlap.  The divergence and pressure fields of the handle
+ * hold the uploaded divergence and the result afterwards. */
 int fluid_pressure_solve_host(fluid_t* h, const float* div_host, float* pressure_host_inout,
                               int iters);
 

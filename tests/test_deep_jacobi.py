@@ -8,8 +8,9 @@ import pytest
 
 from conftest import bits_equal
 from jacobi_tb_model import jacobi_tb_model
+from webgl_fluid_simulation_b200 import slab
+from webgl_fluid_simulation_b200.slab import KMAX as K_MAX
 
-K_MAX = 13                          # csrc/fluid.cu: KMAX
 TINY = 9.4039548e-38                # 2^-123: below it the contracted tail is not exact (EXACT streams)
 
 
@@ -70,3 +71,4 @@ def test_depth13_bitwise_vs_naive_and_oracle(oracle):
             assert bits_equal(got, want), (W, H, iters, jb, flags)
             if not flags:
                 assert launches == -(-iters // K_MAX), (W, H, iters, jb)
+            assert launches == len(slab.jacobi_launches(iters, slab.SlabPlan(H, 8, 0, 1).block(block))), (W, H, iters, flags)

@@ -6,6 +6,7 @@ import pytest
 import gamma_model as G
 import splat_model as M
 from conftest import bits_equal, golden, max_rel
+from webgl_fluid_simulation_b200 import slab
 
 pytestmark = pytest.mark.gpu
 DT = 0.016666
@@ -409,7 +410,9 @@ def test_host_pressure_solve_banded_pipeline(pkg, W, H, iters, jb, launches):
     ph = p.copy()
     n0 = s.stat("jacobi_launches")
     s.pressure_solve_host(d, ph, iters)
-    assert s.stat("jacobi_launches") - n0 == launches
+    n_host = s.stat("jacobi_launches") - n0
+    assert n_host == launches
+    assert n_host == sum(len(b["launches"]) for b in slab.host_bands(H, iters, block=jb))
     assert bits_equal(a, ph)
     assert bits_equal(s.readField("pressure"), ph)
     assert bits_equal(s.readField("divergence"), d)

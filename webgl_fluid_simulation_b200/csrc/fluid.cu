@@ -55,7 +55,6 @@ struct fluid {
     uint64_t gradient_stream_launches = 0; // which of a pass's kernels the grid size picked
     uint64_t div_epoch = 1, div_sent_epoch = 0;   // slab: the divergence ghost rows are re-sent only after divergence was rewritten
     int div_sent_rows = 0;
-    bool pdl_chain = false;                // the next blocked Jacobi launch directly follows another one of the same solve
     bool capturing = false;                // inside the stream capture of a step graph
     bool half = false;                     // FLUID_FLAG_HALF_STORAGE: fields are fp16 (half_passes.cuh), single GPU only
     bool half_fx = false;                  // FLUID_FLAG_HALF_POSTFX: the bloom and sunrays targets are fp16, single GPU only
@@ -72,8 +71,6 @@ struct fluid {
     fluid_timing timing{};
     bool have_timing = false;
     std::string err;
-    int jacobi_rows_override = 0;    // FLUID_JACOBI_ROWS env (tuning)
-    int jacobi_warps_per_sm = 0;     // FLUID_JACOBI_WARPS env (tuning): cap on resident streams per SM used to size the chunks
 
     // ---- row-slab decomposition (SURVEY §8e).  Single GPU: rank 0 of 1, no ghost rows. -------------
     int rank = 0, world = 1;
@@ -245,13 +242,45 @@ int scan_tiny(fluid_t* h, int j_lo, int j_hi) {
 // ---- Jacobi dispatch -----------------------------------------------------------------------------
 
 // Temporal-block depths, at most KMAX (slab.py mirrors both): the depth-13 instantiation fits 255
-// registers without spills.  A single-GPU in-place solve defaults to KMAX (measurements at run_jacobi);
-// row slabs and the banded host solve default to K_DEFAULT, the depth they have been run at.
+// registers without spills.  A single-GPU in-place solve defaults to KMAX: on an H100 at 4096^2 x 50 4
+// launches of 13 / 12 sweeps take 0.500 ms per solve and 5 launches of 10 take 0.524 (80 GB HBM3 card, 400 W
+// power limit; DESIGN §5).  Iteration counts that split into the same number of launches either way (20, 30,
+// 40) keep depth 10 launches.  Row slabs and the banded host solve default to K_DEFAULT, the depth they have
+// been run at.
 constexpr int KMAX = 13;
 constexpr int K_DEFAULT = 10;
 
 bool tb_eligible(const fluid_t* h) {
     return !h->half && (h->cfg.sim_w % 4 == 0) && h->cfg.sim_w >= 16 && h->cfg.sim_h >= 2;
+}
+
+// depth of a solve (slab.py SlabPlan.block, host_bands): config.JACOBI_BLOCK or the default, and on a slab
+// below its ghost rows.  banded: the bands of fluid_pressure_solve_host.
+int block_depth(const fluid_t* h, bool banded) {
+    const int kb = std::min(h->cfg.jacobi_block > 0 ? h->cfg.jacobi_block : (h->slab() || banded ? K_DEFAULT : KMAX), KMAX);
+    return h->slab() ? std::max(1, std::min(kb, h->G - 1)) : kb;
+}
+
+// a solve of depth kb runs the blocked kernel; otherwise one sweep per launch
+bool blocked(const fluid_t* h, int kb) {
+    return tb_eligible(h) && !(h->cfg.flags & FLUID_FLAG_NAIVE_JACOBI) && kb != 1;
+}
+
+// Balanced split of iters > 0 sweeps into ceil(iters/kb) launches (slab.py jacobi_launches): launch k
+// runs depth(k) sweeps, and after(k) sweeps of the solve follow it.
+struct JacobiPlan {
+    int n, base, extra;
+    JacobiPlan(int iters, int kb) : n((iters + kb - 1) / kb), base(iters / n), extra(iters % n) {}
+    int depth(int k) const { return base + (k < extra ? 1 : 0); }
+    int after(int k) const { return (n - 1 - k) * base + std::max(extra - 1 - k, 0); }
+};
+
+// JacobiArgs of a launch whose local row 0 is global row row_off; the caller sets pin, pout and the rows
+JacobiArgs jacobi_args(const fluid_t* h, const float* div, int row_off) {
+    JacobiArgs a{};
+    a.div = div; a.row_off = row_off; a.W = h->cfg.sim_w; a.H = h->cfg.sim_h; a.scale = h->cfg.pressure;
+    a.err = h->halo_flag; a.tiny_map = h->tiny_map; a.exact_streams = h->exact_streams;
+    return a;
 }
 
 // cuTensorMapEncodeTiled through the runtime (no link-time dependency on libcuda)
@@ -301,61 +330,81 @@ int build_tmaps(fluid_t* h) {
     return FLUID_OK;
 }
 
-// `maps` describe a.pin and a.div from their local row 0
-template <int K, bool SCALE>
-int launch_tb(fluid_t* h, const JacobiArgs& a, const TmapPair& maps) {
-    using T = TB<K>;
-    const int nxw = (a.W + T::VALID - 1) / T::VALID;
-    const int nch = (a.out_hi - a.out_lo + a.rows_per_chunk - 1) / a.rows_per_chunk;
-    // chained to the previous launch of the same solve by programmatic dependent launch (jacobi.cuh);
-    // not while a graph is being captured
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cudaLaunchConfig_t lc{};
-    lc.gridDim = dim3(nxw * nch); lc.blockDim = dim3(32); lc.stream = h->stream;   // one warp per CTA
-    lc.attrs = attr; lc.numAttrs = (h->pdl_chain && !h->capturing) ? 1 : 0;
-    lc.dynamicSmemBytes = T::SMEM;
-    cudaLaunchKernelEx(&lc, jacobi_tb_kernel<K, SCALE>, a, maps);
-    ++h->jacobi_kernel_launches;
-    return check_launch(h, "jacobi_tb_kernel");
-}
-
+// kTb[K - 1]: jacobi_tb_kernel<K, SCALE> as kernel[SCALE], and the TB<K> constants its launch needs
+struct TbEntry {
+    void (*kernel[2])(JacobiArgs, TmapPair);
+    int valid, u, smem;
+};
 template <int K>
-int launch_tb_k(fluid_t* h, const JacobiArgs& a, const TmapPair& maps, bool scale) {
-    return scale ? launch_tb<K, true>(h, a, maps) : launch_tb<K, false>(h, a, maps);
+constexpr TbEntry tb_entry() {
+    return {{jacobi_tb_kernel<K, false>, jacobi_tb_kernel<K, true>}, TB<K>::VALID, TB<K>::U, TB<K>::SMEM};
 }
+static const TbEntry kTb[KMAX] = {tb_entry<1>(), tb_entry<2>(), tb_entry<3>(), tb_entry<4>(), tb_entry<5>(),
+                                  tb_entry<6>(), tb_entry<7>(), tb_entry<8>(), tb_entry<9>(), tb_entry<10>(),
+                                  tb_entry<11>(), tb_entry<12>(), tb_entry<13>()};
 
-// rows per warp stream: enough chunks that every SM holds its full complement of resident warps
-// (single wave), rounded so that a stream's step count R + 2K is a multiple of the unroll U.
-template <int K>
-int tb_rows(const fluid_t* h, int W, int rows) {
-    if (h->jacobi_rows_override > 0) return h->jacobi_rows_override;
-    using T = TB<K>;
-    const int nxw = (W + T::VALID - 1) / T::VALID;
+// rows per warp stream of a depth-K launch: enough chunks that every SM holds its full complement of
+// resident warps (single wave), rounded so that a stream's step count R + 2K is a multiple of the unroll
+// U.  Both SCALE instantiations are sized from the occupancy of the SCALE = false one.
+int tb_rows(const fluid_t* h, const TbEntry& e, int K, int W, int rows) {
+    const int nxw = (W + e.valid - 1) / e.valid;
     int occ = 0;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, jacobi_tb_kernel<K, false>, 32, T::SMEM);
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, e.kernel[0], 32, e.smem);
     if (occ < 1) occ = 1;
-    if (h->jacobi_warps_per_sm > 0) occ = std::min(occ, h->jacobi_warps_per_sm);
     const int resident_warps = std::max(nxw, h->sm_count * occ);
     const int nch = std::max(1, resident_warps / nxw);
     int r = (rows + nch - 1) / nch;
     r = std::max(r, 4 * K);                 // keep the 2K warm-up rows a bounded fraction
     // round R up so that (R + 2K) % U == 0: no partially wasted unrolled block
-    const int rem = (r + 2 * K) % T::U;
-    if (rem) r += T::U - rem;
+    const int rem = (r + 2 * K) % e.u;
+    if (rem) r += e.u - rem;
     return std::min(r, rows);
 }
 
-int launch_tb_dyn(fluid_t* h, int K, JacobiArgs a, const TmapPair& maps, bool scale) {
-    const int rows = a.out_hi - a.out_lo;
-    switch (K) {
-#define CASE(KK) case KK: a.rows_per_chunk = tb_rows<KK>(h, a.W, rows); return launch_tb_k<KK>(h, a, maps, scale);
-        CASE(1) CASE(2) CASE(3) CASE(4) CASE(5) CASE(6) CASE(7) CASE(8) CASE(9) CASE(10) CASE(11) CASE(12)
-        CASE(13)
-#undef CASE
+// One blocked launch of depth K, global rows [a.out_lo, a.out_hi); `maps` describe a.pin and a.div from their
+// local row 0.  scale: the clear pass fused into the loads.  chained: programmatic dependent launch behind the
+// previous kernel on the stream (jacobi.cuh), never while a graph is being captured.
+int launch_tb(fluid_t* h, int K, bool scale, bool chained, JacobiArgs a, const TmapPair& maps) {
+    if (K < 1 || K > KMAX) return fail(h, FLUID_ERR_INVALID, "temporal block depth %d out of range", K);
+    const TbEntry& e = kTb[K - 1];
+    a.rows_per_chunk = tb_rows(h, e, K, a.W, a.out_hi - a.out_lo);
+    const int nxw = (a.W + e.valid - 1) / e.valid;
+    const int nch = (a.out_hi - a.out_lo + a.rows_per_chunk - 1) / a.rows_per_chunk;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cudaLaunchConfig_t lc{};
+    lc.gridDim = dim3(nxw * nch); lc.blockDim = dim3(32); lc.stream = h->stream;   // one warp per CTA
+    lc.attrs = attr; lc.numAttrs = (chained && !h->capturing) ? 1 : 0;
+    lc.dynamicSmemBytes = e.smem;
+    cudaLaunchKernelEx(&lc, e.kernel[scale], a, maps);
+    ++h->jacobi_kernel_launches;
+    return check_launch(h, "jacobi_tb_kernel");
+}
+
+// One sweep without temporal blocking, rows [a.out_lo, a.out_hi).  scale: the clear pass fused into the
+// loads (never in half storage, which clears in a launch of its own).
+int launch_sweep(fluid_t* h, const JacobiArgs& a, bool scale) {
+    const int W = a.W, H = a.H;
+    const char* what = "jacobi_sweep_kernel";
+    if (tb_eligible(h)) {
+        dim3 b(32, 8);
+        dim3 g((W / 4 + b.x - 1) / b.x, (a.out_hi - a.out_lo + b.y - 1) / b.y);
+        if (scale) jacobi_sweep_kernel<true><<<g, b, 0, h->stream>>>(a);
+        else jacobi_sweep_kernel<false><<<g, b, 0, h->stream>>>(a);
+    } else if (h->half && W % 8 == 0 && W >= 64) {
+        dim3 b(32, 8), g((W / 8 + 31) / 32, (H + 7) / 8);
+        hs::jacobi8_kernel<<<g, b, 0, h->stream>>>((const hs::h1*)a.pin, (const hs::h1*)a.div, (hs::h1*)a.pout, W, H);
+        what = "hs::jacobi8_kernel";
+    } else {
+        dim3 b(64, 4);
+        with_storage(h, [&](auto s) {
+            jacobi_scalar_kernel<decltype(s)><<<grid2d(W, a.out_hi - a.out_lo, b), b, 0, h->stream>>>(a, scale);
+        });
+        what = "jacobi_scalar_kernel";
     }
-    return fail(h, FLUID_ERR_INVALID, "temporal block depth %d out of range", K);
+    ++h->jacobi_kernel_launches;
+    return check_launch(h, what);
 }
 
 // `iters` sweeps reading pressure.read, result in pressure.read (swaps like S:1265).
@@ -366,19 +415,6 @@ int launch_tb_dyn(fluid_t* h, int K, JacobiArgs a, const TmapPair& maps, bool sc
 int run_jacobi(fluid_t* h, int iters, bool scale_first, int* launches_out) {
     int nl = 0;
     const int W = h->cfg.sim_w, H = h->cfg.sim_h;
-    JacobiArgs a{};
-    a.div = h->divergence; a.W = W; a.H = H; a.row_off = h->roff; a.out_lo = h->row0; a.out_hi = h->row1;
-    a.scale = h->cfg.pressure;
-    a.err = h->halo_flag;
-    a.tiny_map = h->tiny_map;
-    a.exact_streams = h->exact_streams;
-    // default depth: on an H100 at 4096^2 x 50 4 launches of 13 / 12 sweeps take 0.500 ms per solve and 5
-    // launches of 10 take 0.524 (80 GB HBM3 card, 400 W power limit; DESIGN §5).  Iteration counts that
-    // split into the same number of launches either way (20, 30, 40) keep depth 10 launches.
-    int kb = h->cfg.jacobi_block > 0 ? h->cfg.jacobi_block : (h->slab() ? K_DEFAULT : KMAX);
-    kb = std::min(kb, KMAX);
-    if (h->slab()) kb = std::max(1, std::min(kb, h->G - 1));
-    const bool naive = (h->cfg.flags & FLUID_FLAG_NAIVE_JACOBI) || kb == 1;
     // clear pass alone (owned + ghost rows; ghosts are refreshed before use anyway).  Half storage always
     // clears in a launch of its own: the reference rounds the cleared field to fp16 before the first sweep.
     if (scale_first && (iters <= 0 || h->half)) {
@@ -397,9 +433,9 @@ int run_jacobi(fluid_t* h, int iters, bool scale_first, int* launches_out) {
         if (launches_out) *launches_out = nl;
         return FLUID_OK;
     }
-    const bool blocked = tb_eligible(h) && !naive;
-    const int nlaunch = blocked ? (iters + kb - 1) / kb : iters;
-    const int base = iters / nlaunch, extra = iters % nlaunch;
+    const int kb = block_depth(h, false);
+    const bool tb = blocked(h, kb);
+    const JacobiPlan plan(iters, tb ? kb : 1);
     // Slab halos.  Communication-avoiding form (deep): ONE group per solve carries iters+1 rows of
     // pressure and iters rows of divergence; launch i then produces owned rows +- (sweeps still to
     // come + 1), so later launches find their input already there (~1 % redundant rows instead of
@@ -430,63 +466,41 @@ int run_jacobi(fluid_t* h, int iters, bool scale_first, int* launches_out) {
             h->scan_pending = false;
             if (rc) return rc;
         } else {
-            const int kmax = base + (extra ? 1 : 0);
+            const int kmax = plan.depth(0);
             int rc = exchange_rows(h, HB_DIVERGENCE, h->divergence, (size_t)W * sizeof(float), h->roff, h->row0, h->row1, kmax);
             if (rc) return rc;
             if ((rc = scan_tiny(h, std::max(h->row0 - kmax, 0), h->row0))) return rc;
             if ((rc = scan_tiny(h, h->row1, std::min(h->row1 + kmax, H)))) return rc;
         }
     }
-    int remaining = iters;
-    for (int k = 0; k < nlaunch; ++k) {
-        const int K = base + (k < extra ? 1 : 0);
-        const bool last = (k == nlaunch - 1);
-        remaining -= K;
+    JacobiArgs a = jacobi_args(h, h->divergence, h->roff);
+    for (int k = 0; k < plan.n; ++k) {
+        const int K = plan.depth(k);
         a.pin = (const float*)h->pressure.read; a.pout = (float*)h->pressure.write;
-        a.out_lo = h->row0; a.out_hi = h->row1;
+        int ext = 0;                                   // launch k produces the owned rows +- ext
         if (h->slab()) {
-            int ext;
             if (deep) {
-                ext = remaining + 1;
+                ext = plan.after(k) + 1;
             } else {
-                ext = last ? 1 : 0;
+                ext = (k == plan.n - 1) ? 1 : 0;
                 int rc = exchange_rows(h, HB_PRESSURE, h->pressure.read, (size_t)W * sizeof(float), h->roff, h->row0, h->row1, K + ext);
                 if (rc) return rc;
             }
-            a.out_lo = std::max(h->row0 - ext, 0); a.out_hi = std::min(h->row1 + ext, H);
         }
+        a.out_lo = std::max(h->row0 - ext, 0); a.out_hi = std::min(h->row1 + ext, H);
         const bool sc = scale_first && k == 0;
         int rc;
-        if (blocked) {
+        if (tb) {
             // the maps of the buffer this launch reads, found by its address (a resize re-allocates pressure
             // and leaves par_p as it was)
             const int m = (a.pin == h->tmaps.p[0]) ? 0 : (a.pin == h->tmaps.p[1]) ? 1 : -1;
             if (m < 0) return fail(h, FLUID_ERR_CUDA, "jacobi_tb_kernel: the pressure buffer has no tensor map");
-            // programmatic dependent launch: behind another blocked launch of this solve, and — first launch —
-            // behind whatever kernel precedes it on the stream (the previous solve's last launch in a host loop
-            // of solves; a kernel without griddepcontrol.launch_dependents simply triggers at its end)
-            h->pdl_chain = true;
-            rc = launch_tb_dyn(h, K, a, h->tmaps.m[m], sc);
-            h->pdl_chain = false;
-        } else if (tb_eligible(h)) {
-            dim3 b(32, 8);
-            dim3 g((W / 4 + b.x - 1) / b.x, (a.out_hi - a.out_lo + b.y - 1) / b.y);
-            if (sc) jacobi_sweep_kernel<true><<<g, b, 0, h->stream>>>(a);
-            else jacobi_sweep_kernel<false><<<g, b, 0, h->stream>>>(a);
-            ++h->jacobi_kernel_launches;
-            rc = check_launch(h, "jacobi_sweep_kernel");
-        } else if (h->half && W % 8 == 0 && W >= 64) {
-            dim3 b(32, 8), g((W / 8 + 31) / 32, (H + 7) / 8);
-            hs::jacobi8_kernel<<<g, b, 0, h->stream>>>((const hs::h1*)a.pin, (const hs::h1*)a.div, (hs::h1*)a.pout, W, H);
-            ++h->jacobi_kernel_launches;
-            rc = check_launch(h, "hs::jacobi8_kernel");
+            // chained: behind another blocked launch of this solve, and — first launch — behind whatever kernel
+            // precedes it on the stream (the previous solve's last launch in a host loop of solves; a kernel
+            // without griddepcontrol.launch_dependents simply triggers at its end)
+            rc = launch_tb(h, K, sc, true, a, h->tmaps.m[m]);
         } else {
-            dim3 b(64, 4);
-            with_storage(h, [&](auto s) {
-                jacobi_scalar_kernel<decltype(s)><<<grid2d(W, a.out_hi - a.out_lo, b), b, 0, h->stream>>>(a, sc);
-            });
-            ++h->jacobi_kernel_launches;
-            rc = check_launch(h, "jacobi_scalar_kernel");
+            rc = launch_sweep(h, a, sc);
         }
         if (rc) return rc;
         swap_p(h); ++nl;
@@ -670,8 +684,6 @@ int create_common(const fluid_config* cfg, int rank, int world, const void* uid,
         int rc = fail(nullptr, FLUID_ERR_INVALID, "slabs of %d rows are too short for a 14-row halo: use fewer GPUs", cfg->sim_h / world);
         delete h; return rc;
     }
-    if (const char* e = getenv("FLUID_JACOBI_ROWS")) h->jacobi_rows_override = atoi(e);
-    if (const char* e = getenv("FLUID_JACOBI_WARPS")) h->jacobi_warps_per_sm = atoi(e);
     auto body = [&]() -> int {
         CU(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
         for (auto& e : h->mark) CU(cudaEventCreate(&e));
@@ -1430,10 +1442,7 @@ int solve_host_banded(fluid_t* h, const float* div_host, float* p_host, int iter
         for (auto& e : hp.ev_up) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
         for (auto& e : hp.ev_done) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
     }
-    int kb = h->cfg.jacobi_block > 0 ? h->cfg.jacobi_block : K_DEFAULT;
-    kb = std::min(kb, KMAX);
-    const int nlaunch = (iters + kb - 1) / kb;
-    const int base = iters / nlaunch, extra = iters % nlaunch;
+    const JacobiPlan plan(iters, block_depth(h, true));
     const int band = (H + nb - 1) / nb, halo = iters;
     // band-private rows [loc, loc + band + 2*halo): every row a launch of band [b_lo, b_hi) reads or writes lies
     // in [max(b_lo - halo, 0), b_hi + halo).  Boxes staged beyond a map's rows read as zero, and rows past what
@@ -1477,25 +1486,15 @@ int solve_host_banded(fluid_t* h, const float* div_host, float* p_host, int iter
         if ((rc = encode_rows_map(h, m[0].d, h->divergence + (ptrdiff_t)loc * W, W, H - loc))) return rc;
         memcpy(m[1].d, m[0].d, sizeof m[0].d);
         memcpy(m[2].d, m[0].d, sizeof m[0].d);
-        int remaining = iters;
-        for (int k = 0; k < nlaunch; ++k) {
-            const int K = base + (k < extra ? 1 : 0);
-            const bool last = (k == nlaunch - 1);
-            remaining -= K;
-            JacobiArgs a{};
-            a.W = W; a.H = H; a.scale = h->cfg.pressure; a.err = h->halo_flag; a.tiny_map = h->tiny_map;
-            a.exact_streams = h->exact_streams;
-            a.out_lo = std::max(b_lo - remaining, 0); a.out_hi = std::min(b_hi + remaining, H);
+        for (int k = 0; k < plan.n; ++k) {
             // the kernel addresses all three fields as "local row 0 + (row - row_off)": a whole-grid field G is
             // passed as G + loc*W
-            a.row_off = loc;
-            a.div = h->divergence + (ptrdiff_t)loc * W;
+            JacobiArgs a = jacobi_args(h, h->divergence + (ptrdiff_t)loc * W, loc);
+            a.out_lo = std::max(b_lo - plan.after(k), 0); a.out_hi = std::min(b_hi + plan.after(k), H);
             a.pin = (k == 0) ? p_in + (ptrdiff_t)loc * W : hp.s[(k - 1) & 1];
-            a.pout = last ? result + (ptrdiff_t)loc * W : hp.s[k & 1];
-            h->pdl_chain = (k > 0);
-            rc = launch_tb_dyn(h, K, a, m[k == 0 ? 0 : 1 + ((k - 1) & 1)], k == 0);
-            h->pdl_chain = false;
-            if (rc) return rc;
+            a.pout = (k == plan.n - 1) ? result + (ptrdiff_t)loc * W : hp.s[k & 1];
+            // chained only behind the band's previous launch
+            if ((rc = launch_tb(h, plan.depth(k), k == 0, k > 0, a, m[k == 0 ? 0 : 1 + ((k - 1) & 1)]))) return rc;
         }
         CU(cudaEventRecord(hp.ev_done[b], h->stream));
         CU(cudaStreamWaitEvent(hp.down, hp.ev_done[b], 0));
@@ -1517,10 +1516,9 @@ int fluid_pressure_solve_host(fluid_t* h, const float* div_host, float* p_host, 
         if (!rc) rc = fluid_read(h, FLUID_FIELD_PRESSURE, p_host, (size_t)h->cfg.sim_w * h->cfg.sim_h);
         return rc;
     }
-    // one GPU, blocked kernel: solve band by band behind the copies (FLUID_E2E_BANDS=1 keeps the one-piece path)
-    if (!h->slab() && iters > 0 && tb_eligible(h) && !(h->cfg.flags & FLUID_FLAG_NAIVE_JACOBI) && h->cfg.jacobi_block != 1) {
-        static const int bands_env = getenv("FLUID_E2E_BANDS") ? atoi(getenv("FLUID_E2E_BANDS")) : 16;
-        int nb = std::min(std::min(bands_env, 16), h->cfg.sim_h / std::max(256, 4 * iters));
+    // one GPU, blocked kernel: solve band by band behind the copies, unless the grid is too short for two bands
+    if (!h->slab() && iters > 0 && blocked(h, block_depth(h, true))) {
+        const int nb = std::min(16, h->cfg.sim_h / std::max(256, 4 * iters));
         if (nb >= 2) return solve_host_banded(h, div_host, p_host, iters, nb);
     }
     const size_t n = (size_t)h->cfg.sim_w * (h->row1 - h->row0);   // owned rows

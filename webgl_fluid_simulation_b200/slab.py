@@ -1,14 +1,17 @@
 """Row-slab decomposition plan (SURVEY §8e) — the host-side arithmetic of the multi-GPU path.
 
-Mirrors csrc/fluid.cu (create_common / run_jacobi / fluid_step) so that the schedule can be
-checked on CPU (tests/test_slab_schedule_gloo.py) and so that launchers know which rows a rank owns.
+Mirrors csrc/fluid.cu (create_common; block_depth, the depth of a solve; JacobiPlan, the launch split that
+run_jacobi and solve_host_banded iterate over) so that the schedule can be checked on CPU
+(tests/test_slab_schedule_gloo.py, tests/test_band_schedule_cpu.py) and so that launchers know which rows a
+rank owns.
 One process per GPU; rank g of G owns sim rows [g*H//G, (g+1)*H//G) and the matching dye rows.
 Messages (NCCL send/recv inside the library, both neighbours in one group) happen ONLY on:
   * Jacobi, communication-avoiding ("deep") form: ONE group per solve with iters+1 rows of pressure
     and iters rows of divergence; launch i then produces owned rows +- (sweeps still to come + 1).
-    Fallback when the ghost zone is thinner than iters+1: kmax rows of divergence once, then K rows
-    of pressure before each launch of depth K (K+1 before the last, which also produces one row
-    beyond each slab edge so that gradientSubtract needs no message);
+    Fallback when the ghost zone is thinner than iters+1: as many rows of divergence as the first
+    (deepest) launch has sweeps, once, then K rows of pressure before each launch of depth K (K+1
+    before the last, which also produces one row beyond each slab edge so that gradientSubtract
+    needs no message);
   * advection: G rows of the projected velocity, then Gd rows of dye.
 curl / vorticity / divergence run on ghost rows the previous step computed redundantly
 (velocity is advected on owned rows +-3: curl needs +-2, vorticity +-1, divergence +-0).
@@ -28,7 +31,7 @@ def rows(extent: int, rank: int, world: int) -> tuple[int, int]:
 
 
 def jacobi_launches(iters: int, block: int = DEFAULT_BLOCK) -> list[int]:
-    """Balanced split of `iters` sweeps into ceil(iters/block) launches (run_jacobi)."""
+    """Balanced split of `iters` sweeps into ceil(iters/block) launches, deeper ones first (fluid.cu JacobiPlan)."""
     if iters <= 0:
         return []
     block = max(1, min(block, KMAX))
@@ -37,13 +40,15 @@ def jacobi_launches(iters: int, block: int = DEFAULT_BLOCK) -> list[int]:
     return [base + (1 if k < extra else 0) for k in range(n)]
 
 
-def host_bands(sim_h: int, iters: int, bands: int = 16, block: int = DEFAULT_BLOCK) -> list[dict]:
+def host_bands(sim_h: int, iters: int, bands: int = 16, block: int = 0) -> list[dict]:
     """Plan of `fluid_pressure_solve_host` on one GPU (fluid.cu solve_host_banded): the grid is cut into row
     bands; band b is solved as soon as upload chunk b has arrived and is downloaded while later chunks upload.
     Returns one dict per band: owned rows [lo, hi), upload chunk [up_lo, up_hi) (what the band needs beyond the
     earlier chunks: rows up to hi + iters), and per launch (K, out_lo, out_hi) — launch k produces the band's
-    rows +- the sweeps still to come.  Empty list: the one-piece path (grid too short for two bands)."""
+    rows +- the sweeps still to come.  block: JACOBI_BLOCK, 0 = DEFAULT_BLOCK (fluid.cu block_depth of a band).
+    Empty list: the one-piece path (grid too short for two bands)."""
     nb = min(bands, 16, sim_h // max(256, 4 * iters)) if iters > 0 else 0
+    block = block if block > 0 else DEFAULT_BLOCK
     if nb < 2:
         return []
     band = (sim_h + nb - 1) // nb
@@ -84,7 +89,9 @@ class SlabPlan:
             raise ValueError(f"slab of {self.row1 - self.row0} rows is too short for a 14-row halo")
 
     def block(self, requested: int = 0) -> int:
-        kb = requested if requested > 0 else DEFAULT_BLOCK
+        """Depth of the solve's launches (fluid.cu block_depth): `requested` (JACOBI_BLOCK) if > 0, else KMAX on
+        one GPU and DEFAULT_BLOCK on a slab; at most KMAX, and on a slab below the ghost rows."""
+        kb = requested if requested > 0 else (DEFAULT_BLOCK if self.world > 1 else KMAX)
         kb = min(kb, KMAX)
         return min(kb, self.G - 1) if self.world > 1 else kb
 
