@@ -435,12 +435,51 @@ def test_resize_carries_state_like_resizeDoubleFBO(pkg, oracle):
     assert bits_equal(s.readField("dye"), O.resample(dye, 96, 96))
     assert not s.readField("pressure").any() and not s.readField("divergence").any()
     s.close()
-    # and straight against the executed copyShader (power-of-two sizes: bitwise)
+    # and straight against the executed copyShader: power-of-two sizes bitwise, ragged ones at the tolerance
+    # of test_oracle_golden.py (the rasteriser's vUv differs from (i + .5) / W in the last place)
     g = golden("resample_dye_64_to_32")
     s = make(pkg, 16, 16, 64, 64)
     s.writeField("dye", g["src"])
     s._sizes = (16, 16, 32, 32); s.initFramebuffers()
     assert bits_equal(s.readField("dye"), g["linear"])
+    s.close()
+    for name, plane in (("resample_v_32_to_48", "velocity"), ("resample_dye_40x28_to_64x48", "dye")):
+        g = golden(name)
+        Hs, Ws = g["src"].shape[:2]
+        Wn, Hn = int(g["Wd"]), int(g["Hd"])
+        s = make(pkg, *((Ws, Hs, 8, 8) if plane == "velocity" else (8, 8, Ws, Hs)))
+        s.writeField(plane, g["src"])
+        s._sizes = (Wn, Hn, 8, 8) if plane == "velocity" else (8, 8, Wn, Hn)
+        s.initFramebuffers()
+        got = s.readField(plane)
+        assert bits_equal(got, O.resample(g["src"], Wn, Hn)), name
+        assert max_rel(got, g["linear"]) < 2e-6, name
+        s.close()
+
+
+@pytest.mark.parametrize("src,dst", [((36, 20, 54, 30), (23, 41, 97, 31)),          # ragged, down and up
+                                     ((23, 41, 97, 31), (36, 20, 54, 30)),
+                                     ((1024, 512, 1024, 512), (37, 23, 37, 23)),    # a large down-scale
+                                     ((1, 9, 3, 27), (9, 1, 27, 3)),                # 1-column -> 1-row grids
+                                     ((9, 1, 27, 3), (1, 9, 3, 27))])
+def test_resize_ragged_and_degenerate_sizes_like_resizeDoubleFBO(pkg, oracle, src, dst):
+    """initFramebuffers() on an fp32 handle (fluid_resize) at the sizes of its half-storage sibling and
+    beyond: velocity and dye resampled with the LINEAR copy, bitwise against the oracle, inf / NaN dye
+    NaN-aware; pressure, divergence and curl start over at zero."""
+    from test_gpu_fast_paths import same_or_both_nan
+    from test_gpu_splats import nasty_fields
+    O = oracle
+    v, _, p = rand_fields(*src, 9)
+    _, dye, _ = nasty_fields(1, 1, src[2], src[3], 10)             # inf / NaN / subnormal dye
+    s = make(pkg, *src)
+    s.writeField("velocity", v); s.writeField("dye", dye); s.writeField("pressure", p)
+    s._sizes = dst; s.initFramebuffers()
+    W, H, Wd, Hd = dst
+    assert s._dims("velocity")[:2] == (W, H) and s._dims("dye")[:2] == (Wd, Hd)
+    assert bits_equal(s.readField("velocity"), O.resample(v, W, H))
+    assert same_or_both_nan(s.readField("dye"), O.resample(dye, Wd, Hd))
+    for n in ("pressure", "divergence", "curl"):
+        assert not s.readField(n).any(), n
     s.close()
 
 
