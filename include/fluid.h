@@ -137,7 +137,8 @@ int fluid_create_slab(const fluid_config* cfg, int rank, int world, const void* 
 int fluid_nccl_unique_id(void* out_uid, size_t uid_bytes); /* uid_bytes must be >= 128 */
 
 /* Optional peer-memory halo path for slab handles on one NVLink/NVSwitch box (no reference
- * counterpart).  Every rank exports a 256-byte blob (a CUDA IPC handle of its field arena + layout),
+ * counterpart).  Every handle keeps all its fields in one device allocation, its arena.  Every rank
+ * exports a 256-byte blob (a CUDA IPC handle of that arena + its layout),
  * the launcher all-gathers them, and each rank connects to rank-1 / rank+1 (NULL at the ends).
  * Afterwards halo rows are stored straight into the neighbours' ghost rows by one kernel that
  * also carries the free/ready handshake (system-scope release/acquire flag words, bounded spins);
@@ -149,10 +150,12 @@ int fluid_p2p_disable(fluid_t* h);   /* back to NCCL; call on every rank if any 
 void fluid_destroy(fluid_t* h);
 
 /* initFramebuffers() on a live simulation (S:982-1010 else-branches + resizeDoubleFBO S:1116-1126):
- * velocity and dye are bilinearly resampled to the new size (copyShader through a LINEAR sampler),
- * pressure / divergence / curl are re-created zeroed.
+ * the handle's fields move to a new arena.  Velocity and dye are bilinearly resampled to the new size
+ * (copyShader through a LINEAR sampler); one whose size did not change is kept bit for bit.  Pressure /
+ * divergence / curl are re-created zeroed.  Old and new arena coexist during the call.
+ * FLUID_ERR_NOMEM: the new arena does not fit; the handle is left exactly as it was.
  * On a slab handle the call is collective (same sizes on every rank): ghost rows of the old velocity and
- * dye are refreshed, the rank's new rows are resampled into a new arena, and the peer-memory mappings
+ * dye are refreshed, the rank's new rows are resampled, and the peer-memory mappings of the old arena
  * are dropped (export / connect again, or stay on NCCL).  FLUID_ERR_HALO: the factor needs more ghost
  * rows than the slab keeps. */
 int fluid_resize(fluid_t* h, int sim_w, int sim_h, int dye_w, int dye_h);

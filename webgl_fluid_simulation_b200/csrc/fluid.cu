@@ -28,15 +28,33 @@ namespace {
 
 thread_local std::string g_create_error;
 
+// Byte offsets of every field in a handle's arena: both slots of the velocity / pressure / dye pairs,
+// divergence, curl and the peer-memory flag words, and the arena's size.  Fixed-width: it travels in P2PBlob.
+struct FieldLayout {
+    uint64_t v[2], p[2], dye[2], div, curl, flags, bytes;
+};
+
 struct Pair {              // createDoubleFBO, S:1079-1106
     void* read = nullptr;
     void* write = nullptr;
-    void swap() { std::swap(read, write); }
+    int par = 0;           // arena slot of .read (toggles with swap(); SPMD-identical on a slab)
+    void swap() { std::swap(read, write); par ^= 1; }
+    void place(char* arena, const uint64_t (&slot)[2]) { read = arena + slot[par]; write = arena + slot[par ^ 1]; }
+};
+
+// Row ownership and ghost-zone heights of a handle (slab_geometry).  Single GPU: all rows, no ghost rows.
+struct SlabGeometry {
+    int G = 0, Gd = 0;               // ghost rows kept below and above the owned rows (sim / dye)
+    int row0 = 0, row1 = 0;          // owned sim rows  [row0, row1)
+    int drow0 = 0, drow1 = 0;        // owned dye rows  [drow0, drow1)
+    int roff = 0, droff = 0;         // global row index of local row 0  (row0 - G, drow0 - Gd)
+    int lrows() const { return row1 - row0 + 2 * G; }
+    int ldrows() const { return drow1 - drow0 + 2 * Gd; }
 };
 
 }  // namespace
 
-struct fluid {
+struct fluid : SlabGeometry {
     fluid_config cfg{};
     int device = 0;
     int sm_count = 132;
@@ -63,8 +81,8 @@ struct fluid {
     float* dt_dev = nullptr;               // step()'s dt lives in device memory: one graph serves every dt
     unsigned char* tiny_map = nullptr;     // where divergence has 0 < |d| < 2^-123 (jacobi.cuh): 1 byte per 128x32 cells, GLOBAL rows
     size_t tiny_map_bytes = 0;
-    // 2-D tensor maps the blocked Jacobi kernel stages through: m[k] maps pressure buffer p[k] and divergence
-    struct Tmaps { fk::TmapPair m[2]; const void* p[2] = {nullptr, nullptr}; } tmaps;
+    // 2-D tensor maps the blocked Jacobi kernel stages through: m[k] maps pressure slot k and divergence
+    struct Tmaps { fk::TmapPair m[2]; } tmaps;
     double splat_radius_d = 0.25;          // config.SPLAT_RADIUS and the canvas aspect as the JS doubles they are
     double aspect_d = 1.0;                 // (correctRadius S:1457-1462 is double arithmetic, narrowed once)
     int background = 0;                    // FLUID_BACKGROUND: what render() draws the display over (0 colour, 1 checkerboard, 2 none)
@@ -72,25 +90,21 @@ struct fluid {
     bool have_timing = false;
     std::string err;
 
-    // ---- row-slab decomposition (SURVEY §8e).  Single GPU: rank 0 of 1, no ghost rows. -------------
+    // every field lives in ONE allocation, laid out by `layout`: a single CUDA IPC handle maps all that a
+    // slab neighbour may write into
+    char* arena = nullptr;
+    FieldLayout layout{};
+    // ---- row-slab decomposition (SURVEY §8e; the geometry is the SlabGeometry base).  Single GPU: rank 0 of 1
     int rank = 0, world = 1;
-    int G = 0, Gd = 0;               // ghost rows kept below and above the owned rows (sim / dye)
-    int row0 = 0, row1 = 0;          // owned sim rows  [row0, row1)
-    int drow0 = 0, drow1 = 0;        // owned dye rows  [drow0, drow1)
-    int roff = 0, droff = 0;         // global row index of local row 0  (row0 - G, drow0 - Gd)
     ncdl::ncclComm_t comm = nullptr;
     bool v_ghost_valid = true;       // velocity valid on owned rows +-3 (what the next step needs)
     uint64_t halo_groups = 0;        // halo exchanges issued (diagnostics)
     // ---- peer-memory halo path (fluid_p2p_export / fluid_p2p_connect) -------------------------------
-    char* arena = nullptr;           // slab mode: every exchanged field + the flag words live in ONE allocation
-    size_t arena_bytes = 0;
-    size_t off_v[2] = {0, 0}, off_p[2] = {0, 0}, off_dye[2] = {0, 0}, off_div = 0, off_flags = 0;
-    int par_v = 0, par_p = 0, par_dye = 0;   // which half of a pair is .read (toggles with swap(); SPMD-identical)
     struct Peer {
         bool present = false;
         char* base = nullptr;        // neighbour's arena mapped here through CUDA IPC
         int roff = 0, droff = 0;     // neighbour's local-row-0 global row indices
-        size_t off_v[2], off_p[2], off_dye[2], off_div, off_flags;
+        FieldLayout layout{};
     } peer[2];                       // [0] = rank-1 (below), [1] = rank+1 (above)
     bool p2p = false;
     uint32_t p2p_seq = 0;
@@ -125,17 +139,11 @@ struct fluid {
         int dw = 0, dh = 0;
     } pfx;
     bool slab() const { return world > 1; }
-    int lrows() const { return row1 - row0 + 2 * G; }
-    int ldrows() const { return drow1 - drow0 + 2 * Gd; }
 };
 
 namespace {
 
 using namespace fk;
-
-inline void swap_v(fluid_t* h) { h->velocity.swap(); h->par_v ^= 1; }
-inline void swap_p(fluid_t* h) { h->pressure.swap(); h->par_p ^= 1; }
-inline void swap_dye(fluid_t* h) { h->dye.swap(); h->par_dye ^= 1; }
 
 void drop_graphs(fluid_t* h) {
     if (!h->graphs.empty() && h->stream) cudaStreamSynchronize(h->stream);   // an exec may still be in flight
@@ -320,12 +328,10 @@ int encode_rows_map(fluid_t* h, unsigned char (&tm)[128], const void* base, int 
 int build_tmaps(fluid_t* h) {
     h->tmaps = {};
     if (!tb_eligible(h)) return FLUID_OK;
-    const void* p[2] = {h->pressure.read, h->pressure.write};
     for (int k = 0; k < 2; ++k) {
-        int rc = encode_rows_map(h, h->tmaps.m[k].p, p[k], h->cfg.sim_w, h->lrows());
+        int rc = encode_rows_map(h, h->tmaps.m[k].p, h->arena + h->layout.p[k], h->cfg.sim_w, h->lrows());
         if (!rc) rc = encode_rows_map(h, h->tmaps.m[k].d, h->divergence, h->cfg.sim_w, h->lrows());
         if (rc) return rc;
-        h->tmaps.p[k] = p[k];
     }
     return FLUID_OK;
 }
@@ -426,7 +432,7 @@ int run_jacobi(fluid_t* h, int iters, bool scale_first, int* launches_out) {
             return check_launch(h, "scale_kernel");
         });
         if (rc) return rc;
-        swap_p(h); ++nl;
+        h->pressure.swap(); ++nl;
         scale_first = false;
     }
     if (iters <= 0) {
@@ -448,9 +454,7 @@ int run_jacobi(fluid_t* h, int iters, bool scale_first, int* launches_out) {
             // one right-hand side, bench.py's loop): its ghost rows — and their tiny-value flags — are still in
             // place unless some pass rewrote divergence since they were last received (SPMD-identical decision)
             const bool send_div = h->div_sent_epoch != h->div_epoch || h->div_sent_rows < iters;
-            const HaloItem it[2] = {
-                {h->pressure.read, (size_t)W * sizeof(float), h->roff, h->row0, h->row1, iters + 1, HB_PRESSURE},
-                {h->divergence, (size_t)W * sizeof(float), h->roff, h->row0, h->row1, iters, HB_DIVERGENCE}};
+            const HaloItem it[2] = {{HB_PRESSURE, iters + 1}, {HB_DIVERGENCE, iters}};
             // the neighbours' divergence rows get their tiny values flagged like the local producers do:
             // inside the wait kernel on the peer-memory path, by a scan kernel after the NCCL group
             h->scan.div = h->divergence; h->scan.map = h->tiny_map; h->scan.W = W; h->scan.row_off = h->roff;
@@ -467,7 +471,7 @@ int run_jacobi(fluid_t* h, int iters, bool scale_first, int* launches_out) {
             if (rc) return rc;
         } else {
             const int kmax = plan.depth(0);
-            int rc = exchange_rows(h, HB_DIVERGENCE, h->divergence, (size_t)W * sizeof(float), h->roff, h->row0, h->row1, kmax);
+            int rc = exchange_rows(h, HB_DIVERGENCE, kmax);
             if (rc) return rc;
             if ((rc = scan_tiny(h, std::max(h->row0 - kmax, 0), h->row0))) return rc;
             if ((rc = scan_tiny(h, h->row1, std::min(h->row1 + kmax, H)))) return rc;
@@ -483,7 +487,7 @@ int run_jacobi(fluid_t* h, int iters, bool scale_first, int* launches_out) {
                 ext = plan.after(k) + 1;
             } else {
                 ext = (k == plan.n - 1) ? 1 : 0;
-                int rc = exchange_rows(h, HB_PRESSURE, h->pressure.read, (size_t)W * sizeof(float), h->roff, h->row0, h->row1, K + ext);
+                int rc = exchange_rows(h, HB_PRESSURE, K + ext);
                 if (rc) return rc;
             }
         }
@@ -491,90 +495,100 @@ int run_jacobi(fluid_t* h, int iters, bool scale_first, int* launches_out) {
         const bool sc = scale_first && k == 0;
         int rc;
         if (tb) {
-            // the maps of the buffer this launch reads, found by its address (a resize re-allocates pressure
-            // and leaves par_p as it was)
-            const int m = (a.pin == h->tmaps.p[0]) ? 0 : (a.pin == h->tmaps.p[1]) ? 1 : -1;
-            if (m < 0) return fail(h, FLUID_ERR_CUDA, "jacobi_tb_kernel: the pressure buffer has no tensor map");
             // chained: behind another blocked launch of this solve, and — first launch — behind whatever kernel
             // precedes it on the stream (the previous solve's last launch in a host loop of solves; a kernel
             // without griddepcontrol.launch_dependents simply triggers at its end)
-            rc = launch_tb(h, K, sc, true, a, h->tmaps.m[m]);
+            rc = launch_tb(h, K, sc, true, a, h->tmaps.m[h->pressure.par]);
         } else {
             rc = launch_sweep(h, a, sc);
         }
         if (rc) return rc;
-        swap_p(h); ++nl;
+        h->pressure.swap(); ++nl;
     }
     if (launches_out) *launches_out = nl;
     return FLUID_OK;
 }
 
-// pressure, divergence and curl of a single-GPU handle, zeroed (createFBO / createDoubleFBO, S:1004-1006)
-int alloc_scalar_fields(fluid_t* h) {
-    cudaFree(h->pressure.read); cudaFree(h->pressure.write); cudaFree(h->divergence); cudaFree(h->curl);
-    h->pressure = Pair{}; h->divergence = h->curl = nullptr;
-    const size_t bytes = sim_cells(h) * sbytes(h);
-    for (void** p : {&h->pressure.read, &h->pressure.write, (void**)&h->divergence, (void**)&h->curl}) {
-        CU(cudaMalloc(p, bytes));
-        CU(cudaMemsetAsync(*p, 0, bytes, h->stream));
+// The arena of n sim and nd dye cells (local rows) at the handle's bytes per cell.  Every slot starts on a
+// 2 MiB boundary, where a cudaMalloc of its own would put a large field.  The order (velocity, dye, pressure,
+// divergence, curl) is not free: with pressure ahead of dye the 4096^2 x 50 blocked solve measured 0.4 %
+// slower (H100 80GB HBM3, 700 W power limit).  The 1 KiB of peer-memory flag words come last (unused on one GPU).
+FieldLayout field_layout(const fluid_t* h, size_t n, size_t nd) {
+    constexpr uint64_t ALIGN = 2ull << 20;
+    FieldLayout L{};
+    uint64_t o = 0;
+    auto slot = [&o](uint64_t bytes) { const uint64_t at = o; o += (bytes + ALIGN - 1) & ~(ALIGN - 1); return at; };
+    for (int k = 0; k < 2; ++k) L.v[k] = slot(n * vbytes(h));
+    for (int k = 0; k < 2; ++k) L.dye[k] = slot(nd * dbytes(h));
+    for (int k = 0; k < 2; ++k) L.p[k] = slot(n * sbytes(h));
+    L.div = slot(n * sbytes(h));
+    L.curl = slot(n * sbytes(h));
+    L.flags = o;
+    L.bytes = o + 1024;
+    return L;
+}
+
+// A new arena for `L`, zeroed, with dye alpha 1 in both dye slots (createFBO / createDoubleFBO, S:1004-1006).
+// FLUID_ERR_NOMEM when it does not fit: nothing is allocated and the runtime keeps no error.
+int make_arena(fluid_t* h, const FieldLayout& L, size_t nd, char** out) {
+    char* a = nullptr;
+    if (cudaMalloc((void**)&a, L.bytes) != cudaSuccess) {
+        cudaGetLastError();                      // not sticky: keep it out of the next launch check
+        return fail(h, FLUID_ERR_NOMEM, "out of device memory for the fields (%llu bytes)", (unsigned long long)L.bytes);
     }
+    if (cudaMemsetAsync(a, 0, L.bytes, h->stream) != cudaSuccess) {
+        cudaFree(a);
+        return fail(h, FLUID_ERR_CUDA, "cudaMemsetAsync of the field arena failed: %s", cudaGetErrorString(cudaGetLastError()));
+    }
+    int rc = with_storage(h, [&](auto s) {
+        using S = decltype(s);
+        for (const uint64_t o : L.dye)
+            fill_alpha_kernel<S><<<(unsigned)((nd + 255) / 256), 256, 0, h->stream>>>((typename S::T4*)(a + o), nd);
+        return check_launch(h, "fill_alpha_kernel", 2);
+    });
+    if (rc) { cudaFree(a); return rc; }
+    *out = a;
     return FLUID_OK;
 }
 
-int alloc_fields(fluid_t* h) {
-    const size_t n = sim_cells(h), nd = dye_cells(h);
-    if (h->slab()) {
-        // one allocation, so that a single CUDA IPC handle maps everything a neighbour may write into
-        auto al = [](size_t b) { return (b + 1023) & ~(size_t)1023; };
-        size_t o = 0;
-        h->off_flags = o; o += 1024;
-        for (int k = 0; k < 2; ++k) { h->off_v[k] = o; o += al(n * sizeof(float2)); }
-        for (int k = 0; k < 2; ++k) { h->off_p[k] = o; o += al(n * sizeof(float)); }
-        for (int k = 0; k < 2; ++k) { h->off_dye[k] = o; o += al(nd * sizeof(float4)); }
-        h->off_div = o; o += al(n * sizeof(float));
-        const size_t off_curl = o; o += al(n * sizeof(float));
-        h->arena_bytes = o;
-        CU(cudaMalloc((void**)&h->arena, o));
-        CU(cudaMemsetAsync(h->arena, 0, o, h->stream));
-        h->velocity.read = h->arena + h->off_v[0]; h->velocity.write = h->arena + h->off_v[1];
-        h->pressure.read = h->arena + h->off_p[0]; h->pressure.write = h->arena + h->off_p[1];
-        h->dye.read = h->arena + h->off_dye[0]; h->dye.write = h->arena + h->off_dye[1];
-        h->divergence = (float*)(h->arena + h->off_div); h->curl = (float*)(h->arena + off_curl);
-        h->par_v = h->par_p = h->par_dye = 0;
-    } else {
-        CU(cudaMalloc(&h->velocity.read, n * vbytes(h)));
-        CU(cudaMalloc(&h->velocity.write, n * vbytes(h)));
-        CU(cudaMalloc(&h->dye.read, nd * dbytes(h)));
-        CU(cudaMalloc(&h->dye.write, nd * dbytes(h)));
-        CU(cudaMemsetAsync(h->velocity.read, 0, n * vbytes(h), h->stream));
-        CU(cudaMemsetAsync(h->velocity.write, 0, n * vbytes(h), h->stream));
-        int rc = alloc_scalar_fields(h); if (rc) return rc;
-    }
-    { int rc = alloc_tiny_map(h); if (rc) return rc; }
-    { int rc = build_tmaps(h); if (rc) return rc; }
+// the handle's fields now live in arena `a` (each pair keeps its parity); the tiny map and the tensor maps
+// follow the new addresses and sizes
+int adopt_arena(fluid_t* h, char* a, const FieldLayout& L) {
+    h->arena = a; h->layout = L;
+    h->velocity.place(a, L.v); h->pressure.place(a, L.p); h->dye.place(a, L.dye);
+    h->divergence = (float*)(a + L.div); h->curl = (float*)(a + L.curl);
     h->div_sent_epoch = 0;                               // fresh buffers: no divergence ghost rows in place yet
-    return with_storage(h, [&](auto s) {
-        using S = decltype(s);
-        for (void* d : {h->dye.read, h->dye.write})
-            fill_alpha_kernel<S><<<(unsigned)((nd + 255) / 256), 256, 0, h->stream>>>((typename S::T4*)d, nd);
-        return check_launch(h, "fill_alpha_kernel", 2);
-    });
+    int rc = alloc_tiny_map(h);
+    return rc ? rc : build_tmaps(h);
 }
 
-void free_fields(fluid_t* h) {
-    if (h->arena) {
-        for (auto& p : h->peer) if (p.present && p.base) { cudaIpcCloseMemHandle(p.base); p.base = nullptr; p.present = false; }
-        cudaFree(h->arena); h->arena = nullptr;
-    } else {
-        cudaFree(h->velocity.read); cudaFree(h->velocity.write);
-        cudaFree(h->dye.read); cudaFree(h->dye.write);
-        cudaFree(h->pressure.read); cudaFree(h->pressure.write);
-        cudaFree(h->divergence); cudaFree(h->curl);
+int alloc_fields(fluid_t* h) {
+    const FieldLayout L = field_layout(h, sim_cells(h), dye_cells(h));
+    char* a = nullptr;
+    int rc = make_arena(h, L, dye_cells(h), &a);
+    return rc ? rc : adopt_arena(h, a, L);
+}
+
+// One field's rows [j0, j1) of the new grid (Wn x Hn, local row 0 at global row dst_off) from the old grid
+// (W x H, local row 0 at src_off): the LINEAR copy of the old texture written in the storage format (in half
+// storage the reference's blit into an RG16F / RGBA16F target rounds to fp16), or, when the size did not
+// change, the rows as they are — like resizeDoubleFBO, which keeps such a field (S:1116-1126).
+template <class S, class T>
+int carry_field(fluid_t* h, const void* src, int W, int H, int src_off, char* dst, int Wn, int Hn, int dst_off, int j0, int j1) {
+    if (W == Wn && H == Hn) {
+        CU(cudaMemcpyAsync(dst + (size_t)(j0 - dst_off) * W * sizeof(T), (const char*)src + (size_t)(j0 - src_off) * W * sizeof(T),
+                           (size_t)(j1 - j0) * W * sizeof(T), cudaMemcpyDeviceToDevice, h->stream));
+        return FLUID_OK;
     }
-    h->velocity = Pair{}; h->dye = Pair{}; h->pressure = Pair{};
-    h->divergence = h->curl = nullptr;
-    cudaFree(h->tiny_map); h->tiny_map = nullptr;
-    h->tmaps = {};
+    dim3 b(64, 4);
+    resample_kernel<S><<<grid2d(Wn, j1 - j0, b), b, 0, h->stream>>>((const T*)src, W, H, src_off, (T*)dst, Wn, Hn, dst_off, j0, j1);
+    return check_launch(h, "resample_kernel");
+}
+
+// back to NCCL halos: the neighbours' arenas are unmapped
+void close_peers(fluid_t* h) {
+    for (auto& p : h->peer) if (p.present && p.base) { cudaIpcCloseMemHandle(p.base); p.base = nullptr; p.present = false; }
+    h->p2p = false;
 }
 
 // pointer to the first OWNED row of a field's .read buffer, plus its owned extent
@@ -614,8 +628,7 @@ int not_on_slab(fluid_t* h, const char* what) {
 
 // Row ownership + ghost-zone heights of rank `rank` of `world` for a sim_h / dye_h grid (DESIGN.md §7).
 // Returns false when the slabs are too short for the minimum 14-row halo.
-bool slab_geometry(fluid_t* h, int H, int Hd, int iters) {
-    const int rank = h->rank, world = h->world;
+bool slab_geometry(SlabGeometry* h, int rank, int world, int H, int Hd, int iters) {
     h->row0 = (int)((long long)H * rank / world);  h->row1 = (int)((long long)H * (rank + 1) / world);
     h->drow0 = (int)((long long)Hd * rank / world); h->drow1 = (int)((long long)Hd * (rank + 1) / world);
     h->G = h->Gd = 0;
@@ -680,7 +693,7 @@ int create_common(const fluid_config* cfg, int rank, int world, const void* uid,
         int rc = fail(nullptr, FLUID_ERR_INVALID, "FLUID_FLAG_HALF_POSTFX is a single-GPU mode");
         delete h; return rc;
     }
-    if (!slab_geometry(h, cfg->sim_h, cfg->dye_h, cfg->pressure_iterations)) {
+    if (!slab_geometry(h, rank, world, cfg->sim_h, cfg->dye_h, cfg->pressure_iterations)) {
         int rc = fail(nullptr, FLUID_ERR_INVALID, "slabs of %d rows are too short for a 14-row halo: use fewer GPUs", cfg->sim_h / world);
         delete h; return rc;
     }
@@ -772,8 +785,8 @@ int fluid_create_slab(const fluid_config* cfg, int rank, int world, const void* 
 struct P2PBlob {            // what fluid_p2p_export hands to the launcher (opaque to it), 256 bytes
     cudaIpcMemHandle_t mem;
     int32_t rank, roff, droff, reserved;
-    uint64_t off_v[2], off_p[2], off_dye[2], off_div, off_flags, arena_bytes;
-    char pad[256 - sizeof(cudaIpcMemHandle_t) - 16 - 9 * 8];
+    FieldLayout layout;
+    char pad[256 - sizeof(cudaIpcMemHandle_t) - 16 - sizeof(FieldLayout)];
 };
 static_assert(sizeof(P2PBlob) == 256, "blob layout");
 
@@ -788,9 +801,7 @@ int fluid_p2p_export(fluid_t* h, void* blob, size_t blob_bytes) {
     P2PBlob b{};
     CU(cudaStreamSynchronize(h->stream));
     CU(cudaIpcGetMemHandle(&b.mem, h->arena));
-    b.rank = h->rank; b.roff = h->roff; b.droff = h->droff;
-    for (int k = 0; k < 2; ++k) { b.off_v[k] = h->off_v[k]; b.off_p[k] = h->off_p[k]; b.off_dye[k] = h->off_dye[k]; }
-    b.off_div = h->off_div; b.off_flags = h->off_flags; b.arena_bytes = h->arena_bytes;
+    b.rank = h->rank; b.roff = h->roff; b.droff = h->droff; b.layout = h->layout;
     memcpy(blob, &b, sizeof b);
     return FLUID_OK;
 }
@@ -808,10 +819,7 @@ int fluid_p2p_connect(fluid_t* h, const void* blob_below, const void* blob_above
         if (b.rank != h->rank + (side == 0 ? -1 : 1)) return fail(h, FLUID_ERR_INVALID, "blob of rank %d passed as side %d of rank %d", b.rank, side, h->rank);
         void* base = nullptr;
         CU(cudaIpcOpenMemHandle(&base, b.mem, cudaIpcMemLazyEnablePeerAccess));
-        fluid::Peer& P = h->peer[side];
-        P.present = true; P.base = (char*)base; P.roff = b.roff; P.droff = b.droff;
-        for (int k = 0; k < 2; ++k) { P.off_v[k] = b.off_v[k]; P.off_p[k] = b.off_p[k]; P.off_dye[k] = b.off_dye[k]; }
-        P.off_div = b.off_div; P.off_flags = b.off_flags;
+        h->peer[side] = fluid::Peer{true, (char*)base, b.roff, b.droff, b.layout};
     }
     h->p2p = true;
     return FLUID_OK;
@@ -822,8 +830,7 @@ int fluid_p2p_connect(fluid_t* h, const void* blob_below, const void* blob_above
 int fluid_p2p_disable(fluid_t* h) {
     if (!h) return FLUID_ERR_INVALID;
     if (h->stream) CU(cudaStreamSynchronize(h->stream));
-    for (auto& p : h->peer) if (p.present && p.base) { cudaIpcCloseMemHandle(p.base); p.base = nullptr; p.present = false; }
-    h->p2p = false;
+    close_peers(h);
     return FLUID_OK;
 }
 
@@ -832,7 +839,9 @@ void fluid_destroy(fluid_t* h) {
     cudaSetDevice(h->device);
     if (h->stream) cudaStreamSynchronize(h->stream);
     drop_graphs(h);
-    free_fields(h);
+    close_peers(h);
+    cudaFree(h->arena);
+    cudaFree(h->tiny_map);
     cudaFree(h->halo_flag);
     cudaFree(h->exact_streams);
     cudaFree(h->dt_dev);
@@ -921,7 +930,7 @@ static int do_vorticity(fluid_t* h, Grid g) {
         return check_launch(h, "vorticity_kernel");
     });
     if (rc) return rc;
-    swap_v(h);                                   // S:1246
+    h->velocity.swap();                          // S:1246
     return FLUID_OK;
 }
 static int do_divergence(fluid_t* h, Grid g) {
@@ -980,7 +989,7 @@ static int do_cvd(fluid_t* h, Grid g) {
             h->dt_dev, h->tiny_map);
         int rc = check_launch(h, "cvd_stream_kernel"); if (rc) return rc;
         ++h->cvd_stream_launches;
-        swap_v(h);
+        h->velocity.swap();
         return FLUID_OK;
     }
     dim3 b(64, 4);
@@ -989,7 +998,7 @@ static int do_cvd(fluid_t* h, Grid g) {
         (const float2*)h->velocity.read, h->curl, (float2*)h->velocity.write, h->divergence, g,
         h->cfg.curl, h->dt_dev, h->tiny_map);
     int rc = check_launch(h, "curl_vorticity_divergence_kernel"); if (rc) return rc;
-    swap_v(h);
+    h->velocity.swap();
     return FLUID_OK;
 }
 static int do_gradient(fluid_t* h, Grid g) {
@@ -1000,7 +1009,7 @@ static int do_gradient(fluid_t* h, Grid g) {
             (const float*)h->pressure.read, (const float2*)h->velocity.read, (float2*)h->velocity.write, a);
         int rc = check_launch(h, "gradient_stream_kernel"); if (rc) return rc;
         ++h->gradient_stream_launches;
-        swap_v(h);                                   // S:1273
+        h->velocity.swap();                          // S:1273
         return FLUID_OK;
     }
     int rc = with_storage(h, [&](auto s) {
@@ -1011,7 +1020,7 @@ static int do_gradient(fluid_t* h, Grid g) {
         return check_launch(h, "gradient_subtract_kernel");
     });
     if (rc) return rc;
-    swap_v(h);                                   // S:1273
+    h->velocity.swap();                          // S:1273
     return FLUID_OK;
 }
 // valid source rows of a slab buffer: owned + ghost, clipped to the domain
@@ -1040,7 +1049,7 @@ static int do_advect_velocity(fluid_t* h, Grid out) {
             (const typename S::T2*)h->velocity.read, (typename S::T2*)h->velocity.write, a);
     });
     int rc = check_launch(h, "advect_velocity_kernel"); if (rc) return rc;
-    swap_v(h);                                   // S:1285
+    h->velocity.swap();                          // S:1285
     return FLUID_OK;
 }
 static int do_advect_dye(fluid_t* h) {
@@ -1071,7 +1080,7 @@ static int do_advect_dye(fluid_t* h) {
             (const typename S::T2*)h->velocity.read, (const typename S::T4*)h->dye.read, (typename S::T4*)h->dye.write, a);
     });
     int rc = check_launch(h, "advect_dye_kernel"); if (rc) return rc;
-    swap_dye(h);                                        // S:1293
+    h->dye.swap();                                      // S:1293
     return FLUID_OK;
 }
 
@@ -1135,12 +1144,11 @@ int fluid_pass_advect_dye(fluid_t* h, float dt) {
 // rows +- 1) already computed redundantly.
 static int step_enqueue(fluid_t* h, bool timed) {
     const uint64_t l0 = h->launches;
-    const int W = h->cfg.sim_w;
     int rc;
     int jl = 0;
     if (timed) cudaEventRecord(h->tev[0], h->stream);
     if (h->slab() && !h->v_ghost_valid) {   // after fluid_write(velocity): rebuild the +-3 ghost rows
-        if ((rc = exchange_rows(h, HB_VELOCITY, h->velocity.read, (size_t)W * sizeof(float2), h->roff, h->row0, h->row1, 3))) return rc;
+        if ((rc = exchange_rows(h, HB_VELOCITY, 3))) return rc;
         h->v_ghost_valid = true;
     }
     if (h->cfg.flags & FLUID_FLAG_UNFUSED) {
@@ -1156,12 +1164,12 @@ static int step_enqueue(fluid_t* h, bool timed) {
     if ((rc = do_gradient(h, sim_grid(h)))) return rc;
     if (timed) cudaEventRecord(h->tev[3], h->stream);
     if (h->slab()) {   // advection halo #1: G rows of the projected velocity
-        if ((rc = exchange_rows(h, HB_VELOCITY, h->velocity.read, (size_t)W * sizeof(float2), h->roff, h->row0, h->row1, h->G))) return rc;
+        if ((rc = exchange_rows(h, HB_VELOCITY, h->G))) return rc;
     }
     if ((rc = do_advect_velocity(h, sim_grid_ext(h, h->slab() ? 3 : 0)))) return rc;
     if (timed) cudaEventRecord(h->tev[4], h->stream);
     if (h->slab()) {   // advection halo #2: Gd rows of dye
-        if ((rc = exchange_rows(h, HB_DYE, h->dye.read, (size_t)h->cfg.dye_w * sizeof(float4), h->droff, h->drow0, h->drow1, h->Gd))) return rc;
+        if ((rc = exchange_rows(h, HB_DYE, h->Gd))) return rc;
     }
     if ((rc = do_advect_dye(h))) return rc;
     if (timed) cudaEventRecord(h->tev[5], h->stream);
@@ -1187,11 +1195,11 @@ int fluid_step(fluid_t* h, float dt) {
     const fluid_config& c = h->cfg;
     snprintf(key, sizeof key, "%a|%a|%a|%a|%d|%d|%u|%d%d%d|%dx%d|%dx%d",
              c.curl, c.pressure, c.velocity_dissipation, c.density_dissipation, c.pressure_iterations, c.jacobi_block,
-             c.flags, h->par_v, h->par_p, h->par_dye, c.sim_w, c.sim_h, c.dye_w, c.dye_h);
+             c.flags, h->velocity.par, h->pressure.par, h->dye.par, c.sim_w, c.sim_h, c.dye_w, c.dye_h);
     auto it = h->graphs.find(key);
     if (it == h->graphs.end()) {
         if (h->graphs.size() > 64) drop_graphs(h);          // config sliders dragged for a long time: stay bounded
-        const int pv = h->par_v, pp = h->par_p, pd = h->par_dye;
+        const int pv = h->velocity.par, pp = h->pressure.par, pd = h->dye.par;
         const uint64_t l0 = h->launches, j0 = h->jacobi_kernel_launches;
         const uint64_t cs0 = h->cvd_stream_launches, gs0 = h->gradient_stream_launches;
         cudaGraph_t g = nullptr;
@@ -1206,7 +1214,7 @@ int fluid_step(fluid_t* h, float dt) {
         e = cudaGraphInstantiate(&sg.exec, g, 0);
         cudaGraphDestroy(g);
         if (e != cudaSuccess) return fail(h, FLUID_ERR_CUDA, "cudaGraphInstantiate failed: %s", cudaGetErrorString(e));
-        sg.flip_v = pv ^ h->par_v; sg.flip_p = pp ^ h->par_p; sg.flip_dye = pd ^ h->par_dye;
+        sg.flip_v = pv ^ h->velocity.par; sg.flip_p = pp ^ h->pressure.par; sg.flip_dye = pd ^ h->dye.par;
         sg.kernels = (int)(h->launches - l0); sg.jacobi_launches = (int)(h->jacobi_kernel_launches - j0);
         sg.cvd_stream = (int)(h->cvd_stream_launches - cs0); sg.gradient_stream = (int)(h->gradient_stream_launches - gs0);
         h->launches = l0; h->jacobi_kernel_launches = j0;    // captured, not yet executed
@@ -1216,9 +1224,9 @@ int fluid_step(fluid_t* h, float dt) {
         // the capture already performed the host-side swaps of this step
     } else {
         const fluid::StepGraph& sg = it->second;
-        if (sg.flip_v) swap_v(h);
-        if (sg.flip_p) swap_p(h);
-        if (sg.flip_dye) swap_dye(h);
+        if (sg.flip_v) h->velocity.swap();
+        if (sg.flip_p) h->pressure.swap();
+        if (sg.flip_dye) h->dye.swap();
     }
     CU(cudaGraphLaunch(it->second.exec, h->stream));
     h->launches += it->second.kernels;
@@ -1273,8 +1281,8 @@ int fluid_splats(fluid_t* h, const float* splats, int n) {
         });
         if (rc) return rc;
     }
-    swap_v(h);                                   // S:1449
-    swap_dye(h);                                 // S:1454
+    h->velocity.swap();                          // S:1449
+    h->dye.swap();                               // S:1454
     return FLUID_OK;
 }
 
@@ -1288,85 +1296,46 @@ int fluid_splat(fluid_t* h, float x, float y, float dx, float dy, float r, float
 int fluid_resize(fluid_t* h, int sim_w, int sim_h, int dye_w, int dye_h) {
     if (!h) return FLUID_ERR_INVALID;
     if (sim_w < 1 || sim_h < 1 || dye_w < 1 || dye_h < 1) return fail(h, FLUID_ERR_INVALID, "bad size");
+    const int ow = h->cfg.sim_w, oh = h->cfg.sim_h, odw = h->cfg.dye_w, odh = h->cfg.dye_h;
+    int rc;
     if (h->slab()) {
         // Collective among the ranks of the group (all call it with the same sizes).  The new rows a rank
         // owns sample old rows it owns +- ceil(old/new) + 2: refresh that many ghost rows of the old
-        // velocity and dye, resample into a NEW arena, drop the old one.  Peer mappings die with the old
-        // arena: the group is back on NCCL until the launcher exports / connects again
-        // (distributed.connect_peers).
-        const int ow = h->cfg.sim_w, oh = h->cfg.sim_h, odw = h->cfg.dye_w, odh = h->cfg.dye_h;
+        // velocity and dye.
         const int need_v = (oh + sim_h - 1) / sim_h + 2, need_d = (odh + dye_h - 1) / dye_h + 2;
         if (need_v > h->G || need_d > h->Gd)
             return fail(h, FLUID_ERR_HALO, "resize by this factor needs %d / %d ghost rows, the slab keeps %d / %d", need_v, need_d, h->G, h->Gd);
-        int rc;
-        if ((rc = exchange_rows(h, HB_VELOCITY, h->velocity.read, (size_t)ow * sizeof(float2), h->roff, h->row0, h->row1, need_v))) return rc;
-        if ((rc = exchange_rows(h, HB_DYE, h->dye.read, (size_t)odw * sizeof(float4), h->droff, h->drow0, h->drow1, need_d))) return rc;
-        CU(cudaStreamSynchronize(h->stream));
-        // keep the old arena alive while the new one is filled
-        char* old_arena = h->arena; const float2* old_v = (const float2*)h->velocity.read; const float4* old_d = (const float4*)h->dye.read;
-        const int old_roff = h->roff, old_droff = h->droff;
-        for (auto& p : h->peer) if (p.present && p.base) { cudaIpcCloseMemHandle(p.base); p.base = nullptr; p.present = false; }
-        h->p2p = false;
-        h->arena = nullptr;
-        h->cfg.sim_w = sim_w; h->cfg.sim_h = sim_h; h->cfg.dye_w = dye_w; h->cfg.dye_h = dye_h;
-        if (!slab_geometry(h, sim_h, dye_h, h->cfg.pressure_iterations)) {
-            cudaFree(old_arena);
-            return fail(h, FLUID_ERR_INVALID, "new slabs of %d rows are too short for a 14-row halo", sim_h / h->world);
-        }
-        cudaFree(h->tiny_map); h->tiny_map = nullptr;
-        if ((rc = alloc_fields(h))) { cudaFree(old_arena); return rc; }
-        dim3 b(64, 4);
-        resample_kernel<StoreF32><<<grid2d(sim_w, h->row1 - h->row0, b), b, 0, h->stream>>>(old_v, ow, oh, old_roff, (float2*)h->velocity.read,
-                                                                                             sim_w, sim_h, h->roff, h->row0, h->row1);
-        resample_kernel<StoreF32><<<grid2d(dye_w, h->drow1 - h->drow0, b), b, 0, h->stream>>>(old_d, odw, odh, old_droff, (float4*)h->dye.read,
-                                                                                               dye_w, dye_h, h->droff, h->drow0, h->drow1);
-        rc = check_launch(h, "resample_kernel", 2);
-        CU(cudaStreamSynchronize(h->stream));
-        cudaFree(old_arena);
-        h->v_ghost_valid = false;                            // the +-3 velocity ghost rows are rebuilt by the next step
-        return rc;
+        if ((rc = exchange_rows(h, HB_VELOCITY, need_v))) return rc;
+        if ((rc = exchange_rows(h, HB_DYE, need_d))) return rc;
     }
-    CU(cudaStreamSynchronize(h->stream));
-    drop_graphs(h);                                          // graphs hold the old buffers' addresses
-    // velocity and dye: the LINEAR copy of the old texture, written to the new one in the storage format
-    // (in half storage the reference's blit into an RG16F / RGBA16F target rounds to fp16)
-    const int ow = h->cfg.sim_w, oh = h->cfg.sim_h, odw = h->cfg.dye_w, odh = h->cfg.dye_h;
-    const size_t n = (size_t)sim_w * sim_h, nd = (size_t)dye_w * dye_h;
-    int rc = with_storage(h, [&](auto s) -> int {
+    SlabGeometry g;
+    if (!slab_geometry(&g, h->rank, h->world, sim_h, dye_h, h->cfg.pressure_iterations))
+        return fail(h, FLUID_ERR_INVALID, "new slabs of %d rows are too short for a 14-row halo", sim_h / h->world);
+    // the new arena first: if it does not fit, the handle stays as it was
+    const FieldLayout L = field_layout(h, (size_t)sim_w * g.lrows(), (size_t)dye_w * g.ldrows());
+    char* a = nullptr;
+    if ((rc = make_arena(h, L, (size_t)dye_w * g.ldrows(), &a))) return rc;
+    // velocity and dye of the rows this rank owns, into the slots their pairs read next; pressure, divergence
+    // and curl start over at zero
+    rc = with_storage(h, [&](auto s) {
         using S = decltype(s);
-        typedef typename S::T2 V;
-        typedef typename S::T4 D;
-        dim3 b(64, 4);
-        if (dye_w != odw || dye_h != odh) {
-            void *nr = nullptr, *nw = nullptr;
-            CU(cudaMalloc(&nr, nd * dbytes(h)));
-            CU(cudaMalloc(&nw, nd * dbytes(h)));
-            resample_kernel<S><<<grid2d(dye_w, dye_h, b), b, 0, h->stream>>>((const D*)h->dye.read, odw, odh, 0, (D*)nr, dye_w, dye_h, 0, 0, dye_h);
-            fill_alpha_kernel<S><<<(unsigned)((nd + 255) / 256), 256, 0, h->stream>>>((D*)nw, nd);
-            int rc = check_launch(h, "resample_kernel", 2); if (rc) return rc;
-            CU(cudaStreamSynchronize(h->stream));
-            cudaFree(h->dye.read); cudaFree(h->dye.write);
-            h->dye.read = nr; h->dye.write = nw;
-        }
-        if (sim_w != ow || sim_h != oh) {
-            void *nr = nullptr, *nw = nullptr;
-            CU(cudaMalloc(&nr, n * vbytes(h)));
-            CU(cudaMalloc(&nw, n * vbytes(h)));
-            resample_kernel<S><<<grid2d(sim_w, sim_h, b), b, 0, h->stream>>>((const V*)h->velocity.read, ow, oh, 0, (V*)nr, sim_w, sim_h, 0, 0, sim_h);
-            int rc = check_launch(h, "resample_kernel"); if (rc) return rc;
-            CU(cudaMemsetAsync(nw, 0, n * vbytes(h), h->stream));
-            CU(cudaStreamSynchronize(h->stream));
-            cudaFree(h->velocity.read); cudaFree(h->velocity.write);
-            h->velocity.read = nr; h->velocity.write = nw;
-        }
-        return FLUID_OK;
+        const int r = carry_field<S, typename S::T2>(h, h->velocity.read, ow, oh, h->roff, a + L.v[h->velocity.par],
+                                                     sim_w, sim_h, g.roff, g.row0, g.row1);
+        return r ? r : carry_field<S, typename S::T4>(h, h->dye.read, odw, odh, h->droff, a + L.dye[h->dye.par],
+                                                       dye_w, dye_h, g.droff, g.drow0, g.drow1);
     });
-    if (rc) return rc;
+    const cudaError_t e = cudaStreamSynchronize(h->stream);
+    if (!rc && e != cudaSuccess) rc = fail(h, FLUID_ERR_CUDA, "resize of the fields failed: %s", cudaGetErrorString(e));
+    if (rc) { cudaFree(a); return rc; }
+    drop_graphs(h);                                          // graphs hold the old buffers' addresses
+    // slab: the neighbours' mappings die with the old arena, so the group is back on NCCL until the launcher
+    // exports / connects again (distributed.connect_peers); the +-3 velocity ghost rows are rebuilt by the next step
+    close_peers(h);
+    h->v_ghost_valid = false;
+    cudaFree(h->arena);
     h->cfg.sim_w = sim_w; h->cfg.sim_h = sim_h; h->cfg.dye_w = dye_w; h->cfg.dye_h = dye_h;
-    h->row0 = 0; h->row1 = sim_h; h->drow0 = 0; h->drow1 = dye_h; h->roff = 0; h->droff = 0;
-    if ((rc = alloc_scalar_fields(h))) return rc;
-    if ((rc = alloc_tiny_map(h))) return rc;
-    return build_tmaps(h);
+    static_cast<SlabGeometry&>(*h) = g;
+    return adopt_arena(h, a, L);
 }
 
 // ---- data in / out --------------------------------------------------------------------------------
@@ -1501,7 +1470,7 @@ int solve_host_banded(fluid_t* h, const float* div_host, float* p_host, int iter
         const size_t o = (size_t)b_lo * W;
         CU(cudaMemcpyAsync(p_host + o, result + o, (size_t)(b_hi - b_lo) * W * sizeof(float), cudaMemcpyDeviceToHost, hp.down));
     }
-    swap_p(h);                                            // pressure.read = the result, like S:1265 after the loop
+    h->pressure.swap();                                   // pressure.read = the result, like S:1265 after the loop
     CU(cudaStreamSynchronize(hp.down));
     CU(cudaStreamSynchronize(h->stream));
     return FLUID_OK;
@@ -1780,9 +1749,7 @@ static int draw(fluid_t* h, const DrawRequest& r) {
         // the band's display + shading taps reach ceil(Hd / height) + 2 dye rows beyond the owned ones:
         // refresh that many ghost rows (the ghost rows of dye.read are stale after advection)
         const int need = (h->cfg.dye_h + r.height - 1) / r.height + 2;
-        if ((rc = exchange_rows(h, HB_DYE, h->dye.read, (size_t)h->cfg.dye_w * sizeof(float4), h->droff, h->drow0, h->drow1,
-                                std::min(h->Gd, need))))
-            return rc;
+        if ((rc = exchange_rows(h, HB_DYE, std::min(h->Gd, need)))) return rc;
         if (need > h->Gd)
             return fail(h, FLUID_ERR_HALO, "render target of %d rows needs %d dye ghost rows, the slab keeps %d", r.height, need, h->Gd);
     }

@@ -5,14 +5,27 @@
 
 // ---- halo exchange (NCCL point-to-point; all buffers and both neighbours in ONE group) ------------
 // For each item: sends my top `n` owned rows up and my bottom `n` owned rows down, receives the
-// neighbours' rows into my ghost rows.  `base` is local row 0 of a buffer whose local row 0 is
-// global row `off`.  Halo messages are latency-bound (a 4096-float row is 16 KiB), so everything
-// that can travel together does.
-// `which` names the buffer for the peer-memory path: 0 velocity.read, 1 pressure.read, 2 dye.read,
-// 3 divergence (the neighbour's copy of the same buffer is found through its exported offsets and
-// the SPMD-identical swap parity).
+// neighbours' rows into my ghost rows.  Halo messages are latency-bound (a 4096-float row is 16 KiB),
+// so everything that can travel together does.
+// `which` names the buffer: velocity.read, pressure.read, dye.read or divergence.
 enum { HB_VELOCITY = 0, HB_PRESSURE = 1, HB_DYE = 2, HB_DIVERGENCE = 3 };
-struct HaloItem { void* base; size_t row_bytes; int off, r0, r1, n; int which; };
+struct HaloItem { int which, n; };
+
+// Buffer `which` in the arena of `side` (this rank's own, or a neighbour's mapped through CUDA IPC): local
+// row 0 at `base`, which is global row `off`.  The neighbour's copy of a pair's .read is in the same slot as
+// mine (SPMD-identical swap parity).  r0, r1: the rows THIS rank owns in that grid.
+struct HaloRows { char* base; size_t row_bytes; int off, r0, r1; };
+HaloRows halo_rows(const fluid_t* h, const fluid::Peer& side, int which) {
+    const FieldLayout& L = side.layout;
+    const size_t W = h->cfg.sim_w, Wd = h->cfg.dye_w;
+    switch (which) {
+        case HB_VELOCITY: return {side.base + L.v[h->velocity.par], W * sizeof(float2), side.roff, h->row0, h->row1};
+        case HB_PRESSURE: return {side.base + L.p[h->pressure.par], W * sizeof(float), side.roff, h->row0, h->row1};
+        case HB_DYE: return {side.base + L.dye[h->dye.par], Wd * sizeof(float4), side.droff, h->drow0, h->drow1};
+        default: return {side.base + L.div, W * sizeof(float), side.roff, h->row0, h->row1};
+    }
+}
+fluid::Peer own_arena(const fluid_t* h) { return {true, h->arena, h->roff, h->droff, h->layout}; }
 
 struct ScanArgs { const float* div; unsigned char* map; int W, row_off, lo0, hi0, lo1, hi1; };
 struct PushSeg { const float4* src; float4* dst; unsigned long long n4; };
@@ -103,33 +116,28 @@ __global__ void __launch_bounds__(256) halo_push_kernel(PushArgs a) {
 int exchange_p2p(fluid_t* h, const HaloItem* it, int count) {
     PushArgs pa{};
     pa.seq = ++h->p2p_seq;
-    pa.my_flags = (unsigned*)(h->arena + h->off_flags);
+    pa.my_flags = (unsigned*)(h->arena + h->layout.flags);
     pa.counter = pa.my_flags + 8;
     pa.err = h->halo_flag;
     unsigned long long total4 = 0;
     for (int side = 0; side < 2; ++side) {
-        pa.present[side] = h->peer[side].present ? 1 : 0;
-        pa.peer_flags[side] = h->peer[side].present ? (unsigned*)(h->peer[side].base + h->peer[side].off_flags) : nullptr;
+        const fluid::Peer& P = h->peer[side];
+        pa.present[side] = P.present ? 1 : 0;
+        pa.peer_flags[side] = P.present ? (unsigned*)(P.base + P.layout.flags) : nullptr;
     }
     for (int k = 0; k < count; ++k) {
         const HaloItem& q = it[k];
         if (q.n <= 0) continue;
+        const HaloRows me = halo_rows(h, own_arena(h), q.which);
         for (int side = 0; side < 2; ++side) {
-            const fluid::Peer& P = h->peer[side];
-            if (!P.present) continue;
-            size_t poff; int proff;
-            switch (q.which) {
-                case HB_VELOCITY: poff = P.off_v[h->par_v]; proff = P.roff; break;
-                case HB_PRESSURE: poff = P.off_p[h->par_p]; proff = P.roff; break;
-                case HB_DYE: poff = P.off_dye[h->par_dye]; proff = P.droff; break;
-                default: poff = P.off_div; proff = P.roff; break;
-            }
-            const int g0 = (side == 1) ? q.r1 - q.n : q.r0;          // my owned rows that the neighbour needs
-            const char* src = (const char*)q.base + (size_t)(g0 - q.off) * q.row_bytes;
-            char* dst = P.base + poff + (size_t)(g0 - proff) * q.row_bytes;
+            if (!h->peer[side].present) continue;
+            const HaloRows nb = halo_rows(h, h->peer[side], q.which);
+            const int g0 = (side == 1) ? me.r1 - q.n : me.r0;         // my owned rows that the neighbour needs
+            const char* src = me.base + (size_t)(g0 - me.off) * me.row_bytes;
+            char* dst = nb.base + (size_t)(g0 - nb.off) * me.row_bytes;
             if (pa.count >= 8) return fail(h, FLUID_ERR_INVALID, "too many halo segments");
             PushSeg& sg = pa.seg[pa.count++];
-            sg.src = (const float4*)src; sg.dst = (float4*)dst; sg.n4 = (unsigned long long)q.n * q.row_bytes / 16;
+            sg.src = (const float4*)src; sg.dst = (float4*)dst; sg.n4 = (unsigned long long)q.n * me.row_bytes / 16;
             total4 = std::max(total4, sg.n4);
         }
     }
@@ -147,26 +155,28 @@ int exchange_p2p(fluid_t* h, const HaloItem* it, int count) {
 
 int exchange_many(fluid_t* h, const HaloItem* it, int count) {
     if (!h->slab()) return FLUID_OK;
-    for (int k = 0; k < count; ++k)
-        if (it[k].n > it[k].r1 - it[k].r0)
+    for (int k = 0; k < count; ++k) {
+        const HaloRows me = halo_rows(h, own_arena(h), it[k].which);
+        if (it[k].n > me.r1 - me.r0)
             return fail(h, FLUID_ERR_HALO, "halo of %d rows exceeds the slab height %d (use fewer GPUs or a taller grid)",
-                        it[k].n, it[k].r1 - it[k].r0);
+                        it[k].n, me.r1 - me.r0);
+    }
     if (h->p2p) return exchange_p2p(h, it, count);
     ncdl::Api& N = ncdl::api();
     int rc = N.GroupStart();
     for (int k = 0; k < count && !rc; ++k) {
         const HaloItem& q = it[k];
         if (q.n <= 0) continue;
-        char* b = static_cast<char*>(q.base);
-        auto at = [&](int grow) { return b + (size_t)(grow - q.off) * q.row_bytes; };
-        const size_t bytes = (size_t)q.n * q.row_bytes;
+        const HaloRows me = halo_rows(h, own_arena(h), q.which);
+        auto at = [&](int grow) { return me.base + (size_t)(grow - me.off) * me.row_bytes; };
+        const size_t bytes = (size_t)q.n * me.row_bytes;
         if (h->rank + 1 < h->world) {
-            if (!rc) rc = N.Send(at(q.r1 - q.n), bytes, ncdl::ncclInt8, h->rank + 1, h->comm, h->stream);
-            if (!rc) rc = N.Recv(at(q.r1), bytes, ncdl::ncclInt8, h->rank + 1, h->comm, h->stream);
+            if (!rc) rc = N.Send(at(me.r1 - q.n), bytes, ncdl::ncclInt8, h->rank + 1, h->comm, h->stream);
+            if (!rc) rc = N.Recv(at(me.r1), bytes, ncdl::ncclInt8, h->rank + 1, h->comm, h->stream);
         }
         if (h->rank > 0) {
-            if (!rc) rc = N.Send(at(q.r0), bytes, ncdl::ncclInt8, h->rank - 1, h->comm, h->stream);
-            if (!rc) rc = N.Recv(at(q.r0 - q.n), bytes, ncdl::ncclInt8, h->rank - 1, h->comm, h->stream);
+            if (!rc) rc = N.Send(at(me.r0), bytes, ncdl::ncclInt8, h->rank - 1, h->comm, h->stream);
+            if (!rc) rc = N.Recv(at(me.r0 - q.n), bytes, ncdl::ncclInt8, h->rank - 1, h->comm, h->stream);
         }
     }
     const int rc2 = N.GroupEnd();
@@ -175,8 +185,8 @@ int exchange_many(fluid_t* h, const HaloItem* it, int count) {
     return FLUID_OK;
 }
 
-int exchange_rows(fluid_t* h, int which, void* base, size_t row_bytes, int off, int r0, int r1, int n) {
-    HaloItem it{base, row_bytes, off, r0, r1, n, which};
+int exchange_rows(fluid_t* h, int which, int n) {
+    const HaloItem it{which, n};
     return exchange_many(h, &it, 1);
 }
 
