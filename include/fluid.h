@@ -87,6 +87,18 @@ typedef enum fluid_param {
                                         up-pass rounds fragment + widened destination once.  The sunrays mask follows
                                         the dye's storage.  HALF_STORAGE | HALF_POSTFX is the reference's desktop frame.
                                         Single GPU; the render() frame stays fp32, host_bloom / host_sunrays widen  */
+#define FLUID_FLAG_NEAREST_FILTERING 0x40u /* the reference on a device without float linear filtering
+                                        (`!ext.supportLinearFiltering`: OES_texture_float_linear on WebGL2,
+                                        OES_texture_half_float_linear on WebGL1, S:127-134): dye and velocity
+                                        (S:990), the bloom FBO and pyramid (S:1017), sunrays and sunraysTemp
+                                        (S:1039) are sampled NEAREST + CLAMP_TO_EDGE, texel clamp(floor(uv * n),
+                                        0, n - 1), by fluid_render*, fluid_capture and fluid_resize's copy
+                                        (resizeFBO S:1108-1114).  The dithering texture stays LINEAR + REPEAT.
+                                        step(), splats, every fluid_pass_* and the host solves do not change:
+                                        the simulation is already the MANUAL_FILTERING path.  The config
+                                        override of S:109-114 (DYE_RESOLUTION 512, SHADING / BLOOM / SUNRAYS
+                                        off) is the host's (default_config).  Combines with HALF_STORAGE and
+                                        HALF_POSTFX; single GPU                                                */
 #define FLUID_FLAG_TILED_PASSES 0x8u /* generation-1 kernels (one thread per fragment / smem tile) for
                                         curl-vorticity-divergence and gradientSubtract instead of the
                                         row-streaming ones (comparison + fallback path)              */

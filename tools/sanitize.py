@@ -52,4 +52,14 @@ s.config.update(BLOOM=True, SUNRAYS=True, SHADING=True, BLOOM_RESOLUTION=64, SUN
 s.dithering = rs.random_sample((64, 64, 3)).astype(np.float32)
 assert np.isfinite(s.render(96, 72)).all()
 s.close()
+# the same frame on a device without float linear filtering: NEAREST dye, bloom, pyramid and sunrays samplers
+s = pkg.FluidSimulation({"PRESSURE_ITERATIONS": 9}, 96, 72, sizes=(96, 72, 144, 108),
+                        flags=pkg.FLAG_HALF_STORAGE | pkg.FLAG_HALF_POSTFX | pkg.FLAG_NEAREST_FILTERING,
+                        random=rs.random_sample)
+s.multipleSplats(2)
+s.step(0.016666)
+s.config.update(BLOOM=True, SUNRAYS=True, SHADING=True, BLOOM_RESOLUTION=64, SUNRAYS_RESOLUTION=48)
+s.dithering = rs.random_sample((64, 64, 3)).astype(np.float32)
+assert np.isfinite(s.render(96, 72)).all()
+s.close()
 print("sanitize run complete")

@@ -36,6 +36,7 @@ PARAM = {"DENSITY_DISSIPATION": 0, "VELOCITY_DISSIPATION": 1, "PRESSURE": 2,
          "PRESSURE_ITERATIONS": 3, "CURL": 4, "SPLAT_RADIUS": 5, "ASPECT": 6, "JACOBI_BLOCK": 7, "BACKGROUND": 8}
 FLAG_UNFUSED, FLAG_NO_GRAPH, FLAG_NAIVE_JACOBI, FLAG_TILED_PASSES, FLAG_HALF_STORAGE = 0x1, 0x2, 0x4, 0x8, 0x10
 FLAG_HALF_POSTFX = 0x20         # fp16 bloom / sunrays targets like the reference's FBOs (include/fluid.h)
+FLAG_NEAREST_FILTERING = 0x40   # NEAREST display / post-FX / resize samplers, the reference without float linear filtering
 # display keywords of render() (updateKeywords, S:1160-1166): FLUID_DISPLAY_* of include/fluid.h
 DISPLAY_SHADING, DISPLAY_BLOOM, DISPLAY_SUNRAYS = 0x1, 0x2, 0x4
 STAT = {"launches": 0, "jacobi_launches": 1, "halo_launches": 2, "halo_exchanges": 3,

@@ -76,6 +76,7 @@ struct fluid : SlabGeometry {
     bool capturing = false;                // inside the stream capture of a step graph
     bool half = false;                     // FLUID_FLAG_HALF_STORAGE: fields are fp16 (half_passes.cuh), single GPU only
     bool half_fx = false;                  // FLUID_FLAG_HALF_POSTFX: the bloom and sunrays targets are fp16, single GPU only
+    bool nearest = false;                  // FLUID_FLAG_NEAREST_FILTERING: display, post-FX and resize sample NEAREST, single GPU only
     float* scratch = nullptr;              // half mode: fp32 staging of fluid_read / fluid_write / render
     size_t scratch_floats = 0;
     float* dt_dev = nullptr;               // step()'s dt lives in device memory: one graph serves every dt
@@ -570,7 +571,8 @@ int alloc_fields(fluid_t* h) {
 }
 
 // One field's rows [j0, j1) of the new grid (Wn x Hn, local row 0 at global row dst_off) from the old grid
-// (W x H, local row 0 at src_off): the LINEAR copy of the old texture written in the storage format (in half
+// (W x H, local row 0 at src_off): the copy of the old texture through its sampler (LINEAR, or NEAREST with
+// FLUID_FLAG_NEAREST_FILTERING: resizeFBO's `filtering`, S:997 / S:1002) written in the storage format (in half
 // storage the reference's blit into an RG16F / RGBA16F target rounds to fp16), or, when the size did not
 // change, the rows as they are — like resizeDoubleFBO, which keeps such a field (S:1116-1126).
 template <class S, class T>
@@ -581,7 +583,10 @@ int carry_field(fluid_t* h, const void* src, int W, int H, int src_off, char* ds
         return FLUID_OK;
     }
     dim3 b(64, 4);
-    resample_kernel<S><<<grid2d(Wn, j1 - j0, b), b, 0, h->stream>>>((const T*)src, W, H, src_off, (T*)dst, Wn, Hn, dst_off, j0, j1);
+    if (h->nearest)
+        resample_kernel<S, Nearest><<<grid2d(Wn, j1 - j0, b), b, 0, h->stream>>>((const T*)src, W, H, src_off, (T*)dst, Wn, Hn, dst_off, j0, j1);
+    else
+        resample_kernel<S, Linear><<<grid2d(Wn, j1 - j0, b), b, 0, h->stream>>>((const T*)src, W, H, src_off, (T*)dst, Wn, Hn, dst_off, j0, j1);
     return check_launch(h, "resample_kernel");
 }
 
@@ -691,6 +696,11 @@ int create_common(const fluid_config* cfg, int rank, int world, const void* uid,
     h->half_fx = (cfg->flags & FLUID_FLAG_HALF_POSTFX) != 0;
     if (h->half_fx && world > 1) {
         int rc = fail(nullptr, FLUID_ERR_INVALID, "FLUID_FLAG_HALF_POSTFX is a single-GPU mode");
+        delete h; return rc;
+    }
+    h->nearest = (cfg->flags & FLUID_FLAG_NEAREST_FILTERING) != 0;
+    if (h->nearest && world > 1) {
+        int rc = fail(nullptr, FLUID_ERR_INVALID, "FLUID_FLAG_NEAREST_FILTERING is a single-GPU mode");
         delete h; return rc;
     }
     if (!slab_geometry(h, rank, world, cfg->sim_h, cfg->dye_h, cfg->pressure_iterations)) {
@@ -1599,9 +1609,10 @@ struct PostFXOut { int bw, bh, sw, sh; };
 // applySunrays + blur(…, 1) (S:1396-1419; the mask is drawn into dye.write exactly like S:1300) with
 // SUNRAYS.  FBO sizes follow initBloomFramebuffers / initSunraysFramebuffers (S:1012-1043), which size
 // them from the drawing buffer: canvas_w x canvas_h.  Sd: the dye's storage policy (the mask is drawn in
-// it), St: the targets' (postfx.cuh).  Single GPU, arguments checked by the caller.
+// it), St: the targets', Smp: the sampler of every texture the chains read (postfx.cuh).  Single GPU,
+// arguments checked by the caller.
 extern "C++" {
-template <class Sd, class St>
+template <class Sd, class St, class Smp>
 static int post_fx_chains(fluid_t* h, uint32_t keywords, const fluid_postfx* fx, const float* dither_rgb,
                           int dw, int dh, int canvas_w, int canvas_h, PostFXOut* o) {
     using D4 = typename Sd::T4;
@@ -1637,57 +1648,63 @@ static int post_fx_chains(fluid_t* h, uint32_t keywords, const fluid_postfx* fx,
             p += (size_t)pw * ph;
         }
         const double knee = fx->bloom_threshold * fx->bloom_soft_knee + 0.0001;
-        bloom_prefilter_kernel<Sd, St><<<grid2d(bw, bh, b), b, 0, h->stream>>>(
+        bloom_prefilter_kernel<Sd, St, Smp><<<grid2d(bw, bh, b), b, 0, h->stream>>>(
             (const D4*)h->dye.read, Wd, Hd, bloom, bw, bh, (float)(fx->bloom_threshold - knee),
             (float)(knee * 2), (float)(0.25 / knee), (float)fx->bloom_threshold);
         ++nk;
         Lv last{bloom, bw, bh};
         for (auto& d : pyr) {
-            box4_kernel<St><<<grid2d(d.w, d.h, b), b, 0, h->stream>>>(last.p, last.w, last.h, d.p, d.w, d.h, 1.0f, 0);
+            box4_kernel<St, Smp><<<grid2d(d.w, d.h, b), b, 0, h->stream>>>(last.p, last.w, last.h, d.p, d.w, d.h, 1.0f, 0);
             last = d; ++nk;
         }
         for (int i = (int)pyr.size() - 2; i >= 0; --i) {
-            box4_kernel<St><<<grid2d(pyr[i].w, pyr[i].h, b), b, 0, h->stream>>>(last.p, last.w, last.h, pyr[i].p, pyr[i].w, pyr[i].h, 1.0f, 1);
+            box4_kernel<St, Smp><<<grid2d(pyr[i].w, pyr[i].h, b), b, 0, h->stream>>>(last.p, last.w, last.h, pyr[i].p, pyr[i].w, pyr[i].h, 1.0f, 1);
             last = pyr[i]; ++nk;
         }
-        box4_kernel<St><<<grid2d(bw, bh, b), b, 0, h->stream>>>(last.p, last.w, last.h, bloom, bw, bh, (float)fx->bloom_intensity, 0);
+        box4_kernel<St, Smp><<<grid2d(bw, bh, b), b, 0, h->stream>>>(last.p, last.w, last.h, bloom, bw, bh, (float)fx->bloom_intensity, 0);
         ++nk;
     }
     // ---- applySunrays(dye.read, dye.write, sunrays); blur(sunrays, sunraysTemp, 1) -------------------
     if (sun_on) {
-        sunrays_mask_kernel<Sd><<<grid2d(Wd, Hd, b), b, 0, h->stream>>>((const D4*)h->dye.read, (D4*)h->dye.write, Wd, Hd);
-        sunrays_kernel<Sd, St><<<grid2d(sw, sh, b), b, 0, h->stream>>>((const D4*)h->dye.write, Wd, Hd, sun, sw, sh, (float)fx->sunrays_weight);
-        blur3_kernel<St><<<grid2d(sw, sh, b), b, 0, h->stream>>>(sun, sun2, sw, sh, (float)(1.0 / (double)sw), 0.0f);
-        blur3_kernel<St><<<grid2d(sw, sh, b), b, 0, h->stream>>>(sun2, sun, sw, sh, 0.0f, (float)(1.0 / (double)sh));
+        sunrays_mask_kernel<Sd, Smp><<<grid2d(Wd, Hd, b), b, 0, h->stream>>>((const D4*)h->dye.read, (D4*)h->dye.write, Wd, Hd);
+        sunrays_kernel<Sd, St, Smp><<<grid2d(sw, sh, b), b, 0, h->stream>>>((const D4*)h->dye.write, Wd, Hd, sun, sw, sh, (float)fx->sunrays_weight);
+        blur3_kernel<St, Smp><<<grid2d(sw, sh, b), b, 0, h->stream>>>(sun, sun2, sw, sh, (float)(1.0 / (double)sw), 0.0f);
+        blur3_kernel<St, Smp><<<grid2d(sw, sh, b), b, 0, h->stream>>>(sun2, sun, sw, sh, 0.0f, (float)(1.0 / (double)sh));
         nk += 4;
     }
     return check_launch(h, "post-FX kernels", nk);
 }
-}  // extern "C++"
 
-// display_kernel<SHADING, BLOOM, SUNRAYS, Out, Sp>, indexed by [Out == StoreCapture][Sp == hs::StoreHalf]
-// [FLUID_DISPLAY_* mask].  The sets without BLOOM and SUNRAYS read no post-FX target: one instantiation.
+// post_fx_chains<Sd, St, Smp> of a handle: the dye's and the targets' storage, and the sampler
+using Chains = int (*)(fluid_t*, uint32_t, const fluid_postfx*, const float*, int, int, int, int, PostFXOut*);
+template <class Smp>
+static Chains chains_for(const fluid_t* h) {
+    return !h->half_fx ? post_fx_chains<StoreF32, StoreF32, Smp>
+         : !h->half    ? post_fx_chains<StoreF32, hs::StoreHalf, Smp>
+                       : post_fx_chains<hs::StoreHalf, hs::StoreHalf, Smp>;
+}
+
+// display_kernel<SHADING, BLOOM, SUNRAYS, Out, Sp, Smp> for the eight FLUID_DISPLAY_* masks.  The sets
+// without BLOOM and SUNRAYS read no post-FX target: one instantiation.
 using DisplayKernel = void (*)(DisplayArgs);
 using F32 = StoreF32;
 using F16 = hs::StoreHalf;
-static const DisplayKernel kDisplay[2][2][8] = {
-    {{display_kernel<false, false, false, StoreFrame, F32>, display_kernel<true, false, false, StoreFrame, F32>,
-      display_kernel<false, true, false, StoreFrame, F32>, display_kernel<true, true, false, StoreFrame, F32>,
-      display_kernel<false, false, true, StoreFrame, F32>, display_kernel<true, false, true, StoreFrame, F32>,
-      display_kernel<false, true, true, StoreFrame, F32>, display_kernel<true, true, true, StoreFrame, F32>},
-     {display_kernel<false, false, false, StoreFrame, F32>, display_kernel<true, false, false, StoreFrame, F32>,
-      display_kernel<false, true, false, StoreFrame, F16>, display_kernel<true, true, false, StoreFrame, F16>,
-      display_kernel<false, false, true, StoreFrame, F16>, display_kernel<true, false, true, StoreFrame, F16>,
-      display_kernel<false, true, true, StoreFrame, F16>, display_kernel<true, true, true, StoreFrame, F16>}},
-    {{display_kernel<false, false, false, StoreCapture, F32>, display_kernel<true, false, false, StoreCapture, F32>,
-      display_kernel<false, true, false, StoreCapture, F32>, display_kernel<true, true, false, StoreCapture, F32>,
-      display_kernel<false, false, true, StoreCapture, F32>, display_kernel<true, false, true, StoreCapture, F32>,
-      display_kernel<false, true, true, StoreCapture, F32>, display_kernel<true, true, true, StoreCapture, F32>},
-     {display_kernel<false, false, false, StoreCapture, F32>, display_kernel<true, false, false, StoreCapture, F32>,
-      display_kernel<false, true, false, StoreCapture, F16>, display_kernel<true, true, false, StoreCapture, F16>,
-      display_kernel<false, false, true, StoreCapture, F16>, display_kernel<true, false, true, StoreCapture, F16>,
-      display_kernel<false, true, true, StoreCapture, F16>, display_kernel<true, true, true, StoreCapture, F16>}},
+template <class Out, class Sp, class Smp>
+struct DisplaySet {
+    static constexpr DisplayKernel k[8] = {
+        display_kernel<false, false, false, Out, F32, Smp>, display_kernel<true, false, false, Out, F32, Smp>,
+        display_kernel<false, true, false, Out, Sp, Smp>,   display_kernel<true, true, false, Out, Sp, Smp>,
+        display_kernel<false, false, true, Out, Sp, Smp>,   display_kernel<true, false, true, Out, Sp, Smp>,
+        display_kernel<false, true, true, Out, Sp, Smp>,    display_kernel<true, true, true, Out, Sp, Smp>};
 };
+// indexed by [sampler == Nearest][Out == StoreCapture][Sp == hs::StoreHalf][FLUID_DISPLAY_* mask]
+static const DisplayKernel* const kDisplay[2][2][2] = {
+    {{DisplaySet<StoreFrame, F32, Linear>::k, DisplaySet<StoreFrame, F16, Linear>::k},
+     {DisplaySet<StoreCapture, F32, Linear>::k, DisplaySet<StoreCapture, F16, Linear>::k}},
+    {{DisplaySet<StoreFrame, F32, Nearest>::k, DisplaySet<StoreFrame, F16, Nearest>::k},
+     {DisplaySet<StoreCapture, F32, Nearest>::k, DisplaySet<StoreCapture, F16, Nearest>::k}},
+};
+}  // extern "C++"
 
 // Queues the copy of n values of a post-FX target into the caller's fp32 array.  An fp16 target goes
 // into `stage` instead, which widen_staged() widens exactly once the stream has synchronised: no launch.
@@ -1755,9 +1772,7 @@ static int draw(fluid_t* h, const DrawRequest& r) {
     }
     PostFXOut o{};
     if (postfx) {
-        const auto chains = !h->half_fx ? post_fx_chains<StoreF32, StoreF32>
-                          : !h->half    ? post_fx_chains<StoreF32, hs::StoreHalf>
-                                        : post_fx_chains<hs::StoreHalf, hs::StoreHalf>;
+        const Chains chains = h->nearest ? chains_for<Nearest>(h) : chains_for<Linear>(h);
         if ((rc = chains(h, r.keywords, r.fx, r.dither, r.dw, r.dh, r.canvas_w, r.canvas_h, &o))) return rc;
     }
     const float4* dye_src;
@@ -1770,7 +1785,7 @@ static int draw(fluid_t* h, const DrawRequest& r) {
                         sun_on ? h->pfx.sun : nullptr, o.sw, o.sh, bloom_on ? h->pfx.dither : nullptr, r.dw, r.dh,
                         h->frame, r.width, r.height, y0, y1, r.back[0], r.back[1], r.back[2], r.bg_mode, h->cfg.aspect, ts};
     dim3 b(32, 8);
-    kDisplay[r.capture][h->half_fx][r.keywords]<<<grid2d(r.width, y1 - y0, b), b, 0, h->stream>>>(a);
+    kDisplay[h->nearest][r.capture][h->half_fx][r.keywords]<<<grid2d(r.width, y1 - y0, b), b, 0, h->stream>>>(a);
     if ((rc = check_launch(h, "display_kernel"))) return rc;
     CU(cudaMemcpyAsync(r.host, h->frame, r.n * (r.capture ? 1 : sizeof(float)), cudaMemcpyDeviceToHost, h->stream));
     std::vector<__half> bloom16, sun16;

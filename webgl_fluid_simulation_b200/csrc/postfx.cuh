@@ -4,8 +4,10 @@
 // keyword sets, drawn over the background into the fp32 frame of render() or the 8-bit image of
 // captureScreenshot.
 //
-// Every kernel is one reference blit: one thread per target texel, sources fetched through the
-// GL_LINEAR formula of passes.cuh (linear_fetch).  Arithmetic order follows the GLSL; with the
+// Every kernel is one reference blit: one thread per target texel, sources fetched through the sampler
+// policy Smp of passes.cuh: Linear (the GL_LINEAR formula, linear_fetch) or, with
+// FLUID_FLAG_NEAREST_FILTERING, Nearest (nearest_fetch).  The dithering texture is LINEAR + REPEAT
+// either way (createTextureAsync S:1131-1134).  Arithmetic order follows the GLSL; with the
 // library's --fmad=false / IEEE div+sqrt build everything is bit-identical to the CPU oracle except
 // the display's pow() (linearToGamma), which is tolerance-checked like splat's exp().
 #pragma once
@@ -36,17 +38,19 @@ __device__ __forceinline__ float linear_fetch_rgb_r_repeat(const float* __restri
 // hs::StoreHalf): Sd is the dye's, which the sunrays mask shares because it is drawn into dye.write;
 // St is the bloom FBO's, the pyramid's and the sunrays FBOs' (FLUID_FLAG_HALF_POSTFX: fp16, every
 // blit's fp32 result rounded to nearest even when it is stored, like the reference's RGBA16F / R16F
-// targets).  Fetches widen the stored texels exactly and run the same fp32 LINEAR arithmetic.
+// targets).  Fetches widen the stored texels exactly and run the same fp32 LINEAR arithmetic.  Smp is
+// the sampler of every texture a chain reads (S:1017, S:1039: the filter of dye, bloom, pyramid and
+// sunrays follows ext.supportLinearFiltering).
 
 // bloomPrefilterShader S:614-631
-template <class Sd, class St>
+template <class Sd, class St, class Smp>
 __global__ void __launch_bounds__(256) bloom_prefilter_kernel(const typename Sd::T4* __restrict__ dye, int Wd, int Hd,
                                                               typename St::T4* __restrict__ out, int w, int h, float curve0,
                                                               float curve1, float curve2, float threshold) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y * blockDim.y + threadIdx.y;
     if (i >= w || j >= h) return;
     const float uvx = ((float)i + 0.5f) / (float)w, uvy = ((float)j + 0.5f) / (float)h;
-    const float4 c = linear_fetch<Sd>(dye, Wd, Hd, uvx, uvy);
+    const float4 c = Smp::template fetch<Sd>(dye, Wd, Hd, uvx, uvy);
     const float br = fmaxf(c.x, fmaxf(c.y, c.z));
     float rq = fminf(fmaxf(br - curve0, 0.0f), curve1);
     rq = (curve2 * rq) * rq;
@@ -56,15 +60,15 @@ __global__ void __launch_bounds__(256) bloom_prefilter_kernel(const typename Sd:
 
 // bloomBlurShader S:633-651 / bloomFinalShader S:653-674; add = blendFunc(ONE, ONE) (S:1374-1375): the
 // fragment plus the widened destination texel, rounded once by the store
-template <class St>
+template <class St, class Smp>
 __global__ void __launch_bounds__(256) box4_kernel(const typename St::T4* __restrict__ src, int ws, int hs,
                                                    typename St::T4* __restrict__ dst, int w, int h, float scale, int add) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y * blockDim.y + threadIdx.y;
     if (i >= w || j >= h) return;
     const float tsx = (float)(1.0 / (double)ws), tsy = (float)(1.0 / (double)hs);
     const float uvx = ((float)i + 0.5f) / (float)w, uvy = ((float)j + 0.5f) / (float)h;
-    const float4 L = linear_fetch<St>(src, ws, hs, uvx - tsx, uvy), R = linear_fetch<St>(src, ws, hs, uvx + tsx, uvy);
-    const float4 T = linear_fetch<St>(src, ws, hs, uvx, uvy + tsy), B = linear_fetch<St>(src, ws, hs, uvx, uvy - tsy);
+    const float4 L = Smp::template fetch<St>(src, ws, hs, uvx - tsx, uvy), R = Smp::template fetch<St>(src, ws, hs, uvx + tsx, uvy);
+    const float4 T = Smp::template fetch<St>(src, ws, hs, uvx, uvy + tsy), B = Smp::template fetch<St>(src, ws, hs, uvx, uvy - tsy);
     float4 s;
     s.x = ((((0.0f + L.x) + R.x) + T.x) + B.x) * 0.25f * scale;
     s.y = ((((0.0f + L.y) + R.y) + T.y) + B.y) * 0.25f * scale;
@@ -76,20 +80,20 @@ __global__ void __launch_bounds__(256) box4_kernel(const typename St::T4* __rest
 }
 
 // sunraysMaskShader S:676-691 (target = dye.write, like the reference: S:1300, so stored as the dye is)
-template <class Sd>
+template <class Sd, class Smp>
 __global__ void __launch_bounds__(256) sunrays_mask_kernel(const typename Sd::T4* __restrict__ dye,
                                                            typename Sd::T4* __restrict__ mask, int Wd, int Hd) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y * blockDim.y + threadIdx.y;
     if (i >= Wd || j >= Hd) return;
     const float uvx = ((float)i + 0.5f) / (float)Wd, uvy = ((float)j + 0.5f) / (float)Hd;
-    float4 c = linear_fetch<Sd>(dye, Wd, Hd, uvx, uvy);
+    float4 c = Smp::template fetch<Sd>(dye, Wd, Hd, uvx, uvy);
     const float br = fmaxf(c.x, fmaxf(c.y, c.z));
     c.w = 1.0f - fminf(fmaxf(br * 20.0f, 0.0f), 0.8f);
     Sd::st(mask, (size_t)j * Wd + i, c);
 }
 
 // sunraysShader S:693-724
-template <class Sd, class St>
+template <class Sd, class St, class Smp>
 __global__ void __launch_bounds__(256) sunrays_kernel(const typename Sd::T4* __restrict__ mask, int Wm, int Hm,
                                                       typename St::T1* __restrict__ out, int w, int h, float weight) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y * blockDim.y + threadIdx.y;
@@ -101,11 +105,11 @@ __global__ void __launch_bounds__(256) sunrays_kernel(const typename Sd::T4* __r
     float dx = uvx - 0.5f, dy = uvy - 0.5f;
     dx = dx * f; dy = dy * f;
     float illum = 1.0f;
-    float color = linear_fetch<Sd>(mask, Wm, Hm, uvx, uvy).w;
+    float color = Smp::template fetch<Sd>(mask, Wm, Hm, uvx, uvy).w;
 #pragma unroll 1
     for (int k = 0; k < 16; ++k) {
         cx = cx - dx; cy = cy - dy;
-        const float col = linear_fetch<Sd>(mask, Wm, Hm, cx, cy).w;
+        const float col = Smp::template fetch<Sd>(mask, Wm, Hm, cx, cy).w;
         color = color + (col * illum) * weight;
         illum = illum * Decay;
     }
@@ -113,16 +117,16 @@ __global__ void __launch_bounds__(256) sunrays_kernel(const typename Sd::T4* __r
 }
 
 // blurShader S:478-494 + blurVertexShader S:461-476 on the one-channel sunrays texture
-template <class St>
+template <class St, class Smp>
 __global__ void __launch_bounds__(256) blur3_kernel(const typename St::T1* __restrict__ src, typename St::T1* __restrict__ dst,
                                                     int w, int h, float tsx, float tsy) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y * blockDim.y + threadIdx.y;
     if (i >= w || j >= h) return;
     const float off = 1.33333333f;
     const float uvx = ((float)i + 0.5f) / (float)w, uvy = ((float)j + 0.5f) / (float)h;
-    const float c = linear_fetch<St>(src, w, h, uvx, uvy);
-    const float l = linear_fetch<St>(src, w, h, uvx - tsx * off, uvy - tsy * off);
-    const float r = linear_fetch<St>(src, w, h, uvx + tsx * off, uvy + tsy * off);
+    const float c = Smp::template fetch<St>(src, w, h, uvx, uvy);
+    const float l = Smp::template fetch<St>(src, w, h, uvx - tsx * off, uvy - tsy * off);
+    const float r = Smp::template fetch<St>(src, w, h, uvx + tsx * off, uvy + tsy * off);
     float sum = c * 0.29411764f;
     sum = sum + l * 0.35294117f;
     sum = sum + r * 0.35294117f;
@@ -195,9 +199,10 @@ struct DisplayArgs {
 
 // displayShaderSource S:549-612 compiled with the keywords updateKeywords picks (S:1160-1166), over
 // the background of render() (blend_over_background).  Out: the output policy; Sp: the storage policy
-// of the bloom and sunrays targets (post_fx_chains' St).  A slab rank draws the band [y0, y1) of the
+// of the bloom and sunrays targets (post_fx_chains' St); Smp: the sampler of the dye, bloom and sunrays
+// taps (the dithering tap is LINEAR + REPEAT whatever Smp is).  A slab rank draws the band [y0, y1) of the
 // target from its own dye rows (+ ghost rows); one GPU draws the whole target.
-template <bool SHADING, bool BLOOM, bool SUNRAYS, class Out, class Sp>
+template <bool SHADING, bool BLOOM, bool SUNRAYS, class Out, class Sp, class Smp>
 __global__ void __launch_bounds__(256) display_kernel(DisplayArgs a) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x, j = a.y0 + blockIdx.y * blockDim.y + threadIdx.y;
     if (i >= a.w || j >= a.y1) return;
@@ -207,13 +212,13 @@ __global__ void __launch_bounds__(256) display_kernel(DisplayArgs a) {
     // (the capture instantiation spills otherwise)
     typename Out::T* const o = static_cast<typename Out::T*>(a.out) + (size_t)Out::row(j - a.y0, a.y1 - a.y0) * a.w + i;
     const float uvx = ((float)i + 0.5f) / (float)a.w, uvy = ((float)j + 0.5f) / (float)a.h;
-    const float4 c = linear_fetch(a.dye, a.Wd, a.Hd, uvx, uvy, a.dye_row_off);
+    const float4 c = Smp::fetch(a.dye, a.Wd, a.Hd, uvx, uvy, a.dye_row_off);
     float cc[3] = {c.x, c.y, c.z};
     if constexpr (SHADING) {
-        const float4 lc = linear_fetch(a.dye, a.Wd, a.Hd, uvx - tsx, uvy, a.dye_row_off);
-        const float4 rc = linear_fetch(a.dye, a.Wd, a.Hd, uvx + tsx, uvy, a.dye_row_off);
-        const float4 tc = linear_fetch(a.dye, a.Wd, a.Hd, uvx, uvy + tsy, a.dye_row_off);
-        const float4 bc = linear_fetch(a.dye, a.Wd, a.Hd, uvx, uvy - tsy, a.dye_row_off);
+        const float4 lc = Smp::fetch(a.dye, a.Wd, a.Hd, uvx - tsx, uvy, a.dye_row_off);
+        const float4 rc = Smp::fetch(a.dye, a.Wd, a.Hd, uvx + tsx, uvy, a.dye_row_off);
+        const float4 tc = Smp::fetch(a.dye, a.Wd, a.Hd, uvx, uvy + tsy, a.dye_row_off);
+        const float4 bc = Smp::fetch(a.dye, a.Wd, a.Hd, uvx, uvy - tsy, a.dye_row_off);
         const float dx = len3(rc) - len3(lc), dy = len3(tc) - len3(bc);
         const float nz = sqrtf(tsx * tsx + tsy * tsy);
         const float nl = sqrtf((dx * dx + dy * dy) + nz * nz);
@@ -224,11 +229,11 @@ __global__ void __launch_bounds__(256) display_kernel(DisplayArgs a) {
     }
     float bl[3] = {0.0f, 0.0f, 0.0f};
     if constexpr (BLOOM) {
-        const float4 b = linear_fetch<Sp>(static_cast<const typename Sp::T4*>(a.bloom), a.bw, a.bh, uvx, uvy);
+        const float4 b = Smp::template fetch<Sp>(static_cast<const typename Sp::T4*>(a.bloom), a.bw, a.bh, uvx, uvy);
         bl[0] = b.x; bl[1] = b.y; bl[2] = b.z;
     }
     if constexpr (SUNRAYS) {
-        const float s = linear_fetch<Sp>(static_cast<const typename Sp::T1*>(a.sun), a.sw, a.sh, uvx, uvy);
+        const float s = Smp::template fetch<Sp>(static_cast<const typename Sp::T1*>(a.sun), a.sw, a.sh, uvx, uvy);
 #pragma unroll
         for (int k = 0; k < 3; ++k) {
             cc[k] = cc[k] * s;

@@ -30,7 +30,8 @@ const PARAM = {
 };
 // display keywords of render() (updateKeywords, S:1160-1166): FLUID_DISPLAY_* of include/fluid.h
 const DISPLAY = { SHADING: 0x1, BLOOM: 0x2, SUNRAYS: 0x4 };
-const FLAG = { UNFUSED: 0x1, NO_GRAPH: 0x2, NAIVE_JACOBI: 0x4, TILED_PASSES: 0x8, HALF_STORAGE: 0x10, HALF_POSTFX: 0x20 };
+const FLAG = { UNFUSED: 0x1, NO_GRAPH: 0x2, NAIVE_JACOBI: 0x4, TILED_PASSES: 0x8, HALF_STORAGE: 0x10, HALF_POSTFX: 0x20,
+               NEAREST_FILTERING: 0x40 };
 const STAT = { launches: 0, jacobiLaunches: 1, haloLaunches: 2, haloExchanges: 3, graphCaptures: 4, graphLaunches: 5, haloTransportP2P: 6,
                cvdStreamLaunches: 7, gradientStreamLaunches: 8, jacobiExactStreams: 9 };
 
@@ -99,7 +100,10 @@ class FluidSimulation {
             SUNRAYS: false,         // reference default is true
             SUNRAYS_RESOLUTION: 196,
             SUNRAYS_WEIGHT: 1.0,
-        }, config);
+        },
+        // a device without float linear filtering (S:109-114); the caller's keys win, as later GUI edits do
+        (options.flags || 0) & FLAG.NEAREST_FILTERING ? { DYE_RESOLUTION: 512, SHADING: false, BLOOM: false, SUNRAYS: false } : {},
+        config);
         this.dithering = null;                                  // {width, height, data: Float32Array RGB}, LDR_LLL1_0.png / 255
         this.canvas = canvas;
         this.random = options.random || Math.random;            // injectable for reproducible runs

@@ -32,10 +32,12 @@ from . import _lib
 from ._lib import DISPLAY_BLOOM, DISPLAY_SHADING, DISPLAY_SUNRAYS, FIELD, PARAM, STAT, Config, FluidError, PostFX, Timing
 
 
-def default_config() -> dict:
+def default_config(flags: int = 0) -> dict:
     """The simulation keys of the reference `config` literal, S:59-69 + S:73 (render keys are out of
-    scope and kept only so a reference config object can be passed through unchanged)."""
-    return {
+    scope and kept only so a reference config object can be passed through unchanged).  With
+    FLAG_NEAREST_FILTERING in `flags` the reference's override for a device without float linear
+    filtering applies (S:109-114): DYE_RESOLUTION 512, SHADING / BLOOM / SUNRAYS off."""
+    c = {
         "SIM_RESOLUTION": 128,
         "DYE_RESOLUTION": 1024,
         "CAPTURE_RESOLUTION": 512,   # S:62, captureScreenshot's target (S:288)
@@ -62,6 +64,9 @@ def default_config() -> dict:
         "SUNRAYS_RESOLUTION": 196,
         "SUNRAYS_WEIGHT": 1.0,
     }
+    if flags & _lib.FLAG_NEAREST_FILTERING:
+        c.update(DYE_RESOLUTION=512, SHADING=False, BLOOM=False, SUNRAYS=False)
+    return c
 
 
 class Pointer:
@@ -193,7 +198,7 @@ class FluidSimulation:
                  device: int = -1, flags: int = 0, jacobi_block: int = 0, random=None,
                  rank: int = 0, world: int = 1, nccl_uid: bytes | None = None,
                  sizes: tuple | None = None):
-        self.config = default_config()
+        self.config = default_config(flags)          # the caller's keys win, as later GUI edits do
         if config:
             self.config.update(config)
         self.canvas = {"width": int(canvas_width), "height": int(canvas_height)}
