@@ -307,7 +307,7 @@ EncodeTiledFn encode_tiled_fn() {
     return fn;
 }
 
-// fp32 field of `rows` x W from `base` as a 2-D tensor map (`tm`: TmapPair::p or ::d); box = 128 columns
+// fp32 field of `rows` x W from `base` as a 2-D tensor map (`tm`: TmapPair::p or ::d); box = TB_BOX columns
 // x 3 rows, no swizzle, out-of-range elements read as zero (the blocked kernel never lets them reach a
 // valid output)
 int encode_rows_map(fluid_t* h, unsigned char (&tm)[128], const void* base, int W, int rows) {
@@ -315,7 +315,7 @@ int encode_rows_map(fluid_t* h, unsigned char (&tm)[128], const void* base, int 
     EncodeTiledFn enc = encode_tiled_fn();
     const cuuint64_t dims[2] = {(cuuint64_t)W, (cuuint64_t)rows};
     const cuuint64_t strides[1] = {(cuuint64_t)W * sizeof(float)};
-    const cuuint32_t box[2] = {128, 3};
+    const cuuint32_t box[2] = {TB_BOX, 3};
     const cuuint32_t estr[2] = {1, 1};
     if (!enc || enc(reinterpret_cast<CUtensorMap*>(tm), CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(base), dims,
                     strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,

@@ -11,9 +11,13 @@
 //       upward over a chunk of rows; no __syncthreads anywhere, warps are independent;
 //     * time level t (t = 0..K-1) lives in a rotating 3-row register window; when level 0 loads
 //       row r, level t produces row r-t, so the K sweeps form a software pipeline in y;
-//     * x-neighbours across lanes come from __shfl_up/down; the two outermost lanes of a level
-//       hold garbage that creeps inward one column per level: HX = roundup(K,4) halo columns on
-//       each side of the window are recomputed by the neighbouring window (overlapped tiling);
+//     * x-neighbours across lanes come from __shfl_up/down.  Lane 0 has no left neighbour and lane 31
+//       no right one: at level 1 they take the level-0 column just outside the window (x0-1, x0+128)
+//       from the staged p box, which is 4 columns wider than the window on each side, so level 1 is
+//       right on all 128 columns; from level 2 on their shuffles return garbage that creeps inward
+//       one column per level.  Level K is wrong in its outer K-1 columns: HX = roundup(K-1,4) halo
+//       columns on each side of the window are recomputed by the neighbouring window (overlapped
+//       tiling);
 //     * CLAMP_TO_EDGE in x is an even reflection p[-1-m] = p[m]; because L+R is the first add of
 //       the expression (commutative) the reflected columns evolve bit-identically, so mirroring
 //       the LOADS implements the boundary for all K levels.  In y the expression is not
@@ -138,21 +142,32 @@ __global__ void __launch_bounds__(256) jacobi_sweep_kernel(JacobiArgs a) {
 //     proof in tests/test_fma_contraction_cpu.py).  A contracted stream tracks the largest level-0
 //     magnitude it loads (fmaxf: NaN drops out, it meets both tails alike; inf counts) and, if that
 //     reached BIG_IN, runs again through the EXACT instantiation, overwriting the rows it stored.
+//     The edge columns that lanes 0 and 31 read for level 1 are level-0 inputs like any other (they
+//     reach valid outputs whenever K-1 is a multiple of 4), so they are folded into the same maximum.
 // 4 lane-ops per update instead of 5 everywhere else, plus 8 FMNMX per row on the ALU pipe.
 //
 // Staging.  p / div rows reach a warp through a shared-memory ring filled by 2-D tensor-map TMA
 // (cp.async.bulk.tensor.2d, SASS UTMALDG): one elected lane arms an mbarrier and fetches a
-// 128-column x 3-row box of p and of div per pipeline block; columns outside the grid and rows
-// outside the mapped buffer are zero-filled by the hardware (never used by a valid output).
+// 136-column x 3-row box of p and of div at x0-4 per pipeline block: the window plus one float4 on
+// each side.  Rows stay 16-byte aligned for every lane's LDS.128, and the edge columns x0-1 and x0+128
+// of p lie inside.  div goes through the same box although its outer columns are never read: at
+// HX = 12 (depths 10-13) rows from x0-4 start on a 32-byte sector of global memory and rows from x0 do
+// not, and where the box starts moved a launch by 3-5 % (DESIGN 5.10).  Columns outside the grid and
+// rows outside the mapped buffer are zero-filled by the hardware (never used by a valid output).
+constexpr int TB_BOX = 136;                          // columns of a staged box: the window and 4 on each side
 template <int K>
 struct TB {
-    static constexpr int HX = (K + 3) / 4 * 4;       // x halo (columns) on each side of a window
+    static constexpr int HX = (K + 2) / 4 * 4;       // x halo (columns) on each side of a window: roundup(K-1, 4)
     static constexpr int VALID = 128 - 2 * HX;       // columns a window produces
     static constexpr int RD = K + 3;                 // div register-ring slots
     static constexpr int U = 3;                      // pipeline steps per unrolled block
-    // NS stages, each a 3-row box of p followed by a 3-row box of div (row = 512 B), then NS mbarriers
+    // NS stages, each a 3-row box of div followed by a 3-row box of p (row = 544 B), each box padded to a
+    // multiple of 128 B, the alignment TMA needs of its destination; then NS mbarriers
     static constexpr int NS = 4;
-    static constexpr int STAGE4 = 2 * U * 32;        // float4 per stage
+    static constexpr int ROW4 = TB_BOX / 4;          // float4 per staged row
+    static constexpr int P4 = (U * ROW4 + 7) / 8 * 8;                   // float4 offset of the p box in a stage
+    static constexpr int TX = 2 * U * ROW4 * (int)sizeof(float4);       // bytes one stage's two boxes bring
+    static constexpr int STAGE4 = 2 * P4;                               // float4 per stage
     static constexpr int SMEM = NS * STAGE4 * (int)sizeof(float4) + NS * 8;
 };
 
@@ -203,20 +218,30 @@ __device__ __forceinline__ float4 lds128(const float4* p) {
     return v;
 }
 
+__device__ __forceinline__ float lds32(const float* p) {
+    float v;
+    const unsigned a = (unsigned)__cvta_generic_to_shared(p);
+    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(a) : "memory");
+    return v;
+}
+
+__device__ __forceinline__ void sts32(const float* p, float v) {
+    const unsigned a = (unsigned)__cvta_generic_to_shared(p);
+    asm volatile("st.shared.f32 [%0], %1;" ::"r"(a), "f"(v) : "memory");
+}
+
 __device__ __forceinline__ float4 rev4(float4 v, bool rev) {
     return rev ? make_float4(v.w, v.z, v.y, v.x) : v;
 }
 
-// one Jacobi update of a float4 of row `c`, with rows below/above and the shuffled neighbours.
+// one Jacobi update of a float4 of row `c`, with rows below/above and the neighbours l / r across lanes.
 //   EXACT:  o = ((((L + R) + below) + above) - d) * 0.25          (d = divergence)
 //   else :  o = fma(((L + R) + below) + above, 0.25, d)           (d = -0.25 * divergence)
 // Every operation is an explicit IEEE round-to-nearest intrinsic, so the result does not depend on
 // the build's --fmad setting: the fma is the only contraction, and it is the one proven exact above.
 template <bool EXACT>
-__device__ __forceinline__ float4 jacobi4(const float4 below, const float4 c, const float4 above,
-                                          const float4 d) {
-    const float l = __shfl_up_sync(0xffffffffu, c.w, 1);
-    const float r = __shfl_down_sync(0xffffffffu, c.x, 1);
+__device__ __forceinline__ float4 jacobi4(const float l, const float r, const float4 below, const float4 c,
+                                          const float4 above, const float4 d) {
     float4 o;
     o.x = __fadd_rn(__fadd_rn(__fadd_rn(l, c.y), below.x), above.x);
     o.y = __fadd_rn(__fadd_rn(__fadd_rn(c.x, c.z), below.y), above.y);
@@ -266,15 +291,22 @@ struct TBTma {           // warp-uniform TMA bookkeeping
 //     the ALU pipe, beside the fp32 pipe that bounds the kernel);
 //   * EDGE instantiates the wall selects in y, REV the mirrored-lane reversal in x, EXACT the
 //     un-contracted tail; all are chosen by warp-uniform branches OUTSIDE the steady-state loop;
+//   * level 1 is the only level whose edge lanes have a real neighbour outside the window: the row it
+//     centres on was staged one step earlier and is still in shared memory (this block's stage, or row 2
+//     of the previous block's, which is refilled only at the end of this block), so lanes 0 and 31
+//     read that row's column x0-1 / x0+128 through `ering` instead of keeping it in a register;
 //   * a contracted block folds the magnitudes of its level-0 inputs into `big` (BIG_IN above).
 template <int K, bool SCALE, bool EDGE, bool REV, bool EXACT>
 __device__ __forceinline__ void tb_block(float4 (&w)[K][3], float4 (&dr)[TB<K>::RD], TBStream& st, float& big,
-                                         const float4* __restrict__ ring, const TBTma& tm, const int W4,
+                                         const float4* __restrict__ ring, const float* __restrict__ ering,
+                                         const TBTma& tm, const int W4,
                                          const int y0, const int y1, const int H,
                                          const bool rev, const bool lane_out, const float scale) {
     using T = TB<K>;
     mbar_wait(tm.bars + st.stg, st.phase, tm.err);
     const float4* srow = ring + st.stg * T::STAGE4;
+    const float* erow = ering + st.stg * (4 * T::STAGE4);
+    const float* erow_prev = ering + ((unsigned)(st.stg + T::NS - 1) % T::NS) * (4 * T::STAGE4) + 2 * TB_BOX;
     // The K levels x 3 steps of a block form a dependency lattice: node (ph, t) needs node
     // (ph, t-1) of the same step (the fresh row above) and rows of level t-1 from the two previous
     // steps.  Source order is step by step; ptxas interleaves the chains itself.
@@ -284,8 +316,8 @@ __device__ __forceinline__ void tb_block(float4 (&w)[K][3], float4 (&dr)[TB<K>::
         for (int t = 0; t <= K; ++t) {
             if (t == 0) {
                 // ---- level 0: the oldest staged row ---------------------------------------------------
-                float4 in = lds128(srow + ph * 32);
-                float4 dv = lds128(srow + (3 + ph) * 32);
+                float4 in = lds128(srow + ph * T::ROW4);
+                float4 dv = lds128(srow - T::P4 + ph * T::ROW4);    // the div box starts P4 float4 below the p box
                 if (REV) { in = rev4(in, rev); dv = rev4(dv, rev); }
                 if (SCALE) {
                     in.x = scale * in.x; in.y = scale * in.y; in.z = scale * in.z; in.w = scale * in.w;
@@ -309,7 +341,16 @@ __device__ __forceinline__ void tb_block(float4 (&w)[K][3], float4 (&dr)[TB<K>::
                     if (r == H - 1) above = c;    //                p[i,H]  = p[i,H-1]
                 }
                 const float4 d = dr[K + ph - t];  // div row staged t steps ago
-                const float4 o = jacobi4<EXACT>(below, c, above, d);
+                float l = __shfl_up_sync(0xffffffffu, c.w, 1);
+                float r = __shfl_down_sync(0xffffffffu, c.x, 1);
+                if (t == 1) {                     // c is level 0: the edge lanes' neighbours are input data
+                    float e = lds32(ph == 0 ? erow_prev : erow + (ph - 1) * TB_BOX);
+                    if (SCALE) e = scale * e;
+                    if (!EXACT) big = fmaxf(big, fabsf(e));
+                    l = (tm.lane == 0) ? e : l;
+                    r = (tm.lane == 31) ? e : r;
+                }
+                const float4 o = jacobi4<EXACT>(l, r, below, c, above, d);
                 if (t < K) {
                     w[t][(ph + 2) % 3] = o;
                 } else if (lane_out && (unsigned)(st.rout + ph - y0) < (unsigned)(y1 - y0)) {
@@ -328,9 +369,9 @@ __device__ __forceinline__ void tb_block(float4 (&w)[K][3], float4 (&dr)[TB<K>::
     if (tm.lane == 0) {
         const int q = (st.stg == 0) ? T::NS - 1 : st.stg - 1;
         float4* dst = tm.slots + q * T::STAGE4;
-        mbar_expect_tx(tm.bars + q, 2u * 3u * 512u);
-        tma_load_2d(dst, tm.tm_p, tm.x0, st.yfill, tm.bars + q);
-        tma_load_2d(dst + 3 * 32, tm.tm_d, tm.x0, st.yfill, tm.bars + q);
+        mbar_expect_tx(tm.bars + q, (unsigned)T::TX);
+        tma_load_2d(dst, tm.tm_d, tm.x0 - 4, st.yfill, tm.bars + q);
+        tma_load_2d(dst + T::P4, tm.tm_p, tm.x0 - 4, st.yfill, tm.bars + q);
     }
     st.yfill += 3;
     if (st.stg + 1 == T::NS) { st.stg = 0; st.phase ^= 1u; } else { ++st.stg; }
@@ -362,15 +403,33 @@ __device__ __forceinline__ float tb_stream(const JacobiArgs& a, const void* tm_p
 
     TBStream st{};
     TBTma tm{};
-    // every lane reads its (mirrored / clamped) column group out of the staged 128-column box.  In the
-    // last window the mirror image of the outermost lanes lies left of the box (x0 > lc); those lanes
-    // feed no output (beyond lane_out and the shuffle cone), so they read the box's first column
-    // instead of shared memory below it.
-    const float4* ring = smem4 + ((min(max(lc, x0), x0 + 124) - x0) >> 2);
+    // every lane reads its (mirrored / clamped) column group out of the window's 128 columns of the
+    // staged boxes.  In the last window the mirror image of the outermost lanes lies left of the window
+    // (x0 > lc); those lanes feed no output (beyond lane_out and the shuffle cone), so they read the
+    // window's first column instead of shared memory below it.  `ring`: this lane's float4 in p row 0
+    // of stage 0 (the boxes start at column x0 - 4).
+    const float4* ring = smem4 + T::P4 + ((min(max(lc, x0), x0 + 124) - (x0 - 4)) >> 2);
+    // `ering`: in the same row, the column lane 0 / lane 31 takes as its outer neighbour at level 1:
+    // x0 - 1 / x0 + 128, mirrored about the walls like lc, and clamped into the box where the image
+    // lies outside it (the last window again: no output depends on it).  The other lanes read a column
+    // of their own group, which changes nothing about `big`.
+    int ec = min(max(lc, x0), x0 + 124);
+    if (lane == 0 || lane == 31) {
+        ec = (lane == 0) ? x0 - 1 : x0 + 128;
+        if (ec < 0) ec = -1 - ec;                              // p[-1-m] = p[m]
+        else if (ec >= W) ec = 2 * W - 1 - ec;                 // p[W+m]  = p[W-1-m]
+        ec = min(max(min(max(ec, 0), W - 1), x0 - 4), x0 + TB_BOX - 5);
+    }
+    const float* ering = reinterpret_cast<const float*>(smem4 + T::P4) + (ec - (x0 - 4));
+    // the first step's level 1 (a dead warm-up node) reads the row "staged one step earlier" from a stage
+    // no box has reached yet: it must not bring whatever shared memory held into `big`
+    sts32(ering + (T::NS - 1) * (4 * T::STAGE4) + 2 * TB_BOX, 0.0f);
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // ordered before the TMA write that refills that stage
     tm.tm_p = tm_p; tm.tm_d = tm_d;
     tm.bars = reinterpret_cast<unsigned long long*>(smem4 + T::NS * T::STAGE4);
     tm.slots = smem4;
-    tm.x0 = x0; tm.lane = lane; tm.err = a.err;
+    tm.x0 = x0; tm.err = a.err;
+    tm.lane = (int)threadIdx.x;                       // == lane (one warp per CTA): nothing to keep live in the out-of-line streams
     st.stg = 0; st.phase = 0;
     st.yfill = ys - a.row_off;
     if (lane == 0) {
@@ -384,9 +443,9 @@ __device__ __forceinline__ float tb_stream(const JacobiArgs& a, const void* tm_p
     for (int q = 0; q < T::NS - 1; ++q) {
         if (lane == 0) {
             float4* dst = tm.slots + q * T::STAGE4;
-            mbar_expect_tx(tm.bars + q, 2u * 3u * 512u);
-            tma_load_2d(dst, tm_p, x0, st.yfill, tm.bars + q);
-            tma_load_2d(dst + 3 * 32, tm_d, x0, st.yfill, tm.bars + q);
+            mbar_expect_tx(tm.bars + q, (unsigned)T::TX);
+            tma_load_2d(dst, tm_d, x0 - 4, st.yfill, tm.bars + q);
+            tma_load_2d(dst + T::P4, tm_p, x0 - 4, st.yfill, tm.bars + q);
         }
         st.yfill += 3;
     }
@@ -400,16 +459,16 @@ __device__ __forceinline__ float tb_stream(const JacobiArgs& a, const void* tm_p
     int s0 = 0;
     float big = 0.0f;
 #pragma unroll 1
-    for (int part = 0; part < 2; ++part) {
+    while (s0 < nsteps) {                             // at most: wall blocks, steady blocks, wall blocks
 #pragma unroll 1
         for (; s0 < nsteps && ((ys + s0 - K <= 0) || (ys + s0 + 2 >= H - 1)); s0 += 3)
-            tb_block<K, SCALE, true, REV, EXACT>(w, dr, st, big, ring, tm, W4, y0, y1, H, rev, lane_out, a.scale);
+            tb_block<K, SCALE, true, REV, EXACT>(w, dr, st, big, ring, ering, tm, W4, y0, y1, H, rev, lane_out, a.scale);
 #pragma unroll 1
         for (; s0 < nsteps && !((ys + s0 - K <= 0) || (ys + s0 + 2 >= H - 1)); s0 += 3)
-            tb_block<K, SCALE, false, REV, EXACT>(w, dr, st, big, ring, tm, W4, y0, y1, H, rev, lane_out, a.scale);
+            tb_block<K, SCALE, false, REV, EXACT>(w, dr, st, big, ring, ering, tm, W4, y0, y1, H, rev, lane_out, a.scale);
     }
     // drain the over-fetched tail before the CTA (and its shared memory) goes away
-#pragma unroll 1
+#pragma unroll
     for (int q = 0; q < T::NS - 1; ++q) {
         mbar_wait(tm.bars + st.stg, st.phase, tm.err);
         if (st.stg + 1 == T::NS) { st.stg = 0; st.phase ^= 1u; } else { ++st.stg; }
