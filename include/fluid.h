@@ -238,7 +238,8 @@ int fluid_pressure_solve_host(fluid_t* h, const float* div_host, float* pressure
  * render(target) of S:1296-1317 with config.BLOOM = config.SUNRAYS = false and TRANSPARENT = false —
  * drawColor(BACK_COLOR) (S:1319-1323) then drawDisplay (S:1331-1348, displayShaderSource S:549-612,
  * SHADING keyword when `shading` != 0) blended ONE / ONE_MINUS_SRC_ALPHA.  Writes width*height RGBA
- * floats (row 0 = bottom, not yet quantised to 8 bits) to host memory.  back_* are BACK_COLOR / 255. */
+ * floats (row 0 = bottom, not quantised to 8 bits: fluid_render_canvas draws the RGBA8 canvas) to host
+ * memory.  back_* are BACK_COLOR / 255. */
 int fluid_render(fluid_t* h, int width, int height, int shading, float back_r, float back_g,
                  float back_b, float* host_rgba, size_t n_floats);
 /* On a slab handle fluid_render draws (and returns) only the band of target rows [*y0, *y1) that
@@ -306,6 +307,36 @@ int fluid_render_keywords(fluid_t* h, int width, int height, uint32_t keywords, 
 int fluid_capture(fluid_t* h, int width, int height, int canvas_w, int canvas_h, uint32_t keywords,
                   int transparent, const fluid_postfx* fx, const float* dither_rgb, int dw, int dh,
                   float back_r, float back_g, float back_b, uint8_t* host_rgba8, size_t n_bytes);
+
+/* render(null) of S:1296-1317 on the canvas: what a width x height drawing buffer holds after the frame.
+ * The context is created with alpha: true (S:118-119), so the buffer is RGBA8 unsigned-normalised.  The
+ * post-FX FBOs are sized from width x height as in fluid_render_keywords, and texelSize / ditherScale use
+ * it (S:1332-1344).  FLUID_BACKGROUND is not consulted: on the screen blending is always on.
+ * The rule, per channel, in fp32 with every operation rounded on its own (no contraction):
+ *  - (c, a): the display fragment of fluid_render_keywords before any blend (FLUID_BACKGROUND 2).
+ *  - clamp(x) = min(max(x, 0), 1): NaN gives 0, +inf gives 1.
+ *    u8(x) = clamp(x) * 255 rounded to the nearest integer, ties to even (GLES 3.0 §2.1.6.1).
+ *  - Destination byte d8: u8(back_*) (drawColor(BACK_COLOR), S:1319-1323); with transparent != 0,
+ *    u8(v) of drawCheckerboard (S:1325-1329, v = mod(floor(uv.x * 25 * aspect) + floor(uv.y * 25), 2)
+ *    * 0.1 + 0.8 in fp32, aspect = FLUID_ASPECT).  Alpha byte 255 either way.  d = d8 / 255.0f.
+ *  - blendFunc(ONE, ONE_MINUS_SRC_ALPHA) (S:1305-1306) on a fixed-point buffer clamps first (GLES 3.0
+ *    §4.1.7): out = clamp(c) + d * (1 - clamp(a)); alpha clamp(a) + 1 * (1 - clamp(a)).  Stored u8(out).
+ *  - Rows top row first: the order of ImageData, putImageData and PNG (as fluid_capture).
+ * Destination:
+ *  - dst_on_device == 0: dst is host memory.  One device-to-host copy of n_bytes, then a stream sync.
+ *  - dst_on_device != 0: dst is device or managed memory of the handle's device, 4-byte aligned (for
+ *    example a torch uint8 CUDA tensor).  The display kernel stores into it directly; the call is
+ *    stream-ordered and returns without synchronising, like fluid_step: fluid_sync before reading it.
+ *    The handle's stream is non-blocking: work of other streams that uses dst must be complete first
+ *    (sim.py's render_canvas waits for it).
+ * Refused with FLUID_ERR_INVALID, dst untouched and the handle usable: n_bytes != 4 * width * height;
+ * width or height < 1; unknown keyword bits; BLOOM without dither_rgb; fx == NULL with BLOOM or SUNRAYS;
+ * half-storage handles with BLOOM or SUNRAYS unless created with FLUID_FLAG_HALF_POSTFX; dst_on_device with
+ * host memory, memory of another device, or a misaligned dst; slab handles. */
+int fluid_render_canvas(fluid_t* h, int width, int height, uint32_t keywords, int transparent,
+                        const fluid_postfx* fx, const float* dither_rgb, int dw, int dh,
+                        float back_r, float back_g, float back_b,
+                        uint8_t* dst, size_t n_bytes, int dst_on_device);
 
 int fluid_sync(fluid_t* h);
 int fluid_timing_last(fluid_t* h, fluid_timing* out);

@@ -1697,12 +1697,16 @@ struct DisplaySet {
         display_kernel<false, false, true, Out, Sp, Smp>,   display_kernel<true, false, true, Out, Sp, Smp>,
         display_kernel<false, true, true, Out, Sp, Smp>,    display_kernel<true, true, true, Out, Sp, Smp>};
 };
-// indexed by [sampler == Nearest][Out == StoreCapture][Sp == hs::StoreHalf][FLUID_DISPLAY_* mask]
-static const DisplayKernel* const kDisplay[2][2][2] = {
+// What a draw() produces: the output policy of its display kernel
+enum DisplayOut { OUT_FRAME = 0, OUT_CAPTURE = 1, OUT_CANVAS = 2 };
+// indexed by [sampler == Nearest][DisplayOut][Sp == hs::StoreHalf][FLUID_DISPLAY_* mask]
+static const DisplayKernel* const kDisplay[2][3][2] = {
     {{DisplaySet<StoreFrame, F32, Linear>::k, DisplaySet<StoreFrame, F16, Linear>::k},
-     {DisplaySet<StoreCapture, F32, Linear>::k, DisplaySet<StoreCapture, F16, Linear>::k}},
+     {DisplaySet<StoreCapture, F32, Linear>::k, DisplaySet<StoreCapture, F16, Linear>::k},
+     {DisplaySet<StoreCanvas, F32, Linear>::k, DisplaySet<StoreCanvas, F16, Linear>::k}},
     {{DisplaySet<StoreFrame, F32, Nearest>::k, DisplaySet<StoreFrame, F16, Nearest>::k},
-     {DisplaySet<StoreCapture, F32, Nearest>::k, DisplaySet<StoreCapture, F16, Nearest>::k}},
+     {DisplaySet<StoreCapture, F32, Nearest>::k, DisplaySet<StoreCapture, F16, Nearest>::k},
+     {DisplaySet<StoreCanvas, F32, Nearest>::k, DisplaySet<StoreCanvas, F16, Nearest>::k}},
 };
 }  // extern "C++"
 
@@ -1721,7 +1725,8 @@ static void widen_staged(float* host, const std::vector<__half>& stage) {
     for (size_t k = 0; k < stage.size(); ++k) host[k] = __half2float(stage[k]);
 }
 
-// One frame of render() or captureScreenshot(), as the entry points below ask for it.
+// One frame of render(), captureScreenshot() or render(null) on the canvas, as the entry points below ask
+// for it.
 struct DrawRequest {
     const char* what;                  // the entry point, for error messages
     int width, height;                 // the target
@@ -1729,15 +1734,34 @@ struct DrawRequest {
     uint32_t keywords;                 // FLUID_DISPLAY_*
     const fluid_postfx* fx;            // BLOOM or SUNRAYS
     const float* dither; int dw, dh;   // BLOOM
-    float back[3]; int bg_mode;        // the background (blend_over_background)
-    bool capture;                      // the 8-bit image of captureScreenshot instead of the fp32 frame
-    void* host; size_t n;              // where the image goes: n floats (frame) or n bytes (capture)
+    float back[3]; int bg_mode;        // the background the output policy blends over (postfx.cuh)
+    DisplayOut out;                    // the fp32 frame, the 8-bit capture image or the RGBA8 canvas
+    bool on_device;                    // dst is the caller's device memory: no copy, no sync
+    void* dst; size_t n;               // where the image goes: n floats (frame) or n bytes (capture, canvas)
     float* host_bloom;                 // the bloom FBO / sunrays texture, read back when given
     float* host_sunrays;
 };
 
+// A caller's device destination of the canvas: device or managed memory of the handle's device, 4-byte
+// aligned for the uchar4 stores.
+static int check_device_dst(fluid_t* h, const DrawRequest& r) {
+    cudaPointerAttributes at{};
+    if (cudaPointerGetAttributes(&at, r.dst) != cudaSuccess) {
+        cudaGetLastError();                      // not sticky: keep it out of the next launch check
+        return fail(h, FLUID_ERR_INVALID, "%s: dst is not a pointer CUDA knows", r.what);
+    }
+    if ((at.type != cudaMemoryTypeDevice && at.type != cudaMemoryTypeManaged) || at.device != h->device)
+        return fail(h, FLUID_ERR_INVALID, "%s: dst_on_device needs device or managed memory of device %d (dst is %s memory of "
+                    "device %d)", r.what, h->device, at.type == cudaMemoryTypeHost ? "pinned host" : at.type == cudaMemoryTypeUnregistered
+                    ? "pageable host" : "device or managed", at.device);
+    if ((uintptr_t)r.dst % 4)
+        return fail(h, FLUID_ERR_INVALID, "%s: a device dst must be 4-byte aligned", r.what);
+    return FLUID_OK;
+}
+
 // render(target) of S:1296-1317: the post-FX chains of the keywords that are on, then the background and
-// drawDisplay in one display_kernel launch, read back to the host.  Only the fp32 frame without BLOOM and
+// drawDisplay in one display_kernel launch, read back to the host (or, for a canvas into device memory,
+// left on the stream for the caller's fluid_sync).  Only the fp32 frame without BLOOM and
 // SUNRAYS is drawn on a slab handle, and there only the handle's band of the target (fluid_render_band).
 // Half storage draws from a widened copy of dye; its post-FX needs FLUID_FLAG_HALF_POSTFX, and then the
 // chains read the fp16 dye directly and draw the mask into the fp16 dye.write.
@@ -1746,8 +1770,8 @@ static int draw(fluid_t* h, const DrawRequest& r) {
     if (r.keywords & ~(uint32_t)(FLUID_DISPLAY_SHADING | FLUID_DISPLAY_BLOOM | FLUID_DISPLAY_SUNRAYS))
         return fail(h, FLUID_ERR_INVALID, "unknown display keyword bits 0x%x", r.keywords);
     const bool bloom_on = r.keywords & FLUID_DISPLAY_BLOOM, sun_on = r.keywords & FLUID_DISPLAY_SUNRAYS;
-    const bool postfx = bloom_on || sun_on, band = !postfx && !r.capture;
-    if (!r.host || r.width < 1 || r.height < 1 || r.canvas_w < 1 || r.canvas_h < 1 || (postfx && !r.fx) ||
+    const bool postfx = bloom_on || sun_on, band = !postfx && r.out == OUT_FRAME, bytes = r.out != OUT_FRAME;
+    if (!r.dst || r.width < 1 || r.height < 1 || r.canvas_w < 1 || r.canvas_h < 1 || (postfx && !r.fx) ||
         (bloom_on && (!r.dither || r.dw < 1 || r.dh < 1)))
         return fail(h, FLUID_ERR_INVALID, "bad argument");
     int y0 = 0, y1 = r.height;
@@ -1755,13 +1779,15 @@ static int draw(fluid_t* h, const DrawRequest& r) {
     const size_t cells = (size_t)r.width * (y1 - y0);
     if (r.n != 4 * cells)
         return fail(h, FLUID_ERR_INVALID, "%s: the target%s has %zu %s, caller passed %zu", r.what, band ? " band" : "",
-                    4 * cells, r.capture ? "bytes" : "floats", r.n);
+                    4 * cells, bytes ? "bytes" : "floats", r.n);
     if (cells == 0) return FLUID_OK;
     if (h->slab() && !band) return not_on_slab(h, r.what);
     if (h->half && !h->half_fx && postfx)
         return fail(h, FLUID_ERR_INVALID, "%s with BLOOM or SUNRAYS is not built for FLUID_FLAG_HALF_STORAGE "
                     "(the reference's bloom / sunrays FBOs are fp16 too: add FLUID_FLAG_HALF_POSTFX)", r.what);
-    int rc = need_frame(h, r.capture ? (cells + 3) / 4 : cells); if (rc) return rc;   // the capture's uchar4 image lives in the frame
+    int rc = r.on_device ? check_device_dst(h, r)
+                         : need_frame(h, bytes ? (cells + 3) / 4 : cells);     // a uchar4 image lives in the frame
+    if (rc) return rc;
     if (h->slab()) {
         // the band's display + shading taps reach ceil(Hd / height) + 2 dye rows beyond the owned ones:
         // refresh that many ghost rows (the ghost rows of dye.read are stale after advection)
@@ -1783,11 +1809,13 @@ static int draw(fluid_t* h, const DrawRequest& r) {
                                   bloom_on ? (float)((double)r.height / (double)r.dh) : 0.0f);
     const DisplayArgs a{dye_src, h->cfg.dye_w, h->cfg.dye_h, h->droff, bloom_on ? h->pfx.bloom : nullptr, o.bw, o.bh,
                         sun_on ? h->pfx.sun : nullptr, o.sw, o.sh, bloom_on ? h->pfx.dither : nullptr, r.dw, r.dh,
-                        h->frame, r.width, r.height, y0, y1, r.back[0], r.back[1], r.back[2], r.bg_mode, h->cfg.aspect, ts};
+                        r.on_device ? r.dst : h->frame, r.width, r.height, y0, y1, r.back[0], r.back[1], r.back[2], r.bg_mode,
+                        h->cfg.aspect, ts};
     dim3 b(32, 8);
-    kDisplay[h->nearest][r.capture][h->half_fx][r.keywords]<<<grid2d(r.width, y1 - y0, b), b, 0, h->stream>>>(a);
+    kDisplay[h->nearest][r.out][h->half_fx][r.keywords]<<<grid2d(r.width, y1 - y0, b), b, 0, h->stream>>>(a);
     if ((rc = check_launch(h, "display_kernel"))) return rc;
-    CU(cudaMemcpyAsync(r.host, h->frame, r.n * (r.capture ? 1 : sizeof(float)), cudaMemcpyDeviceToHost, h->stream));
+    if (r.on_device) return FLUID_OK;
+    CU(cudaMemcpyAsync(r.dst, h->frame, r.n * (bytes ? 1 : sizeof(float)), cudaMemcpyDeviceToHost, h->stream));
     std::vector<__half> bloom16, sun16;
     if (bloom_on && r.host_bloom && (rc = read_target(h, r.host_bloom, h->pfx.bloom, (size_t)o.bw * o.bh * 4, bloom16))) return rc;
     if (sun_on && r.host_sunrays && (rc = read_target(h, r.host_sunrays, h->pfx.sun, (size_t)o.sw * o.sh, sun16))) return rc;
@@ -1803,7 +1831,7 @@ int fluid_render(fluid_t* h, int width, int height, int shading, float back_r, f
                  float back_b, float* host_rgba, size_t n_floats) {
     return draw(h, {.what = "fluid_render", .width = width, .height = height, .canvas_w = width, .canvas_h = height,
                     .keywords = shading ? (uint32_t)FLUID_DISPLAY_SHADING : 0u, .back = {back_r, back_g, back_b},
-                    .bg_mode = h ? h->background : 0, .host = host_rgba, .n = n_floats});
+                    .bg_mode = h ? h->background : 0, .dst = host_rgba, .n = n_floats});
 }
 
 // render() with the display keywords of updateKeywords (S:1160-1166); the post-FX FBOs are sized from
@@ -1813,7 +1841,7 @@ int fluid_render_keywords(fluid_t* h, int width, int height, uint32_t keywords, 
                           float* host_rgba, size_t n_floats, float* host_bloom, float* host_sunrays) {
     return draw(h, {.what = "fluid_render_keywords", .width = width, .height = height, .canvas_w = width,
                     .canvas_h = height, .keywords = keywords, .fx = fx, .dither = dither_rgb, .dw = dw, .dh = dh,
-                    .back = {back_r, back_g, back_b}, .bg_mode = h ? h->background : 0, .host = host_rgba,
+                    .back = {back_r, back_g, back_b}, .bg_mode = h ? h->background : 0, .dst = host_rgba,
                     .n = n_floats, .host_bloom = host_bloom, .host_sunrays = host_sunrays});
 }
 
@@ -1824,7 +1852,7 @@ int fluid_render_postfx(fluid_t* h, int width, int height, const fluid_postfx* f
     return draw(h, {.what = "fluid_render_postfx", .width = width, .height = height, .canvas_w = width,
                     .canvas_h = height, .keywords = FLUID_DISPLAY_SHADING | FLUID_DISPLAY_BLOOM | FLUID_DISPLAY_SUNRAYS,
                     .fx = fx, .dither = dither_rgb, .dw = dw, .dh = dh, .back = {back_r, back_g, back_b},
-                    .bg_mode = h ? h->background : 0, .host = host_rgba, .n = n_floats, .host_bloom = host_bloom,
+                    .bg_mode = h ? h->background : 0, .dst = host_rgba, .n = n_floats, .host_bloom = host_bloom,
                     .host_sunrays = host_sunrays});
 }
 
@@ -1841,8 +1869,22 @@ int fluid_capture(fluid_t* h, int width, int height, int canvas_w, int canvas_h,
                           __half2float(__float2half_rn(back_b))};
     return draw(h, {.what = "fluid_capture", .width = width, .height = height, .canvas_w = canvas_w,
                     .canvas_h = canvas_h, .keywords = keywords, .fx = fx, .dither = dither_rgb, .dw = dw, .dh = dh,
-                    .back = {b16[0], b16[1], b16[2]}, .bg_mode = transparent ? 2 : 0, .capture = true,
-                    .host = host_rgba8, .n = n_bytes});
+                    .back = {b16[0], b16[1], b16[2]}, .bg_mode = transparent ? 2 : 0, .out = OUT_CAPTURE,
+                    .dst = host_rgba8, .n = n_bytes});
+}
+
+// render(null) (S:1296-1317) on a width x height RGBA8 drawing buffer: the post-FX chains on the canvas-sized
+// FBOs, then the display over drawColor(BACK_COLOR) or drawCheckerboard (TRANSPARENT, S:1304-1315), blended
+// on the fixed-point buffer by the display kernel's StoreCanvas epilogue.  Into host memory through the
+// frame buffer, or straight into the caller's device memory, stream-ordered.
+int fluid_render_canvas(fluid_t* h, int width, int height, uint32_t keywords, int transparent,
+                        const fluid_postfx* fx, const float* dither_rgb, int dw, int dh,
+                        float back_r, float back_g, float back_b,
+                        uint8_t* dst, size_t n_bytes, int dst_on_device) {
+    return draw(h, {.what = "fluid_render_canvas", .width = width, .height = height, .canvas_w = width,
+                    .canvas_h = height, .keywords = keywords, .fx = fx, .dither = dither_rgb, .dw = dw, .dh = dh,
+                    .back = {back_r, back_g, back_b}, .bg_mode = transparent ? 1 : 0, .out = OUT_CANVAS,
+                    .on_device = dst_on_device != 0, .dst = dst, .n = n_bytes});
 }
 
 void* fluid_host_alloc(size_t bytes) {

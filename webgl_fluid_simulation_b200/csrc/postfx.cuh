@@ -1,8 +1,8 @@
 // postfx.cuh — the display side of render() and captureScreenshot() (SURVEY §8f rank 1, second half):
 // the post-FX chains of bloom (applyBloom S:1350-1394; shaders S:614-674) and sunrays (applySunrays +
 // blur S:1396-1419; shaders S:461-494, S:676-724), and the display shader (S:549-612) for all eight
-// keyword sets, drawn over the background into the fp32 frame of render() or the 8-bit image of
-// captureScreenshot.
+// keyword sets, drawn over the background into the fp32 frame of render(), the 8-bit image of
+// captureScreenshot, or the RGBA8 canvas of render(null).
 //
 // Every kernel is one reference blit: one thread per target texel, sources fetched through the sampler
 // policy Smp of passes.cuh: Linear (the GL_LINEAR formula, linear_fetch) or, with
@@ -135,21 +135,22 @@ __global__ void __launch_bounds__(256) blur3_kernel(const typename St::T1* __res
 
 __device__ __forceinline__ float len3(float4 v) { return sqrtf((v.x * v.x + v.y * v.y) + v.z * v.z); }
 
+// checkerboardShader (S:531-547): v = mod(floor(uv.x * 25 * aspect) + floor(uv.y * 25), 2) * 0.1 + 0.8
+__device__ __forceinline__ float checkerboard(float aspect, float uvx, float uvy) {
+    const float x = floorf((uvx * 25.0f) * aspect), y = floorf((uvy * 25.0f) * 1.0f);
+    const float sxy = x + y;
+    const float v = sxy - 2.0f * floorf(sxy / 2.0f);
+    return v * 0.1f + 0.8f;
+}
+
 // What drawDisplay is blended over (render(), S:1296-1317) with blendFunc(ONE, ONE_MINUS_SRC_ALPHA)
-// (S:1305): bg_mode 0 = drawColor(BACK_COLOR) (S:1319-1323); 1 = drawCheckerboard — TRANSPARENT on the
-// screen (S:1325-1329, checkerboardShader S:531-547: v = mod(floor(uv.x * 25 * aspect) + floor(uv.y * 25), 2)
-// * 0.1 + 0.8); 2 = nothing, blending disabled — TRANSPARENT into a capture target (S:1307-1308): the
-// display colour goes out as it is.
+// (S:1305) on a float target: bg_mode 0 = drawColor(BACK_COLOR) (S:1319-1323); 1 = drawCheckerboard —
+// TRANSPARENT on the screen (S:1325-1329); 2 = nothing, blending disabled — TRANSPARENT into a capture
+// target (S:1307-1308): the display colour goes out as it is.
 __device__ __forceinline__ float4 blend_over_background(float cr, float cg, float cb, float a, int bg_mode, float br,
                                                         float bg, float bb, float aspect, float uvx, float uvy) {
     if (bg_mode == 2) return make_float4(cr, cg, cb, a);
-    if (bg_mode == 1) {
-        const float x = floorf((uvx * 25.0f) * aspect), y = floorf((uvy * 25.0f) * 1.0f);
-        const float sxy = x + y;
-        float v = sxy - 2.0f * floorf(sxy / 2.0f);
-        v = v * 0.1f + 0.8f;
-        br = bg = bb = v;
-    }
+    if (bg_mode == 1) br = bg = bb = checkerboard(aspect, uvx, uvy);
     const float k = 1.0f - a;
     return make_float4(cr + br * k, cg + bg * k, cb + bb * k, a + 1.0f * k);
 }
@@ -164,23 +165,12 @@ __device__ __forceinline__ unsigned char capture_byte(float v) {
     return (unsigned char)__float2uint_rz(c * 255.0f);
 }
 
-// Output policies of display_kernel: the element type of `out`, the row of `out` that row r of an
-// n-row band goes to, and what is stored.
-// StoreFrame: the fp32 RGBA frame of render(), row 0 = bottom.
-struct StoreFrame {
-    using T = float4;
-    static __device__ __forceinline__ int row(int r, int) { return r; }
-    static __device__ __forceinline__ float4 pack(float4 v) { return v; }
-};
-// StoreCapture: captureScreenshot (S:287-327) up to the bytes toDataURL encodes: the fp16 store, then
-// normalizeTexture's 8-bit truncation and its flip (top row first).
-struct StoreCapture {
-    using T = uchar4;
-    static __device__ __forceinline__ int row(int r, int n) { return n - 1 - r; }
-    static __device__ __forceinline__ uchar4 pack(float4 v) {
-        return make_uchar4(capture_byte(v.x), capture_byte(v.y), capture_byte(v.z), capture_byte(v.w));
-    }
-};
+// The fixed-point colour buffer of the canvas (RGBA8 unsigned-normalised, S:118-119): clamp01 (NaN gives
+// 0, +inf 1) and the float-to-unorm conversion, round to nearest with ties to even (GLES 3.0 §2.1.6.1).
+__device__ __forceinline__ float clamp01(float x) { return fminf(fmaxf(x, 0.0f), 1.0f); }
+__device__ __forceinline__ unsigned char unorm8(float x) { return (unsigned char)__float2uint_rn(__fmul_rn(clamp01(x), 255.0f)); }
+// a stored byte read back as a blend destination: d8 / 255, correctly rounded
+__device__ __forceinline__ float unorm8_value(unsigned char d8) { return __fdiv_rn((float)d8, 255.0f); }
 
 // The inputs of display_kernel.  Those of a keyword that is off are never read.
 struct DisplayArgs {
@@ -197,8 +187,50 @@ struct DisplayArgs {
     float4 ts;                          // 1/w, 1/h and getTextureScale of the dithering texture (BLOOM)
 };
 
+// Output policies of display_kernel: the element type of `out`, the row of `out` that row r of an
+// n-row band goes to, and what is stored for the display fragment (c, alpha) at uv, blend included.
+// StoreFrame: the fp32 RGBA frame of render(), row 0 = bottom.
+struct StoreFrame {
+    using T = float4;
+    static __device__ __forceinline__ int row(int r, int) { return r; }
+    static __device__ __forceinline__ float4 store(const float (&c)[3], float alpha, const DisplayArgs& a, float uvx, float uvy) {
+        return blend_over_background(c[0], c[1], c[2], alpha, a.bg_mode, a.br, a.bg, a.bb, a.aspect, uvx, uvy);
+    }
+};
+// StoreCapture: captureScreenshot (S:287-327) up to the bytes toDataURL encodes: the blend of render(),
+// the fp16 store, then normalizeTexture's 8-bit truncation and its flip (top row first).
+struct StoreCapture {
+    using T = uchar4;
+    static __device__ __forceinline__ int row(int r, int n) { return n - 1 - r; }
+    static __device__ __forceinline__ uchar4 store(const float (&c)[3], float alpha, const DisplayArgs& a, float uvx, float uvy) {
+        const float4 v = blend_over_background(c[0], c[1], c[2], alpha, a.bg_mode, a.br, a.bg, a.bb, a.aspect, uvx, uvy);
+        return make_uchar4(capture_byte(v.x), capture_byte(v.y), capture_byte(v.z), capture_byte(v.w));
+    }
+};
+// StoreCanvas: render(null) on the RGBA8 drawing buffer (S:1296-1317; the context has alpha: true,
+// S:118-119), top row first like ImageData.  The destination holds bytes: u8(BACK_COLOR) (bg_mode 0) or
+// u8(checkerboard) (bg_mode 1), alpha byte 255.  A fixed-point buffer clamps the source and the blend
+// factors before blending (GLES 3.0 §4.1.7), so ONE, ONE_MINUS_SRC_ALPHA is clamp01(c) + d * (1 -
+// clamp01(a)) on d = d8 / 255, rounded once more to a byte.  Every operation is rounded on its own.
+struct StoreCanvas {
+    using T = uchar4;
+    static __device__ __forceinline__ int row(int r, int n) { return n - 1 - r; }
+    static __device__ __forceinline__ uchar4 store(const float (&c)[3], float alpha, const DisplayArgs& a, float uvx, float uvy) {
+        float d[3];
+        if (a.bg_mode == 1) {
+            d[0] = d[1] = d[2] = unorm8_value(unorm8(checkerboard(a.aspect, uvx, uvy)));
+        } else {
+            d[0] = unorm8_value(unorm8(a.br)); d[1] = unorm8_value(unorm8(a.bg)); d[2] = unorm8_value(unorm8(a.bb));
+        }
+        const float ca = clamp01(alpha), k = __fsub_rn(1.0f, ca);
+        // the destination alpha is u8(1) / 255 = 1 over either background
+        return make_uchar4(unorm8(__fadd_rn(clamp01(c[0]), __fmul_rn(d[0], k))), unorm8(__fadd_rn(clamp01(c[1]), __fmul_rn(d[1], k))),
+                           unorm8(__fadd_rn(clamp01(c[2]), __fmul_rn(d[2], k))), unorm8(__fadd_rn(ca, __fmul_rn(1.0f, k))));
+    }
+};
+
 // displayShaderSource S:549-612 compiled with the keywords updateKeywords picks (S:1160-1166), over
-// the background of render() (blend_over_background).  Out: the output policy; Sp: the storage policy
+// the background of render() (the output policy's store() blends).  Out: the output policy; Sp: the storage policy
 // of the bloom and sunrays targets (post_fx_chains' St); Smp: the sampler of the dye, bloom and sunrays
 // taps (the dithering tap is LINEAR + REPEAT whatever Smp is).  A slab rank draws the band [y0, y1) of the
 // target from its own dye rows (+ ghost rows); one GPU draws the whole target.
@@ -251,7 +283,7 @@ __global__ void __launch_bounds__(256) display_kernel(DisplayArgs a) {
         }
     }
     const float alpha = fmaxf(cc[0], fmaxf(cc[1], cc[2]));
-    *o = Out::pack(blend_over_background(cc[0], cc[1], cc[2], alpha, a.bg_mode, a.br, a.bg, a.bb, a.aspect, uvx, uvy));
+    *o = Out::store(cc, alpha, a, uvx, uvy);
 }
 
 }  // namespace fk

@@ -233,12 +233,14 @@ class FluidSimulation {
         });
     }
 
-    update () {                                                 // S:1176-1186 minus render() and rAF
+    // S:1176-1186 minus rAF.  With draw = true it ends like the reference's, with render(null): the canvas
+    // frame of renderCanvas() is returned (put it on the page with putImageData); otherwise dt.
+    update (draw = false) {
         const dt = this.calcDeltaTime();
         this.updateColors(dt);
         this.applyInputs();
         if (!this.config.PAUSED) this.step(dt);
-        return dt;
+        return draw ? this.renderCanvas() : dt;
     }
 
     // ---- pointer helpers (the caller side of splat(); the DOM listeners S:1464-1525 stay with the page) ----
@@ -322,6 +324,22 @@ class FluidSimulation {
                                     !!c.TRANSPARENT, c, (kw & DISPLAY.BLOOM) ? d.data : null, d ? d.width : 0,
                                     d ? d.height : 0, bc.r / 255, bc.g / 255, bc.b / 255);
         return { width: res.width, height: res.height, data };
+    }
+
+    // render(null) of S:1296-1317 on the canvas's RGBA8 drawing buffer (fluid_render_canvas in
+    // include/fluid.h states the rule): canvas.width x canvas.height, the display over BACK_COLOR or, with
+    // TRANSPARENT, the checkerboard, clamped and quantised like the fixed-point buffer.  Returns {width, height,
+    // data: Uint8ClampedArray RGBA, top row first}: new ImageData(data, width, height) for ctx.putImageData.
+    renderCanvas () {
+        const c = this.config;
+        const bc = c.BACK_COLOR;                                // normalizeColor, S:1599-1606
+        this._pushConfig();                                     // the checkerboard uses canvas.width / canvas.height (S:1327)
+        const kw = this._keywords();
+        const d = this.dithering;
+        const data = native.renderCanvas(this._h, this.canvas.width, this.canvas.height, kw, !!c.TRANSPARENT, c,
+                                         (kw & DISPLAY.BLOOM) ? d.data : null, d ? d.width : 0, d ? d.height : 0,
+                                         bc.r / 255, bc.g / 255, bc.b / 255);
+        return { width: this.canvas.width, height: this.canvas.height, data };
     }
 
     stat (name) { return native.stat(this._h, STAT[name]); }

@@ -19,6 +19,8 @@
  *       SHADING / BLOOM / SUNRAYS set, FLUID_DISPLAY_* bits)
  *   capture(h, width, height, canvasWidth, canvasHeight, keywords, transparent, config, dither, dw, dh,
  *       r, g, b) -> Uint8Array (captureScreenshot's RGBA8 image, top row first)
+ *   renderCanvas(h, width, height, keywords, transparent, config, dither, dw, dh, r, g, b) -> Uint8ClampedArray
+ *       (render(null) on the RGBA8 canvas, top row first: ready for new ImageData + putImageData)
  *   pressureSolveHost(h, div: Float32Array, p: Float32Array, iters)   stat(h, key)
  *   ncclUniqueId() -> ArrayBuffer(128)  p2pExport(h) -> ArrayBuffer(256)  p2pConnect(h, below, above)
  *   p2pDisable(h)  getResolution(res, cw, ch) -> {width, height}  lastError(h?) -> number-free string
@@ -322,6 +324,32 @@ static napi_value Capture(napi_env env, napi_callback_info info) {
     return ta;
 }
 
+/* renderCanvas(h, width, height, keywords, transparent, config, dither, dw, dh, r, g, b): fluid_render_canvas
+ * into host memory, arguments as for renderKeywords.  Returns a new Uint8ClampedArray of width * height * 4
+ * bytes, top row first: the pixels of the drawing buffer after render(null), for new ImageData(data, width,
+ * height) and putImageData. */
+static napi_value RenderCanvas(napi_env env, napi_callback_info info) {
+    ARGS(12)
+    wrap_t* w = wrap_of(env, argv[0]); if (!w) return NULL;
+    int32_t wd = 0, ht = 0, dw = 0, dh = 0; uint32_t kw = 0; bool transparent = false;
+    napi_get_value_int32(env, argv[1], &wd); napi_get_value_int32(env, argv[2], &ht);
+    napi_get_value_uint32(env, argv[3], &kw); napi_get_value_bool(env, argv[4], &transparent);
+    napi_get_value_int32(env, argv[7], &dw); napi_get_value_int32(env, argv[8], &dh);
+    if (wd < 1 || ht < 1) { napi_throw_error(env, NULL, "bad canvas size"); return NULL; }
+    fluid_postfx fx;
+    postfx_from(env, argv[5], &fx);
+    const float* dither;
+    if (!dither_from(env, kw, argv[6], dw, dh, &dither)) return NULL;
+    const size_t n = (size_t)wd * ht * 4;
+    void* data = NULL; napi_value ab, ta;
+    if (napi_create_arraybuffer(env, n, &data, &ab) != napi_ok) return NULL;
+    if (!check(env, w->h, fluid_render_canvas(w->h, wd, ht, kw, transparent ? 1 : 0, &fx, dither, dw, dh,
+                                              (float)num(env, argv[9]), (float)num(env, argv[10]), (float)num(env, argv[11]),
+                                              (uint8_t*)data, n, 0))) return NULL;
+    if (napi_create_typedarray(env, napi_uint8_clamped_array, n, ab, 0, &ta) != napi_ok) return NULL;
+    return ta;
+}
+
 static napi_value Sync(napi_env env, napi_callback_info info) {
     ARGS(1)
     wrap_t* w = wrap_of(env, argv[0]); if (!w) return NULL;
@@ -424,6 +452,7 @@ NAPI_MODULE_INIT() {
         {"render", NULL, Render, NULL, NULL, NULL, napi_enumerable, NULL},
         {"renderKeywords", NULL, RenderKeywords, NULL, NULL, NULL, napi_enumerable, NULL},
         {"capture", NULL, Capture, NULL, NULL, NULL, napi_enumerable, NULL},
+        {"renderCanvas", NULL, RenderCanvas, NULL, NULL, NULL, napi_enumerable, NULL},
         {"sync", NULL, Sync, NULL, NULL, NULL, napi_enumerable, NULL},
         {"stat", NULL, Stat, NULL, NULL, NULL, napi_enumerable, NULL},
         {"dims", NULL, Dims, NULL, NULL, NULL, napi_enumerable, NULL},

@@ -373,13 +373,17 @@ class FluidSimulation:
                 p.moved = False
                 self.splatPointer(p)
 
-    def update(self, now_ms=None):
-        """One iteration of update(), S:1176-1186, minus render() (out of scope) and rAF."""
+    def update(self, now_ms=None, canvas=None):
+        """One iteration of update(), S:1176-1186, minus rAF.  With `canvas` (a destination render_canvas
+        takes as `out`) it ends with render_canvas(out=canvas), as the reference's ends with render(null);
+        without it nothing is drawn."""
         dt = self.calcDeltaTime(now_ms)
         self.updateColors(dt)
         self.applyInputs()
         if not self.config["PAUSED"]:
             self.step(dt)
+        if canvas is not None:
+            self.render_canvas(out=canvas)
         return dt
 
     # pointer helpers, S:1527-1563
@@ -493,6 +497,50 @@ class FluidSimulation:
             write_png(path, out)
         return out
 
+    def render_canvas(self, out=None):
+        """render(null), S:1296-1317, on the canvas: canvas.width x canvas.height RGBA8, the bytes the
+        drawing buffer holds after the frame (fluid_render_canvas in include/fluid.h states the rule:
+        source and blend factors clamped, destination quantised, round to nearest even).  config.SHADING /
+        BLOOM / SUNRAYS / TRANSPARENT (the checkerboard) / BACK_COLOR as in render(); BLOOM needs
+        `sim.dithering`.  Returns the (height, width, 4) uint8 image, top row first (ImageData order).
+        `out`: a C-contiguous uint8 numpy array of 4 * width * height bytes, or a C-contiguous uint8 CUDA
+        array on the handle's device, 4-byte aligned (anything with __cuda_array_interface__, e.g. a torch
+        tensor).  The display kernel writes a CUDA array directly, with no copy to the host.  The handle's
+        stream does not order against other streams, so the call first waits for the work that may still
+        use the array: the producer stream a version-3 interface names, or, where the interface names none
+        (torch's is version 2), every queued kernel and copy of the array's device.  The handle's stream is
+        synchronised before returning, so the array can be read at once.  A CUDA array is returned as it
+        was passed."""
+        cfg = self.config
+        w, h = self.canvas["width"], self.canvas["height"]
+        n = 4 * w * h
+        self._push_config()                                  # the checkerboard uses canvas.width / canvas.height (S:1327)
+        kw, fx, dith = postfx_inputs(cfg, getattr(self, "dithering", None))
+        bc = cfg["BACK_COLOR"]                               # normalizeColor, S:1599-1606
+        cai = getattr(out, "__cuda_array_interface__", None)
+        if cai is not None:
+            shape, strides = tuple(cai["shape"]), cai.get("strides")
+            dense = strides is None or tuple(strides) == tuple(int(np.prod(shape[k + 1:])) for k in range(len(shape)))
+            if cai["typestr"] != "|u1" or int(np.prod(shape)) != n or not dense:
+                raise ValueError(f"render_canvas needs a C-contiguous uint8 CUDA array of {n} bytes, got "
+                                 f"{cai['typestr']} {shape} strides {strides}")
+            _wait_for_users(cai)
+            dst, result = C.c_void_p(cai["data"][0]), out
+        else:
+            if out is None:
+                out = np.empty((h, w, 4), np.uint8)
+            if not isinstance(out, np.ndarray) or out.dtype != np.uint8 or not out.flags.c_contiguous or out.size != n:
+                raise ValueError(f"render_canvas needs a C-contiguous uint8 array of {n} bytes")
+            dst, result = out.ctypes.data_as(C.c_void_p), out.reshape(h, w, 4)
+        ptr = lambda x: None if x is None else x.ctypes.data_as(C.c_void_p)   # noqa: E731
+        self._check(self._L.fluid_render_canvas(
+            self._h, w, h, kw, 1 if cfg.get("TRANSPARENT") else 0, None if fx is None else C.byref(fx), ptr(dith),
+            0 if dith is None else dith.shape[1], 0 if dith is None else dith.shape[0],
+            bc["r"] / 255, bc["g"] / 255, bc["b"] / 255, dst, n, 1 if cai is not None else 0))
+        if cai is not None:
+            self.sync()
+        return result
+
     @staticmethod
     def textureToCanvas(rgba: np.ndarray) -> np.ndarray:
         """normalizeTexture + textureToCanvas (S:309-349): clamp01 * 255 truncated into a Uint8
@@ -563,6 +611,40 @@ class FluidSimulation:
 
     def __exit__(self, *a):
         self.close()
+
+
+_cuda = None
+
+
+def _wait_for_users(cai):
+    """Blocks until no queued GPU work can still read or write the CUDA array whose
+    __cuda_array_interface__ is `cai`, so a kernel on the handle's non-blocking stream may overwrite it.
+    A version-3 interface names the producer's stream ("stream": None means nothing is pending; 1 and 2
+    are the legacy and per-thread default streams, which the driver API takes as handles): that stream is
+    synchronised.  Without the key (version 2, torch's) the array's device is synchronised, every stream.
+    A pointer the driver does not know is left alone: fluid_render_canvas refuses it."""
+    global _cuda
+    if "stream" in cai and cai["stream"] is None:
+        return
+    if _cuda is None:
+        L = C.CDLL("libcuda.so.1")
+        L.cuPointerGetAttribute.argtypes = [C.c_void_p, C.c_int, C.c_uint64]
+        L.cuCtxPushCurrent_v2.argtypes = [C.c_void_p]
+        L.cuCtxPopCurrent_v2.argtypes = [C.POINTER(C.c_void_p)]
+        L.cuStreamSynchronize.argtypes = [C.c_void_p]
+        _cuda = L
+    ctx = C.c_void_p()
+    CU_POINTER_ATTRIBUTE_CONTEXT = 1
+    if _cuda.cuPointerGetAttribute(C.byref(ctx), CU_POINTER_ATTRIBUTE_CONTEXT, int(cai["data"][0])) != 0 or not ctx:
+        return
+    if _cuda.cuCtxPushCurrent_v2(ctx) != 0:
+        raise RuntimeError("cuCtxPushCurrent on the context of the destination failed")
+    try:
+        rc = _cuda.cuStreamSynchronize(C.c_void_p(int(cai["stream"]))) if "stream" in cai else _cuda.cuCtxSynchronize()
+    finally:
+        _cuda.cuCtxPopCurrent_v2(C.byref(C.c_void_p()))
+    if rc != 0:
+        raise RuntimeError(f"waiting for the pending work on the destination failed: CUresult {rc}")
 
 
 def wrap(value, mn, mx):
