@@ -1,0 +1,308 @@
+"""The four post-FX sliders -- BLOOM_INTENSITY, BLOOM_THRESHOLD, BLOOM_SOFT_KNEE, SUNRAYS_WEIGHT (S:79-84, the
+settings panel S:227-232) -- away from their defaults, on the CPU.  This file holds the parameter sets and the
+dye that tests/test_gpu_postfx_params.py draws with them, and shows that they are strong enough to catch a
+wrong kernel:
+
+* branches: for every set, the bloom prefilter (bloomPrefilterShader S:614-631) sees enough texels below
+  curve.x, inside the knee and above it, with rq winning and losing max(rq, br - threshold), and with br
+  under the max(br, 0.0001) guard as zeros, fp32 subnormals and negatives;
+* mutants: each one-change copy of the chain model below -- one slider replaced by its default, threshold
+  and knee swapped, knee / curve derived in fp32 instead of in JS doubles, the intensity applied on the
+  additive up-pass instead of the final blit -- changes the expected bloom FBO or sunrays bits and the
+  expected frame of at least one set, and all but the fp32 curve (a few ulp of bloom) its capture and canvas
+  bytes too;
+* the oracle against the executed reference shaders with these sliders (postfx_params_*.npz, cut by
+  tests/golden/make_golden_postfx_params.py): bloom FBO and sunrays bit for bit, the frame at the tolerance
+  of the power-of-two post-FX goldens."""
+import numpy as np
+import pytest
+
+import canvas_model as CV
+import capture_model as CM
+import display_keywords_model as M
+import half_postfx_model as HP
+import nearest_model as N
+from conftest import golden, max_rel
+from oracle import oracle as O
+from test_gamma_model_cpu import BACK_RGB, golden_dither
+
+F32 = np.float32
+ALL3 = M.SHADING | M.BLOOM | M.SUNRAYS
+DEFAULTS = dict(BLOOM_INTENSITY=0.8, BLOOM_THRESHOLD=0.6, BLOOM_SOFT_KNEE=0.7, SUNRAYS_WEIGHT=1.0)   # S:79-84
+# (I, T, K, W).  t033_k07 and t039_k1 are slider positions where knee / curve narrowed from fp32 arithmetic
+# differ from the JS doubles narrowed once (all three curve components); t005 differs in curve.x and curve.z.
+SETS = {
+    "t0_k1": (0.8, 0.0, 1.0, 1.0),           # threshold 0: curve = (-1e-4, 2e-4, 2500); the knee is wider than the threshold
+    "t0_k0_w4": (0.1, 0.0, 0.0, 4.0),        # sunrays above 1: alpha above 1, the canvas clamps
+    "t005": (1.3, 0.05, 0.7, 0.6),
+    "t033_k07": (0.55, 0.33, 0.7, 0.45),
+    "t039_k1": (1.6, 0.39, 1.0, 0.85),
+    "t1_k0_i2_w03": (2.0, 1.0, 0.0, 0.3),    # knee 0: knee = 1e-4, a hard step
+    "t1_k1": (0.1, 1.0, 1.0, 1.0),
+    "i0_w0": (0.0, 0.6, 0.7, 0.0),
+    "overflow": (70000.0, 0.6, 0.7, 1.0),    # the final blit overflows fp16 to +inf on about half the HALF_POSTFX texels
+    "above": (0.8, 5.0, 0.2, 0.5),           # curve.x = 4 above every br of the dye: the prefilter draws zeros
+}
+KEYS = ("BLOOM_INTENSITY", "BLOOM_THRESHOLD", "BLOOM_SOFT_KNEE", "SUNRAYS_WEIGHT")
+# (dye w, dye h, canvas w, canvas h, BLOOM_RESOLUTION, SUNRAYS_RESOLUTION, CAPTURE_RESOLUTION): every size a
+# power of two (bloom 64 x 32, sunrays 32 x 16, capture 64 x 32), and a ragged dye on a portrait canvas
+# (bloom 48 x 64, sunrays 30 x 40, capture 45 x 60)
+GEOMETRIES = {"pow2": (64, 64, 128, 64, 32, 16, 32), "portrait": (40, 56, 90, 120, 48, 30, 45)}
+DYE_SEED = 2718
+MIN_TEXELS = 8                               # bloom texels each branch must get, per set and geometry
+
+
+def cfg_of(name, geometry="pow2"):
+    """The config keys of parameter set `name` on `geometry`."""
+    I, T, K, W = SETS[name]
+    bres, sres, cres = GEOMETRIES[geometry][4:]
+    return dict(BLOOM_INTENSITY=I, BLOOM_THRESHOLD=T, BLOOM_SOFT_KNEE=K, SUNRAYS_WEIGHT=W, BLOOM_RESOLUTION=bres,
+                SUNRAYS_RESOLUTION=sres, CAPTURE_RESOLUTION=cres)
+
+
+def params_dye(Wd, Hd, seed=DYE_SEED):
+    """Finite dye whose brightest channel br (the prefilter's) falls in 4 x 4 blocks of one kind each, so that a
+    LINEAR fetch at ragged sizes mostly mixes texels of one kind: exact zeros (the other channels in -2e-3 .. -1e-3), fp32
+    subnormals, negatives down to -2, +-1e-7 .. 1e-4 around the threshold-0 knee, values inside the knee
+    [T - knee, T + knee] of a set of SETS but `above` (a hard step's knee is 2e-4 wide: no uniform draw would land there),
+    and bright values 3.2 u^1.5 (u uniform) reaching every knee.  One channel holds br, the other two a
+    fraction of it (more negative for a negative br); which channel is the same across a block.  Alpha 1.  No channel is -0, in fp32 or
+    rounded to fp16: where the display's alpha is fmaxf(-0, +0), the device and C need not agree."""
+    rng = np.random.default_rng(seed)
+    bh, bw = (Hd + 3) // 4, (Wd + 3) // 4
+    up = lambda a: np.kron(a, np.ones((4, 4), a.dtype))[:Hd, :Wd]             # noqa: E731
+    kind = up(rng.choice(6, size=(bh, bw), p=[0.07, 0.06, 0.09, 0.09, 0.19, 0.50]))
+    knees = np.array([(t, t * k + 0.0001) for n, (_, t, k, _) in SETS.items() if n != "above"])
+    pick = up(rng.integers(0, len(knees), (bh, bw)))
+    u = rng.random((Hd, Wd))
+    sign = np.where(rng.random((Hd, Wd)) < 0.5, -1.0, 1.0)
+    br = np.select([kind == 0, kind == 1, kind == 2, kind == 3, kind == 4],
+                   [np.zeros_like(u), 1e-45 + u * 1.1e-38, -np.exp(np.log(1e-6) + u * np.log(2e6)),
+                    sign * np.exp(np.log(1e-7) + u * np.log(1e3)), knees[pick, 0] + knees[pick, 1] * (2 * u - 1)],
+                   3.2 * u ** 1.5).astype(F32)
+    frac = rng.random((Hd, Wd, 3)).astype(F32)
+    c = np.where(br[..., None] >= 0, br[..., None] * frac, br[..., None] * (F32(1) + frac))
+    c[kind == 0] = -(F32(1) + frac[kind == 0]) * F32(1e-3)
+    top = up(rng.integers(0, 3, (bh, bw)))
+    np.put_along_axis(c, top[..., None], br[..., None], axis=-1)
+    dye = np.concatenate([c, np.ones((Hd, Wd, 1), F32)], axis=-1).astype(F32)
+    assert np.isfinite(dye).all() and not ((dye == 0) & np.signbit(dye)).any()
+    assert not ((O.round_half(dye) == 0) & np.signbit(O.round_half(dye))).any()
+    return dye
+
+
+# ---- the chain model, with its mutants -------------------------------------------------------------------
+MUTANTS = [f"default_{k}" for k in KEYS] + ["threshold_knee_swapped", "curve_in_fp32", "intensity_on_up_pass"]
+
+
+def curve(threshold, soft_knee, fp32=False):
+    """(curve.x, curve.y, curve.z, threshold) as the prefilter receives them: applyBloom derives them in JS
+    doubles (S:1358-1363) and gl.uniform narrows each once; `fp32` derives them in fp32 instead."""
+    if fp32:
+        t, k = F32(threshold), F32(soft_knee)
+        knee = t * k + F32(0.0001)
+        return t - knee, knee * F32(2), F32(0.25) / knee, t
+    knee = threshold * soft_knee + 0.0001
+    return F32(threshold - knee), F32(knee * 2), F32(0.25 / knee), F32(threshold)
+
+
+def chains(dye, w, h, cfg, mutant=None, half_targets=False, half_mask=False):
+    """The bloom FBO and the sunrays texture of render() on a w x h canvas: half_postfx_model.render_postfx's
+    chains (the oracle's per-blit C functions, rounded to fp16 after each blit with `half_targets`), with
+    one change when `mutant` names one of MUTANTS."""
+    assert mutant is None or mutant in MUTANTS, mutant
+    c = dict(BLOOM_ITERATIONS=8, BLOOM_RESOLUTION=256, SUNRAYS_RESOLUTION=196, **DEFAULTS)
+    c.update(cfg)
+    if mutant and mutant.startswith("default_"):
+        c[mutant[len("default_"):]] = DEFAULTS[mutant[len("default_"):]]
+    if mutant == "threshold_knee_swapped":
+        c["BLOOM_THRESHOLD"], c["BLOOM_SOFT_KNEE"] = c["BLOOM_SOFT_KNEE"], c["BLOOM_THRESHOLD"]
+    up, final = (c["BLOOM_INTENSITY"], 1.0) if mutant == "intensity_on_up_pass" else (1.0, c["BLOOM_INTENSITY"])
+    L, p = HP._chain_lib(), O._p
+    rt = O.round_half if half_targets else (lambda a: a)
+    dye = np.ascontiguousarray(dye, F32); Hd, Wd, _ = dye.shape
+    bw, bh = N.get_resolution(c["BLOOM_RESOLUTION"], w, h)
+    bloom = np.zeros((bh, bw, 4), F32); bloom[..., 3] = 1
+    sizes = [(bw >> (k + 1), bh >> (k + 1)) for k in range(c["BLOOM_ITERATIONS"])]
+    sizes = sizes[:next((k for k, (pw, ph) in enumerate(sizes) if pw < 2 or ph < 2), len(sizes))]
+    if len(sizes) >= 2:
+        L.oracle_bloom_prefilter(p(dye), Wd, Hd, p(bloom), bw, bh,
+                                 *(float(x) for x in curve(c["BLOOM_THRESHOLD"], c["BLOOM_SOFT_KNEE"], mutant == "curve_in_fp32")))
+        bloom = rt(bloom)
+        last, lw, lh, pyr = bloom, bw, bh, []
+        for pw, ph in sizes:
+            t = np.empty((ph, pw, 4), F32)
+            L.oracle_box4(p(last), lw, lh, p(t), pw, ph, 1.0, 0)
+            t = rt(t); pyr.append(t); last, lw, lh = t, pw, ph
+        for k in range(len(pyr) - 2, -1, -1):
+            pw, ph = sizes[k]
+            L.oracle_box4(p(last), lw, lh, p(pyr[k]), pw, ph, up, 1)
+            pyr[k] = rt(pyr[k]); last, lw, lh = pyr[k], pw, ph
+        L.oracle_box4(p(last), lw, lh, p(bloom), bw, bh, final, 0)
+        bloom = rt(bloom)
+    sw, sh = N.get_resolution(c["SUNRAYS_RESOLUTION"], w, h)
+    mask = np.empty_like(dye)
+    L.oracle_sunrays_mask(p(dye), p(mask), Wd, Hd)
+    mask = O.round_half(mask) if half_mask else mask
+    sun, tmp = np.empty((sh, sw), F32), np.empty((sh, sw), F32)
+    L.oracle_sunrays(p(mask), Wd, Hd, p(sun), sw, sh, c["SUNRAYS_WEIGHT"])
+    sun = rt(sun)
+    L.oracle_blur3(p(sun), p(tmp), sw, sh, 1.0 / sw, 0.0)
+    tmp = rt(tmp)
+    L.oracle_blur3(p(tmp), p(sun), sw, sh, 0.0, 1.0 / sh)
+    return dict(bloom=bloom, sunrays=rt(sun))
+
+
+def outputs(dye, geometry, name, mutant=None, kw=ALL3):
+    """What the fp32 handle is checked on, from the chains: the frame over BACK_COLOR, the capture bytes and the
+    canvas bytes over BACK_COLOR and over the checkerboard."""
+    Wd, Hd, w, h = GEOMETRIES[geometry][:4]
+    cfg = cfg_of(name, geometry)
+    dither = golden_dither()
+    with np.errstate(invalid="ignore", over="ignore"):
+        r = chains(dye, w, h, cfg, mutant)
+        frame = M._display(dye, w, h, kw, r["bloom"], r["sunrays"], dither, BACK_RGB, O.BG_COLOR, w / h)
+        bare = M._display(dye, w, h, kw, r["bloom"], r["sunrays"], dither, BACK_RGB, O.BG_NONE, w / h)
+        cw_, ch_ = N.get_resolution(cfg["CAPTURE_RESOLUTION"], w, h)
+        pre = M._display(dye, cw_, ch_, kw, r["bloom"], r["sunrays"], dither, CM.back16(BACK_RGB), O.BG_COLOR, cw_ / ch_)
+        canvas = [CV.canvas(bare, BACK_RGB, t, w / h) for t in (False, True)]
+    return dict(r, frame=frame, capture=CM.to_bytes(pre)[::-1], canvas=canvas)
+
+
+# ---- the prefilter's branches ----------------------------------------------------------------------------
+def fetched(dye, geometry, nearest=False):
+    """The dye colour the prefilter fetches at every bloom texel (LINEAR or NEAREST, the library's vUv)."""
+    Wd, Hd, w, h, bres = GEOMETRIES[geometry][:5]
+    bw, bh = N.get_resolution(bres, w, h)
+    uv = M.uv_grid(bw, bh)
+    return (N.fetch(dye, *uv) if nearest else M._fetch(dye, *uv))[..., :3].astype(F32)
+
+
+def branches(c, threshold, soft_knee):
+    """{branch: number of texels} of the prefilter on fetched colours c, in its fp32 arithmetic."""
+    c0, c1, c2, th = curve(threshold, soft_knee)
+    br = np.fmax(c[..., 0], np.fmax(c[..., 1], c[..., 2]))
+    x = br - c0
+    rq = np.fmin(np.fmax(x, F32(0)), c1)
+    rq = (c2 * rq) * rq
+    tiny = F32(np.finfo(F32).tiny)
+    return dict(below_curve0=int(np.count_nonzero(x < 0)), in_knee=int(np.count_nonzero((x > 0) & (x < c1))),
+                above_knee=int(np.count_nonzero(x > c1)), rq_wins=int(np.count_nonzero(rq > br - th)),
+                rq_loses=int(np.count_nonzero(rq < br - th)), zero=int(np.count_nonzero(br == 0)),
+                subnormal=int(np.count_nonzero((br > 0) & (br < tiny))), negative=int(np.count_nonzero(br < 0)),
+                small=int(np.count_nonzero((br >= tiny) & (br < F32(0.0001)))))
+
+
+@pytest.mark.parametrize("half", [False, True])
+@pytest.mark.parametrize("nearest", [False, True])
+@pytest.mark.parametrize("geometry", list(GEOMETRIES))
+def test_every_set_reaches_every_prefilter_branch(geometry, nearest, half):
+    """Every branch on at least MIN_TEXELS bloom texels of every set but `above`, whose br all lie below curve.x
+    (its prefilter draws zeros, and so its bloom FBO is zero).  A half-storage dye has no fp32 subnormal left."""
+    dye = params_dye(*GEOMETRIES[geometry][:2])
+    if half:
+        dye = O.round_half(dye)
+    c = fetched(dye, geometry, nearest)
+    for name, (_, T, K, _) in SETS.items():
+        n = branches(c, T, K)
+        if name == "above":
+            assert n["below_curve0"] == c.shape[0] * c.shape[1], n
+            continue
+        for b, k in n.items():
+            if b == "subnormal" and half:
+                assert k == 0
+            else:
+                assert k >= MIN_TEXELS, (name, b, n)
+
+
+def test_sets_cover_the_slider_values():
+    I, T, K, W = (set(v[k] for v in SETS.values()) for k in range(4))
+    assert {0.0, 0.05, 0.6, 1.0} <= T and max(T) > params_dye(64, 64)[..., :3].max() + max(T) * 0.2 + 1e-4
+    assert {0.0, 1.0} <= K and {0.0, 0.1, 2.0} <= I and max(I) > 3000 and {0.0, 0.3} <= W and max(W) > 1
+    differ = [n for n, (_, t, k, _) in SETS.items() if 0 < t <= 1 and 0 < k <= 1
+              and not np.array_equal(np.array(curve(t, k), F32), np.array(curve(t, k, fp32=True), F32))]
+    assert len(differ) >= 2, differ
+
+
+def test_above_and_overflow_sets_do_what_they_are_for(oracle):
+    """`above`: a zero bloom FBO.  `overflow`: +inf in the fp16 bloom FBO (not everywhere), finite in fp32."""
+    Wd, Hd, w, h = GEOMETRIES["pow2"][:4]
+    dye = params_dye(Wd, Hd)
+    assert not chains(dye, w, h, cfg_of("above"))["bloom"][..., :3].any()
+    with np.errstate(over="ignore"):
+        half = chains(dye, w, h, cfg_of("overflow"), half_targets=True)["bloom"][..., :3]
+    assert 0 < np.count_nonzero(np.isposinf(half)) < half.size
+    assert np.isfinite(chains(dye, w, h, cfg_of("overflow"))["bloom"]).all()
+
+
+@pytest.mark.parametrize("half", [(False, False), (True, False), (True, True)])
+@pytest.mark.parametrize("geometry", list(GEOMETRIES))
+def test_chain_model_is_the_models_chains(oracle, geometry, half):
+    """Unmutated, chains() is half_postfx_model.render_postfx (and so oracle.render_postfx) bit for bit."""
+    Wd, Hd, w, h = GEOMETRIES[geometry][:4]
+    dye = params_dye(Wd, Hd)
+    for name in SETS:
+        cfg = cfg_of(name, geometry)
+        with np.errstate(over="ignore", invalid="ignore"):
+            mine = chains(dye, w, h, cfg, half_targets=half[0], half_mask=half[1])
+            ref = HP.render_postfx(dye, w, h, golden_dither(), cfg=cfg, half_targets=half[0], half_mask=half[1])
+        for k in ("bloom", "sunrays"):
+            assert np.array_equal(mine[k].view(np.uint32), ref[k].view(np.uint32)), (name, k)
+
+
+# Mutants whose change stays below one byte of every capture and canvas: curve_in_fp32 moves a curve
+# component by an ulp, and so the bloom FBO by a few ulp.  The bloom FBO's bits and the frame catch it.
+SUB_BYTE = {"curve_in_fp32"}
+
+
+@pytest.mark.parametrize("mutant", MUTANTS)
+def test_mutant_changes_the_expected_bits(oracle, mutant):
+    """Each mutant changes the bloom FBO or the sunrays texture of at least one set, and the frame of at least
+    one set; all but SUB_BYTE change the capture bytes and the canvas bytes of at least one set too."""
+    hits = dict(chain=[], frame=[], capture=[], canvas=[])
+    for geometry in GEOMETRIES:
+        dye = params_dye(*GEOMETRIES[geometry][:2])
+        for name in SETS:
+            good, bad = outputs(dye, geometry, name), outputs(dye, geometry, name, mutant)
+            same = lambda a, b: np.array_equal(np.asarray(a).view(np.uint8), np.asarray(b).view(np.uint8))  # noqa: E731
+            if not (same(good["bloom"], bad["bloom"]) and same(good["sunrays"], bad["sunrays"])):
+                hits["chain"].append((geometry, name))
+            if not same(good["frame"], bad["frame"]):
+                hits["frame"].append((geometry, name))
+            if not same(good["capture"], bad["capture"]):
+                hits["capture"].append((geometry, name))
+            if not all(same(a, b) for a, b in zip(good["canvas"], bad["canvas"])):
+                hits["canvas"].append((geometry, name))
+    want = ("chain", "frame") if mutant in SUB_BYTE else tuple(hits)
+    assert all(hits[k] for k in want), (mutant, hits)
+
+
+# ---- the oracle against the executed shaders ------------------------------------------------------------
+FIXTURES = [f"postfx_params_{n}_64_to_128x64" for n in ("t033_k07", "t0_k1", "t1_k0_i2_w03")]
+
+
+def fixture_cfg(g):
+    return dict(BLOOM_RESOLUTION=int(g["bloom_res"]), SUNRAYS_RESOLUTION=int(g["sun_res"]),
+                BLOOM_INTENSITY=float(g["intensity"]), BLOOM_THRESHOLD=float(g["threshold"]),
+                BLOOM_SOFT_KNEE=float(g["soft_knee"]), SUNRAYS_WEIGHT=float(g["weight"]))
+
+
+@pytest.mark.parametrize("name", FIXTURES)
+def test_oracle_equals_executed_shaders(oracle, name):
+    """Bloom FBO and sunrays bit for bit, the frame within the power-of-two post-FX goldens' 2e-6
+    (test_oracle_golden.py: pow() is implementation-defined).  The fixture's sliders and dye are the set's."""
+    g = golden(name)
+    assert tuple(fixture_cfg(g)[k] for k in KEYS) == SETS[str(g["set"])]
+    assert np.array_equal(g["in_dye"].view(np.uint32), params_dye(int(g["Wd"]), int(g["Hd"])).view(np.uint32))
+    r = oracle.render_postfx(g["in_dye"], int(g["w"]), int(g["h"]), g["dither"].astype(F32), cfg=fixture_cfg(g),
+                             back_rgb=tuple(float(x) / 255 for x in g["back"]))
+    for k in ("bloom", "sunrays"):
+        assert np.array_equal(r[k].view(np.uint32), g[k].view(np.uint32)), k
+    assert max_rel(r["target"], g["target"]) < 2e-6
+
+
+def test_fixtures_tell_the_fp32_curve_from_the_double_one(oracle):
+    """On t033_k07's fixture the curve derived in fp32 gives another bloom FBO than the executed shaders'."""
+    g = golden(FIXTURES[0])
+    bad = chains(g["in_dye"], int(g["w"]), int(g["h"]), fixture_cfg(g), mutant="curve_in_fp32")["bloom"]
+    assert not np.array_equal(bad.view(np.uint32), g["bloom"].view(np.uint32))
