@@ -50,10 +50,19 @@ def lib():
         L.oracle_resample.argtypes = [_f, i, i, _f, i, i, i]
         L.oracle_round_half.argtypes = [_f, sz]
         L.oracle_display.argtypes = [_f, i, i, _f, i, i, i, _f, i, f]; L.oracle_display.restype = None
+        # the post-FX blits, one per shader pass (render_postfx, tests/display_model.py)
+        L.oracle_bloom_prefilter.argtypes = [_f, i, i, _f, i, i, f, f, f, f]
+        L.oracle_box4.argtypes = [_f, i, i, _f, i, i, f, i]
+        L.oracle_sunrays_mask.argtypes = [_f, _f, i, i]
+        L.oracle_sunrays.argtypes = [_f, i, i, _f, i, i, f]
+        L.oracle_blur3.argtypes = [_f, _f, i, i, f, f]
+        L.oracle_display_full.argtypes = [_f, i, i, _f, i, i, _f, i, i, _f, i, i, _f, i, i, _f, i, f]
         L.oracle_num_threads.restype = i
         for fn in (L.oracle_curl, L.oracle_vorticity, L.oracle_divergence, L.oracle_clear,
                    L.oracle_jacobi, L.oracle_jacobi_iters, L.oracle_gradient_subtract,
-                   L.oracle_advect, L.oracle_splat, L.oracle_resample, L.oracle_round_half):
+                   L.oracle_advect, L.oracle_splat, L.oracle_resample, L.oracle_round_half,
+                   L.oracle_bloom_prefilter, L.oracle_box4, L.oracle_sunrays_mask, L.oracle_sunrays,
+                   L.oracle_blur3, L.oracle_display_full):
             fn.restype = None
         _lib = L
     return _lib
@@ -195,16 +204,7 @@ def render_postfx(dye, w, h, dither, cfg=None, back_rgb=(0.0, 0.0, 0.0), backgro
     """render(null) with SHADING + BLOOM + SUNRAYS (reference desktop defaults S:70-84): applyBloom
     (S:1350-1394), applySunrays + blur (S:1396-1419), drawColor + drawDisplay (S:1296-1348), FBO
     sizes from getResolution (S:1012-1043).  dither: (dh, dw, 3) float in [0,1], row 0 = first image row (no UNPACK_FLIP_Y)."""
-    L = lib(); i, f = C.c_int, C.c_float
-    L.oracle_bloom_prefilter.argtypes = [_f, i, i, _f, i, i, f, f, f, f]
-    L.oracle_box4.argtypes = [_f, i, i, _f, i, i, f, i]
-    L.oracle_sunrays_mask.argtypes = [_f, _f, i, i]
-    L.oracle_sunrays.argtypes = [_f, i, i, _f, i, i, f]
-    L.oracle_blur3.argtypes = [_f, _f, i, i, f, f]
-    L.oracle_display_full.argtypes = [_f, i, i, _f, i, i, _f, i, i, _f, i, i, _f, i, i, _f, i, f]
-    for fn in (L.oracle_bloom_prefilter, L.oracle_box4, L.oracle_sunrays_mask, L.oracle_sunrays, L.oracle_blur3,
-               L.oracle_display_full):
-        fn.restype = None
+    L = lib()
     c = dict(BLOOM_ITERATIONS=8, BLOOM_RESOLUTION=256, BLOOM_INTENSITY=0.8, BLOOM_THRESHOLD=0.6,
              BLOOM_SOFT_KNEE=0.7, SUNRAYS_RESOLUTION=196, SUNRAYS_WEIGHT=1.0)
     c.update(cfg or {})

@@ -19,6 +19,8 @@ from the right one: "no_clamp" (the fp32 blend of render(), quantised afterwards
 """
 import numpy as np
 
+from display_model import checkerboard
+
 F = np.float32
 MUTANTS = ("no_clamp", "truncate", "unquantised_dst", "fused", "bottom_first")
 
@@ -31,23 +33,6 @@ def u8(x, truncate=False):
     """The float-to-unorm conversion of the drawing buffer: clamp(x) * 255 rounded to nearest even."""
     s = clamp(x) * F(255)
     return (np.trunc(s) if truncate else np.rint(s)).astype(np.uint8)
-
-
-def uv_grid(w, h):
-    """((i + .5) / w, (j + .5) / h) in fp32, (h, w) each, row 0 = bottom."""
-    uvx = (np.arange(w, dtype=F) + F(0.5)) / F(w)
-    uvy = (np.arange(h, dtype=F) + F(0.5)) / F(h)
-    return np.broadcast_to(uvx[None, :], (h, w)), np.broadcast_to(uvy[:, None], (h, w))
-
-
-def checkerboard(w, h, aspect):
-    """checkerboardShader (S:531-547) as the display kernel computes it: (h, w) fp32, row 0 = bottom."""
-    uvx, uvy = uv_grid(w, h)
-    x = np.floor((uvx * F(25)) * F(aspect))
-    y = np.floor((uvy * F(25)) * F(1))
-    sxy = x + y
-    v = sxy - F(2) * np.floor(sxy / F(2))
-    return v * F(0.1) + F(0.8)
 
 
 def background(w, h, back_rgb, transparent, aspect):

@@ -1,5 +1,6 @@
 """A per-texel interval for the display shader with BLOOM (displayShaderSource S:549-612, linearToGamma
-S:565-568), independent of the library: numpy plus the fetches of display_keywords_model.py.
+S:565-568), independent of the library: the powf bounds display_model.display builds it from, and the
+comparisons the tests make against it.
 
 Everything before linearToGamma's pow is fp32 arithmetic that numpy reproduces bit for bit in the
 kernel's order (no contraction; the library is built with --fmad=false): the LINEAR fetches of dye and
@@ -27,16 +28,13 @@ from __future__ import annotations
 
 import numpy as np
 
-import capture_model as CM
-import display_keywords_model as M
-from oracle import oracle as O
 from splat_model import check_splat, step_ulps
 
 F32 = np.float32
 # CUDA C++ Programming Guide, Mathematical Functions, single precision: powf(x, y) maximum error
 # 4 ulp (full range, without -use_fast_math)
 POWF_ULP = 4
-Y = M.GAMMA_EXPONENT
+Y = F32(0.416666667)                     # linearToGamma's exponent
 
 
 def pow_rn(bk, y=Y) -> np.ndarray:
@@ -54,48 +52,6 @@ def powf_bounds(bk, ulp: int = POWF_ULP):
     return lo, hi
 
 
-def gamma_interval(dye, w, h, keywords, bloom, sun, dither, scale=None):
-    """[lo, hi] of the display colour c + linearToGamma(bloom) of a w x h target, (h, w, 3) each, before
-    alpha and the background.  `scale`: getTextureScale of the target unless given."""
-    assert keywords & M.BLOOM, keywords
-    with np.errstate(invalid="ignore", over="ignore"):
-        c, bl = M.colour_terms(np.ascontiguousarray(dye, F32), w, h, keywords, bloom, sun)
-        bk = M.gamma_argument(bl, np.ascontiguousarray(dither, F32), w, h, scale)
-        plo, phi = powf_bounds(bk)
-        return c + M.linear_to_gamma(plo), c + M.linear_to_gamma(phi)
-
-
-def blend_interval(clo, chi, back_rgb, background, aspect):
-    """[lo, hi] (h, w, 4) of the frame from the colour interval: alpha and render()'s blend over the
-    background (O.BG_COLOR / BG_CHECKERBOARD), or bare (BG_NONE)."""
-    alo, ahi = M.alpha_of(clo), M.alpha_of(chi)
-    if background == O.BG_NONE:
-        return np.concatenate([clo, alo], axis=-1), np.concatenate([chi, ahi], axis=-1)
-    h, w = clo.shape[:2]
-    bg = M.background_colour(w, h, back_rgb, background, aspect)
-    one = F32(1)
-    with np.errstate(invalid="ignore", over="ignore"):
-        lo = np.concatenate([clo + bg * (one - ahi), alo + one * (one - ahi)], axis=-1)
-        hi = np.concatenate([chi + bg * (one - alo), ahi + one * (one - alo)], axis=-1)
-    return lo, hi
-
-
-def display_interval(dye, w, h, keywords, bloom, sun, dither, back_rgb, background, aspect):
-    """[lo, hi] of every value of render()'s frame with `keywords` (which include BLOOM)."""
-    clo, chi = gamma_interval(dye, w, h, keywords, bloom, sun, dither)
-    return blend_interval(clo, chi, back_rgb, background, aspect)
-
-
-def capture_interval(dye, w, h, canvas_w, canvas_h, dither, keywords, transparent, back_rgb, cfg=None, scale=None):
-    """[lo, hi] of every byte of captureScreenshot() with `keywords` (which include BLOOM), top row first:
-    the bloom and sunrays chains of the oracle at the canvas size, the display at the target size over
-    the fp16 background, then B.  `scale` overrides the target's getTextureScale (a negative control)."""
-    r = O.render_postfx(np.ascontiguousarray(dye, F32), canvas_w, canvas_h, np.ascontiguousarray(dither, F32), cfg=cfg)
-    clo, chi = gamma_interval(dye, w, h, keywords, r["bloom"], r["sunrays"], dither, scale)
-    lo, hi = blend_interval(clo, chi, CM.back16(back_rgb), O.BG_NONE if transparent else O.BG_COLOR, w / h)
-    return CM.to_bytes(lo)[::-1], CM.to_bytes(hi)[::-1]
-
-
 def check_display(got, lo, hi, limit: int = 8):
     """The values of `got` outside [lo, hi]: NaN where the interval is NaN and nowhere else, infinities
     exactly, the sign of a zero where both ends are that zero (check_splat's rule).  Returns (number of
@@ -105,7 +61,7 @@ def check_display(got, lo, hi, limit: int = 8):
 
 
 def bytes_outside(got, lo, hi) -> int:
-    """How many bytes of `got` lie outside [lo, hi] (capture_interval)."""
+    """How many bytes of `got` lie outside [lo, hi] (the byte bracket of display_model.capture)."""
     return int(np.count_nonzero((got < lo) | (got > hi)))
 
 

@@ -14,7 +14,7 @@ operation, built from what already exists:
                         host inputs too (they travel through fluid_write)
   splat, splats         splat_model.splat_interval: the handle's result is checked against the interval,
                         then ADOPTED, so that later operations stay comparable bit for bit
-  render, capture       display_keywords_model / half_postfx_model / gamma_model / capture_model; read-only
+  render, capture       display_model with the handle's storage; read-only
 
 Every array an operation writes is derived from the operation tuple alone (op_data), so a logged
 session can be replayed from its log.
@@ -29,10 +29,7 @@ from __future__ import annotations
 
 import numpy as np
 
-import capture_model as CM
-import display_keywords_model as M
-import gamma_model as G
-import half_postfx_model as HP
+import display_model as M
 import splat_model as SM
 from oracle import oracle as O
 from test_gpu_half_storage_special import special_fields
@@ -298,15 +295,6 @@ def host_inputs(W, H, seed, half: bool):
     return d, p
 
 
-def get_resolution(res, w, h):
-    """getResolution, S:1612-1624."""
-    ar = w / h
-    if ar < 1:
-        ar = 1.0 / ar
-    mn, mx = int(np.floor(res + 0.5)), int(np.floor(res * ar + 0.5))
-    return (mx, mn) if w > h else (mn, mx)
-
-
 # ---- the model ---------------------------------------------------------------------------------------
 class SessionModel:
     """What one handle holds.  config: the simulation keys the host mirror pushes live (SIM_KEYS)."""
@@ -391,35 +379,19 @@ class SessionModel:
         self.sim.dye = np.ascontiguousarray(dye, F32).copy()
 
     def render(self, keywords, background, dither, fxcfg):
-        """render() at the canvas size: the dict of render_keywords (target, bloom, sunrays)."""
+        """render() at the canvas size: display_model.render with the handle's storage (chains, target, and the
+        powf interval lo / hi with BLOOM)."""
         w, h = self.canvas
-        with np.errstate(invalid="ignore", over="ignore"):
-            if self.half:
-                return HP.render_keywords(self.sim.dye, w, h, dither, cfg=fxcfg, back_rgb=BACK_RGB, background=background,
-                                          aspect=w / h, keywords=keywords, half_targets=True, half_mask=True)
-            return M.render_keywords(self.sim.dye, w, h, dither, cfg=fxcfg, back_rgb=BACK_RGB, background=background,
-                                     aspect=w / h, keywords=keywords)
-
-    def frame_interval(self, keywords, background, dither, bloom, sun):
-        """[lo, hi] of a frame with BLOOM, from the handle's own (already checked) chains."""
-        w, h = self.canvas
-        with np.errstate(invalid="ignore", over="ignore"):
-            return G.display_interval(self.sim.dye, w, h, keywords, bloom, sun, dither, BACK_RGB, background, w / h)
+        return M.render(self.sim.dye, w, h, dither, keywords, fxcfg, back_rgb=BACK_RGB, background=background,
+                        aspect=w / h, half_targets=self.half, half_mask=self.half)
 
     def capture_size(self, capture_res):
-        return get_resolution(capture_res, *self.canvas)
+        return M.get_resolution(capture_res, *self.canvas)
 
     def capture(self, keywords, transparent, dither, fxcfg, capture_res):
-        """captureScreenshot(): ("exact", bytes) without BLOOM, ("interval", lo, hi) with it."""
+        """captureScreenshot(): display_model.capture with the handle's storage (rgba8, and the byte bracket
+        lo / hi with BLOOM)."""
         cw, ch = self.canvas
         w, h = self.capture_size(capture_res)
-        args = (self.sim.dye, w, h, cw, ch, dither, keywords, transparent, BACK_RGB)
-        with np.errstate(invalid="ignore", over="ignore"):
-            if self.half:
-                kw = dict(cfg=fxcfg, half_targets=True, half_mask=True)
-                if keywords & M.BLOOM:
-                    return ("interval",) + tuple(HP.capture_interval(*args, **kw))
-                return ("exact", HP.capture(*args, **kw)["rgba8"])
-            if keywords & M.BLOOM:
-                return ("interval",) + tuple(G.capture_interval(*args, cfg=fxcfg))
-            return ("exact", CM.capture(*args, cfg=fxcfg)["rgba8"])
+        return M.capture(self.sim.dye, w, h, cw, ch, dither, keywords, transparent, BACK_RGB, cfg=fxcfg,
+                         half_targets=self.half, half_mask=self.half)

@@ -26,8 +26,8 @@ def test_checkerboard_bytes_are_derived_in_fp32():
 
 
 def test_checkerboard_matches_the_display_model():
-    """The fp32 checkerboard is the one render() draws (display_keywords_model.background_colour)."""
-    import display_keywords_model as M
+    """The fp32 checkerboard is the one render() draws (display_model.background_colour)."""
+    import display_model as M
     from oracle import oracle as O
     for w, h in ((128, 128), (807, 640), (64, 48)):
         ours = CM.background(w, h, BLACK, True, w / h)

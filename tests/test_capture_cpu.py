@@ -1,4 +1,4 @@
-"""captureScreenshot() (S:287-349) on the CPU: the capture model (capture_model.py) against the executed
+"""captureScreenshot() (S:287-349) on the CPU: the capture model (display_model.py, capture_model.py) against the executed
 reference shaders (capture_*.npz), a negative control for the canvas-sized post-FX, the PNG writer, and
 the host-side mapping from `config` and the canvas to what fluid_capture is given.  Runs without a GPU."""
 import struct
@@ -8,13 +8,12 @@ import numpy as np
 import pytest
 
 import capture_model as CM
+import display_model as M
 import webgl_fluid_simulation_b200 as pkg
 from conftest import golden
 
 GEOMETRIES = {"pow2": "capture_64_canvas_128", "ragged": "capture_48x32_canvas_807x640"}
-SETS = {"none": 0, "shading": CM.SHADING, "bloom": CM.BLOOM, "shading_bloom": CM.SHADING | CM.BLOOM,
-        "sunrays": CM.SUNRAYS, "shading_sunrays": CM.SHADING | CM.SUNRAYS, "bloom_sunrays": CM.BLOOM | CM.SUNRAYS,
-        "shading_bloom_sunrays": CM.SHADING | CM.BLOOM | CM.SUNRAYS}
+SETS = M.SETS
 
 
 def executed_delta(geometry, kw):
@@ -23,14 +22,14 @@ def executed_delta(geometry, kw):
     ragged one."""
     if geometry == "ragged":
         return 3e-4
-    return 0.0 if not kw & (CM.BLOOM | CM.SUNRAYS) else 2e-6
+    return 0.0 if not kw & (M.BLOOM | M.SUNRAYS) else 2e-6
 
 
 def model(g, kw, fx_size=None):
-    return CM.capture(g["in_dye"], int(g["w"]), int(g["h"]), int(g["canvas_w"]), int(g["canvas_h"]),
-                      g["dither"].astype(np.float32), kw, bool(g["transparent"]),
-                      tuple(float(x) / 255 for x in g["back"]),
-                      cfg=dict(BLOOM_RESOLUTION=int(g["bloom_res"]), SUNRAYS_RESOLUTION=int(g["sun_res"])), fx_size=fx_size)
+    return M.capture(g["in_dye"], int(g["w"]), int(g["h"]), int(g["canvas_w"]), int(g["canvas_h"]),
+                     g["dither"].astype(np.float32), kw, bool(g["transparent"]),
+                     tuple(float(x) / 255 for x in g["back"]),
+                     cfg=dict(BLOOM_RESOLUTION=int(g["bloom_res"]), SUNRAYS_RESOLUTION=int(g["sun_res"])), fx_size=fx_size)
 
 
 @pytest.mark.parametrize("bg", ["back", "transparent"])
@@ -63,7 +62,7 @@ def test_target_sized_post_fx_fails_on_the_canvas_fixture(oracle, bg):
     assert pkg.getResolution(int(g["sun_res"]), 807, 640) == {"width": 50, "height": 40}
     assert pkg.getResolution(int(g["sun_res"]), w, h) == {"width": 51, "height": 40}
     for tag, kw in SETS.items():
-        if not kw & (CM.BLOOM | CM.SUNRAYS):
+        if not kw & (M.BLOOM | M.SUNRAYS):
             continue
         wrong = model(g, kw, fx_size=(w, h))
         assert CM.bytes_outside(g[f"{tag}_rgba8"], wrong["pre"], executed_delta("ragged", kw)) > 0, tag

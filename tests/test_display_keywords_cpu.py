@@ -1,11 +1,11 @@
-"""The display keyword sets of render() (updateKeywords, S:1160-1166) on the CPU: the keyword model
-(display_keywords_model.py, over the oracle) against the executed reference shaders for the five sets
+"""The display keyword sets of render() (updateKeywords, S:1160-1166) on the CPU: the display model
+(display_model.py, over the oracle's chains) against the executed reference shaders for the five sets
 that are neither none / SHADING (test_oracle_golden's display tests) nor all three (its postfx tests),
 and the host-side mapping from `config` to the keyword mask.  Runs without a GPU."""
 import numpy as np
 import pytest
 
-import display_keywords_model as M
+import display_model as M
 import webgl_fluid_simulation_b200 as pkg
 from conftest import bits_equal, golden, max_rel
 
@@ -16,9 +16,9 @@ KEYWORDS = {"bloom": pkg.DISPLAY_BLOOM, "sunrays": pkg.DISPLAY_SUNRAYS,
 
 
 def _render(O, g, keywords, background=0):
-    return M.render_keywords(g["in_dye"], int(g["w"]), int(g["h"]), g["dither"].astype(np.float32),
-                             cfg=dict(BLOOM_RESOLUTION=int(g["bloom_res"]), SUNRAYS_RESOLUTION=int(g["sun_res"])),
-                             back_rgb=tuple(float(x) / 255 for x in g["back"]), background=background, keywords=keywords)
+    return M.render(g["in_dye"], int(g["w"]), int(g["h"]), g["dither"].astype(np.float32), keywords,
+                    cfg=dict(BLOOM_RESOLUTION=int(g["bloom_res"]), SUNRAYS_RESOLUTION=int(g["sun_res"])),
+                    back_rgb=tuple(float(x) / 255 for x in g["back"]), background=background)
 
 
 def _check_chains(r, g, keywords, pow2):
@@ -73,15 +73,15 @@ def test_keyword_set_transparent_matches_executed_reference_shaders(oracle):
 def test_keyword_model_restates_the_oracle_display(oracle, keywords):
     """The model's numpy display shader against the oracle's C one where the oracle has it: without
     BLOOM and SUNRAYS bit for bit vs oracle.display, and with all three within pow()'s last places of
-    oracle.render_postfx (numpy's and glibc's powf round differently).  render_keywords returns the
-    oracle's own frames for those sets; this pins the restatement it uses for the five others."""
+    oracle.render_postfx (numpy's and glibc's powf round differently).  This pins the restatement the model draws every set
+    with."""
     g = golden("keywords_48x32_to_50x75")
     w, h = int(g["w"]), int(g["h"])
     full = oracle.render_postfx(g["in_dye"], w, h, g["dither"].astype(np.float32),
                                 cfg=dict(BLOOM_RESOLUTION=int(g["bloom_res"]), SUNRAYS_RESOLUTION=int(g["sun_res"])))
     for bg in (oracle.BG_COLOR, oracle.BG_CHECKERBOARD, oracle.BG_NONE):
-        mine = M._display(g["in_dye"], w, h, keywords, full["bloom"], full["sunrays"], g["dither"].astype(np.float32),
-                          tuple(float(x) / 255 for x in g["back"]), bg, w / h)
+        mine = M.display(g["in_dye"], w, h, keywords, full["bloom"], full["sunrays"], g["dither"].astype(np.float32),
+                         tuple(float(x) / 255 for x in g["back"]), bg, w / h)["target"]
         if not keywords & (pkg.DISPLAY_BLOOM | pkg.DISPLAY_SUNRAYS):
             ref = oracle.display(g["in_dye"], w, h, bool(keywords & pkg.DISPLAY_SHADING),
                                  tuple(float(x) / 255 for x in g["back"]), bg)

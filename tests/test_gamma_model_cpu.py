@@ -1,4 +1,4 @@
-"""Premises of the per-texel display interval (tests/gamma_model.py), on the CPU:
+"""Premises of the per-texel display interval (display_model.display, tests/gamma_model.py), on the CPU:
 
 * the oracle (glibc powf, within 1 ulp) lies inside it at every texel, under every background, on the
   inputs the GPU file draws: the executed-shader goldens, seeded, zero and dim dye (bk across the knee
@@ -19,48 +19,18 @@ pins both halves."""
 import numpy as np
 import pytest
 
-import capture_model as CM
-import display_keywords_model as M
+import display_model as M
 import gamma_model as G
 from conftest import golden
+from display_harness import BACK_RGB, BACKGROUNDS, FXCFG, golden_dither, nonfinite_dye, seeded_dye
+from oracle import oracle as O
 
 F32 = np.float32
-ALL3 = M.SHADING | M.BLOOM | M.SUNRAYS
+ALL3 = M.ALL3
 BLOOM_SETS = [M.BLOOM, M.SHADING | M.BLOOM, M.BLOOM | M.SUNRAYS, ALL3]
-BACK_RGB = (10 / 255, 20 / 255, 30 / 255)
-FXCFG = dict(BLOOM_RESOLUTION=64, SUNRAYS_RESOLUTION=48)
 # dim dye (seeded_dye(scale=1) * 0.25) with bloom this faint puts bk on both sides of linearToGamma's knee
 # (fmaxf(1.055 p - 0.055, 0) = 0 below bk = 8.3e-4): about 10 % of values at 0, 10 % between 0 and the knee
 DIM_CFG = dict(FXCFG, BLOOM_INTENSITY=0.005, BLOOM_THRESHOLD=0.0)
-
-
-def seeded_dye(Wd, Hd, seed, scale=3.0):
-    rng = np.random.default_rng(seed)
-    dye = (rng.random((Hd, Wd, 4), dtype=F32) ** 4 * F32(scale)).astype(F32)
-    dye[..., 3] = 1
-    return dye
-
-
-def nonfinite_dye(Wd, Hd, seed):
-    """Seeded dye with +-inf, NaN, -2, a subnormal and 1e30 in whole texels and in single channels: at
-    the four corners, along the four edges and inside."""
-    dye = seeded_dye(Wd, Hd, seed)
-    specials = [np.inf, -np.inf, np.nan, -2.0, 1e-40, 1e30]
-    rng = np.random.default_rng(seed + 1)
-    spots = [(0, 0), (0, Wd - 1), (Hd - 1, 0), (Hd - 1, Wd - 1), (0, Wd // 2), (Hd - 1, Wd // 3),
-             (Hd // 2, 0), (Hd // 3, Wd - 1)] + [tuple(rng.integers(1, (Hd - 1, Wd - 1))) for _ in range(16)]
-    for k, (j, i) in enumerate(spots):
-        v = F32(specials[k % len(specials)])
-        if k < 12:
-            dye[j, i, :3] = v                    # the whole colour
-        else:                                    # one channel of a bright texel
-            dye[j, i, :3] = 2.0
-            dye[j, i, k % 3] = v
-    return dye
-
-
-def golden_dither():
-    return golden("postfx_64_to_128")["dither"].astype(F32)
 
 
 def wide_dither(seed, shape=(64, 64)):
@@ -111,7 +81,6 @@ def make_cases():
 
 
 CASES = make_cases()
-BACKGROUNDS = {"back": M.O.BG_COLOR, "checker": M.O.BG_CHECKERBOARD, "bare": M.O.BG_NONE}
 
 
 def oracle_frame(O, c, background):
@@ -124,9 +93,9 @@ def oracle_frame(O, c, background):
 def test_oracle_inside_interval(oracle, name, bg):
     c = CASES[name]
     r = oracle_frame(oracle, c, BACKGROUNDS[bg])
-    lo, hi = G.display_interval(c["dye"], c["w"], c["h"], ALL3, r["bloom"], r["sunrays"], c["dither"], BACK_RGB,
-                                BACKGROUNDS[bg], c["w"] / c["h"])
-    n, bad = G.check_display(r["target"], lo, hi)
+    d = M.display(c["dye"], c["w"], c["h"], ALL3, r["bloom"], r["sunrays"], c["dither"], BACK_RGB, BACKGROUNDS[bg],
+                  c["w"] / c["h"])
+    n, bad = G.check_display(r["target"], d["lo"], d["hi"])
     assert n == 0, (n, bad)
 
 
@@ -135,7 +104,7 @@ def unclamped_argument(c, bl):
     w, h, dither = c["w"], c["h"], c["dither"]
     dsx, dsy = M.dither_scale(w, h, dither)
     uvx, uvy = M.uv_grid(w, h)
-    noise = M._fetch(dither, uvx * dsx, uvy * dsy, repeat=True)[..., :1] * F32(2) - F32(1)
+    noise = M.linear_fetch(dither, uvx * dsx, uvy * dsy, repeat=True)[..., :1] * F32(2) - F32(1)
     return bl + noise / F32(255)
 
 
@@ -172,8 +141,8 @@ def test_model_equals_oracle_on_nonfinite_dye(oracle, shading, bg):
     """none / SHADING: the model's display shader == oracle.display, NaN in the same places."""
     c = CASES["nonfinite"]
     with np.errstate(invalid="ignore", over="ignore"):
-        mine = M._display(c["dye"], c["w"], c["h"], M.SHADING if shading else 0, None, None, None, BACK_RGB,
-                          BACKGROUNDS[bg], c["w"] / c["h"])
+        mine = M.display(c["dye"], c["w"], c["h"], M.SHADING if shading else 0, None, None, None, BACK_RGB,
+                         BACKGROUNDS[bg], c["w"] / c["h"])["target"]
     ref = oracle.display(c["dye"], c["w"], c["h"], shading, BACK_RGB, BACKGROUNDS[bg])
     assert np.isnan(ref).any()
     assert G.same_bits(mine, ref)
@@ -204,7 +173,7 @@ def test_powf_bounds_special_cases():
 # the interval must accept the unchanged restatement everywhere and reject each mutant on hundreds of
 # texels of at least one input.
 MUTANT_INPUTS = ["seeded", "zero", "dim", "wide_dither"]
-MUTANT_BACKGROUNDS = [M.O.BG_COLOR, M.O.BG_NONE]
+MUTANT_BACKGROUNDS = [O.BG_COLOR, O.BG_NONE]
 
 
 def restate(c, r, background, power=None, gamma=M.linear_to_gamma, repeat=True, alpha_before_bloom=False):
@@ -212,13 +181,7 @@ def restate(c, r, background, power=None, gamma=M.linear_to_gamma, repeat=True, 
     w, h, dither = c["w"], c["h"], c["dither"]
     with np.errstate(invalid="ignore", over="ignore", divide="ignore"):
         col, bl = M.colour_terms(c["dye"], w, h, ALL3, r["bloom"], r["sunrays"])
-        if repeat:
-            bk = M.gamma_argument(bl, dither, w, h)
-        else:
-            dsx, dsy = M.dither_scale(w, h, dither)
-            uvx, uvy = M.uv_grid(w, h)
-            noise = M._fetch(dither, uvx * dsx, uvy * dsy)[..., :1] * F32(2) - F32(1)
-            bk = np.fmax(bl + noise / F32(255), F32(0))
+        bk = M.gamma_argument(bl, dither, w, h, repeat=repeat)
         p = np.power(bk, G.Y) if power is None else power(bk)
         out = col + gamma(p)
         a = M.alpha_of(col if alpha_before_bloom else out)
@@ -227,15 +190,15 @@ def restate(c, r, background, power=None, gamma=M.linear_to_gamma, repeat=True, 
 
 def rejected(mutant_kwargs):
     """{input: texels rejected, summed over MUTANT_BACKGROUNDS}."""
-    from oracle import oracle as O
     out = {}
     for name in MUTANT_INPUTS:
         c = CASES[name]
         r = oracle_frame(O, c, 0)
         n = 0
         for bg in MUTANT_BACKGROUNDS:
-            lo, hi = G.display_interval(c["dye"], c["w"], c["h"], ALL3, r["bloom"], r["sunrays"], c["dither"], BACK_RGB,
-                                        bg, c["w"] / c["h"])
+            d = M.display(c["dye"], c["w"], c["h"], ALL3, r["bloom"], r["sunrays"], c["dither"], BACK_RGB, bg,
+                          c["w"] / c["h"])
+            lo, hi = d["lo"], d["hi"]
             good = restate(c, r, bg)
             assert G.check_display(good, lo, hi)[0] == 0, name
             bad = restate(c, r, bg, **mutant_kwargs)
@@ -283,18 +246,13 @@ def test_mutant_dither_scale_of_the_canvas_in_capture_is_rejected(oracle):
     cfg = dict(BLOOM_RESOLUTION=int(g["bloom_res"]), SUNRAYS_RESOLUTION=int(g["sun_res"]))
     w, h, cw, ch = int(g["w"]), int(g["h"]), int(g["canvas_w"]), int(g["canvas_h"])
     assert (w, cw) == (64, 128)
-    r = oracle.render_postfx(dye, cw, ch, dither, cfg=cfg)
-    col, bl = M.colour_terms(dye, w, h, ALL3, r["bloom"], r["sunrays"])
-    bk = M.gamma_argument(bl, dither, w, h, scale=M.dither_scale(cw, ch, dither))
-    out = col + M.linear_to_gamma(np.power(bk, G.Y))
     n = 0
     for transparent in (False, True):
-        lo, hi = G.capture_interval(dye, w, h, cw, ch, dither, ALL3, transparent, BACK_RGB, cfg=cfg)
-        good = CM.capture(dye, w, h, cw, ch, dither, ALL3, transparent, BACK_RGB, cfg=cfg)["rgba8"]
-        assert G.bytes_outside(good, lo, hi) == 0
-        bad = M.over_background(out, M.alpha_of(out), CM.back16(BACK_RGB), M.O.BG_NONE if transparent else M.O.BG_COLOR,
-                                w / h)
-        n += G.bytes_outside(CM.to_bytes(bad)[::-1], lo, hi)
+        good = M.capture(dye, w, h, cw, ch, dither, ALL3, transparent, BACK_RGB, cfg=cfg)
+        assert G.bytes_outside(good["rgba8"], good["lo"], good["hi"]) == 0
+        bad = M.capture(dye, w, h, cw, ch, dither, ALL3, transparent, BACK_RGB, cfg=cfg,
+                        scale=M.dither_scale(cw, ch, dither))["rgba8"]
+        n += G.bytes_outside(bad, good["lo"], good["hi"])
     assert n >= 300, n
 
 

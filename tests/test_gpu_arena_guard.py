@@ -19,13 +19,10 @@ import numpy as np
 import pytest
 
 import arena_model as A
-import nearest_model as N
+import display_harness as DH
+import display_model as DM
 import splat_model as SM
-import test_gpu_display_keywords as DK
-import test_gpu_half_postfx as HPT
-import test_gpu_nearest_filtering as NF
 from conftest import bits_equal
-from test_gamma_model_cpu import golden_dither
 from test_gpu_fast_paths import same_or_both_nan
 from test_gpu_jacobi_range import near_max_patch
 from test_gpu_parity import STREAM_SHAPES, make, rand_fields
@@ -413,7 +410,6 @@ def test_whole_step(pkg, torch, oracle, W, H, Wd, Hd, mode):
 
 
 FRAME_GEOMETRIES = [(64, 64, 128, 128), (48, 32, 50, 75)]
-FX = dict(BLOOM_RESOLUTION=64, SUNRAYS_RESOLUTION=48)
 
 
 @pytest.mark.parametrize("handle", ["fp32", "half_half_postfx", "nearest"])
@@ -422,39 +418,27 @@ def test_frames_and_captures(pkg, torch, oracle, handle, Wd, Hd, w, h):
     """render() with all eight keyword sets: the arena is untouched except dye.write with SUNRAYS (the mask),
     and with dye.write poisoned the frame equals the display model.  captureScreenshot() the same way; its
     bytes equal the capture this handle drew before anything was poisoned."""
-    dither = golden_dither()
-    dye_in = DK.seeded_dye(Wd, Hd, Wd + w)
-    if handle == "fp32":
-        s = DK.make(pkg, Wd, Hd, w, h)
-        dye = dye_in
-    elif handle == "nearest":
-        s = NF.make(pkg, Wd, Hd, w, h, NF.flags_of(pkg, "fp32"))
-        dye = dye_in
-    else:
-        s = HPT.make(pkg, Wd, Hd, w, h, "half")
-        dye = oracle.round_half(dye_in)
+    kind = "nearest_fp32" if handle == "nearest" else handle
+    dither = DH.golden_dither()
+    dye = DH.stored(kind, DH.seeded_dye(Wd, Hd, Wd + w))
+    s = DH.make(pkg, Wd, Hd, w, h, DH.flags_of(pkg, kind))
     s.config["CAPTURE_RESOLUTION"] = min(w, h)
     s.writeField("dye", dye)
     s.dithering = dither
     clean = []
     for kw in range(8):
-        DK.set_keywords(pkg, s, kw)
+        DH.set_keywords(s, kw)
         clean.append(s.captureScreenshot())
     g = Arena(torch, s, handle.startswith("half"))
     with np.errstate(invalid="ignore", over="ignore"):
         for kw in range(8):
-            DK.set_keywords(pkg, s, kw)
+            DH.set_keywords(s, kw)
+            want = DH.model_frame(kind, dye, w, h, kw, dither, DH.FXCFG, oracle.BG_COLOR)
             call = "render_sunrays" if kw & pkg.DISPLAY_SUNRAYS else "render"
             frames, caps = [], []
             for value in POISONS:
                 got = g.run(call, lambda: s.render(w, h), ("dye",), value, swaps=())
-                if handle == "fp32":
-                    ref = DK.M.render_keywords(dye, w, h, dither, cfg=FX, back_rgb=DK.BACK_RGB, keywords=kw)
-                    DK.check_vs_oracle(pkg, s, got, ref, kw, dye, dither)
-                elif handle == "nearest":
-                    NF.check_frame(s, got, dye, w, h, kw, dither, FX, "back", "fp32")
-                else:
-                    HPT.check_frame(s, got, dye, w, h, kw, dither, FX, "back", half_mask=True)
+                DH.check_frame(s, got, want, kw, (handle, kw, hex(value)))
                 frames.append(got)
                 caps.append(g.run(call, lambda: s.captureScreenshot(), ("dye",), value, swaps=()))
                 assert np.array_equal(caps[-1], clean[kw]), (kw, hex(value))
@@ -480,7 +464,7 @@ def test_resize_builds_a_clean_arena(pkg, torch, oracle, mode, src, dst):
     v, dye, p = (R(a) for a in rand_fields(*src, 41))
     W, H, Wd, Hd = dst
     if mode == "nearest":
-        v2, dye2 = N.resize(v, W, H), N.resize(dye, Wd, Hd)
+        v2, dye2 = DM.resize(v, W, H), DM.resize(dye, Wd, Hd)
     else:
         v2 = v if (W, H) == src[:2] else R(O.resample(v, W, H))
         dye2 = R(O.resample(dye, Wd, Hd))

@@ -9,18 +9,16 @@ import pytest
 
 import arena_model as A
 import canvas_model as CM
-from conftest import golden
+from display_harness import BACK, BACK_RGB, flags_of, golden_dither, make, set_keywords
+from display_model import ALL3, BLOOM, SHADING, SUNRAYS
 from test_gpu_arena_guard import POISONS, Arena
 
 pytestmark = pytest.mark.gpu
 F = np.float32
-SHADING, BLOOM, SUNRAYS = 0x1, 0x2, 0x4
-ALL3 = SHADING | BLOOM | SUNRAYS
-BACK = {"r": 10, "g": 20, "b": 30}
-BACK_RGB = (10 / 255, 20 / 255, 30 / 255)
 # (dye w, dye h, canvas w, canvas h, plant fused-rule witnesses): the capture goldens' geometries, and one
 # where the canvas samples the dye at its texel centres, so planted texels reach the fragment unchanged
 GEOMETRIES = [(64, 64, 128, 128, False), (48, 32, 807, 640, False), (64, 64, 64, 64, True)]
+KINDS = {"fp32": "fp32", "half": "half_half_postfx", "nearest": "nearest_fp32"}
 
 
 @pytest.fixture(scope="module")
@@ -38,22 +36,11 @@ def torch():
 
 @pytest.fixture(scope="module")
 def dither():
-    return golden("postfx_64_to_128")["dither"].astype(np.float32)
+    return golden_dither()
 
 
 def mode_flags(pkg, mode):
-    return {"fp32": 0, "half": pkg.FLAG_HALF_STORAGE | pkg.FLAG_HALF_POSTFX, "nearest": pkg.FLAG_NEAREST_FILTERING}[mode]
-
-
-def make(pkg, Wd, Hd, cw, ch, flags=0, **cfg):
-    s = pkg.FluidSimulation({"SIM_RESOLUTION": 16, "DYE_RESOLUTION": min(Wd, Hd)}, canvas_width=cw, canvas_height=ch,
-                            flags=flags, sizes=(16, 16, Wd, Hd))
-    s.config.update({"BACK_COLOR": BACK, "BLOOM_RESOLUTION": 64, "SUNRAYS_RESOLUTION": 48, **cfg})
-    return s
-
-
-def set_keywords(s, kw):
-    s.config.update(SHADING=bool(kw & SHADING), BLOOM=bool(kw & BLOOM), SUNRAYS=bool(kw & SUNRAYS))
+    return flags_of(pkg, KINDS[mode])
 
 
 def seeded_dye(Wd, Hd, seed, special=True):

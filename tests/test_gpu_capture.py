@@ -1,4 +1,4 @@
-"""captureScreenshot() (S:287-327) on the GPU: fluid_capture against the CPU model (capture_model.py) and the
+"""captureScreenshot() (S:287-327) on the GPU: fluid_capture against the CPU model (display_model.py) and the
 executed reference shaders (capture_*.npz) under the byte tolerance rule, bit for bit against the fp32
 render() path it fuses, the kernels it launches, what it leaves alone, and what it refuses."""
 import ctypes as C
@@ -7,16 +7,12 @@ import numpy as np
 import pytest
 
 import capture_model as CM
-import gamma_model as G
+import display_model as M
 from conftest import bits_equal, golden
+from display_harness import BACK_RGB, check_capture, golden_dither, make, model_capture, seeded_dye, set_keywords
 
 pytestmark = pytest.mark.gpu
-BACK = {"r": 10, "g": 20, "b": 30}
-BACK_RGB = (10 / 255, 20 / 255, 30 / 255)
 GEOMETRIES = ["capture_64_canvas_128", "capture_48x32_canvas_807x640"]
-SETS = {"none": 0, "shading": CM.SHADING, "bloom": CM.BLOOM, "shading_bloom": CM.SHADING | CM.BLOOM,
-        "sunrays": CM.SUNRAYS, "shading_sunrays": CM.SHADING | CM.SUNRAYS, "bloom_sunrays": CM.BLOOM | CM.SUNRAYS,
-        "shading_bloom_sunrays": CM.SHADING | CM.BLOOM | CM.SUNRAYS}
 
 
 @pytest.fixture(scope="module")
@@ -27,25 +23,7 @@ def pkg():
 
 @pytest.fixture(scope="module")
 def dither():
-    return golden("postfx_64_to_128")["dither"].astype(np.float32)
-
-
-def make(pkg, Wd, Hd, canvas_w, canvas_h, flags=0, **cfg):
-    s = pkg.FluidSimulation({"SIM_RESOLUTION": 16, "DYE_RESOLUTION": min(Wd, Hd)}, canvas_width=canvas_w,
-                            canvas_height=canvas_h, flags=flags, sizes=(16, 16, Wd, Hd))
-    s.config.update(BACK_COLOR=BACK, **cfg)
-    return s
-
-
-def seeded_dye(Wd, Hd, seed):
-    rng = np.random.default_rng(seed)
-    dye = (rng.random((Hd, Wd, 4), dtype=np.float32) ** 4).astype(np.float32)
-    dye[..., 3] = 1
-    return dye
-
-
-def set_keywords(s, kw):
-    s.config.update(SHADING=bool(kw & CM.SHADING), BLOOM=bool(kw & CM.BLOOM), SUNRAYS=bool(kw & CM.SUNRAYS))
+    return golden_dither()
 
 
 def outside_executed(got, half, delta):
@@ -77,18 +55,15 @@ def test_capture_vs_model_and_executed_shaders(pkg, name):
                  SUNRAYS_RESOLUTION=int(g["sun_res"]), TRANSPARENT=bool(g["transparent"]))
         s.writeField("dye", g["in_dye"])
         s.dithering = g["dither"].astype(np.float32)
-        for tag, kw in SETS.items():
+        for tag, kw in M.SETS.items():
             set_keywords(s, kw)
             got = s.captureScreenshot()
             assert got.dtype == np.uint8 and got.shape == (int(g["h"]), int(g["w"]), 4)
-            args = (g["in_dye"], int(g["w"]), int(g["h"]), int(g["canvas_w"]), int(g["canvas_h"]),
-                    g["dither"].astype(np.float32), kw, bool(g["transparent"]), BACK_RGB)
             cfg = dict(BLOOM_RESOLUTION=int(g["bloom_res"]), SUNRAYS_RESOLUTION=int(g["sun_res"]))
-            if kw & CM.BLOOM:
-                assert G.bytes_outside(got, *G.capture_interval(*args, cfg=cfg)) == 0, (name, bg, tag)
-            else:
-                assert np.array_equal(got, CM.capture(*args, cfg=cfg)["rgba8"]), (name, bg, tag)
-            if pow2 and not kw & (CM.BLOOM | CM.SUNRAYS):
+            want = model_capture("fp32", g["in_dye"], int(g["w"]), int(g["h"]), int(g["canvas_w"]), int(g["canvas_h"]), kw,
+                                 g["dither"].astype(np.float32), cfg, bool(g["transparent"]))
+            check_capture(got, want, kw, (name, bg, tag))
+            if pow2 and not kw & (M.BLOOM | M.SUNRAYS):
                 assert np.array_equal(got, g[f"{tag}_rgba8"]), (name, bg, tag)
             else:
                 delta = 2e-6 if pow2 else 3e-4
@@ -104,7 +79,7 @@ def test_capture_equals_quantised_render_frame(pkg, dither, Wd, Hd, w, h):
     through the same.  All eight sets."""
     s = make(pkg, Wd, Hd, w, h, CAPTURE_RESOLUTION=min(w, h), BLOOM_RESOLUTION=32, SUNRAYS_RESOLUTION=24)
     s.config["BACK_COLOR"] = {"r": 0, "g": 0, "b": 0}
-    s.writeField("dye", seeded_dye(Wd, Hd, 11))
+    s.writeField("dye", seeded_dye(Wd, Hd, 11, scale=1.0))
     s.dithering = dither
     assert pkg.capture_inputs(s.config, w, h, dither)["width"] == w
     for kw in range(8):
@@ -124,11 +99,11 @@ def test_capture_launches_what_render_launches(pkg, dither, iterations, levels):
     it reuses the post-FX targets (remaking the bloom FBO would add a fill_alpha_kernel launch)."""
     s = make(pkg, 64, 64, 128, 128, CAPTURE_RESOLUTION=64, BLOOM_RESOLUTION=64, SUNRAYS_RESOLUTION=48,
              BLOOM_ITERATIONS=iterations)
-    s.writeField("dye", seeded_dye(64, 64, 5))
+    s.writeField("dye", seeded_dye(64, 64, 5, scale=1.0))
     s.dithering = dither
     for kw in range(8):
         set_keywords(s, kw)
-        want = 1 + (4 if kw & CM.SUNRAYS else 0) + (2 * levels + 1 if kw & CM.BLOOM and levels >= 2 else 0)
+        want = 1 + (4 if kw & M.SUNRAYS else 0) + (2 * levels + 1 if kw & M.BLOOM and levels >= 2 else 0)
         s.render(128, 128)
         n0 = s.launch_count()
         s.render(128, 128)
@@ -145,7 +120,7 @@ def test_capture_launches_what_render_launches(pkg, dither, iterations, levels):
 def test_capture_leaves_dye_and_render_alone(pkg, dither):
     """dye.read is unchanged by a capture (SUNRAYS draws its mask into dye.write, as the reference does), and
     the render() after it is the render() before it: FLUID_BACKGROUND (the checkerboard here) is untouched."""
-    dye = seeded_dye(64, 48, 9)
+    dye = seeded_dye(64, 48, 9, scale=1.0)
     s = make(pkg, 64, 48, 128, 96, CAPTURE_RESOLUTION=48, BLOOM_RESOLUTION=32, SUNRAYS_RESOLUTION=24, TRANSPARENT=True)
     s.writeField("dye", dye)
     s.dithering = dither
@@ -167,7 +142,7 @@ def test_half_storage_capture(pkg, oracle, dither):
     kernel and the display."""
     s = make(pkg, 64, 64, 64, 64, flags=pkg.FLAG_HALF_STORAGE, CAPTURE_RESOLUTION=64)
     s.config["BACK_COLOR"] = {"r": 0, "g": 0, "b": 0}
-    s.writeField("dye", oracle.round_half(seeded_dye(64, 64, 3)))
+    s.writeField("dye", oracle.round_half(seeded_dye(64, 64, 3, scale=1.0)))
     s.dithering = dither
     for bloom, sunrays in ((True, False), (False, True), (True, True)):
         s.config.update(SHADING=True, BLOOM=bloom, SUNRAYS=sunrays)
@@ -189,20 +164,20 @@ def test_half_storage_capture(pkg, oracle, dither):
 def test_refusals_leave_the_handle_usable(pkg, dither):
     """Every bad argument gets FLUID_ERR_INVALID, and the next good capture on the same handle succeeds."""
     s = make(pkg, 64, 64, 128, 128, CAPTURE_RESOLUTION=64, BLOOM_RESOLUTION=64, SUNRAYS_RESOLUTION=48)
-    s.writeField("dye", seeded_dye(64, 64, 7))
+    s.writeField("dye", seeded_dye(64, 64, 7, scale=1.0))
     s.dithering = dither
     s.config.update(SHADING=True, BLOOM=True, SUNRAYS=True)
     _, fx, dith = pkg.postfx_inputs(s.config, dither)
     good = s.captureScreenshot()
     out = np.empty((64, 64, 4), np.uint8)
     ptr = lambda a: a.ctypes.data_as(C.c_void_p)        # noqa: E731
-    all3 = CM.SHADING | CM.BLOOM | CM.SUNRAYS
+    all3 = M.SHADING | M.BLOOM | M.SUNRAYS
 
     def call(w=64, h=64, cw=128, ch=128, kw=all3, fx_=C.byref(fx), d=ptr(dith), n=out.size, dst=ptr(out)):
         return s._L.fluid_capture(s._h, w, h, cw, ch, kw, 0, fx_, d, dith.shape[1], dith.shape[0], *BACK_RGB, dst, n)
 
     bad = [dict(kw=8), dict(kw=all3 | 0x10), dict(n=out.size - 1), dict(n=out.size + 4), dict(w=0), dict(h=0),
-           dict(cw=0), dict(ch=-1), dict(kw=CM.BLOOM, d=None), dict(kw=CM.BLOOM, fx_=None), dict(kw=CM.SUNRAYS, fx_=None),
+           dict(cw=0), dict(ch=-1), dict(kw=M.BLOOM, d=None), dict(kw=M.BLOOM, fx_=None), dict(kw=M.SUNRAYS, fx_=None),
            dict(dst=None)]
     for b in bad:
         assert call(**b) == -1, b
@@ -215,7 +190,7 @@ def test_capture_writes_png(pkg, dither, tmp_path):
     """captureScreenshot(path) writes the returned bytes as an RGBA PNG."""
     import zlib
     s = make(pkg, 64, 64, 128, 128, CAPTURE_RESOLUTION=64)
-    s.writeField("dye", seeded_dye(64, 64, 1))
+    s.writeField("dye", seeded_dye(64, 64, 1, scale=1.0))
     p = tmp_path / "fluid.png"
     img = s.captureScreenshot(str(p))
     data = p.read_bytes()

@@ -1,19 +1,15 @@
 """render() with every display keyword set (updateKeywords, S:1160-1166) on the GPU: fluid_render_keywords
-against the CPU model over the oracle (display_keywords_model.py) and the executed reference shaders,
+against the CPU model over the oracle (display_model.py) and the executed reference shaders,
 the passes it launches, the reuse of its post-FX targets across frames, and what it refuses."""
 import ctypes as C
 
 import numpy as np
 import pytest
 
-import display_keywords_model as M
-import gamma_model as G
 from conftest import bits_equal, golden, max_rel
+from display_harness import BACK_RGB, FXCFG, check_frame, golden_dither, make, model_frame, seeded_dye, set_keywords
 
 pytestmark = pytest.mark.gpu
-FXCFG = dict(BLOOM_RESOLUTION=64, SUNRAYS_RESOLUTION=48)
-BACK = {"r": 10, "g": 20, "b": 30}
-BACK_RGB = (10 / 255, 20 / 255, 30 / 255)
 
 
 @pytest.fixture(scope="module")
@@ -24,45 +20,7 @@ def pkg():
 
 @pytest.fixture(scope="module")
 def dither():
-    return golden("postfx_64_to_128")["dither"].astype(np.float32)
-
-
-def make(pkg, Wd, Hd, w, h, flags=0):
-    s = pkg.FluidSimulation({"SIM_RESOLUTION": 16, "DYE_RESOLUTION": min(Wd, Hd)}, canvas_width=w, canvas_height=h,
-                            flags=flags, sizes=(16, 16, Wd, Hd))
-    s.config.update(BACK_COLOR=BACK, **FXCFG)
-    return s
-
-
-def seeded_dye(Wd, Hd, seed):
-    rng = np.random.default_rng(seed)
-    dye = (rng.random((Hd, Wd, 4), dtype=np.float32) ** 4 * 3).astype(np.float32)
-    dye[..., 3] = 1
-    return dye
-
-
-def set_keywords(pkg, s, kw):
-    s.config.update(SHADING=bool(kw & pkg.DISPLAY_SHADING), BLOOM=bool(kw & pkg.DISPLAY_BLOOM),
-                    SUNRAYS=bool(kw & pkg.DISPLAY_SUNRAYS))
-
-
-def check_vs_oracle(pkg, s, got, ref, kw, dye, dither, background=M.O.BG_COLOR):
-    """Sets without BLOOM: frame bitwise.  With BLOOM: bloom FBO bitwise, every value of the frame within
-    the per-texel powf interval of gamma_model.py.  With SUNRAYS: sunrays texture bitwise.  The textures
-    of keywords that are off are not returned."""
-    if kw & pkg.DISPLAY_BLOOM:
-        assert bits_equal(s.last_bloom, ref["bloom"])
-        h, w = got.shape[:2]
-        lo, hi = G.display_interval(dye, w, h, kw, s.last_bloom, s.last_sunrays, dither, BACK_RGB, background, w / h)
-        n, bad = G.check_display(got, lo, hi)
-        assert n == 0, (kw, background, n, bad)
-    else:
-        assert bits_equal(got, ref["target"])
-        assert s.last_bloom is None
-    if kw & pkg.DISPLAY_SUNRAYS:
-        assert bits_equal(s.last_sunrays, ref["sunrays"])
-    else:
-        assert s.last_sunrays is None
+    return golden_dither()
 
 
 @pytest.mark.parametrize("Wd,Hd,w,h", [(64, 64, 128, 128), (48, 32, 50, 75)])
@@ -74,13 +32,12 @@ def test_every_keyword_set_and_background_vs_oracle(pkg, oracle, dither, Wd, Hd,
     s.writeField("dye", dye)
     s.dithering = dither
     for kw in range(8):
-        set_keywords(pkg, s, kw)
+        set_keywords(s, kw)
         for bg, transparent, target in ((oracle.BG_COLOR, False, False), (oracle.BG_CHECKERBOARD, True, False),
                                         (oracle.BG_NONE, True, True)):
             s.config["TRANSPARENT"] = transparent
             got = s.render(w, h, target=target)
-            ref = M.render_keywords(dye, w, h, dither, cfg=FXCFG, back_rgb=BACK_RGB, background=bg, keywords=kw)
-            check_vs_oracle(pkg, s, got, ref, kw, dye, dither, bg)
+            check_frame(s, got, model_frame("fp32", dye, w, h, kw, dither, FXCFG, bg), kw, (kw, bg))
             assert bits_equal(s.readField("dye"), dye), (kw, bg)
     s.close()
 
@@ -117,7 +74,7 @@ def test_only_enabled_passes_launch(pkg, dither, iterations, levels):
     s.dithering = dither
     s.config["BLOOM_ITERATIONS"] = iterations
     for kw in range(8):
-        set_keywords(pkg, s, kw)
+        set_keywords(s, kw)
         s.render(128, 128)
         n0 = s.launch_count()
         s.render(128, 128)
@@ -135,7 +92,7 @@ def test_post_fx_targets_are_reused_and_remade_on_resize(pkg, oracle, dither):
     s.writeField("dye", dye)
     s.dithering = dither
     kw = pkg.DISPLAY_SHADING | pkg.DISPLAY_BLOOM | pkg.DISPLAY_SUNRAYS
-    set_keywords(pkg, s, kw)
+    set_keywords(s, kw)
     frames = [(128, 96, dict(BLOOM_RESOLUTION=64, BLOOM_ITERATIONS=8, SUNRAYS_RESOLUTION=48)),
               (90, 160, dict(BLOOM_RESOLUTION=40, BLOOM_ITERATIONS=3, SUNRAYS_RESOLUTION=30)),
               (128, 96, dict(BLOOM_RESOLUTION=64, BLOOM_ITERATIONS=8, SUNRAYS_RESOLUTION=48)),
@@ -144,8 +101,7 @@ def test_post_fx_targets_are_reused_and_remade_on_resize(pkg, oracle, dither):
         s.config.update(fx)
         s.canvas = {"width": w, "height": h}
         got = s.render(w, h)
-        ref = M.render_keywords(dye, w, h, dither, cfg=fx, back_rgb=BACK_RGB, keywords=kw)
-        check_vs_oracle(pkg, s, got, ref, kw, dye, dither)
+        check_frame(s, got, model_frame("fp32", dye, w, h, kw, dither, fx, oracle.BG_COLOR), kw, (w, h))
     assert np.all(s.last_bloom == np.array([0, 0, 0, 1], np.float32))
     s.close()
 
@@ -179,7 +135,7 @@ def test_refusals_leave_the_handle_usable(pkg, dither, entry):
     s.writeField("dye", seeded_dye(64, 64, 7))
     s.dithering = dither
     all3 = pkg.DISPLAY_SHADING | pkg.DISPLAY_BLOOM | pkg.DISPLAY_SUNRAYS
-    set_keywords(pkg, s, all3)
+    set_keywords(s, all3)
     _, fx, dith = pkg.postfx_inputs(s.config, dither)
     out = np.empty((128, 128, 4), np.float32)
     ptr = lambda a: a.ctypes.data_as(C.c_void_p)        # noqa: E731

@@ -1,8 +1,8 @@
 """render() and captureScreenshot() with BLOOM on the GPU against the per-texel interval of
-tests/gamma_model.py: every value of the frame and every byte of the capture must lie within the fp32
+display_model.display (tests/gamma_model.py): every value of the frame and every byte of the capture must lie within the fp32
 arithmetic of the display shader with a powf inside POWF_ULP of float64 pow.  The interval of a frame is
-built from the GPU's own bloom FBO and sunrays texture, after checking them against the oracle's bit for
-bit (NaN in the same places).
+built from the model's bloom FBO and sunrays texture (the oracle's blits), after checking the GPU's against
+them bit for bit (NaN in the same places).
 
 Inputs are those of test_gamma_model_cpu.py (goldens, seeded, zero and dim dye, dithering of other
 shapes, of a wide range and overflowing, non-finite dye) plus one frame at the reference's sizes; the
@@ -11,17 +11,15 @@ device powf itself closes the file."""
 import numpy as np
 import pytest
 
-import capture_model as CM
-import display_keywords_model as M
+import display_harness as DH
+import display_model as M
 import gamma_model as G
 from conftest import golden
-from test_gamma_model_cpu import (ALL3, BACK_RGB, BACKGROUNDS, BLOOM_SETS, CASES, DIM_CFG, FXCFG, golden_dither,
-                                  nonfinite_dye, seeded_dye)
+from display_harness import BACK_RGB, BACKGROUNDS, MODES, golden_dither, make, nonfinite_dye, seeded_dye, set_keywords
+from test_gamma_model_cpu import ALL3, BLOOM_SETS, CASES, DIM_CFG, FXCFG
 
 pytestmark = pytest.mark.gpu
 F32 = np.float32
-BACK = {"r": 10, "g": 20, "b": 30}
-MODES = {"back": (False, False), "checker": (True, False), "bare": (True, True)}     # (TRANSPARENT, target)
 NO_BLOOM_SETS = [0, M.SHADING, M.SUNRAYS, M.SHADING | M.SUNRAYS]
 HALF = 0x10
 
@@ -32,47 +30,15 @@ def pkg():
     return p
 
 
-def make(pkg, Wd, Hd, canvas_w, canvas_h, flags=0, **cfg):
-    s = pkg.FluidSimulation({"SIM_RESOLUTION": 16, "DYE_RESOLUTION": min(Wd, Hd)}, canvas_width=canvas_w,
-                            canvas_height=canvas_h, flags=flags, sizes=(16, 16, Wd, Hd))
-    s.config.update(BACK_COLOR=BACK, **cfg)
-    return s
-
-
-def set_keywords(s, kw):
-    s.config.update(SHADING=bool(kw & M.SHADING), BLOOM=bool(kw & M.BLOOM), SUNRAYS=bool(kw & M.SUNRAYS))
-
-
-def draw_and_check(pkg, oracle, c, sets=BLOOM_SETS, modes=MODES):
-    """Each keyword set with BLOOM x background: the chains equal the oracle's, the frame lies within the
-    interval built from the GPU's chains."""
-    dye, w, h, dither = c["dye"], c["w"], c["h"], c["dither"]
-    s = make(pkg, dye.shape[1], dye.shape[0], w, h, **c["cfg"])
-    s.writeField("dye", dye)
-    s.dithering = dither
-    with np.errstate(invalid="ignore", over="ignore"):
-        ref = oracle.render_postfx(dye, w, h, dither, cfg=c["cfg"])
-    for kw in sets:
-        set_keywords(s, kw)
-        colour = None
-        for bg in modes:
-            transparent, target = MODES[bg]
-            s.config["TRANSPARENT"] = transparent
-            got = s.render(w, h, target=target)
-            assert G.same_bits(s.last_bloom, ref["bloom"]), (kw, bg)
-            if kw & M.SUNRAYS:
-                assert G.same_bits(s.last_sunrays, ref["sunrays"]), (kw, bg)
-            if colour is None:
-                colour = G.gamma_interval(dye, w, h, kw, s.last_bloom, s.last_sunrays, dither)
-            lo, hi = G.blend_interval(*colour, BACK_RGB, BACKGROUNDS[bg], w / h)
-            n, bad = G.check_display(got, lo, hi)
-            assert n == 0, (kw, bg, f"{n} values outside", bad)
-    s.close()
+def draw_and_check(pkg, c, sets=BLOOM_SETS):
+    """Each keyword set with BLOOM x background: the chains equal the model's (the oracle's blits), the frame lies
+    within the interval of display_model."""
+    DH.draw_all(pkg, "fp32", c["dye"], c["w"], c["h"], c["dither"], cfg=c["cfg"], sets=sets)
 
 
 @pytest.mark.parametrize("name", list(CASES))
 def test_frames_within_interval(pkg, oracle, name):
-    draw_and_check(pkg, oracle, CASES[name])
+    draw_and_check(pkg, CASES[name])
 
 
 def test_reference_size_frame_within_interval(pkg, oracle):
@@ -80,7 +46,7 @@ def test_reference_size_frame_within_interval(pkg, oracle):
     keywords."""
     c = dict(dye=seeded_dye(1024, 1024, 1920), w=1920, h=1080, dither=golden_dither(),
              cfg=dict(BLOOM_RESOLUTION=256, SUNRAYS_RESOLUTION=196))
-    draw_and_check(pkg, oracle, c, sets=[ALL3])
+    draw_and_check(pkg, c, sets=[ALL3])
 
 
 def capture_inputs():
@@ -117,12 +83,7 @@ def test_captures_within_interval(pkg, name):
             set_keywords(s, kw)
             got = s.captureScreenshot()
             assert got.shape == (h, w, 4)
-            if kw & M.BLOOM:
-                lo, hi = G.capture_interval(dye, w, h, cw, ch, dither, kw, transparent, BACK_RGB, cfg=cfg)
-                assert G.bytes_outside(got, lo, hi) == 0, (name, kw)
-            else:
-                want = CM.capture(dye, w, h, cw, ch, dither, kw, transparent, BACK_RGB, cfg=cfg)["rgba8"]
-                assert np.array_equal(got, want), (name, kw)
+            DH.check_capture(got, DH.model_capture("fp32", dye, w, h, cw, ch, kw, dither, cfg, transparent), kw, (name, kw))
     s.close()
 
 
@@ -140,8 +101,7 @@ def test_nonfinite_frames_without_bloom(pkg, oracle):
             for bg, (transparent, target) in MODES.items():
                 s.config["TRANSPARENT"] = transparent
                 got = s.render(w, h, target=target)
-                ref = M.render_keywords(dye, w, h, None, cfg=c["cfg"], back_rgb=BACK_RGB, background=BACKGROUNDS[bg],
-                                        keywords=kw)
+                ref = DH.model_frame("fp32", dye, w, h, kw, None, c["cfg"], BACKGROUNDS[bg])
                 assert np.isnan(ref["target"]).any()
                 assert G.same_bits(got, ref["target"]), (kw, bg)
                 if kw & M.SUNRAYS:
@@ -168,7 +128,7 @@ def test_nonfinite_half_storage(pkg, oracle):
                 assert G.same_bits(s.render(w, h, target=target), ref), (kw, bg)
             for transparent in (False, True):
                 s.config["TRANSPARENT"] = transparent
-                want = CM.capture(dye16, 64, 64, w, h, None, kw, transparent, BACK_RGB)["rgba8"]
+                want = DH.model_capture("half", dye16, 64, 64, w, h, kw, None, None, transparent)["rgba8"]
                 assert np.array_equal(s.captureScreenshot(), want), (kw, transparent)
     s.close()
 
@@ -188,7 +148,7 @@ def test_direct_powf_readout(pkg, capsys):
     e = rng.uniform(-14, 120, (H, W))
     d = ((np.exp2(e) * 255 + 1) / 2).astype(F32)
     dither = np.repeat(d[..., None], 3, axis=-1)
-    s = make(pkg, 64, 64, W, H, TRANSPARENT=True)
+    s = make(pkg, 64, 64, W, H, TRANSPARENT=True, BLOOM_RESOLUTION=256, SUNRAYS_RESOLUTION=196)
     s.writeField("dye", np.zeros((64, 64, 4), F32))
     s.dithering = dither
     set_keywords(s, M.BLOOM)

@@ -1,6 +1,6 @@
 """FLUID_FLAG_HALF_POSTFX on the GPU: fp16 bloom FBO, pyramid, sunrays and sunraysTemp, on an fp32 handle
 and on a half-storage handle (FLUID_FLAG_HALF_STORAGE | FLUID_FLAG_HALF_POSTFX: the reference's desktop
-frame), against half_postfx_model.render_postfx(half_targets=True) and the executed half-float
+frame), against display_model with half_targets and the executed half-float
 shaders; overflow and non-finite dye; captures; launches and target reuse; the slab refusal."""
 import ctypes as C
 
@@ -8,18 +8,17 @@ import numpy as np
 import pytest
 
 import capture_model as CM
-import display_keywords_model as M
+import display_model as M
 import gamma_model as G
-import half_postfx_model as HP
 from conftest import golden, max_rel
-from test_gamma_model_cpu import ALL3, BACK_RGB, BACKGROUNDS, golden_dither, nonfinite_dye, seeded_dye
+from display_harness import (FXCFG, check_capture, check_frame, draw_all, flags_of, golden_dither, make, model_capture,
+                             model_frame, nonfinite_dye, seeded_dye, set_keywords, stored)
+from oracle import oracle as O
 from test_half_postfx_cpu import CAPTURE_SETS, FRAME_TOL, POW2, RAGGED, RAGGED_CHAIN_TEXELS, cfg_of, fp16_ulps
 
 pytestmark = pytest.mark.gpu
 F32 = np.float32
-BACK = {"r": 10, "g": 20, "b": 30}
-FXCFG = dict(BLOOM_RESOLUTION=64, SUNRAYS_RESOLUTION=48)
-MODES = {"back": (False, False), "checker": (True, False), "bare": (True, True)}     # (TRANSPARENT, target)
+ALL3 = M.ALL3
 HANDLES = ["fp32", "half"]
 
 
@@ -29,67 +28,16 @@ def pkg():
     return p
 
 
-def flags_of(pkg, handle):
-    return pkg.FLAG_HALF_POSTFX | (pkg.FLAG_HALF_STORAGE if handle == "half" else 0)
-
-
-def make(pkg, Wd, Hd, w, h, handle, **cfg):
-    s = pkg.FluidSimulation({"SIM_RESOLUTION": 16, "DYE_RESOLUTION": min(Wd, Hd)}, canvas_width=w, canvas_height=h,
-                            flags=flags_of(pkg, handle), sizes=(16, 16, Wd, Hd))
-    s.config.update(BACK_COLOR=BACK, **FXCFG)
-    s.config.update(cfg)
-    return s
-
-
-def set_keywords(s, kw):
-    s.config.update(SHADING=bool(kw & M.SHADING), BLOOM=bool(kw & M.BLOOM), SUNRAYS=bool(kw & M.SUNRAYS))
-
-
-def stored_dye(oracle, handle, dye):
-    """What the handle holds after writeField: fp16-rounded on a half-storage handle."""
-    return oracle.round_half(dye) if handle == "half" else np.ascontiguousarray(dye, F32)
-
-
-def check_frame(s, got, dye, w, h, kw, dither, cfg, bg, half_mask):
-    """Chains bit for bit vs the half_targets model (NaN in the same places); the frame bit for bit without
-    BLOOM, inside gamma_model's interval built from the GPU's own chains with it."""
-    ref = HP.render_keywords(dye, w, h, dither, cfg=cfg, back_rgb=BACK_RGB, background=BACKGROUNDS[bg], keywords=kw,
-                            half_targets=True, half_mask=half_mask)
-    if kw & M.BLOOM:
-        assert G.same_bits(s.last_bloom, ref["bloom"]), (kw, bg)
-        lo, hi = G.display_interval(dye, w, h, kw, s.last_bloom, s.last_sunrays, dither, BACK_RGB, BACKGROUNDS[bg], w / h)
-        n, bad = G.check_display(got, lo, hi)
-        assert n == 0, (kw, bg, n, bad)
-    else:
-        assert s.last_bloom is None
-        assert G.same_bits(got, ref["target"]), (kw, bg)
-    if kw & M.SUNRAYS:
-        assert G.same_bits(s.last_sunrays, ref["sunrays"]), (kw, bg)
-    return ref
-
-
-def draw_all(pkg, oracle, handle, dye_in, w, h, dither, cfg=FXCFG, sets=range(8), modes=MODES):
-    Wd, Hd = dye_in.shape[1], dye_in.shape[0]
-    s = make(pkg, Wd, Hd, w, h, handle, **cfg)
-    s.writeField("dye", dye_in)
-    s.dithering = dither
-    dye = stored_dye(oracle, handle, dye_in)
-    with np.errstate(invalid="ignore", over="ignore"):
-        for kw in sets:
-            set_keywords(s, kw)
-            for bg in modes:
-                s.config["TRANSPARENT"] = MODES[bg][0]
-                got = s.render(w, h, target=MODES[bg][1])
-                check_frame(s, got, dye, w, h, kw, dither, cfg, bg, half_mask=handle == "half")
-                assert G.same_bits(s.readField("dye"), dye), (kw, bg)
-    s.close()
+def kind(handle):
+    """The display_harness kind of a handle with FLUID_FLAG_HALF_POSTFX."""
+    return handle + "_half_postfx"
 
 
 @pytest.mark.parametrize("handle", HANDLES)
 @pytest.mark.parametrize("Wd,Hd,w,h", [(64, 64, 128, 128), (48, 32, 50, 75)])
 def test_every_keyword_set_and_background(pkg, oracle, handle, Wd, Hd, w, h):
     """All eight sets x the three backgrounds; dye.read is unchanged afterwards."""
-    draw_all(pkg, oracle, handle, seeded_dye(Wd, Hd, Wd + w), w, h, golden_dither())
+    draw_all(pkg, kind(handle), seeded_dye(Wd, Hd, Wd + w), w, h, golden_dither())
 
 
 @pytest.mark.parametrize("name", [POW2, RAGGED])
@@ -98,7 +46,7 @@ def test_vs_executed_half_float_shaders(pkg, name):
     within the measured ragged bound (test_half_postfx_cpu.py) on the other; frames within FRAME_TOL."""
     g = golden(name)
     Wd, Hd, w, h = (int(g[k]) for k in ("Wd", "Hd", "w", "h"))
-    s = make(pkg, Wd, Hd, w, h, "half", **cfg_of(g))
+    s = make(pkg, Wd, Hd, w, h, flags_of(pkg, "half_half_postfx"), **cfg_of(g))
     s.writeField("dye", g["in_dye"])
     s.dithering = g["dither"].astype(F32)
     for tag in (str(t) for t in g["sets"]):
@@ -121,47 +69,43 @@ def test_bloom_overflow_goes_to_inf_where_the_model_does(pkg, oracle):
     dye = seeded_dye(64, 64, 77)
     dye[20:24, 30:34, 0] = 2.0e5
     dye[40, 10, 1] = 1.0e6
-    ref = HP.render_postfx(dye, 128, 128, golden_dither(), cfg=FXCFG, half_targets=True)
+    ref = M.chains(dye, 128, 128, M.BLOOM, FXCFG, half_targets=True)
     assert np.isinf(ref["bloom"]).any() and not np.isinf(dye).any()
-    draw_all(pkg, oracle, "fp32", dye, 128, 128, golden_dither(), sets=[M.BLOOM, ALL3], modes=["back", "bare"])
+    draw_all(pkg, "fp32_half_postfx", dye, 128, 128, golden_dither(), sets=[M.BLOOM, ALL3], modes=["back", "bare"])
 
 
 @pytest.mark.parametrize("handle", HANDLES)
 def test_nonfinite_dye_every_set(pkg, oracle, handle):
     """The non-finite dye of test_gamma_model_cpu.py through all eight sets and backgrounds: bit for bit
     without BLOOM (NaN in the same places), inside the interval with it."""
-    draw_all(pkg, oracle, handle, nonfinite_dye(64, 64, 8), 128, 128, golden_dither())
+    draw_all(pkg, kind(handle), nonfinite_dye(64, 64, 8), 128, 128, golden_dither())
 
 
 @pytest.mark.parametrize("bg", ["back", "transparent"])
 def test_half_storage_captures(pkg, oracle, bg):
     """The executed-shader capture fixture on a half-storage handle with the flag, all eight sets: with BLOOM
-    every byte within [B(lo), B(hi)] of the half_targets interval, without it half_postfx_model.capture's (= the
+    every byte within [B(lo), B(hi)] of the half_targets interval, without it the model's (= the
     executed) bytes exactly; every byte within the byte rule at FRAME_TOL of the model; and each capture equals the quantised
     render(target=True) frame of a canvas-sized copy where canvas = target."""
     g = golden(f"capture_half_64_canvas_128_{bg}")
     dye, w, h, cw, ch = g["in_dye"], int(g["w"]), int(g["h"]), int(g["canvas_w"]), int(g["canvas_h"])
     cfg, dither, transparent = cfg_of(g), g["dither"].astype(F32), bool(g["transparent"])
-    s = make(pkg, dye.shape[1], dye.shape[0], cw, ch, "half", CAPTURE_RESOLUTION=int(g["capture_res"]),
-             TRANSPARENT=transparent, **cfg)
+    s = make(pkg, dye.shape[1], dye.shape[0], cw, ch, flags_of(pkg, "half_half_postfx"),
+             CAPTURE_RESOLUTION=int(g["capture_res"]), TRANSPARENT=transparent, **cfg)
     s.writeField("dye", dye)
     s.dithering = dither
     for kw, tag in enumerate(CAPTURE_SETS):
         set_keywords(s, kw)
         got = s.captureScreenshot()
-        model = HP.capture(dye, w, h, cw, ch, dither, kw, transparent, BACK_RGB, cfg=cfg, half_targets=True, half_mask=True)
-        if kw & M.BLOOM:
-            lo, hi = HP.capture_interval(dye, w, h, cw, ch, dither, kw, transparent, BACK_RGB, cfg=cfg, half_targets=True,
-                                        half_mask=True)
-            assert G.bytes_outside(got, lo, hi) == 0, tag
-        else:
-            assert np.array_equal(got, model["rgba8"]), tag
+        model = model_capture("half_half_postfx", dye, w, h, cw, ch, kw, dither, cfg, transparent)
+        check_capture(got, model, kw, tag)
         assert CM.bytes_outside(got, model["pre"], FRAME_TOL) == 0, tag
         if not kw & M.BLOOM:                          # the model's bytes are the executed ones (CPU test)
             assert np.array_equal(got, g[f"{tag}_rgba8"]), tag
     s.close()
     # canvas = target: capture == flip(B(render frame))
-    s = make(pkg, 64, 64, 64, 64, "half", CAPTURE_RESOLUTION=64, BLOOM_RESOLUTION=32, SUNRAYS_RESOLUTION=24)
+    s = make(pkg, 64, 64, 64, 64, flags_of(pkg, "half_half_postfx"), CAPTURE_RESOLUTION=64, BLOOM_RESOLUTION=32,
+             SUNRAYS_RESOLUTION=24)
     s.config["BACK_COLOR"] = {"r": 0, "g": 0, "b": 0}
     s.writeField("dye", dye)
     s.dithering = dither
@@ -178,7 +122,7 @@ def test_half_storage_captures(pkg, oracle, bg):
 def test_launches(pkg, handle, iterations, levels):
     """Steady state: 1 display, + 4 with SUNRAYS, + 2L + 1 with BLOOM and L >= 2, and on a half-storage handle
     the one dye widen of the display source; a capture launches what render() does."""
-    s = make(pkg, 64, 64, 128, 128, handle, CAPTURE_RESOLUTION=64, BLOOM_ITERATIONS=iterations)
+    s = make(pkg, 64, 64, 128, 128, flags_of(pkg, kind(handle)), CAPTURE_RESOLUTION=64, BLOOM_ITERATIONS=iterations)
     s.writeField("dye", seeded_dye(64, 64, 5))
     s.dithering = golden_dither()
     for kw in range(8):
@@ -198,10 +142,10 @@ def test_targets_reused_and_remade_on_resize(pkg, oracle, handle):
     """w1 x h1, then w2 x h2 with another BLOOM_RESOLUTION and BLOOM_ITERATIONS, then w1 x h1 again, then a
     pyramid too short to run (the fp16 bloom FBO reads as freshly cleared: (0, 0, 0, 1))."""
     dye_in = seeded_dye(64, 48, 9)
-    s = make(pkg, 64, 48, 128, 96, handle)
+    s = make(pkg, 64, 48, 128, 96, flags_of(pkg, kind(handle)))
     s.writeField("dye", dye_in)
     s.dithering = golden_dither()
-    dye = stored_dye(oracle, handle, dye_in)
+    dye = stored(kind(handle), dye_in)
     set_keywords(s, ALL3)
     frames = [(128, 96, dict(BLOOM_RESOLUTION=64, BLOOM_ITERATIONS=8, SUNRAYS_RESOLUTION=48)),
               (90, 160, dict(BLOOM_RESOLUTION=40, BLOOM_ITERATIONS=3, SUNRAYS_RESOLUTION=30)),
@@ -211,7 +155,8 @@ def test_targets_reused_and_remade_on_resize(pkg, oracle, handle):
         s.config.update(fx)
         s.canvas = {"width": w, "height": h}
         got = s.render(w, h)
-        check_frame(s, got, dye, w, h, ALL3, golden_dither(), dict(FXCFG, **fx), "back", half_mask=handle == "half")
+        check_frame(s, got, model_frame(kind(handle), dye, w, h, ALL3, golden_dither(), dict(FXCFG, **fx), O.BG_COLOR),
+                    ALL3, (handle, w, h))
     assert np.all(s.last_bloom == np.array([0, 0, 0, 1], F32))
     s.close()
 
@@ -219,7 +164,7 @@ def test_targets_reused_and_remade_on_resize(pkg, oracle, handle):
 def test_reference_size_frame_within_interval(pkg, oracle):
     """The reference's desktop frame: 1024^2 fp16 dye drawn to 1920 x 1080 with BLOOM_RESOLUTION 256 and
     SUNRAYS_RESOLUTION 196, all three keywords."""
-    draw_all(pkg, oracle, "half", seeded_dye(1024, 1024, 1920), 1920, 1080, golden_dither(),
+    draw_all(pkg, "half_half_postfx", seeded_dye(1024, 1024, 1920), 1920, 1080, golden_dither(),
              cfg=dict(BLOOM_RESOLUTION=256, SUNRAYS_RESOLUTION=196), sets=[ALL3], modes=["back"])
 
 

@@ -1,5 +1,5 @@
 """FLUID_FLAG_NEAREST_FILTERING on the GPU: display, post-FX chains, captures and resize through NEAREST
-samplers, against nearest_model.py with the library's vUv (bit for bit; BLOOM frames inside gamma_model's
+samplers, against display_model.py's NEAREST sampler with the library's vUv (bit for bit; BLOOM frames inside gamma_model's
 powf interval after the bloom FBO and sunrays texture matched bit for bit) and against the executed
 NEAREST shaders; non-finite dye; a simulation that does not change by one bit or one launch; refusals.
 No comparison uses a value tolerance for a NEAREST fetch."""
@@ -8,19 +8,16 @@ import ctypes as C
 import numpy as np
 import pytest
 
-import display_keywords_model as M
+import display_model as M
 import gamma_model as G
-import nearest_model as N
 from conftest import golden
-from test_gamma_model_cpu import BACK_RGB, BACKGROUNDS, golden_dither, nonfinite_dye, seeded_dye
+from display_harness import (BACK_RGB, BACKGROUNDS, MODES, allowed, check_capture, draw_all, flags_of, golden_dither,
+                             make, model_capture, nonfinite_dye, seeded_dye, set_keywords)
 
 pytestmark = pytest.mark.gpu
 F32 = np.float32
-BACK = {"r": 10, "g": 20, "b": 30}
-FXCFG = dict(BLOOM_RESOLUTION=64, SUNRAYS_RESOLUTION=48)
-MODES = {"back": (False, False), "checker": (True, False), "bare": (True, True)}     # (TRANSPARENT, target)
 HANDLES = ["fp32", "fp32_half_postfx", "half", "half_half_postfx"]
-ALL3 = M.SHADING | M.BLOOM | M.SUNRAYS
+ALL3 = M.ALL3
 
 
 @pytest.fixture(scope="module")
@@ -29,76 +26,21 @@ def pkg():
     return p
 
 
-def flags_of(pkg, handle):
-    return (pkg.FLAG_NEAREST_FILTERING | (pkg.FLAG_HALF_STORAGE if handle.startswith("half") else 0)
-            | (pkg.FLAG_HALF_POSTFX if handle.endswith("half_postfx") else 0))
-
-
-def allowed(handle, kw):
-    """Half storage without HALF_POSTFX draws only the sets without BLOOM and SUNRAYS."""
-    return handle != "half" or not kw & (M.BLOOM | M.SUNRAYS)
-
-
-def make(pkg, Wd, Hd, w, h, flags, **cfg):
-    s = pkg.FluidSimulation({"SIM_RESOLUTION": 16, "DYE_RESOLUTION": min(Wd, Hd)}, canvas_width=w, canvas_height=h,
-                            flags=flags, sizes=(16, 16, Wd, Hd))
-    s.config.update(BACK_COLOR=BACK, **FXCFG)
-    s.config.update(cfg)
-    return s
-
-
-def set_keywords(s, kw):
-    s.config.update(SHADING=bool(kw & M.SHADING), BLOOM=bool(kw & M.BLOOM), SUNRAYS=bool(kw & M.SUNRAYS))
-
-
-def stored(oracle, half, a):
-    return oracle.round_half(a) if half else np.ascontiguousarray(a, F32)
-
-
-def check_frame(s, got, dye, w, h, kw, dither, cfg, bg, handle):
-    half_t, half_m = handle.endswith("half_postfx"), handle.startswith("half")
-    r = N.chains(dye, w, h, kw, cfg, half_targets=half_t, half_mask=half_m)
-    if kw & M.BLOOM:
-        assert G.same_bits(s.last_bloom, r["bloom"]), (kw, bg, handle)
-    else:
-        assert s.last_bloom is None
-    if kw & M.SUNRAYS:
-        assert G.same_bits(s.last_sunrays, r["sunrays"]), (kw, bg, handle)
-    d = N.display(dye, w, h, kw, r["bloom"], r["sunrays"], dither, BACK_RGB, BACKGROUNDS[bg], w / h)
-    if kw & M.BLOOM:
-        n, bad = G.check_display(got, d["lo"], d["hi"])
-        assert n == 0, (kw, bg, handle, n, bad)
-    else:
-        assert G.same_bits(got, d["target"]), (kw, bg, handle)
-
-
-def draw_all(pkg, oracle, handle, dye_in, w, h, dither, cfg=FXCFG, sets=range(8), modes=MODES):
-    Wd, Hd = dye_in.shape[1], dye_in.shape[0]
-    s = make(pkg, Wd, Hd, w, h, flags_of(pkg, handle), **cfg)
-    s.writeField("dye", dye_in)
-    s.dithering = dither
-    dye = stored(oracle, handle.startswith("half"), dye_in)
-    with np.errstate(invalid="ignore", over="ignore"):
-        for kw in (k for k in sets if allowed(handle, k)):
-            set_keywords(s, kw)
-            for bg in modes:
-                s.config["TRANSPARENT"] = MODES[bg][0]
-                got = s.render(w, h, target=MODES[bg][1])
-                check_frame(s, got, dye, w, h, kw, dither, dict(FXCFG, **cfg), bg, handle)
-                assert G.same_bits(s.readField("dye"), dye), (kw, bg)
-    s.close()
+def kind(handle):
+    """The display_harness kind of a handle with FLUID_FLAG_NEAREST_FILTERING."""
+    return "nearest_" + handle
 
 
 @pytest.mark.parametrize("handle", HANDLES)
 @pytest.mark.parametrize("Wd,Hd,w,h", [(64, 64, 128, 128), (48, 32, 50, 75)])
 def test_every_keyword_set_and_background(pkg, oracle, handle, Wd, Hd, w, h):
-    draw_all(pkg, oracle, handle, seeded_dye(Wd, Hd, Wd + w), w, h, golden_dither())
+    draw_all(pkg, kind(handle), seeded_dye(Wd, Hd, Wd + w), w, h, golden_dither())
 
 
 @pytest.mark.parametrize("handle", HANDLES)
 def test_minification(pkg, oracle, handle):
     """A 1024^2 dye drawn on a 300 x 200 canvas."""
-    draw_all(pkg, oracle, handle, seeded_dye(1024, 1024, 300), 300, 200, golden_dither(), modes=["back", "bare"])
+    draw_all(pkg, kind(handle), seeded_dye(1024, 1024, 300), 300, 200, golden_dither(), modes=["back", "bare"])
 
 
 @pytest.mark.parametrize("handle", ["fp32", "half_half_postfx"])
@@ -108,7 +50,7 @@ def test_the_profiles_own_frame(pkg, oracle, handle):
     OES_texture_float_linear."""
     import webgl_fluid_simulation_b200 as p
     assert (p.getResolution(512, 1920, 1080)["width"], p.getResolution(512, 1920, 1080)["height"]) == (910, 512)
-    draw_all(pkg, oracle, handle, seeded_dye(910, 512, 1080), 1920, 1080, golden_dither(),
+    draw_all(pkg, kind(handle), seeded_dye(910, 512, 1080), 1920, 1080, golden_dither(),
              cfg=dict(BLOOM_RESOLUTION=256, SUNRAYS_RESOLUTION=196), sets=[ALL3], modes=["back"])
 
 
@@ -116,7 +58,7 @@ def test_the_profiles_own_frame(pkg, oracle, handle):
 def test_nonfinite_dye_every_set(pkg, oracle, handle):
     """+-inf and NaN in dye: bit for bit without BLOOM (NaN in the model's texels only: NEAREST reads one
     texel, so a NaN does not reach its neighbours), inside the interval with it."""
-    draw_all(pkg, oracle, handle, nonfinite_dye(64, 64, 8), 128, 128, golden_dither())
+    draw_all(pkg, kind(handle), nonfinite_dye(64, 64, 8), 128, 128, golden_dither())
 
 
 def test_nan_stays_in_its_own_texels(pkg):
@@ -144,7 +86,7 @@ def test_vs_executed_nearest_shaders(pkg, name):
     s.dithering = dither
     keys = {"target": "back", "checker": "checker", "bare": "bare"}
     for tag in (str(t) for t in g["sets"]):
-        kw = N.SETS[tag]
+        kw = M.SETS[tag]
         set_keywords(s, kw)
         for key, bg in keys.items():
             if f"{tag}_{key}" not in g:
@@ -155,8 +97,8 @@ def test_vs_executed_nearest_shaders(pkg, name):
                 if tex is not None:
                     assert G.same_bits(tex, g[k]), (tag, k)
             if kw & M.BLOOM:
-                d = N.display(g["in_dye"], w, h, kw, g["bloom"], g["sunrays"] if kw & M.SUNRAYS else None, dither,
-                              BACK_RGB, BACKGROUNDS[bg], w / h)
+                d = M.display(g["in_dye"], w, h, kw, g["bloom"], g["sunrays"] if kw & M.SUNRAYS else None, dither,
+                              BACK_RGB, BACKGROUNDS[bg], w / h, nearest=True)
                 n, bad = G.check_display(got, d["lo"], d["hi"])
                 assert n == 0 and G.check_display(g[f"{tag}_{key}"], d["lo"], d["hi"])[0] == 0, (tag, key, bad)
             else:
@@ -173,24 +115,20 @@ def test_captures(pkg, handle, bg):
     dye_in, w, h, cw, ch = g["in_dye"], int(g["w"]), int(g["h"]), int(g["canvas_w"]), int(g["canvas_h"])
     cfg = dict(BLOOM_RESOLUTION=int(g["bloom_res"]), SUNRAYS_RESOLUTION=int(g["sun_res"]))
     dither, transparent = g["dither"].astype(F32), bool(g["transparent"])
-    s = make(pkg, 64, 64, cw, ch, flags_of(pkg, handle), CAPTURE_RESOLUTION=int(g["capture_res"]), TRANSPARENT=transparent, **cfg)
+    s = make(pkg, 64, 64, cw, ch, flags_of(pkg, kind(handle)), CAPTURE_RESOLUTION=int(g["capture_res"]),
+             TRANSPARENT=transparent, **cfg)
     s.writeField("dye", dye_in)
     s.dithering = dither
     dye = s.readField("dye")                           # fp16-rounded on a half-storage handle
     for tag in (str(t) for t in g["sets"]):
-        kw = N.SETS[tag]
-        if not allowed(handle, kw):
+        kw = M.SETS[tag]
+        if not allowed(kind(handle), kw):
             continue
         set_keywords(s, kw)
         got = s.captureScreenshot()
-        r = N.capture(dye, w, h, cw, ch, dither, kw, transparent, BACK_RGB, cfg=cfg,
-                      half_targets=handle.endswith("half_postfx"), half_mask=handle.startswith("half"))
-        if "rgba8" in r:
-            assert np.array_equal(got, r["rgba8"]), (tag, handle)
-            if handle == "fp32":
-                assert np.array_equal(got, g[f"{tag}_rgba8"]), tag
-        else:
-            assert G.bytes_outside(got, r["lo"], r["hi"]) == 0, (tag, handle)
+        check_capture(got, model_capture(kind(handle), dye, w, h, cw, ch, kw, dither, cfg, transparent), kw, (tag, handle))
+        if handle == "fp32" and not kw & M.BLOOM:
+            assert np.array_equal(got, g[f"{tag}_rgba8"]), tag
     s.close()
 
 
@@ -213,7 +151,7 @@ def test_resize_copies_through_nearest(pkg, oracle, half):
             if old.shape[:2] == (H, W):
                 assert G.same_bits(new, old), sizes
             else:
-                assert G.same_bits(new, N.resize(old, W, H, half=half)), sizes
+                assert G.same_bits(new, M.resize(old, W, H, half=half)), sizes
     s.close()
 
 
@@ -248,9 +186,9 @@ def test_simulation_is_unchanged(pkg):
 
 @pytest.mark.parametrize("handle", ["fp32", "half_half_postfx"])
 def test_frame_launches_equal_the_linear_frame(pkg, handle):
-    linear_flags = flags_of(pkg, handle) & ~pkg.FLAG_NEAREST_FILTERING
+    linear_flags = flags_of(pkg, handle)
     counts = []
-    for flags in (flags_of(pkg, handle), linear_flags):
+    for flags in (flags_of(pkg, kind(handle)), linear_flags):
         s = make(pkg, 64, 64, 128, 128, flags, CAPTURE_RESOLUTION=64)
         s.writeField("dye", seeded_dye(64, 64, 5))
         s.dithering = golden_dither()

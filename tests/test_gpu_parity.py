@@ -3,6 +3,7 @@ vectors.  Bitwise for every pass whose arithmetic is IEEE-exact (all but splat's
 import numpy as np
 import pytest
 
+import display_model as DM
 import gamma_model as G
 import splat_model as M
 from conftest import bits_equal, golden, max_rel
@@ -578,7 +579,7 @@ def test_render_display_bitwise_vs_oracle(pkg, oracle, Wd, Hd, w, h):
 @pytest.mark.parametrize("name", ["postfx_64_to_128", "postfx_48x32_to_50x75"])
 def test_render_postfx_vs_oracle_and_executed_shaders(pkg, oracle, name):
     """render() with SHADING + BLOOM + SUNRAYS: bloom FBO and sunrays texture bit-identical to the
-    oracle, every value of the final frame within the per-texel powf interval of gamma_model.py, and
+    oracle, every value of the final frame within the per-texel powf interval of display_model.py, and
     within the golden's tolerance of the executed reference shaders."""
     g = golden(name)
     Wd, Hd, w, h = (int(g[k]) for k in ("Wd", "Hd", "w", "h"))
@@ -592,9 +593,9 @@ def test_render_postfx_vs_oracle_and_executed_shaders(pkg, oracle, name):
     ref = oracle.render_postfx(g["in_dye"], w, h, dither, cfg=fxcfg, back_rgb=(10 / 255, 20 / 255, 30 / 255))
     assert bits_equal(s.last_bloom, ref["bloom"])
     assert bits_equal(s.last_sunrays, ref["sunrays"])
-    lo, hi = G.display_interval(g["in_dye"], w, h, G.M.SHADING | G.M.BLOOM | G.M.SUNRAYS, s.last_bloom, s.last_sunrays,
-                                dither, (10 / 255, 20 / 255, 30 / 255), oracle.BG_COLOR, w / h)
-    n, bad = G.check_display(got, lo, hi)                     # powf: per texel, within POWF_ULP of pow
+    d = DM.display(g["in_dye"], w, h, DM.ALL3, s.last_bloom, s.last_sunrays, dither, (10 / 255, 20 / 255, 30 / 255),
+                   oracle.BG_COLOR, w / h)
+    n, bad = G.check_display(got, d["lo"], d["hi"])           # powf: per texel, within POWF_ULP of pow
     assert n == 0, (n, bad)
     assert max_rel(got, g["target"]) < 3e-4
     assert bits_equal(s.readField("dye"), g["in_dye"])        # the mask scribbles on dye.write only (S:1300)

@@ -2,26 +2,23 @@
 parameter set of test_postfx_params_cpu.py on every handle kind that draws post-FX (fp32, fp32 + HALF_POSTFX,
 HALF_STORAGE | HALF_POSTFX, NEAREST_FILTERING, NEAREST_FILTERING | HALF_STORAGE | HALF_POSTFX) with BLOOM,
 SUNRAYS, BLOOM + SUNRAYS and SHADING + BLOOM + SUNRAYS: the bloom FBO and sunrays texture bit for bit against
-the matching model, the frame inside gamma_model's interval (bit for bit without BLOOM), captures and canvases
+the matching model (display_model), the frame inside its powf interval (bit for bit without BLOOM), captures and canvases
 against their models; sliders changed between frames on one handle; the executed reference shaders."""
 import numpy as np
 import pytest
 
 import canvas_model as CV
-import display_keywords_model as M
+import display_model as M
 import gamma_model as G
-import half_postfx_model as HP
-import nearest_model as N
-import test_gpu_half_postfx as HPG
-import test_gpu_nearest_filtering as NF
 from conftest import golden, max_rel
-from test_gamma_model_cpu import BACK_RGB, golden_dither
+from display_harness import (BACK_RGB, check_capture, check_frame, flags_of, golden_dither, make, model_capture,
+                             model_frame, set_keywords, stored)
 from test_postfx_params_cpu import DEFAULTS, FIXTURES, GEOMETRIES, KEYS, SETS, cfg_of, fixture_cfg, params_dye
 
 pytestmark = pytest.mark.gpu
 F32 = np.float32
 HANDLES = ["fp32", "fp32_half_postfx", "half_half_postfx", "nearest_fp32", "nearest_half_half_postfx"]
-KEYWORD_SETS = [M.BLOOM, M.SUNRAYS, M.BLOOM | M.SUNRAYS, M.SHADING | M.BLOOM | M.SUNRAYS]
+KEYWORD_SETS = [M.BLOOM, M.SUNRAYS, M.BLOOM | M.SUNRAYS, M.ALL3]
 
 
 @pytest.fixture(scope="module")
@@ -37,67 +34,14 @@ def torch():
     return t
 
 
-def flags_of(pkg, handle):
-    if handle.startswith("nearest_"):
-        return NF.flags_of(pkg, handle[len("nearest_"):])
-    return 0 if handle == "fp32" else HPG.flags_of(pkg, handle.split("_")[0])
-
-
-def storage(handle):
-    """(half_targets, half_mask) of the handle's post-FX targets and dye."""
-    return "half_postfx" in handle, "half_half" in handle
-
-
-def handle_for(pkg, oracle, handle, geometry, cfg):
+def handle_for(pkg, handle, geometry, cfg):
     """A handle of kind `handle` on `geometry` holding the parameter dye, and the dye as it holds it."""
     Wd, Hd, w, h = GEOMETRIES[geometry][:4]
-    s = NF.make(pkg, Wd, Hd, w, h, flags_of(pkg, handle), **cfg)
+    s = make(pkg, Wd, Hd, w, h, flags_of(pkg, handle), **cfg)
     dye = params_dye(Wd, Hd)
     s.writeField("dye", dye)
     s.dithering = golden_dither()
-    return s, NF.stored(oracle, storage(handle)[1], dye)
-
-
-def model_frame(handle, dye, w, h, kw, cfg, background):
-    """dict(bloom, sunrays) of the handle's model, and target (exact, without BLOOM) or lo / hi (with it)."""
-    half_t, half_m = storage(handle)
-    dither = golden_dither()
-    if handle.startswith("nearest"):
-        r = N.chains(dye, w, h, kw, cfg, half_targets=half_t, half_mask=half_m)
-        r.update(N.display(dye, w, h, kw, r["bloom"], r["sunrays"], dither, BACK_RGB, background, w / h))
-        return r
-    r = HP.render_keywords(dye, w, h, dither, cfg=cfg, back_rgb=BACK_RGB, background=background, keywords=kw,
-                           half_targets=half_t, half_mask=half_m)
-    if kw & M.BLOOM:
-        r["lo"], r["hi"] = G.display_interval(dye, w, h, kw, r["bloom"], r["sunrays"], dither, BACK_RGB, background, w / h)
-    else:
-        r["target"] = M._display(dye, w, h, kw, None, r["sunrays"], dither, BACK_RGB, background, w / h)
-    return r
-
-
-def model_capture(handle, dye, w, h, cw, ch, kw, cfg, transparent):
-    """dict(rgba8) exact without BLOOM, dict(lo, hi) byte bracket with it."""
-    half_t, half_m = storage(handle)
-    args = (dye, w, h, cw, ch, golden_dither(), kw, transparent, BACK_RGB)
-    if handle.startswith("nearest"):
-        return N.capture(*args, cfg=cfg, half_targets=half_t, half_mask=half_m)
-    if kw & M.BLOOM:
-        lo, hi = HP.capture_interval(*args, cfg=cfg, half_targets=half_t, half_mask=half_m)
-        return dict(lo=lo, hi=hi)
-    return dict(rgba8=HP.capture(*args, cfg=cfg, half_targets=half_t, half_mask=half_m)["rgba8"])
-
-
-def check_frame(s, got, want, kw, what):
-    if kw & M.BLOOM:
-        assert G.same_bits(s.last_bloom, want["bloom"]), what
-        n, bad = G.check_display(got, want["lo"], want["hi"])
-        assert n == 0, (what, n, bad)
-    else:
-        assert s.last_bloom is None and G.same_bits(got, want["target"]), what
-    if kw & M.SUNRAYS:
-        assert G.same_bits(s.last_sunrays, want["sunrays"]), what
-    else:
-        assert s.last_sunrays is None, what
+    return s, stored(handle, dye)
 
 
 @pytest.mark.parametrize("name", list(SETS))
@@ -109,24 +53,21 @@ def test_set_on_every_handle_kind(pkg, oracle, torch, handle, geometry, name):
     memory, against canvas_model applied to the handle's bare fragment."""
     cfg = cfg_of(name, geometry)
     w, h = GEOMETRIES[geometry][2:4]
-    tw, th = N.get_resolution(cfg["CAPTURE_RESOLUTION"], w, h)            # the capture target
-    s, dye = handle_for(pkg, oracle, handle, geometry, cfg)
+    tw, th = M.get_resolution(cfg["CAPTURE_RESOLUTION"], w, h)            # the capture target
+    s, dye = handle_for(pkg, handle, geometry, cfg)
     dev = torch.empty((h, w, 4), dtype=torch.uint8, device="cuda")
     with np.errstate(invalid="ignore", over="ignore", divide="ignore"):
         for kw in KEYWORD_SETS:
-            NF.set_keywords(s, kw)
+            set_keywords(s, kw)
             for transparent in (False, True):
                 what = (handle, geometry, name, kw, transparent)
                 s.config["TRANSPARENT"] = transparent
                 frame = s.render(w, h, target=transparent)
-                check_frame(s, frame, model_frame(handle, dye, w, h, kw, cfg, oracle.BG_NONE if transparent else oracle.BG_COLOR),
-                            kw, what)
+                want = model_frame(handle, dye, w, h, kw, golden_dither(), cfg,
+                                   oracle.BG_NONE if transparent else oracle.BG_COLOR)
+                check_frame(s, frame, want, kw, what)
                 got = s.captureScreenshot()
-                want = model_capture(handle, dye, tw, th, w, h, kw, cfg, transparent)
-                if "rgba8" in want:
-                    assert np.array_equal(got, want["rgba8"]), what
-                else:
-                    assert G.bytes_outside(got, want["lo"], want["hi"]) == 0, what
+                check_capture(got, model_capture(handle, dye, tw, th, w, h, kw, golden_dither(), cfg, transparent), kw, what)
                 if transparent:
                     bare = frame
             for transparent in (False, True):
@@ -166,8 +107,8 @@ def test_sliders_changed_between_frames(pkg, oracle, torch, handle):
     geometry = "pow2"
     w, h = GEOMETRIES[geometry][2:4]
     base = cfg_of("t1_k0_i2_w03", geometry)
-    s, _ = handle_for(pkg, oracle, handle, geometry, base)
-    NF.set_keywords(s, M.SHADING | M.BLOOM | M.SUNRAYS)
+    s, _ = handle_for(pkg, handle, geometry, base)
+    set_keywords(s, M.ALL3)
     seen = []
     with np.errstate(invalid="ignore", over="ignore"):
         for name in ("t1_k0_i2_w03", "t039_k1", "t1_k0_i2_w03", None):
@@ -178,8 +119,8 @@ def test_sliders_changed_between_frames(pkg, oracle, torch, handle):
             assert (fx.bloom_intensity, fx.bloom_threshold, fx.bloom_soft_knee, fx.sunrays_weight) == \
                 tuple(float(sliders[k]) for k in KEYS)
             got = outputs(s, torch, w, h)
-            fresh, _ = handle_for(pkg, oracle, handle, geometry, dict(base, **{k: sliders[k] for k in KEYS}))
-            NF.set_keywords(fresh, M.SHADING | M.BLOOM | M.SUNRAYS)
+            fresh, _ = handle_for(pkg, handle, geometry, dict(base, **{k: sliders[k] for k in KEYS}))
+            set_keywords(fresh, M.ALL3)
             assert same(got, outputs(fresh, torch, w, h)), (handle, name)
             fresh.close()
             seen.append(got)
@@ -193,10 +134,10 @@ def test_vs_executed_shaders(pkg, name):
     for bit, the frame within the keyword goldens' 3e-4 (test_gpu_display_keywords.py)."""
     g = golden(name)
     Wd, Hd, w, h = (int(g[k]) for k in ("Wd", "Hd", "w", "h"))
-    s = NF.make(pkg, Wd, Hd, w, h, 0, **fixture_cfg(g))
+    s = make(pkg, Wd, Hd, w, h, 0, **fixture_cfg(g))
     s.writeField("dye", g["in_dye"])
     s.dithering = g["dither"].astype(F32)
-    NF.set_keywords(s, M.SHADING | M.BLOOM | M.SUNRAYS)
+    set_keywords(s, M.ALL3)
     got = s.render(w, h)
     assert G.same_bits(s.last_bloom, g["bloom"]) and G.same_bits(s.last_sunrays, g["sunrays"])
     assert max_rel(got, g["target"]) < 3e-4

@@ -12,11 +12,12 @@ operations so far; replay(pkg, half, ops) runs a logged session again."""
 import numpy as np
 import pytest
 
-import display_keywords_model as M
+import display_harness as DH
+import display_model as M
 import gamma_model as G
 import session_model as S
 import splat_model as SM
-from conftest import bits_equal, golden
+from conftest import bits_equal
 from oracle import oracle as O
 from test_gpu_fast_paths import same_or_both_nan
 from webgl_fluid_simulation_b200 import slab
@@ -41,7 +42,7 @@ class Session:
         self.pkg, self.half = pkg, half
         self.sched = S.schedule(half)
         self.si = 0
-        self.dither = golden("postfx_64_to_128")["dither"].astype(np.float32)
+        self.dither = DH.golden_dither()
         W, H, Wd, Hd, cw, ch, _ = self.sched[0]
         flags = pkg.FLAG_HALF_STORAGE | pkg.FLAG_HALF_POSTFX if half else 0
         self.sims = [self._make(flags), self._make(flags | pkg.FLAG_NO_GRAPH)]
@@ -214,8 +215,8 @@ class Session:
 
     @staticmethod
     def _keywords(s, kw, transparent):
-        s.config.update(SHADING=bool(kw & M.SHADING), BLOOM=bool(kw & M.BLOOM), SUNRAYS=bool(kw & M.SUNRAYS),
-                        TRANSPARENT=transparent)
+        DH.set_keywords(s, kw)
+        s.config["TRANSPARENT"] = transparent
 
     def op_render(self, kw, transparent, target):
         frames = []
@@ -224,16 +225,7 @@ class Session:
             frames.append(s.render(target=target))
         g, t = self.sims
         bg = O.BG_NONE if transparent and target else O.BG_CHECKERBOARD if transparent else O.BG_COLOR
-        ref = self.model.render(kw, bg, self.dither, FX)
-        if kw & M.BLOOM:
-            assert G.same_bits(g.last_bloom, ref["bloom"]), "bloom FBO differs from the model"
-            lo, hi = self.model.frame_interval(kw, bg, self.dither, g.last_bloom, g.last_sunrays)
-            bad, first = G.check_display(frames[0], lo, hi)
-            assert bad == 0, ("frame outside the powf interval", bad, first)
-        else:
-            assert G.same_bits(frames[0], ref["target"]), "frame differs from the model"
-        if kw & M.SUNRAYS:
-            assert G.same_bits(g.last_sunrays, ref["sunrays"]), "sunrays texture differs from the model"
+        DH.check_frame(g, frames[0], self.model.render(kw, bg, self.dither, FX), kw, ("render", kw, transparent, target))
         assert G.same_bits(frames[1], frames[0])
 
     def op_capture(self, kw, transparent):
@@ -242,10 +234,7 @@ class Session:
             self._keywords(s, kw, transparent)
             got.append(s.captureScreenshot())
         ref = self.model.capture(kw, transparent, self.dither, FX, S.FXCFG["CAPTURE_RESOLUTION"])
-        if ref[0] == "exact":
-            assert np.array_equal(got[0], ref[1]), "capture differs from the model"
-        else:
-            assert G.bytes_outside(got[0], ref[1], ref[2]) == 0, "capture outside the powf interval"
+        DH.check_capture(got[0], ref, kw, ("capture", kw, transparent))
         assert np.array_equal(got[1], got[0])
 
 

@@ -1,13 +1,12 @@
-"""The storage of FLUID_FLAG_HALF_POSTFX on the CPU: half_postfx_model.render_postfx with half-float
+"""The storage of FLUID_FLAG_HALF_POSTFX on the CPU: display_model's chains with half-float
 targets (and, for a half-storage handle, a half-float sunrays mask) against the executed reference shaders
 with half-float textures (keywords_half_*.npz, capture_half_*.npz from tests/golden/make_golden_half_postfx.py),
 and the frame tolerance the GPU tests use against those fixtures."""
 import numpy as np
 import pytest
 
-import display_keywords_model as M
+import display_model as M
 import gamma_model as G
-import half_postfx_model as HP
 from conftest import golden, max_rel
 
 F32 = np.float32
@@ -35,8 +34,7 @@ def cfg_of(g):
 
 def half_chains(g, half_mask=True):
     w, h = int(g["w"]), int(g["h"])
-    return HP.render_postfx(g["in_dye"], w, h, g["dither"].astype(F32), cfg=cfg_of(g), half_targets=True,
-                           half_mask=half_mask)
+    return M.chains(g["in_dye"], w, h, M.BLOOM | M.SUNRAYS, cfg_of(g), half_targets=True, half_mask=half_mask)
 
 
 def fp16_ulps(a, b):
@@ -84,8 +82,8 @@ def test_frames_within_frame_tolerance(oracle, name):
     worst = 0.0
     for tag in (str(t) for t in g["sets"]):
         kw = KEYWORDS[tag]
-        ref = HP.render_keywords(g["in_dye"], w, h, g["dither"].astype(F32), cfg=cfg_of(g), back_rgb=BACK_RGB,
-                                keywords=kw, half_targets=True, half_mask=True)
+        ref = M.render(g["in_dye"], w, h, g["dither"].astype(F32), kw, cfg_of(g), back_rgb=BACK_RGB, half_targets=True,
+                       half_mask=True)
         if name == POW2:
             assert G.same_bits(ref["target"], g[f"{tag}_target"]), tag
         worst = max(worst, max_rel(ref["target"], g[f"{tag}_target"]))
@@ -99,30 +97,33 @@ def test_fp32_chains_are_not_the_half_float_frame(oracle):
     some set: the flag is needed to draw the reference's frame."""
     g = golden(POW2)
     w, h = int(g["w"]), int(g["h"])
-    worst = max(max_rel(M.render_keywords(g["in_dye"], w, h, g["dither"].astype(F32), cfg=cfg_of(g), back_rgb=BACK_RGB,
-                                          keywords=KEYWORDS[str(t)])["target"], g[f"{t}_target"]) for t in g["sets"])
+    worst = max(max_rel(M.render(g["in_dye"], w, h, g["dither"].astype(F32), KEYWORDS[str(t)], cfg_of(g),
+                                 back_rgb=BACK_RGB)["target"], g[f"{t}_target"]) for t in g["sets"])
     assert worst > FRAME_TOL, worst
 
 
 def test_defaults_are_the_oracle(oracle):
-    """render_postfx without the half keywords is oracle.render_postfx, bit for bit."""
+    """The model without half-float storage is oracle.render_postfx: chains bit for bit, the oracle's frame (glibc
+    powf) inside the model's powf interval at every value."""
     g = golden(POW2)
     w, h = int(g["w"]), int(g["h"])
-    a = HP.render_postfx(g["in_dye"], w, h, g["dither"].astype(F32), cfg=cfg_of(g), back_rgb=BACK_RGB)
+    a = M.render(g["in_dye"], w, h, g["dither"].astype(F32), M.ALL3, cfg_of(g), back_rgb=BACK_RGB)
     b = oracle.render_postfx(g["in_dye"], w, h, g["dither"].astype(F32), cfg=cfg_of(g), back_rgb=BACK_RGB)
-    for k in ("target", "bloom", "sunrays", "mask_alpha"):
+    for k in ("bloom", "sunrays", "mask_alpha"):
         assert G.same_bits(a[k], b[k]), k
+    assert len(a["pyramid"]) == len(b["pyramid"]) and all(G.same_bits(x, y) for x, y in zip(a["pyramid"], b["pyramid"]))
+    assert G.check_display(b["target"], a["lo"], a["hi"])[0] == 0
 
 
 @pytest.mark.parametrize("bg", ["back", "transparent"])
 def test_captures_equal_executed_shaders(oracle, bg):
-    """half_postfx_model.capture gives the executed capture's bytes exactly, all eight sets."""
+    """display_model.capture with half-float chains gives the executed capture's bytes exactly, all eight sets."""
     g = golden(f"capture_half_64_canvas_128_{bg}")
     cfg = cfg_of(g)
     for kw, tag in enumerate(CAPTURE_SETS):
-        c = HP.capture(g["in_dye"], int(g["w"]), int(g["h"]), int(g["canvas_w"]), int(g["canvas_h"]),
-                       g["dither"].astype(F32), kw, bool(g["transparent"]), BACK_RGB, cfg=cfg, half_targets=True,
-                       half_mask=True)
+        c = M.capture(g["in_dye"], int(g["w"]), int(g["h"]), int(g["canvas_w"]), int(g["canvas_h"]),
+                      g["dither"].astype(F32), kw, bool(g["transparent"]), BACK_RGB, cfg=cfg, half_targets=True,
+                      half_mask=True)
         assert np.array_equal(c["rgba8"], g[f"{tag}_rgba8"]), tag
 
 
@@ -131,9 +132,9 @@ def test_overflow_rounds_to_inf(oracle):
     finite values elsewhere (the input of the GPU overflow test)."""
     dye = np.full((64, 64, 4), 0.5, F32); dye[..., 3] = 1
     dye[20:24, 30:34, 0] = 2.0e5
-    dither, cfg = golden("postfx_64_to_128")["dither"].astype(F32), dict(BLOOM_RESOLUTION=64, SUNRAYS_RESOLUTION=48)
+    cfg = dict(BLOOM_RESOLUTION=64, SUNRAYS_RESOLUTION=48)
     with np.errstate(invalid="ignore", over="ignore"):
-        r = HP.render_postfx(dye, 128, 128, dither, cfg=cfg, half_targets=True)
-        r32 = HP.render_postfx(dye, 128, 128, dither, cfg=cfg)
+        r = M.chains(dye, 128, 128, M.BLOOM, cfg, half_targets=True)
+        r32 = M.chains(dye, 128, 128, M.BLOOM, cfg)
     assert np.isposinf(r["bloom"][..., 0]).any() and np.isfinite(r["bloom"][..., 1:3]).all()
     assert np.isfinite(r32["bloom"]).all() and r32["bloom"].max() > 65504

@@ -1,4 +1,4 @@
-"""FLUID_FLAG_NEAREST_FILTERING without a GPU: nearest_model.py against the executed NEAREST shaders
+"""FLUID_FLAG_NEAREST_FILTERING without a GPU: display_model.py's NEAREST sampler against the executed NEAREST shaders
 (tests/golden/make_golden_nearest.py) and the `nearest` keys of the resize fixtures; the two vUv
 conventions; the flag's value in every binding; default_config's override (S:109-114).
 
@@ -11,9 +11,8 @@ import numpy as np
 import pytest
 
 import capture_model as CM
-import display_keywords_model as M
+import display_model as M
 import gamma_model as G
-import nearest_model as N
 from conftest import golden
 from oracle import oracle as O
 
@@ -33,8 +32,8 @@ def cfg_of(g):
 def model_of(g, tag, conv, key="target"):
     w, h = int(g["w"]), int(g["h"])
     half = bool(g["half"])
-    return N.render(g["in_dye"], w, h, g["dither"].astype(F32), N.SETS[tag], cfg_of(g), back_rgb=tuple(g["back"] / 255),
-                    background=BACKGROUNDS[key], half_targets=half, half_mask=half, conv=conv)
+    return M.render(g["in_dye"], w, h, g["dither"].astype(F32), M.SETS[tag], cfg_of(g), back_rgb=tuple(g["back"] / 255),
+                    background=BACKGROUNDS[key], nearest=True, half_targets=half, half_mask=half, conv=conv)
 
 
 def check_against(g, conv):
@@ -49,7 +48,7 @@ def check_against(g, conv):
             for k, t in enumerate(r["pyramid"]):
                 assert G.same_bits(t, g[f"pyr{k}"]), (tag, k)
             want = g[f"{tag}_{key}"]
-            if "target" in r:
+            if not M.SETS[tag] & M.BLOOM:
                 assert G.same_bits(r["target"], want), (tag, key)
             else:
                 n, bad = G.check_display(want, r["lo"], r["hi"])
@@ -58,24 +57,24 @@ def check_against(g, conv):
 
 @pytest.mark.parametrize("name", POW2 + [RAGGED] + HALF + [TRANSPARENT])
 def test_raster_convention_equals_executed_shaders(name):
-    check_against(golden(name), N.RASTER)
+    check_against(golden(name), M.RASTER)
 
 
 @pytest.mark.parametrize("name", POW2 + HALF + [TRANSPARENT])
 def test_library_convention_equals_executed_shaders_at_power_of_two(name):
-    check_against(golden(name), N.LIBRARY)
+    check_against(golden(name), M.LIBRARY)
 
 
 @pytest.mark.parametrize("bg", ["back", "transparent"])
-@pytest.mark.parametrize("conv", [N.RASTER, N.LIBRARY])
+@pytest.mark.parametrize("conv", [M.RASTER, M.LIBRARY])
 def test_captures_equal_executed_shaders(bg, conv):
     g = golden(f"nearest_capture_64_canvas_128_{bg}")
     dye, w, h, cw, ch = g["in_dye"], int(g["w"]), int(g["h"]), int(g["canvas_w"]), int(g["canvas_h"])
     for tag in (str(t) for t in g["sets"]):
-        r = N.capture(dye, w, h, cw, ch, g["dither"].astype(F32), N.SETS[tag], bool(g["transparent"]),
-                      tuple(g["back"] / 255), cfg=cfg_of(g), conv=conv)
+        r = M.capture(dye, w, h, cw, ch, g["dither"].astype(F32), M.SETS[tag], bool(g["transparent"]),
+                      tuple(g["back"] / 255), cfg=cfg_of(g), nearest=True, conv=conv)
         want = g[f"{tag}_rgba8"]
-        if "rgba8" in r:
+        if not M.SETS[tag] & M.BLOOM:
             assert np.array_equal(r["rgba8"], want), tag
         else:
             assert G.bytes_outside(want, r["lo"], r["hi"]) == 0, tag
@@ -86,25 +85,25 @@ class Taps:
     """Records the (j, i) texel of every NEAREST fetch a call makes."""
 
     def __enter__(self):
-        self.taps, self._fetch = [], N.fetch
+        self.taps, self._fetch = [], M.nearest_fetch
 
         def fetch(tex, uvx, uvy):
-            self.taps.append(N.texel(tex, uvx, uvy))
+            self.taps.append(M.texel(tex, uvx, uvy))
             return self._fetch(tex, uvx, uvy)
-        N.fetch = fetch
+        M.nearest_fetch = fetch
         return self
 
     def __exit__(self, *exc):
-        N.fetch = self._fetch
+        M.nearest_fetch = self._fetch
 
 
 def flips(call):
     """Runs call(conv) in both conventions on the same inputs: (texels where the outputs differ, texels
     where some tap picked another texel)."""
     with Taps() as a:
-        out_l = call(N.LIBRARY)
+        out_l = call(M.LIBRARY)
     with Taps() as b:
-        out_r = call(N.RASTER)
+        out_r = call(M.RASTER)
     assert len(a.taps) == len(b.taps)
     shape = out_l.shape[:2]
     moved = np.zeros(shape, bool)
@@ -120,33 +119,35 @@ def ragged_passes(g):
     """Every NEAREST pass of the ragged fixture, each fed the executed shaders' own input textures."""
     w, h = int(g["w"]), int(g["h"])
     dye = g["in_dye"]
-    c = dict(N.chains(dye, w, h, N.BLOOM | N.SUNRAYS, cfg_of(g), conv=N.RASTER))
+    c = dict(M.chains(dye, w, h, M.BLOOM | M.SUNRAYS, cfg_of(g), nearest=True, conv=M.RASTER))
     bh, bw = c["bloom"].shape[:2]
     sh, sw = c["sunrays"].shape
     pyr = [g[f"pyr{k}"] for k in range(len(c["pyramid"]))]
-    mask = N.sunrays_mask(dye, N.RASTER)
-    tmp = N.blur3(N.sunrays(mask, sw, sh, 1.0, N.RASTER), 1.0 / sw, 0.0, N.RASTER)
-    prefiltered = N.prefilter(dye, bw, bh, 0.6, 0.7, N.RASTER)
-    passes = {"prefilter": lambda cv: N.prefilter(dye, bw, bh, 0.6, 0.7, cv),
-              "down0": lambda cv: N.box4(prefiltered, *pyr[0].shape[1::-1], conv=cv),
-              "mask": lambda cv: N.sunrays_mask(dye, cv),
-              "sunrays": lambda cv: N.sunrays(mask, sw, sh, 1.0, cv),
-              "blur_y": lambda cv: N.blur3(tmp, 0.0, 1.0 / sh, cv)}
+    N, crv = M.Nearest(M.RASTER), M.curve(0.6, 0.7)
+    mask = N.sunrays_mask(dye)
+    tmp = N.blur3(N.sunrays(mask, sw, sh, 1.0), 1.0 / sw, 0.0)
+    prefiltered = N.prefilter(dye, bw, bh, crv)
+    passes = {"prefilter": lambda cv: M.Nearest(cv).prefilter(dye, bw, bh, crv),
+              "down0": lambda cv: M.Nearest(cv).box4(prefiltered, *pyr[0].shape[1::-1]),
+              "mask": lambda cv: M.Nearest(cv).sunrays_mask(dye),
+              "sunrays": lambda cv: M.Nearest(cv).sunrays(mask, sw, sh, 1.0),
+              "blur_y": lambda cv: M.Nearest(cv).blur3(tmp, 0.0, 1.0 / sh)}
     for k in range(1, len(pyr)):
-        passes[f"down{k}"] = (lambda src, size: lambda cv: N.box4(src, *size, conv=cv))(_down(dye, g, k - 1), pyr[k].shape[1::-1])
+        passes[f"down{k}"] = (lambda src, size: lambda cv: M.Nearest(cv).box4(src, *size))(_down(dye, g, k - 1), pyr[k].shape[1::-1])
     for tag in ("none", "shading", "sunrays", "shading_sunrays"):
-        passes[f"display_{tag}"] = (lambda kw: lambda cv: N.display(dye, w, h, kw, None, g["sunrays"], None, tuple(g["back"] / 255),
-                                                                      O.BG_COLOR, w / h, cv)["target"])(N.SETS[tag])
+        passes[f"display_{tag}"] = (lambda kw: lambda cv: M.display(dye, w, h, kw, None, g["sunrays"], None, tuple(g["back"] / 255),
+                                                                      O.BG_COLOR, w / h, nearest=True, conv=cv)["target"])(M.SETS[tag])
     return passes
 
 
 def _down(dye, g, k):
     """Level k of the bloom pyramid on the way down, before the up-pass adds to it."""
     w, h = int(g["w"]), int(g["h"])
-    bw, bh = N.get_resolution(int(g["bloom_res"]), w, h)
-    last = N.prefilter(dye, bw, bh, 0.6, 0.7, N.RASTER)
+    bw, bh = M.get_resolution(int(g["bloom_res"]), w, h)
+    N = M.Nearest(M.RASTER)
+    last = N.prefilter(dye, bw, bh, M.curve(0.6, 0.7))
     for i in range(k + 1):
-        last = N.box4(last, bw >> (i + 1), bh >> (i + 1), conv=N.RASTER)
+        last = N.box4(last, bw >> (i + 1), bh >> (i + 1))
     return last
 
 
@@ -171,23 +172,23 @@ def test_index_arithmetic_of_the_conventions():
     """Centre taps agree at 48->50, 32->75, 910->1920 and 1024->300; the SHADING tap uv + texelSize does not
     at dye 512 -> target 1080 and at 40 -> 50."""
     def centre(n_tex, n_tgt, conv):
-        u = N.uv_grid(n_tgt, 1, conv)[0][0]
-        return N.texel(np.zeros((1, n_tex)), u, np.zeros_like(u))[1]
+        u = M.uv_grid(n_tgt, 1, conv)[0][0]
+        return M.texel(np.zeros((1, n_tex)), u, np.zeros_like(u))[1]
 
     def plus_ts(n_tex, n_tgt, conv):
-        u = N.uv_grid(n_tgt, 1, conv)[0][0] + F32(1.0 / n_tgt)
-        return N.texel(np.zeros((1, n_tex)), u, np.zeros_like(u))[1]
+        u = M.uv_grid(n_tgt, 1, conv)[0][0] + F32(1.0 / n_tgt)
+        return M.texel(np.zeros((1, n_tex)), u, np.zeros_like(u))[1]
     for n_tex, n_tgt in ((50, 48), (32, 75), (910, 1920), (1024, 300)):
-        assert np.array_equal(centre(n_tex, n_tgt, N.LIBRARY), centre(n_tex, n_tgt, N.RASTER)), (n_tex, n_tgt)
+        assert np.array_equal(centre(n_tex, n_tgt, M.LIBRARY), centre(n_tex, n_tgt, M.RASTER)), (n_tex, n_tgt)
     for n_tex, n_tgt in ((512, 1080), (40, 50)):
-        assert not np.array_equal(plus_ts(n_tex, n_tgt, N.LIBRARY), plus_ts(n_tex, n_tgt, N.RASTER)), (n_tex, n_tgt)
+        assert not np.array_equal(plus_ts(n_tex, n_tgt, M.LIBRARY), plus_ts(n_tex, n_tgt, M.RASTER)), (n_tex, n_tgt)
 
 
 @pytest.mark.parametrize("name", ["resample_dye_40x28_to_64x48", "resample_dye_64_to_32", "resample_v_32_to_48"])
 def test_resample_nearest_keys(name):
     g = golden(name)
-    for conv in (N.LIBRARY, N.RASTER):
-        assert G.same_bits(N.resize(g["src"], int(g["Wd"]), int(g["Hd"]), conv=conv), g["nearest"]), (name, conv)
+    for conv in (M.LIBRARY, M.RASTER):
+        assert G.same_bits(M.resize(g["src"], int(g["Wd"]), int(g["Hd"]), conv=conv), g["nearest"]), (name, conv)
 
 
 @pytest.mark.parametrize("name", POW2 + [RAGGED] + HALF)
@@ -197,8 +198,7 @@ def test_fixtures_discriminate_linear_from_nearest(name):
     w, h = int(g["w"]), int(g["h"])
     dye = g["in_dye"]
     for tag in (str(t) for t in g["sets"]):
-        kw = N.SETS[tag]
-        lin = M.render_keywords(dye, w, h, g["dither"].astype(F32), cfg=cfg_of(g), back_rgb=tuple(g["back"] / 255), keywords=kw)
+        lin = M.render(dye, w, h, g["dither"].astype(F32), M.SETS[tag], cfg_of(g), back_rgb=tuple(g["back"] / 255))
         assert not np.array_equal(lin["target"], g[f"{tag}_target"]), tag
 
 
@@ -226,9 +226,9 @@ def test_model_nearest_fetch_on_nonfinite_and_out_of_range_coordinates():
     """NaN -> texel 0, -inf / negative -> 0, +inf / >= 1 -> n - 1; a NaN texel reaches only its own texels."""
     tex = np.arange(12, dtype=F32).reshape(3, 4, 1)
     u = np.array([np.nan, -np.inf, -0.3, 0.0, 0.24, 0.26, 0.99, 1.0, np.inf], F32)
-    got = N.fetch(tex, u, np.zeros_like(u))[..., 0]
+    got = M.nearest_fetch(tex, u, np.zeros_like(u))[..., 0]
     assert got.tolist() == [0, 0, 0, 0, 0, 1, 3, 3, 3]
     dye = np.zeros((4, 4, 4), F32); dye[..., 3] = 1; dye[1, 2, 0] = np.nan
-    frame = N.display(dye, 8, 8, 0, None, None, None, (0, 0, 0), O.BG_COLOR, 1.0)["target"]
+    frame = M.display(dye, 8, 8, 0, None, None, None, (0, 0, 0), O.BG_COLOR, 1.0, nearest=True)["target"]
     assert np.argwhere(np.isnan(frame[..., 0])).tolist() == [[2, 4], [2, 5], [3, 4], [3, 5]]
     assert CM.to_bytes(frame).shape == frame.shape

@@ -6,7 +6,7 @@ wrong kernel:
 * branches: for every set, the bloom prefilter (bloomPrefilterShader S:614-631) sees enough texels below
   curve.x, inside the knee and above it, with rq winning and losing max(rq, br - threshold), and with br
   under the max(br, 0.0001) guard as zeros, fp32 subnormals and negatives;
-* mutants: each one-change copy of the chain model below -- one slider replaced by its default, threshold
+* mutants: each one-change variant of the chain model below -- one slider replaced by its default, threshold
   and knee swapped, knee / curve derived in fp32 instead of in JS doubles, the intensity applied on the
   additive up-pass instead of the final blit -- changes the expected bloom FBO or sunrays bits and the
   expected frame of at least one set, and all but the fp32 curve (a few ulp of bloom) its capture and canvas
@@ -19,15 +19,14 @@ import pytest
 
 import canvas_model as CV
 import capture_model as CM
-import display_keywords_model as M
-import half_postfx_model as HP
-import nearest_model as N
+import display_model as M
+import gamma_model as G
 from conftest import golden, max_rel
+from display_harness import BACK_RGB, golden_dither
 from oracle import oracle as O
-from test_gamma_model_cpu import BACK_RGB, golden_dither
 
 F32 = np.float32
-ALL3 = M.SHADING | M.BLOOM | M.SUNRAYS
+ALL3 = M.ALL3
 DEFAULTS = dict(BLOOM_INTENSITY=0.8, BLOOM_THRESHOLD=0.6, BLOOM_SOFT_KNEE=0.7, SUNRAYS_WEIGHT=1.0)   # S:79-84
 # (I, T, K, W).  t033_k07 and t039_k1 are slider positions where knee / curve narrowed from fp32 arithmetic
 # differ from the JS doubles narrowed once (all three curve components); t005 differs in curve.x and curve.z.
@@ -95,62 +94,17 @@ def params_dye(Wd, Hd, seed=DYE_SEED):
 MUTANTS = [f"default_{k}" for k in KEYS] + ["threshold_knee_swapped", "curve_in_fp32", "intensity_on_up_pass"]
 
 
-def curve(threshold, soft_knee, fp32=False):
-    """(curve.x, curve.y, curve.z, threshold) as the prefilter receives them: applyBloom derives them in JS
-    doubles (S:1358-1363) and gl.uniform narrows each once; `fp32` derives them in fp32 instead."""
-    if fp32:
-        t, k = F32(threshold), F32(soft_knee)
-        knee = t * k + F32(0.0001)
-        return t - knee, knee * F32(2), F32(0.25) / knee, t
-    knee = threshold * soft_knee + 0.0001
-    return F32(threshold - knee), F32(knee * 2), F32(0.25 / knee), F32(threshold)
-
-
 def chains(dye, w, h, cfg, mutant=None, half_targets=False, half_mask=False):
-    """The bloom FBO and the sunrays texture of render() on a w x h canvas: half_postfx_model.render_postfx's
-    chains (the oracle's per-blit C functions, rounded to fp16 after each blit with `half_targets`), with
-    one change when `mutant` names one of MUTANTS."""
+    """The bloom and sunrays chains of render() on a w x h canvas (display_model.chains, the fp16 stores with
+    `half_targets` / `half_mask`), with one change when `mutant` names one of MUTANTS."""
     assert mutant is None or mutant in MUTANTS, mutant
-    c = dict(BLOOM_ITERATIONS=8, BLOOM_RESOLUTION=256, SUNRAYS_RESOLUTION=196, **DEFAULTS)
-    c.update(cfg)
+    c = dict(cfg)
     if mutant and mutant.startswith("default_"):
         c[mutant[len("default_"):]] = DEFAULTS[mutant[len("default_"):]]
     if mutant == "threshold_knee_swapped":
         c["BLOOM_THRESHOLD"], c["BLOOM_SOFT_KNEE"] = c["BLOOM_SOFT_KNEE"], c["BLOOM_THRESHOLD"]
-    up, final = (c["BLOOM_INTENSITY"], 1.0) if mutant == "intensity_on_up_pass" else (1.0, c["BLOOM_INTENSITY"])
-    L, p = HP._chain_lib(), O._p
-    rt = O.round_half if half_targets else (lambda a: a)
-    dye = np.ascontiguousarray(dye, F32); Hd, Wd, _ = dye.shape
-    bw, bh = N.get_resolution(c["BLOOM_RESOLUTION"], w, h)
-    bloom = np.zeros((bh, bw, 4), F32); bloom[..., 3] = 1
-    sizes = [(bw >> (k + 1), bh >> (k + 1)) for k in range(c["BLOOM_ITERATIONS"])]
-    sizes = sizes[:next((k for k, (pw, ph) in enumerate(sizes) if pw < 2 or ph < 2), len(sizes))]
-    if len(sizes) >= 2:
-        L.oracle_bloom_prefilter(p(dye), Wd, Hd, p(bloom), bw, bh,
-                                 *(float(x) for x in curve(c["BLOOM_THRESHOLD"], c["BLOOM_SOFT_KNEE"], mutant == "curve_in_fp32")))
-        bloom = rt(bloom)
-        last, lw, lh, pyr = bloom, bw, bh, []
-        for pw, ph in sizes:
-            t = np.empty((ph, pw, 4), F32)
-            L.oracle_box4(p(last), lw, lh, p(t), pw, ph, 1.0, 0)
-            t = rt(t); pyr.append(t); last, lw, lh = t, pw, ph
-        for k in range(len(pyr) - 2, -1, -1):
-            pw, ph = sizes[k]
-            L.oracle_box4(p(last), lw, lh, p(pyr[k]), pw, ph, up, 1)
-            pyr[k] = rt(pyr[k]); last, lw, lh = pyr[k], pw, ph
-        L.oracle_box4(p(last), lw, lh, p(bloom), bw, bh, final, 0)
-        bloom = rt(bloom)
-    sw, sh = N.get_resolution(c["SUNRAYS_RESOLUTION"], w, h)
-    mask = np.empty_like(dye)
-    L.oracle_sunrays_mask(p(dye), p(mask), Wd, Hd)
-    mask = O.round_half(mask) if half_mask else mask
-    sun, tmp = np.empty((sh, sw), F32), np.empty((sh, sw), F32)
-    L.oracle_sunrays(p(mask), Wd, Hd, p(sun), sw, sh, c["SUNRAYS_WEIGHT"])
-    sun = rt(sun)
-    L.oracle_blur3(p(sun), p(tmp), sw, sh, 1.0 / sw, 0.0)
-    tmp = rt(tmp)
-    L.oracle_blur3(p(tmp), p(sun), sw, sh, 0.0, 1.0 / sh)
-    return dict(bloom=bloom, sunrays=rt(sun))
+    return M.chains(dye, w, h, M.BLOOM | M.SUNRAYS, c, half_targets=half_targets, half_mask=half_mask,
+                    fp32_curve=mutant == "curve_in_fp32", intensity_on_up_pass=mutant == "intensity_on_up_pass")
 
 
 def outputs(dye, geometry, name, mutant=None, kw=ALL3):
@@ -161,10 +115,11 @@ def outputs(dye, geometry, name, mutant=None, kw=ALL3):
     dither = golden_dither()
     with np.errstate(invalid="ignore", over="ignore"):
         r = chains(dye, w, h, cfg, mutant)
-        frame = M._display(dye, w, h, kw, r["bloom"], r["sunrays"], dither, BACK_RGB, O.BG_COLOR, w / h)
-        bare = M._display(dye, w, h, kw, r["bloom"], r["sunrays"], dither, BACK_RGB, O.BG_NONE, w / h)
-        cw_, ch_ = N.get_resolution(cfg["CAPTURE_RESOLUTION"], w, h)
-        pre = M._display(dye, cw_, ch_, kw, r["bloom"], r["sunrays"], dither, CM.back16(BACK_RGB), O.BG_COLOR, cw_ / ch_)
+        frame = M.display(dye, w, h, kw, r["bloom"], r["sunrays"], dither, BACK_RGB, O.BG_COLOR, w / h)["target"]
+        bare = M.display(dye, w, h, kw, r["bloom"], r["sunrays"], dither, BACK_RGB, O.BG_NONE, w / h)["target"]
+        cw_, ch_ = M.get_resolution(cfg["CAPTURE_RESOLUTION"], w, h)
+        pre = M.display(dye, cw_, ch_, kw, r["bloom"], r["sunrays"], dither, CM.back16(BACK_RGB), O.BG_COLOR,
+                        cw_ / ch_)["target"]
         canvas = [CV.canvas(bare, BACK_RGB, t, w / h) for t in (False, True)]
     return dict(r, frame=frame, capture=CM.to_bytes(pre)[::-1], canvas=canvas)
 
@@ -173,14 +128,13 @@ def outputs(dye, geometry, name, mutant=None, kw=ALL3):
 def fetched(dye, geometry, nearest=False):
     """The dye colour the prefilter fetches at every bloom texel (LINEAR or NEAREST, the library's vUv)."""
     Wd, Hd, w, h, bres = GEOMETRIES[geometry][:5]
-    bw, bh = N.get_resolution(bres, w, h)
-    uv = M.uv_grid(bw, bh)
-    return (N.fetch(dye, *uv) if nearest else M._fetch(dye, *uv))[..., :3].astype(F32)
+    bw, bh = M.get_resolution(bres, w, h)
+    return M.fetch(dye, *M.uv_grid(bw, bh), nearest)[..., :3].astype(F32)
 
 
 def branches(c, threshold, soft_knee):
     """{branch: number of texels} of the prefilter on fetched colours c, in its fp32 arithmetic."""
-    c0, c1, c2, th = curve(threshold, soft_knee)
+    c0, c1, c2, th = M.curve(threshold, soft_knee)
     br = np.fmax(c[..., 0], np.fmax(c[..., 1], c[..., 2]))
     x = br - c0
     rq = np.fmin(np.fmax(x, F32(0)), c1)
@@ -220,7 +174,7 @@ def test_sets_cover_the_slider_values():
     assert {0.0, 0.05, 0.6, 1.0} <= T and max(T) > params_dye(64, 64)[..., :3].max() + max(T) * 0.2 + 1e-4
     assert {0.0, 1.0} <= K and {0.0, 0.1, 2.0} <= I and max(I) > 3000 and {0.0, 0.3} <= W and max(W) > 1
     differ = [n for n, (_, t, k, _) in SETS.items() if 0 < t <= 1 and 0 < k <= 1
-              and not np.array_equal(np.array(curve(t, k), F32), np.array(curve(t, k, fp32=True), F32))]
+              and not np.array_equal(np.array(M.curve(t, k), F32), np.array(M.curve(t, k, fp32=True), F32))]
     assert len(differ) >= 2, differ
 
 
@@ -238,16 +192,27 @@ def test_above_and_overflow_sets_do_what_they_are_for(oracle):
 @pytest.mark.parametrize("half", [(False, False), (True, False), (True, True)])
 @pytest.mark.parametrize("geometry", list(GEOMETRIES))
 def test_chain_model_is_the_models_chains(oracle, geometry, half):
-    """Unmutated, chains() is half_postfx_model.render_postfx (and so oracle.render_postfx) bit for bit."""
+    """Unmutated, chains() is display_model.render's chains bit for bit.  With fp32 targets those are
+    oracle.render_postfx's bit for bit (bloom FBO, pyramid, sunrays, mask), and the oracle's frame lies inside
+    the model's powf interval."""
     Wd, Hd, w, h = GEOMETRIES[geometry][:4]
     dye = params_dye(Wd, Hd)
+    bits = lambda a, b: np.array_equal(a.view(np.uint32), b.view(np.uint32))          # noqa: E731
     for name in SETS:
         cfg = cfg_of(name, geometry)
         with np.errstate(over="ignore", invalid="ignore"):
             mine = chains(dye, w, h, cfg, half_targets=half[0], half_mask=half[1])
-            ref = HP.render_postfx(dye, w, h, golden_dither(), cfg=cfg, half_targets=half[0], half_mask=half[1])
+            ref = M.render(dye, w, h, golden_dither(), ALL3, cfg, back_rgb=BACK_RGB, half_targets=half[0],
+                           half_mask=half[1])
         for k in ("bloom", "sunrays"):
-            assert np.array_equal(mine[k].view(np.uint32), ref[k].view(np.uint32)), (name, k)
+            assert bits(mine[k], ref[k]), (name, k)
+        if half[0]:
+            continue
+        o = O.render_postfx(dye, w, h, golden_dither(), cfg=cfg, back_rgb=BACK_RGB)
+        for k in ("bloom", "sunrays", "mask_alpha"):
+            assert bits(ref[k], o[k]), (name, k)
+        assert len(ref["pyramid"]) == len(o["pyramid"]) and all(map(bits, ref["pyramid"], o["pyramid"])), name
+        assert G.check_display(o["target"], ref["lo"], ref["hi"])[0] == 0, name
 
 
 # Mutants whose change stays below one byte of every capture and canvas: curve_in_fp32 moves a curve
