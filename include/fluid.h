@@ -95,10 +95,33 @@ typedef enum fluid_param {
                                         0, n - 1), by fluid_render*, fluid_capture and fluid_resize's copy
                                         (resizeFBO S:1108-1114).  The dithering texture stays LINEAR + REPEAT.
                                         step(), splats, every fluid_pass_* and the host solves do not change:
-                                        the simulation is already the MANUAL_FILTERING path.  The config
-                                        override of S:109-114 (DYE_RESOLUTION 512, SHADING / BLOOM / SUNRAYS
-                                        off) is the host's (default_config).  Combines with HALF_STORAGE and
-                                        HALF_POSTFX; single GPU                                                */
+                                        advection is the MANUAL_FILTERING shader on every handle created
+                                        without FLUID_FLAG_LINEAR_ADVECTION, which is exactly this device's.
+                                        The config override of S:109-114 (DYE_RESOLUTION 512, SHADING / BLOOM /
+                                        SUNRAYS off) is the host's (default_config).  Combines with HALF_STORAGE
+                                        and HALF_POSTFX; single GPU                                            */
+#define FLUID_FLAG_LINEAR_ADVECTION 0x80u /* step() advects like the reference on a device WITH float linear
+                                        filtering (every desktop browser): the advectionShader's #else branch
+                                        (S:776-779) samples uVelocity and uSource through the LINEAR samplers
+                                        of dye and velocity (S:990).  Without this flag advection is the
+                                        MANUAL_FILTERING branch (bilerp S:758-770 over NEAREST fetches) on
+                                        every handle.  fluid_step (graph and pass by pass),
+                                        fluid_pass_advect_velocity and fluid_pass_advect_dye compute, in fp32
+                                        with every operation rounded on its own:
+                                          L(tex, n_x, n_y, uv): u = uv.x*n_x - .5, v = uv.y*n_y - .5,
+                                            i0 = floor(u), a = u - i0 (b likewise), taps clamped to the grid,
+                                            ((w00 t00 + w10 t10) + w01 t01) + w11 t11 with w00 = (1-a)(1-b),
+                                            w10 = a(1-b), w01 = (1-a)b, w11 = ab, taps widened from storage;
+                                          velocity: uv = cell centre, c = uv - (dt * L(vel, W, H, uv)) * ts,
+                                            out = L(vel, W, H, c) / (1 + VELOCITY_DISSIPATION * dt);
+                                          dye: uv = dye cell centre, c = uv - (dt * L(vel, W, H, uv)) * ts
+                                            (ts = the SIM texel size, S:1276),
+                                            out = L(dye, Wd, Hd, c) / (1 + DENSITY_DISSIPATION * dt);
+                                        rounded to fp16 when stored with HALF_STORAGE.  Splats, every other
+                                        pass, the host solves, resize and the display do not change.
+                                        HALF_STORAGE | HALF_POSTFX | LINEAR_ADVECTION is the desktop browser's
+                                        frame and step.  FLUID_ERR_INVALID with NEAREST_FILTERING (a device
+                                        without linear filtering runs MANUAL_FILTERING) and on slab handles  */
 #define FLUID_FLAG_TILED_PASSES 0x8u /* generation-1 kernels (one thread per fragment / smem tile) for
                                         curl-vorticity-divergence and gradientSubtract instead of the
                                         row-streaming ones (comparison + fallback path)              */
@@ -367,8 +390,10 @@ typedef enum fluid_stat_key {
     FLUID_STAT_HALO_TRANSPORT_P2P = 6, /* 1 when the peer-memory halo path is active                   */
     FLUID_STAT_CVD_STREAM_LAUNCHES = 7,      /* row-streaming curl-vorticity-divergence kernels executed */
     FLUID_STAT_GRADIENT_STREAM_LAUNCHES = 8, /* row-streaming gradientSubtract kernels executed          */
-    FLUID_STAT_JACOBI_EXACT_STREAMS = 9      /* blocked Jacobi warps that ran the un-contracted tail:
+    FLUID_STAT_JACOBI_EXACT_STREAMS = 9,     /* blocked Jacobi warps that ran the un-contracted tail:
                                                 tiny divergence, or inputs near FLT_MAX (synchronises)  */
+    FLUID_STAT_ADVECT4_LAUNCHES = 10         /* 4-cell advection kernels executed (velocity or dye, MANUAL
+                                                or LINEAR filter): fp32, power-of-two, width >= 128     */
 } fluid_stat_key;
 uint64_t fluid_stat(fluid_t* h, int key);
 

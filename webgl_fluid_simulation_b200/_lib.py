@@ -37,11 +37,12 @@ PARAM = {"DENSITY_DISSIPATION": 0, "VELOCITY_DISSIPATION": 1, "PRESSURE": 2,
 FLAG_UNFUSED, FLAG_NO_GRAPH, FLAG_NAIVE_JACOBI, FLAG_TILED_PASSES, FLAG_HALF_STORAGE = 0x1, 0x2, 0x4, 0x8, 0x10
 FLAG_HALF_POSTFX = 0x20         # fp16 bloom / sunrays targets like the reference's FBOs (include/fluid.h)
 FLAG_NEAREST_FILTERING = 0x40   # NEAREST display / post-FX / resize samplers, the reference without float linear filtering
+FLAG_LINEAR_ADVECTION = 0x80    # advection through LINEAR samplers, the reference with float linear filtering
 # display keywords of render() (updateKeywords, S:1160-1166): FLUID_DISPLAY_* of include/fluid.h
 DISPLAY_SHADING, DISPLAY_BLOOM, DISPLAY_SUNRAYS = 0x1, 0x2, 0x4
 STAT = {"launches": 0, "jacobi_launches": 1, "halo_launches": 2, "halo_exchanges": 3,
         "graph_captures": 4, "graph_launches": 5, "halo_transport_p2p": 6, "cvd_stream_launches": 7,
-        "gradient_stream_launches": 8, "jacobi_exact_streams": 9}
+        "gradient_stream_launches": 8, "jacobi_exact_streams": 9, "advect4_launches": 10}
 
 
 class FluidError(RuntimeError):

@@ -71,12 +71,14 @@ struct fluid : SlabGeometry {
     uint64_t halo_kernel_launches = 0;     // halo_push / halo_wait kernels of the peer-memory transport
     uint64_t cvd_stream_launches = 0;      // cvd_stream_kernel / gradient_stream_kernel (FLUID_STAT_*_STREAM_LAUNCHES):
     uint64_t gradient_stream_launches = 0; // which of a pass's kernels the grid size picked
+    uint64_t advect4_launches = 0;         // 4-cell advection kernels, either filter (FLUID_STAT_ADVECT4_LAUNCHES)
     uint64_t div_epoch = 1, div_sent_epoch = 0;   // slab: the divergence ghost rows are re-sent only after divergence was rewritten
     int div_sent_rows = 0;
     bool capturing = false;                // inside the stream capture of a step graph
     bool half = false;                     // FLUID_FLAG_HALF_STORAGE: fields are fp16 (half_passes.cuh), single GPU only
     bool half_fx = false;                  // FLUID_FLAG_HALF_POSTFX: the bloom and sunrays targets are fp16, single GPU only
     bool nearest = false;                  // FLUID_FLAG_NEAREST_FILTERING: display, post-FX and resize sample NEAREST, single GPU only
+    bool linear_adv = false;               // FLUID_FLAG_LINEAR_ADVECTION: advection samples LINEAR (passes.cuh LinearSampler), single GPU only
     float* scratch = nullptr;              // half mode: fp32 staging of fluid_read / fluid_write / render
     size_t scratch_floats = 0;
     float* dt_dev = nullptr;               // step()'s dt lives in device memory: one graph serves every dt
@@ -123,7 +125,8 @@ struct fluid : SlabGeometry {
     // ---- step() as a CUDA graph (single GPU): one instantiated graph per (dt, config scalars, parity)
     struct StepGraph {
         cudaGraphExec_t exec = nullptr;
-        int flip_v = 0, flip_p = 0, flip_dye = 0, kernels = 0, jacobi_launches = 0, cvd_stream = 0, gradient_stream = 0;
+        int flip_v = 0, flip_p = 0, flip_dye = 0, kernels = 0, jacobi_launches = 0, cvd_stream = 0, gradient_stream = 0,
+            advect4 = 0;
     };
     std::map<std::string, StepGraph> graphs;
     uint64_t graph_launches = 0, graph_captures = 0;
@@ -703,6 +706,16 @@ int create_common(const fluid_config* cfg, int rank, int world, const void* uid,
         int rc = fail(nullptr, FLUID_ERR_INVALID, "FLUID_FLAG_NEAREST_FILTERING is a single-GPU mode");
         delete h; return rc;
     }
+    h->linear_adv = (cfg->flags & FLUID_FLAG_LINEAR_ADVECTION) != 0;
+    if (h->linear_adv && h->nearest) {   // no float linear filtering means the MANUAL_FILTERING shader (S:783)
+        int rc = fail(nullptr, FLUID_ERR_INVALID, "FLUID_FLAG_LINEAR_ADVECTION needs linear filtering: it cannot be "
+                      "combined with FLUID_FLAG_NEAREST_FILTERING");
+        delete h; return rc;
+    }
+    if (h->linear_adv && world > 1) {
+        int rc = fail(nullptr, FLUID_ERR_INVALID, "FLUID_FLAG_LINEAR_ADVECTION is a single-GPU mode");
+        delete h; return rc;
+    }
     if (!slab_geometry(h, rank, world, cfg->sim_h, cfg->dye_h, cfg->pressure_iterations)) {
         int rc = fail(nullptr, FLUID_ERR_INVALID, "slabs of %d rows are too short for a 14-row halo: use fewer GPUs", cfg->sim_h / world);
         delete h; return rc;
@@ -1049,9 +1062,19 @@ static int do_advect_velocity(fluid_t* h, Grid out) {
     const bool p2 = !h->half && is_pow2(h->cfg.sim_w) && is_pow2(h->cfg.sim_h);
     if (p2 && h->cfg.sim_w >= 128 && !(h->cfg.flags & FLUID_FLAG_TILED_PASSES)) {    // 4 cells per thread, 32 apart
         dim3 b4(32, 8), g4(out.W / 128, (out.j_hi - out.j_lo + 7) / 8);
-        if (h->slab()) advect_velocity4_kernel<true><<<g4, b4, 0, h->stream>>>((const float2*)h->velocity.read, (float2*)h->velocity.write, a);
+        if (h->linear_adv) advect_velocity4_kernel<false, LinearSampler><<<g4, b4, 0, h->stream>>>((const float2*)h->velocity.read, (float2*)h->velocity.write, a);
+        else if (h->slab()) advect_velocity4_kernel<true><<<g4, b4, 0, h->stream>>>((const float2*)h->velocity.read, (float2*)h->velocity.write, a);
         else advect_velocity4_kernel<false><<<g4, b4, 0, h->stream>>>((const float2*)h->velocity.read, (float2*)h->velocity.write, a);
-    } else if (p2) advect_velocity_kernel<StoreF32, true><<<grid2d(out.W, out.j_hi - out.j_lo, b), b, 0, h->stream>>>(
+        ++h->advect4_launches;
+    } else if (h->linear_adv) with_storage(h, [&](auto s) {     // the LINEAR one-cell kernel, POW2 on fp32 or fp16
+        using S = decltype(s);
+        const bool q2 = is_pow2(h->cfg.sim_w) && is_pow2(h->cfg.sim_h);
+        const dim3 gr = grid2d(out.W, out.j_hi - out.j_lo, b);
+        const auto* V = (const typename S::T2*)h->velocity.read; auto* Vw = (typename S::T2*)h->velocity.write;
+        if (q2) advect_velocity_linear_kernel<S, true><<<gr, b, 0, h->stream>>>(V, Vw, a);
+        else advect_velocity_linear_kernel<S, false><<<gr, b, 0, h->stream>>>(V, Vw, a);
+    });
+    else if (p2) advect_velocity_kernel<StoreF32, true><<<grid2d(out.W, out.j_hi - out.j_lo, b), b, 0, h->stream>>>(
         (const float2*)h->velocity.read, (float2*)h->velocity.write, a);
     else with_storage(h, [&](auto s) {
         using S = decltype(s);
@@ -1078,11 +1101,21 @@ static int do_advect_dye(fluid_t* h) {
     const float2* V = (const float2*)h->velocity.read; const float4* Dr = (const float4*)h->dye.read; float4* Dw = (float4*)h->dye.write;
     if (p2 && a.src.W >= 128 && !(h->cfg.flags & FLUID_FLAG_TILED_PASSES)) {         // 4 cells per thread, 32 apart
         dim3 b4(32, 8), g4(a.src.W / 128, (a.src.j_hi - a.src.j_lo + 7) / 8);
-        if (same && h->slab()) advect_dye4_kernel<true, true><<<g4, b4, 0, h->stream>>>(V, Dr, Dw, a);
+        if (h->linear_adv) advect_dye4_kernel<false, false, LinearSampler><<<g4, b4, 0, h->stream>>>(V, Dr, Dw, a);   // SAME changes nothing for it
+        else if (same && h->slab()) advect_dye4_kernel<true, true><<<g4, b4, 0, h->stream>>>(V, Dr, Dw, a);
         else if (same) advect_dye4_kernel<true, false><<<g4, b4, 0, h->stream>>>(V, Dr, Dw, a);
         else if (h->slab()) advect_dye4_kernel<false, true><<<g4, b4, 0, h->stream>>>(V, Dr, Dw, a);
         else advect_dye4_kernel<false, false><<<g4, b4, 0, h->stream>>>(V, Dr, Dw, a);
-    } else if (p2 && same) advect_dye_kernel<StoreF32, true, true><<<gr, b, 0, h->stream>>>(V, Dr, Dw, a);
+        ++h->advect4_launches;
+    } else if (h->linear_adv) with_storage(h, [&](auto s) {     // the LINEAR one-cell kernel, POW2 on fp32 or fp16
+        using S = decltype(s);
+        const bool q2 = is_pow2(h->cfg.sim_w) && is_pow2(h->cfg.sim_h) && is_pow2(h->cfg.dye_w) && is_pow2(h->cfg.dye_h);
+        const auto* Vs = (const typename S::T2*)h->velocity.read;
+        const auto* Ds = (const typename S::T4*)h->dye.read; auto* Dws = (typename S::T4*)h->dye.write;
+        if (q2) advect_dye_linear_kernel<S, true><<<gr, b, 0, h->stream>>>(Vs, Ds, Dws, a);
+        else advect_dye_linear_kernel<S, false><<<gr, b, 0, h->stream>>>(Vs, Ds, Dws, a);
+    });
+    else if (p2 && same) advect_dye_kernel<StoreF32, true, true><<<gr, b, 0, h->stream>>>(V, Dr, Dw, a);
     else if (p2) advect_dye_kernel<StoreF32, true, false><<<gr, b, 0, h->stream>>>(V, Dr, Dw, a);
     else with_storage(h, [&](auto s) {
         using S = decltype(s);
@@ -1211,7 +1244,7 @@ int fluid_step(fluid_t* h, float dt) {
         if (h->graphs.size() > 64) drop_graphs(h);          // config sliders dragged for a long time: stay bounded
         const int pv = h->velocity.par, pp = h->pressure.par, pd = h->dye.par;
         const uint64_t l0 = h->launches, j0 = h->jacobi_kernel_launches;
-        const uint64_t cs0 = h->cvd_stream_launches, gs0 = h->gradient_stream_launches;
+        const uint64_t cs0 = h->cvd_stream_launches, gs0 = h->gradient_stream_launches, a40 = h->advect4_launches;
         cudaGraph_t g = nullptr;
         CU(cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeThreadLocal));
         h->capturing = true;
@@ -1227,8 +1260,9 @@ int fluid_step(fluid_t* h, float dt) {
         sg.flip_v = pv ^ h->velocity.par; sg.flip_p = pp ^ h->pressure.par; sg.flip_dye = pd ^ h->dye.par;
         sg.kernels = (int)(h->launches - l0); sg.jacobi_launches = (int)(h->jacobi_kernel_launches - j0);
         sg.cvd_stream = (int)(h->cvd_stream_launches - cs0); sg.gradient_stream = (int)(h->gradient_stream_launches - gs0);
+        sg.advect4 = (int)(h->advect4_launches - a40);
         h->launches = l0; h->jacobi_kernel_launches = j0;    // captured, not yet executed
-        h->cvd_stream_launches = cs0; h->gradient_stream_launches = gs0;
+        h->cvd_stream_launches = cs0; h->gradient_stream_launches = gs0; h->advect4_launches = a40;
         ++h->graph_captures;
         it = h->graphs.emplace(key, sg).first;
         // the capture already performed the host-side swaps of this step
@@ -1243,6 +1277,7 @@ int fluid_step(fluid_t* h, float dt) {
     h->jacobi_kernel_launches += it->second.jacobi_launches;
     h->cvd_stream_launches += it->second.cvd_stream;
     h->gradient_stream_launches += it->second.gradient_stream;
+    h->advect4_launches += it->second.advect4;
     h->timing.jacobi_launches = it->second.jacobi_launches;
     h->timing.total_launches = it->second.kernels;
     h->have_timing = false;
@@ -1940,6 +1975,7 @@ uint64_t fluid_stat(fluid_t* h, int key) {
         case FLUID_STAT_HALO_TRANSPORT_P2P: return h->p2p ? 1 : 0;
         case FLUID_STAT_CVD_STREAM_LAUNCHES: return h->cvd_stream_launches;
         case FLUID_STAT_GRADIENT_STREAM_LAUNCHES: return h->gradient_stream_launches;
+        case FLUID_STAT_ADVECT4_LAUNCHES: return h->advect4_launches;
         case FLUID_STAT_JACOBI_EXACT_STREAMS: {          // counted on the device: waits for the handle's work
             unsigned long long n = 0;
             if (cudaMemcpyAsync(&n, h->exact_streams, sizeof n, cudaMemcpyDeviceToHost, h->stream) != cudaSuccess ||

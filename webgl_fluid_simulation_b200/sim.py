@@ -194,6 +194,14 @@ class _Field:
 
 
 class FluidSimulation:
+    """The reference's simulation state and frame functions on one handle.  `flags` pick the device the
+    reference runs on: FLAG_NEAREST_FILTERING is a device without float linear filtering (NEAREST display /
+    post-FX / resize samplers, with its config override); FLAG_LINEAR_ADVECTION is a device with it, whose
+    step() advects through LINEAR samplers (the advectionShader's #else branch, S:776-779) instead of the
+    MANUAL_FILTERING bilerp every other handle runs.  FLAG_HALF_STORAGE | FLAG_HALF_POSTFX |
+    FLAG_LINEAR_ADVECTION is the desktop browser's frame and step.  LINEAR_ADVECTION is single-GPU and
+    refused with NEAREST_FILTERING; it adds no config override (the reference has none)."""
+
     def __init__(self, config: dict | None = None, canvas_width: int = 1024, canvas_height: int = 1024,
                  device: int = -1, flags: int = 0, jacobi_block: int = 0, random=None,
                  rank: int = 0, world: int = 1, nccl_uid: bytes | None = None,
@@ -443,7 +451,8 @@ class FluidSimulation:
         config.SHADING / BLOOM / SUNRAYS pick the display keywords like updateKeywords (S:1160-1166);
         BLOOM needs `sim.dithering`.  BLOOM or SUNRAYS need a single-GPU handle, fp32 or created with
         FLAG_HALF_POSTFX (then the bloom and sunrays targets are fp16, as are the reference's; with
-        FLAG_HALF_STORAGE | FLAG_HALF_POSTFX this is the reference's desktop frame).  last_bloom /
+        FLAG_HALF_STORAGE | FLAG_HALF_POSTFX this is the reference's desktop frame; FLAG_LINEAR_ADVECTION
+        changes how step() advects, not how a frame is drawn).  last_bloom /
         last_sunrays hold the bloom FBO / sunrays texture of the frame (widened to float32), or None when
         that keyword is off."""
         w = int(width or self.canvas["width"]); h = int(height or self.canvas["height"])
