@@ -247,6 +247,25 @@ int fluid_read(fluid_t* h, int field, float* host, size_t n_floats);
 /* Test / checkpoint hook with no reference counterpart: overwrites the `.read` buffer. */
 int fluid_write(fluid_t* h, int field, const float* host, size_t n_floats);
 
+/* fluid_read / fluid_write with the caller's DEVICE memory in place of host memory (for example a torch
+ * float32 CUDA tensor), for pipelines whose data already lives on the GPU: no PCIe transfer, no host stall.
+ *  - Layout, element count and bits are those of fluid_read / fluid_write: fp32, owned rows, row 0 at the
+ *    bottom, channels interleaved.  On a half-storage handle fluid_read_device widens exactly and
+ *    fluid_write_device narrows to nearest even (overflow to +-inf), on the device, allocating nothing.
+ *  - Written divergence rebuilds the blocked Jacobi solve's tiny-divergence map on the stream, as
+ *    fluid_write does: the solve that follows gives the same bits either way.
+ *  - Stream-ordered on the handle's stream; the calls return without synchronising, like
+ *    fluid_render_canvas(..., dst_on_device = 1).  The handle's stream is non-blocking: work of other
+ *    streams that uses the buffer must be complete before the call (sim.py's readField / writeField wait
+ *    for it), and the caller must call fluid_sync before it reads `dst` or reuses `src`.
+ * Refused with FLUID_ERR_INVALID, the buffer and every field untouched and the handle usable: n_floats !=
+ * fluid_field_elems; a NULL buffer; a bad field id; pageable or pinned host memory; memory of another
+ * device (managed memory of the handle's device is accepted); a buffer not 4-byte aligned; a buffer whose
+ * [ptr, ptr + 4 * n_floats) overlaps the handle's field arena (such as fluid_device_ptr of a field);
+ * slab handles (single-GPU entry points, like fluid_capture). */
+int fluid_read_device(fluid_t* h, int field, float* dst, size_t n_floats);
+int fluid_write_device(fluid_t* h, int field, const float* src, size_t n_floats);
+
 /* End-to-end form of the pressure solve for callers that keep fields in HOST memory: uploads
  * divergence and pressure, runs clear + `iters` Jacobi sweeps, downloads pressure.  All three
  * copies are inside the call (this is what bench.py's `e2e` times).  On a single-GPU handle the grid
@@ -330,6 +349,15 @@ int fluid_render_keywords(fluid_t* h, int width, int height, uint32_t keywords, 
 int fluid_capture(fluid_t* h, int width, int height, int canvas_w, int canvas_h, uint32_t keywords,
                   int transparent, const fluid_postfx* fx, const float* dither_rgb, int dw, int dh,
                   float back_r, float back_g, float back_b, uint8_t* host_rgba8, size_t n_bytes);
+/* fluid_capture into the caller's device memory (for example a torch uint8 CUDA tensor): the same bytes,
+ * stored by the display kernel itself, with the same launches and no device-to-host copy.  Stream-ordered
+ * and returning without synchronising, with the ordering rules of fluid_read_device: work of other streams
+ * that uses dst complete before the call, fluid_sync before reading dst.  Refused with FLUID_ERR_INVALID, dst
+ * untouched and the handle usable: everything fluid_capture refuses, and dst as fluid_read_device refuses it
+ * (NULL, host memory, another device, not 4-byte aligned, overlapping the field arena). */
+int fluid_capture_device(fluid_t* h, int width, int height, int canvas_w, int canvas_h, uint32_t keywords,
+                         int transparent, const fluid_postfx* fx, const float* dither_rgb, int dw, int dh,
+                         float back_r, float back_g, float back_b, uint8_t* dst, size_t n_bytes);
 
 /* render(null) of S:1296-1317 on the canvas: what a width x height drawing buffer holds after the frame.
  * The context is created with alpha: true (S:118-119), so the buffer is RGBA8 unsigned-normalised.  The
@@ -355,7 +383,7 @@ int fluid_capture(fluid_t* h, int width, int height, int canvas_w, int canvas_h,
  * Refused with FLUID_ERR_INVALID, dst untouched and the handle usable: n_bytes != 4 * width * height;
  * width or height < 1; unknown keyword bits; BLOOM without dither_rgb; fx == NULL with BLOOM or SUNRAYS;
  * half-storage handles with BLOOM or SUNRAYS unless created with FLUID_FLAG_HALF_POSTFX; dst_on_device with
- * host memory, memory of another device, or a misaligned dst; slab handles. */
+ * host memory, memory of another device, a misaligned dst, or a dst overlapping the field arena; slab handles. */
 int fluid_render_canvas(fluid_t* h, int width, int height, uint32_t keywords, int transparent,
                         const fluid_postfx* fx, const float* dither_rgb, int dw, int dh,
                         float back_r, float back_g, float back_b,

@@ -22,7 +22,7 @@ SYMBOLS = [
     "fluid_pass_divergence", "fluid_pass_clear_pressure", "fluid_pass_jacobi",
     "fluid_pass_pressure_solve", "fluid_pass_gradient_subtract", "fluid_pass_advect_velocity",
     "fluid_pass_advect_dye", "fluid_pass_curl_vorticity_divergence", "fluid_field_elems",
-    "fluid_field_dims", "fluid_read", "fluid_write", "fluid_pressure_solve_host", "fluid_render", "fluid_render_band", "fluid_render_postfx", "fluid_render_keywords", "fluid_capture", "fluid_render_canvas", "fluid_sync",
+    "fluid_field_dims", "fluid_read", "fluid_write", "fluid_read_device", "fluid_write_device", "fluid_pressure_solve_host", "fluid_render", "fluid_render_band", "fluid_render_postfx", "fluid_render_keywords", "fluid_capture", "fluid_capture_device", "fluid_render_canvas", "fluid_sync",
     "fluid_timing_last", "fluid_host_alloc", "fluid_host_free", "fluid_mark", "fluid_elapsed_ms", "fluid_launch_count", "fluid_device_ptr",
     "fluid_last_error",
 ]
@@ -121,12 +121,15 @@ def lib():
     L.fluid_field_dims.argtypes = [vp, i] + [C.POINTER(i)] * 4
     L.fluid_read.argtypes = [vp, i, vp, sz]
     L.fluid_write.argtypes = [vp, i, vp, sz]
+    L.fluid_read_device.argtypes = [vp, i, vp, sz]
+    L.fluid_write_device.argtypes = [vp, i, vp, sz]
     L.fluid_pressure_solve_host.argtypes = [vp, vp, vp, i]
     L.fluid_render.argtypes = [vp, i, i, i, f, f, f, vp, sz]
     L.fluid_render_band.argtypes = [vp, i, C.POINTER(i), C.POINTER(i)]
     L.fluid_render_postfx.argtypes = [vp, i, i, C.POINTER(PostFX), vp, i, i, f, f, f, vp, sz, vp, vp]
     L.fluid_render_keywords.argtypes = [vp, i, i, C.c_uint32, C.POINTER(PostFX), vp, i, i, f, f, f, vp, sz, vp, vp]
     L.fluid_capture.argtypes = [vp, i, i, i, i, C.c_uint32, i, C.POINTER(PostFX), vp, i, i, f, f, f, vp, sz]
+    L.fluid_capture_device.argtypes = L.fluid_capture.argtypes
     L.fluid_render_canvas.argtypes = [vp, i, i, C.c_uint32, i, C.POINTER(PostFX), vp, i, i, f, f, f, vp, sz, i]
     L.fluid_sync.argtypes = [vp]
     L.fluid_host_alloc.argtypes = [sz]; L.fluid_host_alloc.restype = vp

@@ -1438,6 +1438,70 @@ int fluid_write(fluid_t* h, int field, const float* host, size_t n_floats) {
     return FLUID_OK;
 }
 
+// A caller's device buffer [p, p + bytes): device or managed memory of the handle's device, 4-byte aligned
+// (float and uchar4 accesses), and outside the field arena, where it would alias a field.
+static int check_device_buf(fluid_t* h, const char* what, const void* p, size_t bytes) {
+    cudaPointerAttributes at{};
+    if (cudaPointerGetAttributes(&at, p) != cudaSuccess) {
+        cudaGetLastError();                      // not sticky: keep it out of the next launch check
+        return fail(h, FLUID_ERR_INVALID, "%s: the buffer is not a pointer CUDA knows", what);
+    }
+    if ((at.type != cudaMemoryTypeDevice && at.type != cudaMemoryTypeManaged) || at.device != h->device)
+        return fail(h, FLUID_ERR_INVALID, "%s needs device or managed memory of device %d (the buffer is %s memory of "
+                    "device %d)", what, h->device, at.type == cudaMemoryTypeHost ? "pinned host" : at.type == cudaMemoryTypeUnregistered
+                    ? "pageable host" : "device or managed", at.device);
+    if ((uintptr_t)p % 4)
+        return fail(h, FLUID_ERR_INVALID, "%s: a device buffer must be 4-byte aligned", what);
+    const uintptr_t a = (uintptr_t)h->arena, q = (uintptr_t)p;
+    if (q < a + h->layout.bytes && a < q + bytes)
+        return fail(h, FLUID_ERR_INVALID, "%s: the buffer overlaps the handle's field arena", what);
+    return FLUID_OK;
+}
+
+// The checks fluid_read_device / fluid_write_device share; *p / *n: the field's owned rows and their floats.
+static int device_io_args(fluid_t* h, const char* what, int field, const void* buf, size_t n_floats, void** p, size_t* n) {
+    int w, rows, ch;
+    if (!h) return FLUID_ERR_INVALID;
+    if (field_info(h, field, p, &w, &rows, &ch)) return fail(h, FLUID_ERR_INVALID, "%s: bad field %d", what, field);
+    *n = (size_t)w * rows * ch;
+    if (n_floats != *n) return fail(h, FLUID_ERR_INVALID, "%s: field %d has %zu floats, caller passed %zu", what, field, *n, n_floats);
+    if (!buf) return fail(h, FLUID_ERR_INVALID, "%s: NULL buffer", what);
+    if (h->slab()) return not_on_slab(h, what);
+    return check_device_buf(h, what, buf, *n * sizeof(float));
+}
+
+// fluid_read into device memory: the same bits, stream-ordered, no host copy and no sync.  Half storage widens
+// straight into the caller's buffer, so the call allocates nothing.
+int fluid_read_device(fluid_t* h, int field, float* dst, size_t n_floats) {
+    void* p = nullptr; size_t n = 0;
+    int rc = device_io_args(h, "fluid_read_device", field, dst, n_floats, &p, &n);
+    if (rc) return rc;
+    if (h->half) {
+        hs::widen_kernel<<<(unsigned)((n + 255) / 256), 256, 0, h->stream>>>((const hs::h1*)p, dst, n);
+        return check_launch(h, "hs::widen_kernel");
+    }
+    CU(cudaMemcpyAsync(dst, p, n * sizeof(float), cudaMemcpyDeviceToDevice, h->stream));
+    return FLUID_OK;
+}
+
+// fluid_write from device memory: the field ends with the bits fluid_write leaves, stream-ordered.  Written
+// divergence rebuilds the tiny-divergence map on the stream, as after a host write.
+int fluid_write_device(fluid_t* h, int field, const float* src, size_t n_floats) {
+    void* p = nullptr; size_t n = 0;
+    int rc = device_io_args(h, "fluid_write_device", field, src, n_floats, &p, &n);
+    if (rc) return rc;
+    if (h->half) {
+        hs::narrow_kernel<<<(unsigned)((n + 255) / 256), 256, 0, h->stream>>>(src, (hs::h1*)p, n);
+        return check_launch(h, "hs::narrow_kernel");
+    }
+    CU(cudaMemcpyAsync(p, src, n * sizeof(float), cudaMemcpyDeviceToDevice, h->stream));
+    if (field == FLUID_FIELD_DIVERGENCE) {
+        if ((rc = clear_tiny_map(h))) return rc;
+        if ((rc = scan_tiny(h, h->row0, h->row1))) return rc;
+    }
+    return FLUID_OK;
+}
+
 // fluid_pressure_solve_host on one GPU is PCIe-bound (4096^2: 128 MiB up, 64 MiB down per call), so
 // the solve is hidden behind the copies: the grid is cut into row bands, band b is solved as soon as its rows
 // (+ `iters` rows beyond it) have arrived and is copied back while the later bands still upload — the slab
@@ -1777,26 +1841,9 @@ struct DrawRequest {
     float* host_sunrays;
 };
 
-// A caller's device destination of the canvas: device or managed memory of the handle's device, 4-byte
-// aligned for the uchar4 stores.
-static int check_device_dst(fluid_t* h, const DrawRequest& r) {
-    cudaPointerAttributes at{};
-    if (cudaPointerGetAttributes(&at, r.dst) != cudaSuccess) {
-        cudaGetLastError();                      // not sticky: keep it out of the next launch check
-        return fail(h, FLUID_ERR_INVALID, "%s: dst is not a pointer CUDA knows", r.what);
-    }
-    if ((at.type != cudaMemoryTypeDevice && at.type != cudaMemoryTypeManaged) || at.device != h->device)
-        return fail(h, FLUID_ERR_INVALID, "%s: dst_on_device needs device or managed memory of device %d (dst is %s memory of "
-                    "device %d)", r.what, h->device, at.type == cudaMemoryTypeHost ? "pinned host" : at.type == cudaMemoryTypeUnregistered
-                    ? "pageable host" : "device or managed", at.device);
-    if ((uintptr_t)r.dst % 4)
-        return fail(h, FLUID_ERR_INVALID, "%s: a device dst must be 4-byte aligned", r.what);
-    return FLUID_OK;
-}
-
 // render(target) of S:1296-1317: the post-FX chains of the keywords that are on, then the background and
-// drawDisplay in one display_kernel launch, read back to the host (or, for a canvas into device memory,
-// left on the stream for the caller's fluid_sync).  Only the fp32 frame without BLOOM and
+// drawDisplay in one display_kernel launch, read back to the host (or, for a capture or canvas into device
+// memory, left on the stream for the caller's fluid_sync).  Only the fp32 frame without BLOOM and
 // SUNRAYS is drawn on a slab handle, and there only the handle's band of the target (fluid_render_band).
 // Half storage draws from a widened copy of dye; its post-FX needs FLUID_FLAG_HALF_POSTFX, and then the
 // chains read the fp16 dye directly and draw the mask into the fp16 dye.write.
@@ -1820,7 +1867,7 @@ static int draw(fluid_t* h, const DrawRequest& r) {
     if (h->half && !h->half_fx && postfx)
         return fail(h, FLUID_ERR_INVALID, "%s with BLOOM or SUNRAYS is not built for FLUID_FLAG_HALF_STORAGE "
                     "(the reference's bloom / sunrays FBOs are fp16 too: add FLUID_FLAG_HALF_POSTFX)", r.what);
-    int rc = r.on_device ? check_device_dst(h, r)
+    int rc = r.on_device ? check_device_buf(h, r.what, r.dst, r.n)
                          : need_frame(h, bytes ? (cells + 3) / 4 : cells);     // a uchar4 image lives in the frame
     if (rc) return rc;
     if (h->slab()) {
@@ -1896,16 +1943,32 @@ int fluid_render_postfx(fluid_t* h, int width, int height, const fluid_postfx* f
 // draws at the target's size over drawColor(BACK_COLOR) stored in fp16 (not TRANSPARENT) or bare with
 // blending off (TRANSPARENT), never over the checkerboard (S:1303-1314).  The display kernel's epilogue
 // does the fp16 store, the 8-bit truncation and the flip; the fp32 frame never reaches memory.
-int fluid_capture(fluid_t* h, int width, int height, int canvas_w, int canvas_h, uint32_t keywords,
-                  int transparent, const fluid_postfx* fx, const float* dither_rgb, int dw, int dh,
-                  float back_r, float back_g, float back_b, uint8_t* host_rgba8, size_t n_bytes) {
+static int capture(fluid_t* h, const char* what, int width, int height, int canvas_w, int canvas_h, uint32_t keywords,
+                   int transparent, const fluid_postfx* fx, const float* dither_rgb, int dw, int dh,
+                   float back_r, float back_g, float back_b, uint8_t* dst, size_t n_bytes, bool on_device) {
     // drawColor's store of normalizeColor(BACK_COLOR) into the half-float target
     const float b16[3] = {__half2float(__float2half_rn(back_r)), __half2float(__float2half_rn(back_g)),
                           __half2float(__float2half_rn(back_b))};
-    return draw(h, {.what = "fluid_capture", .width = width, .height = height, .canvas_w = canvas_w,
+    return draw(h, {.what = what, .width = width, .height = height, .canvas_w = canvas_w,
                     .canvas_h = canvas_h, .keywords = keywords, .fx = fx, .dither = dither_rgb, .dw = dw, .dh = dh,
                     .back = {b16[0], b16[1], b16[2]}, .bg_mode = transparent ? 2 : 0, .out = OUT_CAPTURE,
-                    .dst = host_rgba8, .n = n_bytes});
+                    .on_device = on_device, .dst = dst, .n = n_bytes});
+}
+
+int fluid_capture(fluid_t* h, int width, int height, int canvas_w, int canvas_h, uint32_t keywords,
+                  int transparent, const fluid_postfx* fx, const float* dither_rgb, int dw, int dh,
+                  float back_r, float back_g, float back_b, uint8_t* host_rgba8, size_t n_bytes) {
+    return capture(h, "fluid_capture", width, height, canvas_w, canvas_h, keywords, transparent, fx, dither_rgb, dw, dh,
+                   back_r, back_g, back_b, host_rgba8, n_bytes, false);
+}
+
+// The same image stored by the display kernel's StoreCapture epilogue straight into the caller's device memory,
+// stream-ordered.
+int fluid_capture_device(fluid_t* h, int width, int height, int canvas_w, int canvas_h, uint32_t keywords,
+                         int transparent, const fluid_postfx* fx, const float* dither_rgb, int dw, int dh,
+                         float back_r, float back_g, float back_b, uint8_t* dst, size_t n_bytes) {
+    return capture(h, "fluid_capture_device", width, height, canvas_w, canvas_h, keywords, transparent, fx, dither_rgb,
+                   dw, dh, back_r, back_g, back_b, dst, n_bytes, true);
 }
 
 // render(null) (S:1296-1317) on a width x height RGBA8 drawing buffer: the post-FX chains on the canvas-sized

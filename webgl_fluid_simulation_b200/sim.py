@@ -428,18 +428,37 @@ class FluidSimulation:
     def readField(self, name, out: np.ndarray | None = None) -> np.ndarray:
         """framebufferToTexture (S:301-307) generalised: rows x width [x channels] float32, row 0 =
         bottom.  On a slab rank: the rows this rank owns.  `out`: a caller-owned float32 buffer of
-        the right size (e.g. pinned host memory) to read into instead of allocating."""
+        the right size (e.g. pinned host memory) to read into instead of allocating, or a C-contiguous
+        float32 CUDA array on the handle's device (anything with __cuda_array_interface__, e.g. a torch
+        tensor) of exactly that many elements: the field is copied (widened, in half storage) on the GPU,
+        with no host copy, and the array is returned as it was passed.  The waits are render_canvas's:
+        pending work that may use the array first, the handle's stream before returning."""
         w, h, c, _ = self._dims(name)
+        n = w * h * c
+        dst = _device_array(out, "<f4", n, "readField")
+        if dst is not None:
+            self._check(self._L.fluid_read_device(self._h, FIELD[name], dst, n))
+            self.sync()
+            return out
         shape = (h, w, c) if c > 1 else (h, w)
         if out is None:
             out = np.empty(shape, np.float32)
         else:
-            assert out.dtype == np.float32 and out.flags.c_contiguous and out.size == h * w * c
+            assert out.dtype == np.float32 and out.flags.c_contiguous and out.size == n
             out = out.reshape(shape)
         self._check(self._L.fluid_read(self._h, FIELD[name], out.ctypes.data_as(C.c_void_p), out.size))
         return out
 
     def writeField(self, name, array):
+        """Overwrites a field with `array` (rows x width [x channels], row 0 = bottom): anything numpy turns
+        into float32, or a C-contiguous float32 CUDA array of exactly the field's element count, copied
+        (narrowed, in half storage) on the GPU with render_canvas's waits."""
+        if hasattr(array, "__cuda_array_interface__"):
+            w, h, c, _ = self._dims(name)
+            src = _device_array(array, "<f4", w * h * c, "writeField")
+            self._check(self._L.fluid_write_device(self._h, FIELD[name], src, w * h * c))
+            self.sync()
+            return
         a = np.ascontiguousarray(array, np.float32)
         self._check(self._L.fluid_write(self._h, FIELD[name], a.ctypes.data_as(C.c_void_p), a.size))
 
@@ -484,27 +503,39 @@ class FluidSimulation:
             bc["r"] / 255, bc["g"] / 255, bc["b"] / 255, ptr(out), out.size, ptr(self.last_bloom), ptr(self.last_sunrays)))
         return out
 
-    def captureScreenshot(self, path=None) -> np.ndarray:
+    def captureScreenshot(self, path=None, out=None) -> np.ndarray:
         """captureScreenshot(), S:287-299: render() into an RGBA half-float target of
         getResolution(CAPTURE_RESOLUTION) and normalizeTexture (S:309-327), all on the GPU.  Returns the
         (h, w, 4) uint8 image, TOP row first.  The bloom and sunrays FBOs keep the canvas sizes, as in the
         reference; config.TRANSPARENT stores the display bare (no checkerboard); BLOOM needs `sim.dithering`.
         BLOOM or SUNRAYS need the same handles as render().
-        With `path`, also writes the image as a PNG (write_png: the bytes unchanged)."""
+        With `path`, also writes the image as a PNG (write_png: the bytes unchanged).
+        `out`: a C-contiguous uint8 CUDA array on the handle's device of exactly 4 * w * h bytes (e.g. a torch
+        tensor): the display kernel stores the image into it, with no host copy and render_canvas's waits, and
+        the array is returned as it was passed.  A PNG needs host bytes, so `path` with `out` is refused."""
         cfg = self.config
         cw, ch = self.canvas["width"], self.canvas["height"]
         a = capture_inputs(cfg, cw, ch, getattr(self, "dithering", None))
         w, h, fx, dith = a["width"], a["height"], a["fx"], a["dither"]
         bc = cfg["BACK_COLOR"]                               # normalizeColor, S:1599-1606
-        out = np.empty((h, w, 4), np.uint8)
+        if out is not None:
+            if not hasattr(out, "__cuda_array_interface__"):
+                raise ValueError("captureScreenshot(out=...) takes a CUDA array; without `out` it returns a numpy image")
+            if path is not None:
+                raise ValueError("captureScreenshot writes a PNG from host bytes: pass `path` or a CUDA `out`, not both")
+        dst = _device_array(out, "|u1", 4 * w * h, "captureScreenshot")
+        img = np.empty((h, w, 4), np.uint8) if dst is None else None
         ptr = lambda x: None if x is None else x.ctypes.data_as(C.c_void_p)   # noqa: E731
-        self._check(self._L.fluid_capture(
+        self._check((self._L.fluid_capture if dst is None else self._L.fluid_capture_device)(
             self._h, w, h, cw, ch, a["keywords"], 1 if a["transparent"] else 0, None if fx is None else C.byref(fx),
             ptr(dith), 0 if dith is None else dith.shape[1], 0 if dith is None else dith.shape[0],
-            bc["r"] / 255, bc["g"] / 255, bc["b"] / 255, ptr(out), out.size))
+            bc["r"] / 255, bc["g"] / 255, bc["b"] / 255, ptr(img) if dst is None else dst, 4 * w * h))
+        if dst is not None:
+            self.sync()
+            return out
         if path is not None:
-            write_png(path, out)
-        return out
+            write_png(path, img)
+        return img
 
     def render_canvas(self, out=None):
         """render(null), S:1296-1317, on the canvas: canvas.width x canvas.height RGBA8, the bytes the
@@ -526,15 +557,10 @@ class FluidSimulation:
         self._push_config()                                  # the checkerboard uses canvas.width / canvas.height (S:1327)
         kw, fx, dith = postfx_inputs(cfg, getattr(self, "dithering", None))
         bc = cfg["BACK_COLOR"]                               # normalizeColor, S:1599-1606
-        cai = getattr(out, "__cuda_array_interface__", None)
-        if cai is not None:
-            shape, strides = tuple(cai["shape"]), cai.get("strides")
-            dense = strides is None or tuple(strides) == tuple(int(np.prod(shape[k + 1:])) for k in range(len(shape)))
-            if cai["typestr"] != "|u1" or int(np.prod(shape)) != n or not dense:
-                raise ValueError(f"render_canvas needs a C-contiguous uint8 CUDA array of {n} bytes, got "
-                                 f"{cai['typestr']} {shape} strides {strides}")
-            _wait_for_users(cai)
-            dst, result = C.c_void_p(cai["data"][0]), out
+        dst = _device_array(out, "|u1", n, "render_canvas")
+        on_device = dst is not None
+        if on_device:
+            result = out
         else:
             if out is None:
                 out = np.empty((h, w, 4), np.uint8)
@@ -545,8 +571,8 @@ class FluidSimulation:
         self._check(self._L.fluid_render_canvas(
             self._h, w, h, kw, 1 if cfg.get("TRANSPARENT") else 0, None if fx is None else C.byref(fx), ptr(dith),
             0 if dith is None else dith.shape[1], 0 if dith is None else dith.shape[0],
-            bc["r"] / 255, bc["g"] / 255, bc["b"] / 255, dst, n, 1 if cai is not None else 0))
-        if cai is not None:
+            bc["r"] / 255, bc["g"] / 255, bc["b"] / 255, dst, n, 1 if on_device else 0))
+        if on_device:
             self.sync()
         return result
 
@@ -623,6 +649,24 @@ class FluidSimulation:
 
 
 _cuda = None
+_TYPES = {"|u1": "uint8", "<f4": "float32"}
+
+
+def _device_array(a, typestr, n, what):
+    """None unless `a` has __cuda_array_interface__.  For a CUDA array: ValueError unless it is C-contiguous
+    with n elements of `typestr`; then, once _wait_for_users has returned, its device pointer."""
+    cai = getattr(a, "__cuda_array_interface__", None)
+    if cai is None:
+        return None
+    shape, strides = tuple(cai["shape"]), cai.get("strides")
+    item = np.dtype(typestr).itemsize
+    dense = strides is None or tuple(strides) == tuple(item * int(np.prod(shape[k + 1:])) for k in range(len(shape)))
+    if cai["typestr"] != typestr or int(np.prod(shape)) != n or not dense:
+        unit = "bytes" if item == 1 else "elements"
+        raise ValueError(f"{what} needs a C-contiguous {_TYPES[typestr]} CUDA array of {n} {unit}, got "
+                         f"{cai['typestr']} {shape} strides {strides}")
+    _wait_for_users(cai)
+    return C.c_void_p(cai["data"][0])
 
 
 def _wait_for_users(cai):
@@ -631,7 +675,7 @@ def _wait_for_users(cai):
     A version-3 interface names the producer's stream ("stream": None means nothing is pending; 1 and 2
     are the legacy and per-thread default streams, which the driver API takes as handles): that stream is
     synchronised.  Without the key (version 2, torch's) the array's device is synchronised, every stream.
-    A pointer the driver does not know is left alone: fluid_render_canvas refuses it."""
+    A pointer the driver does not know is left alone: the library refuses it."""
     global _cuda
     if "stream" in cai and cai["stream"] is None:
         return
