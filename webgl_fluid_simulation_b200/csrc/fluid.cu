@@ -15,6 +15,7 @@
 #include <cstring>
 #include <map>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "jacobi.cuh"
@@ -52,6 +53,28 @@ struct SlabGeometry {
     int ldrows() const { return drow1 - drow0 + 2 * Gd; }
 };
 
+// Kernel launches of a handle by kind (fluid_stat).  A step graph holds the counts of the step it captured
+// and adds them at every replay.
+struct LaunchCounts {
+    uint64_t all = 0;
+    uint64_t jacobi = 0;            // Jacobi kernels only (FLUID_STAT_JACOBI_LAUNCHES)
+    uint64_t halo = 0;              // halo_push / halo_wait kernels of the peer-memory transport
+    uint64_t cvd_stream = 0;        // cvd_stream_kernel / gradient_stream_kernel (FLUID_STAT_*_STREAM_LAUNCHES):
+    uint64_t gradient_stream = 0;   // which of a pass's kernels the grid size picked
+    uint64_t advect4 = 0;           // 4-cell advection kernels, either filter (FLUID_STAT_ADVECT4_LAUNCHES)
+    LaunchCounts& operator+=(const LaunchCounts& o) {
+        all += o.all; jacobi += o.jacobi; halo += o.halo;
+        cvd_stream += o.cvd_stream; gradient_stream += o.gradient_stream; advect4 += o.advect4;
+        return *this;
+    }
+    LaunchCounts operator-(const LaunchCounts& o) const {
+        LaunchCounts d = *this;
+        d.all -= o.all; d.jacobi -= o.jacobi; d.halo -= o.halo;
+        d.cvd_stream -= o.cvd_stream; d.gradient_stream -= o.gradient_stream; d.advect4 -= o.advect4;
+        return d;
+    }
+};
+
 }  // namespace
 
 struct fluid : SlabGeometry {
@@ -66,12 +89,7 @@ struct fluid : SlabGeometry {
     float* curl = nullptr;
     int* halo_flag = nullptr;        // device flag set by advection when a tap leaves the ghost zone
     unsigned long long* exact_streams = nullptr;   // device counter: blocked Jacobi warps that ran the exact tail
-    uint64_t launches = 0;
-    uint64_t jacobi_kernel_launches = 0;   // Jacobi kernels only (fluid_stat FLUID_STAT_JACOBI_LAUNCHES)
-    uint64_t halo_kernel_launches = 0;     // halo_push / halo_wait kernels of the peer-memory transport
-    uint64_t cvd_stream_launches = 0;      // cvd_stream_kernel / gradient_stream_kernel (FLUID_STAT_*_STREAM_LAUNCHES):
-    uint64_t gradient_stream_launches = 0; // which of a pass's kernels the grid size picked
-    uint64_t advect4_launches = 0;         // 4-cell advection kernels, either filter (FLUID_STAT_ADVECT4_LAUNCHES)
+    LaunchCounts launches;
     uint64_t div_epoch = 1, div_sent_epoch = 0;   // slab: the divergence ghost rows are re-sent only after divergence was rewritten
     int div_sent_rows = 0;
     bool capturing = false;                // inside the stream capture of a step graph
@@ -125,8 +143,8 @@ struct fluid : SlabGeometry {
     // ---- step() as a CUDA graph (single GPU): one instantiated graph per (dt, config scalars, parity)
     struct StepGraph {
         cudaGraphExec_t exec = nullptr;
-        int flip_v = 0, flip_p = 0, flip_dye = 0, kernels = 0, jacobi_launches = 0, cvd_stream = 0, gradient_stream = 0,
-            advect4 = 0;
+        int flip_v = 0, flip_p = 0, flip_dye = 0;
+        LaunchCounts launches;       // what one replay launches
     };
     std::map<std::string, StepGraph> graphs;
     uint64_t graph_launches = 0, graph_captures = 0;
@@ -196,7 +214,7 @@ int check_launch(fluid_t* h, const char* what, int n = 1) {
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess)
         return fail(h, FLUID_ERR_CUDA, "launch of %s failed: %s", what, cudaGetErrorString(e));
-    h->launches += n;
+    h->launches.all += n;
     return FLUID_OK;
 }
 
@@ -227,6 +245,24 @@ int need_scratch(fluid_t* h, size_t floats) {
 template <class F>
 auto with_storage(const fluid_t* h, F&& f) {
     return h->half ? f(hs::StoreHalf{}) : f(StoreF32{});
+}
+
+// Which advection kernel a pass runs, for the handle's filter policy F and storage S (passes.cuh), when
+// the sim grid and the advected grid are powers of two (p2) and the advected grid is w cells wide:
+//   4-cell    fp32 storage, p2, w >= 128 and no FLUID_FLAG_TILED_PASSES.  SLAB only on slab handles, which are
+//             always MANUAL.
+//   one-cell  otherwise; the POW2 form when p2, except for MANUAL half storage (pow2_form): its own-texel
+//             shortcut would give other bits than the reference's bilerp next to an inf or NaN neighbour.
+// The own texel, and SAME (dye grid == sim grid) with it, only with F::kOwnTexel.
+bool advect4_runs(const fluid_t* h, bool p2, int w) {
+    return p2 && !h->half && w >= 128 && !(h->cfg.flags & FLUID_FLAG_TILED_PASSES);
+}
+template <class S, class F>
+constexpr bool pow2_form = std::is_same<S, StoreF32>::value || !F::kOwnTexel;
+// f(LinearSampler{}) or f(ManualBilerp{}): an advection launch written once for the handle's filter policy
+template <class Fn>
+auto with_filter(const fluid_t* h, Fn&& f) {
+    return h->linear_adv ? f(LinearSampler{}) : f(ManualBilerp{});
 }
 
 // ---- the tiny-divergence map (jacobi.cuh): one byte per 128 x 32 cells of the GLOBAL grid -------------
@@ -388,7 +424,7 @@ int launch_tb(fluid_t* h, int K, bool scale, bool chained, JacobiArgs a, const T
     lc.attrs = attr; lc.numAttrs = (chained && !h->capturing) ? 1 : 0;
     lc.dynamicSmemBytes = e.smem;
     cudaLaunchKernelEx(&lc, e.kernel[scale], a, maps);
-    ++h->jacobi_kernel_launches;
+    ++h->launches.jacobi;
     return check_launch(h, "jacobi_tb_kernel");
 }
 
@@ -413,7 +449,7 @@ int launch_sweep(fluid_t* h, const JacobiArgs& a, bool scale) {
         });
         what = "jacobi_scalar_kernel";
     }
-    ++h->jacobi_kernel_launches;
+    ++h->launches.jacobi;
     return check_launch(h, what);
 }
 
@@ -1011,7 +1047,7 @@ static int do_cvd(fluid_t* h, Grid g) {
             (const float2*)h->velocity.read, h->curl, (float2*)h->velocity.write, h->divergence, a, h->cfg.curl,
             h->dt_dev, h->tiny_map);
         int rc = check_launch(h, "cvd_stream_kernel"); if (rc) return rc;
-        ++h->cvd_stream_launches;
+        ++h->launches.cvd_stream;
         h->velocity.swap();
         return FLUID_OK;
     }
@@ -1031,7 +1067,7 @@ static int do_gradient(fluid_t* h, Grid g) {
         gradient_stream_kernel<<<(nwarps + GS_WARPS - 1) / GS_WARPS, 32 * GS_WARPS, 0, h->stream>>>(
             (const float*)h->pressure.read, (const float2*)h->velocity.read, (float2*)h->velocity.write, a);
         int rc = check_launch(h, "gradient_stream_kernel"); if (rc) return rc;
-        ++h->gradient_stream_launches;
+        ++h->launches.gradient_stream;
         h->velocity.swap();                          // S:1273
         return FLUID_OK;
     }
@@ -1051,42 +1087,34 @@ static void valid_rows(int r0, int r1, int g, int H, int* lo, int* hi) {
     *lo = std::max(r0 - g, 0); *hi = std::min(r1 + g, H);
 }
 static int do_advect_velocity(fluid_t* h, Grid out) {
-    dim3 b(64, 4);
     AdvectArgs a{};
     a.vel = sim_grid(h); a.src = out;
     valid_rows(h->row0, h->row1, h->G, h->cfg.sim_h, &a.vel_lo, &a.vel_hi);
     a.src_lo = a.vel_lo; a.src_hi = a.vel_hi;
     a.dtp = h->dt_dev; a.dissipation = h->cfg.velocity_dissipation; a.halo_violation = h->halo_flag;
     a.tsx = a.dsx = (float)(1.0 / (double)h->cfg.sim_w); a.tsy = a.dsy = (float)(1.0 / (double)h->cfg.sim_h);
-    // half storage: the !POW2 kernel, which bilerps the own-texel velocity like the reference (passes.cuh)
-    const bool p2 = !h->half && is_pow2(h->cfg.sim_w) && is_pow2(h->cfg.sim_h);
-    if (p2 && h->cfg.sim_w >= 128 && !(h->cfg.flags & FLUID_FLAG_TILED_PASSES)) {    // 4 cells per thread, 32 apart
-        dim3 b4(32, 8), g4(out.W / 128, (out.j_hi - out.j_lo + 7) / 8);
-        if (h->linear_adv) advect_velocity4_kernel<false, LinearSampler><<<g4, b4, 0, h->stream>>>((const float2*)h->velocity.read, (float2*)h->velocity.write, a);
-        else if (h->slab()) advect_velocity4_kernel<true><<<g4, b4, 0, h->stream>>>((const float2*)h->velocity.read, (float2*)h->velocity.write, a);
-        else advect_velocity4_kernel<false><<<g4, b4, 0, h->stream>>>((const float2*)h->velocity.read, (float2*)h->velocity.write, a);
-        ++h->advect4_launches;
-    } else if (h->linear_adv) with_storage(h, [&](auto s) {     // the LINEAR one-cell kernel, POW2 on fp32 or fp16
-        using S = decltype(s);
-        const bool q2 = is_pow2(h->cfg.sim_w) && is_pow2(h->cfg.sim_h);
-        const dim3 gr = grid2d(out.W, out.j_hi - out.j_lo, b);
-        const auto* V = (const typename S::T2*)h->velocity.read; auto* Vw = (typename S::T2*)h->velocity.write;
-        if (q2) advect_velocity_linear_kernel<S, true><<<gr, b, 0, h->stream>>>(V, Vw, a);
-        else advect_velocity_linear_kernel<S, false><<<gr, b, 0, h->stream>>>(V, Vw, a);
+    const bool p2 = is_pow2(h->cfg.sim_w) && is_pow2(h->cfg.sim_h);
+    int rc = with_filter(h, [&](auto f) {
+        using F = decltype(f);
+        if (advect4_runs(h, p2, out.W)) {    // 4 cells per thread, 32 apart
+            auto* k = h->slab() ? advect_velocity4_kernel<true> : advect_velocity4_kernel<false, F>;
+            k<<<dim3(out.W / 128, (out.j_hi - out.j_lo + 7) / 8), dim3(32, 8), 0, h->stream>>>(
+                (const float2*)h->velocity.read, (float2*)h->velocity.write, a);
+            ++h->launches.advect4;
+        } else with_storage(h, [&](auto s) {
+            using S = decltype(s);
+            auto* k = p2 ? advect_velocity_kernel<S, F, pow2_form<S, F>> : advect_velocity_kernel<S, F, false>;
+            const dim3 b(64, 4);
+            k<<<grid2d(out.W, out.j_hi - out.j_lo, b), b, 0, h->stream>>>(
+                (const typename S::T2*)h->velocity.read, (typename S::T2*)h->velocity.write, a);
+        });
+        return check_launch(h, "advect_velocity_kernel");
     });
-    else if (p2) advect_velocity_kernel<StoreF32, true><<<grid2d(out.W, out.j_hi - out.j_lo, b), b, 0, h->stream>>>(
-        (const float2*)h->velocity.read, (float2*)h->velocity.write, a);
-    else with_storage(h, [&](auto s) {
-        using S = decltype(s);
-        advect_velocity_kernel<S, false><<<grid2d(out.W, out.j_hi - out.j_lo, b), b, 0, h->stream>>>(
-            (const typename S::T2*)h->velocity.read, (typename S::T2*)h->velocity.write, a);
-    });
-    int rc = check_launch(h, "advect_velocity_kernel"); if (rc) return rc;
+    if (rc) return rc;
     h->velocity.swap();                          // S:1285
     return FLUID_OK;
 }
 static int do_advect_dye(fluid_t* h) {
-    dim3 b(64, 4);
     AdvectArgs a{};
     a.vel = sim_grid(h); a.src = dye_grid(h);
     // after the velocity advection the slab holds valid velocity on owned rows +- 3
@@ -1095,34 +1123,30 @@ static int do_advect_dye(fluid_t* h) {
     a.dtp = h->dt_dev; a.dissipation = h->cfg.density_dissipation; a.halo_violation = h->halo_flag;
     a.tsx = (float)(1.0 / (double)h->cfg.sim_w); a.tsy = (float)(1.0 / (double)h->cfg.sim_h);
     a.dsx = (float)(1.0 / (double)h->cfg.dye_w); a.dsy = (float)(1.0 / (double)h->cfg.dye_h);
-    const bool p2 = !h->half && is_pow2(h->cfg.sim_w) && is_pow2(h->cfg.sim_h) && is_pow2(h->cfg.dye_w) && is_pow2(h->cfg.dye_h);
+    const bool p2 = is_pow2(h->cfg.sim_w) && is_pow2(h->cfg.sim_h) && is_pow2(h->cfg.dye_w) && is_pow2(h->cfg.dye_h);
     const bool same = h->cfg.sim_w == h->cfg.dye_w && h->cfg.sim_h == h->cfg.dye_h;
-    const dim3 gr = grid2d(a.src.W, a.src.j_hi - a.src.j_lo, b);
-    const float2* V = (const float2*)h->velocity.read; const float4* Dr = (const float4*)h->dye.read; float4* Dw = (float4*)h->dye.write;
-    if (p2 && a.src.W >= 128 && !(h->cfg.flags & FLUID_FLAG_TILED_PASSES)) {         // 4 cells per thread, 32 apart
-        dim3 b4(32, 8), g4(a.src.W / 128, (a.src.j_hi - a.src.j_lo + 7) / 8);
-        if (h->linear_adv) advect_dye4_kernel<false, false, LinearSampler><<<g4, b4, 0, h->stream>>>(V, Dr, Dw, a);   // SAME changes nothing for it
-        else if (same && h->slab()) advect_dye4_kernel<true, true><<<g4, b4, 0, h->stream>>>(V, Dr, Dw, a);
-        else if (same) advect_dye4_kernel<true, false><<<g4, b4, 0, h->stream>>>(V, Dr, Dw, a);
-        else if (h->slab()) advect_dye4_kernel<false, true><<<g4, b4, 0, h->stream>>>(V, Dr, Dw, a);
-        else advect_dye4_kernel<false, false><<<g4, b4, 0, h->stream>>>(V, Dr, Dw, a);
-        ++h->advect4_launches;
-    } else if (h->linear_adv) with_storage(h, [&](auto s) {     // the LINEAR one-cell kernel, POW2 on fp32 or fp16
-        using S = decltype(s);
-        const bool q2 = is_pow2(h->cfg.sim_w) && is_pow2(h->cfg.sim_h) && is_pow2(h->cfg.dye_w) && is_pow2(h->cfg.dye_h);
-        const auto* Vs = (const typename S::T2*)h->velocity.read;
-        const auto* Ds = (const typename S::T4*)h->dye.read; auto* Dws = (typename S::T4*)h->dye.write;
-        if (q2) advect_dye_linear_kernel<S, true><<<gr, b, 0, h->stream>>>(Vs, Ds, Dws, a);
-        else advect_dye_linear_kernel<S, false><<<gr, b, 0, h->stream>>>(Vs, Ds, Dws, a);
+    const Grid& out = a.src;
+    int rc = with_filter(h, [&](auto f) {
+        using F = decltype(f);
+        constexpr bool own = F::kOwnTexel;
+        if (advect4_runs(h, p2, out.W)) {    // 4 cells per thread, 32 apart
+            auto* k = h->slab() ? (same ? advect_dye4_kernel<true, true> : advect_dye4_kernel<false, true>)
+                                : (same ? advect_dye4_kernel<own, false, F> : advect_dye4_kernel<false, false, F>);
+            k<<<dim3(out.W / 128, (out.j_hi - out.j_lo + 7) / 8), dim3(32, 8), 0, h->stream>>>(
+                (const float2*)h->velocity.read, (const float4*)h->dye.read, (float4*)h->dye.write, a);
+            ++h->launches.advect4;
+        } else with_storage(h, [&](auto s) {
+            using S = decltype(s);
+            constexpr bool pf = pow2_form<S, F>;
+            auto* k = !p2  ? advect_dye_kernel<S, F, false, false>
+                    : same ? advect_dye_kernel<S, F, pf, pf && own> : advect_dye_kernel<S, F, pf, false>;
+            const dim3 b(64, 4);
+            k<<<grid2d(out.W, out.j_hi - out.j_lo, b), b, 0, h->stream>>>(
+                (const typename S::T2*)h->velocity.read, (const typename S::T4*)h->dye.read, (typename S::T4*)h->dye.write, a);
+        });
+        return check_launch(h, "advect_dye_kernel");
     });
-    else if (p2 && same) advect_dye_kernel<StoreF32, true, true><<<gr, b, 0, h->stream>>>(V, Dr, Dw, a);
-    else if (p2) advect_dye_kernel<StoreF32, true, false><<<gr, b, 0, h->stream>>>(V, Dr, Dw, a);
-    else with_storage(h, [&](auto s) {
-        using S = decltype(s);
-        advect_dye_kernel<S, false, false><<<gr, b, 0, h->stream>>>(
-            (const typename S::T2*)h->velocity.read, (const typename S::T4*)h->dye.read, (typename S::T4*)h->dye.write, a);
-    });
-    int rc = check_launch(h, "advect_dye_kernel"); if (rc) return rc;
+    if (rc) return rc;
     h->dye.swap();                                      // S:1293
     return FLUID_OK;
 }
@@ -1186,7 +1210,7 @@ int fluid_pass_advect_dye(fluid_t* h, float dt) {
 // step's advection (velocity on owned rows +- 3) and the last Jacobi launch (pressure on owned
 // rows +- 1) already computed redundantly.
 static int step_enqueue(fluid_t* h, bool timed) {
-    const uint64_t l0 = h->launches;
+    const uint64_t l0 = h->launches.all;
     int rc;
     int jl = 0;
     if (timed) cudaEventRecord(h->tev[0], h->stream);
@@ -1217,7 +1241,7 @@ static int step_enqueue(fluid_t* h, bool timed) {
     if ((rc = do_advect_dye(h))) return rc;
     if (timed) cudaEventRecord(h->tev[5], h->stream);
     h->timing.jacobi_launches = jl;
-    h->timing.total_launches = (int)(h->launches - l0);
+    h->timing.total_launches = (int)(h->launches.all - l0);
     h->have_timing = timed;
     return FLUID_OK;
 }
@@ -1243,8 +1267,7 @@ int fluid_step(fluid_t* h, float dt) {
     if (it == h->graphs.end()) {
         if (h->graphs.size() > 64) drop_graphs(h);          // config sliders dragged for a long time: stay bounded
         const int pv = h->velocity.par, pp = h->pressure.par, pd = h->dye.par;
-        const uint64_t l0 = h->launches, j0 = h->jacobi_kernel_launches;
-        const uint64_t cs0 = h->cvd_stream_launches, gs0 = h->gradient_stream_launches, a40 = h->advect4_launches;
+        const LaunchCounts n0 = h->launches;
         cudaGraph_t g = nullptr;
         CU(cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeThreadLocal));
         h->capturing = true;
@@ -1258,11 +1281,8 @@ int fluid_step(fluid_t* h, float dt) {
         cudaGraphDestroy(g);
         if (e != cudaSuccess) return fail(h, FLUID_ERR_CUDA, "cudaGraphInstantiate failed: %s", cudaGetErrorString(e));
         sg.flip_v = pv ^ h->velocity.par; sg.flip_p = pp ^ h->pressure.par; sg.flip_dye = pd ^ h->dye.par;
-        sg.kernels = (int)(h->launches - l0); sg.jacobi_launches = (int)(h->jacobi_kernel_launches - j0);
-        sg.cvd_stream = (int)(h->cvd_stream_launches - cs0); sg.gradient_stream = (int)(h->gradient_stream_launches - gs0);
-        sg.advect4 = (int)(h->advect4_launches - a40);
-        h->launches = l0; h->jacobi_kernel_launches = j0;    // captured, not yet executed
-        h->cvd_stream_launches = cs0; h->gradient_stream_launches = gs0; h->advect4_launches = a40;
+        sg.launches = h->launches - n0;
+        h->launches = n0;                                   // captured, not yet executed
         ++h->graph_captures;
         it = h->graphs.emplace(key, sg).first;
         // the capture already performed the host-side swaps of this step
@@ -1273,13 +1293,9 @@ int fluid_step(fluid_t* h, float dt) {
         if (sg.flip_dye) h->dye.swap();
     }
     CU(cudaGraphLaunch(it->second.exec, h->stream));
-    h->launches += it->second.kernels;
-    h->jacobi_kernel_launches += it->second.jacobi_launches;
-    h->cvd_stream_launches += it->second.cvd_stream;
-    h->gradient_stream_launches += it->second.gradient_stream;
-    h->advect4_launches += it->second.advect4;
-    h->timing.jacobi_launches = it->second.jacobi_launches;
-    h->timing.total_launches = it->second.kernels;
+    h->launches += it->second.launches;
+    h->timing.jacobi_launches = (int)it->second.launches.jacobi;
+    h->timing.total_launches = (int)it->second.launches.all;
     h->have_timing = false;
     ++h->graph_launches;
     return FLUID_OK;
@@ -2024,21 +2040,21 @@ int fluid_elapsed_ms(fluid_t* h, float* ms) {
     return FLUID_OK;
 }
 
-uint64_t fluid_launch_count(fluid_t* h) { return h ? h->launches : 0; }
+uint64_t fluid_launch_count(fluid_t* h) { return h ? h->launches.all : 0; }
 
 uint64_t fluid_stat(fluid_t* h, int key) {
     if (!h) return 0;
     switch (key) {
-        case FLUID_STAT_LAUNCHES: return h->launches;
-        case FLUID_STAT_JACOBI_LAUNCHES: return h->jacobi_kernel_launches;
-        case FLUID_STAT_HALO_LAUNCHES: return h->halo_kernel_launches;
+        case FLUID_STAT_LAUNCHES: return h->launches.all;
+        case FLUID_STAT_JACOBI_LAUNCHES: return h->launches.jacobi;
+        case FLUID_STAT_HALO_LAUNCHES: return h->launches.halo;
         case FLUID_STAT_HALO_EXCHANGES: return h->halo_groups;
         case FLUID_STAT_GRAPH_CAPTURES: return h->graph_captures;
         case FLUID_STAT_GRAPH_LAUNCHES: return h->graph_launches;
         case FLUID_STAT_HALO_TRANSPORT_P2P: return h->p2p ? 1 : 0;
-        case FLUID_STAT_CVD_STREAM_LAUNCHES: return h->cvd_stream_launches;
-        case FLUID_STAT_GRADIENT_STREAM_LAUNCHES: return h->gradient_stream_launches;
-        case FLUID_STAT_ADVECT4_LAUNCHES: return h->advect4_launches;
+        case FLUID_STAT_CVD_STREAM_LAUNCHES: return h->launches.cvd_stream;
+        case FLUID_STAT_GRADIENT_STREAM_LAUNCHES: return h->launches.gradient_stream;
+        case FLUID_STAT_ADVECT4_LAUNCHES: return h->launches.advect4;
         case FLUID_STAT_JACOBI_EXACT_STREAMS: {          // counted on the device: waits for the handle's work
             unsigned long long n = 0;
             if (cudaMemcpyAsync(&n, h->exact_streams, sizeof n, cudaMemcpyDeviceToHost, h->stream) != cudaSuccess ||

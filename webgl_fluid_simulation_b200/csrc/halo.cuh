@@ -148,7 +148,7 @@ int exchange_p2p(fluid_t* h, const HaloItem* it, int count) {
     }
     halo_push_kernel<<<blocks, 256, 0, h->stream>>>(pa);     // push + handshake + wait + scan: one launch per exchange
     int rc = check_launch(h, "halo_push_kernel"); if (rc) return rc;
-    h->halo_kernel_launches += 1;
+    h->launches.halo += 1;
     ++h->halo_groups;
     return FLUID_OK;
 }
