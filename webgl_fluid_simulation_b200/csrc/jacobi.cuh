@@ -163,7 +163,9 @@ struct TB {
     static constexpr int U = 3;                      // pipeline steps per unrolled block
     // NS stages, each a 3-row box of div followed by a 3-row box of p (row = 544 B), each box padded to a
     // multiple of 128 B, the alignment TMA needs of its destination; then NS mbarriers
-    static constexpr int NS = 4;
+    // Three stages: the boxes of a block are requested at the end of the block two before it.  A fourth
+    // stage, more bytes in flight per warp, made the solve slower (DESIGN 5.12).
+    static constexpr int NS = 3;
     static constexpr int ROW4 = TB_BOX / 4;          // float4 per staged row
     static constexpr int P4 = (U * ROW4 + 7) / 8 * 8;                   // float4 offset of the p box in a stage
     static constexpr int TX = 2 * U * ROW4 * (int)sizeof(float4);       // bytes one stage's two boxes bring
