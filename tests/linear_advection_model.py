@@ -23,6 +23,7 @@ from oracle import oracle as O
 
 F = np.float32
 ROWS = 256          # rows per chunk: bounds the temporaries at 4096^2 dye
+P4_HALF_GATE = 1e-6  # max_rel of the fp16 desktop scenario after one step (p4_linear_half_32), CPU and GPU
 
 
 def texel_index(f, n):

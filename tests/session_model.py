@@ -23,7 +23,7 @@ Data restrictions: fp32 sessions keep inf / NaN out of velocity, pressure and di
 power-of-two advection takes a texel's own velocity where the oracle bilerps it, so a non-finite
 neighbour legitimately differs -- test_advection_far_outside_the_grid_vs_oracle); dye may hold them, and
 subnormals and large finite values go everywhere.  Half-storage sessions write the special values of
-test_gpu_half_storage_special.special_fields.
+sim_harness.special_fields.
 """
 from __future__ import annotations
 
@@ -32,8 +32,7 @@ import numpy as np
 import display_model as M
 import splat_model as SM
 from oracle import oracle as O
-from test_gpu_half_storage_special import special_fields
-from test_gpu_splats import nasty_fields, nasty_records
+from sim_harness import nasty_fields, nasty_records, special_fields
 
 F32 = np.float32
 FIELDS = ("velocity", "dye", "pressure", "divergence", "curl")
@@ -47,7 +46,7 @@ DT_CLAMP = 0.016666         # calcDeltaTime's min(dt, 0.016666), S:1188-1194
 
 # ---- sizes -------------------------------------------------------------------------------------------
 # (W, H, Wd, Hd, canvas_w, canvas_h, classes): classes name what fluid.cu selects at that size, as the
-# suite's other tests establish it (test_gpu_parity STREAM_SHAPES / TILED_SHAPES / HALF_SIZES,
+# suite's other tests establish it (sim_harness STREAM_SHAPES / TILED_SHAPES, test_gpu_parity HALF_SIZES,
 # test_gpu_fast_paths ADVECT_SHAPES, test_host_pressure_solve_banded_pipeline).  They are labels, not
 # a restatement of the selection rules: the GPU test checks them through fluid_stat.
 #   stream / tiled       curl-vorticity-divergence + gradientSubtract kernels
@@ -105,6 +104,9 @@ CONFIG_VALUES = {
 JACOBI_BLOCKS = (0, 1, 7, 13)
 SPLATS_N = (2, 5, 127, 128, 129, 200)
 TINY_DT = 1e-30
+# the committed sessions: together their seeds reach every class (test_session_model_cpu.py)
+SEEDS = {False: (3, 10, 76, 4, 5), True: (1, 3, 12, 2, 4)}
+N_OPS = 40
 
 
 def random_dt(rng) -> float:

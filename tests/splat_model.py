@@ -20,10 +20,15 @@ the subnormal ulp).  Every later step is monotone in e and in the base -- e*c (n
 c >= 0, non-increasing for c < 0), base + t, the fp16 rounding of half storage -- so [lo, hi] carries
 through any number of records, texel by texel.  A NaN base stays NaN and an inf base the same inf;
 where lo and hi are zeros of one sign the result is that zero (-0 + e*c with e*c == +0 is +0).
+
+The cases the CPU premises (tests/test_splat_model_cpu.py) and the GPU bounds (tests/test_gpu_splat_bounds.py)
+share close the file: grids, starting fields, radii, canvases and records.
 """
 from __future__ import annotations
 
 import numpy as np
+
+from sim_harness import SIZES, exp_tiled, nasty_fields, nasty_records
 
 F32 = np.float32
 # CUDA Math API, expf: maximum error 2 ulp (full range, without -use_fast_math)
@@ -141,3 +146,36 @@ def check_splat(got, lo, hi, limit: int = 8):
     out = [(tuple(int(t) for t in ix), float(got[tuple(ix)]), float(lo[tuple(ix)]), float(hi[tuple(ix)]))
            for ix in bad[:limit]]
     return int(len(bad)), out
+
+
+# ---- the cases -------------------------------------------------------------------------------------------
+# SIZES plus partial 128x16 splat tiles in both directions on both planes
+GRIDS = SIZES + [(129, 17, 257, 33)]
+BASES = ["zero", "exp_tiled", "nasty"]
+RADII = [0.25, 0.01, 1.0, 5e-5]          # 5e-5: radius 5e-7 < 2^-20, every warp takes the IEEE division
+# aspect 1, > 1, < 1, and a canvas whose radius depends on narrowing the aspect before the multiply
+CANVASES = [(100, 100), (300, 200), (200, 300), (142, 100)]
+NARROWING_CANVAS = (142, 100)
+
+
+def records(n, seed, planes):
+    """nasty_records (far points, points outside [0, 1], large forces, (.5, .5)) with every 4th record
+    from the second on moved onto a texel centre of one of `planes` ((W, H) pairs): d == 0 there."""
+    r = nasty_records(n, seed)
+    rng = np.random.default_rng(seed + 1)
+    for k in range(1, n, 4):
+        W, H = planes[(k // 4) % len(planes)]
+        r[k, 0] = uv(W)[rng.integers(0, W)]
+        r[k, 1] = uv(H)[rng.integers(0, H)]
+    return r
+
+
+def bases(kind, W, H, Wd, Hd, seed):
+    """(velocity, dye) starting fields: zeros, one binary exponent in [-149, 100] per tile with random
+    mantissas and signs, or nasty_fields (-0, subnormals, +-inf, NaN over ordinary values)."""
+    if kind == "zero":
+        return np.zeros((H, W, 2), F32), np.zeros((Hd, Wd, 4), F32)
+    if kind == "exp_tiled":
+        return exp_tiled((H, W, 2), seed, tile=(4, 8)), exp_tiled((Hd, Wd, 4), seed + 1, tile=(4, 8))
+    v, d, _ = nasty_fields(W, H, Wd, Hd, seed)
+    return v, d

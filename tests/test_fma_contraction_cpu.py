@@ -17,84 +17,13 @@ from fractions import Fraction
 
 import numpy as np
 
-from jacobi_tb_model import BIG_IN, fma_tail
+from jacobi_tb_model import BIG_IN, _finite, add32, fma, fma32, fma_tail, mul32, ref
 
 F32 = np.float32
 TINY = 2.0 ** -123
 FLT_MAX = float(np.finfo(np.float32).max)              # 2^128 - 2^104
 OVERFLOW = Fraction(2) ** 128 - Fraction(2) ** 103     # rn32(x) is +-inf iff |x| >= this
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def rn32(x: Fraction) -> np.float32:
-    """Correctly rounded (nearest-even) fp32 of a nonzero exact rational, subnormals and overflow included.
-    A result that underflows to zero keeps the sign of x."""
-    s = -1 if x < 0 else 1
-    a = abs(x)
-    # exponent e with 2^e <= a < 2^(e+1)
-    e = a.numerator.bit_length() - a.denominator.bit_length()
-    if Fraction(2) ** e > a:
-        e -= 1
-    e = max(e, -126)                      # subnormals share the exponent of the smallest normal
-    ulp = Fraction(2) ** (e - 23)
-    q, r = divmod(a, ulp)
-    q = int(q)
-    if r * 2 > ulp or (r * 2 == ulp and (q & 1)):
-        q += 1
-    v = Fraction(q) * ulp
-    if v >= Fraction(2) ** 128:
-        return F32(s * np.inf)
-    return F32(s * float(v))              # exactly representable: float() is exact
-
-
-def _finite(*xs):
-    return all(np.isfinite(x) for x in xs)
-
-
-def _neg0(*signs):
-    """An exact zero sum is -0 only when every addend is a zero of negative sign (round to nearest)."""
-    return F32(-0.0) if all(signs) else F32(0.0)
-
-
-def add32(a, b):
-    """rn32(a + b) for fp32 a, b, with IEEE rules for inf / NaN and the sign of zero."""
-    if not _finite(a, b):
-        with np.errstate(invalid="ignore"):
-            return F32(np.float64(a) + np.float64(b))      # inf +- finite, inf - inf = NaN, NaN: as IEEE
-    s = Fraction(float(a)) + Fraction(float(b))
-    if s == 0:
-        return _neg0(np.signbit(a), np.signbit(b)) if a == 0 and b == 0 else F32(0.0)
-    return rn32(s)
-
-
-def mul32(a, b):
-    if not _finite(a, b):
-        with np.errstate(invalid="ignore"):
-            return F32(np.float64(a) * np.float64(b))
-    s = Fraction(float(a)) * Fraction(float(b))
-    if s == 0:
-        return F32(-0.0) if np.signbit(a) != np.signbit(b) else F32(0.0)
-    return rn32(s)
-
-
-def fma32(a, b, c):
-    """rn32(a*b + c), one rounding.  float64 a*b of fp32 operands is exact, so the special cases follow IEEE."""
-    if not _finite(a, b, c):
-        with np.errstate(invalid="ignore"):
-            return F32(np.float64(a) * np.float64(b) + np.float64(c))
-    p = Fraction(float(a)) * Fraction(float(b))
-    s = p + Fraction(float(c))
-    if s == 0:
-        return _neg0(np.signbit(a) != np.signbit(b), np.signbit(c)) if p == 0 and c == 0 else F32(0.0)
-    return rn32(s)
-
-
-def ref(S, d):     # the reference tail: (S - d) * 0.25, two roundings
-    return mul32(add32(S, -d), F32(0.25))
-
-
-def fma(S, d):     # the contracted tail: d' = rn(-0.25 d), then one rounding of S*0.25 + d'
-    return fma32(S, F32(0.25), mul32(d, F32(-0.25)))
 
 
 def _bits(x):

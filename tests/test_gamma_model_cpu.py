@@ -22,67 +22,11 @@ import pytest
 import display_model as M
 import gamma_model as G
 from conftest import golden
-from display_harness import BACK_RGB, BACKGROUNDS, FXCFG, golden_dither, nonfinite_dye, seeded_dye
+from display_harness import BACK_RGB, BACKGROUNDS, CASES
 from oracle import oracle as O
 
 F32 = np.float32
 ALL3 = M.ALL3
-BLOOM_SETS = [M.BLOOM, M.SHADING | M.BLOOM, M.BLOOM | M.SUNRAYS, ALL3]
-# dim dye (seeded_dye(scale=1) * 0.25) with bloom this faint puts bk on both sides of linearToGamma's knee
-# (fmaxf(1.055 p - 0.055, 0) = 0 below bk = 8.3e-4): about 10 % of values at 0, 10 % between 0 and the knee
-DIM_CFG = dict(FXCFG, BLOOM_INTENSITY=0.005, BLOOM_THRESHOLD=0.0)
-
-
-def wide_dither(seed, shape=(64, 64)):
-    """Dithering values 2^-1 .. 2^60 (random exponent and mantissa)."""
-    rng = np.random.default_rng(seed)
-    e = rng.integers(-1, 60, shape + (3,))
-    return (np.ldexp(1.0 + rng.random(shape + (3,)), e) / 2).clip(0.5, 2.0 ** 60).astype(F32)
-
-
-def overflow_dither(seed, shape=(64, 64)):
-    """The golden dithering texture with a third of its texels above FLT_MAX / 2 in magnitude, of either
-    sign: noise = d * 2 - 1 is +-inf there, and so is bk."""
-    d = golden_dither().copy()
-    rng = np.random.default_rng(seed)
-    m = rng.random(shape) < 1 / 3
-    big = F32(2.0 ** 127) * (1 + rng.random((int(m.sum()), 3)).astype(F32) * F32(0.99))
-    d[m] = np.where(rng.random((int(m.sum()), 1)) < 0.5, big, -big).astype(F32)
-    return d
-
-
-def case(dye, w, h, dither, cfg=FXCFG):
-    return dict(dye=np.ascontiguousarray(dye, F32), w=w, h=h, dither=np.ascontiguousarray(dither, F32), cfg=dict(cfg))
-
-
-def golden_case(name):
-    g = golden(name)
-    return case(g["in_dye"], int(g["w"]), int(g["h"]), g["dither"].astype(F32),
-                dict(BLOOM_RESOLUTION=int(g["bloom_res"]), SUNRAYS_RESOLUTION=int(g["sun_res"])))
-
-
-def make_cases():
-    """The inputs, by name: (dye, target w x h, dithering texture, post-FX keys)."""
-    s = seeded_dye(64, 64, 192)
-    rng = np.random.default_rng(5)
-    return {
-        "postfx_64_to_128": golden_case("postfx_64_to_128"),
-        "postfx_48x32_to_50x75": golden_case("postfx_48x32_to_50x75"),
-        "keywords_transparent_64x32_to_128x64": golden_case("keywords_transparent_64x32_to_128x64"),
-        "seeded": case(s, 128, 128, golden_dither()),
-        "zero": case(np.zeros((64, 64, 4), F32), 128, 128, golden_dither()),
-        "dim": case(seeded_dye(64, 64, 192, scale=1.0) * F32(0.25), 128, 128, golden_dither(), DIM_CFG),
-        "wide_dither": case(s, 128, 128, wide_dither(3)),
-        "overflow_dither": case(s, 128, 128, overflow_dither(4)),
-        "dither_37x23": case(s, 128, 128, rng.random((23, 37, 3), dtype=F32)),
-        "dither_1x1": case(s, 128, 128, np.full((1, 1, 3), 0.6, F32)),
-        "nonfinite": case(nonfinite_dye(64, 64, 8), 128, 128, golden_dither()),
-    }
-
-
-CASES = make_cases()
-
-
 def oracle_frame(O, c, background):
     return O.render_postfx(c["dye"], c["w"], c["h"], c["dither"], cfg=c["cfg"], back_rgb=BACK_RGB,
                            background=background, aspect=c["w"] / c["h"])

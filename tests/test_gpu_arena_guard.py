@@ -13,8 +13,6 @@ __cuda_array_interface__ alias, and nothing outside arena_model.may_change may m
 comes from fluid_device_ptr before and after.  The outputs must equal the oracle (splats: inside the
 splat_model interval; frames: the display models) and be bit-identical between the two poisons.  The
 size-selected kernels are pinned with fluid_stat where a counter tells them apart."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
@@ -23,151 +21,14 @@ import display_harness as DH
 import display_model as DM
 import splat_model as SM
 from conftest import bits_equal
-from test_gpu_fast_paths import same_or_both_nan
-from test_gpu_jacobi_range import near_max_patch
-from test_gpu_parity import STREAM_SHAPES, make, rand_fields
-from test_gpu_splats import nasty_records
-from webgl_fluid_simulation_b200 import slab
+from sim_harness import (POISONS, STREAM_SHAPES, Arena, check, delta, jacobi_plan, make, nasty_records, near_max_patch,
+                         pressure_swaps, rand_fields, same_bits)
+from sim_harness import pkg, torch  # noqa: F401 -- fixtures
 
 pytestmark = pytest.mark.gpu
 DT = 0.016666
-POISONS = (0xFF, 0x3C)
 FIELDS = ("velocity", "dye", "pressure", "divergence", "curl")
 FLUID_ERR_NOMEM = -6
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    import webgl_fluid_simulation_b200 as p
-    return p
-
-
-@pytest.fixture(scope="module")
-def torch():
-    import torch as t
-    assert t.cuda.is_available()
-    return t
-
-
-def address_range(ptr):
-    """cuMemGetAddressRange: (base, size) of the allocation holding device address `ptr`."""
-    cuda = C.CDLL("libcuda.so.1")
-    base, size = C.c_uint64(), C.c_size_t()
-    rc = cuda.cuMemGetAddressRange_v2(C.byref(base), C.byref(size), C.c_uint64(ptr))
-    assert rc == 0, rc
-    return base.value, size.value
-
-
-class _DeviceBytes:
-    def __init__(self, ptr, n):
-        self.__cuda_array_interface__ = {"shape": (n,), "typestr": "|u1", "data": (ptr, False), "version": 2}
-
-
-class Arena:
-    """A handle's arena as a uint8 torch tensor, and the guarded call."""
-
-    def __init__(self, torch, s, half=False):
-        self.torch, self.s, self.half = torch, s, half
-        self.attach()
-
-    def attach(self):
-        """(Re)reads the layout from the handle's sizes: after creation and after fluid_resize."""
-        s = self.s
-        (W, H), (Wd, Hd) = s._dims("velocity")[:2], s._dims("dye")[:2]
-        self.L = L = A.layout(W, H, Wd, Hd, self.half)
-        s.sync()
-        self.base, size = address_range(s.device_ptr("velocity"))
-        assert size >= L.bytes, (size, L.bytes)
-        par = self.parity()
-        assert self.base == s.device_ptr("velocity") - L.v[par["velocity"]]
-        self.t = self.torch.as_tensor(_DeviceBytes(self.base, L.bytes), device="cuda")
-
-    def parity(self):
-        """The slot each pair's .read is in, from fluid_device_ptr; every .read pointer must sit at a slot."""
-        L, par = self.L, {}
-        for f in A.PAIRS:
-            off = self.s.device_ptr(f) - self.base
-            assert off in (L.slot(f, 0), L.slot(f, 1)), (f, off)
-            par[f] = int(off == L.slot(f, 1))
-        for f in ("divergence", "curl"):
-            assert self.s.device_ptr(f) - self.base == L.slot(f), f
-        return par
-
-    def poison(self, inputs, value):
-        """Every byte but the .read extents of `inputs` set to `value`; returns the parity."""
-        par = self.parity()
-        self.s.sync()
-        keep = [A.extent_range(self.L, f + ".read" if f in A.PAIRS else f, par) for f in inputs]
-        saved = [self.t[lo:hi].clone() for lo, hi in keep]
-        self.t.fill_(value)
-        for (lo, hi), x in zip(keep, saved):
-            self.t[lo:hi] = x
-        return par
-
-    def image(self):
-        self.s.sync()
-        return self.t.cpu().numpy()
-
-    def run(self, call, fn, inputs, value, field=None, swaps=None):
-        """Poison, snapshot, fn(), snapshot: nothing outside may_change(call) moved.  swaps: the pairs whose
-        .read must have changed slot (None: not checked).  Returns fn()'s result."""
-        torch, L = self.torch, self.L
-        par = self.poison(inputs, value)
-        before = self.t.clone()
-        torch.cuda.synchronize()
-        out = fn()
-        self.s.sync()
-        after = self.parity()
-        if swaps is not None:
-            assert after == {f: par[f] ^ (f in swaps) for f in A.PAIRS}, (call, par, after)
-        moved = before != self.t
-        for lo, hi in A.may_change(call, L, par, field):
-            moved[lo:hi] = False
-        n = int(moved.sum())
-        offs = moved.nonzero()[:8, 0].cpu().numpy() if n else []
-        del before, moved
-        torch.cuda.synchronize()
-        assert n == 0, (call, hex(value), n, A.report(L, offs))
-        return out
-
-
-def check(g, call, fn, inputs, expect, field=None, swaps=None, cmp=bits_equal):
-    """g.run under both poisons, inputs written fresh before each; every field of `expect` read back equals
-    it (or satisfies it, when callable) and is bit-identical between the two runs."""
-    runs = []
-    for value in POISONS:
-        for n, a in inputs.items():
-            g.s.writeField(n, a)
-        torch = g.torch
-        torch.cuda.synchronize()
-        g.run(call, fn, tuple(inputs), value, field, swaps)
-        got = {n: g.s.readField(n) for n in expect}
-        for n, want in expect.items():
-            assert want(got[n]) if callable(want) else cmp(got[n], want), (call, n, hex(value))
-        runs.append(got)
-    for n in expect:
-        assert bits_equal(runs[0][n], runs[1][n]), (call, n)
-
-
-def delta(s, stat, fn):
-    n0 = s.stat(stat)
-    fn()
-    return s.stat(stat) - n0
-
-
-def jacobi_plan(W, H, half, iters, jb=0, naive=False):
-    """Depths of the Jacobi launches of a device solve (fluid.cu run_jacobi): JacobiPlan's balanced split
-    (slab.jacobi_launches) when the blocked kernel runs (tb_eligible, not FLAG_NAIVE_JACOBI, depth != 1),
-    otherwise one sweep per launch."""
-    kb = min(jb if jb > 0 else slab.KMAX, slab.KMAX)
-    if not half and W % 4 == 0 and W >= 16 and H >= 2 and not naive and kb != 1:
-        return slab.jacobi_launches(iters, kb)
-    return [1] * iters
-
-
-def pressure_swaps(n):
-    """The pressure pair after n swaps: .read changed slot iff n is odd."""
-    return ("pressure",) if n % 2 else ()
 
 
 def every_pass(pkg, torch, O, W, H, Wd, Hd, half, jacobi_iters=(1, 13)):
@@ -327,7 +188,7 @@ def test_blocked_jacobi_exact_streams(pkg, torch, oracle, case):
     else:
         near_max_patch(p, d, 300, 340, 400, 440, 0.8)
     with np.errstate(over="ignore", invalid="ignore"):
-        s = solve_case(pkg, torch, oracle, W, H, [(0, 20, [10, 10])], p, d, cmp=same_or_both_nan)
+        s = solve_case(pkg, torch, oracle, W, H, [(0, 20, [10, 10])], p, d, cmp=same_bits)
     assert s.stat("jacobi_exact_streams") > 0                  # counted since the handle was created
     s.close()
 

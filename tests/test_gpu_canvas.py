@@ -9,9 +9,11 @@ import pytest
 
 import arena_model as A
 import canvas_model as CM
-from display_harness import BACK, BACK_RGB, flags_of, golden_dither, make, set_keywords
+from display_harness import BACK, BACK_RGB, flags_of, make, set_keywords
+from display_harness import dither  # noqa: F401 -- a fixture
 from display_model import ALL3, BLOOM, SHADING, SUNRAYS
-from test_gpu_arena_guard import POISONS, Arena
+from sim_harness import POISONS, SLEEP_CYCLES, V3, Arena
+from sim_harness import pkg, torch  # noqa: F401 -- fixtures
 
 pytestmark = pytest.mark.gpu
 F = np.float32
@@ -19,24 +21,6 @@ F = np.float32
 # where the canvas samples the dye at its texel centres, so planted texels reach the fragment unchanged
 GEOMETRIES = [(64, 64, 128, 128, False), (48, 32, 807, 640, False), (64, 64, 64, 64, True)]
 KINDS = {"fp32": "fp32", "half": "half_half_postfx", "nearest": "nearest_fp32"}
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    import webgl_fluid_simulation_b200 as p
-    return p
-
-
-@pytest.fixture(scope="module")
-def torch():
-    import torch as t
-    assert t.cuda.is_available()
-    return t
-
-
-@pytest.fixture(scope="module")
-def dither():
-    return golden_dither()
 
 
 def mode_flags(pkg, mode):
@@ -131,16 +115,6 @@ def test_host_and_device_destinations_agree(pkg, torch, dither, mode):
             s.render_canvas(out=img)
             assert np.array_equal(img.cpu().numpy(), host), (kw, transparent)
     s.close()
-
-
-SLEEP_CYCLES = 200_000_000                               # about 0.1 s of torch.cuda._sleep at 1.98 GHz
-
-
-class V3:
-    """A version-3 __cuda_array_interface__ of tensor `t` naming `stream` as its producer."""
-
-    def __init__(self, t, stream):
-        self.__cuda_array_interface__ = dict(t.__cuda_array_interface__, version=3, stream=stream.cuda_stream or 1)
 
 
 def test_device_destination_waits_for_pending_torch_work(pkg, torch, dither):

@@ -9,21 +9,12 @@ import pytest
 import capture_model as CM
 import display_model as M
 from conftest import bits_equal, golden
-from display_harness import BACK_RGB, check_capture, golden_dither, make, model_capture, seeded_dye, set_keywords
+from display_harness import BACK_RGB, check_capture, make, model_capture, seeded_dye, set_keywords
+from display_harness import dither  # noqa: F401 -- a fixture
+from sim_harness import pkg  # noqa: F401 -- a fixture
 
 pytestmark = pytest.mark.gpu
 GEOMETRIES = ["capture_64_canvas_128", "capture_48x32_canvas_807x640"]
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    import webgl_fluid_simulation_b200 as p
-    return p
-
-
-@pytest.fixture(scope="module")
-def dither():
-    return golden_dither()
 
 
 def outside_executed(got, half, delta):

@@ -11,11 +11,9 @@ import pytest
 
 import display_harness as DH
 from conftest import bits_equal
-from test_gpu_arena_guard import POISONS, Arena
-from test_gpu_canvas import SLEEP_CYCLES, V3
-from test_gpu_parity import make
-from test_gpu_resize import special
-from test_gpu_tiny_guard import ITERS, JB, blocked, cases, expected
+from jacobi_tb_model import ITERS, JB, blocked, cases, expected
+from sim_harness import POISONS, SLEEP_CYCLES, V3, Arena, make, special_values
+from sim_harness import pkg, torch  # noqa: F401 -- fixtures
 
 pytestmark = pytest.mark.gpu
 F = np.float32
@@ -24,19 +22,6 @@ FIELDS = ("velocity", "dye", "pressure", "divergence", "curl")
 SIZES = [(128, 128, 1024, 1024), (1024, 1024, 2048, 2048), (36, 20, 54, 30), (1, 9, 3, 27), (9, 1, 27, 3)]
 KINDS = ["fp32", "half", "desktop", "nearest"]
 INVALID = -1
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    import webgl_fluid_simulation_b200 as p
-    return p
-
-
-@pytest.fixture(scope="module")
-def torch():
-    import torch as t
-    assert t.cuda.is_available()
-    return t
 
 
 def flags_of(pkg, kind):
@@ -67,25 +52,6 @@ def seeded(pkg, s, seed, steps=2):
     s.multipleSplats(3)
     for _ in range(steps):
         s.step(DT)
-
-
-def special_values(shape, seed, half):
-    """Seeded values with a quarter replaced by +-0, fp32 and fp16 subnormals, +-inf and NaN (test_gpu_resize);
-    for half storage also values that overflow fp16 or sit exactly between two fp16 values."""
-    rng = np.random.default_rng(seed)
-    a = special((rng.standard_normal(shape) * 50).astype(F), rng)
-    if half:
-        flat = a.reshape(-1)
-        extra = np.array([65520.0, -65520.0, 1e5, -7e4, 65504.0, 65519.0, 1.0 + 2.0 ** -11, 1.0 + 3 * 2.0 ** -11,
-                          -(2.0 ** -24) * 1.5, 2.0 ** -25], F)
-        k = min(flat.size, 3 * extra.size)
-        flat[rng.choice(flat.size, k, replace=False)] = np.resize(extra, k)
-    flat = a.reshape(-1)                        # a field of a few cells: NaN and inf all the same
-    if not np.isnan(flat).any():
-        flat[0] = np.nan
-    if not np.isinf(flat).any():
-        flat[-1] = -np.inf
-    return a
 
 
 # ---- 1. and 2.: the same bits as fluid_read / fluid_write --------------------------------------------------
@@ -185,7 +151,7 @@ def test_session_twin(pkg, torch, kind, start):
 @pytest.mark.parametrize("jb", JB)
 @pytest.mark.parametrize("W,H", [(1024, 512), (1000, 520), (1000, 37), (16900, 3)])
 def test_device_written_divergence_flags_every_placed_cell(pkg, torch, oracle, W, H, jb):
-    """Divergence written from device memory with the tiny-value placements of test_gpu_tiny_guard: the solve
+    """Divergence written from device memory with the tiny-value placements of jacobi_tb_model: the solve
     equals the fluid_write twin's and the oracle bit for bit, and the blocked kernel ran the same number of
     exact-tail streams on both (none where the blocked kernel does not run)."""
     a = make(pkg, W, H, 8, 8, jb=jb, PRESSURE_ITERATIONS=ITERS)

@@ -7,20 +7,11 @@ import numpy as np
 import pytest
 
 from conftest import bits_equal, golden, max_rel
-from display_harness import BACK_RGB, FXCFG, check_frame, golden_dither, make, model_frame, seeded_dye, set_keywords
+from display_harness import BACK_RGB, FXCFG, check_frame, make, model_frame, seeded_dye, set_keywords
+from display_harness import dither  # noqa: F401 -- a fixture
+from sim_harness import pkg  # noqa: F401 -- a fixture
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    import webgl_fluid_simulation_b200 as p
-    return p
-
-
-@pytest.fixture(scope="module")
-def dither():
-    return golden_dither()
 
 
 @pytest.mark.parametrize("Wd,Hd,w,h", [(64, 64, 128, 128), (48, 32, 50, 75)])

@@ -12,9 +12,9 @@ import numpy as np
 import pytest
 
 from conftest import bits_equal
-from test_gpu_fast_paths import same_or_both_nan
-from test_gpu_jacobi_range import handle, solve
-from test_jacobi_tb_model import special_fields
+from jacobi_tb_model import special_fields
+from sim_harness import make, same_bits, solve
+from sim_harness import pkg  # noqa: F401 -- a fixture
 
 pytestmark = pytest.mark.gpu
 WIDTHS = (104, 108, 112, 120, 128, 132, 208, 1000, 1040, 4096)
@@ -22,12 +22,6 @@ HEIGHTS = (40, 300)                 # one chunk of rows per window; several
 # (jacobi_block, sweeps): K and 3K - 1 sweeps at depths 5, 9, 13 and the default; one sweep alone is a depth-1
 # launch (a handle asked for jacobi_block = 1 does not run the blocked kernel at all)
 PLANS = [(5, 5), (5, 14), (9, 9), (9, 26), (13, 13), (13, 38), (13, 1), (0, 13), (0, 38)]
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    import webgl_fluid_simulation_b200 as p
-    return p
 
 
 def fields(kind, W, H, seed):
@@ -44,7 +38,7 @@ def fields(kind, W, H, seed):
 @pytest.mark.parametrize("H", HEIGHTS)
 @pytest.mark.parametrize("W", WIDTHS)
 def test_blocked_equals_one_sweep_per_launch(pkg, W, H):
-    blocked, naive = handle(pkg, W, H), handle(pkg, W, H, pkg.FLAG_NAIVE_JACOBI, 1)
+    blocked, naive = make(pkg, W, H, 8, 8), make(pkg, W, H, 8, 8, pkg.FLAG_NAIVE_JACOBI, 1)
     for n, (jb, iters) in enumerate(PLANS):
         for kind in ("random", "spikes"):
             p, d = fields(kind, W, H, 7 * W + H + n)
@@ -61,11 +55,11 @@ def test_blocked_equals_one_sweep_per_launch(pkg, W, H):
 
 @pytest.mark.parametrize("W,H", [(104, 40), (132, 300), (1040, 300), (4096, 96)])
 def test_nonfinite_inputs(pkg, W, H):
-    blocked, naive = handle(pkg, W, H), handle(pkg, W, H, pkg.FLAG_NAIVE_JACOBI, 1)
+    blocked, naive = make(pkg, W, H, 8, 8), make(pkg, W, H, 8, 8, pkg.FLAG_NAIVE_JACOBI, 1)
     for jb, iters in ((13, 13), (9, 9), (5, 14), (0, 38)):
         p, d = special_fields("nonfinite", W, H, W + H + jb)
         for pressure in (0.8, None):
-            assert same_or_both_nan(solve(blocked, p, d, iters, pressure, jb), solve(naive, p, d, iters, pressure))
+            assert same_bits(solve(blocked, p, d, iters, pressure, jb), solve(naive, p, d, iters, pressure))
     blocked.close(); naive.close()
 
 
@@ -76,7 +70,7 @@ def test_a_huge_edge_column_sends_its_window_through_the_exact_tail(pkg, W, H):
     reference at column 127 - HX while fma(S, 0.25, -0.25 d) stays finite, and that cell reaches window 0's
     last valid column.  No other input of window 0 reaches 2^122: only folding the edge column into the
     stream's largest magnitude sends it through the exact tail."""
-    blocked, naive = handle(pkg, W, H), handle(pkg, W, H, pkg.FLAG_NAIVE_JACOBI, 1)
+    blocked, naive = make(pkg, W, H, 8, 8), make(pkg, W, H, 8, 8, pkg.FLAG_NAIVE_JACOBI, 1)
     for jb, iters, hx in ((13, 13, 12), (9, 9, 8), (5, 5, 4), (0, 38, 12)):
         p, d = fields("random", W, H, W + jb)
         col = 128 - hx
@@ -84,14 +78,14 @@ def test_a_huge_edge_column_sends_its_window_through_the_exact_tail(pkg, W, H):
         e0 = blocked.stat("jacobi_exact_streams")
         got, ref = solve(blocked, p, d, iters, None, jb), solve(naive, p, d, iters, None)
         assert np.isinf(ref[:, col - 1 - hx]).any() or np.isnan(ref[:, col - 1 - hx]).any()
-        assert same_or_both_nan(got, ref), (W, H, jb)
+        assert same_bits(got, ref), (W, H, jb)
         assert blocked.stat("jacobi_exact_streams") > e0
     blocked.close(); naive.close()
 
 
 @pytest.mark.parametrize("W,H", [(208, 300), (1000, 96)])
 def test_tiny_divergence_runs_exact_streams(pkg, W, H):
-    blocked, naive = handle(pkg, W, H), handle(pkg, W, H, pkg.FLAG_NAIVE_JACOBI, 1)
+    blocked, naive = make(pkg, W, H, 8, 8), make(pkg, W, H, 8, 8, pkg.FLAG_NAIVE_JACOBI, 1)
     for jb, iters in ((13, 13), (9, 26), (5, 5), (13, 1)):
         p, d = fields("spikes", W, H, W + jb)
         d[H // 2, ::7] = np.float32(2.0 ** -130)
@@ -106,7 +100,7 @@ def test_tiny_divergence_runs_exact_streams(pkg, W, H):
 def test_banded_host_solve_equals_the_resident_solve(pkg, jb, launches):
     W, H, iters = 4096, 512, 50
     p, d = fields("spikes", W, H, 99)
-    s = handle(pkg, W, H, jb=jb); s.config["PRESSURE_ITERATIONS"] = iters
+    s = make(pkg, W, H, 8, 8, jb=jb); s.config["PRESSURE_ITERATIONS"] = iters
     want = solve(s, p, d, iters, 0.8)
     n0 = s.stat("jacobi_launches")
     ph = p.copy()

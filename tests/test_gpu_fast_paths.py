@@ -16,59 +16,13 @@ import numpy as np
 import pytest
 
 from conftest import bits_equal
-from test_gpu_parity import STREAM_SHAPES, make
-from test_gpu_splats import nasty_fields
+from sim_harness import STREAM_SHAPES, exp_tiled, far_field, make, nasty_fields, same_bits
+from sim_harness import pkg  # noqa: F401 -- a fixture
 
 DT = 0.016666
 FIELDS = ("velocity", "dye", "pressure", "divergence", "curl")
 TILED = [(520, 33), (130, 66)]            # too few warps / W % 4 != 0: the tiled kernels
 DATA = ["exp_tiled", "far_field", "special"]
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    import webgl_fluid_simulation_b200 as p
-    return p
-
-
-def same_or_both_nan(a, b):
-    """NaN in the same places, every other element bitwise."""
-    a = np.ascontiguousarray(a, np.float32); b = np.ascontiguousarray(b, np.float32)
-    if a.shape != b.shape:
-        return False
-    na, nb = np.isnan(a), np.isnan(b)
-    return np.array_equal(na, nb) and np.array_equal(a[~na].view(np.uint32), b[~nb].view(np.uint32))
-
-
-def exp_tiled(shape, seed, lo=-149, hi=100, tile=(16, 128), zeros=0.03):
-    """Random signs and mantissas, one binary exponent in [lo, hi] per tile of (rows, columns) --
-    a 128x16 tile is a warp's window of the streaming kernels -- plus exact +-0 cells.  Exponents near
-    -149 give subnormals."""
-    rng = np.random.default_rng(seed)
-    H, W = shape[:2]
-    e = rng.integers(lo, hi + 1, (-(-H // tile[0]), -(-W // tile[1])))
-    e = np.repeat(np.repeat(e, tile[0], 0), tile[1], 1)[:H, :W]
-    e = e.reshape(e.shape + (1,) * (len(shape) - 2))
-    m = rng.uniform(1.0, 2.0, shape) * rng.choice([-1.0, 1.0], shape)
-    a = np.ldexp(m, e).astype(np.float32)
-    z = rng.random(shape) < zeros
-    a[z] = np.where(rng.random(int(z.sum())) < 0.5, np.float32(0.0), np.float32(-0.0))
-    return a
-
-
-def far_field(O, W, H, C, seed):
-    """Gaussian splats on a zero field (dye: alpha 1): the far field underflows gradually through the
-    subnormal range to exact zeros."""
-    rng = np.random.default_rng(seed)
-    f = np.zeros((H, W, C), np.float32)
-    if C == 4:
-        f[..., 3] = 1.0
-    rad = O.correct_radius(0.25, W / H)
-    for _ in range(2):
-        x, y = rng.uniform(0.2, 0.8, 2)
-        col = rng.uniform(-400, 400, 3) if C == 2 else rng.uniform(0.2, 1.5, 3)
-        f = O.splat(f, W / H, float(x), float(y), tuple(float(c) for c in col), rad)
-    return f
 
 
 def stencil_fields(O, W, H, data, seed):
@@ -132,7 +86,7 @@ def test_cvd_and_gradient_fast_arithmetic_vs_oracle(pkg, oracle, W, H, data):
     """curl-vorticity-divergence then gradientSubtract, per pass, against the oracle."""
     O = oracle
     v, p = stencil_fields(O, W, H, data, W * 3 + H)
-    cmp = same_or_both_nan if data == "special" else bits_equal
+    cmp = same_bits if data == "special" else bits_equal
     s = make(pkg, W, H, W, H)
     s.writeField("velocity", v); s.writeField("pressure", p)
     c0, g0 = s.stat("cvd_stream_launches"), s.stat("gradient_stream_launches")
@@ -229,7 +183,7 @@ def test_advection_far_outside_the_grid_vs_oracle(pkg, oracle, W, H, Wd, Hd, dat
         # oracle's manual bilerp adds neighbour * 0 terms -- the same value unless a neighbour is inf / NaN
         v, dye, _ = nasty_fields(W, H, Wd, Hd, W + Hd)
         v[~np.isfinite(v)] = np.float32(-0.0)
-        cmp = same_or_both_nan
+        cmp = same_bits
     s = make(pkg, W, H, Wd, Hd)
     for diss in (0.0, 0.2, 1.0, 4.0):
         s.config["VELOCITY_DISSIPATION"] = diss; s.config["DENSITY_DISSIPATION"] = diss

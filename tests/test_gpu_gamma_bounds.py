@@ -4,7 +4,7 @@ arithmetic of the display shader with a powf inside POWF_ULP of float64 pow.  Th
 built from the model's bloom FBO and sunrays texture (the oracle's blits), after checking the GPU's against
 them bit for bit (NaN in the same places).
 
-Inputs are those of test_gamma_model_cpu.py (goldens, seeded, zero and dim dye, dithering of other
+Inputs are display_harness.CASES, those of test_gamma_model_cpu.py (goldens, seeded, zero and dim dye, dithering of other
 shapes, of a wide range and overflowing, non-finite dye) plus one frame at the reference's sizes; the
 non-finite dye goes through all eight keyword sets, on fp32 and half-storage handles.  A readout of the
 device powf itself closes the file."""
@@ -16,18 +16,15 @@ import display_model as M
 import gamma_model as G
 from conftest import golden
 from display_harness import BACK_RGB, BACKGROUNDS, MODES, golden_dither, make, nonfinite_dye, seeded_dye, set_keywords
-from test_gamma_model_cpu import ALL3, BLOOM_SETS, CASES, DIM_CFG, FXCFG
+from display_harness import CASES, DIM_CFG, FXCFG
+from display_model import ALL3
+from sim_harness import pkg  # noqa: F401 -- a fixture
 
 pytestmark = pytest.mark.gpu
 F32 = np.float32
+BLOOM_SETS = [M.BLOOM, M.SHADING | M.BLOOM, M.BLOOM | M.SUNRAYS, ALL3]
 NO_BLOOM_SETS = [0, M.SHADING, M.SUNRAYS, M.SHADING | M.SUNRAYS]
 HALF = 0x10
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    import webgl_fluid_simulation_b200 as p
-    return p
 
 
 def draw_and_check(pkg, c, sets=BLOOM_SETS):

@@ -14,18 +14,13 @@ from conftest import golden, max_rel
 from display_harness import (FXCFG, check_capture, check_frame, draw_all, flags_of, golden_dither, make, model_capture,
                              model_frame, nonfinite_dye, seeded_dye, set_keywords, stored)
 from oracle import oracle as O
-from test_half_postfx_cpu import CAPTURE_SETS, FRAME_TOL, POW2, RAGGED, RAGGED_CHAIN_TEXELS, cfg_of, fp16_ulps
+from sim_harness import pkg  # noqa: F401 -- a fixture
+from gamma_model import CAPTURE_SETS, FRAME_TOL, POW2, RAGGED, RAGGED_CHAIN_TEXELS, cfg_of, fp16_ulps
 
 pytestmark = pytest.mark.gpu
 F32 = np.float32
 ALL3 = M.ALL3
 HANDLES = ["fp32", "half"]
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    import webgl_fluid_simulation_b200 as p
-    return p
 
 
 def kind(handle):

@@ -6,30 +6,12 @@ fp16 when they are stored.  NaN-aware comparison: NaN in the same places, every 
 import numpy as np
 import pytest
 
-from test_gpu_fast_paths import same_or_both_nan
-from test_gpu_parity import make
-from test_gpu_splats import nasty_fields
+from sim_harness import make, same_bits, special_fields
+from sim_harness import pkg  # noqa: F401 -- a fixture
 
 pytestmark = pytest.mark.gpu
 DT = 0.016666
 SHAPES = [(64, 48, 128, 96), (128, 128, 256, 256), (100, 60, 150, 90)]
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    import webgl_fluid_simulation_b200 as p
-    return p
-
-
-def special_fields(O, W, H, Wd, Hd, seed):
-    """nasty_fields rounded to fp16, with a band of +-6e4 pressure whose sign flips every two cells in
-    x and y: the cells two apart across a flip differ by 1.2e5."""
-    v, dye, p = nasty_fields(W, H, Wd, Hd, seed)
-    s = lambda n: np.where((np.arange(n) // 2) % 2 == 0, 1.0, -1.0).astype(np.float32)
-    big = np.float32(6e4) * s(H)[:, None] * s(W)[None, :]
-    band = slice(H // 4, max(H // 2, H // 4 + 4))
-    p[band] = big[band]
-    return tuple(O.round_half(a) for a in (v, dye, p))
 
 
 @pytest.mark.parametrize("W,H,Wd,Hd", SHAPES)
@@ -42,24 +24,24 @@ def test_half_storage_special_values_every_pass_vs_oracle(pkg, oracle, W, H, Wd,
     v, dye, p = special_fields(O, W, H, Wd, Hd, W + H)
     s = make(pkg, W, H, Wd, Hd, flags=pkg.FLAG_HALF_STORAGE)
     s.writeField("velocity", v); s.writeField("dye", dye); s.writeField("pressure", p)
-    assert same_or_both_nan(s.readField("velocity"), v)
-    s.pass_("curl"); c = s.readField("curl"); assert same_or_both_nan(c, R(O.curl(v)))
+    assert same_bits(s.readField("velocity"), v)
+    s.pass_("curl"); c = s.readField("curl"); assert same_bits(c, R(O.curl(v)))
     s.pass_("vorticity", DT); v2 = s.readField("velocity")
-    assert same_or_both_nan(v2, R(O.vorticity(v, c, 30.0, DT)))
-    s.pass_("divergence"); d = s.readField("divergence"); assert same_or_both_nan(d, R(O.divergence(v2)))
-    s.pass_("clear_pressure"); p1 = s.readField("pressure"); assert same_or_both_nan(p1, R(O.clear(p, 0.8)))
+    assert same_bits(v2, R(O.vorticity(v, c, 30.0, DT)))
+    s.pass_("divergence"); d = s.readField("divergence"); assert same_bits(d, R(O.divergence(v2)))
+    s.pass_("clear_pressure"); p1 = s.readField("pressure"); assert same_bits(p1, R(O.clear(p, 0.8)))
     s.pass_("jacobi", 5); p2 = p1
     for _ in range(5):
         p2 = R(O.jacobi(p2, d, 1))
-    assert same_or_both_nan(s.readField("pressure"), p2)
+    assert same_bits(s.readField("pressure"), p2)
     s.writeField("pressure", p)
     s.pass_("gradient_subtract"); v3 = s.readField("velocity")
     ref_v3 = R(O.gradient_subtract(p, v2))
-    assert same_or_both_nan(v3, ref_v3)
+    assert same_bits(v3, ref_v3)
     assert np.isinf(ref_v3[H // 4:H // 2]).any()                     # the premise: stores that overflow fp16
     s.pass_("advect_velocity", DT); v4 = s.readField("velocity")
-    assert same_or_both_nan(v4, R(O.advect(v3, v3, DT, 0.2)))
-    s.pass_("advect_dye", DT); assert same_or_both_nan(s.readField("dye"), R(O.advect(v4, dye, DT, 1.0)))
+    assert same_bits(v4, R(O.advect(v3, v3, DT, 0.2)))
+    s.pass_("advect_dye", DT); assert same_bits(s.readField("dye"), R(O.advect(v4, dye, DT, 1.0)))
     s.close()
 
 
@@ -74,5 +56,5 @@ def test_half_storage_special_values_whole_step_vs_oracle(pkg, oracle, W, H, Wd,
     ref.velocity, ref.dye, ref.pressure = v.copy(), dye.copy(), p.copy()
     s.step(DT); ref.step(DT)
     for n in ("velocity", "dye", "pressure", "divergence", "curl"):
-        assert same_or_both_nan(s.readField(n), getattr(ref, n)), n
+        assert same_bits(s.readField(n), getattr(ref, n)), n
     s.close()

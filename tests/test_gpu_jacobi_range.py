@@ -3,7 +3,7 @@
 Its contracted tail fma(S, 0.25, -0.25 d) differs from the reference's (S - d) * 0.25 where S and d are
 finite and S - d rounds to +-inf (tests/test_fma_contraction_cpu.py).  A warp stream whose level-0 inputs
 reach 2^122 therefore runs again with the exact tail (csrc/jacobi.cuh).  On the data sets of
-tests/test_jacobi_tb_model.py -- a patch of p near FLT_MAX / 4 over d = -1e37, its mirror image, divergence
+tests/jacobi_tb_model.py -- a patch of p near FLT_MAX / 4 over d = -1e37, its mirror image, divergence
 in [2^126, FLT_MAX], inf / NaN sprinkled, binary exponents -149..127 -- the blocked solve equals one sweep
 per launch and the oracle: mirrored windows and ragged widths, every depth, with and without the fused
 clear, the host solve banded and in one piece, and whole steps after such a solve.  The
@@ -12,8 +12,9 @@ import numpy as np
 import pytest
 
 from conftest import bits_equal
-from test_gpu_fast_paths import same_or_both_nan
-from test_jacobi_tb_model import KINDS, equal, overflow_sweep, special_fields
+from jacobi_tb_model import KINDS, equal, overflow_sweep, special_fields
+from sim_harness import make, near_max_patch, same_bits, solve
+from sim_harness import pkg  # noqa: F401 -- a fixture
 
 pytestmark = pytest.mark.gpu
 DT = 0.016666
@@ -25,35 +26,10 @@ SHAPES = [(4096, 96, (10, 0)), (1000, 64, tuple(range(2, 14)) + (0,)), (132, 45,
           (112, 2, tuple(range(2, 14)) + (0,))]
 
 
-@pytest.fixture(scope="module")
-def pkg():
-    import webgl_fluid_simulation_b200 as p
-    return p
-
-
-def handle(pkg, W, H, flags=0, jb=0):
-    return pkg.FluidSimulation({"SIM_RESOLUTION": min(W, H), "DYE_RESOLUTION": 8}, canvas_width=W, canvas_height=H,
-                               flags=flags, jacobi_block=jb, sizes=(W, H, 8, 8))
-
-
-def solve(s, p, d, iters, pressure, jb=None):
-    """fused clear + `iters` sweeps (pressure given) or `iters` sweeps alone (pressure None)"""
-    if jb is not None:
-        s.set_param("JACOBI_BLOCK", jb)
-    s.config["PRESSURE_ITERATIONS"] = iters
-    s.config["PRESSURE"] = 1.0 if pressure is None else pressure
-    s.writeField("pressure", p); s.writeField("divergence", d)
-    if pressure is None:
-        s.pass_("jacobi", iters)
-    else:
-        s.pass_("pressure_solve")
-    return s.readField("pressure")
-
-
 @pytest.mark.parametrize("kind", KINDS)
 @pytest.mark.parametrize("W,H,depths", SHAPES)
 def test_blocked_equals_naive_and_oracle_at_the_top_of_the_range(pkg, oracle, kind, W, H, depths):
-    blocked, naive = handle(pkg, W, H), handle(pkg, W, H, pkg.FLAG_NAIVE_JACOBI, 1)
+    blocked, naive = make(pkg, W, H, 8, 8), make(pkg, W, H, 8, 8, pkg.FLAG_NAIVE_JACOBI, 1)
     for n, jb in enumerate(depths):
         iters = 2 * jb + 1 if jb else 30
         for pressure in (PRESSURES[n % 3], None):
@@ -78,11 +54,6 @@ def test_blocked_equals_naive_and_oracle_at_the_top_of_the_range(pkg, oracle, ki
     blocked.close(); naive.close()
 
 
-def near_max_patch(p, d, r0, r1, c0, c1, pressure):
-    p[r0:r1, c0:c1] = np.float32(8.5e37 / pressure)
-    d[r0 - 1:r1 + 1, c0 - 1:c1 + 1] = np.float32(-1e37)
-
-
 @pytest.mark.parametrize("W,H,iters,jb,launches", [(1024, 2048, 50, 0, 8 * 5), (1000, 2048, 50, 13, 8 * 4),
                                                    (1000, 300, 50, 0, 4)])
 def test_host_pressure_solve_with_a_near_max_patch(pkg, oracle, W, H, iters, jb, launches):
@@ -95,14 +66,14 @@ def test_host_pressure_solve_with_a_near_max_patch(pkg, oracle, W, H, iters, jb,
     near_max_patch(p, d, r0, r1, 400, 440, 0.8)
     crop = (slice(r0 - 8, r1 + 8), slice(392, 448))
     assert overflow_sweep(oracle, p[crop], d[crop], 1, 0.8) == 1
-    s = handle(pkg, W, H, jb=jb); s.config["PRESSURE_ITERATIONS"] = iters
+    s = make(pkg, W, H, 8, 8, jb=jb); s.config["PRESSURE_ITERATIONS"] = iters
     n0, e0 = s.stat("jacobi_launches"), s.stat("jacobi_exact_streams")
     ph = p.copy()
     s.pressure_solve_host(d, ph, iters)
     assert s.stat("jacobi_launches") - n0 == launches
     assert s.stat("jacobi_exact_streams") > e0
     s.close()
-    s = handle(pkg, W, H, pkg.FLAG_NAIVE_JACOBI, 1)
+    s = make(pkg, W, H, 8, 8, pkg.FLAG_NAIVE_JACOBI, 1)
     ref = solve(s, p, d, iters, 0.8)
     s.close()
     assert np.isinf(ref).any()
@@ -131,10 +102,10 @@ def test_steps_after_a_near_max_solve_bitwise_vs_oracle(pkg, oracle, flags):
     ref.velocity, ref.dye = v.copy(), dye.copy()
     ref.pressure = O.jacobi(O.clear(p, 0.8), d, 20)
     assert np.isinf(ref.pressure).any()
-    assert same_or_both_nan(s.readField("pressure"), ref.pressure)
+    assert same_bits(s.readField("pressure"), ref.pressure)
     for _ in range(2):
         s.step(DT); ref.step(DT)
     for n in ("velocity", "dye", "pressure", "divergence", "curl"):
-        assert same_or_both_nan(s.readField(n), getattr(ref, n)), n
+        assert same_bits(s.readField(n), getattr(ref, n)), n
     assert s.stat("jacobi_exact_streams") > 0
     s.close()

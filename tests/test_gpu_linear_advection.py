@@ -12,11 +12,8 @@ import pytest
 
 import linear_advection_model as M
 from conftest import bits_equal, golden, max_rel
-from test_gpu_arena_guard import Arena, check, jacobi_plan, pressure_swaps
-from test_gpu_fast_paths import exp_tiled, same_or_both_nan
-from test_gpu_parity import make, rand_fields
-from test_gpu_splats import nasty_fields
-from test_linear_advection_cpu import P4_HALF_GATE
+from sim_harness import Arena, check, exp_tiled, jacobi_plan, make, nasty_fields, pressure_swaps, rand_fields, same_bits
+from sim_harness import pkg, torch  # noqa: F401 -- fixtures
 
 pytestmark = pytest.mark.gpu
 
@@ -25,19 +22,6 @@ FIELDS = ("velocity", "dye", "pressure", "divergence", "curl")
 ADVECT_SHAPES = [(256, 256, 256, 256, False), (128, 128, 256, 256, False), (64, 64, 128, 128, False),
                  (64, 64, 64, 64, False), (36, 20, 54, 30, False), (1, 9, 3, 27, False), (9, 1, 27, 3, False),
                  (256, 256, 256, 256, True)]
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    import webgl_fluid_simulation_b200 as p
-    return p
-
-
-@pytest.fixture(scope="module")
-def torch():
-    import torch as t
-    assert t.cuda.is_available()
-    return t
 
 
 def pow2(n):
@@ -84,10 +68,10 @@ def test_advection_passes_vs_model(pkg, oracle, W, H, Wd, Hd, tiled, half, data)
         s.pass_("advect_velocity", DT); v2 = s.readField("velocity")
         n1 = s.stat("advect4_launches")
         assert n1 - n0 == ev, diss
-        assert same_or_both_nan(v2, R(M.advect(v, v, DT, diss))), diss
+        assert same_bits(v2, R(M.advect(v, v, DT, diss))), diss
         s.pass_("advect_dye", DT)
         assert s.stat("advect4_launches") - n1 == ed, diss
-        assert same_or_both_nan(s.readField("dye"), R(M.advect(v2, dye, DT, diss))), diss
+        assert same_bits(s.readField("dye"), R(M.advect(v2, dye, DT, diss))), diss
     s.close()
 
 
@@ -169,9 +153,9 @@ def test_passes_vs_executed_linear_shaders(pkg, tag, shape):
             continue
         s.writeField("velocity", g[pre + "in_velocity"]); s.writeField("dye", g[pre + "in_dye"])
         s.pass_("advect_velocity", float(g["dt"]))
-        assert same_or_both_nan(s.readField("velocity"), g[pre + "advect_velocity"]), pre
+        assert same_bits(s.readField("velocity"), g[pre + "advect_velocity"]), pre
         s.pass_("advect_dye", float(g["dt"]))
-        assert same_or_both_nan(s.readField("dye"), g[pre + "advect_dye"]), pre
+        assert same_bits(s.readField("dye"), g[pre + "advect_dye"]), pre
     s.close()
 
 
@@ -207,7 +191,7 @@ def test_desktop_configuration(pkg, capsys):
     s.close()
     with capsys.disabled():
         print("\n[desktop configuration] 1-step max-rel vs executed shaders: " + ", ".join(f"{k}={v:.2e}" for k, v in e.items()))
-    assert max(e.values()) < P4_HALF_GATE
+    assert max(e.values()) < M.P4_HALF_GATE
 
 
 @pytest.mark.parametrize("half", [False, True], ids=["fp32", "half"])

@@ -13,17 +13,12 @@ import gamma_model as G
 from conftest import golden
 from display_harness import (BACK_RGB, BACKGROUNDS, MODES, allowed, check_capture, draw_all, flags_of, golden_dither,
                              make, model_capture, nonfinite_dye, seeded_dye, set_keywords)
+from sim_harness import pkg  # noqa: F401 -- a fixture
 
 pytestmark = pytest.mark.gpu
 F32 = np.float32
 HANDLES = ["fp32", "fp32_half_postfx", "half", "half_half_postfx"]
 ALL3 = M.ALL3
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    import webgl_fluid_simulation_b200 as p
-    return p
 
 
 def kind(handle):

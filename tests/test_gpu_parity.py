@@ -7,40 +7,13 @@ import display_model as DM
 import gamma_model as G
 import splat_model as M
 from conftest import bits_equal, golden, max_rel
+from sim_harness import SIZES, STREAM_SHAPES, TILED_SHAPES, make, nasty_fields, rand_fields, same_bits
+from sim_harness import pkg  # noqa: F401 -- a fixture
 from webgl_fluid_simulation_b200 import slab
 
 pytestmark = pytest.mark.gpu
 DT = 0.016666
 SPLAT_TOL = 2e-6   # expf: CUDA <= 2 ulp, glibc < 1 ulp; on a term that is added to the base
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    import webgl_fluid_simulation_b200 as p
-    return p
-
-
-def make(pkg, W, H, Wd, Hd, flags=0, jb=0, **cfg):
-    c = {"SIM_RESOLUTION": min(W, H), "DYE_RESOLUTION": min(Wd, Hd)}
-    c.update(cfg)
-    # canvas aspect = W/H like the reference; exact sizes are forced through the test hook because
-    # getResolution rounds (e.g. a 9x6 dye grid is not reachable from a 7:5 canvas)
-    s = pkg.FluidSimulation(c, canvas_width=W, canvas_height=H, flags=flags, jacobi_block=jb,
-                            sizes=(W, H, Wd, Hd))
-    assert s._dims("velocity")[:2] == (W, H), s._dims("velocity")
-    assert s._dims("dye")[:2] == (Wd, Hd), s._dims("dye")
-    return s
-
-
-def rand_fields(W, H, Wd, Hd, seed):
-    rng = np.random.default_rng(seed)
-    return ((rng.standard_normal((H, W, 2)) * 50).astype(np.float32),
-            rng.random((Hd, Wd, 4), dtype=np.float32),
-            rng.standard_normal((H, W)).astype(np.float32))
-
-
-SIZES = [(32, 32, 64, 64), (48, 32, 96, 64), (128, 128, 128, 128), (36, 20, 54, 30), (7, 5, 9, 6),
-         (256, 64, 512, 128), (1, 9, 3, 27), (9, 1, 27, 3)]
 
 
 @pytest.mark.parametrize("W,H,Wd,Hd", SIZES)
@@ -96,23 +69,6 @@ def test_passes_vs_golden_reference_shader_outputs(pkg, name):
     assert max_rel(s.readField("velocity"), g["splat_velocity"]) < SPLAT_TOL
     assert max_rel(s.readField("dye"), g["splat_dye"]) < SPLAT_TOL
     s.close()
-
-
-# Grids too small to give every SM a warp stream run the tiled kernels of passes.cuh; these run
-# curl_vorticity_divergence_kernel and gradient_subtract_kernel (and (16, 2) at 16 columns too).
-TILED_SHAPES = [(64, 40), (128, 128), (256, 96), (16, 2), (132, 77), (520, 33)]
-# Grids that select the row-streaming kernels of stream_passes.cuh (cvd: 120 output columns per
-# warp, lanes 1..30; gradient: 128 columns, lanes 0..31).  Warp counts from stream_args, for 132 SMs:
-#   8x4096    one window; both x walls inside one warp, only lanes 1 and 2 produce output
-#   12x4093   W/4 odd; the last 16-row chunk is partial (4093 = 255*16 + 13)
-#   124x2050  the second cvd window has one output lane; W % 128 = 124 for gradient
-#   964x600   964 = 8*120 + 4: the last cvd window produces only its wall lane
-#   132x2051  gradient: the last 128-column window has one live lane; H % 4 = 3, so the GS_U tail re-reads
-#   16900xH   141 cvd / 133 gradient windows fill the SMs in one chunk; H = 1 puts both y walls on one
-#             row; gradient's last window is a single wall lane
-#   1024x512  an ordinary power-of-two grid
-STREAM_SHAPES = [(8, 4096), (12, 4093), (124, 2050), (964, 600), (132, 2051), (16900, 1), (16900, 2),
-                 (16900, 3), (1024, 512)]
 
 
 @pytest.mark.parametrize("W,H", TILED_SHAPES + STREAM_SHAPES)
@@ -467,8 +423,6 @@ def test_resize_ragged_and_degenerate_sizes_like_resizeDoubleFBO(pkg, oracle, sr
     """initFramebuffers() on an fp32 handle (fluid_resize) at the sizes of its half-storage sibling and
     beyond: velocity and dye resampled with the LINEAR copy, bitwise against the oracle, inf / NaN dye
     NaN-aware; pressure, divergence and curl start over at zero."""
-    from test_gpu_fast_paths import same_or_both_nan
-    from test_gpu_splats import nasty_fields
     O = oracle
     v, _, p = rand_fields(*src, 9)
     _, dye, _ = nasty_fields(1, 1, src[2], src[3], 10)             # inf / NaN / subnormal dye
@@ -478,7 +432,7 @@ def test_resize_ragged_and_degenerate_sizes_like_resizeDoubleFBO(pkg, oracle, sr
     W, H, Wd, Hd = dst
     assert s._dims("velocity")[:2] == (W, H) and s._dims("dye")[:2] == (Wd, Hd)
     assert bits_equal(s.readField("velocity"), O.resample(v, W, H))
-    assert same_or_both_nan(s.readField("dye"), O.resample(dye, Wd, Hd))
+    assert same_bits(s.readField("dye"), O.resample(dye, Wd, Hd))
     for n in ("pressure", "divergence", "curl"):
         assert not s.readField(n).any(), n
     s.close()

@@ -1,5 +1,5 @@
 """The post-FX sliders BLOOM_INTENSITY / BLOOM_THRESHOLD / BLOOM_SOFT_KNEE / SUNRAYS_WEIGHT on the GPU: every
-parameter set of test_postfx_params_cpu.py on every handle kind that draws post-FX (fp32, fp32 + HALF_POSTFX,
+parameter set of display_harness.SETS on every handle kind that draws post-FX (fp32, fp32 + HALF_POSTFX,
 HALF_STORAGE | HALF_POSTFX, NEAREST_FILTERING, NEAREST_FILTERING | HALF_STORAGE | HALF_POSTFX) with BLOOM,
 SUNRAYS, BLOOM + SUNRAYS and SHADING + BLOOM + SUNRAYS: the bloom FBO and sunrays texture bit for bit against
 the matching model (display_model), the frame inside its powf interval (bit for bit without BLOOM), captures and canvases
@@ -11,27 +11,15 @@ import canvas_model as CV
 import display_model as M
 import gamma_model as G
 from conftest import golden, max_rel
-from display_harness import (BACK_RGB, check_capture, check_frame, flags_of, golden_dither, make, model_capture,
-                             model_frame, set_keywords, stored)
-from test_postfx_params_cpu import DEFAULTS, FIXTURES, GEOMETRIES, KEYS, SETS, cfg_of, fixture_cfg, params_dye
+from display_harness import (BACK_RGB, DEFAULTS, FIXTURES, GEOMETRIES, KEYS, SETS, cfg_of, check_capture, check_frame,
+                             fixture_cfg, flags_of, golden_dither, make, model_capture, model_frame, params_dye,
+                             set_keywords, stored)
+from sim_harness import pkg, torch  # noqa: F401 -- fixtures
 
 pytestmark = pytest.mark.gpu
 F32 = np.float32
 HANDLES = ["fp32", "fp32_half_postfx", "half_half_postfx", "nearest_fp32", "nearest_half_half_postfx"]
 KEYWORD_SETS = [M.BLOOM, M.SUNRAYS, M.BLOOM | M.SUNRAYS, M.ALL3]
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    import webgl_fluid_simulation_b200 as p
-    return p
-
-
-@pytest.fixture(scope="module")
-def torch():
-    import torch as t
-    assert t.cuda.is_available()
-    return t
 
 
 def handle_for(pkg, handle, geometry, cfg):

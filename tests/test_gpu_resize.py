@@ -5,34 +5,13 @@ import numpy as np
 import pytest
 
 from conftest import bits_equal
+from sim_harness import make, special
+from sim_harness import pkg  # noqa: F401 -- a fixture
 
 pytestmark = pytest.mark.gpu
 DT = 0.016666
 FIELDS = ("velocity", "dye", "pressure", "divergence", "curl")
 FLUID_ERR_NOMEM = -6
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    import webgl_fluid_simulation_b200 as p
-    return p
-
-
-def make(pkg, sizes, flags=0):
-    W, H, Wd, Hd = sizes
-    s = pkg.FluidSimulation({"SIM_RESOLUTION": min(W, H), "DYE_RESOLUTION": min(Wd, Hd)},
-                            canvas_width=W, canvas_height=H, flags=flags, sizes=sizes)
-    assert s._dims("velocity")[:2] == (W, H) and s._dims("dye")[:2] == (Wd, Hd)
-    return s
-
-
-def special(a, rng):
-    """`a` with a quarter of its values replaced by +-0, fp32 and fp16 subnormals, +-inf and NaN (each present)."""
-    specials = np.array([-0.0, 0.0, 1e-40, -3e-39, 1.4e-45, 6e-8, -3e-7, np.inf, -np.inf, np.nan], np.float32)
-    flat = a.reshape(-1)
-    k = flat.size // 4
-    flat[rng.choice(flat.size, k, replace=False)] = np.resize(specials, k)
-    return a
 
 
 def resize(s, sizes):
@@ -49,7 +28,7 @@ def assert_zero(s, names):
 @pytest.mark.parametrize("half", [False, True], ids=["fp32", "half"])
 def test_resize_keeps_a_same_size_field_bit_for_bit(pkg, half):
     rng = np.random.default_rng(11)
-    s = make(pkg, (36, 20, 54, 30), pkg.FLAG_HALF_STORAGE if half else 0)
+    s = make(pkg, 36, 20, 54, 30, pkg.FLAG_HALF_STORAGE if half else 0)
     # a step first: pressure, divergence and curl hold values and the pairs have been swapped
     s.writeField("velocity", (rng.standard_normal((20, 36, 2)) * 50).astype(np.float32))
     s.writeField("dye", rng.random((30, 54, 4), dtype=np.float32))
@@ -81,7 +60,7 @@ def test_resize_that_does_not_fit_changes_nothing(pkg):
     rng = np.random.default_rng(12)
     v = (rng.standard_normal((64, 64, 2)) * 50).astype(np.float32)
     d = rng.random((128, 128, 4), dtype=np.float32)
-    s, twin = make(pkg, sizes), make(pkg, sizes)
+    s, twin = make(pkg, *sizes), make(pkg, *sizes)
     for x in (s, twin):
         x.writeField("velocity", v); x.writeField("dye", d)
         x.step(DT)

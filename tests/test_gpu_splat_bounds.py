@@ -3,7 +3,7 @@ velocity and dye must lie within the fp32 arithmetic of the shader with an expf 
 float64 exp, carried through every record and the storage format's rounding.  The base each check
 starts from is the field as the library stores it (read back after the write).
 
-Covers fp32 and half storage; the grids of test_gpu_parity.SIZES plus partial 128x16 splat tiles in
+Covers fp32 and half storage; the grids of sim_harness.SIZES plus partial 128x16 splat tiles in
 both directions; 4096^2 on a subset of rows; one splat() per record and splats() with n = 1, 24 and 129
 (across the 128-record launch boundary); SPLAT_RADIUS down to 5e-5, where div_fast_ok fails for every
 texel; records on texel centres (d == 0) and far away (e subnormal or 0); canvases of aspect 1, > 1,
@@ -13,19 +13,14 @@ import numpy as np
 import pytest
 
 import splat_model as M
-from test_gpu_parity import make
-from test_splat_model_cpu import BASES, CANVASES, GRIDS, NARROWING_CANVAS, RADII, bases, records
+from sim_harness import make
+from sim_harness import pkg  # noqa: F401 -- a fixture
+from splat_model import BASES, CANVASES, GRIDS, NARROWING_CANVAS, RADII, bases, records
 
 pytestmark = pytest.mark.gpu
 F32 = np.float32
 HALF = 0x10
 STORAGE = pytest.mark.parametrize("flags", [0, HALF], ids=["fp32", "half"])
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    import webgl_fluid_simulation_b200 as p
-    return p
 
 
 def apply_calls(s, recs, call):

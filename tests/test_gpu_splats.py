@@ -7,48 +7,12 @@ import pytest
 
 import splat_model as M
 from conftest import bits_equal
-from test_gpu_parity import SIZES, make
+from sim_harness import SIZES, make, nasty_fields, nasty_records
+from sim_harness import pkg  # noqa: F401 -- a fixture
 
 pytestmark = pytest.mark.gpu
 DT = 0.016666
 FIELDS = ("velocity", "dye", "pressure", "divergence", "curl")
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    import webgl_fluid_simulation_b200 as p
-    return p
-
-
-def nasty_fields(W, H, Wd, Hd, seed):
-    """Seeded fields with -0.0, subnormals, +-inf and NaN sprinkled over ordinary values."""
-    rng = np.random.default_rng(seed)
-
-    def sprinkle(a):
-        flat = a.reshape(-1)
-        specials = np.array([-0.0, 0.0, 1e-40, -3e-39, 1.4e-45, np.inf, -np.inf, np.nan], np.float32)
-        k = max(1, flat.size // 7)
-        flat[rng.integers(0, flat.size, k)] = rng.choice(specials, k)
-        return a
-    v = sprinkle((rng.standard_normal((H, W, 2)) * 50).astype(np.float32))
-    d = sprinkle(rng.uniform(-1, 2, (Hd, Wd, 4)).astype(np.float32))
-    p = rng.standard_normal((H, W)).astype(np.float32)
-    return v, d, p
-
-
-def nasty_records(n, seed):
-    """Points inside and outside [0, 1], negative colours, large forces, and far points whose weights
-    end in the subnormal range or at zero."""
-    rng = np.random.default_rng(seed)
-    r = np.empty((n, 7), np.float32)
-    r[:, 0:2] = rng.uniform(-0.5, 1.5, (n, 2))
-    r[:, 2:4] = rng.uniform(-1, 1, (n, 2)) * 10.0 ** rng.integers(0, 5, (n, 1))
-    r[:, 4:7] = rng.uniform(-1.5, 1.5, (n, 3))
-    far = rng.random(n) < 0.2
-    r[far, 0] = rng.choice([-0.45, 1.45, 3.0, -40.0], far.sum())
-    exact = rng.random(n) < 0.1                         # a point on a texel centre: d == 0 there
-    r[exact, 0:2] = 0.5
-    return r
 
 
 def pair(pkg, W, H, Wd, Hd, seed, flags=0):

@@ -8,39 +8,15 @@ import pytest
 import display_model as M
 import gamma_model as G
 from conftest import golden, max_rel
+from gamma_model import CAPTURE_SETS, FRAME_TOL, POW2, RAGGED, RAGGED_CHAIN_TEXELS, cfg_of, fp16_ulps
 
 F32 = np.float32
 BACK_RGB = (10 / 255, 20 / 255, 30 / 255)
 KEYWORDS = {"bloom": M.BLOOM, "sunrays": M.SUNRAYS, "bloom_sunrays": M.BLOOM | M.SUNRAYS,
             "shading_bloom": M.SHADING | M.BLOOM, "shading_sunrays": M.SHADING | M.SUNRAYS}
-CAPTURE_SETS = ["none", "shading", "bloom", "shading_bloom", "sunrays", "shading_sunrays", "bloom_sunrays",
-                "shading_bloom_sunrays"]        # index = FLUID_DISPLAY_* mask
-POW2, RAGGED = "keywords_half_64_to_128", "keywords_half_48x32_to_50x75"
-# Frames against the executed shaders, max_rel (field-normalised).  Measured, oracle vs executed: 0 on
-# the power-of-two fixture (bit for bit), 2.52e-4 on the ragged one (shading_sunrays 2.40e-4, bloom
-# 4.7e-5), all from the ragged chains below.  The GPU adds powf's <= 4 ulp with BLOOM.
-FRAME_TOL = 3e-4
-# The ragged fixture's chains, measured: at most 1 fp16 ulp, in 2 of 24576 bloom values, 3 of 3456
-# sunrays texels and 1 of 1536 mask texels.  Cause: the rasteriser's vUv = aPosition * 0.5 + 0.5 is not
-# (i + .5) / W in fp32 for a W that is not a power of two (DESIGN §2, non-power-of-two advection); the
-# LINEAR weights move by an fp32 ulp and now and then that flips an fp16 rounding.  The pyramid levels
-# are bit for bit.
-RAGGED_CHAIN_TEXELS = {"bloom": 2, "sunrays": 3, "mask_alpha": 1}
-
-
-def cfg_of(g):
-    return dict(BLOOM_RESOLUTION=int(g["bloom_res"]), SUNRAYS_RESOLUTION=int(g["sun_res"]))
-
-
 def half_chains(g, half_mask=True):
     w, h = int(g["w"]), int(g["h"])
     return M.chains(g["in_dye"], w, h, M.BLOOM | M.SUNRAYS, cfg_of(g), half_targets=True, half_mask=half_mask)
-
-
-def fp16_ulps(a, b):
-    a = np.asarray(a, np.float16).view(np.int16).astype(np.int64)
-    b = np.asarray(b, np.float16).view(np.int16).astype(np.int64)
-    return int(np.abs(a - b).max())
 
 
 @pytest.mark.parametrize("name", [POW2, RAGGED])

@@ -4,7 +4,7 @@ import numpy as np
 import pytest
 
 from conftest import bits_equal
-from jacobi_tb_model import jacobi_tb_model
+from jacobi_tb_model import KINDS, NONFINITE_KINDS, equal, jacobi_tb_model, overflow_sweep, special_fields
 
 
 @pytest.mark.parametrize("W,H,K,R", [(128, 40, 3, 16), (256, 33, 8, 12), (16, 9, 2, 4),
@@ -40,67 +40,6 @@ def test_model_on_a_slab_with_ghost_rows(oracle):
 
 
 # ---- the top of the fp32 range, inf and NaN ------------------------------------------------------------
-# Data sets the contracted tail must survive (shared with the GPU tests).  Stored pressure is divided by
-# PRESSURE so that the fused clear brings the patch to the magnitude that overflows at once.
-KINDS = ["near_max", "near_max_neg", "huge_div", "nonfinite", "full_range"]
-NONFINITE_KINDS = {"nonfinite", "full_range"}          # inf / NaN in the inputs
-# results that can hold NaN (inf - inf of overflowed neighbours), whose bits differ between x86 and the GPU:
-# compared NaN-aware, the others bitwise
-NAN_KINDS = NONFINITE_KINDS | {"huge_div"}
-
-
-def special_fields(kind, W, H, seed, pressure=1.0):
-    """(p, d) of one data set: ordinary fields with
-    near_max      p = 8.5e37 / PRESSURE over a patch and d = -1e37 under it: four such neighbours sum to
-                  3.4e38 and S - d rounds to +inf in the first sweep, while S/4 - d/4 is finite;
-    near_max_neg  the same with both signs flipped;
-    huge_div      |d| in [2^126, FLT_MAX] over a patch of ordinary p: the first sweep leaves p ~ -d/4 and
-                  the second one overflows;
-    nonfinite     +-inf and NaN sprinkled into both p and d;
-    full_range    binary exponents -149..127 tile by tile for both (subnormals to inf)."""
-    from test_gpu_fast_paths import exp_tiled
-    rng = np.random.default_rng(seed)
-    p = rng.standard_normal((H, W)).astype(np.float32)
-    d = rng.uniform(-1, 1, (H, W)).astype(np.float32)
-    r0, r1 = H // 4, min(H // 4 + max(3, H // 3), H)
-    c0, c1 = W // 3, W // 3 + max(8, W // 4)
-    if kind in ("near_max", "near_max_neg"):
-        sg = np.float32(1.0 if kind == "near_max" else -1.0)
-        p[r0:r1, c0:c1] = sg * np.float32(8.5e37 / pressure)
-        d[max(r0 - 1, 0):r1 + 1, c0 - 1:c1 + 1] = -sg * np.float32(1e37)
-    elif kind == "huge_div":
-        mag = rng.uniform(2.0 ** 126, float(np.finfo(np.float32).max), (r1 - r0, c1 - c0))
-        d[r0:r1, c0:c1] = (mag * rng.choice([-1.0, 1.0], mag.shape)).astype(np.float32)
-    elif kind == "nonfinite":
-        for a in (p, d):
-            k = rng.choice(H * W, size=max(6, H * W // 500), replace=False)
-            a.flat[k] = rng.choice(np.array([np.inf, -np.inf, np.nan], np.float32), k.size)
-    else:
-        p = exp_tiled((H, W), seed, lo=-149, hi=127, tile=(4, 16))
-        d = exp_tiled((H, W), seed + 1, lo=-149, hi=127, tile=(4, 16))
-    return p, d
-
-
-def overflow_sweep(oracle, p, d, iters, pressure):
-    """First sweep (1-based) of the oracle's clear + `iters` sweeps with a cell whose S and d are finite and
-    whose rn(S - d) is infinite -- where the contracted tail would differ -- or None."""
-    q = oracle.clear(p, pressure)
-    for k in range(1, iters + 1):
-        e = np.pad(q, 1, mode="edge")
-        with np.errstate(invalid="ignore", over="ignore"):
-            S = ((e[1:-1, :-2] + e[1:-1, 2:]) + e[:-2, 1:-1]) + e[2:, 1:-1]
-            hit = np.isfinite(S) & np.isfinite(d) & np.isinf(S - d)
-        if hit.any():
-            return k
-        q = oracle.jacobi(q, d, 1)
-    return None
-
-
-def equal(kind, a, b):
-    from test_gpu_fast_paths import same_or_both_nan
-    return same_or_both_nan(a, b) if kind in NAN_KINDS else bits_equal(a, b)
-
-
 @pytest.mark.parametrize("kind", ["near_max", "near_max_neg", "huge_div"])
 def test_model_with_the_tiny_map_rule_alone_differs_from_the_oracle(oracle, kind):
     """The premise, on the CPU: selecting the exact tail by the tiny-divergence map only (the rule before

@@ -9,6 +9,7 @@ import pytest
 
 import linear_advection_model as M
 from conftest import ROOT, bits_equal, golden, max_rel
+from sim_harness import same_bits
 
 PASS = ["32x32_64x64", "64x32_128x64", "16x16_16x16", "128x128_256x256", "24x16_40x28"]
 STEP = ["32x32_64x64", "64x32_128x64"]
@@ -16,12 +17,6 @@ TAGS = ["fp32", "half"]
 RAGGED = "24x16_40x28"
 NONPOW2_ADVECT_TOL = 2e-5       # the MANUAL goldens' bound for the library's (i + .5) / n against the rasteriser's vUv
 NONPOW2_ADVECT_TOL_HALF = 1e-3  # the same ulp of vUv, seen through fp16 storage: one fp16 ulp (2^-10) of the field's largest value
-
-
-def same_or_both_nan(a, b):
-    a = np.ascontiguousarray(a, np.float32); b = np.ascontiguousarray(b, np.float32)
-    na, nb = np.isnan(a), np.isnan(b)
-    return a.shape == b.shape and np.array_equal(na, nb) and np.array_equal(a[~na].view(np.uint32), b[~nb].view(np.uint32))
 
 
 def store(half):
@@ -51,7 +46,7 @@ def test_model_matches_executed_linear_shader_per_pass(oracle, tag, shape, capsy
         if "special_in_velocity" in g:
             sv, sd = run_pass(g, "special_")
             assert np.isnan(g["special_advect_velocity"]).any() and np.isinf(g["special_in_velocity"]).any()
-            assert same_or_both_nan(sv, g["special_advect_velocity"]) and same_or_both_nan(sd, g["special_advect_dye"])
+            assert same_bits(sv, g["special_advect_velocity"]) and same_bits(sd, g["special_advect_dye"])
         return
     rv, rd = run_pass(g, uv="raster")
     assert bits_equal(rv, g["advect_velocity"]) and bits_equal(rd, g["advect_dye"])
@@ -108,7 +103,7 @@ def _rejected(**mutant):
                 return True
             if "special_in_velocity" in g:
                 sv, sd = run_pass(g, "special_", **kw)
-                if not (same_or_both_nan(sv, g["special_advect_velocity"]) and same_or_both_nan(sd, g["special_advect_dye"])):
+                if not (same_bits(sv, g["special_advect_velocity"]) and same_bits(sd, g["special_advect_dye"])):
                     return True
     return False
 
@@ -126,13 +121,10 @@ def test_own_texel_mutant_is_caught_only_by_a_non_finite_neighbour(oracle):
     a, _ = run_pass(g, own_texel=True)
     assert bits_equal(a, g["advect_velocity"])
     b, _ = run_pass(g, "special_", own_texel=True)
-    assert not same_or_both_nan(b, g["special_advect_velocity"])
+    assert not same_bits(b, g["special_advect_velocity"])
 
 
-P4_HALF_GATE = 1e-6
-
-
-@pytest.mark.parametrize("name,gate", [("p4_linear_fp32_32", 1e-5), ("p4_linear_half_32", P4_HALF_GATE)])
+@pytest.mark.parametrize("name,gate", [("p4_linear_fp32_32", 1e-5), ("p4_linear_half_32", M.P4_HALF_GATE)])
 def test_p4_desktop_scenarios_after_one_step(oracle, name, gate, capsys):
     """The desktop-browser scenarios (8 splats, LINEAR samplers, fp32 or fp16 textures) one step on.  With
     LINEAR advection only the splats' expf can differ from the executed shaders (numpy's against glibc's,

@@ -1,7 +1,7 @@
 """The four post-FX sliders -- BLOOM_INTENSITY, BLOOM_THRESHOLD, BLOOM_SOFT_KNEE, SUNRAYS_WEIGHT (S:79-84, the
-settings panel S:227-232) -- away from their defaults, on the CPU.  This file holds the parameter sets and the
-dye that tests/test_gpu_postfx_params.py draws with them, and shows that they are strong enough to catch a
-wrong kernel:
+settings panel S:227-232) -- away from their defaults, on the CPU.  The parameter sets and the dye that
+tests/test_gpu_postfx_params.py draws with them live in tests/display_harness.py; this file shows that they
+are strong enough to catch a wrong kernel:
 
 * branches: for every set, the bloom prefilter (bloomPrefilterShader S:614-631) sees enough texels below
   curve.x, inside the knee and above it, with rq winning and losing max(rq, br - threshold), and with br
@@ -22,72 +22,13 @@ import capture_model as CM
 import display_model as M
 import gamma_model as G
 from conftest import golden, max_rel
-from display_harness import BACK_RGB, golden_dither
+from display_harness import (BACK_RGB, DEFAULTS, FIXTURES, GEOMETRIES, KEYS, SETS, cfg_of, fixture_cfg, golden_dither,
+                             params_dye)
 from oracle import oracle as O
 
 F32 = np.float32
 ALL3 = M.ALL3
-DEFAULTS = dict(BLOOM_INTENSITY=0.8, BLOOM_THRESHOLD=0.6, BLOOM_SOFT_KNEE=0.7, SUNRAYS_WEIGHT=1.0)   # S:79-84
-# (I, T, K, W).  t033_k07 and t039_k1 are slider positions where knee / curve narrowed from fp32 arithmetic
-# differ from the JS doubles narrowed once (all three curve components); t005 differs in curve.x and curve.z.
-SETS = {
-    "t0_k1": (0.8, 0.0, 1.0, 1.0),           # threshold 0: curve = (-1e-4, 2e-4, 2500); the knee is wider than the threshold
-    "t0_k0_w4": (0.1, 0.0, 0.0, 4.0),        # sunrays above 1: alpha above 1, the canvas clamps
-    "t005": (1.3, 0.05, 0.7, 0.6),
-    "t033_k07": (0.55, 0.33, 0.7, 0.45),
-    "t039_k1": (1.6, 0.39, 1.0, 0.85),
-    "t1_k0_i2_w03": (2.0, 1.0, 0.0, 0.3),    # knee 0: knee = 1e-4, a hard step
-    "t1_k1": (0.1, 1.0, 1.0, 1.0),
-    "i0_w0": (0.0, 0.6, 0.7, 0.0),
-    "overflow": (70000.0, 0.6, 0.7, 1.0),    # the final blit overflows fp16 to +inf on about half the HALF_POSTFX texels
-    "above": (0.8, 5.0, 0.2, 0.5),           # curve.x = 4 above every br of the dye: the prefilter draws zeros
-}
-KEYS = ("BLOOM_INTENSITY", "BLOOM_THRESHOLD", "BLOOM_SOFT_KNEE", "SUNRAYS_WEIGHT")
-# (dye w, dye h, canvas w, canvas h, BLOOM_RESOLUTION, SUNRAYS_RESOLUTION, CAPTURE_RESOLUTION): every size a
-# power of two (bloom 64 x 32, sunrays 32 x 16, capture 64 x 32), and a ragged dye on a portrait canvas
-# (bloom 48 x 64, sunrays 30 x 40, capture 45 x 60)
-GEOMETRIES = {"pow2": (64, 64, 128, 64, 32, 16, 32), "portrait": (40, 56, 90, 120, 48, 30, 45)}
-DYE_SEED = 2718
 MIN_TEXELS = 8                               # bloom texels each branch must get, per set and geometry
-
-
-def cfg_of(name, geometry="pow2"):
-    """The config keys of parameter set `name` on `geometry`."""
-    I, T, K, W = SETS[name]
-    bres, sres, cres = GEOMETRIES[geometry][4:]
-    return dict(BLOOM_INTENSITY=I, BLOOM_THRESHOLD=T, BLOOM_SOFT_KNEE=K, SUNRAYS_WEIGHT=W, BLOOM_RESOLUTION=bres,
-                SUNRAYS_RESOLUTION=sres, CAPTURE_RESOLUTION=cres)
-
-
-def params_dye(Wd, Hd, seed=DYE_SEED):
-    """Finite dye whose brightest channel br (the prefilter's) falls in 4 x 4 blocks of one kind each, so that a
-    LINEAR fetch at ragged sizes mostly mixes texels of one kind: exact zeros (the other channels in -2e-3 .. -1e-3), fp32
-    subnormals, negatives down to -2, +-1e-7 .. 1e-4 around the threshold-0 knee, values inside the knee
-    [T - knee, T + knee] of a set of SETS but `above` (a hard step's knee is 2e-4 wide: no uniform draw would land there),
-    and bright values 3.2 u^1.5 (u uniform) reaching every knee.  One channel holds br, the other two a
-    fraction of it (more negative for a negative br); which channel is the same across a block.  Alpha 1.  No channel is -0, in fp32 or
-    rounded to fp16: where the display's alpha is fmaxf(-0, +0), the device and C need not agree."""
-    rng = np.random.default_rng(seed)
-    bh, bw = (Hd + 3) // 4, (Wd + 3) // 4
-    up = lambda a: np.kron(a, np.ones((4, 4), a.dtype))[:Hd, :Wd]             # noqa: E731
-    kind = up(rng.choice(6, size=(bh, bw), p=[0.07, 0.06, 0.09, 0.09, 0.19, 0.50]))
-    knees = np.array([(t, t * k + 0.0001) for n, (_, t, k, _) in SETS.items() if n != "above"])
-    pick = up(rng.integers(0, len(knees), (bh, bw)))
-    u = rng.random((Hd, Wd))
-    sign = np.where(rng.random((Hd, Wd)) < 0.5, -1.0, 1.0)
-    br = np.select([kind == 0, kind == 1, kind == 2, kind == 3, kind == 4],
-                   [np.zeros_like(u), 1e-45 + u * 1.1e-38, -np.exp(np.log(1e-6) + u * np.log(2e6)),
-                    sign * np.exp(np.log(1e-7) + u * np.log(1e3)), knees[pick, 0] + knees[pick, 1] * (2 * u - 1)],
-                   3.2 * u ** 1.5).astype(F32)
-    frac = rng.random((Hd, Wd, 3)).astype(F32)
-    c = np.where(br[..., None] >= 0, br[..., None] * frac, br[..., None] * (F32(1) + frac))
-    c[kind == 0] = -(F32(1) + frac[kind == 0]) * F32(1e-3)
-    top = up(rng.integers(0, 3, (bh, bw)))
-    np.put_along_axis(c, top[..., None], br[..., None], axis=-1)
-    dye = np.concatenate([c, np.ones((Hd, Wd, 1), F32)], axis=-1).astype(F32)
-    assert np.isfinite(dye).all() and not ((dye == 0) & np.signbit(dye)).any()
-    assert not ((O.round_half(dye) == 0) & np.signbit(O.round_half(dye))).any()
-    return dye
 
 
 # ---- the chain model, with its mutants -------------------------------------------------------------------
@@ -243,15 +184,6 @@ def test_mutant_changes_the_expected_bits(oracle, mutant):
 
 
 # ---- the oracle against the executed shaders ------------------------------------------------------------
-FIXTURES = [f"postfx_params_{n}_64_to_128x64" for n in ("t033_k07", "t0_k1", "t1_k0_i2_w03")]
-
-
-def fixture_cfg(g):
-    return dict(BLOOM_RESOLUTION=int(g["bloom_res"]), SUNRAYS_RESOLUTION=int(g["sun_res"]),
-                BLOOM_INTENSITY=float(g["intensity"]), BLOOM_THRESHOLD=float(g["threshold"]),
-                BLOOM_SOFT_KNEE=float(g["soft_knee"]), SUNRAYS_WEIGHT=float(g["weight"]))
-
-
 @pytest.mark.parametrize("name", FIXTURES)
 def test_oracle_equals_executed_shaders(oracle, name):
     """Bloom FBO and sunrays bit for bit, the frame within the power-of-two post-FX goldens' 2e-6

@@ -116,14 +116,13 @@ def test_generator_is_deterministic_and_reaches_every_class(half):
     """Same seed, same session; another seed, another session; and over the committed seeds of
     test_gpu_session.py every operation kind, config key, JACOBI_BLOCK value, dt kind, splat count class,
     resize direction and size class of the schedule is reached, the session ending at its starting size."""
-    from test_gpu_session import N_OPS, SEEDS
-    seeds = SEEDS[half]
-    a = S.generate(seeds[0], half, N_OPS)
-    assert a == S.generate(seeds[0], half, N_OPS)
-    assert a != S.generate(seeds[0] + 1000, half, N_OPS)
+    seeds = S.SEEDS[half]
+    a = S.generate(seeds[0], half, S.N_OPS)
+    assert a == S.generate(seeds[0], half, S.N_OPS)
+    assert a != S.generate(seeds[0] + 1000, half, S.N_OPS)
     reached = set()
     for seed in seeds:
-        ops = S.generate(seed, half, N_OPS)
+        ops = S.generate(seed, half, S.N_OPS)
         assert 30 <= len(ops) <= 60, len(ops)
         resizes = [op[1] for op in ops if op[0] == "resize"]
         assert resizes == list(range(1, len(S.schedule(half))))

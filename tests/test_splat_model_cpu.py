@@ -10,43 +10,9 @@ import numpy as np
 import pytest
 
 import splat_model as M
-from test_gpu_fast_paths import exp_tiled
-from test_gpu_parity import SIZES
-from test_gpu_splats import nasty_fields, nasty_records
+from splat_model import BASES, CANVASES, GRIDS, NARROWING_CANVAS, RADII, bases, records
 
 F32 = np.float32
-# SIZES plus partial 128x16 splat tiles in both directions on both planes
-GRIDS = SIZES + [(129, 17, 257, 33)]
-BASES = ["zero", "exp_tiled", "nasty"]
-RADII = [0.25, 0.01, 1.0, 5e-5]          # 5e-5: radius 5e-7 < 2^-20, every warp takes the IEEE division
-# aspect 1, > 1, < 1, and a canvas whose radius depends on narrowing the aspect before the multiply
-CANVASES = [(100, 100), (300, 200), (200, 300), (142, 100)]
-NARROWING_CANVAS = (142, 100)
-
-
-def records(n, seed, planes):
-    """nasty_records (far points, points outside [0, 1], large forces, (.5, .5)) with every 4th record
-    from the second on moved onto a texel centre of one of `planes` ((W, H) pairs): d == 0 there."""
-    r = nasty_records(n, seed)
-    rng = np.random.default_rng(seed + 1)
-    for k in range(1, n, 4):
-        W, H = planes[(k // 4) % len(planes)]
-        r[k, 0] = M.uv(W)[rng.integers(0, W)]
-        r[k, 1] = M.uv(H)[rng.integers(0, H)]
-    return r
-
-
-def bases(kind, W, H, Wd, Hd, seed):
-    """(velocity, dye) starting fields: zeros, one binary exponent in [-149, 100] per tile with random
-    mantissas and signs, or nasty_fields (-0, subnormals, +-inf, NaN over ordinary values)."""
-    if kind == "zero":
-        return np.zeros((H, W, 2), F32), np.zeros((Hd, Wd, 4), F32)
-    if kind == "exp_tiled":
-        return exp_tiled((H, W, 2), seed, tile=(4, 8)), exp_tiled((Hd, Wd, 4), seed + 1, tile=(4, 8))
-    v, d, _ = nasty_fields(W, H, Wd, Hd, seed)
-    return v, d
-
-
 def oracle_splats(O, base, recs, aspect, radius, half):
     """The oracle's splat() per record on one plane, rounded to fp16 after each in half storage."""
     out = O.round_half(base) if half else base.copy()
