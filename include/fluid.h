@@ -182,6 +182,30 @@ int fluid_p2p_export(fluid_t* h, void* blob, size_t blob_bytes);   /* blob_bytes
 int fluid_p2p_connect(fluid_t* h, const void* blob_below, const void* blob_above);
 int fluid_p2p_disable(fluid_t* h);   /* back to NCCL; call on every rank if any rank failed to connect */
 
+/* Batch handles (no reference counterpart): B = `members` independent simulations of cfg's sizes, scalars
+ * and flags in one handle, stepped and splatted together through the same launches.  Member m ends every call
+ * with the bits an ordinary handle given member m's inputs would hold.  All fields start zero with dye alpha
+ * 1 in every member, as after fluid_create.
+ *  - fluid_step steps every member with one dt (a CUDA graph unless FLUID_FLAG_NO_GRAPH); fluid_set_param,
+ *    fluid_set_param_f64 and fluid_get_param apply to all members.
+ *  - fluid_field_elems is B x w x rows x channels, and fluid_field_dims gives one member's w, rows and
+ *    channels with row0 = 0.  fluid_read, fluid_write, fluid_read_device and fluid_write_device move all
+ *    members in member order as a (B, H, W[, C]) C-contiguous array; fluid_device_ptr is member 0's .read,
+ *    the other members following it contiguously.
+ *  - fluid_sync, fluid_stat, fluid_launch_count, fluid_mark, fluid_elapsed_ms, fluid_timing_last,
+ *    fluid_last_error and fluid_destroy behave as on any handle.
+ *  - Every other entry point refuses a batch handle with FLUID_ERR_INVALID and leaves it usable: render,
+ *    capture and the canvas, fluid_render_band, fluid_resize, fluid_pass_*, fluid_pressure_solve_host,
+ *    fluid_splat and fluid_splats (use fluid_splats_batch) and the p2p calls.
+ * fluid_create_batch refuses with FLUID_ERR_INVALID: members < 1 or > FLUID_MAX_MEMBERS (the member is the
+ * kernels' grid z index); any flag but FLUID_FLAG_NO_GRAPH; sizes that are not powers of two, a sim or dye
+ * width under 128 or a height under 2.  The reference default 128^2 / 1024^2 qualifies.  FLUID_ERR_NOMEM:
+ * the fields of B members do not fit; nothing is left allocated. */
+#define FLUID_MAX_MEMBERS 65535
+int fluid_create_batch(const fluid_config* cfg, int members, fluid_t** out);
+/* B of a batch handle; 1 for ordinary and slab handles (0 for NULL). */
+int fluid_members(fluid_t* h);
+
 void fluid_destroy(fluid_t* h);
 
 /* initFramebuffers() on a live simulation (S:982-1010 else-branches + resizeDoubleFBO S:1116-1126):
@@ -212,6 +236,14 @@ int fluid_splat(fluid_t* h, float x, float y, float dx, float dy, float r, float
  * before the call returns.  n == 0 does nothing (dye alpha included); n < 0, or splats == NULL with
  * n > 0, is FLUID_ERR_INVALID and leaves the fields untouched. */
 int fluid_splats(fluid_t* h, const float* splats, int n);
+
+/* fluid_splats for a batch handle: record k (the 7 floats of fluid_splats) goes to member member[k].  Each
+ * member receives its records in call order, with the bits fluid_splats would give an ordinary handle;
+ * a member named by no record is not touched (dye alpha included).  The records are applied in place on the
+ * named members' .read, in launches of at most 128 records for at most 64 members; no other member costs a
+ * block.  n == 0 does nothing.  n < 0, a NULL array with n > 0, a member index outside [0, B) or an
+ * ordinary handle is FLUID_ERR_INVALID, with every field untouched. */
+int fluid_splats_batch(fluid_t* h, const int32_t* member, const float* splats, int n);
 
 /* config.<KEY> = value (S:59-69).  PRESSURE_ITERATIONS / JACOBI_BLOCK are rounded to int. */
 int fluid_set_param(fluid_t* h, int key, float value);

@@ -24,7 +24,7 @@ SYMBOLS = [
     "fluid_pass_advect_dye", "fluid_pass_curl_vorticity_divergence", "fluid_field_elems",
     "fluid_field_dims", "fluid_read", "fluid_write", "fluid_read_device", "fluid_write_device", "fluid_pressure_solve_host", "fluid_render", "fluid_render_band", "fluid_render_postfx", "fluid_render_keywords", "fluid_capture", "fluid_capture_device", "fluid_render_canvas", "fluid_sync",
     "fluid_timing_last", "fluid_host_alloc", "fluid_host_free", "fluid_mark", "fluid_elapsed_ms", "fluid_launch_count", "fluid_device_ptr",
-    "fluid_last_error",
+    "fluid_last_error", "fluid_create_batch", "fluid_members", "fluid_splats_batch",
 ]
 
 FLUID_OK = 0
@@ -98,6 +98,8 @@ def lib():
     L.fluid_config_default.argtypes = [C.POINTER(Config)]; L.fluid_config_default.restype = None
     L.fluid_get_resolution.argtypes = [i, i, i, C.POINTER(i), C.POINTER(i)]; L.fluid_get_resolution.restype = None
     L.fluid_create.argtypes = [C.POINTER(Config), C.POINTER(vp)]
+    L.fluid_create_batch.argtypes = [C.POINTER(Config), i, C.POINTER(vp)]
+    L.fluid_members.argtypes = [vp]
     L.fluid_create_slab.argtypes = [C.POINTER(Config), i, i, vp, sz, C.POINTER(vp)]
     L.fluid_nccl_unique_id.argtypes = [vp, sz]
     L.fluid_p2p_export.argtypes = [vp, vp, sz]
@@ -108,6 +110,7 @@ def lib():
     L.fluid_step.argtypes = [vp, f]
     L.fluid_splat.argtypes = [vp] + [f] * 7
     L.fluid_splats.argtypes = [vp, fp, i]
+    L.fluid_splats_batch.argtypes = [vp, C.POINTER(C.c_int32), fp, i]
     L.fluid_set_param.argtypes = [vp, i, f]
     L.fluid_set_param_f64.argtypes = [vp, i, C.c_double]
     L.fluid_get_param.argtypes = [vp, i, fp]

@@ -97,6 +97,10 @@ struct fluid : SlabGeometry {
     bool half_fx = false;                  // FLUID_FLAG_HALF_POSTFX: the bloom and sunrays targets are fp16, single GPU only
     bool nearest = false;                  // FLUID_FLAG_NEAREST_FILTERING: display, post-FX and resize sample NEAREST, single GPU only
     bool linear_adv = false;               // FLUID_FLAG_LINEAR_ADVECTION: advection samples LINEAR (passes.cuh LinearSampler), single GPU only
+    // fluid_create_batch: `members` simulations of one size and config.  Every slot of the arena holds them as a
+    // dense (B, H, W) array, the tiny map one region per member, and the step kernels take the member as blockIdx.z
+    bool batch = false;
+    int members = 1;
     float* scratch = nullptr;              // half mode: fp32 staging of fluid_read / fluid_write / render
     size_t scratch_floats = 0;
     float* dt_dev = nullptr;               // step()'s dt lives in device memory: one graph serves every dt
@@ -268,7 +272,7 @@ auto with_filter(const fluid_t* h, Fn&& f) {
 // ---- the tiny-divergence map (jacobi.cuh): one byte per 128 x 32 cells of the GLOBAL grid -------------
 int alloc_tiny_map(fluid_t* h) {
     cudaFree(h->tiny_map); h->tiny_map = nullptr;
-    h->tiny_map_bytes = (size_t)tiny_map_w(h->cfg.sim_w) * tiny_map_h(h->cfg.sim_h);
+    h->tiny_map_bytes = (size_t)tiny_map_w(h->cfg.sim_w) * tiny_map_h(h->cfg.sim_h) * h->members;
     CU(cudaMalloc((void**)&h->tiny_map, h->tiny_map_bytes));
     CU(cudaMemsetAsync(h->tiny_map, 0, h->tiny_map_bytes, h->stream));
     return FLUID_OK;
@@ -279,12 +283,16 @@ int clear_tiny_map(fluid_t* h) {
     ++h->div_epoch;                       // every writer of divergence comes through here
     return FLUID_OK;
 }
-// divergence rows [j_lo, j_hi) came from outside (host write, neighbour rank): flag their cells
+// divergence rows [j_lo, j_hi) came from outside (host write, neighbour rank): flag their cells.  A batch
+// handle scans those rows of every member into the member's region of the map.
 int scan_tiny(fluid_t* h, int j_lo, int j_hi) {
     if (j_hi <= j_lo) return FLUID_OK;
     dim3 b(256), g((h->cfg.sim_w + 255) / 256, j_hi - j_lo);
-    tiny_scan_kernel<<<g, b, 0, h->stream>>>(h->divergence, h->tiny_map, h->cfg.sim_w, h->roff, j_lo, j_hi);
-    return check_launch(h, "tiny_scan_kernel");
+    const size_t region = h->tiny_map_bytes / h->members;
+    for (int m = 0; m < h->members; ++m)
+        tiny_scan_kernel<<<g, b, 0, h->stream>>>(h->divergence + m * sim_cells(h), h->tiny_map + m * region, h->cfg.sim_w,
+                                                 h->roff, j_lo, j_hi);
+    return check_launch(h, "tiny_scan_kernel", h->members);
 }
 
 // ---- Jacobi dispatch -----------------------------------------------------------------------------
@@ -363,39 +371,62 @@ int encode_rows_map(fluid_t* h, unsigned char (&tm)[128], const void* base, int 
     return FLUID_OK;
 }
 
+// The B members of a batch handle's fp32 field at `base` as a 3-D tensor map (W, H, B); box = TB_BOX columns x
+// 3 rows x 1 member, so that a box reaching past a member's first or last row reads zeros, as on a 2-D map.
+int encode_members_map(fluid_t* h, unsigned char (&tm)[128], const void* base, int W, int H, int B) {
+    EncodeTiledFn enc = encode_tiled_fn();
+    const cuuint64_t dims[3] = {(cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
+    const cuuint64_t strides[2] = {(cuuint64_t)W * sizeof(float), (cuuint64_t)W * H * sizeof(float)};
+    const cuuint32_t box[3] = {TB_BOX, 3, 1};
+    const cuuint32_t estr[3] = {1, 1, 1};
+    if (!enc || enc(reinterpret_cast<CUtensorMap*>(tm), CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<void*>(base), dims,
+                    strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
+                    CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
+        return fail(h, FLUID_ERR_CUDA, "cuTensorMapEncodeTiled of %d members of a %d x %d fp32 field failed", B, W, H);
+    return FLUID_OK;
+}
+
 // (re)build the tensor maps after the pressure / divergence buffers were allocated.  The blocked kernel
 // stages only through them, so a handle that runs it cannot do without.
 int build_tmaps(fluid_t* h) {
     h->tmaps = {};
     if (!tb_eligible(h)) return FLUID_OK;
+    const int W = h->cfg.sim_w;
     for (int k = 0; k < 2; ++k) {
-        int rc = encode_rows_map(h, h->tmaps.m[k].p, h->arena + h->layout.p[k], h->cfg.sim_w, h->lrows());
-        if (!rc) rc = encode_rows_map(h, h->tmaps.m[k].d, h->divergence, h->cfg.sim_w, h->lrows());
+        fk::TmapPair& m = h->tmaps.m[k];
+        const void* p = h->arena + h->layout.p[k];
+        int rc = h->batch ? encode_members_map(h, m.p, p, W, h->cfg.sim_h, h->members) : encode_rows_map(h, m.p, p, W, h->lrows());
+        if (!rc) rc = h->batch ? encode_members_map(h, m.d, h->divergence, W, h->cfg.sim_h, h->members)
+                               : encode_rows_map(h, m.d, h->divergence, W, h->lrows());
         if (rc) return rc;
     }
     return FLUID_OK;
 }
 
-// kTb[K - 1]: jacobi_tb_kernel<K, SCALE> as kernel[SCALE], and the TB<K> constants its launch needs
+// kTb[K - 1]: jacobi_tb_kernel<K, SCALE> as kernel[SCALE], its batch-handle form as batch[SCALE], and the TB<K>
+// constants their launches need
 struct TbEntry {
     void (*kernel[2])(JacobiArgs, TmapPair);
     int valid, u, smem;
+    void (*batch[2])(JacobiArgs, TmapPair);
 };
 template <int K>
 constexpr TbEntry tb_entry() {
-    return {{jacobi_tb_kernel<K, false>, jacobi_tb_kernel<K, true>}, TB<K>::VALID, TB<K>::U, TB<K>::SMEM};
+    return {{jacobi_tb_kernel<K, false>, jacobi_tb_kernel<K, true>}, TB<K>::VALID, TB<K>::U, TB<K>::SMEM,
+            {jacobi_tb_kernel<K, false, true>, jacobi_tb_kernel<K, true, true>}};
 }
 static const TbEntry kTb[KMAX] = {tb_entry<1>(), tb_entry<2>(), tb_entry<3>(), tb_entry<4>(), tb_entry<5>(),
                                   tb_entry<6>(), tb_entry<7>(), tb_entry<8>(), tb_entry<9>(), tb_entry<10>(),
                                   tb_entry<11>(), tb_entry<12>(), tb_entry<13>()};
 
 // rows per warp stream of a depth-K launch: enough chunks that every SM holds its full complement of
-// resident warps (single wave), rounded so that a stream's step count R + 2K is a multiple of the unroll
-// U.  Both SCALE instantiations are sized from the occupancy of the SCALE = false one.
+// resident warps (single wave) across the members x windows x chunks, rounded so that a stream's step count
+// R + 2K is a multiple of the unroll U.  Both SCALE instantiations are sized from the occupancy of the
+// SCALE = false one.
 int tb_rows(const fluid_t* h, const TbEntry& e, int K, int W, int rows) {
-    const int nxw = (W + e.valid - 1) / e.valid;
+    const int nxw = (W + e.valid - 1) / e.valid * h->members;     // windows of all members
     int occ = 0;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, e.kernel[0], 32, e.smem);
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, h->batch ? e.batch[0] : e.kernel[0], 32, e.smem);
     if (occ < 1) occ = 1;
     const int resident_warps = std::max(nxw, h->sm_count * occ);
     const int nch = std::max(1, resident_warps / nxw);
@@ -420,10 +451,10 @@ int launch_tb(fluid_t* h, int K, bool scale, bool chained, JacobiArgs a, const T
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cudaLaunchConfig_t lc{};
-    lc.gridDim = dim3(nxw * nch); lc.blockDim = dim3(32); lc.stream = h->stream;   // one warp per CTA
+    lc.gridDim = dim3(nxw * nch, 1, h->members); lc.blockDim = dim3(32); lc.stream = h->stream;   // one warp per CTA
     lc.attrs = attr; lc.numAttrs = (chained && !h->capturing) ? 1 : 0;
     lc.dynamicSmemBytes = e.smem;
-    cudaLaunchKernelEx(&lc, e.kernel[scale], a, maps);
+    cudaLaunchKernelEx(&lc, h->batch ? e.batch[scale] : e.kernel[scale], a, maps);
     ++h->launches.jacobi;
     return check_launch(h, "jacobi_tb_kernel");
 }
@@ -464,7 +495,7 @@ int run_jacobi(fluid_t* h, int iters, bool scale_first, int* launches_out) {
     // clear pass alone (owned + ghost rows; ghosts are refreshed before use anyway).  Half storage always
     // clears in a launch of its own: the reference rounds the cleared field to fp16 before the first sweep.
     if (scale_first && (iters <= 0 || h->half)) {
-        const size_t n = sim_cells(h);
+        const size_t n = sim_cells(h) * h->members;
         int rc = with_storage(h, [&](auto s) {
             using S = decltype(s);
             scale_kernel<S><<<(unsigned)((n + 255) / 256), 256, 0, h->stream>>>(
@@ -480,7 +511,7 @@ int run_jacobi(fluid_t* h, int iters, bool scale_first, int* launches_out) {
         return FLUID_OK;
     }
     const int kb = block_depth(h, false);
-    const bool tb = blocked(h, kb);
+    const bool tb = h->batch || blocked(h, kb);          // a batch runs the blocked kernel at every depth, 1 included
     const JacobiPlan plan(iters, tb ? kb : 1);
     // Slab halos.  Communication-avoiding form (deep): ONE group per solve carries iters+1 rows of
     // pressure and iters rows of divergence; launch i then produces owned rows +- (sweeps still to
@@ -603,9 +634,9 @@ int adopt_arena(fluid_t* h, char* a, const FieldLayout& L) {
 }
 
 int alloc_fields(fluid_t* h) {
-    const FieldLayout L = field_layout(h, sim_cells(h), dye_cells(h));
+    const FieldLayout L = field_layout(h, sim_cells(h) * h->members, dye_cells(h) * h->members);
     char* a = nullptr;
-    int rc = make_arena(h, L, dye_cells(h), &a);
+    int rc = make_arena(h, L, dye_cells(h) * h->members, &a);
     return rc ? rc : adopt_arena(h, a, L);
 }
 
@@ -670,6 +701,12 @@ int not_on_slab(fluid_t* h, const char* what) {
                 "fluid_step / fluid_splat / fluid_pass_pressure_solve / fluid_pass_jacobi / read / write", what);
 }
 
+// what a batch handle refuses: everything but fluid_step, fluid_splats_batch, the config, field I/O and the stats
+int not_on_batch(fluid_t* h, const char* what) {
+    return fail(h, FLUID_ERR_INVALID, "%s does not take a batch handle; one supports fluid_step / fluid_splats_batch / "
+                "read / write / set_param / stat", what);
+}
+
 // Row ownership + ghost-zone heights of rank `rank` of `world` for a sim_h / dye_h grid (DESIGN.md §7).
 // Returns false when the slabs are too short for the minimum 14-row halo.
 bool slab_geometry(SlabGeometry* h, int rank, int world, int H, int Hd, int iters) {
@@ -696,8 +733,8 @@ bool slab_geometry(SlabGeometry* h, int rank, int world, int H, int Hd, int iter
     return true;
 }
 
-// shared by fluid_create and fluid_create_slab
-int create_common(const fluid_config* cfg, int rank, int world, const void* uid, fluid_t** out) {
+// shared by fluid_create, fluid_create_slab and fluid_create_batch (batch_members > 0, checked by the caller)
+int create_common(const fluid_config* cfg, int rank, int world, const void* uid, fluid_t** out, int batch_members = 0) {
     fluid_t* h = nullptr;
     if (!cfg || !out) return fail(h, FLUID_ERR_INVALID, "null argument");
     *out = nullptr;
@@ -727,6 +764,8 @@ int create_common(const fluid_config* cfg, int rank, int world, const void* uid,
     h->aspect_d = (cfg->aspect > 0.0f) ? (double)cfg->aspect : (double)cfg->sim_w / (double)cfg->sim_h;
     h->splat_radius_d = (double)cfg->splat_radius;
     h->rank = rank; h->world = world;
+    h->batch = batch_members > 0;
+    h->members = std::max(batch_members, 1);
     h->half = (cfg->flags & FLUID_FLAG_HALF_STORAGE) != 0;
     if (h->half && world > 1) {
         int rc = fail(nullptr, FLUID_ERR_INVALID, "FLUID_FLAG_HALF_STORAGE is a single-GPU mode");
@@ -822,6 +861,26 @@ const char* fluid_last_error(fluid_t* h) { return h ? h->err.c_str() : g_create_
 
 int fluid_create(const fluid_config* cfg, fluid_t** out) { return create_common(cfg, 0, 1, nullptr, out); }
 
+// B simulations of cfg's size and config in one handle.  The step kernels take the member as blockIdx.z,
+// whose grid extent caps B at FLUID_MAX_MEMBERS; they exist for power-of-two grids at least 128 columns wide
+// (the 4-cell advection) and 2 rows high (the blocked Jacobi kernel), in fp32 storage with the MANUAL
+// advection filter, so every flag that would pick another kernel is refused.
+int fluid_create_batch(const fluid_config* cfg, int members, fluid_t** out) {
+    if (!cfg || !out) return fail(nullptr, FLUID_ERR_INVALID, "null argument");
+    *out = nullptr;
+    if (members < 1 || members > FLUID_MAX_MEMBERS)
+        return fail(nullptr, FLUID_ERR_INVALID, "a batch holds 1 to %d members, not %d", FLUID_MAX_MEMBERS, members);
+    if (cfg->flags & ~(uint32_t)FLUID_FLAG_NO_GRAPH)
+        return fail(nullptr, FLUID_ERR_INVALID, "a batch handle takes no flag but FLUID_FLAG_NO_GRAPH (got 0x%x)", cfg->flags);
+    if (!is_pow2(cfg->sim_w) || !is_pow2(cfg->sim_h) || !is_pow2(cfg->dye_w) || !is_pow2(cfg->dye_h) ||
+        cfg->sim_w < 128 || cfg->dye_w < 128 || cfg->sim_h < 2 || cfg->dye_h < 2)
+        return fail(nullptr, FLUID_ERR_INVALID, "a batch needs power-of-two sizes, widths >= 128 and heights >= 2 "
+                    "(got %dx%d / %dx%d)", cfg->sim_w, cfg->sim_h, cfg->dye_w, cfg->dye_h);
+    return create_common(cfg, 0, 1, nullptr, out, members);
+}
+
+int fluid_members(fluid_t* h) { return h ? h->members : 0; }
+
 int fluid_nccl_unique_id(void* out_uid, size_t uid_bytes) {
     if (!out_uid || uid_bytes < sizeof(ncdl::ncclUniqueId)) return fail(nullptr, FLUID_ERR_INVALID, "uid buffer must hold 128 bytes");
     ncdl::Api& N = ncdl::api();
@@ -850,6 +909,7 @@ struct P2PBlob {            // what fluid_p2p_export hands to the launcher (opaq
 static_assert(sizeof(P2PBlob) == 256, "blob layout");
 
 int fluid_p2p_export(fluid_t* h, void* blob, size_t blob_bytes) {
+    if (h && h->batch) return not_on_batch(h, "fluid_p2p_export");
     if (!h || !blob || blob_bytes < sizeof(P2PBlob)) return fail(h, FLUID_ERR_INVALID, "blob must hold 256 bytes");
     if (!h->slab() || !h->arena) return fail(h, FLUID_ERR_INVALID, "fluid_p2p_export needs a slab handle");
     // halo_push_kernel moves rows as 16-byte words: every exchanged row (4*W pressure / divergence,
@@ -868,6 +928,7 @@ int fluid_p2p_export(fluid_t* h, void* blob, size_t blob_bytes) {
 // blob_below / blob_above: the 256-byte exports of rank-1 / rank+1 (NULL at the domain ends).
 // Collective in spirit: every rank of the slab group must connect before the next fluid_step.
 int fluid_p2p_connect(fluid_t* h, const void* blob_below, const void* blob_above) {
+    if (h && h->batch) return not_on_batch(h, "fluid_p2p_connect");
     if (!h || !h->slab() || !h->arena) return fail(h, FLUID_ERR_INVALID, "fluid_p2p_connect needs a slab handle");
     const void* blobs[2] = {blob_below, blob_above};
     for (int side = 0; side < 2; ++side) {
@@ -888,6 +949,7 @@ int fluid_p2p_connect(fluid_t* h, const void* blob_below, const void* blob_above
 // that all ranks keep using the same one).
 int fluid_p2p_disable(fluid_t* h) {
     if (!h) return FLUID_ERR_INVALID;
+    if (h->batch) return not_on_batch(h, "fluid_p2p_disable");
     if (h->stream) CU(cudaStreamSynchronize(h->stream));
     close_peers(h);
     return FLUID_OK;
@@ -1004,14 +1066,15 @@ static int do_divergence(fluid_t* h, Grid g) {
     });
 }
 // rows per warp stream of the row-streaming kernels: one full wave of resident warps (`warps_per_sm`
-// from the occupancy calculator), at least `rmin` rows each so that the halo rows a stream re-reads
-// stay a bounded fraction.  Grids too small to give every SM a warp use the tiled kernels instead.
+// from the occupancy calculator) across all members, at least `rmin` rows each so that the halo rows a
+// stream re-reads stay a bounded fraction.  Grids too small to give every SM a warp use the tiled kernels
+// instead, except on a batch handle, which always streams: its kernels have a member axis, the tiled ones do not.
 static StreamArgs stream_args(const fluid_t* h, Grid g, int cols_per_window, int rmin, int warps_per_sm, int round_to) {
     StreamArgs a{};
     a.g = g;
     a.nxw = (g.W + cols_per_window - 1) / cols_per_window;
     const int rows = g.j_hi - g.j_lo;
-    const int chunks = std::max(1, h->sm_count * warps_per_sm / a.nxw);
+    const int chunks = std::max(1, h->sm_count * warps_per_sm / (a.nxw * h->members));
     int r = std::max((rows + chunks - 1) / chunks, rmin);
     r = (r + round_to - 1) / round_to * round_to;
     a.rows_per_chunk = std::min(r, std::max(rows, 1));
@@ -1037,13 +1100,15 @@ static int do_cvd(fluid_t* h, Grid g) {
     static int cvd_occ = 0;
     if (!cvd_occ) {
         int blocks = 0;
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, cvd_stream_kernel, 32 * CVD2_WARPS, CVD2_SMEM);
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, cvd_stream_kernel<false>, 32 * CVD2_WARPS, CVD2_SMEM);
         cvd_occ = std::max(1, blocks) * CVD2_WARPS;
     }
     const StreamArgs a = stream_args(h, g, CVD2_VALID, 16, cvd_occ, 1);
     const int nwarps = stream_warps(a);
-    if (streaming_ok(h) && nwarps >= h->sm_count) {
-        cvd_stream_kernel<<<(nwarps + CVD2_WARPS - 1) / CVD2_WARPS, 32 * CVD2_WARPS, CVD2_SMEM, h->stream>>>(
+    if (h->batch || (streaming_ok(h) && nwarps >= h->sm_count)) {
+        const dim3 grid((nwarps + CVD2_WARPS - 1) / CVD2_WARPS, 1, h->members);
+        auto* k = h->batch ? cvd_stream_kernel<true> : cvd_stream_kernel<false>;
+        k<<<grid, 32 * CVD2_WARPS, CVD2_SMEM, h->stream>>>(
             (const float2*)h->velocity.read, h->curl, (float2*)h->velocity.write, h->divergence, a, h->cfg.curl,
             h->dt_dev, h->tiny_map);
         int rc = check_launch(h, "cvd_stream_kernel"); if (rc) return rc;
@@ -1063,8 +1128,10 @@ static int do_cvd(fluid_t* h, Grid g) {
 static int do_gradient(fluid_t* h, Grid g) {
     const StreamArgs a = stream_args(h, g, 128, 8, 32, GS_U);
     const int nwarps = stream_warps(a);
-    if (streaming_ok(h) && nwarps >= h->sm_count) {
-        gradient_stream_kernel<<<(nwarps + GS_WARPS - 1) / GS_WARPS, 32 * GS_WARPS, 0, h->stream>>>(
+    if (h->batch || (streaming_ok(h) && nwarps >= h->sm_count)) {
+        const dim3 grid((nwarps + GS_WARPS - 1) / GS_WARPS, 1, h->members);
+        auto* k = h->batch ? gradient_stream_kernel<true> : gradient_stream_kernel<false>;
+        k<<<grid, 32 * GS_WARPS, 0, h->stream>>>(
             (const float*)h->pressure.read, (const float2*)h->velocity.read, (float2*)h->velocity.write, a);
         int rc = check_launch(h, "gradient_stream_kernel"); if (rc) return rc;
         ++h->launches.gradient_stream;
@@ -1096,9 +1163,10 @@ static int do_advect_velocity(fluid_t* h, Grid out) {
     const bool p2 = is_pow2(h->cfg.sim_w) && is_pow2(h->cfg.sim_h);
     int rc = with_filter(h, [&](auto f) {
         using F = decltype(f);
-        if (advect4_runs(h, p2, out.W)) {    // 4 cells per thread, 32 apart
-            auto* k = h->slab() ? advect_velocity4_kernel<true> : advect_velocity4_kernel<false, F>;
-            k<<<dim3(out.W / 128, (out.j_hi - out.j_lo + 7) / 8), dim3(32, 8), 0, h->stream>>>(
+        if (advect4_runs(h, p2, out.W)) {    // 4 cells per thread, 32 apart; a batch handle's members along z
+            auto* k = h->slab()  ? advect_velocity4_kernel<true>
+                    : h->batch ? advect_velocity4_kernel<false, F, true> : advect_velocity4_kernel<false, F>;
+            k<<<dim3(out.W / 128, (out.j_hi - out.j_lo + 7) / 8, h->members), dim3(32, 8), 0, h->stream>>>(
                 (const float2*)h->velocity.read, (float2*)h->velocity.write, a);
             ++h->launches.advect4;
         } else with_storage(h, [&](auto s) {
@@ -1129,10 +1197,11 @@ static int do_advect_dye(fluid_t* h) {
     int rc = with_filter(h, [&](auto f) {
         using F = decltype(f);
         constexpr bool own = F::kOwnTexel;
-        if (advect4_runs(h, p2, out.W)) {    // 4 cells per thread, 32 apart
-            auto* k = h->slab() ? (same ? advect_dye4_kernel<true, true> : advect_dye4_kernel<false, true>)
-                                : (same ? advect_dye4_kernel<own, false, F> : advect_dye4_kernel<false, false, F>);
-            k<<<dim3(out.W / 128, (out.j_hi - out.j_lo + 7) / 8), dim3(32, 8), 0, h->stream>>>(
+        if (advect4_runs(h, p2, out.W)) {    // 4 cells per thread, 32 apart; a batch handle's members along z
+            auto* k = h->slab()  ? (same ? advect_dye4_kernel<true, true> : advect_dye4_kernel<false, true>)
+                    : h->batch ? (same ? advect_dye4_kernel<own, false, F, true> : advect_dye4_kernel<false, false, F, true>)
+                               : (same ? advect_dye4_kernel<own, false, F> : advect_dye4_kernel<false, false, F>);
+            k<<<dim3(out.W / 128, (out.j_hi - out.j_lo + 7) / 8, h->members), dim3(32, 8), 0, h->stream>>>(
                 (const float2*)h->velocity.read, (const float4*)h->dye.read, (float4*)h->dye.write, a);
             ++h->launches.advect4;
         } else with_storage(h, [&](auto s) {
@@ -1153,52 +1222,62 @@ static int do_advect_dye(fluid_t* h) {
 
 int fluid_pass_curl(fluid_t* h) {
     if (!h) return FLUID_ERR_INVALID;
+    if (h->batch) return not_on_batch(h, "fluid_pass_curl");
     if (h->slab()) return not_on_slab(h, "fluid_pass_curl");
     return do_curl(h, sim_grid(h));
 }
 int fluid_pass_vorticity(fluid_t* h, float dt) {
     if (!h) return FLUID_ERR_INVALID;
+    if (h->batch) return not_on_batch(h, "fluid_pass_vorticity");
     if (h->slab()) return not_on_slab(h, "fluid_pass_vorticity");
     int rc = set_dt(h, dt); if (rc) return rc;
     return do_vorticity(h, sim_grid(h));
 }
 int fluid_pass_divergence(fluid_t* h) {
     if (!h) return FLUID_ERR_INVALID;
+    if (h->batch) return not_on_batch(h, "fluid_pass_divergence");
     if (h->slab()) return not_on_slab(h, "fluid_pass_divergence");
     return do_divergence(h, sim_grid(h));
 }
 int fluid_pass_curl_vorticity_divergence(fluid_t* h, float dt) {
     if (!h) return FLUID_ERR_INVALID;
+    if (h->batch) return not_on_batch(h, "fluid_pass_curl_vorticity_divergence");
     if (h->slab()) return not_on_slab(h, "fluid_pass_curl_vorticity_divergence");
     int rc = set_dt(h, dt); if (rc) return rc;
     return do_cvd(h, sim_grid(h));
 }
 int fluid_pass_clear_pressure(fluid_t* h) {
     if (!h) return FLUID_ERR_INVALID;
+    if (h->batch) return not_on_batch(h, "fluid_pass_clear_pressure");
     return run_jacobi(h, 0, true, nullptr);
 }
 int fluid_pass_jacobi(fluid_t* h, int iters) {
     if (!h) return FLUID_ERR_INVALID;
+    if (h->batch) return not_on_batch(h, "fluid_pass_jacobi");
     if (iters < 0) return fail(h, FLUID_ERR_INVALID, "iters < 0");
     return run_jacobi(h, iters, false, nullptr);
 }
 int fluid_pass_pressure_solve(fluid_t* h) {
     if (!h) return FLUID_ERR_INVALID;
+    if (h->batch) return not_on_batch(h, "fluid_pass_pressure_solve");
     return run_jacobi(h, h->cfg.pressure_iterations, true, nullptr);
 }
 int fluid_pass_gradient_subtract(fluid_t* h) {
     if (!h) return FLUID_ERR_INVALID;
+    if (h->batch) return not_on_batch(h, "fluid_pass_gradient_subtract");
     if (h->slab()) return not_on_slab(h, "fluid_pass_gradient_subtract");
     return do_gradient(h, sim_grid(h));
 }
 int fluid_pass_advect_velocity(fluid_t* h, float dt) {
     if (!h) return FLUID_ERR_INVALID;
+    if (h->batch) return not_on_batch(h, "fluid_pass_advect_velocity");
     if (h->slab()) return not_on_slab(h, "fluid_pass_advect_velocity");
     int rc = set_dt(h, dt); if (rc) return rc;
     return do_advect_velocity(h, sim_grid(h));
 }
 int fluid_pass_advect_dye(fluid_t* h, float dt) {
     if (!h) return FLUID_ERR_INVALID;
+    if (h->batch) return not_on_batch(h, "fluid_pass_advect_dye");
     if (h->slab()) return not_on_slab(h, "fluid_pass_advect_dye");
     int rc = set_dt(h, dt); if (rc) return rc;
     return do_advect_dye(h);
@@ -1260,9 +1339,9 @@ int fluid_step(fluid_t* h, float dt) {
     if (no_graph || h->slab()) return step_enqueue(h, no_graph);
     char key[256];
     const fluid_config& c = h->cfg;
-    snprintf(key, sizeof key, "%a|%a|%a|%a|%d|%d|%u|%d%d%d|%dx%d|%dx%d",
+    snprintf(key, sizeof key, "%a|%a|%a|%a|%d|%d|%u|%d%d%d|%dx%d|%dx%d|%d",
              c.curl, c.pressure, c.velocity_dissipation, c.density_dissipation, c.pressure_iterations, c.jacobi_block,
-             c.flags, h->velocity.par, h->pressure.par, h->dye.par, c.sim_w, c.sim_h, c.dye_w, c.dye_h);
+             c.flags, h->velocity.par, h->pressure.par, h->dye.par, c.sim_w, c.sim_h, c.dye_w, c.dye_h, h->members);
     auto it = h->graphs.find(key);
     if (it == h->graphs.end()) {
         if (h->graphs.size() > 64) drop_graphs(h);          // config sliders dragged for a long time: stay bounded
@@ -1310,19 +1389,26 @@ static SplatPlane splat_plane(const Grid& g) {
 }
 static int splat_blocks(const SplatPlane& p) { return p.bx * ((p.g.j_hi - p.g.j_lo + SPL_BH - 1) / SPL_BH); }
 
-// n x splat(x,y,dx,dy,color) of S:1441-1455, in order, SPLATS_PER_LAUNCH records per launch
-int fluid_splats(fluid_t* h, const float* splats, int n) {
-    if (!h) return FLUID_ERR_INVALID;
-    if (n < 0 || (n > 0 && !splats)) return fail(h, FLUID_ERR_INVALID, "fluid_splats: bad record block (%d records at %p)", n, (const void*)splats);
-    if (n == 0) return FLUID_OK;
-    static_assert(sizeof(SplatRec) == 7 * sizeof(float), "records are 7 packed floats");
-    static_assert(sizeof(SplatsArgs) <= 4096, "the records travel in the 4 KB kernel parameter block");
+// what every splat launch shares: correctRadius(config.SPLAT_RADIUS / 100.0), JS double arithmetic narrowed
+// by gl.uniform1f, and the aspect
+static SplatsArgs splats_args(const fluid_t* h) {
     SplatsArgs a{};
-    // correctRadius(config.SPLAT_RADIUS / 100.0): JS double arithmetic, narrowed by gl.uniform1f
     double rad = h->splat_radius_d / 100.0;
     if (h->aspect_d > 1.0) rad *= h->aspect_d;
     a.radius = (float)rad;
     a.aspect = h->cfg.aspect;
+    return a;
+}
+
+// n x splat(x,y,dx,dy,color) of S:1441-1455, in order, SPLATS_PER_LAUNCH records per launch
+int fluid_splats(fluid_t* h, const float* splats, int n) {
+    if (!h) return FLUID_ERR_INVALID;
+    if (h->batch) return not_on_batch(h, "fluid_splats");
+    if (n < 0 || (n > 0 && !splats)) return fail(h, FLUID_ERR_INVALID, "fluid_splats: bad record block (%d records at %p)", n, (const void*)splats);
+    if (n == 0) return FLUID_OK;
+    static_assert(sizeof(SplatRec) == 7 * sizeof(float), "records are 7 packed floats");
+    static_assert(sizeof(SplatsArgs) <= 4096, "the records travel in the 4 KB kernel parameter block");
+    SplatsArgs a = splats_args(h);
     // a splat is point-wise, so the +-3 velocity ghost rows of a slab are simply splatted as well
     a.v = splat_plane(sim_grid_ext(h, h->slab() ? 3 : 0));
     a.d = splat_plane(dye_grid(h));
@@ -1347,6 +1433,48 @@ int fluid_splats(fluid_t* h, const float* splats, int n) {
     return FLUID_OK;
 }
 
+// Record k to member[k] of a batch handle.  The records are ordered by member (stably: each member keeps
+// the call order) and cut into launches of at most SPLATS_PER_LAUNCH records in SPLAT_GROUPS member groups.
+// Each launch updates its members' .read in place and launches no block for any other member: a splat is
+// point-wise, so the bits are those of fluid_splats' read-write-swap on an ordinary handle.
+int fluid_splats_batch(fluid_t* h, const int32_t* member, const float* splats, int n) {
+    if (!h) return FLUID_ERR_INVALID;
+    if (!h->batch) return fail(h, FLUID_ERR_INVALID, "fluid_splats_batch needs a batch handle (fluid_create_batch)");
+    if (n < 0 || (n > 0 && (!member || !splats)))
+        return fail(h, FLUID_ERR_INVALID, "fluid_splats_batch: bad record block (%d records)", n);
+    for (int k = 0; k < n; ++k)
+        if (member[k] < 0 || member[k] >= h->members)
+            return fail(h, FLUID_ERR_INVALID, "fluid_splats_batch: record %d names member %d of %d", k, member[k], h->members);
+    if (n == 0) return FLUID_OK;
+    std::vector<int> order(n);
+    for (int k = 0; k < n; ++k) order[k] = k;
+    std::stable_sort(order.begin(), order.end(), [&](int x, int y) { return member[x] < member[y]; });
+    SplatsArgs a = splats_args(h);
+    a.v = splat_plane(sim_grid(h));
+    a.d = splat_plane(dye_grid(h));
+    a.blocks_v = splat_blocks(a.v);
+    const int blocks = a.blocks_v + splat_blocks(a.d);
+    SplatGroups g{};
+    int ng = 0;
+    a.n = 0;
+    auto flush = [&]() {
+        g.start[ng] = (unsigned char)a.n;
+        splats_batch_kernel<<<dim3(blocks, ng), 256, 0, h->stream>>>((float2*)h->velocity.read, (float4*)h->dye.read, a, g);
+        a.n = 0; ng = 0;
+        return check_launch(h, "splats_batch_kernel");
+    };
+    for (int k = 0; k < n; ++k) {
+        const int r = order[k], m = member[r];
+        const bool new_group = ng == 0 || g.member[ng - 1] != m;
+        if (a.n == SPLATS_PER_LAUNCH || (new_group && ng == SPLAT_GROUPS)) {
+            if (int rc = flush()) return rc;
+        }
+        if (ng == 0 || g.member[ng - 1] != m) { g.member[ng] = m; g.start[ng] = (unsigned char)a.n; ++ng; }
+        memcpy(&a.rec[a.n++], splats + 7 * (size_t)r, sizeof(SplatRec));
+    }
+    return flush();
+}
+
 // splat(x,y,dx,dy,color), S:1441-1455
 int fluid_splat(fluid_t* h, float x, float y, float dx, float dy, float r, float g, float b) {
     const float rec[7] = {x, y, dx, dy, r, g, b};
@@ -1356,6 +1484,7 @@ int fluid_splat(fluid_t* h, float x, float y, float dx, float dy, float r, float
 // initFramebuffers() on a live simulation: S:982-1010 + resizeDoubleFBO S:1116-1126
 int fluid_resize(fluid_t* h, int sim_w, int sim_h, int dye_w, int dye_h) {
     if (!h) return FLUID_ERR_INVALID;
+    if (h->batch) return not_on_batch(h, "fluid_resize");
     if (sim_w < 1 || sim_h < 1 || dye_w < 1 || dye_h < 1) return fail(h, FLUID_ERR_INVALID, "bad size");
     const int ow = h->cfg.sim_w, oh = h->cfg.sim_h, odw = h->cfg.dye_w, odh = h->cfg.dye_h;
     int rc;
@@ -1401,10 +1530,11 @@ int fluid_resize(fluid_t* h, int sim_w, int sim_h, int dye_w, int dye_h) {
 
 // ---- data in / out --------------------------------------------------------------------------------
 
+// a batch handle's fields hold all members: B x w x rows x channels floats
 size_t fluid_field_elems(fluid_t* h, int field) {
     void* p; int w, rows, ch;
     if (!h || field_info(h, field, &p, &w, &rows, &ch)) return 0;
-    return (size_t)w * rows * ch;
+    return (size_t)w * rows * ch * h->members;
 }
 
 int fluid_field_dims(fluid_t* h, int field, int* w, int* rows, int* ch, int* row0) {
@@ -1418,7 +1548,7 @@ int fluid_field_dims(fluid_t* h, int field, int* w, int* rows, int* ch, int* row
 int fluid_read(fluid_t* h, int field, float* host, size_t n_floats) {
     void* p; int w, rows, ch;
     if (!h || !host || field_info(h, field, &p, &w, &rows, &ch)) return fail(h, FLUID_ERR_INVALID, "bad field %d", field);
-    const size_t n = (size_t)w * rows * ch;
+    const size_t n = (size_t)w * rows * ch * h->members;
     if (n_floats != n) return fail(h, FLUID_ERR_INVALID, "field %d has %zu floats, caller passed %zu", field, n, n_floats);
     if (h->half) {                                   // the ABI speaks fp32: widen on the device, then copy
         int rc = need_scratch(h, n); if (rc) return rc;
@@ -1434,7 +1564,7 @@ int fluid_read(fluid_t* h, int field, float* host, size_t n_floats) {
 int fluid_write(fluid_t* h, int field, const float* host, size_t n_floats) {
     void* p; int w, rows, ch;
     if (!h || !host || field_info(h, field, &p, &w, &rows, &ch)) return fail(h, FLUID_ERR_INVALID, "bad field %d", field);
-    const size_t n = (size_t)w * rows * ch;
+    const size_t n = (size_t)w * rows * ch * h->members;
     if (n_floats != n) return fail(h, FLUID_ERR_INVALID, "field %d has %zu floats, caller passed %zu", field, n, n_floats);
     if (h->half) {                                   // narrow with round-to-nearest-even, like a texture upload would
         int rc = need_scratch(h, n); if (rc) return rc;
@@ -1479,7 +1609,7 @@ static int device_io_args(fluid_t* h, const char* what, int field, const void* b
     int w, rows, ch;
     if (!h) return FLUID_ERR_INVALID;
     if (field_info(h, field, p, &w, &rows, &ch)) return fail(h, FLUID_ERR_INVALID, "%s: bad field %d", what, field);
-    *n = (size_t)w * rows * ch;
+    *n = (size_t)w * rows * ch * h->members;
     if (n_floats != *n) return fail(h, FLUID_ERR_INVALID, "%s: field %d has %zu floats, caller passed %zu", what, field, *n, n_floats);
     if (!buf) return fail(h, FLUID_ERR_INVALID, "%s: NULL buffer", what);
     if (h->slab()) return not_on_slab(h, what);
@@ -1602,6 +1732,7 @@ int solve_host_banded(fluid_t* h, const float* div_host, float* p_host, int iter
 }
 
 int fluid_pressure_solve_host(fluid_t* h, const float* div_host, float* p_host, int iters) {
+    if (h && h->batch) return not_on_batch(h, "fluid_pressure_solve_host");
     if (!h || !div_host || !p_host || iters < 0) return fail(h, FLUID_ERR_INVALID, "bad argument");
     if (h->half) {
         int rc = fluid_write(h, FLUID_FIELD_DIVERGENCE, div_host, (size_t)h->cfg.sim_w * h->cfg.sim_h);
@@ -1632,6 +1763,7 @@ int fluid_pressure_solve_host(fluid_t* h, const float* div_host, float* p_host, 
 // The band of a width x height target this handle draws: the whole target on one GPU, rows
 // [height*rank/world, height*(rank+1)/world) on a slab rank (the same fractions as the dye rows it owns).
 int fluid_render_band(fluid_t* h, int height, int* y0, int* y1) {
+    if (h && h->batch) return not_on_batch(h, "fluid_render_band");
     if (!h || height < 1 || !y0 || !y1) return FLUID_ERR_INVALID;
     *y0 = (int)((long long)height * h->rank / h->world);
     *y1 = (int)((long long)height * (h->rank + 1) / h->world);
@@ -1865,6 +1997,7 @@ struct DrawRequest {
 // chains read the fp16 dye directly and draw the mask into the fp16 dye.write.
 static int draw(fluid_t* h, const DrawRequest& r) {
     if (!h) return FLUID_ERR_INVALID;
+    if (h->batch) return not_on_batch(h, r.what);
     if (r.keywords & ~(uint32_t)(FLUID_DISPLAY_SHADING | FLUID_DISPLAY_BLOOM | FLUID_DISPLAY_SUNRAYS))
         return fail(h, FLUID_ERR_INVALID, "unknown display keyword bits 0x%x", r.keywords);
     const bool bloom_on = r.keywords & FLUID_DISPLAY_BLOOM, sun_on = r.keywords & FLUID_DISPLAY_SUNRAYS;

@@ -196,6 +196,18 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const void* tmap, in
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
                  ::"r"(smem_u32(smem_dst)), "l"(tmap), "r"(x), "r"(y), "r"(smem_u32(bar)) : "memory");
 }
+// the box of member m of a batch handle's (W, H, B) tensor map, one member deep: rows past the member's
+// first or last read as zero, exactly like rows past a single handle's 2-D map
+__device__ __forceinline__ void tma_load_3d(void* smem_dst, const void* tmap, int x, int y, int m, void* bar) {
+    asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
+                 ::"r"(smem_u32(smem_dst)), "l"(tmap), "r"(x), "r"(y), "r"(m), "r"(smem_u32(bar)) : "memory");
+}
+// BATCH: blockIdx.z is the member
+template <bool BATCH>
+__device__ __forceinline__ void tma_load_box(void* smem_dst, const void* tmap, int x, int y, void* bar) {
+    if constexpr (BATCH) tma_load_3d(smem_dst, tmap, x, y, (int)blockIdx.z, bar);
+    else tma_load_2d(smem_dst, tmap, x, y, bar);
+}
 __device__ __forceinline__ void mbar_inval(void* bar) {
     asm volatile("mbarrier.inval.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
@@ -298,7 +310,7 @@ struct TBTma {           // warp-uniform TMA bookkeeping
 //     of the previous block's, which is refilled only at the end of this block), so lanes 0 and 31
 //     read that row's column x0-1 / x0+128 through `ering` instead of keeping it in a register;
 //   * a contracted block folds the magnitudes of its level-0 inputs into `big` (BIG_IN above).
-template <int K, bool SCALE, bool EDGE, bool REV, bool EXACT>
+template <int K, bool SCALE, bool EDGE, bool REV, bool EXACT, bool BATCH>
 __device__ __forceinline__ void tb_block(float4 (&w)[K][3], float4 (&dr)[TB<K>::RD], TBStream& st, float& big,
                                          const float4* __restrict__ ring, const float* __restrict__ ering,
                                          const TBTma& tm, const int W4,
@@ -372,15 +384,15 @@ __device__ __forceinline__ void tb_block(float4 (&w)[K][3], float4 (&dr)[TB<K>::
         const int q = (st.stg == 0) ? T::NS - 1 : st.stg - 1;
         float4* dst = tm.slots + q * T::STAGE4;
         mbar_expect_tx(tm.bars + q, (unsigned)T::TX);
-        tma_load_2d(dst, tm.tm_d, tm.x0 - 4, st.yfill, tm.bars + q);
-        tma_load_2d(dst + T::P4, tm.tm_p, tm.x0 - 4, st.yfill, tm.bars + q);
+        tma_load_box<BATCH>(dst, tm.tm_d, tm.x0 - 4, st.yfill, tm.bars + q);
+        tma_load_box<BATCH>(dst + T::P4, tm.tm_p, tm.x0 - 4, st.yfill, tm.bars + q);
     }
     st.yfill += 3;
     if (st.stg + 1 == T::NS) { st.stg = 0; st.phase ^= 1u; } else { ++st.stg; }
 }
 
 // returns this lane's largest level-0 magnitude (0 for an EXACT stream)
-template <int K, bool SCALE, bool REV, bool EXACT>
+template <int K, bool SCALE, bool REV, bool EXACT, bool BATCH>
 __device__ __forceinline__ float tb_stream(const JacobiArgs& a, const void* tm_p, const void* tm_d,
                                           float4* __restrict__ smem4, const int lane, const int x0,
                                           const int lc, const int gx, const bool rev,
@@ -446,8 +458,8 @@ __device__ __forceinline__ float tb_stream(const JacobiArgs& a, const void* tm_p
         if (lane == 0) {
             float4* dst = tm.slots + q * T::STAGE4;
             mbar_expect_tx(tm.bars + q, (unsigned)T::TX);
-            tma_load_2d(dst, tm_d, x0 - 4, st.yfill, tm.bars + q);
-            tma_load_2d(dst + T::P4, tm_p, x0 - 4, st.yfill, tm.bars + q);
+            tma_load_box<BATCH>(dst, tm_d, x0 - 4, st.yfill, tm.bars + q);
+            tma_load_box<BATCH>(dst + T::P4, tm_p, x0 - 4, st.yfill, tm.bars + q);
         }
         st.yfill += 3;
     }
@@ -464,10 +476,10 @@ __device__ __forceinline__ float tb_stream(const JacobiArgs& a, const void* tm_p
     while (s0 < nsteps) {                             // at most: wall blocks, steady blocks, wall blocks
 #pragma unroll 1
         for (; s0 < nsteps && ((ys + s0 - K <= 0) || (ys + s0 + 2 >= H - 1)); s0 += 3)
-            tb_block<K, SCALE, true, REV, EXACT>(w, dr, st, big, ring, ering, tm, W4, y0, y1, H, rev, lane_out, a.scale);
+            tb_block<K, SCALE, true, REV, EXACT, BATCH>(w, dr, st, big, ring, ering, tm, W4, y0, y1, H, rev, lane_out, a.scale);
 #pragma unroll 1
         for (; s0 < nsteps && !((ys + s0 - K <= 0) || (ys + s0 + 2 >= H - 1)); s0 += 3)
-            tb_block<K, SCALE, false, REV, EXACT>(w, dr, st, big, ring, ering, tm, W4, y0, y1, H, rev, lane_out, a.scale);
+            tb_block<K, SCALE, false, REV, EXACT, BATCH>(w, dr, st, big, ring, ering, tm, W4, y0, y1, H, rev, lane_out, a.scale);
     }
     // drain the over-fetched tail before the CTA (and its shared memory) goes away
 #pragma unroll
@@ -478,14 +490,14 @@ __device__ __forceinline__ float tb_stream(const JacobiArgs& a, const void* tm_p
     return big;
 }
 
-template <int K, bool SCALE>
+template <int K, bool SCALE, bool BATCH>
 __device__ __noinline__ void tb_stream_exact(const JacobiArgs& a, const void* tm_p, const void* tm_d,
                                              float4* __restrict__ smem4, const int lane, const int x0,
                                              const int lc, const int gx, const bool rev, const bool lane_out,
                                              const int y0, const int y1, const int ys, const bool any_rev) {
     if (lane == 0 && a.exact_streams) atomicAdd(a.exact_streams, 1ull);
-    if (any_rev) tb_stream<K, SCALE, true, true>(a, tm_p, tm_d, smem4, lane, x0, lc, gx, rev, lane_out, y0, y1, ys);
-    else tb_stream<K, SCALE, false, true>(a, tm_p, tm_d, smem4, lane, x0, lc, gx, rev, lane_out, y0, y1, ys);
+    if (any_rev) tb_stream<K, SCALE, true, true, BATCH>(a, tm_p, tm_d, smem4, lane, x0, lc, gx, rev, lane_out, y0, y1, ys);
+    else tb_stream<K, SCALE, false, true, BATCH>(a, tm_p, tm_d, smem4, lane, x0, lc, gx, rev, lane_out, y0, y1, ys);
 }
 
 // One warp per CTA: every quantity that steers control flow derives from blockIdx and kernel
@@ -499,9 +511,15 @@ __device__ __noinline__ void tb_stream_exact(const JacobiArgs& a, const void* tm
 #else
 #define FLUID_TB_BOUNDS __launch_bounds__(32, FLUID_TB_MINBLOCKS)
 #endif
-template <int K, bool SCALE>
+// BATCH: a batch handle's launch, blockIdx.z the member.  The maps are 3-D (W, H, B); pout and the tiny map
+// move to the member's array and map region.
+template <int K, bool SCALE, bool BATCH = false>
 __global__ void FLUID_TB_BOUNDS jacobi_tb_kernel(JacobiArgs a, const __grid_constant__ TmapPair maps) {
     using T = TB<K>;
+    if constexpr (BATCH) {
+        a.pout += (size_t)blockIdx.z * a.W * a.H;
+        if (a.tiny_map) a.tiny_map += (size_t)blockIdx.z * tiny_map_w(a.W) * tiny_map_h(a.H);
+    }
     extern __shared__ __align__(128) float4 smem4[];
     // Programmatic dependent launch: back-to-back blocked launches of one solve are chained with
     // cudaLaunchAttributeProgrammaticStreamSerialization, so the NEXT launch's CTAs are already
@@ -555,7 +573,7 @@ __global__ void FLUID_TB_BOUNDS jacobi_tb_kernel(JacobiArgs a, const __grid_cons
     // an SM whose resident warps ran two separate steady-state loops would keep two loop bodies in its
     // instruction cache, and a loop body twice as large measured 11 % slower (DESIGN §5.8).
     if (!exact) {
-        const float big = tb_stream<K, SCALE, true, false>(a, tp, td, smem4, lane, x0, lc, gx, rev, lane_out, y0, y1, ys);
+        const float big = tb_stream<K, SCALE, true, false, BATCH>(a, tp, td, smem4, lane, x0, lc, gx, rev, lane_out, y0, y1, ys);
         // an input that could make S - d overflow within this launch: solve the stream again with the exact
         // tail.  It stores the same rows, nobody else reads pout before the grid ends (pin != pout), and its
         // stages were drained, so the barriers are retired and made afresh
@@ -567,7 +585,7 @@ __global__ void FLUID_TB_BOUNDS jacobi_tb_kernel(JacobiArgs a, const __grid_cons
         __syncwarp();
         if (!exact) return;
     }
-    tb_stream_exact<K, SCALE>(a, tp, td, smem4, lane, x0, lc, gx, rev, lane_out, y0, y1, ys, any_rev);
+    tb_stream_exact<K, SCALE, BATCH>(a, tp, td, smem4, lane, x0, lc, gx, rev, lane_out, y0, y1, ys, any_rev);
 }
 
 // ---- producers of the tiny-divergence map ----------------------------------------------------------

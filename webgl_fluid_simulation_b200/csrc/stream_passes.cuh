@@ -34,9 +34,15 @@ __device__ __forceinline__ float4 ldg4(const float* p) { return __ldg(reinterpre
 // warp fetch their one missing neighbour with a scalar load (L1/L2 hit: the next warp streams it).
 constexpr int GS_WARPS = 4;
 constexpr int GS_U = 4;                                          // rows per software-pipeline group
+// BATCH: blockIdx.z is the member of a batch handle, whose fields are dense (B, H, W) arrays (one GPU)
+template <bool BATCH = false>
 __global__ void __launch_bounds__(32 * GS_WARPS) gradient_stream_kernel(const float* __restrict__ p,
                                                                        const float2* __restrict__ v,
                                                                        float2* __restrict__ vout, StreamArgs a) {
+    if constexpr (BATCH) {
+        const size_t mo = (size_t)blockIdx.z * a.g.W * a.g.H;
+        p += mo; v += mo; vout += mo;
+    }
     const int lane = threadIdx.x & 31;
     const int wid = blockIdx.x * GS_WARPS + (threadIdx.x >> 5);
     const int wx = wid % a.nxw, cy = wid / a.nxw;
@@ -246,12 +252,19 @@ __device__ __forceinline__ void cvd_step(Vel4 (&V)[3], float (&C)[3][4], Vel4 (&
     st.o_curl += W4; st.o_vel += 2 * W4; st.o_div += W4;
 }
 
+// BATCH: blockIdx.z is the member of a batch handle; each member flags its own region of the tiny map
+template <bool BATCH = false>
 __global__ void __launch_bounds__(32 * CVD2_WARPS, CVD2_MINBLOCKS) cvd_stream_kernel(const float2* __restrict__ v,
                                                                     float* __restrict__ curl,
                                                                     float2* __restrict__ vout,
                                                                     float* __restrict__ div, StreamArgs a,
                                                                     float curl_k, const float* __restrict__ dtp,
                                                                     unsigned char* __restrict__ tiny_map) {
+    if constexpr (BATCH) {
+        const size_t mo = (size_t)blockIdx.z * a.g.W * a.g.H;
+        v += mo; curl += mo; vout += mo; div += mo;
+        if (tiny_map) tiny_map += (size_t)blockIdx.z * tiny_map_w(a.g.W) * tiny_map_h(a.g.H);
+    }
     extern __shared__ __align__(16) float4 cvd_smem[];
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     const int wid = blockIdx.x * CVD2_WARPS + wib;

@@ -193,7 +193,116 @@ class _Field:
         return self._sim.readField(self._name)
 
 
-class FluidSimulation:
+class _Handle:
+    """What FluidSimulation and FluidBatch share: a library handle `_h`, the live `config` pushed before each
+    call, and the calls that take any handle."""
+
+    def _check(self, rc):
+        if rc != 0:
+            msg = self._L.fluid_last_error(self._h if self._h else None)
+            raise FluidError(rc, msg.decode() if msg else "")
+
+    def _aspect(self):
+        return self.canvas["width"] / self.canvas["height"]
+
+    def _config(self, sim_w, sim_h, dye_w, dye_h):
+        """The fluid_config of a new handle: the simulation keys as they stand now (a slab handle sizes its
+        ghost zone from PRESSURE_ITERATIONS); later changes are pushed live by _push_config()."""
+        cfg = Config()
+        self._L.fluid_config_default(C.byref(cfg))
+        cfg.sim_w, cfg.sim_h, cfg.dye_w, cfg.dye_h = sim_w, sim_h, dye_w, dye_h
+        cfg.aspect = self._aspect()
+        cfg.device, cfg.flags, cfg.jacobi_block = self._device, self._flags, self._jb
+        cfg.density_dissipation = float(self.config["DENSITY_DISSIPATION"])
+        cfg.velocity_dissipation = float(self.config["VELOCITY_DISSIPATION"])
+        cfg.pressure = float(self.config["PRESSURE"])
+        cfg.pressure_iterations = int(self.config["PRESSURE_ITERATIONS"])
+        cfg.curl = float(self.config["CURL"])
+        cfg.splat_radius = float(self.config["SPLAT_RADIUS"])
+        return cfg
+
+    def _push_config(self):
+        """The reference reads `config` live inside step()/splat(); mirror that by pushing every
+        changed scalar before the call."""
+        vals = {
+            "DENSITY_DISSIPATION": self.config["DENSITY_DISSIPATION"],
+            "VELOCITY_DISSIPATION": self.config["VELOCITY_DISSIPATION"],
+            "PRESSURE": self.config["PRESSURE"],
+            "PRESSURE_ITERATIONS": self.config["PRESSURE_ITERATIONS"],
+            "CURL": self.config["CURL"],
+            "SPLAT_RADIUS": self.config["SPLAT_RADIUS"],
+            "ASPECT": self._aspect(),
+        }
+        for k, v in vals.items():
+            if self._pushed.get(k) != v:
+                # JS numbers are doubles: SPLAT_RADIUS and the aspect enter double arithmetic in
+                # correctRadius (S:1457-1462) before the single fp32 narrowing of gl.uniform1f
+                self._check(self._L.fluid_set_param_f64(self._h, PARAM[k], float(v)))
+                self._pushed[k] = v
+
+    def _dims(self, name):
+        w, h, c, r0 = C.c_int(), C.c_int(), C.c_int(), C.c_int()
+        self._check(self._L.fluid_field_dims(self._h, FIELD[name], C.byref(w), C.byref(h), C.byref(c), C.byref(r0)))
+        return w.value, h.value, c.value, r0.value
+
+    def step(self, dt):
+        """step(dt), S:1231-1294."""
+        self._push_config()
+        self._check(self._L.fluid_step(self._h, float(dt)))
+
+    def sync(self):
+        self._check(self._L.fluid_sync(self._h))
+
+    def mark(self, slot):
+        self._check(self._L.fluid_mark(self._h, slot))
+
+    def elapsed_ms(self) -> float:
+        ms = C.c_float()
+        self._check(self._L.fluid_elapsed_ms(self._h, C.byref(ms)))
+        return ms.value
+
+    def timing(self) -> dict:
+        t = Timing()
+        self._check(self._L.fluid_timing_last(self._h, C.byref(t)))
+        return {k: getattr(t, k) for k, _ in Timing._fields_}
+
+    def launch_count(self) -> int:
+        return int(self._L.fluid_launch_count(self._h))
+
+    def stat(self, name) -> int:
+        """Library counters (fluid_stat): launches, jacobi_launches, halo_launches, halo_exchanges,
+        graph_captures, graph_launches, halo_transport_p2p, cvd_stream_launches and
+        gradient_stream_launches (how many curl-vorticity-divergence / gradientSubtract passes ran
+        the row-streaming kernel rather than the tiled one; graph replays included), and
+        jacobi_exact_streams (warps of the blocked Jacobi kernel that ran the un-contracted tail, for
+        tiny divergence or inputs near FLT_MAX; waits for the handle's queued work)."""
+        return int(self._L.fluid_stat(self._h, STAT[name]))
+
+    def device_ptr(self, name) -> int:
+        return int(self._L.fluid_device_ptr(self._h, FIELD[name]) or 0)
+
+    def set_param(self, key, value):
+        self._check(self._L.fluid_set_param(self._h, PARAM[key], float(value)))
+
+    def close(self):
+        if self._h:
+            self._L.fluid_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
+
+
+class FluidSimulation(_Handle):
     """The reference's simulation state and frame functions on one handle.  `flags` pick the device the
     reference runs on: FLAG_NEAREST_FILTERING is a device without float linear filtering (NEAREST display /
     post-FX / resize samplers, with its config override); FLAG_LINEAR_ADVECTION is a device with it, whose
@@ -229,39 +338,6 @@ class FluidSimulation:
         self.curl = _Field(self, "curl")
         self.initFramebuffers()
 
-    # ---- plumbing ----------------------------------------------------------------------------------
-    def _check(self, rc):
-        if rc != 0:
-            msg = self._L.fluid_last_error(self._h if self._h else None)
-            raise FluidError(rc, msg.decode() if msg else "")
-
-    def _aspect(self):
-        return self.canvas["width"] / self.canvas["height"]
-
-    def _push_config(self):
-        """The reference reads `config` live inside step()/splat(); mirror that by pushing every
-        changed scalar before the call."""
-        vals = {
-            "DENSITY_DISSIPATION": self.config["DENSITY_DISSIPATION"],
-            "VELOCITY_DISSIPATION": self.config["VELOCITY_DISSIPATION"],
-            "PRESSURE": self.config["PRESSURE"],
-            "PRESSURE_ITERATIONS": self.config["PRESSURE_ITERATIONS"],
-            "CURL": self.config["CURL"],
-            "SPLAT_RADIUS": self.config["SPLAT_RADIUS"],
-            "ASPECT": self._aspect(),
-        }
-        for k, v in vals.items():
-            if self._pushed.get(k) != v:
-                # JS numbers are doubles: SPLAT_RADIUS and the aspect enter double arithmetic in
-                # correctRadius (S:1457-1462) before the single fp32 narrowing of gl.uniform1f
-                self._check(self._L.fluid_set_param_f64(self._h, PARAM[k], float(v)))
-                self._pushed[k] = v
-
-    def _dims(self, name):
-        w, h, c, r0 = C.c_int(), C.c_int(), C.c_int(), C.c_int()
-        self._check(self._L.fluid_field_dims(self._h, FIELD[name], C.byref(w), C.byref(h), C.byref(c), C.byref(r0)))
-        return w.value, h.value, c.value, r0.value
-
     # ---- initFramebuffers, S:982-1010 --------------------------------------------------------------
     def initFramebuffers(self):
         simRes = getResolution(self.config["SIM_RESOLUTION"], self.canvas["width"], self.canvas["height"])
@@ -270,20 +346,7 @@ class FluidSimulation:
             simRes = {"width": self._sizes[0], "height": self._sizes[1]}
             dyeRes = {"width": self._sizes[2], "height": self._sizes[3]}
         if not self._h:                                  # `dye == null` branch: create
-            cfg = Config()
-            self._L.fluid_config_default(C.byref(cfg))
-            cfg.sim_w, cfg.sim_h = simRes["width"], simRes["height"]
-            cfg.dye_w, cfg.dye_h = dyeRes["width"], dyeRes["height"]
-            cfg.aspect = self._aspect()
-            cfg.device, cfg.flags, cfg.jacobi_block = self._device, self._flags, self._jb
-            # the simulation keys as they stand now (a slab handle sizes its ghost zone from
-            # PRESSURE_ITERATIONS); later changes are pushed live by _push_config()
-            cfg.density_dissipation = float(self.config["DENSITY_DISSIPATION"])
-            cfg.velocity_dissipation = float(self.config["VELOCITY_DISSIPATION"])
-            cfg.pressure = float(self.config["PRESSURE"])
-            cfg.pressure_iterations = int(self.config["PRESSURE_ITERATIONS"])
-            cfg.curl = float(self.config["CURL"])
-            cfg.splat_radius = float(self.config["SPLAT_RADIUS"])
+            cfg = self._config(simRes["width"], simRes["height"], dyeRes["width"], dyeRes["height"])
             if self._world > 1:
                 uid = C.create_string_buffer(self._uid, len(self._uid))
                 self._check(self._L.fluid_create_slab(C.byref(cfg), self._rank, self._world, uid,
@@ -300,12 +363,7 @@ class FluidSimulation:
         self._pushed = {}
         self._push_config()
 
-    # ---- the hot path ------------------------------------------------------------------------------
-    def step(self, dt):
-        """step(dt), S:1231-1294."""
-        self._push_config()
-        self._check(self._L.fluid_step(self._h, float(dt)))
-
+    # ---- the hot path (step(dt): _Handle) ------------------------------------------------------------
     def splat(self, x, y, dx, dy, color):
         """splat(x, y, dx, dy, color), S:1441-1455; color is {r,g,b} like the reference's."""
         self._push_config()
@@ -583,9 +641,6 @@ class FluidSimulation:
         img = (np.clip(rgba, 0.0, 1.0) * 255.0).astype(np.uint8)
         return img[::-1].copy()
 
-    def sync(self):
-        self._check(self._L.fluid_sync(self._h))
-
     # ---- per-pass entry points (test surface; one reference blit each) -------------------------------
     def pass_(self, name, *args):
         self._push_config()
@@ -599,53 +654,84 @@ class FluidSimulation:
         self._check(self._L.fluid_pressure_solve_host(self._h, div_host.ctypes.data_as(C.c_void_p),
                                                       p_host.ctypes.data_as(C.c_void_p), int(iters)))
 
-    def mark(self, slot):
-        self._check(self._L.fluid_mark(self._h, slot))
 
-    def elapsed_ms(self) -> float:
-        ms = C.c_float()
-        self._check(self._L.fluid_elapsed_ms(self._h, C.byref(ms)))
-        return ms.value
 
-    def timing(self) -> dict:
-        t = Timing()
-        self._check(self._L.fluid_timing_last(self._h, C.byref(t)))
-        return {k: getattr(t, k) for k, _ in Timing._fields_}
+class FluidBatch(_Handle):
+    """`members` independent simulations of one size and config in one handle (fluid_create_batch): step(),
+    splats(), readField() and writeField() act on all of them through the same kernel launches, and member m
+    holds the bits a FluidSimulation given member m's inputs would hold.  Sizes come from `sizes` (sim_w,
+    sim_h, dye_w, dye_h) or from getResolution of config SIM_RESOLUTION / DYE_RESOLUTION on the canvas; they
+    must be powers of two with widths >= 128 and heights >= 2.  `config` is read live before each call and
+    applies to every member.  flags: FLAG_NO_GRAPH or 0.  Display, capture, resize and the per-pass entry
+    points are FluidSimulation's only."""
 
-    def launch_count(self) -> int:
-        return int(self._L.fluid_launch_count(self._h))
+    def __init__(self, members: int, config: dict | None = None, canvas_width: int = 1024, canvas_height: int = 1024,
+                 sizes: tuple | None = None, flags: int = 0, jacobi_block: int = 0, device: int = -1):
+        self.config = default_config(flags)
+        if config:
+            self.config.update(config)
+        self.canvas = {"width": int(canvas_width), "height": int(canvas_height)}
+        self._L = _lib.lib()
+        self._h = C.c_void_p()
+        self._device, self._flags, self._jb = device, flags, jacobi_block
+        self._pushed = {}
+        if sizes is None:
+            sim = getResolution(self.config["SIM_RESOLUTION"], canvas_width, canvas_height)
+            dye = getResolution(self.config["DYE_RESOLUTION"], canvas_width, canvas_height)
+            sizes = (sim["width"], sim["height"], dye["width"], dye["height"])
+        self._check(self._L.fluid_create_batch(C.byref(self._config(*sizes)), int(members), C.byref(self._h)))
+        self._push_config()
 
-    def stat(self, name) -> int:
-        """Library counters (fluid_stat): launches, jacobi_launches, halo_launches, halo_exchanges,
-        graph_captures, graph_launches, halo_transport_p2p, cvd_stream_launches and
-        gradient_stream_launches (how many curl-vorticity-divergence / gradientSubtract passes ran
-        the row-streaming kernel rather than the tiled one; graph replays included), and
-        jacobi_exact_streams (warps of the blocked Jacobi kernel that ran the un-contracted tail, for
-        tiny divergence or inputs near FLT_MAX; waits for the handle's queued work)."""
-        return int(self._L.fluid_stat(self._h, STAT[name]))
+    @property
+    def members(self) -> int:
+        return int(self._L.fluid_members(self._h))
 
-    def device_ptr(self, name) -> int:
-        return int(self._L.fluid_device_ptr(self._h, FIELD[name]) or 0)
+    def splats(self, members, records):
+        """Row k of records ((n, 7): x, y, dx, dy, r, g, b) splatted into member members[k]; each member takes
+        its rows in order, with the bits of FluidSimulation.splats, and members named by no row are untouched."""
+        m = np.ascontiguousarray(members, np.int32).reshape(-1)
+        a = np.asarray(records)
+        if a.ndim != 2 or a.shape[1] != 7 or a.shape[0] != m.size:
+            raise ValueError(f"splats() takes n member indices and an (n, 7) array, got {m.size} and {a.shape}")
+        a = np.ascontiguousarray(a, np.float32)
+        self._push_config()
+        self._check(self._L.fluid_splats_batch(self._h, m.ctypes.data_as(C.POINTER(C.c_int32)),
+                                               a.ctypes.data_as(C.POINTER(C.c_float)), m.size))
 
-    def set_param(self, key, value):
-        self._check(self._L.fluid_set_param(self._h, PARAM[key], float(value)))
+    def _shape(self, name):
+        w, h, c, _ = self._dims(name)
+        return (self.members, h, w, c) if c > 1 else (self.members, h, w)
 
-    def close(self):
-        if self._h:
-            self._L.fluid_destroy(self._h)
-            self._h = C.c_void_p()
+    def readField(self, name, out=None) -> np.ndarray:
+        """(B, H, W[, C]) float32, member by member, row 0 = bottom.  `out` as FluidSimulation.readField: a
+        float32 host buffer of that size, or a C-contiguous float32 CUDA array of that many elements, filled on
+        the GPU and returned as passed."""
+        shape = self._shape(name)
+        n = int(np.prod(shape))
+        dst = _device_array(out, "<f4", n, "readField")
+        if dst is not None:
+            self._check(self._L.fluid_read_device(self._h, FIELD[name], dst, n))
+            self.sync()
+            return out
+        if out is None:
+            out = np.empty(shape, np.float32)
+        else:
+            assert out.dtype == np.float32 and out.flags.c_contiguous and out.size == n
+            out = out.reshape(shape)
+        self._check(self._L.fluid_read(self._h, FIELD[name], out.ctypes.data_as(C.c_void_p), out.size))
+        return out
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *a):
-        self.close()
+    def writeField(self, name, array):
+        """Overwrites a field of every member with `array` ((B, H, W[, C])): anything numpy turns into float32,
+        or a C-contiguous float32 CUDA array of exactly that many elements."""
+        n = int(np.prod(self._shape(name)))
+        if hasattr(array, "__cuda_array_interface__"):
+            src = _device_array(array, "<f4", n, "writeField")
+            self._check(self._L.fluid_write_device(self._h, FIELD[name], src, n))
+            self.sync()
+            return
+        a = np.ascontiguousarray(array, np.float32)
+        self._check(self._L.fluid_write(self._h, FIELD[name], a.ctypes.data_as(C.c_void_p), a.size))
 
 
 _cuda = None
