@@ -194,9 +194,11 @@ int fluid_p2p_disable(fluid_t* h);   /* back to NCCL; call on every rank if any 
  *    the other members following it contiguously.
  *  - fluid_sync, fluid_stat, fluid_launch_count, fluid_mark, fluid_elapsed_ms, fluid_timing_last,
  *    fluid_last_error and fluid_destroy behave as on any handle.
- *  - Every other entry point refuses a batch handle with FLUID_ERR_INVALID and leaves it usable: render,
- *    capture and the canvas, fluid_render_band, fluid_resize, fluid_pass_*, fluid_pressure_solve_host,
- *    fluid_splat and fluid_splats (use fluid_splats_batch) and the p2p calls.
+ *  - fluid_render_canvas_batch and fluid_capture_batch draw every member's canvas or capture in one call.
+ *  - Every other entry point refuses a batch handle with FLUID_ERR_INVALID and leaves it usable: the fp32
+ *    frames (fluid_render, fluid_render_keywords, fluid_render_postfx), fluid_capture, fluid_capture_device
+ *    and fluid_render_canvas (use the batch calls), fluid_render_band, fluid_resize, fluid_pass_*,
+ *    fluid_pressure_solve_host, fluid_splat and fluid_splats (use fluid_splats_batch) and the p2p calls.
  * fluid_create_batch refuses with FLUID_ERR_INVALID: members < 1 or > FLUID_MAX_MEMBERS (the member is the
  * kernels' grid z index); any flag but FLUID_FLAG_NO_GRAPH; sizes that are not powers of two, a sim or dye
  * width under 128 or a height under 2.  The reference default 128^2 / 1024^2 qualifies.  FLUID_ERR_NOMEM:
@@ -418,6 +420,29 @@ int fluid_capture_device(fluid_t* h, int width, int height, int canvas_w, int ca
  * host memory, memory of another device, a misaligned dst, or a dst overlapping the field arena; slab handles. */
 int fluid_render_canvas(fluid_t* h, int width, int height, uint32_t keywords, int transparent,
                         const fluid_postfx* fx, const float* dither_rgb, int dw, int dh,
+                        float back_r, float back_g, float back_b,
+                        uint8_t* dst, size_t n_bytes, int dst_on_device);
+
+/* fluid_render_canvas and fluid_capture for a batch handle (fluid_create_batch): every member drawn through
+ * the launches one draw of an ordinary handle makes, each launch one layer of blocks per member.
+ *  - Member m's image is the bytes fluid_render_canvas, or fluid_capture / fluid_capture_device, give an
+ *    ordinary handle of the batch's config whose dye equals member m's.  Keywords, sliders, background and
+ *    sizes apply to every member.
+ *  - dst is one C-contiguous (B, height, width, 4) array, member by member, each image top row first;
+ *    n_bytes == B * 4 * width * height.
+ *  - dst_on_device == 0: host memory, one device-to-host copy, then a stream sync.  dst_on_device != 0:
+ *    device memory with the rules and ordering of fluid_render_canvas(..., dst_on_device = 1).
+ *  - The post-FX targets hold B members each (the bloom FBO and pyramid, the sunrays FBOs), and the sunrays
+ *    mask goes into every member's dye.write, as on an ordinary handle.  The dithering texture is shared.
+ * Refused with FLUID_ERR_INVALID, dst untouched and the handle usable: an ordinary or slab handle; every
+ * argument the single-handle call refuses; a device dst fluid_render_canvas refuses.  FLUID_ERR_NOMEM, the
+ * handle usable: the post-FX targets of B members, or the host path's frame buffer of B images, do not fit. */
+int fluid_render_canvas_batch(fluid_t* h, int width, int height, uint32_t keywords, int transparent,
+                              const fluid_postfx* fx, const float* dither_rgb, int dw, int dh,
+                              float back_r, float back_g, float back_b,
+                              uint8_t* dst, size_t n_bytes, int dst_on_device);
+int fluid_capture_batch(fluid_t* h, int width, int height, int canvas_w, int canvas_h, uint32_t keywords,
+                        int transparent, const fluid_postfx* fx, const float* dither_rgb, int dw, int dh,
                         float back_r, float back_g, float back_b,
                         uint8_t* dst, size_t n_bytes, int dst_on_device);
 

@@ -24,7 +24,8 @@ SYMBOLS = [
     "fluid_pass_advect_dye", "fluid_pass_curl_vorticity_divergence", "fluid_field_elems",
     "fluid_field_dims", "fluid_read", "fluid_write", "fluid_read_device", "fluid_write_device", "fluid_pressure_solve_host", "fluid_render", "fluid_render_band", "fluid_render_postfx", "fluid_render_keywords", "fluid_capture", "fluid_capture_device", "fluid_render_canvas", "fluid_sync",
     "fluid_timing_last", "fluid_host_alloc", "fluid_host_free", "fluid_mark", "fluid_elapsed_ms", "fluid_launch_count", "fluid_device_ptr",
-    "fluid_last_error", "fluid_create_batch", "fluid_members", "fluid_splats_batch",
+    "fluid_last_error", "fluid_create_batch", "fluid_members", "fluid_splats_batch", "fluid_render_canvas_batch",
+    "fluid_capture_batch",
 ]
 
 FLUID_OK = 0
@@ -134,6 +135,8 @@ def lib():
     L.fluid_capture.argtypes = [vp, i, i, i, i, C.c_uint32, i, C.POINTER(PostFX), vp, i, i, f, f, f, vp, sz]
     L.fluid_capture_device.argtypes = L.fluid_capture.argtypes
     L.fluid_render_canvas.argtypes = [vp, i, i, C.c_uint32, i, C.POINTER(PostFX), vp, i, i, f, f, f, vp, sz, i]
+    L.fluid_render_canvas_batch.argtypes = L.fluid_render_canvas.argtypes
+    L.fluid_capture_batch.argtypes = L.fluid_capture.argtypes + [i]
     L.fluid_sync.argtypes = [vp]
     L.fluid_host_alloc.argtypes = [sz]; L.fluid_host_alloc.restype = vp
     L.fluid_host_free.argtypes = [vp]; L.fluid_host_free.restype = None

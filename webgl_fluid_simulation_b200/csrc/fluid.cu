@@ -197,8 +197,9 @@ int fail(fluid_t* h, int code, const char* fmt, ...) {
 
 inline bool is_pow2(int n) { return n > 0 && (n & (n - 1)) == 0; }
 
-inline dim3 grid2d(int W, int rows, dim3 b) {
-    return dim3((W + b.x - 1) / b.x, (rows + b.y - 1) / b.y);
+// z: one layer of blocks per member of a batch handle (the kernels take the member from blockIdx.z)
+inline dim3 grid2d(int W, int rows, dim3 b, int z = 1) {
+    return dim3((W + b.x - 1) / b.x, (rows + b.y - 1) / b.y, z);
 }
 
 Grid sim_grid(const fluid_t* h) { return Grid{h->cfg.sim_w, h->cfg.sim_h, h->roff, h->row0, h->row1}; }
@@ -701,10 +702,11 @@ int not_on_slab(fluid_t* h, const char* what) {
                 "fluid_step / fluid_splat / fluid_pass_pressure_solve / fluid_pass_jacobi / read / write", what);
 }
 
-// what a batch handle refuses: everything but fluid_step, fluid_splats_batch, the config, field I/O and the stats
+// what a batch handle refuses: everything but fluid_step, fluid_splats_batch, the config, field I/O, the stats and
+// the batch draw calls
 int not_on_batch(fluid_t* h, const char* what) {
     return fail(h, FLUID_ERR_INVALID, "%s does not take a batch handle; one supports fluid_step / fluid_splats_batch / "
-                "read / write / set_param / stat", what);
+                "read / write / set_param / stat / fluid_render_canvas_batch / fluid_capture_batch", what);
 }
 
 // Row ownership + ghost-zone heights of rank `rank` of `world` for a sim_h / dye_h grid (DESIGN.md §7).
@@ -1770,16 +1772,6 @@ int fluid_render_band(fluid_t* h, int height, int* y0, int* y1) {
     return FLUID_OK;
 }
 
-// grows the render target to at least `cells` RGBA texels
-static int need_frame(fluid_t* h, size_t cells) {
-    if (cells <= h->frame_cells) return FLUID_OK;
-    CU(cudaStreamSynchronize(h->stream));
-    cudaFree(h->frame); h->frame = nullptr; h->frame_cells = 0;
-    CU(cudaMalloc((void**)&h->frame, cells * sizeof(float4)));
-    h->frame_cells = cells;
-    return FLUID_OK;
-}
-
 // The fp32 dye the display kernels sample: dye.read, or in half storage its widened copy in the scratch
 // buffer (the sampler widens fp16 texels exactly; shading is fp32 as in the shader).
 static int display_source(fluid_t* h, const float4** src) {
@@ -1806,6 +1798,16 @@ static int remake_target(fluid_t* h, void** p, size_t bytes, const char* what) {
     return FLUID_OK;
 }
 
+// grows the render target to at least `cells` RGBA texels (a batch draw's B images into host memory pass through
+// it, so it is made like a post-FX target: out of memory leaves the handle usable)
+static int need_frame(fluid_t* h, size_t cells) {
+    if (cells <= h->frame_cells) return FLUID_OK;
+    h->frame_cells = 0;
+    if (int rc = remake_target(h, (void**)&h->frame, cells * sizeof(float4), "the frame buffer")) return rc;
+    h->frame_cells = cells;
+    return FLUID_OK;
+}
+
 // bytes per texel of the RGBA bloom targets and of the one-channel sunrays targets (fp16 with
 // FLUID_FLAG_HALF_POSTFX, like the reference's RGBA16F / R16F FBOs)
 inline size_t fx4bytes(const fluid_t* h) { return h->half_fx ? 8 : 16; }
@@ -1813,11 +1815,13 @@ inline size_t fx1bytes(const fluid_t* h) { return h->half_fx ? 2 : 4; }
 
 // The bloom FBO and its pyramid (initBloomFramebuffers S:1012-1032), cleared like createFBO (S:1059).
 // A pyramid shorter than 2 levels leaves the FBO as cleared (applyBloom returns early, S:1351-1352).
+// A batch handle's FBO and each of its levels hold the B members back to back.
 static int need_bloom_targets(fluid_t* h, int bw, int bh, int levels) {
     auto& t = h->pfx;
     if (t.bloom && t.bw == bw && t.bh == bh && t.levels == levels) return FLUID_OK;
     size_t n = (size_t)bw * bh;
     for (int i = 0; i < levels; ++i) n += (size_t)(bw >> (i + 1)) * (bh >> (i + 1));
+    n *= h->members;
     t.bw = t.bh = t.levels = 0;
     if (int rc = remake_target(h, &t.bloom, n * fx4bytes(h), "the bloom FBO and pyramid")) return rc;
     t.bw = bw; t.bh = bh; t.levels = levels;
@@ -1828,11 +1832,11 @@ static int need_bloom_targets(fluid_t* h, int bw, int bh, int levels) {
 }
 
 // sunrays + sunraysTemp (initSunraysFramebuffers S:1034-1043): one-channel FBOs, cleared to 0 (all-zero
-// bits in fp32 and fp16 alike)
+// bits in fp32 and fp16 alike); on a batch handle each holds the B members back to back
 static int need_sunrays_targets(fluid_t* h, int sw, int sh) {
     auto& t = h->pfx;
     if (t.sun && t.sw == sw && t.sh == sh) return FLUID_OK;
-    const size_t bytes = 2 * (size_t)sw * sh * fx1bytes(h);
+    const size_t bytes = 2 * (size_t)sw * sh * h->members * fx1bytes(h);
     t.sw = t.sh = 0;
     if (int rc = remake_target(h, &t.sun, bytes, "the sunrays FBOs")) return rc;
     t.sw = sw; t.sh = sh;
@@ -1856,10 +1860,11 @@ struct PostFXOut { int bw, bh, sw, sh; };
 // applySunrays + blur(…, 1) (S:1396-1419; the mask is drawn into dye.write exactly like S:1300) with
 // SUNRAYS.  FBO sizes follow initBloomFramebuffers / initSunraysFramebuffers (S:1012-1043), which size
 // them from the drawing buffer: canvas_w x canvas_h.  Sd: the dye's storage policy (the mask is drawn in
-// it), St: the targets', Smp: the sampler of every texture the chains read (postfx.cuh).  Single GPU,
-// arguments checked by the caller.
+// it), St: the targets', Smp: the sampler of every texture the chains read (postfx.cuh).  BATCH: a batch
+// handle's B members, each target a dense (B, h, w) array and each launch B layers of blocks deep.  Single
+// GPU, arguments checked by the caller.
 extern "C++" {
-template <class Sd, class St, class Smp>
+template <class Sd, class St, class Smp, bool BATCH = false>
 static int post_fx_chains(fluid_t* h, uint32_t keywords, const fluid_postfx* fx, const float* dither_rgb,
                           int dw, int dh, int canvas_w, int canvas_h, PostFXOut* o) {
     using D4 = typename Sd::T4;
@@ -1879,50 +1884,51 @@ static int post_fx_chains(fluid_t* h, uint32_t keywords, const fluid_postfx* fx,
     }
     if (sun_on && (rc = need_sunrays_targets(h, sw, sh))) return rc;
     *o = {bw, bh, sw, sh};
-    const int Wd = h->cfg.dye_w, Hd = h->cfg.dye_h;
+    const int Wd = h->cfg.dye_w, Hd = h->cfg.dye_h, B = h->members;
     T4* bloom = static_cast<T4*>(h->pfx.bloom);
-    T1 *sun = static_cast<T1*>(h->pfx.sun), *sun2 = sun ? sun + (size_t)sw * sh : nullptr;
+    T1 *sun = static_cast<T1*>(h->pfx.sun), *sun2 = sun ? sun + (size_t)sw * sh * B : nullptr;
     dim3 b(32, 8);
     int nk = 0;
     // ---- applyBloom(dye.read, bloom) ----------------------------------------------------------------
     if (bloom_on && levels >= 2) {
         struct Lv { T4* p; int w, h; };
         std::vector<Lv> pyr;
-        T4* p = bloom + (size_t)bw * bh;
+        T4* p = bloom + (size_t)bw * bh * B;
         for (int i = 0; i < levels; ++i) {
             const int pw = bw >> (i + 1), ph = bh >> (i + 1);
             pyr.push_back({p, pw, ph});
-            p += (size_t)pw * ph;
+            p += (size_t)pw * ph * B;
         }
         const double knee = fx->bloom_threshold * fx->bloom_soft_knee + 0.0001;
-        bloom_prefilter_kernel<Sd, St, Smp><<<grid2d(bw, bh, b), b, 0, h->stream>>>(
+        bloom_prefilter_kernel<Sd, St, Smp, BATCH><<<grid2d(bw, bh, b, B), b, 0, h->stream>>>(
             (const D4*)h->dye.read, Wd, Hd, bloom, bw, bh, (float)(fx->bloom_threshold - knee),
             (float)(knee * 2), (float)(0.25 / knee), (float)fx->bloom_threshold);
         ++nk;
         Lv last{bloom, bw, bh};
         for (auto& d : pyr) {
-            box4_kernel<St, Smp><<<grid2d(d.w, d.h, b), b, 0, h->stream>>>(last.p, last.w, last.h, d.p, d.w, d.h, 1.0f, 0);
+            box4_kernel<St, Smp, BATCH><<<grid2d(d.w, d.h, b, B), b, 0, h->stream>>>(last.p, last.w, last.h, d.p, d.w, d.h, 1.0f, 0);
             last = d; ++nk;
         }
         for (int i = (int)pyr.size() - 2; i >= 0; --i) {
-            box4_kernel<St, Smp><<<grid2d(pyr[i].w, pyr[i].h, b), b, 0, h->stream>>>(last.p, last.w, last.h, pyr[i].p, pyr[i].w, pyr[i].h, 1.0f, 1);
+            box4_kernel<St, Smp, BATCH><<<grid2d(pyr[i].w, pyr[i].h, b, B), b, 0, h->stream>>>(last.p, last.w, last.h, pyr[i].p, pyr[i].w, pyr[i].h, 1.0f, 1);
             last = pyr[i]; ++nk;
         }
-        box4_kernel<St, Smp><<<grid2d(bw, bh, b), b, 0, h->stream>>>(last.p, last.w, last.h, bloom, bw, bh, (float)fx->bloom_intensity, 0);
+        box4_kernel<St, Smp, BATCH><<<grid2d(bw, bh, b, B), b, 0, h->stream>>>(last.p, last.w, last.h, bloom, bw, bh, (float)fx->bloom_intensity, 0);
         ++nk;
     }
     // ---- applySunrays(dye.read, dye.write, sunrays); blur(sunrays, sunraysTemp, 1) -------------------
     if (sun_on) {
-        sunrays_mask_kernel<Sd, Smp><<<grid2d(Wd, Hd, b), b, 0, h->stream>>>((const D4*)h->dye.read, (D4*)h->dye.write, Wd, Hd);
-        sunrays_kernel<Sd, St, Smp><<<grid2d(sw, sh, b), b, 0, h->stream>>>((const D4*)h->dye.write, Wd, Hd, sun, sw, sh, (float)fx->sunrays_weight);
-        blur3_kernel<St, Smp><<<grid2d(sw, sh, b), b, 0, h->stream>>>(sun, sun2, sw, sh, (float)(1.0 / (double)sw), 0.0f);
-        blur3_kernel<St, Smp><<<grid2d(sw, sh, b), b, 0, h->stream>>>(sun2, sun, sw, sh, 0.0f, (float)(1.0 / (double)sh));
+        sunrays_mask_kernel<Sd, Smp, BATCH><<<grid2d(Wd, Hd, b, B), b, 0, h->stream>>>((const D4*)h->dye.read, (D4*)h->dye.write, Wd, Hd);
+        sunrays_kernel<Sd, St, Smp, BATCH><<<grid2d(sw, sh, b, B), b, 0, h->stream>>>((const D4*)h->dye.write, Wd, Hd, sun, sw, sh, (float)fx->sunrays_weight);
+        blur3_kernel<St, Smp, BATCH><<<grid2d(sw, sh, b, B), b, 0, h->stream>>>(sun, sun2, sw, sh, (float)(1.0 / (double)sw), 0.0f);
+        blur3_kernel<St, Smp, BATCH><<<grid2d(sw, sh, b, B), b, 0, h->stream>>>(sun2, sun, sw, sh, 0.0f, (float)(1.0 / (double)sh));
         nk += 4;
     }
     return check_launch(h, "post-FX kernels", nk);
 }
 
-// post_fx_chains<Sd, St, Smp> of a handle: the dye's and the targets' storage, and the sampler
+// post_fx_chains<Sd, St, Smp> of a handle: the dye's and the targets' storage, and the sampler.  A batch handle
+// is fp32 and LINEAR.
 using Chains = int (*)(fluid_t*, uint32_t, const fluid_postfx*, const float*, int, int, int, int, PostFXOut*);
 template <class Smp>
 static Chains chains_for(const fluid_t* h) {
@@ -1930,19 +1936,22 @@ static Chains chains_for(const fluid_t* h) {
          : !h->half    ? post_fx_chains<StoreF32, hs::StoreHalf, Smp>
                        : post_fx_chains<hs::StoreHalf, hs::StoreHalf, Smp>;
 }
+static Chains chains_of(const fluid_t* h) {
+    return h->batch ? post_fx_chains<StoreF32, StoreF32, Linear, true> : h->nearest ? chains_for<Nearest>(h) : chains_for<Linear>(h);
+}
 
 // display_kernel<SHADING, BLOOM, SUNRAYS, Out, Sp, Smp> for the eight FLUID_DISPLAY_* masks.  The sets
 // without BLOOM and SUNRAYS read no post-FX target: one instantiation.
 using DisplayKernel = void (*)(DisplayArgs);
 using F32 = StoreF32;
 using F16 = hs::StoreHalf;
-template <class Out, class Sp, class Smp>
+template <class Out, class Sp, class Smp, bool BATCH = false>
 struct DisplaySet {
     static constexpr DisplayKernel k[8] = {
-        display_kernel<false, false, false, Out, F32, Smp>, display_kernel<true, false, false, Out, F32, Smp>,
-        display_kernel<false, true, false, Out, Sp, Smp>,   display_kernel<true, true, false, Out, Sp, Smp>,
-        display_kernel<false, false, true, Out, Sp, Smp>,   display_kernel<true, false, true, Out, Sp, Smp>,
-        display_kernel<false, true, true, Out, Sp, Smp>,    display_kernel<true, true, true, Out, Sp, Smp>};
+        display_kernel<false, false, false, Out, F32, Smp, BATCH>, display_kernel<true, false, false, Out, F32, Smp, BATCH>,
+        display_kernel<false, true, false, Out, Sp, Smp, BATCH>,   display_kernel<true, true, false, Out, Sp, Smp, BATCH>,
+        display_kernel<false, false, true, Out, Sp, Smp, BATCH>,   display_kernel<true, false, true, Out, Sp, Smp, BATCH>,
+        display_kernel<false, true, true, Out, Sp, Smp, BATCH>,    display_kernel<true, true, true, Out, Sp, Smp, BATCH>};
 };
 // What a draw() produces: the output policy of its display kernel
 enum DisplayOut { OUT_FRAME = 0, OUT_CAPTURE = 1, OUT_CANVAS = 2 };
@@ -1955,6 +1964,9 @@ static const DisplayKernel* const kDisplay[2][3][2] = {
      {DisplaySet<StoreCapture, F32, Nearest>::k, DisplaySet<StoreCapture, F16, Nearest>::k},
      {DisplaySet<StoreCanvas, F32, Nearest>::k, DisplaySet<StoreCanvas, F16, Nearest>::k}},
 };
+// a batch handle's (fp32, LINEAR; no fp32 frame), indexed by [DisplayOut][FLUID_DISPLAY_* mask]
+static const DisplayKernel* const kDisplayBatch[3] = {
+    nullptr, DisplaySet<StoreCapture, F32, Linear, true>::k, DisplaySet<StoreCanvas, F32, Linear, true>::k};
 }  // extern "C++"
 
 // Queues the copy of n values of a post-FX target into the caller's fp32 array.  An fp16 target goes
@@ -1987,6 +1999,7 @@ struct DrawRequest {
     void* dst; size_t n;               // where the image goes: n floats (frame) or n bytes (capture, canvas)
     float* host_bloom;                 // the bloom FBO / sunrays texture, read back when given
     float* host_sunrays;
+    bool batch;                        // a batch handle's call: one image per member, member by member in dst
 };
 
 // render(target) of S:1296-1317: the post-FX chains of the keywords that are on, then the background and
@@ -1994,10 +2007,13 @@ struct DrawRequest {
 // memory, left on the stream for the caller's fluid_sync).  Only the fp32 frame without BLOOM and
 // SUNRAYS is drawn on a slab handle, and there only the handle's band of the target (fluid_render_band).
 // Half storage draws from a widened copy of dye; its post-FX needs FLUID_FLAG_HALF_POSTFX, and then the
-// chains read the fp16 dye directly and draw the mask into the fp16 dye.write.
+// chains read the fp16 dye directly and draw the mask into the fp16 dye.write.  A batch request draws every
+// member of a batch handle through the same launches, each launch B layers of blocks deep; only batch requests
+// take a batch handle.
 static int draw(fluid_t* h, const DrawRequest& r) {
     if (!h) return FLUID_ERR_INVALID;
-    if (h->batch) return not_on_batch(h, r.what);
+    if (h->batch && !r.batch) return not_on_batch(h, r.what);
+    if (r.batch && !h->batch) return fail(h, FLUID_ERR_INVALID, "%s takes a batch handle (fluid_create_batch)", r.what);
     if (r.keywords & ~(uint32_t)(FLUID_DISPLAY_SHADING | FLUID_DISPLAY_BLOOM | FLUID_DISPLAY_SUNRAYS))
         return fail(h, FLUID_ERR_INVALID, "unknown display keyword bits 0x%x", r.keywords);
     const bool bloom_on = r.keywords & FLUID_DISPLAY_BLOOM, sun_on = r.keywords & FLUID_DISPLAY_SUNRAYS;
@@ -2007,8 +2023,11 @@ static int draw(fluid_t* h, const DrawRequest& r) {
         return fail(h, FLUID_ERR_INVALID, "bad argument");
     int y0 = 0, y1 = r.height;
     if (band) fluid_render_band(h, r.height, &y0, &y1);
-    const size_t cells = (size_t)r.width * (y1 - y0);
-    if (r.n != 4 * cells)
+    const size_t cells = (size_t)r.width * (y1 - y0), images = h->members;
+    if (r.batch && r.n != 4 * cells * images)
+        return fail(h, FLUID_ERR_INVALID, "%s: the targets of %d members have %zu bytes, caller passed %zu", r.what,
+                    h->members, 4 * cells * images, r.n);
+    if (r.n != 4 * cells * images)
         return fail(h, FLUID_ERR_INVALID, "%s: the target%s has %zu %s, caller passed %zu", r.what, band ? " band" : "",
                     4 * cells, bytes ? "bytes" : "floats", r.n);
     if (cells == 0) return FLUID_OK;
@@ -2017,7 +2036,7 @@ static int draw(fluid_t* h, const DrawRequest& r) {
         return fail(h, FLUID_ERR_INVALID, "%s with BLOOM or SUNRAYS is not built for FLUID_FLAG_HALF_STORAGE "
                     "(the reference's bloom / sunrays FBOs are fp16 too: add FLUID_FLAG_HALF_POSTFX)", r.what);
     int rc = r.on_device ? check_device_buf(h, r.what, r.dst, r.n)
-                         : need_frame(h, bytes ? (cells + 3) / 4 : cells);     // a uchar4 image lives in the frame
+                         : need_frame(h, bytes ? (cells * images + 3) / 4 : cells);     // uchar4 images live in the frame
     if (rc) return rc;
     if (h->slab()) {
         // the band's display + shading taps reach ceil(Hd / height) + 2 dye rows beyond the owned ones:
@@ -2029,8 +2048,7 @@ static int draw(fluid_t* h, const DrawRequest& r) {
     }
     PostFXOut o{};
     if (postfx) {
-        const Chains chains = h->nearest ? chains_for<Nearest>(h) : chains_for<Linear>(h);
-        if ((rc = chains(h, r.keywords, r.fx, r.dither, r.dw, r.dh, r.canvas_w, r.canvas_h, &o))) return rc;
+        if ((rc = chains_of(h)(h, r.keywords, r.fx, r.dither, r.dw, r.dh, r.canvas_w, r.canvas_h, &o))) return rc;
     }
     const float4* dye_src;
     if ((rc = display_source(h, &dye_src))) return rc;
@@ -2043,7 +2061,8 @@ static int draw(fluid_t* h, const DrawRequest& r) {
                         r.on_device ? r.dst : h->frame, r.width, r.height, y0, y1, r.back[0], r.back[1], r.back[2], r.bg_mode,
                         h->cfg.aspect, ts};
     dim3 b(32, 8);
-    kDisplay[h->nearest][r.out][h->half_fx][r.keywords]<<<grid2d(r.width, y1 - y0, b), b, 0, h->stream>>>(a);
+    const DisplayKernel k = h->batch ? kDisplayBatch[r.out][r.keywords] : kDisplay[h->nearest][r.out][h->half_fx][r.keywords];
+    k<<<grid2d(r.width, y1 - y0, b, h->members), b, 0, h->stream>>>(a);
     if ((rc = check_launch(h, "display_kernel"))) return rc;
     if (r.on_device) return FLUID_OK;
     CU(cudaMemcpyAsync(r.dst, h->frame, r.n * (bytes ? 1 : sizeof(float)), cudaMemcpyDeviceToHost, h->stream));
@@ -2094,14 +2113,15 @@ int fluid_render_postfx(fluid_t* h, int width, int height, const fluid_postfx* f
 // does the fp16 store, the 8-bit truncation and the flip; the fp32 frame never reaches memory.
 static int capture(fluid_t* h, const char* what, int width, int height, int canvas_w, int canvas_h, uint32_t keywords,
                    int transparent, const fluid_postfx* fx, const float* dither_rgb, int dw, int dh,
-                   float back_r, float back_g, float back_b, uint8_t* dst, size_t n_bytes, bool on_device) {
+                   float back_r, float back_g, float back_b, uint8_t* dst, size_t n_bytes, bool on_device,
+                   bool batch = false) {
     // drawColor's store of normalizeColor(BACK_COLOR) into the half-float target
     const float b16[3] = {__half2float(__float2half_rn(back_r)), __half2float(__float2half_rn(back_g)),
                           __half2float(__float2half_rn(back_b))};
     return draw(h, {.what = what, .width = width, .height = height, .canvas_w = canvas_w,
                     .canvas_h = canvas_h, .keywords = keywords, .fx = fx, .dither = dither_rgb, .dw = dw, .dh = dh,
                     .back = {b16[0], b16[1], b16[2]}, .bg_mode = transparent ? 2 : 0, .out = OUT_CAPTURE,
-                    .on_device = on_device, .dst = dst, .n = n_bytes});
+                    .on_device = on_device, .dst = dst, .n = n_bytes, .batch = batch});
 }
 
 int fluid_capture(fluid_t* h, int width, int height, int canvas_w, int canvas_h, uint32_t keywords,
@@ -2120,18 +2140,42 @@ int fluid_capture_device(fluid_t* h, int width, int height, int canvas_w, int ca
                    dw, dh, back_r, back_g, back_b, dst, n_bytes, true);
 }
 
+// The captures of every member of a batch handle, member by member into dst, through the launches of one capture.
+int fluid_capture_batch(fluid_t* h, int width, int height, int canvas_w, int canvas_h, uint32_t keywords,
+                        int transparent, const fluid_postfx* fx, const float* dither_rgb, int dw, int dh,
+                        float back_r, float back_g, float back_b, uint8_t* dst, size_t n_bytes, int dst_on_device) {
+    return capture(h, "fluid_capture_batch", width, height, canvas_w, canvas_h, keywords, transparent, fx, dither_rgb,
+                   dw, dh, back_r, back_g, back_b, dst, n_bytes, dst_on_device != 0, true);
+}
+
 // render(null) (S:1296-1317) on a width x height RGBA8 drawing buffer: the post-FX chains on the canvas-sized
 // FBOs, then the display over drawColor(BACK_COLOR) or drawCheckerboard (TRANSPARENT, S:1304-1315), blended
 // on the fixed-point buffer by the display kernel's StoreCanvas epilogue.  Into host memory through the
 // frame buffer, or straight into the caller's device memory, stream-ordered.
+static int canvas(fluid_t* h, const char* what, int width, int height, uint32_t keywords, int transparent,
+                  const fluid_postfx* fx, const float* dither_rgb, int dw, int dh, float back_r, float back_g,
+                  float back_b, uint8_t* dst, size_t n_bytes, int dst_on_device, bool batch) {
+    return draw(h, {.what = what, .width = width, .height = height, .canvas_w = width,
+                    .canvas_h = height, .keywords = keywords, .fx = fx, .dither = dither_rgb, .dw = dw, .dh = dh,
+                    .back = {back_r, back_g, back_b}, .bg_mode = transparent ? 1 : 0, .out = OUT_CANVAS,
+                    .on_device = dst_on_device != 0, .dst = dst, .n = n_bytes, .batch = batch});
+}
+
 int fluid_render_canvas(fluid_t* h, int width, int height, uint32_t keywords, int transparent,
                         const fluid_postfx* fx, const float* dither_rgb, int dw, int dh,
                         float back_r, float back_g, float back_b,
                         uint8_t* dst, size_t n_bytes, int dst_on_device) {
-    return draw(h, {.what = "fluid_render_canvas", .width = width, .height = height, .canvas_w = width,
-                    .canvas_h = height, .keywords = keywords, .fx = fx, .dither = dither_rgb, .dw = dw, .dh = dh,
-                    .back = {back_r, back_g, back_b}, .bg_mode = transparent ? 1 : 0, .out = OUT_CANVAS,
-                    .on_device = dst_on_device != 0, .dst = dst, .n = n_bytes});
+    return canvas(h, "fluid_render_canvas", width, height, keywords, transparent, fx, dither_rgb, dw, dh,
+                  back_r, back_g, back_b, dst, n_bytes, dst_on_device, false);
+}
+
+// The canvases of every member of a batch handle, member by member into dst, through the launches of one canvas.
+int fluid_render_canvas_batch(fluid_t* h, int width, int height, uint32_t keywords, int transparent,
+                              const fluid_postfx* fx, const float* dither_rgb, int dw, int dh,
+                              float back_r, float back_g, float back_b,
+                              uint8_t* dst, size_t n_bytes, int dst_on_device) {
+    return canvas(h, "fluid_render_canvas_batch", width, height, keywords, transparent, fx, dither_rgb, dw, dh,
+                  back_r, back_g, back_b, dst, n_bytes, dst_on_device, true);
 }
 
 void* fluid_host_alloc(size_t bytes) {

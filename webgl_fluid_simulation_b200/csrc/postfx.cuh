@@ -41,12 +41,28 @@ __device__ __forceinline__ float linear_fetch_rgb_r_repeat(const float* __restri
 // targets).  Fetches widen the stored texels exactly and run the same fp32 LINEAR arithmetic.  Smp is
 // the sampler of every texture a chain reads (S:1017, S:1039: the filter of dye, bloom, pyramid and
 // sunrays follows ext.supportLinearFiltering).
+//
+// BATCH: a batch handle's draw, blockIdx.z the member.  Every array a kernel reads or writes holds the B
+// members back to back, as a dense (B, h, w[, C]) array of its own size, so member m of a w x h array starts
+// member_offset(w, h) texels in.  The pointers move before any tap, so the sampler's clamp keeps every tap
+// inside the member.
+
+// texels before member blockIdx.z of a dense (B, h, w) array, in 64 bits
+__device__ __forceinline__ size_t member_offset(int w, int h) { return (size_t)blockIdx.z * w * h; }
+// p as T texels, at member blockIdx.z of a w x h array when BATCH
+template <bool BATCH, class T>
+__device__ __forceinline__ const T* member_of(const void* p, int w, int h) {
+    const T* q = static_cast<const T*>(p);
+    if constexpr (BATCH) q += member_offset(w, h);
+    return q;
+}
 
 // bloomPrefilterShader S:614-631
-template <class Sd, class St, class Smp>
+template <class Sd, class St, class Smp, bool BATCH = false>
 __global__ void __launch_bounds__(256) bloom_prefilter_kernel(const typename Sd::T4* __restrict__ dye, int Wd, int Hd,
                                                               typename St::T4* __restrict__ out, int w, int h, float curve0,
                                                               float curve1, float curve2, float threshold) {
+    if constexpr (BATCH) { dye += member_offset(Wd, Hd); out += member_offset(w, h); }
     const int i = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y * blockDim.y + threadIdx.y;
     if (i >= w || j >= h) return;
     const float uvx = ((float)i + 0.5f) / (float)w, uvy = ((float)j + 0.5f) / (float)h;
@@ -60,9 +76,10 @@ __global__ void __launch_bounds__(256) bloom_prefilter_kernel(const typename Sd:
 
 // bloomBlurShader S:633-651 / bloomFinalShader S:653-674; add = blendFunc(ONE, ONE) (S:1374-1375): the
 // fragment plus the widened destination texel, rounded once by the store
-template <class St, class Smp>
+template <class St, class Smp, bool BATCH = false>
 __global__ void __launch_bounds__(256) box4_kernel(const typename St::T4* __restrict__ src, int ws, int hs,
                                                    typename St::T4* __restrict__ dst, int w, int h, float scale, int add) {
+    if constexpr (BATCH) { src += member_offset(ws, hs); dst += member_offset(w, h); }
     const int i = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y * blockDim.y + threadIdx.y;
     if (i >= w || j >= h) return;
     const float tsx = (float)(1.0 / (double)ws), tsy = (float)(1.0 / (double)hs);
@@ -80,9 +97,10 @@ __global__ void __launch_bounds__(256) box4_kernel(const typename St::T4* __rest
 }
 
 // sunraysMaskShader S:676-691 (target = dye.write, like the reference: S:1300, so stored as the dye is)
-template <class Sd, class Smp>
+template <class Sd, class Smp, bool BATCH = false>
 __global__ void __launch_bounds__(256) sunrays_mask_kernel(const typename Sd::T4* __restrict__ dye,
                                                            typename Sd::T4* __restrict__ mask, int Wd, int Hd) {
+    if constexpr (BATCH) { dye += member_offset(Wd, Hd); mask += member_offset(Wd, Hd); }
     const int i = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y * blockDim.y + threadIdx.y;
     if (i >= Wd || j >= Hd) return;
     const float uvx = ((float)i + 0.5f) / (float)Wd, uvy = ((float)j + 0.5f) / (float)Hd;
@@ -93,9 +111,10 @@ __global__ void __launch_bounds__(256) sunrays_mask_kernel(const typename Sd::T4
 }
 
 // sunraysShader S:693-724
-template <class Sd, class St, class Smp>
+template <class Sd, class St, class Smp, bool BATCH = false>
 __global__ void __launch_bounds__(256) sunrays_kernel(const typename Sd::T4* __restrict__ mask, int Wm, int Hm,
                                                       typename St::T1* __restrict__ out, int w, int h, float weight) {
+    if constexpr (BATCH) { mask += member_offset(Wm, Hm); out += member_offset(w, h); }
     const int i = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y * blockDim.y + threadIdx.y;
     if (i >= w || j >= h) return;
     const float Density = 0.3f, Decay = 0.95f, Exposure = 0.7f;
@@ -117,9 +136,10 @@ __global__ void __launch_bounds__(256) sunrays_kernel(const typename Sd::T4* __r
 }
 
 // blurShader S:478-494 + blurVertexShader S:461-476 on the one-channel sunrays texture
-template <class St, class Smp>
+template <class St, class Smp, bool BATCH = false>
 __global__ void __launch_bounds__(256) blur3_kernel(const typename St::T1* __restrict__ src, typename St::T1* __restrict__ dst,
                                                     int w, int h, float tsx, float tsy) {
+    if constexpr (BATCH) { src += member_offset(w, h); dst += member_offset(w, h); }
     const int i = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y * blockDim.y + threadIdx.y;
     if (i >= w || j >= h) return;
     const float off = 1.33333333f;
@@ -233,9 +253,16 @@ struct StoreCanvas {
 // the background of render() (the output policy's store() blends).  Out: the output policy; Sp: the storage policy
 // of the bloom and sunrays targets (post_fx_chains' St); Smp: the sampler of the dye, bloom and sunrays
 // taps (the dithering tap is LINEAR + REPEAT whatever Smp is).  A slab rank draws the band [y0, y1) of the
-// target from its own dye rows (+ ghost rows); one GPU draws the whole target.
-template <bool SHADING, bool BLOOM, bool SUNRAYS, class Out, class Sp, class Smp>
+// target from its own dye rows (+ ghost rows); one GPU draws the whole target.  BATCH: member blockIdx.z
+// reads its own dye, bloom FBO and sunrays texture and draws its own image; the dithering texture is shared.
+template <bool SHADING, bool BLOOM, bool SUNRAYS, class Out, class Sp, class Smp, bool BATCH = false>
 __global__ void __launch_bounds__(256) display_kernel(DisplayArgs a) {
+    // the bloom FBO and the sunrays texture are offset where they are read: a member pointer kept across the
+    // shading's IEEE div / sqrt slow paths spills the SHADING | SUNRAYS capture
+    if constexpr (BATCH) {
+        a.dye += member_offset(a.Wd, a.Hd);
+        a.out = static_cast<typename Out::T*>(a.out) + member_offset(a.w, a.y1 - a.y0);
+    }
     const int i = blockIdx.x * blockDim.x + threadIdx.x, j = a.y0 + blockIdx.y * blockDim.y + threadIdx.y;
     if (i >= a.w || j >= a.y1) return;
     const float tsx = a.ts.x, tsy = a.ts.y;     // 1/width, 1/height (S:1337) and getTextureScale (S:1626-1631): JS doubles, narrowed on the host
@@ -261,11 +288,11 @@ __global__ void __launch_bounds__(256) display_kernel(DisplayArgs a) {
     }
     float bl[3] = {0.0f, 0.0f, 0.0f};
     if constexpr (BLOOM) {
-        const float4 b = Smp::template fetch<Sp>(static_cast<const typename Sp::T4*>(a.bloom), a.bw, a.bh, uvx, uvy);
+        const float4 b = Smp::template fetch<Sp>(member_of<BATCH, typename Sp::T4>(a.bloom, a.bw, a.bh), a.bw, a.bh, uvx, uvy);
         bl[0] = b.x; bl[1] = b.y; bl[2] = b.z;
     }
     if constexpr (SUNRAYS) {
-        const float s = Smp::template fetch<Sp>(static_cast<const typename Sp::T1*>(a.sun), a.sw, a.sh, uvx, uvy);
+        const float s = Smp::template fetch<Sp>(member_of<BATCH, typename Sp::T1>(a.sun, a.sw, a.sh), a.sw, a.sh, uvx, uvy);
 #pragma unroll
         for (int k = 0; k < 3; ++k) {
             cc[k] = cc[k] * s;

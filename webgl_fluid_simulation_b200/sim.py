@@ -240,6 +240,26 @@ class _Handle:
                 self._check(self._L.fluid_set_param_f64(self._h, PARAM[k], float(v)))
                 self._pushed[k] = v
 
+    def _canvas_args(self):
+        """What render(null) on the canvas hands fluid_render_canvas and fluid_render_canvas_batch: (width, height,
+        the arguments from `keywords` to `back_b`).  config.SHADING / BLOOM / SUNRAYS / TRANSPARENT (the
+        checkerboard) / BACK_COLOR and the post-FX sliders are read now; BLOOM needs `self.dithering`."""
+        cfg = self.config
+        w, h = self.canvas["width"], self.canvas["height"]
+        self._push_config()                                  # the checkerboard uses canvas.width / canvas.height (S:1327)
+        kw, fx, dith = postfx_inputs(cfg, getattr(self, "dithering", None))
+        return w, h, (kw, 1 if cfg.get("TRANSPARENT") else 0, *_fx_args(fx, dith), *_back_rgb(cfg))
+
+    def _capture_args(self):
+        """What captureScreenshot hands fluid_capture, fluid_capture_device and fluid_capture_batch: (width, height,
+        the arguments from `canvas_w` to `back_b`).  The target is getResolution(CAPTURE_RESOLUTION) of the canvas;
+        config is read as in _canvas_args."""
+        cfg = self.config
+        cw, ch = self.canvas["width"], self.canvas["height"]
+        a = capture_inputs(cfg, cw, ch, getattr(self, "dithering", None))
+        return a["width"], a["height"], (cw, ch, a["keywords"], 1 if a["transparent"] else 0,
+                                         *_fx_args(a["fx"], a["dither"]), *_back_rgb(cfg))
+
     def _dims(self, name):
         w, h, c, r0 = C.c_int(), C.c_int(), C.c_int(), C.c_int()
         self._check(self._L.fluid_field_dims(self._h, FIELD[name], C.byref(w), C.byref(h), C.byref(c), C.byref(r0)))
@@ -571,11 +591,7 @@ class FluidSimulation(_Handle):
         `out`: a C-contiguous uint8 CUDA array on the handle's device of exactly 4 * w * h bytes (e.g. a torch
         tensor): the display kernel stores the image into it, with no host copy and render_canvas's waits, and
         the array is returned as it was passed.  A PNG needs host bytes, so `path` with `out` is refused."""
-        cfg = self.config
-        cw, ch = self.canvas["width"], self.canvas["height"]
-        a = capture_inputs(cfg, cw, ch, getattr(self, "dithering", None))
-        w, h, fx, dith = a["width"], a["height"], a["fx"], a["dither"]
-        bc = cfg["BACK_COLOR"]                               # normalizeColor, S:1599-1606
+        w, h, args = self._capture_args()
         if out is not None:
             if not hasattr(out, "__cuda_array_interface__"):
                 raise ValueError("captureScreenshot(out=...) takes a CUDA array; without `out` it returns a numpy image")
@@ -583,11 +599,8 @@ class FluidSimulation(_Handle):
                 raise ValueError("captureScreenshot writes a PNG from host bytes: pass `path` or a CUDA `out`, not both")
         dst = _device_array(out, "|u1", 4 * w * h, "captureScreenshot")
         img = np.empty((h, w, 4), np.uint8) if dst is None else None
-        ptr = lambda x: None if x is None else x.ctypes.data_as(C.c_void_p)   # noqa: E731
         self._check((self._L.fluid_capture if dst is None else self._L.fluid_capture_device)(
-            self._h, w, h, cw, ch, a["keywords"], 1 if a["transparent"] else 0, None if fx is None else C.byref(fx),
-            ptr(dith), 0 if dith is None else dith.shape[1], 0 if dith is None else dith.shape[0],
-            bc["r"] / 255, bc["g"] / 255, bc["b"] / 255, ptr(img) if dst is None else dst, 4 * w * h))
+            self._h, w, h, *args, img.ctypes.data_as(C.c_void_p) if dst is None else dst, 4 * w * h))
         if dst is not None:
             self.sync()
             return out
@@ -609,27 +622,9 @@ class FluidSimulation(_Handle):
         (torch's is version 2), every queued kernel and copy of the array's device.  The handle's stream is
         synchronised before returning, so the array can be read at once.  A CUDA array is returned as it
         was passed."""
-        cfg = self.config
-        w, h = self.canvas["width"], self.canvas["height"]
-        n = 4 * w * h
-        self._push_config()                                  # the checkerboard uses canvas.width / canvas.height (S:1327)
-        kw, fx, dith = postfx_inputs(cfg, getattr(self, "dithering", None))
-        bc = cfg["BACK_COLOR"]                               # normalizeColor, S:1599-1606
-        dst = _device_array(out, "|u1", n, "render_canvas")
-        on_device = dst is not None
-        if on_device:
-            result = out
-        else:
-            if out is None:
-                out = np.empty((h, w, 4), np.uint8)
-            if not isinstance(out, np.ndarray) or out.dtype != np.uint8 or not out.flags.c_contiguous or out.size != n:
-                raise ValueError(f"render_canvas needs a C-contiguous uint8 array of {n} bytes")
-            dst, result = out.ctypes.data_as(C.c_void_p), out.reshape(h, w, 4)
-        ptr = lambda x: None if x is None else x.ctypes.data_as(C.c_void_p)   # noqa: E731
-        self._check(self._L.fluid_render_canvas(
-            self._h, w, h, kw, 1 if cfg.get("TRANSPARENT") else 0, None if fx is None else C.byref(fx), ptr(dith),
-            0 if dith is None else dith.shape[1], 0 if dith is None else dith.shape[0],
-            bc["r"] / 255, bc["g"] / 255, bc["b"] / 255, dst, n, 1 if on_device else 0))
+        w, h, args = self._canvas_args()
+        dst, result, on_device = _u8_destination(out, (h, w, 4), "render_canvas")
+        self._check(self._L.fluid_render_canvas(self._h, w, h, *args, dst, 4 * w * h, 1 if on_device else 0))
         if on_device:
             self.sync()
         return result
@@ -662,8 +657,9 @@ class FluidBatch(_Handle):
     holds the bits a FluidSimulation given member m's inputs would hold.  Sizes come from `sizes` (sim_w,
     sim_h, dye_w, dye_h) or from getResolution of config SIM_RESOLUTION / DYE_RESOLUTION on the canvas; they
     must be powers of two with widths >= 128 and heights >= 2.  `config` is read live before each call and
-    applies to every member.  flags: FLAG_NO_GRAPH or 0.  Display, capture, resize and the per-pass entry
-    points are FluidSimulation's only."""
+    applies to every member.  flags: FLAG_NO_GRAPH or 0.  render_canvas() and captureScreenshot() draw every
+    member through one set of launches; render(), resize and the per-pass entry points are FluidSimulation's
+    only."""
 
     def __init__(self, members: int, config: dict | None = None, canvas_width: int = 1024, canvas_height: int = 1024,
                  sizes: tuple | None = None, flags: int = 0, jacobi_block: int = 0, device: int = -1):
@@ -732,6 +728,59 @@ class FluidBatch(_Handle):
             return
         a = np.ascontiguousarray(array, np.float32)
         self._check(self._L.fluid_write(self._h, FIELD[name], a.ctypes.data_as(C.c_void_p), a.size))
+
+    def render_canvas(self, out=None):
+        """FluidSimulation.render_canvas for every member (fluid_render_canvas_batch): (B, canvas height, canvas
+        width, 4) uint8, member by member, member m's image the bytes a FluidSimulation of this config and canvas
+        draws from member m's dye.  Config, canvas and `self.dithering` as there.  `out`: a C-contiguous uint8 numpy
+        array of that many bytes, or a C-contiguous uint8 CUDA array of them with render_canvas's waits, returned
+        as it was passed."""
+        w, h, args = self._canvas_args()
+        B = self.members
+        dst, result, on_device = _u8_destination(out, (B, h, w, 4), "render_canvas")
+        self._check(self._L.fluid_render_canvas_batch(self._h, w, h, *args, dst, 4 * w * h * B, 1 if on_device else 0))
+        if on_device:
+            self.sync()
+        return result
+
+    def captureScreenshot(self, out=None):
+        """FluidSimulation.captureScreenshot for every member (fluid_capture_batch): (B, h, w, 4) uint8 at
+        getResolution(CAPTURE_RESOLUTION) of the canvas, member by member, each top row first.  No PNG is written.
+        `out` as in render_canvas."""
+        w, h, args = self._capture_args()
+        B = self.members
+        dst, result, on_device = _u8_destination(out, (B, h, w, 4), "captureScreenshot")
+        self._check(self._L.fluid_capture_batch(self._h, w, h, *args, dst, 4 * w * h * B, 1 if on_device else 0))
+        if on_device:
+            self.sync()
+        return result
+
+
+def _fx_args(fx, dith):
+    """fx, dither_rgb, dw and dh of the draw calls, from the PostFX and dithering texture of postfx_inputs."""
+    return (None if fx is None else C.byref(fx), None if dith is None else dith.ctypes.data_as(C.c_void_p),
+            0 if dith is None else dith.shape[1], 0 if dith is None else dith.shape[0])
+
+
+def _back_rgb(cfg):
+    """back_r, back_g, back_b of the draw calls: normalizeColor(BACK_COLOR), S:1599-1606."""
+    bc = cfg["BACK_COLOR"]
+    return bc["r"] / 255, bc["g"] / 255, bc["b"] / 255
+
+
+def _u8_destination(out, shape, what):
+    """Where an 8-bit draw of `shape` goes: (dst pointer, the array to return, on_device).  `out` is None (a new
+    numpy array), a C-contiguous uint8 numpy array of that many bytes (returned reshaped), or a C-contiguous
+    uint8 CUDA array of them (waited for by _device_array, returned as passed)."""
+    n = int(np.prod(shape))
+    dst = _device_array(out, "|u1", n, what)
+    if dst is not None:
+        return dst, out, True
+    if out is None:
+        out = np.empty(shape, np.uint8)
+    if not isinstance(out, np.ndarray) or out.dtype != np.uint8 or not out.flags.c_contiguous or out.size != n:
+        raise ValueError(f"{what} needs a C-contiguous uint8 array of {n} bytes")
+    return out.ctypes.data_as(C.c_void_p), out.reshape(shape), False
 
 
 _cuda = None
