@@ -186,8 +186,10 @@ int fluid_p2p_disable(fluid_t* h);   /* back to NCCL; call on every rank if any 
  * and flags in one handle, stepped and splatted together through the same launches.  Member m ends every call
  * with the bits an ordinary handle given member m's inputs would hold.  All fields start zero with dye alpha
  * 1 in every member, as after fluid_create.
- *  - fluid_step steps every member with one dt (a CUDA graph unless FLUID_FLAG_NO_GRAPH); fluid_set_param,
- *    fluid_set_param_f64 and fluid_get_param apply to all members.
+ *  - fluid_step steps every member with one dt (a CUDA graph unless FLUID_FLAG_NO_GRAPH); fluid_set_param and
+ *    fluid_set_param_f64 set the key for every member, and fluid_get_param returns member 0's value.
+ *  - Parameter sweeps: fluid_set_param_members gives each member its own DENSITY_DISSIPATION,
+ *    VELOCITY_DISSIPATION, PRESSURE, CURL or SPLAT_RADIUS, and fluid_step_members its own dt (below).
  *  - fluid_field_elems is B x w x rows x channels, and fluid_field_dims gives one member's w, rows and
  *    channels with row0 = 0.  fluid_read, fluid_write, fluid_read_device and fluid_write_device move all
  *    members in member order as a (B, H, W[, C]) C-contiguous array; fluid_device_ptr is member 0's .read,
@@ -207,6 +209,19 @@ int fluid_p2p_disable(fluid_t* h);   /* back to NCCL; call on every rank if any 
 int fluid_create_batch(const fluid_config* cfg, int members, fluid_t** out);
 /* B of a batch handle; 1 for ordinary and slab handles (0 for NULL). */
 int fluid_members(fluid_t* h);
+/* Per-member values of a batch handle.  values[m] becomes member m's value of `key`, narrowed as
+ * fluid_set_param_f64 narrows it; SPLAT_RADIUS stays a double until correctRadius, with the batch's ASPECT.  Only
+ * FLUID_DENSITY_DISSIPATION, FLUID_VELOCITY_DISSIPATION, FLUID_PRESSURE, FLUID_CURL and FLUID_SPLAT_RADIUS have
+ * per-member values: PRESSURE_ITERATIONS and JACOBI_BLOCK choose the launches all members share, ASPECT and
+ * BACKGROUND are canvas-wide.  fluid_step_members is fluid_step with member m stepped by dt[m].  After every call
+ * member m holds the bits of an ordinary handle created with the batch's config, given member m's values through
+ * fluid_set_param_f64 and stepped with member m's dt.  fluid_set_param / fluid_set_param_f64 of a key later set it
+ * for every member again.  Neither per-member values nor dts recapture a step graph.  n must be B: n != B, a NULL
+ * array, another key, or an ordinary or slab handle is FLUID_ERR_INVALID, with every value and field untouched.
+ * fluid_get_param_members returns the B values as fluid_get_param would return them. */
+int fluid_set_param_members(fluid_t* h, int key, const double* values, int n);
+int fluid_get_param_members(fluid_t* h, int key, float* values, int n);
+int fluid_step_members(fluid_t* h, const float* dt, int n);
 
 void fluid_destroy(fluid_t* h);
 

@@ -211,7 +211,7 @@ int main(int argc, char** argv) {
         if (v == 0) stage_kernel<1><<<nxw * nch, 32, pad(1)>>>(a, maps.m[0]);
         if (v == 1) stage_kernel<2><<<(nxw + 1) / 2 * nch, 64, pad(2)>>>(a, maps.m[1]);
         if (v == 2) stage_kernel<4><<<(nxw + 3) / 4 * nch, 128, pad(4)>>>(a, maps.m[2]);
-        if (v == 3) jacobi_tb_kernel<K, false><<<nxw * nch, 32, TB<K>::SMEM>>>(a, maps.m[0]);
+        if (v == 3) jacobi_tb_kernel<K, false><<<nxw * nch, 32, TB<K>::SMEM>>>(a, maps.m[0], nullptr);
     };
     cudaEvent_t e0, e1;
     CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));

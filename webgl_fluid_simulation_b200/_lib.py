@@ -25,7 +25,7 @@ SYMBOLS = [
     "fluid_field_dims", "fluid_read", "fluid_write", "fluid_read_device", "fluid_write_device", "fluid_pressure_solve_host", "fluid_render", "fluid_render_band", "fluid_render_postfx", "fluid_render_keywords", "fluid_capture", "fluid_capture_device", "fluid_render_canvas", "fluid_sync",
     "fluid_timing_last", "fluid_host_alloc", "fluid_host_free", "fluid_mark", "fluid_elapsed_ms", "fluid_launch_count", "fluid_device_ptr",
     "fluid_last_error", "fluid_create_batch", "fluid_members", "fluid_splats_batch", "fluid_render_canvas_batch",
-    "fluid_capture_batch",
+    "fluid_capture_batch", "fluid_set_param_members", "fluid_get_param_members", "fluid_step_members",
 ]
 
 FLUID_OK = 0
@@ -115,6 +115,9 @@ def lib():
     L.fluid_set_param.argtypes = [vp, i, f]
     L.fluid_set_param_f64.argtypes = [vp, i, C.c_double]
     L.fluid_get_param.argtypes = [vp, i, fp]
+    L.fluid_set_param_members.argtypes = [vp, i, C.POINTER(C.c_double), i]
+    L.fluid_get_param_members.argtypes = [vp, i, fp, i]
+    L.fluid_step_members.argtypes = [vp, fp, i]
     L.fluid_stat.argtypes = [vp, i]; L.fluid_stat.restype = C.c_uint64
     for n in ("curl", "divergence", "clear_pressure", "pressure_solve", "gradient_subtract"):
         getattr(L, "fluid_pass_" + n).argtypes = [vp]

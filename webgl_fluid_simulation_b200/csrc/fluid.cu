@@ -103,7 +103,12 @@ struct fluid : SlabGeometry {
     int members = 1;
     float* scratch = nullptr;              // half mode: fp32 staging of fluid_read / fluid_write / render
     size_t scratch_floats = 0;
-    float* dt_dev = nullptr;               // step()'s dt lives in device memory: one graph serves every dt
+    // step()'s dt lives in device memory: one graph serves every dt.  On a batch handle this is the member table
+    // (jacobi.cuh), whose first row is every member's dt; member_host is its host copy, and member_radius_d each
+    // member's SPLAT_RADIUS as the JS double it is (MP_RADIUS is correctRadius of it and aspect_d)
+    float* dt_dev = nullptr;
+    std::vector<float> member_host;
+    std::vector<double> member_radius_d;
     unsigned char* tiny_map = nullptr;     // where divergence has 0 < |d| < 2^-123 (jacobi.cuh): 1 byte per 128x32 cells, GLOBAL rows
     size_t tiny_map_bytes = 0;
     // 2-D tensor maps the blocked Jacobi kernel stages through: m[k] maps pressure slot k and divergence
@@ -223,12 +228,77 @@ int check_launch(fluid_t* h, const char* what, int n = 1) {
     return FLUID_OK;
 }
 
+// Row k of a batch handle's member table from its host copy: a stream-ordered upload from pageable memory (the
+// driver stages it before returning), issued outside any capture like set_dt's.
+int upload_member_row(fluid_t* h, int k) {
+    const size_t B = h->members;
+    CU(cudaMemcpyAsync(h->dt_dev + k * B, h->member_host.data() + k * B, B * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+    return FLUID_OK;
+}
+
 // dt of the current step()/pass, in device memory.  Stream-ordered 4-byte upload from a pageable
 // host word (the driver stages it before returning), issued OUTSIDE any capture: an instantiated
 // step graph therefore never bakes dt in, and the reference's calcDeltaTime() (S:1188-1194, a new
-// dt every frame) replays the same graph.
+// dt every frame) replays the same graph.  A batch handle: every member's dt.
 int set_dt(fluid_t* h, float dt) {
+    if (h->batch) {
+        std::fill_n(h->member_host.begin() + MP_DT * h->members, h->members, dt);
+        return upload_member_row(h, MP_DT);
+    }
     CU(cudaMemcpyAsync(h->dt_dev, &dt, sizeof(float), cudaMemcpyHostToDevice, h->stream));
+    return FLUID_OK;
+}
+
+// correctRadius(config.SPLAT_RADIUS / 100.0), S:1457-1462: JS double arithmetic, narrowed by gl.uniform1f
+float splat_radius(double splat_radius_d, double aspect_d) {
+    double rad = splat_radius_d / 100.0;
+    if (aspect_d > 1.0) rad *= aspect_d;
+    return (float)rad;
+}
+
+// the member table row of a key a batch member can hold a value of its own for; -1 for every other key
+int member_row(int key) {
+    switch (key) {
+        case FLUID_DENSITY_DISSIPATION: return MP_DENSITY_DISSIPATION;
+        case FLUID_VELOCITY_DISSIPATION: return MP_VELOCITY_DISSIPATION;
+        case FLUID_PRESSURE: return MP_PRESSURE;
+        case FLUID_CURL: return MP_CURL;
+        case FLUID_SPLAT_RADIUS: return MP_RADIUS;
+    }
+    return -1;
+}
+// member m's value of row `row` in the host copy, narrowed as fluid_set_param_f64 narrows it (upload_member_row
+// makes it the device's)
+void set_member_value(fluid_t* h, int row, int m, double v) {
+    const size_t at = (size_t)row * h->members + m;
+    if (row == MP_RADIUS) {
+        h->member_radius_d[m] = v;
+        h->member_host[at] = splat_radius(v, h->aspect_d);
+    } else {
+        h->member_host[at] = (float)v;
+    }
+}
+// what fluid_get_param returns for member m's value of row `row`
+float member_value(const fluid_t* h, int row, int m) {
+    return row == MP_RADIUS ? (float)h->member_radius_d[m] : h->member_host[(size_t)row * h->members + m];
+}
+
+// A batch handle's member table, every member holding the config's values and dt 0.  Outside the field arena,
+// so the arena layout is an ordinary handle's; FLUID_ERR_NOMEM when it does not fit.
+int alloc_member_table(fluid_t* h) {
+    const size_t B = h->members;
+    if (cudaMalloc((void**)&h->dt_dev, MP_KEYS * B * sizeof(float)) != cudaSuccess) {
+        cudaGetLastError();                      // not sticky: keep it out of the next launch check
+        return fail(h, FLUID_ERR_NOMEM, "out of device memory for the member table of %d members", h->members);
+    }
+    h->member_host.assign(MP_KEYS * B, 0.0f);
+    h->member_radius_d.assign(B, 0.0);
+    const fluid_config& c = h->cfg;
+    const double init[][2] = {{FLUID_DENSITY_DISSIPATION, c.density_dissipation}, {FLUID_VELOCITY_DISSIPATION, c.velocity_dissipation},
+                              {FLUID_PRESSURE, c.pressure}, {FLUID_CURL, c.curl}, {FLUID_SPLAT_RADIUS, h->splat_radius_d}};
+    for (const auto& kv : init)
+        for (size_t m = 0; m < B; ++m) set_member_value(h, member_row((int)kv[0]), (int)m, kv[1]);
+    CU(cudaMemcpyAsync(h->dt_dev, h->member_host.data(), MP_KEYS * B * sizeof(float), cudaMemcpyHostToDevice, h->stream));
     return FLUID_OK;
 }
 
@@ -335,7 +405,8 @@ struct JacobiPlan {
 // JacobiArgs of a launch whose local row 0 is global row row_off; the caller sets pin, pout and the rows
 JacobiArgs jacobi_args(const fluid_t* h, const float* div, int row_off) {
     JacobiArgs a{};
-    a.div = div; a.row_off = row_off; a.W = h->cfg.sim_w; a.H = h->cfg.sim_h; a.scale = h->cfg.pressure;
+    a.div = div; a.row_off = row_off; a.W = h->cfg.sim_w; a.H = h->cfg.sim_h;
+    a.scale = h->cfg.pressure;
     a.err = h->halo_flag; a.tiny_map = h->tiny_map; a.exact_streams = h->exact_streams;
     return a;
 }
@@ -406,10 +477,11 @@ int build_tmaps(fluid_t* h) {
 
 // kTb[K - 1]: jacobi_tb_kernel<K, SCALE> as kernel[SCALE], its batch-handle form as batch[SCALE], and the TB<K>
 // constants their launches need
+typedef void (*TbKernel)(JacobiArgs, TmapPair, const float*);
 struct TbEntry {
-    void (*kernel[2])(JacobiArgs, TmapPair);
+    TbKernel kernel[2];
     int valid, u, smem;
-    void (*batch[2])(JacobiArgs, TmapPair);
+    TbKernel batch[2];
 };
 template <int K>
 constexpr TbEntry tb_entry() {
@@ -455,7 +527,8 @@ int launch_tb(fluid_t* h, int K, bool scale, bool chained, JacobiArgs a, const T
     lc.gridDim = dim3(nxw * nch, 1, h->members); lc.blockDim = dim3(32); lc.stream = h->stream;   // one warp per CTA
     lc.attrs = attr; lc.numAttrs = (chained && !h->capturing) ? 1 : 0;
     lc.dynamicSmemBytes = e.smem;
-    cudaLaunchKernelEx(&lc, h->batch ? e.batch[scale] : e.kernel[scale], a, maps);
+    const float* member_table = h->batch ? h->dt_dev : nullptr;
+    cudaLaunchKernelEx(&lc, h->batch ? e.batch[scale] : e.kernel[scale], a, maps, member_table);
     ++h->launches.jacobi;
     return check_launch(h, "jacobi_tb_kernel");
 }
@@ -497,12 +570,20 @@ int run_jacobi(fluid_t* h, int iters, bool scale_first, int* launches_out) {
     // clears in a launch of its own: the reference rounds the cleared field to fp16 before the first sweep.
     if (scale_first && (iters <= 0 || h->half)) {
         const size_t n = sim_cells(h) * h->members;
-        int rc = with_storage(h, [&](auto s) {
-            using S = decltype(s);
-            scale_kernel<S><<<(unsigned)((n + 255) / 256), 256, 0, h->stream>>>(
-                (const typename S::T1*)h->pressure.read, (typename S::T1*)h->pressure.write, n, h->cfg.pressure);
-            return check_launch(h, "scale_kernel");
-        });
+        int rc;
+        if (h->batch) {                                  // each member by its own PRESSURE
+            const size_t nm = sim_cells(h);
+            scale_members_kernel<<<dim3((unsigned)((nm + 255) / 256), 1, h->members), 256, 0, h->stream>>>(
+                (const float*)h->pressure.read, (float*)h->pressure.write, nm, h->dt_dev);
+            rc = check_launch(h, "scale_members_kernel");
+        } else {
+            rc = with_storage(h, [&](auto s) {
+                using S = decltype(s);
+                scale_kernel<S><<<(unsigned)((n + 255) / 256), 256, 0, h->stream>>>(
+                    (const typename S::T1*)h->pressure.read, (typename S::T1*)h->pressure.write, n, h->cfg.pressure);
+                return check_launch(h, "scale_kernel");
+            });
+        }
         if (rc) return rc;
         h->pressure.swap(); ++nl;
         scale_first = false;
@@ -805,8 +886,12 @@ int create_common(const fluid_config* cfg, int rank, int world, const void* uid,
         CU(cudaMemsetAsync(h->halo_flag, 0, sizeof(int), h->stream));
         CU(cudaMalloc((void**)&h->exact_streams, sizeof(unsigned long long)));
         CU(cudaMemsetAsync(h->exact_streams, 0, sizeof(unsigned long long), h->stream));
-        CU(cudaMalloc((void**)&h->dt_dev, sizeof(float)));
-        CU(cudaMemsetAsync(h->dt_dev, 0, sizeof(float), h->stream));
+        if (h->batch) {
+            int r = alloc_member_table(h); if (r) return r;
+        } else {
+            CU(cudaMalloc((void**)&h->dt_dev, sizeof(float)));
+            CU(cudaMemsetAsync(h->dt_dev, 0, sizeof(float), h->stream));
+        }
         int r = alloc_fields(h); if (r) return r;
         CU(cudaStreamSynchronize(h->stream));
         if (world > 1) {
@@ -984,21 +1069,32 @@ void fluid_destroy(fluid_t* h) {
     delete h;
 }
 
-int fluid_set_param(fluid_t* h, int key, float v) {
-    if (!h) return FLUID_ERR_INVALID;
+// config.<key> = v, where SPLAT_RADIUS and ASPECT keep vd, the value as the caller's double.  On a batch handle
+// every member takes a per-member key's value, and ASPECT moves every member's splat radius.
+static int set_param(fluid_t* h, int key, float v, double vd) {
     switch (key) {
         case FLUID_DENSITY_DISSIPATION: h->cfg.density_dissipation = v; break;
         case FLUID_VELOCITY_DISSIPATION: h->cfg.velocity_dissipation = v; break;
         case FLUID_PRESSURE: h->cfg.pressure = v; break;
         case FLUID_PRESSURE_ITERATIONS: h->cfg.pressure_iterations = (int)(v + 0.5f); break;
         case FLUID_CURL: h->cfg.curl = v; break;
-        case FLUID_SPLAT_RADIUS: h->cfg.splat_radius = v; h->splat_radius_d = (double)v; break;
-        case FLUID_ASPECT: h->cfg.aspect = v; h->aspect_d = (double)v; break;
+        case FLUID_SPLAT_RADIUS: h->cfg.splat_radius = v; h->splat_radius_d = vd; break;
+        case FLUID_ASPECT: h->cfg.aspect = v; h->aspect_d = vd; break;
         case FLUID_JACOBI_BLOCK: h->cfg.jacobi_block = (int)(v + 0.5f); break;
         case FLUID_BACKGROUND: h->background = (int)(v + 0.5f); break;
         default: return fail(h, FLUID_ERR_INVALID, "unknown param key %d", key);
     }
-    return FLUID_OK;
+    if (!h->batch) return FLUID_OK;
+    const int row = key == FLUID_ASPECT ? MP_RADIUS : member_row(key);
+    if (row < 0) return FLUID_OK;
+    for (int m = 0; m < h->members; ++m)
+        set_member_value(h, row, m, key == FLUID_ASPECT ? h->member_radius_d[m] : vd);
+    return upload_member_row(h, row);
+}
+
+int fluid_set_param(fluid_t* h, int key, float v) {
+    if (!h) return FLUID_ERR_INVALID;
+    return set_param(h, key, v, (double)v);
 }
 
 // The JS config values are doubles; two of them enter double arithmetic on the host before the
@@ -1006,15 +1102,47 @@ int fluid_set_param(fluid_t* h, int key, float v) {
 // so a host mirror passes them at full precision.  Every other key narrows like fluid_set_param.
 int fluid_set_param_f64(fluid_t* h, int key, double v) {
     if (!h) return FLUID_ERR_INVALID;
-    int rc = fluid_set_param(h, key, (float)v);
+    return set_param(h, key, (float)v, v);
+}
+
+// what fluid_set_param_members, fluid_get_param_members and fluid_step_members refuse before they change anything
+static int check_members(fluid_t* h, const char* what, const void* values, int n) {
+    if (!h->batch) return fail(h, FLUID_ERR_INVALID, "%s needs a batch handle (fluid_create_batch)", what);
+    if (!values || n != h->members)
+        return fail(h, FLUID_ERR_INVALID, "%s takes one value for each of the %d members (got %d at %p)", what, h->members, n, values);
+    return FLUID_OK;
+}
+static int check_member_key(fluid_t* h, const char* what, int key) {
+    if (member_row(key) >= 0) return FLUID_OK;
+    return fail(h, FLUID_ERR_INVALID, "%s: key %d has no per-member values (DENSITY_DISSIPATION, VELOCITY_DISSIPATION, "
+                "PRESSURE, CURL and SPLAT_RADIUS do)", what, key);
+}
+
+int fluid_set_param_members(fluid_t* h, int key, const double* values, int n) {
+    if (!h) return FLUID_ERR_INVALID;
+    int rc = check_members(h, "fluid_set_param_members", values, n);
+    if (!rc) rc = check_member_key(h, "fluid_set_param_members", key);
     if (rc) return rc;
-    if (key == FLUID_SPLAT_RADIUS) h->splat_radius_d = v;
-    if (key == FLUID_ASPECT) h->aspect_d = v;
+    const int row = member_row(key);
+    for (int m = 0; m < n; ++m) set_member_value(h, row, m, values[m]);
+    return upload_member_row(h, row);
+}
+
+int fluid_get_param_members(fluid_t* h, int key, float* values, int n) {
+    if (!h) return FLUID_ERR_INVALID;
+    int rc = check_members(h, "fluid_get_param_members", values, n);
+    if (!rc) rc = check_member_key(h, "fluid_get_param_members", key);
+    if (rc) return rc;
+    for (int m = 0; m < n; ++m) values[m] = member_value(h, member_row(key), m);
     return FLUID_OK;
 }
 
 int fluid_get_param(fluid_t* h, int key, float* v) {
     if (!h || !v) return FLUID_ERR_INVALID;
+    if (h->batch && member_row(key) >= 0) {            // member 0's
+        *v = member_value(h, member_row(key), 0);
+        return FLUID_OK;
+    }
     switch (key) {
         case FLUID_DENSITY_DISSIPATION: *v = h->cfg.density_dissipation; break;
         case FLUID_VELOCITY_DISSIPATION: *v = h->cfg.velocity_dissipation; break;
@@ -1334,15 +1462,17 @@ static int step_enqueue(fluid_t* h, bool timed) {
 // each ping-pong pair is currently `.read`.  dt is NOT part of the key: kernels read it from
 // device memory (set_dt), so the reference's frame loop — calcDeltaTime() yields a different dt
 // on every frame (S:1188-1194) — replays the same two graphs (one per ping-pong parity).
-int fluid_step(fluid_t* h, float dt) {
-    if (!h) return FLUID_ERR_INVALID;
+// A batch handle's kernels read CURL, PRESSURE and the dissipations from the member table, like dt, so they are
+// not part of its key either: per-member values and dts change every step and still replay the same graphs.
+static int step_after_dt(fluid_t* h) {
     const bool no_graph = (h->cfg.flags & FLUID_FLAG_NO_GRAPH) != 0;
-    { int rc = set_dt(h, dt); if (rc) return rc; }
     if (no_graph || h->slab()) return step_enqueue(h, no_graph);
     char key[256];
     const fluid_config& c = h->cfg;
+    const bool b = h->batch;
     snprintf(key, sizeof key, "%a|%a|%a|%a|%d|%d|%u|%d%d%d|%dx%d|%dx%d|%d",
-             c.curl, c.pressure, c.velocity_dissipation, c.density_dissipation, c.pressure_iterations, c.jacobi_block,
+             b ? 0.0f : c.curl, b ? 0.0f : c.pressure, b ? 0.0f : c.velocity_dissipation, b ? 0.0f : c.density_dissipation,
+             c.pressure_iterations, c.jacobi_block,
              c.flags, h->velocity.par, h->pressure.par, h->dye.par, c.sim_w, c.sim_h, c.dye_w, c.dye_h, h->members);
     auto it = h->graphs.find(key);
     if (it == h->graphs.end()) {
@@ -1382,6 +1512,20 @@ int fluid_step(fluid_t* h, float dt) {
     return FLUID_OK;
 }
 
+int fluid_step(fluid_t* h, float dt) {
+    if (!h) return FLUID_ERR_INVALID;
+    { int rc = set_dt(h, dt); if (rc) return rc; }
+    return step_after_dt(h);
+}
+
+int fluid_step_members(fluid_t* h, const float* dt, int n) {
+    if (!h) return FLUID_ERR_INVALID;
+    if (int rc = check_members(h, "fluid_step_members", dt, n)) return rc;
+    std::copy(dt, dt + n, h->member_host.begin() + (size_t)MP_DT * n);
+    if (int rc = upload_member_row(h, MP_DT)) return rc;
+    return step_after_dt(h);
+}
+
 static SplatPlane splat_plane(const Grid& g) {
     SplatPlane p{};
     p.g = g; p.pow2 = is_pow2(g.W) && is_pow2(g.H);
@@ -1391,13 +1535,10 @@ static SplatPlane splat_plane(const Grid& g) {
 }
 static int splat_blocks(const SplatPlane& p) { return p.bx * ((p.g.j_hi - p.g.j_lo + SPL_BH - 1) / SPL_BH); }
 
-// what every splat launch shares: correctRadius(config.SPLAT_RADIUS / 100.0), JS double arithmetic narrowed
-// by gl.uniform1f, and the aspect
+// what every splat launch shares: correctRadius(config.SPLAT_RADIUS / 100.0) and the aspect
 static SplatsArgs splats_args(const fluid_t* h) {
     SplatsArgs a{};
-    double rad = h->splat_radius_d / 100.0;
-    if (h->aspect_d > 1.0) rad *= h->aspect_d;
-    a.radius = (float)rad;
+    a.radius = splat_radius(h->splat_radius_d, h->aspect_d);
     a.aspect = h->cfg.aspect;
     return a;
 }
@@ -1461,7 +1602,8 @@ int fluid_splats_batch(fluid_t* h, const int32_t* member, const float* splats, i
     a.n = 0;
     auto flush = [&]() {
         g.start[ng] = (unsigned char)a.n;
-        splats_batch_kernel<<<dim3(blocks, ng), 256, 0, h->stream>>>((float2*)h->velocity.read, (float4*)h->dye.read, a, g);
+        splats_batch_kernel<<<dim3(blocks, ng), 256, 0, h->stream>>>((float2*)h->velocity.read, (float4*)h->dye.read, a, g,
+                                                                     h->dt_dev + (size_t)MP_RADIUS * h->members);
         a.n = 0; ng = 0;
         return check_launch(h, "splats_batch_kernel");
     };

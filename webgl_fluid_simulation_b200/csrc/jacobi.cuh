@@ -36,6 +36,16 @@
 
 namespace fk {
 
+// ---- the member table of a batch handle --------------------------------------------------------------
+// Each member's step scalars and dt in device memory: MP_KEYS rows of B floats, row k holding every member's
+// value of scalar k (MP_RADIUS: correctRadius(SPLAT_RADIUS / 100) as splats use it).  The host changes it only
+// by stream-ordered copies, so a step graph never bakes a value in.  A kernel whose grid has one layer per member
+// reads member blockIdx.z's value (B == gridDim.z).
+enum MemberParam { MP_DT, MP_CURL, MP_PRESSURE, MP_VELOCITY_DISSIPATION, MP_DENSITY_DISSIPATION, MP_RADIUS, MP_KEYS };
+__device__ __forceinline__ float member_param(const float* __restrict__ tab, MemberParam k) {
+    return __ldg(tab + (size_t)k * gridDim.z + blockIdx.z);
+}
+
 struct JacobiArgs {
     const float* pin;    // local row 0 of the source pressure buffer
     const float* div;    // local row 0 of divergence
@@ -512,13 +522,16 @@ __device__ __noinline__ void tb_stream_exact(const JacobiArgs& a, const void* tm
 #define FLUID_TB_BOUNDS __launch_bounds__(32, FLUID_TB_MINBLOCKS)
 #endif
 // BATCH: a batch handle's launch, blockIdx.z the member.  The maps are 3-D (W, H, B); pout and the tiny map
-// move to the member's array and map region.
+// move to the member's array and map region, and SCALE takes the member's PRESSURE from member_table (a.scale is
+// not read).  Only that instantiation reads member_table.
 template <int K, bool SCALE, bool BATCH = false>
-__global__ void FLUID_TB_BOUNDS jacobi_tb_kernel(JacobiArgs a, const __grid_constant__ TmapPair maps) {
+__global__ void FLUID_TB_BOUNDS jacobi_tb_kernel(JacobiArgs a, const __grid_constant__ TmapPair maps,
+                                                 const float* __restrict__ member_table) {
     using T = TB<K>;
     if constexpr (BATCH) {
         a.pout += (size_t)blockIdx.z * a.W * a.H;
         if (a.tiny_map) a.tiny_map += (size_t)blockIdx.z * tiny_map_w(a.W) * tiny_map_h(a.H);
+        if constexpr (SCALE) a.scale = member_param(member_table, MP_PRESSURE);
     }
     extern __shared__ __align__(128) float4 smem4[];
     // Programmatic dependent launch: back-to-back blocked launches of one solve are chained with

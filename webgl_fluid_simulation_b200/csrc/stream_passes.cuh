@@ -252,7 +252,8 @@ __device__ __forceinline__ void cvd_step(Vel4 (&V)[3], float (&C)[3][4], Vel4 (&
     st.o_curl += W4; st.o_vel += 2 * W4; st.o_div += W4;
 }
 
-// BATCH: blockIdx.z is the member of a batch handle; each member flags its own region of the tiny map
+// BATCH: blockIdx.z is the member of a batch handle; each member flags its own region of the tiny map, and
+// dtp is the member table (jacobi.cuh), from which the member takes its dt and CURL (curl_k is not read)
 template <bool BATCH = false>
 __global__ void __launch_bounds__(32 * CVD2_WARPS, CVD2_MINBLOCKS) cvd_stream_kernel(const float2* __restrict__ v,
                                                                     float* __restrict__ curl,
@@ -273,7 +274,8 @@ __global__ void __launch_bounds__(32 * CVD2_WARPS, CVD2_MINBLOCKS) cvd_stream_ke
     const int y0 = a.g.j_lo + cy * a.rows_per_chunk;
     const int y1 = min(y0 + a.rows_per_chunk, a.g.j_hi);
     if (y0 >= y1) return;                                   // warp-uniform
-    const float dt = __ldg(dtp);
+    const float dt = BATCH ? member_param(dtp, MP_DT) : __ldg(dtp);
+    if constexpr (BATCH) curl_k = member_param(dtp, MP_CURL);
 
     const int c0 = wx * CVD2_VALID - 4 + 4 * lane;          // first column of this lane (may be off-grid)
     const bool out_lane = (lane >= 1) && (lane <= 30) && (c0 >= 0) && (c0 < W);

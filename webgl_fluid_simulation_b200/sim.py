@@ -221,10 +221,9 @@ class _Handle:
         cfg.splat_radius = float(self.config["SPLAT_RADIUS"])
         return cfg
 
-    def _push_config(self):
-        """The reference reads `config` live inside step()/splat(); mirror that by pushing every
-        changed scalar before the call."""
-        vals = {
+    def _live_values(self):
+        """What _push_config pushes: each key's value as `config` and the canvas hold it now."""
+        return {
             "DENSITY_DISSIPATION": self.config["DENSITY_DISSIPATION"],
             "VELOCITY_DISSIPATION": self.config["VELOCITY_DISSIPATION"],
             "PRESSURE": self.config["PRESSURE"],
@@ -233,11 +232,18 @@ class _Handle:
             "SPLAT_RADIUS": self.config["SPLAT_RADIUS"],
             "ASPECT": self._aspect(),
         }
-        for k, v in vals.items():
+
+    def _push(self, key, value):
+        # JS numbers are doubles: SPLAT_RADIUS and the aspect enter double arithmetic in
+        # correctRadius (S:1457-1462) before the single fp32 narrowing of gl.uniform1f
+        self._check(self._L.fluid_set_param_f64(self._h, PARAM[key], float(value)))
+
+    def _push_config(self):
+        """The reference reads `config` live inside step()/splat(); mirror that by pushing every
+        changed scalar before the call."""
+        for k, v in self._live_values().items():
             if self._pushed.get(k) != v:
-                # JS numbers are doubles: SPLAT_RADIUS and the aspect enter double arithmetic in
-                # correctRadius (S:1457-1462) before the single fp32 narrowing of gl.uniform1f
-                self._check(self._L.fluid_set_param_f64(self._h, PARAM[k], float(v)))
+                self._push(k, v)
                 self._pushed[k] = v
 
     def _canvas_args(self):
@@ -657,9 +663,13 @@ class FluidBatch(_Handle):
     holds the bits a FluidSimulation given member m's inputs would hold.  Sizes come from `sizes` (sim_w,
     sim_h, dye_w, dye_h) or from getResolution of config SIM_RESOLUTION / DYE_RESOLUTION on the canvas; they
     must be powers of two with widths >= 128 and heights >= 2.  `config` is read live before each call and
-    applies to every member.  flags: FLAG_NO_GRAPH or 0.  render_canvas() and captureScreenshot() draw every
-    member through one set of launches; render(), resize and the per-pass entry points are FluidSimulation's
-    only."""
+    applies to every member, except that `member_config[m]` (a dict per member, empty at creation) overrides the
+    MEMBER_KEYS for member m: a parameter sweep.  step() takes one dt, or one per member.  flags: FLAG_NO_GRAPH or
+    0.  render_canvas() and captureScreenshot() draw every member through one set of launches; render(), resize and
+    the per-pass entry points are FluidSimulation's only."""
+
+    # the config keys a member can hold a value of its own for (fluid_set_param_members)
+    MEMBER_KEYS = ("DENSITY_DISSIPATION", "VELOCITY_DISSIPATION", "PRESSURE", "CURL", "SPLAT_RADIUS")
 
     def __init__(self, members: int, config: dict | None = None, canvas_width: int = 1024, canvas_height: int = 1024,
                  sizes: tuple | None = None, flags: int = 0, jacobi_block: int = 0, device: int = -1):
@@ -676,11 +686,55 @@ class FluidBatch(_Handle):
             dye = getResolution(self.config["DYE_RESOLUTION"], canvas_width, canvas_height)
             sizes = (sim["width"], sim["height"], dye["width"], dye["height"])
         self._check(self._L.fluid_create_batch(C.byref(self._config(*sizes)), int(members), C.byref(self._h)))
+        self.member_config = [{} for _ in range(self.members)]
         self._push_config()
 
     @property
     def members(self) -> int:
         return int(self._L.fluid_members(self._h))
+
+    def _live_values(self):
+        """A MEMBER_KEYS value is the float64 vector of every member's value, `member_config` over `config`."""
+        B = self.members
+        if len(self.member_config) != B:
+            raise ValueError(f"member_config holds {len(self.member_config)} dicts for {B} members")
+        for m, over in enumerate(self.member_config):
+            bad = sorted(set(over) - set(self.MEMBER_KEYS))
+            if bad:
+                raise ValueError(f"member_config[{m}] sets {bad}: only {list(self.MEMBER_KEYS)} can differ between members")
+        vals = super()._live_values()
+        for k in self.MEMBER_KEYS:
+            vec = np.array([float(over.get(k, self.config[k])) for over in self.member_config], np.float64)
+            vals[k] = vec.tobytes()                       # compared bit for bit: -0.0 is not 0.0
+        return vals
+
+    def _push(self, key, value):
+        if key not in self.MEMBER_KEYS:
+            return super()._push(key, value)
+        vec = np.frombuffer(value, np.float64)
+        bits = vec.view(np.int64)
+        if (bits == bits[0]).all():                       # one value for every member: as a FluidSimulation pushes it
+            return super()._push(key, vec[0])
+        self._check(self._L.fluid_set_param_members(self._h, PARAM[key], vec.ctypes.data_as(C.POINTER(C.c_double)),
+                                                     vec.size))
+
+    def member_params(self, key):
+        """The B values of a MEMBER_KEYS key the handle holds, float32, as FluidSimulation's get_param would
+        return them (fluid_get_param_members)."""
+        out = np.empty(self.members, np.float32)
+        self._check(self._L.fluid_get_param_members(self._h, PARAM[key], out.ctypes.data_as(C.POINTER(C.c_float)),
+                                                    out.size))
+        return out
+
+    def step(self, dt):
+        """step(dt) of every member: one number for all of them, or a sequence of B numbers, dt[m] for member m."""
+        if np.ndim(dt) == 0:
+            return super().step(dt)
+        d = np.ascontiguousarray(dt, np.float32)
+        if d.ndim != 1 or d.size != self.members:
+            raise ValueError(f"step() takes one dt or {self.members} of them, got shape {d.shape}")
+        self._push_config()
+        self._check(self._L.fluid_step_members(self._h, d.ctypes.data_as(C.POINTER(C.c_float)), d.size))
 
     def splats(self, members, records):
         """Row k of records ((n, 7): x, y, dx, dy, r, g, b) splatted into member members[k]; each member takes
