@@ -200,7 +200,8 @@ int fluid_p2p_disable(fluid_t* h);   /* back to NCCL; call on every rank if any 
  *  - Every other entry point refuses a batch handle with FLUID_ERR_INVALID and leaves it usable: the fp32
  *    frames (fluid_render, fluid_render_keywords, fluid_render_postfx), fluid_capture, fluid_capture_device
  *    and fluid_render_canvas (use the batch calls), fluid_render_band, fluid_resize, fluid_pass_*,
- *    fluid_pressure_solve_host, fluid_splat and fluid_splats (use fluid_splats_batch) and the p2p calls.
+ *    fluid_pressure_solve_host, fluid_splat, fluid_splats and fluid_splats_device (use fluid_splats_batch or
+ *    fluid_splats_batch_device) and the p2p calls.
  * fluid_create_batch refuses with FLUID_ERR_INVALID: members < 1 or > FLUID_MAX_MEMBERS (the member is the
  * kernels' grid z index); any flag but FLUID_FLAG_NO_GRAPH; sizes that are not powers of two, a sim or dye
  * width under 128 or a height under 2.  The reference default 128^2 / 1024^2 qualifies.  FLUID_ERR_NOMEM:
@@ -261,6 +262,29 @@ int fluid_splats(fluid_t* h, const float* splats, int n);
  * block.  n == 0 does nothing.  n < 0, a NULL array with n > 0, a member index outside [0, B) or an
  * ordinary handle is FLUID_ERR_INVALID, with every field untouched. */
 int fluid_splats_batch(fluid_t* h, const int32_t* member, const float* splats, int n);
+
+/* fluid_splats and fluid_splats_batch with the arrays in CUDA memory (for example torch tensors), for pipelines
+ * that make their splats on the GPU: no host copy, and each call reads and writes each field once whatever n is.
+ *  - fluid_splats_device(h, splats, n) gives the bits of fluid_splats(h, host copy, n): the same .read -> .write
+ *    and swap of velocity and dye, the same rows written.  One launch for every n >= 1.  Ordinary handles of every
+ *    flag; a batch handle is refused (use fluid_splats_batch_device).
+ *  - fluid_splats_batch_device(h, member, splats, n): member m ends with the bits fluid_splats_batch gives with
+ *    the same arrays on the host: its own records in call order, in place on its .read, with its own
+ *    SPLAT_RADIUS.  A member no record names is not touched.  Two launches whatever n, B or the spread of the
+ *    records (one orders the records by member, one splats).  An ordinary handle is refused.
+ *  - Stream-ordered with the rules of fluid_write_device: work of other streams that writes the arrays must be
+ *    complete before the call, and the caller calls fluid_sync before reusing them.
+ *  - A member index outside [0, B) cannot be checked on the host without a sync.  The call then splats no member
+ *    and changes nothing, and the next fluid_sync (or fluid_read) returns FLUID_ERR_INVALID once, with a message;
+ *    calls after it work normally.
+ *  - fluid_splats_batch_device keeps the grouped records in a scratch buffer outside the field arena.  It grows
+ *    on demand, never during a graph capture (FLUID_ERR_INVALID there); FLUID_ERR_NOMEM when it does not fit,
+ *    with the handle usable.
+ * n == 0 launches nothing and touches nothing.  Refused with FLUID_ERR_INVALID, every field and buffer untouched
+ * and the handle usable: n < 0; a NULL array with n > 0; an array fluid_read_device refuses (host memory, another
+ * device's memory, not 4-byte aligned, overlapping the field arena), `member` and `splats` alike; slab handles. */
+int fluid_splats_device(fluid_t* h, const float* splats, int n);
+int fluid_splats_batch_device(fluid_t* h, const int32_t* member, const float* splats, int n);
 
 /* config.<KEY> = value (S:59-69).  PRESSURE_ITERATIONS / JACOBI_BLOCK are rounded to int. */
 int fluid_set_param(fluid_t* h, int key, float value);

@@ -26,6 +26,7 @@ SYMBOLS = [
     "fluid_timing_last", "fluid_host_alloc", "fluid_host_free", "fluid_mark", "fluid_elapsed_ms", "fluid_launch_count", "fluid_device_ptr",
     "fluid_last_error", "fluid_create_batch", "fluid_members", "fluid_splats_batch", "fluid_render_canvas_batch",
     "fluid_capture_batch", "fluid_set_param_members", "fluid_get_param_members", "fluid_step_members",
+    "fluid_splats_device", "fluid_splats_batch_device",
 ]
 
 FLUID_OK = 0
@@ -112,6 +113,8 @@ def lib():
     L.fluid_splat.argtypes = [vp] + [f] * 7
     L.fluid_splats.argtypes = [vp, fp, i]
     L.fluid_splats_batch.argtypes = [vp, C.POINTER(C.c_int32), fp, i]
+    L.fluid_splats_device.argtypes = [vp, vp, i]
+    L.fluid_splats_batch_device.argtypes = [vp, vp, vp, i]
     L.fluid_set_param.argtypes = [vp, i, f]
     L.fluid_set_param_f64.argtypes = [vp, i, C.c_double]
     L.fluid_get_param.argtypes = [vp, i, fp]

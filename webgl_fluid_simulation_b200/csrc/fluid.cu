@@ -103,6 +103,8 @@ struct fluid : SlabGeometry {
     int members = 1;
     float* scratch = nullptr;              // half mode: fp32 staging of fluid_read / fluid_write / render
     size_t scratch_floats = 0;
+    int* splat_scratch = nullptr;          // fluid_splats_batch_device: grouped order, per-member offsets, staged records
+    size_t splat_scratch_bytes = 0;        // (outside the arena, grown on demand)
     // step()'s dt lives in device memory: one graph serves every dt.  On a batch handle this is the member table
     // (jacobi.cuh), whose first row is every member's dt; member_host is its host copy, and member_radius_d each
     // member's SPLAT_RADIUS as the JS double it is (MP_RADIUS is correctRadius of it and aspect_d)
@@ -772,6 +774,9 @@ int check_halo(fluid_t* h) {
         return fail(h, FLUID_ERR_HALO, "peer-memory halo exchange timed out waiting for a neighbour rank");
     if (flag == 3)
         return fail(h, FLUID_ERR_CUDA, "jacobi_tb_kernel: a TMA staging barrier never completed");
+    if (flag == DEV_ERR_MEMBER)
+        return fail(h, FLUID_ERR_INVALID, "fluid_splats_batch_device: a record named a member outside [0, %d); "
+                    "that call splatted nothing", h->members);
     if (flag)
         return fail(h, FLUID_ERR_HALO, "advection back-trace left the %d-row ghost zone: |v|*dt exceeds it; "
                     "re-create the slab handle with a taller halo (FLUID_HALO_ROWS)", h->G);
@@ -783,10 +788,10 @@ int not_on_slab(fluid_t* h, const char* what) {
                 "fluid_step / fluid_splat / fluid_pass_pressure_solve / fluid_pass_jacobi / read / write", what);
 }
 
-// what a batch handle refuses: everything but fluid_step, fluid_splats_batch, the config, field I/O, the stats and
+// what a batch handle refuses: everything but fluid_step, fluid_splats_batch[_device], the config, field I/O, the stats and
 // the batch draw calls
 int not_on_batch(fluid_t* h, const char* what) {
-    return fail(h, FLUID_ERR_INVALID, "%s does not take a batch handle; one supports fluid_step / fluid_splats_batch / "
+    return fail(h, FLUID_ERR_INVALID, "%s does not take a batch handle; one supports fluid_step / fluid_splats_batch[_device] / "
                 "read / write / set_param / stat / fluid_render_canvas_batch / fluid_capture_batch", what);
 }
 
@@ -1054,6 +1059,7 @@ void fluid_destroy(fluid_t* h) {
     cudaFree(h->exact_streams);
     cudaFree(h->dt_dev);
     cudaFree(h->scratch);
+    cudaFree(h->splat_scratch);
     cudaFree(h->frame);
     cudaFree(h->pfx.bloom); cudaFree(h->pfx.sun); cudaFree(h->pfx.dither);
     if (h->comm) { ncdl::api().CommDestroy(h->comm); h->comm = nullptr; }
@@ -1617,6 +1623,92 @@ int fluid_splats_batch(fluid_t* h, const int32_t* member, const float* splats, i
         memcpy(&a.rec[a.n++], splats + 7 * (size_t)r, sizeof(SplatRec));
     }
     return flush();
+}
+
+static int check_device_buf(fluid_t* h, const char* what, const void* p, size_t bytes);   // data in / out, below
+
+// fluid_splats from device memory: one launch applies all n records, each tile reading and writing its texels once
+int fluid_splats_device(fluid_t* h, const float* splats, int n) {
+    const char* what = "fluid_splats_device";
+    if (!h) return FLUID_ERR_INVALID;
+    if (h->batch) return not_on_batch(h, what);
+    if (h->slab()) return not_on_slab(h, what);
+    if (n < 0 || (n > 0 && !splats)) return fail(h, FLUID_ERR_INVALID, "%s: bad record block (%d records at %p)", what, n, (const void*)splats);
+    if (n == 0) return FLUID_OK;
+    if (int rc = check_device_buf(h, what, splats, 7 * sizeof(float) * (size_t)n)) return rc;
+    SplatsDeviceArgs a{};
+    a.radius = splat_radius(h->splat_radius_d, h->aspect_d);
+    a.aspect = h->cfg.aspect;
+    a.v = splat_plane(sim_grid(h));
+    a.d = splat_plane(dye_grid(h));
+    a.blocks_v = splat_blocks(a.v);
+    a.n = n;
+    a.rec = splats;
+    const int blocks = a.blocks_v + splat_blocks(a.d);
+    int rc = with_storage(h, [&](auto s) {
+        using S = decltype(s);
+        splats_device_kernel<S><<<blocks, 256, 0, h->stream>>>((const typename S::T2*)h->velocity.read, (typename S::T2*)h->velocity.write,
+                                                               (const typename S::T4*)h->dye.read, (typename S::T4*)h->dye.write, a);
+        return check_launch(h, "splats_device_kernel");
+    });
+    if (rc) return rc;
+    h->velocity.swap();                          // S:1449
+    h->dye.swap();                               // S:1454
+    return FLUID_OK;
+}
+
+// The scratch of fluid_splats_batch_device, at least `bytes`.  It grows outside any capture: a graph must not
+// hold an allocation, and the old buffer may still be in use by queued launches.
+static int need_splat_scratch(fluid_t* h, size_t bytes) {
+    if (bytes <= h->splat_scratch_bytes) return FLUID_OK;
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    CU(cudaStreamIsCapturing(h->stream, &cs));
+    if (h->capturing || cs != cudaStreamCaptureStatusNone)
+        return fail(h, FLUID_ERR_INVALID, "fluid_splats_batch_device: the splat scratch cannot grow during a graph capture");
+    CU(cudaStreamSynchronize(h->stream));
+    cudaFree(h->splat_scratch); h->splat_scratch = nullptr; h->splat_scratch_bytes = 0;
+    bytes = std::max(bytes, (size_t)64 << 10);
+    if (cudaMalloc((void**)&h->splat_scratch, bytes) != cudaSuccess) {
+        cudaGetLastError();                      // not sticky: keep it out of the next launch check
+        h->splat_scratch = nullptr;
+        return fail(h, FLUID_ERR_NOMEM, "fluid_splats_batch_device: out of device memory for %zu bytes of splat scratch", bytes);
+    }
+    h->splat_scratch_bytes = bytes;
+    return FLUID_OK;
+}
+
+// fluid_splats_batch from device memory in two launches whatever n, B or the spread of the records: a grouping
+// launch (splat_group_kernel) checks the member indices and orders the records by member, and one splat launch
+// applies each named member's records in place on its .read.  An index outside [0, B) cannot be seen here without
+// a sync: the grouping launch then names no member, so nothing is splatted, and sets the device error word that
+// the next fluid_sync reports.
+int fluid_splats_batch_device(fluid_t* h, const int32_t* member, const float* splats, int n) {
+    const char* what = "fluid_splats_batch_device";
+    if (!h) return FLUID_ERR_INVALID;
+    if (!h->batch) return fail(h, FLUID_ERR_INVALID, "%s needs a batch handle (fluid_create_batch)", what);
+    if (n < 0 || (n > 0 && (!member || !splats)))
+        return fail(h, FLUID_ERR_INVALID, "%s: bad record block (%d records)", what, n);
+    if (n == 0) return FLUID_OK;
+    if (int rc = check_device_buf(h, what, member, sizeof(int32_t) * (size_t)n)) return rc;
+    if (int rc = check_device_buf(h, what, splats, 7 * sizeof(float) * (size_t)n)) return rc;
+    const SplatGroupLayout L = splat_group_layout(n, h->members);
+    if (int rc = need_splat_scratch(h, L.ints * sizeof(int) + 7 * sizeof(float) * (size_t)n)) return rc;
+    splat_group_kernel<<<1, GROUP_THREADS, 0, h->stream>>>(member, splats, n, h->members, h->splat_scratch, h->halo_flag);
+    if (int rc = check_launch(h, "splat_group_kernel")) return rc;
+    SplatsBatchDeviceArgs a{};
+    a.aspect = h->cfg.aspect;
+    a.v = splat_plane(sim_grid(h));
+    a.d = splat_plane(dye_grid(h));
+    a.blocks_v = splat_blocks(a.v);
+    a.g = h->splat_scratch;
+    a.named = L.named; a.start = L.start;
+    a.rec = reinterpret_cast<const float*>(h->splat_scratch + L.ints);
+    a.radius = h->dt_dev + (size_t)MP_RADIUS * h->members;
+    const int tiles = a.blocks_v + splat_blocks(a.d);
+    // enough member rows for about 16 blocks per SM, and never more than can be named
+    const int rows = std::min({n, h->members, std::max(1, 16 * h->sm_count / tiles)});
+    splats_batch_device_kernel<<<dim3(tiles, rows), 256, 0, h->stream>>>((float2*)h->velocity.read, (float4*)h->dye.read, a);
+    return check_launch(h, "splats_batch_device_kernel");
 }
 
 // splat(x,y,dx,dy,color), S:1441-1455

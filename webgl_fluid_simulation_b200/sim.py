@@ -402,7 +402,17 @@ class FluidSimulation(_Handle):
 
     def splats(self, records):
         """len(records) splat() calls in one: records is (n, 7) of (x, y, dx, dy, r, g, b), applied in
-        order with the same bits as one splat() per row, in ceil(n/128) launches."""
+        order with the same bits as one splat() per row, in ceil(n/128) launches.  `records` may also be a
+        C-contiguous (n, 7) float32 CUDA array on the handle's device (anything with __cuda_array_interface__,
+        e.g. a torch tensor): the records are read on the GPU in one launch (fluid_splats_device), with the same
+        bits and no host copy, after the waits of writeField."""
+        if hasattr(records, "__cuda_array_interface__"):
+            n = _records_rows(records)
+            src = _device_array(records, "<f4", 7 * n, "splats")
+            self._push_config()
+            self._check(self._L.fluid_splats_device(self._h, src, n))
+            self.sync()
+            return
         a = np.asarray(records)
         if a.ndim != 2 or a.shape[1] != 7:
             raise ValueError(f"splats() takes an (n, 7) array of (x, y, dx, dy, r, g, b), got shape {a.shape}")
@@ -738,7 +748,23 @@ class FluidBatch(_Handle):
 
     def splats(self, members, records):
         """Row k of records ((n, 7): x, y, dx, dy, r, g, b) splatted into member members[k]; each member takes
-        its rows in order, with the bits of FluidSimulation.splats, and members named by no row are untouched."""
+        its rows in order, with the bits of FluidSimulation.splats, and members named by no row are untouched.
+        Both may instead be CUDA arrays on the handle's device (an int32 vector of n and a C-contiguous (n, 7)
+        float32 array): the records are grouped and applied on the GPU in two launches (fluid_splats_batch_device),
+        with the same bits and no host copy, after the waits of writeField.  One on the host and the other on the
+        device is a ValueError.  A member index outside [0, B) in a CUDA array makes the call splat nothing and is
+        reported by the sync that ends it (FluidError)."""
+        dev_m, dev_r = hasattr(members, "__cuda_array_interface__"), hasattr(records, "__cuda_array_interface__")
+        if dev_m != dev_r:
+            raise ValueError("splats() takes members and records both in host memory or both as CUDA arrays")
+        if dev_m:
+            n = _records_rows(records)
+            mem = _device_array(members, "<i4", n, "splats")
+            src = _device_array(records, "<f4", 7 * n, "splats")
+            self._push_config()
+            self._check(self._L.fluid_splats_batch_device(self._h, mem, src, n))
+            self.sync()
+            return
         m = np.ascontiguousarray(members, np.int32).reshape(-1)
         a = np.asarray(records)
         if a.ndim != 2 or a.shape[1] != 7 or a.shape[0] != m.size:
@@ -837,8 +863,16 @@ def _u8_destination(out, shape, what):
     return out.ctypes.data_as(C.c_void_p), out.reshape(shape), False
 
 
+def _records_rows(records):
+    """n of a CUDA array of splat records, which must have shape (n, 7)."""
+    shape = tuple(records.__cuda_array_interface__["shape"])
+    if len(shape) != 2 or shape[1] != 7:
+        raise ValueError(f"splats() takes an (n, 7) array of (x, y, dx, dy, r, g, b), got shape {shape}")
+    return int(shape[0])
+
+
 _cuda = None
-_TYPES = {"|u1": "uint8", "<f4": "float32"}
+_TYPES = {"|u1": "uint8", "<i4": "int32", "<f4": "float32"}
 
 
 def _device_array(a, typestr, n, what):
