@@ -19,11 +19,9 @@ operation, built from what already exists:
 Every array an operation writes is derived from the operation tuple alone (op_data), so a logged
 session can be replayed from its log.
 
-Data restrictions: fp32 sessions keep inf / NaN out of velocity, pressure and divergence (the
-power-of-two advection takes a texel's own velocity where the oracle bilerps it, so a non-finite
-neighbour legitimately differs -- test_advection_far_outside_the_grid_vs_oracle); dye may hold them, and
-subnormals and large finite values go everywhere.  Half-storage sessions write the special values of
-sim_harness.special_fields.
+Data: every session writes the special values of sim_harness.special_fields (+-0, subnormals, +-inf, NaN
+and a band of large pressure) into velocity, pressure and divergence, rounded to fp16 in half storage; fp32
+sessions add large finite values, and their dye may hold inf and NaN too.
 """
 from __future__ import annotations
 
@@ -221,10 +219,6 @@ def op_classes(ops, half: bool) -> set:
 
 
 # ---- the data an operation writes ---------------------------------------------------------------------
-def ordinary(shape, rng, scale=1.0):
-    return (rng.standard_normal(shape) * scale).astype(F32)
-
-
 def fp32_special(a, rng, big):
     """Subnormals, signed zeros and large finite values sprinkled over `a` (finite only)."""
     flat = a.reshape(-1)
@@ -248,14 +242,15 @@ def field_data(name, W, H, Wd, Hd, seed, half: bool):
         v2, _, _ = nasty_fields(W, H, 1, 1, seed + 1)
         return O.round_half(v2[..., 0] if name == "divergence" else v2[..., 1] * F32(0.01))
     if name == "velocity":
-        return fp32_special(ordinary((H, W, 2), rng, 50.0), rng, F32(1e30))
+        return fp32_special(special_fields(O, W, H, 1, 1, seed, half=False)[0], rng, F32(1e30))
     if name == "dye":
-        _, dye, _ = nasty_fields(1, 1, Wd, Hd, seed)       # inf / NaN allowed in dye
+        _, dye, _ = nasty_fields(1, 1, Wd, Hd, seed)
         return dye
     if name == "pressure":
-        return fp32_special(ordinary((H, W), rng), rng, F32(1e20))
+        return fp32_special(special_fields(O, W, H, 1, 1, seed, half=False)[2], rng, F32(1e20))
     if name == "divergence":
-        return fp32_special(rng.uniform(-1, 1, (H, W)).astype(F32), rng, F32(1e20))
+        v2, _, _ = nasty_fields(W, H, 1, 1, seed + 1)
+        return fp32_special(v2[..., 0], rng, F32(1e20))
     _, _, c = nasty_fields(W, H, 1, 1, seed)                  # curl: recomputed before any pass reads it
     c.reshape(-1)[rng.integers(0, c.size, max(1, c.size // 9))] = np.nan
     return c

@@ -137,15 +137,54 @@ def special_values(shape, seed, half):
     return a
 
 
-def special_fields(O, W, H, Wd, Hd, seed):
-    """nasty_fields rounded to fp16, with a band of +-6e4 pressure whose sign flips every two cells in
-    x and y: the cells two apart across a flip differ by 1.2e5."""
+def special_fields(O, W, H, Wd, Hd, seed, half=True):
+    """nasty_fields with a band of +-6e4 pressure whose sign flips every two cells in x and y: the cells two
+    apart across a flip differ by 1.2e5 (fp16 overflows).  half: rounded to fp16."""
     v, dye, p = nasty_fields(W, H, Wd, Hd, seed)
     s = lambda n: np.where((np.arange(n) // 2) % 2 == 0, 1.0, -1.0).astype(np.float32)
     big = np.float32(6e4) * s(H)[:, None] * s(W)[None, :]
     band = slice(H // 4, max(H // 2, H // 4 + 4))
     p[band] = big[band]
-    return tuple(O.round_half(a) for a in (v, dye, p))
+    return tuple(O.round_half(a) for a in (v, dye, p)) if half else (v, dye, p)
+
+
+CENTRE_SPECIALS = (np.inf, -np.inf, np.nan)
+
+
+def centre_placements(W, H):
+    """{class: (row, col)} of the cells where centre_special_velocity puts its special value.  The manual
+    bilerp's velocity sample at a cell centre weighs the +x, +y and +xy neighbours (clamped to the edge) by 0, so
+    a special at (r, c) reaches the samples of (r, c - 1), (r - 1, c) and (r - 1, c - 1) and its own.  The
+    classes cross the 4-cell kernels' lane layout (column 31 -> 32: lane 31, k = 0 -> lane 0, k = 1), their
+    blocks in x (column 127 -> 128) and in y (row 7 -> 8), and sit on the last column and row, where the
+    clamped neighbour is the cell itself."""
+    p = {"interior": (min(5, H - 1), min(5, W - 1)), "last_col": (H // 2, W - 1), "last_row": (H - 1, min(9, W - 1)),
+         "corner": (H - 1, W - 1)}
+    if W > 40:
+        p["lane"] = (min(3, H - 1), 32)
+    if W > 136:
+        p["block"] = (min(3, H - 1), 128)
+    if H > 10:
+        p["row_block"] = (8, min(12, W - 1))
+    return p
+
+
+def centre_special_velocity(W, H, value, comp, seed, coarse=False):
+    """Ordinary velocity with `value` (+-inf or NaN) in component `comp` at every centre_placements cell.  The
+    cells left of and below each one move up and right, so that their back-traces stay off the special texel and
+    only their centre sample meets it; the cell right of it holds a finite -0.0.  coarse: multiples of 4 in
+    [-64, 60], which compress (golden files)."""
+    rng = np.random.default_rng(seed)
+    if coarse:
+        v = (rng.integers(-16, 16, (H, W, 2)) * 4).astype(F)
+    else:
+        v = (rng.standard_normal((H, W, 2)) * 50).astype(F)
+    for r, c in centre_placements(W, H).values():
+        v[max(r - 1, 0):r + 1, max(c - 1, 0):c + 1] = F(4.0)
+        v[r, c, comp] = F(value)
+        if c + 1 < W:
+            v[r, c + 1, comp] = F(-0.0)
+    return v
 
 
 def exp_tiled(shape, seed, lo=-149, hi=100, tile=(16, 128), zeros=0.03):

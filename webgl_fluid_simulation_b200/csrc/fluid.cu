@@ -328,9 +328,10 @@ auto with_storage(const fluid_t* h, F&& f) {
 // the sim grid and the advected grid are powers of two (p2) and the advected grid is w cells wide:
 //   4-cell    fp32 storage, p2, w >= 128 and no FLUID_FLAG_TILED_PASSES.  SLAB only on slab handles, which are
 //             always MANUAL.
-//   one-cell  otherwise; the POW2 form when p2, except for MANUAL half storage (pow2_form): its own-texel
-//             shortcut would give other bits than the reference's bilerp next to an inf or NaN neighbour.
-// The own texel, and SAME (dye grid == sim grid) with it, only with F::kOwnTexel.
+//   one-cell  otherwise; the POW2 form when p2, except for MANUAL half storage (pow2_form), which runs the
+//             !POW2 forms: the reference's coordinates and bilerp on every sample.
+// The cell-centre velocity sample without a coordinate (centre taps), and SAME (dye grid == sim grid) with it,
+// only with F::kOwnTexel.
 bool advect4_runs(const fluid_t* h, bool p2, int w) {
     return p2 && !h->half && w >= 128 && !(h->cfg.flags & FLUID_FLAG_TILED_PASSES);
 }
