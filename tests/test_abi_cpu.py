@@ -4,6 +4,7 @@ colours, dt clamp) follows the reference."""
 import ctypes as C
 import os
 import re
+import subprocess
 
 import numpy as np
 import pytest
@@ -28,6 +29,14 @@ def test_header_and_library_agree(L):
     for s in declared:
         assert hasattr(L, s), s
     assert L.fluid_abi_version() == 2
+
+
+def test_no_loopback_transport_in_the_product(L):
+    """The in-process halo transport of the slab tests (tests/slab_loopback.cu, FLUID_TEST_LOOPBACK) is compiled
+    only into the test build: the product exports no loopback symbol and carries no loopback code."""
+    out = subprocess.run(["nm", "-C", _lib.SO_PATH], capture_output=True, text=True, check=True).stdout
+    assert "loopback" not in out.lower()
+    assert not hasattr(L, "fluid_loopback_link")
 
 
 def test_stat_tables_match_the_header_enum():

@@ -900,6 +900,7 @@ int create_common(const fluid_config* cfg, int rank, int world, const void* uid,
         }
         int r = alloc_fields(h); if (r) return r;
         CU(cudaStreamSynchronize(h->stream));
+#ifndef FLUID_TEST_LOOPBACK   // the loopback test build links its ranks in-process (tests/slab_loopback.cu)
         if (world > 1) {
             ncdl::Api& N = ncdl::api();
             if (!N.handle) return fail(h, FLUID_ERR_NCCL, "NCCL not available: %s", N.why);
@@ -908,6 +909,7 @@ int create_common(const fluid_config* cfg, int rank, int world, const void* uid,
             int rc = N.CommInitRank(&h->comm, world, id, rank);
             if (rc) return fail(h, FLUID_ERR_NCCL, "ncclCommInitRank failed: %s", N.GetErrorString(rc));
         }
+#endif
         return FLUID_OK;
     };
     int rc = body();
