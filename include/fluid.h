@@ -335,7 +335,7 @@ int fluid_write(fluid_t* h, int field, const float* host, size_t n_floats);
  * fluid_field_elems; a NULL buffer; a bad field id; pageable or pinned host memory; memory of another
  * device (managed memory of the handle's device is accepted); a buffer not 4-byte aligned; a buffer whose
  * [ptr, ptr + 4 * n_floats) overlaps the handle's field arena (such as fluid_device_ptr of a field);
- * slab handles (single-GPU entry points, like fluid_capture). */
+ * slab handles (single-GPU entry points). */
 int fluid_read_device(fluid_t* h, int field, float* dst, size_t n_floats);
 int fluid_write_device(fluid_t* h, int field, const float* src, size_t n_floats);
 
@@ -357,10 +357,23 @@ int fluid_pressure_solve_host(fluid_t* h, const float* div_host, float* pressure
  * memory.  back_* are BACK_COLOR / 255. */
 int fluid_render(fluid_t* h, int width, int height, int shading, float back_r, float back_g,
                  float back_b, float* host_rgba, size_t n_floats);
-/* On a slab handle fluid_render draws (and returns) only the band of target rows [*y0, *y1) that
- * corresponds to the dye rows the rank owns — width * (*y1 - *y0) RGBA texels — after refreshing
- * the few dye ghost rows the display / shading taps reach; on a single GPU the band is the whole
- * target.  Ranks concatenate their bands in rank order. */
+/* On a slab handle every draw — fluid_render, fluid_render_keywords and fluid_render_postfx with any of the
+ * eight keyword sets, fluid_capture, fluid_capture_device and fluid_render_canvas into host or device memory —
+ * draws (and returns) only the band of target rows [*y0, *y1) that corresponds to the dye rows the rank owns,
+ * after one refresh of the dye ghost rows the frame's taps reach; on a single GPU the band is the whole target.
+ *  - Size: n_floats / n_bytes must be 4 * width * (*y1 - *y0).
+ *  - Row order: the fp32 frame is bottom row first, so the bands concatenate in rank order.  Captures and
+ *    canvases are top row first, each band too, so the whole image is the bands in REVERSE rank order.
+ *  - With BLOOM or SUNRAYS the call is collective, like fluid_resize: every rank calls it with the same
+ *    arguments.  Each rank prefilters its band of the bloom FBO and draws the sunrays mask on its own dye rows;
+ *    the bands are all-gathered over NCCL (FLUID_STAT_GATHERS), and every rank then holds the bloom FBO and the
+ *    sunrays texture one GPU computes, bit for bit.  host_bloom / host_sunrays, when given, receive them whole
+ *    on every rank.
+ *  - Every argument check comes before the first exchange, so a refused call is refused on every rank with
+ *    nothing sent.  A frame whose taps need more dye ghost rows than the slab keeps (slab.py
+ *    draw_ghost_rows) returns FLUID_ERR_HALO on every rank.
+ *  - Slab handles are fp32 with LINEAR samplers: the half-storage, half-post-FX and NEAREST flags are refused
+ *    by fluid_create_slab. */
 int fluid_render_band(fluid_t* h, int height, int* y0, int* y1);
 
 /* The same with the reference's desktop defaults SHADING = BLOOM = SUNRAYS = true (S:70-84):
@@ -388,8 +401,8 @@ int fluid_render_postfx(fluid_t* h, int width, int height, const fluid_postfx* f
  * textures only for the keywords that are on (S:1339-1346).  The background follows FLUID_BACKGROUND.
  *  - Without BLOOM and SUNRAYS this is fluid_render(…, keywords & FLUID_DISPLAY_SHADING, …): slab bands
  *    and half storage work, and fx / dither_rgb may be NULL.
- *  - With BLOOM or SUNRAYS the handle must be single-GPU, with fp32 storage or with
- *    FLUID_FLAG_HALF_POSTFX (FLUID_ERR_INVALID otherwise), fx is required, and dither_rgb only with BLOOM.  host_bloom / host_sunrays (as for
+ *  - With BLOOM or SUNRAYS the handle must have fp32 storage or FLUID_FLAG_HALF_POSTFX (FLUID_ERR_INVALID
+ *    otherwise; a slab handle draws its band, fluid_render_band), fx is required, and dither_rgb only with BLOOM.  host_bloom / host_sunrays (as for
  *    fluid_render_postfx, may be NULL) are written only when their keyword is on.
  * The bloom FBO + pyramid, the sunrays FBOs and the dithering texture live in the handle: made on first
  * use, made again only when a size changes (FLUID_ERR_NOMEM if that fails; the handle stays usable), and
@@ -417,8 +430,9 @@ int fluid_render_keywords(fluid_t* h, int width, int height, uint32_t keywords, 
  *    first.  One device-to-host copy of n_bytes, then a stream sync.
  * Refused with FLUID_ERR_INVALID, the handle staying usable: unknown keyword bits; n_bytes !=
  * 4 * width * height; width, height, canvas_w or canvas_h < 1; BLOOM without dither_rgb; fx == NULL with
- * BLOOM or SUNRAYS; slab handles; half-storage handles with BLOOM or SUNRAYS unless created with
- * FLUID_FLAG_HALF_POSTFX (without them half storage works, as in fluid_render). */
+ * BLOOM or SUNRAYS; half-storage handles with BLOOM or SUNRAYS unless created with
+ * FLUID_FLAG_HALF_POSTFX (without them half storage works, as in fluid_render).  A slab handle draws its band
+ * (fluid_render_band): n_bytes = 4 * width * (y1 - y0). */
 int fluid_capture(fluid_t* h, int width, int height, int canvas_w, int canvas_h, uint32_t keywords,
                   int transparent, const fluid_postfx* fx, const float* dither_rgb, int dw, int dh,
                   float back_r, float back_g, float back_b, uint8_t* host_rgba8, size_t n_bytes);
@@ -456,7 +470,8 @@ int fluid_capture_device(fluid_t* h, int width, int height, int canvas_w, int ca
  * Refused with FLUID_ERR_INVALID, dst untouched and the handle usable: n_bytes != 4 * width * height;
  * width or height < 1; unknown keyword bits; BLOOM without dither_rgb; fx == NULL with BLOOM or SUNRAYS;
  * half-storage handles with BLOOM or SUNRAYS unless created with FLUID_FLAG_HALF_POSTFX; dst_on_device with
- * host memory, memory of another device, a misaligned dst, or a dst overlapping the field arena; slab handles. */
+ * host memory, memory of another device, a misaligned dst, or a dst overlapping the field arena.  A slab
+ * handle draws its band (fluid_render_band): n_bytes = 4 * width * (y1 - y0). */
 int fluid_render_canvas(fluid_t* h, int width, int height, uint32_t keywords, int transparent,
                         const fluid_postfx* fx, const float* dither_rgb, int dw, int dh,
                         float back_r, float back_g, float back_b,
@@ -516,8 +531,10 @@ typedef enum fluid_stat_key {
     FLUID_STAT_GRADIENT_STREAM_LAUNCHES = 8, /* row-streaming gradientSubtract kernels executed          */
     FLUID_STAT_JACOBI_EXACT_STREAMS = 9,     /* blocked Jacobi warps that ran the un-contracted tail:
                                                 tiny divergence, or inputs near FLT_MAX (synchronises)  */
-    FLUID_STAT_ADVECT4_LAUNCHES = 10         /* 4-cell advection kernels executed (velocity or dye, MANUAL
+    FLUID_STAT_ADVECT4_LAUNCHES = 10,        /* 4-cell advection kernels executed (velocity or dye, MANUAL
                                                 or LINEAR filter): fp32, power-of-two, width >= 128     */
+    FLUID_STAT_GATHERS = 11                  /* row-band all-gathers of a slab's post-FX: one per frame for
+                                                BLOOM (with >= 2 pyramid levels), one for SUNRAYS        */
 } fluid_stat_key;
 uint64_t fluid_stat(fluid_t* h, int key);
 

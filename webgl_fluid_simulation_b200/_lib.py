@@ -44,7 +44,7 @@ FLAG_LINEAR_ADVECTION = 0x80    # advection through LINEAR samplers, the referen
 DISPLAY_SHADING, DISPLAY_BLOOM, DISPLAY_SUNRAYS = 0x1, 0x2, 0x4
 STAT = {"launches": 0, "jacobi_launches": 1, "halo_launches": 2, "halo_exchanges": 3,
         "graph_captures": 4, "graph_launches": 5, "halo_transport_p2p": 6, "cvd_stream_launches": 7,
-        "gradient_stream_launches": 8, "jacobi_exact_streams": 9, "advect4_launches": 10}
+        "gradient_stream_launches": 8, "jacobi_exact_streams": 9, "advect4_launches": 10, "gathers": 11}
 
 
 class FluidError(RuntimeError):

@@ -131,6 +131,7 @@ struct fluid : SlabGeometry {
     ncdl::ncclComm_t comm = nullptr;
     bool v_ghost_valid = true;       // velocity valid on owned rows +-3 (what the next step needs)
     uint64_t halo_groups = 0;        // halo exchanges issued (diagnostics)
+    uint64_t gathers = 0;            // row-band all-gathers issued (post-FX on slabs, halo.cuh gather_bands)
     // ---- peer-memory halo path (fluid_p2p_export / fluid_p2p_connect) -------------------------------
     struct Peer {
         bool present = false;
@@ -170,6 +171,8 @@ struct fluid : SlabGeometry {
         int sw = 0, sh = 0;
         float* dither = nullptr;     // dw x dh RGB dithering texture, uploaded every BLOOM frame
         int dw = 0, dh = 0;
+        float* mask = nullptr;       // slab SUNRAYS: the mask's alpha, Wd x Hd, every rank's band gathered
+        int mw = 0, mh = 0;
     } pfx;
     bool slab() const { return world > 1; }
 };
@@ -786,7 +789,7 @@ int check_halo(fluid_t* h) {
 
 int not_on_slab(fluid_t* h, const char* what) {
     return fail(h, FLUID_ERR_INVALID, "%s is a single-GPU test entry point; a slab handle supports "
-                "fluid_step / fluid_splat / fluid_pass_pressure_solve / fluid_pass_jacobi / read / write", what);
+                "fluid_step / fluid_splat / fluid_pass_pressure_solve / fluid_pass_jacobi / read / write / the draw calls", what);
 }
 
 // what a batch handle refuses: everything but fluid_step, fluid_splats_batch[_device], the config, field I/O, the stats and
@@ -1064,7 +1067,7 @@ void fluid_destroy(fluid_t* h) {
     cudaFree(h->scratch);
     cudaFree(h->splat_scratch);
     cudaFree(h->frame);
-    cudaFree(h->pfx.bloom); cudaFree(h->pfx.sun); cudaFree(h->pfx.dither);
+    cudaFree(h->pfx.bloom); cudaFree(h->pfx.sun); cudaFree(h->pfx.dither); cudaFree(h->pfx.mask);
     if (h->comm) { ncdl::api().CommDestroy(h->comm); h->comm = nullptr; }
     for (auto& e : h->mark) if (e) cudaEventDestroy(e);
     for (auto& e : h->tev) if (e) cudaEventDestroy(e);
@@ -2090,23 +2093,32 @@ static int need_dither_target(fluid_t* h, int dw, int dh) {
     return FLUID_OK;
 }
 
-// The bloom FBO and the sunrays texture a display kernel samples, as post_fx_chains left them
-struct PostFXOut { int bw, bh, sw, sh; };
+// slab SUNRAYS: the one-channel Wd x Hd buffer the ranks gather the mask's alpha into; made like a post-FX target
+static int need_mask_target(fluid_t* h, int w, int hh) {
+    auto& t = h->pfx;
+    if (t.mask && t.mw == w && t.mh == hh) return FLUID_OK;
+    t.mw = t.mh = 0;
+    if (int rc = remake_target(h, (void**)&t.mask, (size_t)w * hh * sizeof(float), "the gathered sunrays mask")) return rc;
+    t.mw = w; t.mh = hh;
+    return FLUID_OK;
+}
 
-// The post-FX chains of render() for the keywords that are on: applyBloom (S:1350-1394) with BLOOM,
-// applySunrays + blur(…, 1) (S:1396-1419; the mask is drawn into dye.write exactly like S:1300) with
-// SUNRAYS.  FBO sizes follow initBloomFramebuffers / initSunraysFramebuffers (S:1012-1043), which size
-// them from the drawing buffer: canvas_w x canvas_h.  Sd: the dye's storage policy (the mask is drawn in
-// it), St: the targets', Smp: the sampler of every texture the chains read (postfx.cuh).  BATCH: a batch
-// handle's B members, each target a dense (B, h, w) array and each launch B layers of blocks deep.  Single
-// GPU, arguments checked by the caller.
-extern "C++" {
-template <class Sd, class St, class Smp, bool BATCH = false>
-static int post_fx_chains(fluid_t* h, uint32_t keywords, const fluid_postfx* fx, const float* dither_rgb,
-                          int dw, int dh, int canvas_w, int canvas_h, PostFXOut* o) {
-    using D4 = typename Sd::T4;
-    using T4 = typename St::T4;
-    using T1 = typename St::T1;
+// Dye ghost rows a slab frame samples beyond the rows a rank owns (slab.py draw_ghost_rows).  A band starts at
+// floor(n * rank / world) on every grid, so a target band may begin up to one target row before the dye rows it
+// covers: the display + shading taps of a `height`-row target reach less than 1.5 Hd / height + 1.5 rows, the
+// bloom prefilter's taps of a bh-row FBO less than Hd / (2 bh) + 1.5, the sunrays mask's (at dye texel centres)
+// one.  bh = 0: no prefilter.  The same on every rank: the exchange sizes must match.
+int draw_ghost_rows(int Hd, int height, int bh, bool mask) {
+    long long need = (3LL * Hd + 2LL * height - 1) / (2LL * height) + 2;
+    if (bh > 0) need = std::max(need, ((long long)Hd + 2LL * bh - 1) / (2LL * bh) + 2);
+    if (mask) need = std::max(need, 1LL);
+    return (int)std::min<long long>(need, 1 << 30);
+}
+
+// The FBO sizes of a frame's post-FX chains (initBloomFramebuffers / initSunraysFramebuffers, S:1012-1043, sized
+// from the canvas_w x canvas_h drawing buffer) and the bloom pyramid's depth
+struct PostFXOut { int bw, bh, sw, sh, levels; };
+static int post_fx_sizes(fluid_t* h, uint32_t keywords, const fluid_postfx* fx, int canvas_w, int canvas_h, PostFXOut* o) {
     const bool bloom_on = keywords & FLUID_DISPLAY_BLOOM, sun_on = keywords & FLUID_DISPLAY_SUNRAYS;
     int bw = 1, bh = 1, sw = 1, sh = 1, levels = 0;
     if (bloom_on) fluid_get_resolution(fx->bloom_resolution, canvas_w, canvas_h, &bw, &bh);
@@ -2114,18 +2126,48 @@ static int post_fx_chains(fluid_t* h, uint32_t keywords, const fluid_postfx* fx,
     if (bw < 1 || bh < 1 || sw < 1 || sh < 1) return fail(h, FLUID_ERR_INVALID, "bad post-FX resolution");
     if (bloom_on)
         while (levels < fx->bloom_iterations && (bw >> (levels + 1)) >= 2 && (bh >> (levels + 1)) >= 2) ++levels;
+    *o = {bw, bh, sw, sh, levels};
+    return FLUID_OK;
+}
+
+// The targets of the chains that are on, and the dithering texture's upload (BLOOM); a slab's gathered mask (SUNRAYS)
+static int post_fx_targets(fluid_t* h, uint32_t keywords, const PostFXOut& o, const float* dither_rgb, int dw, int dh) {
     int rc;
-    if (bloom_on) {
-        if ((rc = need_bloom_targets(h, bw, bh, levels)) || (rc = need_dither_target(h, dw, dh))) return rc;
+    if (keywords & FLUID_DISPLAY_BLOOM) {
+        if ((rc = need_bloom_targets(h, o.bw, o.bh, o.levels)) || (rc = need_dither_target(h, dw, dh))) return rc;
         CU(cudaMemcpyAsync(h->pfx.dither, dither_rgb, (size_t)dw * dh * 3 * sizeof(float), cudaMemcpyHostToDevice, h->stream));
     }
-    if (sun_on && (rc = need_sunrays_targets(h, sw, sh))) return rc;
-    *o = {bw, bh, sw, sh};
+    if (keywords & FLUID_DISPLAY_SUNRAYS) {
+        if ((rc = need_sunrays_targets(h, o.sw, o.sh))) return rc;
+        if (h->slab() && (rc = need_mask_target(h, h->cfg.dye_w, h->cfg.dye_h))) return rc;
+    }
+    return FLUID_OK;
+}
+
+// The post-FX chains of render() for the keywords that are on, into the targets post_fx_targets made: applyBloom
+// (S:1350-1394) with BLOOM, applySunrays + blur(…, 1) (S:1396-1419; the mask is drawn into dye.write exactly like
+// S:1300) with SUNRAYS.  Sd: the dye's storage policy (the mask is drawn in it), St: the targets', Smp: the sampler
+// of every texture the chains read (postfx.cuh).  BATCH: a batch handle's B members, each target a dense (B, h, w)
+// array and each launch B layers of blocks deep.  Arguments checked by the caller.
+// A slab rank (fp32, LINEAR) prefilters its band of the bloom FBO's rows and draws the mask on the dye rows it
+// owns; the bands are gathered (halo.cuh gather_bands), so every rank runs the pyramid, the sunrays and the blurs
+// on the inputs one GPU has and ends with its bits.  The dye ghost rows must be fresh (draw_ghost_rows).
+extern "C++" {
+template <class Sd, class St, class Smp, bool BATCH = false>
+static int post_fx_chains(fluid_t* h, uint32_t keywords, const fluid_postfx* fx, const PostFXOut& o) {
+    using D4 = typename Sd::T4;
+    using T4 = typename St::T4;
+    using T1 = typename St::T1;
+    constexpr bool kSlab = !BATCH && std::is_same<Sd, StoreF32>::value && std::is_same<St, StoreF32>::value &&
+                           std::is_same<Smp, Linear>::value;
+    if (h->slab() && !kSlab) return fail(h, FLUID_ERR_INVALID, "post-FX on a slab handle is fp32 and LINEAR only");
+    const bool bloom_on = keywords & FLUID_DISPLAY_BLOOM, sun_on = keywords & FLUID_DISPLAY_SUNRAYS;
+    const int bw = o.bw, bh = o.bh, sw = o.sw, sh = o.sh, levels = o.levels;
     const int Wd = h->cfg.dye_w, Hd = h->cfg.dye_h, B = h->members;
     T4* bloom = static_cast<T4*>(h->pfx.bloom);
     T1 *sun = static_cast<T1*>(h->pfx.sun), *sun2 = sun ? sun + (size_t)sw * sh * B : nullptr;
     dim3 b(32, 8);
-    int nk = 0;
+    int nk = 0, rc;
     // ---- applyBloom(dye.read, bloom) ----------------------------------------------------------------
     if (bloom_on && levels >= 2) {
         struct Lv { T4* p; int w, h; };
@@ -2137,10 +2179,14 @@ static int post_fx_chains(fluid_t* h, uint32_t keywords, const fluid_postfx* fx,
             p += (size_t)pw * ph * B;
         }
         const double knee = fx->bloom_threshold * fx->bloom_soft_knee + 0.0001;
-        bloom_prefilter_kernel<Sd, St, Smp, BATCH><<<grid2d(bw, bh, b, B), b, 0, h->stream>>>(
-            (const D4*)h->dye.read, Wd, Hd, bloom, bw, bh, (float)(fx->bloom_threshold - knee),
-            (float)(knee * 2), (float)(0.25 / knee), (float)fx->bloom_threshold);
-        ++nk;
+        const int j_lo = band_row(bh, h->rank, h->world), j_hi = band_row(bh, h->rank + 1, h->world);
+        if (j_hi > j_lo) {
+            bloom_prefilter_kernel<Sd, St, Smp, BATCH><<<grid2d(bw, j_hi - j_lo, b, B), b, 0, h->stream>>>(
+                (const D4*)h->dye.read, Wd, Hd, h->droff, bloom, bw, bh, j_lo, j_hi, (float)(fx->bloom_threshold - knee),
+                (float)(knee * 2), (float)(0.25 / knee), (float)fx->bloom_threshold);
+            ++nk;
+        }
+        if ((rc = gather_bands(h, GB_BLOOM))) return rc;
         Lv last{bloom, bw, bh};
         for (auto& d : pyr) {
             box4_kernel<St, Smp, BATCH><<<grid2d(d.w, d.h, b, B), b, 0, h->stream>>>(last.p, last.w, last.h, d.p, d.w, d.h, 1.0f, 0);
@@ -2155,8 +2201,20 @@ static int post_fx_chains(fluid_t* h, uint32_t keywords, const fluid_postfx* fx,
     }
     // ---- applySunrays(dye.read, dye.write, sunrays); blur(sunrays, sunraysTemp, 1) -------------------
     if (sun_on) {
-        sunrays_mask_kernel<Sd, Smp, BATCH><<<grid2d(Wd, Hd, b, B), b, 0, h->stream>>>((const D4*)h->dye.read, (D4*)h->dye.write, Wd, Hd);
-        sunrays_kernel<Sd, St, Smp, BATCH><<<grid2d(sw, sh, b, B), b, 0, h->stream>>>((const D4*)h->dye.write, Wd, Hd, sun, sw, sh, (float)fx->sunrays_weight);
+        bool gathered = false;
+        if constexpr (kSlab) {
+            if (h->slab()) {
+                sunrays_mask_kernel<Sd, Smp><<<grid2d(Wd, h->drow1 - h->drow0, b), b, 0, h->stream>>>(
+                    (const D4*)h->dye.read, (D4*)h->dye.write, Wd, Hd, h->drow0, h->drow1, h->droff, h->pfx.mask);
+                if ((rc = gather_bands(h, GB_MASK))) return rc;
+                sunrays_kernel<Sd, St, Smp, false, float><<<grid2d(sw, sh, b), b, 0, h->stream>>>(h->pfx.mask, Wd, Hd, sun, sw, sh, (float)fx->sunrays_weight);
+                gathered = true;
+            }
+        }
+        if (!gathered) {
+            sunrays_mask_kernel<Sd, Smp, BATCH><<<grid2d(Wd, Hd, b, B), b, 0, h->stream>>>((const D4*)h->dye.read, (D4*)h->dye.write, Wd, Hd, 0, Hd, 0, nullptr);
+            sunrays_kernel<Sd, St, Smp, BATCH><<<grid2d(sw, sh, b, B), b, 0, h->stream>>>((const D4*)h->dye.write, Wd, Hd, sun, sw, sh, (float)fx->sunrays_weight);
+        }
         blur3_kernel<St, Smp, BATCH><<<grid2d(sw, sh, b, B), b, 0, h->stream>>>(sun, sun2, sw, sh, (float)(1.0 / (double)sw), 0.0f);
         blur3_kernel<St, Smp, BATCH><<<grid2d(sw, sh, b, B), b, 0, h->stream>>>(sun2, sun, sw, sh, 0.0f, (float)(1.0 / (double)sh));
         nk += 4;
@@ -2166,7 +2224,7 @@ static int post_fx_chains(fluid_t* h, uint32_t keywords, const fluid_postfx* fx,
 
 // post_fx_chains<Sd, St, Smp> of a handle: the dye's and the targets' storage, and the sampler.  A batch handle
 // is fp32 and LINEAR.
-using Chains = int (*)(fluid_t*, uint32_t, const fluid_postfx*, const float*, int, int, int, int, PostFXOut*);
+using Chains = int (*)(fluid_t*, uint32_t, const fluid_postfx*, const PostFXOut&);
 template <class Smp>
 static Chains chains_for(const fluid_t* h) {
     return !h->half_fx ? post_fx_chains<StoreF32, StoreF32, Smp>
@@ -2241,8 +2299,9 @@ struct DrawRequest {
 
 // render(target) of S:1296-1317: the post-FX chains of the keywords that are on, then the background and
 // drawDisplay in one display_kernel launch, read back to the host (or, for a capture or canvas into device
-// memory, left on the stream for the caller's fluid_sync).  Only the fp32 frame without BLOOM and
-// SUNRAYS is drawn on a slab handle, and there only the handle's band of the target (fluid_render_band).
+// memory, left on the stream for the caller's fluid_sync).  A slab handle draws its band of the target
+// (fluid_render_band) after one refresh of the dye ghost rows the frame samples; with BLOOM or SUNRAYS the
+// call is collective (post_fx_chains gathers), so every argument check comes before the first exchange.
 // Half storage draws from a widened copy of dye; its post-FX needs FLUID_FLAG_HALF_POSTFX, and then the
 // chains read the fp16 dye directly and draw the mask into the fp16 dye.write.  A batch request draws every
 // member of a batch handle through the same launches, each launch B layers of blocks deep; only batch requests
@@ -2254,39 +2313,39 @@ static int draw(fluid_t* h, const DrawRequest& r) {
     if (r.keywords & ~(uint32_t)(FLUID_DISPLAY_SHADING | FLUID_DISPLAY_BLOOM | FLUID_DISPLAY_SUNRAYS))
         return fail(h, FLUID_ERR_INVALID, "unknown display keyword bits 0x%x", r.keywords);
     const bool bloom_on = r.keywords & FLUID_DISPLAY_BLOOM, sun_on = r.keywords & FLUID_DISPLAY_SUNRAYS;
-    const bool postfx = bloom_on || sun_on, band = !postfx && r.out == OUT_FRAME, bytes = r.out != OUT_FRAME;
+    const bool postfx = bloom_on || sun_on, bytes = r.out != OUT_FRAME;
     if (!r.dst || r.width < 1 || r.height < 1 || r.canvas_w < 1 || r.canvas_h < 1 || (postfx && !r.fx) ||
         (bloom_on && (!r.dither || r.dw < 1 || r.dh < 1)))
         return fail(h, FLUID_ERR_INVALID, "bad argument");
     int y0 = 0, y1 = r.height;
-    if (band) fluid_render_band(h, r.height, &y0, &y1);
+    if (h->slab()) fluid_render_band(h, r.height, &y0, &y1);
     const size_t cells = (size_t)r.width * (y1 - y0), images = h->members;
     if (r.batch && r.n != 4 * cells * images)
         return fail(h, FLUID_ERR_INVALID, "%s: the targets of %d members have %zu bytes, caller passed %zu", r.what,
                     h->members, 4 * cells * images, r.n);
     if (r.n != 4 * cells * images)
-        return fail(h, FLUID_ERR_INVALID, "%s: the target%s has %zu %s, caller passed %zu", r.what, band ? " band" : "",
+        return fail(h, FLUID_ERR_INVALID, "%s: the target%s has %zu %s, caller passed %zu", r.what, h->slab() ? " band" : "",
                     4 * cells, bytes ? "bytes" : "floats", r.n);
-    if (cells == 0) return FLUID_OK;
-    if (h->slab() && !band) return not_on_slab(h, r.what);
+    if (cells == 0 && !h->slab()) return FLUID_OK;      // a slab rank with no rows still takes part in the exchanges
     if (h->half && !h->half_fx && postfx)
         return fail(h, FLUID_ERR_INVALID, "%s with BLOOM or SUNRAYS is not built for FLUID_FLAG_HALF_STORAGE "
                     "(the reference's bloom / sunrays FBOs are fp16 too: add FLUID_FLAG_HALF_POSTFX)", r.what);
-    int rc = r.on_device ? check_device_buf(h, r.what, r.dst, r.n)
-                         : need_frame(h, bytes ? (cells * images + 3) / 4 : cells);     // uchar4 images live in the frame
+    PostFXOut o{};
+    int rc = postfx ? post_fx_sizes(h, r.keywords, r.fx, r.canvas_w, r.canvas_h, &o) : FLUID_OK;
     if (rc) return rc;
+    rc = r.on_device ? check_device_buf(h, r.what, r.dst, r.n)
+                     : need_frame(h, bytes ? (cells * images + 3) / 4 : cells);     // uchar4 images live in the frame
+    if (rc) return rc;
+    if (postfx && (rc = post_fx_targets(h, r.keywords, o, r.dither, r.dw, r.dh))) return rc;
     if (h->slab()) {
-        // the band's display + shading taps reach ceil(Hd / height) + 2 dye rows beyond the owned ones:
-        // refresh that many ghost rows (the ghost rows of dye.read are stale after advection)
-        const int need = (h->cfg.dye_h + r.height - 1) / r.height + 2;
+        // refresh the dye ghost rows the frame's taps reach (those of dye.read are stale after advection); every
+        // rank computes the same depth
+        const int need = draw_ghost_rows(h->cfg.dye_h, r.height, bloom_on && o.levels >= 2 ? o.bh : 0, sun_on);
         if ((rc = exchange_rows(h, HB_DYE, std::min(h->Gd, need)))) return rc;
         if (need > h->Gd)
-            return fail(h, FLUID_ERR_HALO, "render target of %d rows needs %d dye ghost rows, the slab keeps %d", r.height, need, h->Gd);
+            return fail(h, FLUID_ERR_HALO, "a frame of a %d-row target needs %d dye ghost rows, the slab keeps %d", r.height, need, h->Gd);
     }
-    PostFXOut o{};
-    if (postfx) {
-        if ((rc = chains_of(h)(h, r.keywords, r.fx, r.dither, r.dw, r.dh, r.canvas_w, r.canvas_h, &o))) return rc;
-    }
+    if (postfx && (rc = chains_of(h)(h, r.keywords, r.fx, o))) return rc;
     const float4* dye_src;
     if ((rc = display_source(h, &dye_src))) return rc;
     // texelSize = 1 / width, 1 / height (S:1337) and getTextureScale (S:1626-1631) are JS doubles, narrowed here
@@ -2299,8 +2358,10 @@ static int draw(fluid_t* h, const DrawRequest& r) {
                         h->cfg.aspect, ts};
     dim3 b(32, 8);
     const DisplayKernel k = h->batch ? kDisplayBatch[r.out][r.keywords] : kDisplay[h->nearest][r.out][h->half_fx][r.keywords];
-    k<<<grid2d(r.width, y1 - y0, b, h->members), b, 0, h->stream>>>(a);
-    if ((rc = check_launch(h, "display_kernel"))) return rc;
+    if (cells > 0) {
+        k<<<grid2d(r.width, y1 - y0, b, h->members), b, 0, h->stream>>>(a);
+        if ((rc = check_launch(h, "display_kernel"))) return rc;
+    }
     if (r.on_device) return FLUID_OK;
     CU(cudaMemcpyAsync(r.dst, h->frame, r.n * (bytes ? 1 : sizeof(float)), cudaMemcpyDeviceToHost, h->stream));
     std::vector<__half> bloom16, sun16;
@@ -2469,6 +2530,7 @@ uint64_t fluid_stat(fluid_t* h, int key) {
         case FLUID_STAT_CVD_STREAM_LAUNCHES: return h->launches.cvd_stream;
         case FLUID_STAT_GRADIENT_STREAM_LAUNCHES: return h->launches.gradient_stream;
         case FLUID_STAT_ADVECT4_LAUNCHES: return h->launches.advect4;
+        case FLUID_STAT_GATHERS: return h->gathers;
         case FLUID_STAT_JACOBI_EXACT_STREAMS: {          // counted on the device: waits for the handle's work
             unsigned long long n = 0;
             if (cudaMemcpyAsync(&n, h->exact_streams, sizeof n, cudaMemcpyDeviceToHost, h->stream) != cudaSuccess ||

@@ -1,6 +1,7 @@
 // halo.cuh — slab halo exchange: the peer-memory transport (IPC-mapped arenas, one push kernel with
-// the free/ready handshake) and the NCCL send/recv fallback.  Included by fluid.cu inside its
-// anonymous namespace, after `struct fluid`, fail(), CU() and check_launch() are defined.
+// the free/ready handshake) and the NCCL send/recv fallback; and the all-gather of row bands that
+// post-FX on slabs runs (NCCL only).  Included by fluid.cu inside its anonymous namespace, after
+// `struct fluid`, fail(), CU() and check_launch() are defined.
 #pragma once
 
 // ---- halo exchange (NCCL point-to-point; all buffers and both neighbours in ONE group) ------------
@@ -198,3 +199,49 @@ int exchange_rows(fluid_t* h, int which, int n) {
     return exchange_many(h, &it, 1);
 }
 
+
+// ---- all-gather of row bands (post-FX on slabs) ----------------------------------------------------------
+// A dense `rows` x row_bytes buffer of which rank k computed the band [rows*k/world, rows*(k+1)/world) (the
+// fractions of the rows a rank owns): afterwards every rank holds every band.  One NCCL group in which each rank
+// sends its band to every other rank and receives theirs in place.  NCCL even when the peer-memory halo path is
+// on: its IPC mappings reach only the two neighbours.
+// `which` names the buffer: the bloom FBO (prefiltered) or the sunrays mask's one-channel alpha.
+enum { GB_BLOOM = 0, GB_MASK = 1 };
+struct GatherRows { char* base; size_t row_bytes; int rows; };
+GatherRows gather_rows(const fluid_t* h, int which) {
+    if (which == GB_BLOOM) return {(char*)h->pfx.bloom, (size_t)h->pfx.bw * sizeof(float4), h->pfx.bh};
+    return {(char*)h->pfx.mask, (size_t)h->cfg.dye_w * sizeof(float), h->cfg.dye_h};
+}
+inline int band_row(int rows, int k, int world) { return (int)((long long)rows * k / world); }
+
+#ifdef FLUID_TEST_LOOPBACK_GATHER
+// tests/slab_loopback_gather.cu: the ranks of one process on one device, bands moved by stream-ordered device copies
+int gather_loopback(fluid_t* h, int which);
+#endif
+
+int gather_bands(fluid_t* h, int which) {
+    if (!h->slab()) return FLUID_OK;
+#ifdef FLUID_TEST_LOOPBACK
+#ifdef FLUID_TEST_LOOPBACK_GATHER
+    const int lrc = gather_loopback(h, which);
+    if (!lrc) ++h->gathers;
+    return lrc;
+#else
+    return fail(h, FLUID_ERR_INVALID, "this loopback build has no row-band gather (build it with FLUID_TEST_LOOPBACK_GATHER)");
+#endif
+#endif
+    const GatherRows g = gather_rows(h, which);
+    ncdl::Api& N = ncdl::api();
+    int rc = N.GroupStart();
+    for (int k = 0; k < h->world && !rc; ++k) {
+        if (k == h->rank) continue;
+        const int my0 = band_row(g.rows, h->rank, h->world), my1 = band_row(g.rows, h->rank + 1, h->world);
+        const int k0 = band_row(g.rows, k, h->world), k1 = band_row(g.rows, k + 1, h->world);
+        if (my1 > my0) rc = N.Send(g.base + (size_t)my0 * g.row_bytes, (size_t)(my1 - my0) * g.row_bytes, ncdl::ncclInt8, k, h->comm, h->stream);
+        if (!rc && k1 > k0) rc = N.Recv(g.base + (size_t)k0 * g.row_bytes, (size_t)(k1 - k0) * g.row_bytes, ncdl::ncclInt8, k, h->comm, h->stream);
+    }
+    const int rc2 = N.GroupEnd();
+    if (rc || rc2) return fail(h, FLUID_ERR_NCCL, "NCCL row-band gather failed: %s", N.GetErrorString(rc ? rc : rc2));
+    ++h->gathers;
+    return FLUID_OK;
+}

@@ -57,16 +57,19 @@ __device__ __forceinline__ const T* member_of(const void* p, int w, int h) {
     return q;
 }
 
-// bloomPrefilterShader S:614-631
+// bloomPrefilterShader S:614-631, on rows [j_lo, j_hi) of the w x h bloom FBO.  The dye's first row is global
+// row dye_row_off: a slab rank draws its band of the FBO from its own dye rows (+ ghost rows); one GPU draws
+// every row from the whole dye.
 template <class Sd, class St, class Smp, bool BATCH = false>
 __global__ void __launch_bounds__(256) bloom_prefilter_kernel(const typename Sd::T4* __restrict__ dye, int Wd, int Hd,
-                                                              typename St::T4* __restrict__ out, int w, int h, float curve0,
-                                                              float curve1, float curve2, float threshold) {
+                                                              int dye_row_off, typename St::T4* __restrict__ out, int w,
+                                                              int h, int j_lo, int j_hi, float curve0, float curve1,
+                                                              float curve2, float threshold) {
     if constexpr (BATCH) { dye += member_offset(Wd, Hd); out += member_offset(w, h); }
-    const int i = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y * blockDim.y + threadIdx.y;
-    if (i >= w || j >= h) return;
+    const int i = blockIdx.x * blockDim.x + threadIdx.x, j = j_lo + blockIdx.y * blockDim.y + threadIdx.y;
+    if (i >= w || j >= j_hi) return;
     const float uvx = ((float)i + 0.5f) / (float)w, uvy = ((float)j + 0.5f) / (float)h;
-    const float4 c = Smp::template fetch<Sd>(dye, Wd, Hd, uvx, uvy);
+    const float4 c = Smp::template fetch<Sd>(dye, Wd, Hd, uvx, uvy, dye_row_off);
     const float br = fmaxf(c.x, fmaxf(c.y, c.z));
     float rq = fminf(fmaxf(br - curve0, 0.0f), curve1);
     rq = (curve2 * rq) * rq;
@@ -96,23 +99,33 @@ __global__ void __launch_bounds__(256) box4_kernel(const typename St::T4* __rest
     St::st(dst, o, s);
 }
 
-// sunraysMaskShader S:676-691 (target = dye.write, like the reference: S:1300, so stored as the dye is)
+// sunraysMaskShader S:676-691 (target = dye.write, like the reference: S:1300, so stored as the dye is), on dye
+// rows [j_lo, j_hi); dye and mask are buffers whose first row is global row row_off.  alpha, when not null, also
+// receives the mask's alpha at global row j of a dense Wd x Hd array: the band a slab rank gathers (fp32 dye only).
 template <class Sd, class Smp, bool BATCH = false>
 __global__ void __launch_bounds__(256) sunrays_mask_kernel(const typename Sd::T4* __restrict__ dye,
-                                                           typename Sd::T4* __restrict__ mask, int Wd, int Hd) {
+                                                           typename Sd::T4* __restrict__ mask, int Wd, int Hd,
+                                                           int j_lo, int j_hi, int row_off, float* __restrict__ alpha) {
     if constexpr (BATCH) { dye += member_offset(Wd, Hd); mask += member_offset(Wd, Hd); }
-    const int i = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y * blockDim.y + threadIdx.y;
-    if (i >= Wd || j >= Hd) return;
+    const int i = blockIdx.x * blockDim.x + threadIdx.x, j = j_lo + blockIdx.y * blockDim.y + threadIdx.y;
+    if (i >= Wd || j >= j_hi) return;
     const float uvx = ((float)i + 0.5f) / (float)Wd, uvy = ((float)j + 0.5f) / (float)Hd;
-    float4 c = Smp::template fetch<Sd>(dye, Wd, Hd, uvx, uvy);
+    float4 c = Smp::template fetch<Sd>(dye, Wd, Hd, uvx, uvy, row_off);
     const float br = fmaxf(c.x, fmaxf(c.y, c.z));
     c.w = 1.0f - fminf(fmaxf(br * 20.0f, 0.0f), 0.8f);
-    Sd::st(mask, (size_t)j * Wd + i, c);
+    Sd::st(mask, (size_t)(j - row_off) * Wd + i, c);
+    if (alpha) alpha[(size_t)j * Wd + i] = c.w;
 }
 
-// sunraysShader S:693-724
-template <class Sd, class St, class Smp, bool BATCH = false>
-__global__ void __launch_bounds__(256) sunrays_kernel(const typename Sd::T4* __restrict__ mask, int Wm, int Hm,
+// the mask value the sunrays shader reads: .a of the RGBA mask, or the one-channel gathered alpha.  LINEAR and
+// NEAREST filter each channel on its own, so both give the same bits.
+__device__ __forceinline__ float mask_alpha(float4 v) { return v.w; }
+__device__ __forceinline__ float mask_alpha(float v) { return v; }
+
+// sunraysShader S:693-724.  M: the mask's texel type, Sd::T4 (the mask in dye.write) or float (a slab's
+// gathered alpha).
+template <class Sd, class St, class Smp, bool BATCH = false, class M = typename Sd::T4>
+__global__ void __launch_bounds__(256) sunrays_kernel(const M* __restrict__ mask, int Wm, int Hm,
                                                       typename St::T1* __restrict__ out, int w, int h, float weight) {
     if constexpr (BATCH) { mask += member_offset(Wm, Hm); out += member_offset(w, h); }
     const int i = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y * blockDim.y + threadIdx.y;
@@ -124,11 +137,11 @@ __global__ void __launch_bounds__(256) sunrays_kernel(const typename Sd::T4* __r
     float dx = uvx - 0.5f, dy = uvy - 0.5f;
     dx = dx * f; dy = dy * f;
     float illum = 1.0f;
-    float color = Smp::template fetch<Sd>(mask, Wm, Hm, uvx, uvy).w;
+    float color = mask_alpha(Smp::template fetch<Sd>(mask, Wm, Hm, uvx, uvy));
 #pragma unroll 1
     for (int k = 0; k < 16; ++k) {
         cx = cx - dx; cy = cy - dy;
-        const float col = Smp::template fetch<Sd>(mask, Wm, Hm, cx, cy).w;
+        const float col = mask_alpha(Smp::template fetch<Sd>(mask, Wm, Hm, cx, cy));
         color = color + (col * illum) * weight;
         illum = illum * Decay;
     }

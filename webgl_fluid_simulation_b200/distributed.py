@@ -5,6 +5,8 @@ from __future__ import annotations
 import ctypes as C
 import os
 
+import numpy as np
+
 from . import _lib
 from .sim import FluidSimulation
 
@@ -56,3 +58,16 @@ def connect_peers(sim: FluidSimulation) -> bool:
         sim._check(L.fluid_p2p_disable(sim._h))
         return False
     return True
+
+
+def gather_image(band, bottom_first: bool = False):
+    """Every rank of the group calls this with the band its slab drew; rank 0 gets the whole image, the others
+    None.  bottom_first: render()'s fp32 frame (row 0 at the bottom), whose bands stack in rank order; otherwise a
+    canvas or capture (top row first), whose bands stack in reverse rank order."""
+    import torch.distributed as dist
+    rank, world = dist.get_rank(), dist.get_world_size()
+    parts = [None] * world if rank == 0 else None
+    dist.gather_object(np.ascontiguousarray(band), parts, dst=0)
+    if rank != 0:
+        return None
+    return np.concatenate(parts if bottom_first else parts[::-1], axis=0)

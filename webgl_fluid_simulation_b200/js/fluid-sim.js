@@ -33,7 +33,7 @@ const DISPLAY = { SHADING: 0x1, BLOOM: 0x2, SUNRAYS: 0x4 };
 const FLAG = { UNFUSED: 0x1, NO_GRAPH: 0x2, NAIVE_JACOBI: 0x4, TILED_PASSES: 0x8, HALF_STORAGE: 0x10, HALF_POSTFX: 0x20,
                NEAREST_FILTERING: 0x40, LINEAR_ADVECTION: 0x80 };
 const STAT = { launches: 0, jacobiLaunches: 1, haloLaunches: 2, haloExchanges: 3, graphCaptures: 4, graphLaunches: 5, haloTransportP2P: 6,
-               cvdStreamLaunches: 7, gradientStreamLaunches: 8, jacobiExactStreams: 9, advect4Launches: 10 };
+               cvdStreamLaunches: 7, gradientStreamLaunches: 8, jacobiExactStreams: 9, advect4Launches: 10, gathers: 11 };
 
 function pointerPrototype () {                                  // S:87-98
     this.id = -1;

@@ -562,12 +562,15 @@ class FluidSimulation(_Handle):
         drawn over the checkerboard on the screen (target=False, S:1311-1312) and bare, un-blended,
         into a capture target (target=True: what captureScreenshot renders into, S:287-299).
         config.SHADING / BLOOM / SUNRAYS pick the display keywords like updateKeywords (S:1160-1166);
-        BLOOM needs `sim.dithering`.  BLOOM or SUNRAYS need a single-GPU handle, fp32 or created with
+        BLOOM needs `sim.dithering`.  BLOOM or SUNRAYS need an fp32 handle or one created with
         FLAG_HALF_POSTFX (then the bloom and sunrays targets are fp16, as are the reference's; with
         FLAG_HALF_STORAGE | FLAG_HALF_POSTFX this is the reference's desktop frame; FLAG_LINEAR_ADVECTION
         changes how step() advects, not how a frame is drawn).  last_bloom /
         last_sunrays hold the bloom FBO / sunrays texture of the frame (widened to float32), or None when
-        that keyword is off."""
+        that keyword is off.
+        On a slab rank: the rank's band of the target, rows render_band = (y0, y1) (fluid_render_band), for
+        every keyword set; bands concatenate in rank order.  With BLOOM or SUNRAYS every rank must call with
+        the same arguments (the ranks gather the post-FX inputs), and last_bloom / last_sunrays are whole."""
         w = int(width or self.canvas["width"]); h = int(height or self.canvas["height"])
         bc = self.config["BACK_COLOR"]                       # normalizeColor, S:1599-1606
         out = np.empty((h, w, 4), np.float32)
@@ -585,11 +588,8 @@ class FluidSimulation(_Handle):
         if kw & DISPLAY_SUNRAYS:
             sr = getResolution(cfg["SUNRAYS_RESOLUTION"], w, h)
             self.last_sunrays = np.empty((sr["height"], sr["width"]), np.float32)
-        if fx is None:                                       # a slab rank draws its band of the target only
-            y0, y1 = C.c_int(), C.c_int()
-            self._check(self._L.fluid_render_band(self._h, h, C.byref(y0), C.byref(y1)))
-            out = out[: y1.value - y0.value]
-            self.render_band = (y0.value, y1.value)
+        y0, y1 = self._band(h)                               # a slab rank draws its band of the target only
+        out = out[: y1 - y0]
         ptr = lambda a: None if a is None else a.ctypes.data_as(C.c_void_p)   # noqa: E731
         self._check(self._L.fluid_render_keywords(
             self._h, w, h, kw, None if fx is None else C.byref(fx), ptr(dith),
@@ -606,17 +606,25 @@ class FluidSimulation(_Handle):
         With `path`, also writes the image as a PNG (write_png: the bytes unchanged).
         `out`: a C-contiguous uint8 CUDA array on the handle's device of exactly 4 * w * h bytes (e.g. a torch
         tensor): the display kernel stores the image into it, with no host copy and render_canvas's waits, and
-        the array is returned as it was passed.  A PNG needs host bytes, so `path` with `out` is refused."""
+        the array is returned as it was passed.  A PNG needs host bytes, so `path` with `out` is refused.
+        On a slab rank: the rank's band, (y1 - y0, w, 4) top row first, rows render_band = (y0, y1) of the
+        bottom-up target; the whole image is the bands in reverse rank order (distributed.gather_image).  A PNG
+        needs the whole image, so `path` is refused there."""
         w, h, args = self._capture_args()
         if out is not None:
             if not hasattr(out, "__cuda_array_interface__"):
                 raise ValueError("captureScreenshot(out=...) takes a CUDA array; without `out` it returns a numpy image")
             if path is not None:
                 raise ValueError("captureScreenshot writes a PNG from host bytes: pass `path` or a CUDA `out`, not both")
-        dst = _device_array(out, "|u1", 4 * w * h, "captureScreenshot")
-        img = np.empty((h, w, 4), np.uint8) if dst is None else None
+        if path is not None and self._world > 1:
+            raise ValueError("captureScreenshot(path=...) needs the whole image: a slab rank draws only its band "
+                             "(gather the bands with distributed.gather_image and write_png them)")
+        y0, y1 = self._band(h)
+        n = 4 * w * (y1 - y0)
+        dst = _device_array(out, "|u1", n, "captureScreenshot")
+        img = np.empty((y1 - y0, w, 4), np.uint8) if dst is None else None
         self._check((self._L.fluid_capture if dst is None else self._L.fluid_capture_device)(
-            self._h, w, h, *args, img.ctypes.data_as(C.c_void_p) if dst is None else dst, 4 * w * h))
+            self._h, w, h, *args, img.ctypes.data_as(C.c_void_p) if dst is None else dst, n))
         if dst is not None:
             self.sync()
             return out
@@ -637,13 +645,25 @@ class FluidSimulation(_Handle):
         use the array: the producer stream a version-3 interface names, or, where the interface names none
         (torch's is version 2), every queued kernel and copy of the array's device.  The handle's stream is
         synchronised before returning, so the array can be read at once.  A CUDA array is returned as it
-        was passed."""
+        was passed.
+        On a slab rank: the rank's band, (y1 - y0, width, 4) top row first, rows render_band = (y0, y1) of the
+        bottom-up canvas; the whole canvas is the bands in reverse rank order (distributed.gather_image), and
+        `out` holds the band.  With BLOOM or SUNRAYS every rank must call with the same config."""
         w, h, args = self._canvas_args()
-        dst, result, on_device = _u8_destination(out, (h, w, 4), "render_canvas")
-        self._check(self._L.fluid_render_canvas(self._h, w, h, *args, dst, 4 * w * h, 1 if on_device else 0))
+        y0, y1 = self._band(h)
+        dst, result, on_device = _u8_destination(out, (y1 - y0, w, 4), "render_canvas")
+        self._check(self._L.fluid_render_canvas(self._h, w, h, *args, dst, 4 * w * (y1 - y0), 1 if on_device else 0))
         if on_device:
             self.sync()
         return result
+
+    def _band(self, height):
+        """(y0, y1): the rows of a `height`-row target this handle draws (fluid_render_band; all of them on one
+        GPU), also kept as render_band."""
+        y0, y1 = C.c_int(), C.c_int()
+        self._check(self._L.fluid_render_band(self._h, int(height), C.byref(y0), C.byref(y1)))
+        self.render_band = (y0.value, y1.value)
+        return self.render_band
 
     @staticmethod
     def textureToCanvas(rgba: np.ndarray) -> np.ndarray:

@@ -1,9 +1,9 @@
 """Row-slab decomposition plan (SURVEY §8e) — the host-side arithmetic of the multi-GPU path.
 
 Mirrors csrc/fluid.cu (create_common; block_depth, the depth of a solve; JacobiPlan, the launch split that
-run_jacobi and solve_host_banded iterate over) so that the schedule can be checked on CPU
-(tests/test_slab_schedule_gloo.py, tests/test_band_schedule_cpu.py) and so that launchers know which rows a
-rank owns.
+run_jacobi and solve_host_banded iterate over; draw_ghost_rows and the bands of a slab frame) so that the schedule
+can be checked on CPU (tests/test_slab_schedule_gloo.py, tests/test_band_schedule_cpu.py,
+tests/test_slab_draw_plan_cpu.py) and so that launchers know which rows a rank owns.
 One process per GPU; rank g of G owns sim rows [g*H//G, (g+1)*H//G) and the matching dye rows.
 Messages (NCCL send/recv inside the library, both neighbours in one group) happen ONLY on:
   * Jacobi, communication-avoiding ("deep") form: ONE group per solve with iters+1 rows of pressure
@@ -12,7 +12,9 @@ Messages (NCCL send/recv inside the library, both neighbours in one group) happe
     (deepest) launch has sweeps, once, then K rows of pressure before each launch of depth K (K+1
     before the last, which also produces one row beyond each slab edge so that gradientSubtract
     needs no message);
-  * advection: G rows of the projected velocity, then Gd rows of dye.
+  * advection: G rows of the projected velocity, then Gd rows of dye;
+  * a frame (render, canvas, capture): draw_ghost_rows of dye, then with BLOOM / SUNRAYS one all-gather each of
+    the bands draw_plan gives (every rank ends with the whole prefiltered bloom FBO / sunrays mask).
 curl / vorticity / divergence run on ghost rows the previous step computed redundantly
 (velocity is advected on owned rows +-3: curl needs +-2, vorticity +-1, divergence +-0).
 """
@@ -127,3 +129,37 @@ class SlabPlan:
     def max_backtrace_rows(self) -> int:
         """Largest dt*|v| (in sim rows) the advection halo covers: G - ghost compute - bilinear tap."""
         return self.G - VELOCITY_GHOST - 2
+
+
+def draw_ghost_rows(dye_h: int, height: int, bloom_h: int = 0, sunrays: bool = False) -> int:
+    """Dye ghost rows a slab frame samples beyond the rows a rank owns (fluid.cu draw_ghost_rows), the same on every
+    rank.  Every band starts at floor(n * rank / world) of its own grid, so a band of a `height`-row target may begin
+    up to one target row before the dye rows it covers.  The display and shading taps (+-1 target row) then reach
+    less than 1.5 * dye_h / height + 1.5 dye rows beyond the owned ones, the bloom prefilter's band of a bloom_h-row
+    FBO less than dye_h / (2 * bloom_h) + 1.5, and the sunrays mask (at dye texel centres, its +y tap weighted 0)
+    one.  bloom_h = 0: no prefilter (BLOOM off, or a pyramid of fewer than 2 levels)."""
+    need = -(-3 * dye_h // (2 * height)) + 2
+    if bloom_h > 0:
+        need = max(need, -(-dye_h // (2 * bloom_h)) + 2)
+    if sunrays:
+        need = max(need, 1)
+    return need
+
+
+def draw_plan(dye_h: int, height: int, rank: int, world: int, bloom_h: int = 0, sunrays: bool = False) -> dict:
+    """What rank `rank` of `world` does for one frame of a `height`-row target: `band`, the target rows it draws
+    (fluid_render_band); `bloom_rows`, the rows of the bloom_h-row FBO it prefilters (None without a prefilter);
+    `mask_rows`, the dye rows it draws the sunrays mask on (its own; None without SUNRAYS); `ghost`, the dye ghost
+    rows it refreshes first; `gathers`, the all-gathers that follow."""
+    return dict(band=rows(height, rank, world),
+                bloom_rows=rows(bloom_h, rank, world) if bloom_h > 0 else None,
+                mask_rows=rows(dye_h, rank, world) if sunrays else None,
+                ghost=draw_ghost_rows(dye_h, height, bloom_h, sunrays),
+                gathers=int(bloom_h > 0) + int(sunrays))
+
+
+def gather_bytes(dye_w: int, dye_h: int, bloom_w: int = 0, bloom_h: int = 0, sunrays: bool = False) -> int:
+    """Bytes of the buffers one frame's gathers assemble: the prefiltered bloom FBO (RGBA fp32) and the sunrays
+    mask's alpha (fp32).  Each rank receives all of them but its own band, so a frame moves (world - 1) times this
+    in all."""
+    return 16 * bloom_w * bloom_h + (4 * dye_w * dye_h if sunrays else 0)
