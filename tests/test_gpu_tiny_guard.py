@@ -6,7 +6,9 @@ flagged in the tiny map (one byte per 128 columns x 32 rows, global rows), so th
 footprint covers it run the un-contracted tail.  The map has one producer per writer of divergence, each
 with its own indexing: cvd_stream_kernel (per lane, 120-column windows), the tiled fused kernel, the unfused
 divergence_kernel, tiny_scan_kernel behind fluid_write(DIVERGENCE), the one-piece host solve and every
-upload chunk of the banded host solve, and the map's allocation on create and resize.
+upload chunk of the banded host solve, and the map's allocation on create and resize.  The batch writer,
+cvd_stream_kernel<true>, flags one region of the map per member, which the batch form of the blocked kernel
+reads; tests/test_gpu_batch_edges.py places the same sites in different members of a batch step.
 
 The data here places tiny divergence on purpose where that indexing can go wrong: the grid's walls, both
 sides of every map-cell edge (columns 128k - 1 / 128k / 128k + 1, rows 32k - 1 / 32k / 32k + 1), both sides
