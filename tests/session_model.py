@@ -3,18 +3,23 @@ drives it.  Test infrastructure (CPU only).
 
 A session is a list of operations, each a plain tuple, applied in order to a handle and to a
 SessionModel in lockstep (tests/test_gpu_session.py).  The model holds what the handle should hold --
-velocity, dye, pressure, divergence, curl, sizes, canvas, config, storage mode -- and has one method per
+velocity, dye, pressure, divergence, curl, sizes, canvas, config, handle mode -- and has one method per
 operation, built from what already exists:
 
-  step                  oracle.OracleSim (fp32 or half_storage), its config attributes set live
-  resize                oracle.resample (+ round_half in half storage) when a size changes; pressure,
-                        divergence and curl start over at zero (fluid_resize, S:982-1010 + S:1116-1126)
+  step                  oracle.OracleSim (fp32 or half_storage), its config attributes set live;
+                        linear_advection_model.LinearOracleSim in the LINEAR modes
+  resize                oracle.resample (+ round_half in half storage) when a size changes, the NEAREST
+                        copy display_model.resize in the NEAREST modes; pressure, divergence and curl start
+                        over at zero (fluid_resize, S:982-1010 + S:1116-1126)
   pressure_solve, jacobi, pressure_solve_host
                         oracle.clear + oracle.jacobi; in half storage every blit rounded to fp16, the
                         host inputs too (they travel through fluid_write)
   splat, splats         splat_model.splat_interval: the handle's result is checked against the interval,
                         then ADOPTED, so that later operations stay comparable bit for bit
-  render, capture       display_model with the handle's storage; read-only
+  render, capture       display_model with the handle's storage and sampler; read-only
+
+A handle mode (MODES) is its storage and its sampler.  The storage picks the schedule, the generated
+operations and the data they write; the sampler changes only the model's step, resize and draws.
 
 Every array an operation writes is derived from the operation tuple alone (op_data), so a logged
 session can be replayed from its log.
@@ -29,10 +34,27 @@ import numpy as np
 
 import display_model as M
 import splat_model as SM
+from linear_advection_model import LinearOracleSim
 from oracle import oracle as O
 from sim_harness import nasty_fields, nasty_records, special_fields
 
 F32 = np.float32
+# handle modes: mode -> (half, sampler).  half: FLUID_FLAG_HALF_STORAGE | FLUID_FLAG_HALF_POSTFX (HALF_SCHEDULE);
+# sampler "manual": the MANUAL advection and LINEAR draws of an ordinary handle, "linear":
+# FLUID_FLAG_LINEAR_ADVECTION (with half storage the desktop browser's configuration), "nearest":
+# FLUID_FLAG_NEAREST_FILTERING (a WebGL device without float linear filtering: NEAREST draws and resize copy)
+MODES = {
+    "fp32": (False, "manual"),
+    "half": (True, "manual"),
+    "linear": (False, "linear"),
+    "desktop": (True, "linear"),
+    "nearest": (False, "nearest"),
+    "nearest_half": (True, "nearest"),
+}
+
+
+def is_half(mode: str) -> bool:
+    return MODES[mode][0]
 FIELDS = ("velocity", "dye", "pressure", "divergence", "curl")
 SIM_KEYS = ("DENSITY_DISSIPATION", "VELOCITY_DISSIPATION", "PRESSURE", "PRESSURE_ITERATIONS", "CURL", "SPLAT_RADIUS")
 TINY = 2.0 ** -123          # divergence below this defeats the blocked Jacobi's contracted tail (jacobi.cuh)
@@ -102,8 +124,15 @@ CONFIG_VALUES = {
 JACOBI_BLOCKS = (0, 1, 7, 13)
 SPLATS_N = (2, 5, 127, 128, 129, 200)
 TINY_DT = 1e-30
-# the committed sessions: together their seeds reach every class (test_session_model_cpu.py)
-SEEDS = {False: (3, 10, 76, 4, 5), True: (1, 3, 12, 2, 4)}
+# the committed sessions of each mode: together its seeds reach every class (test_session_model_cpu.py)
+SEEDS = {
+    "fp32": (3, 10, 76, 4, 5),
+    "half": (1, 3, 12, 2, 4),
+    "linear": (100, 103, 183),
+    "desktop": (100, 101, 104),
+    "nearest": (101, 104, 249),
+    "nearest_half": (102, 103, 106),
+}
 N_OPS = 40
 
 
@@ -294,11 +323,15 @@ def host_inputs(W, H, seed, half: bool):
 
 # ---- the model ---------------------------------------------------------------------------------------
 class SessionModel:
-    """What one handle holds.  config: the simulation keys the host mirror pushes live (SIM_KEYS)."""
+    """What one handle of `mode` (MODES) holds.  config: the simulation keys the host mirror pushes live
+    (SIM_KEYS)."""
 
-    def __init__(self, W, H, Wd, Hd, canvas, half=False, config=None):
-        self.half = half
-        self.sim = O.OracleSim(W, H, Wd, Hd, half_storage=half)
+    def __init__(self, W, H, Wd, Hd, canvas, mode="fp32", config=None):
+        self.mode = mode
+        self.half, sampler = MODES[mode]
+        self.nearest = sampler == "nearest"
+        sim = LinearOracleSim if sampler == "linear" else O.OracleSim
+        self.sim = sim(W, H, Wd, Hd, half_storage=self.half)
         self.canvas = tuple(canvas)
         self.config = {k: getattr(self.sim, k) for k in SIM_KEYS}
         self.config.update(config or {})
@@ -351,12 +384,16 @@ class SessionModel:
         self.sim.pressure = self._solve(self._st(p), int(iters))
         return self.sim.pressure
 
+    def _copy(self, a, W, H):
+        """resizeFBO's copy of a field into W x H through the handle's sampler, in the storage format."""
+        return M.resize(a, W, H, half=self.half) if self.nearest else self._st(O.resample(a, W, H))
+
     def resize(self, W, H, Wd, Hd, canvas):
         s = self.sim
         if (W, H) != (s.W, s.H):
-            s.velocity = self._st(O.resample(s.velocity, W, H))
+            s.velocity = self._copy(s.velocity, W, H)
         if (Wd, Hd) != (s.Wd, s.Hd):
-            s.dye = self._st(O.resample(s.dye, Wd, Hd))
+            s.dye = self._copy(s.dye, Wd, Hd)
         s.W, s.H, s.Wd, s.Hd = W, H, Wd, Hd
         s.pressure = np.zeros((H, W), F32)
         s.divergence = np.zeros((H, W), F32)
@@ -376,19 +413,19 @@ class SessionModel:
         self.sim.dye = np.ascontiguousarray(dye, F32).copy()
 
     def render(self, keywords, background, dither, fxcfg):
-        """render() at the canvas size: display_model.render with the handle's storage (chains, target, and the
-        powf interval lo / hi with BLOOM)."""
+        """render() at the canvas size: display_model.render with the handle's storage and sampler (chains,
+        target, and the powf interval lo / hi with BLOOM)."""
         w, h = self.canvas
         return M.render(self.sim.dye, w, h, dither, keywords, fxcfg, back_rgb=BACK_RGB, background=background,
-                        aspect=w / h, half_targets=self.half, half_mask=self.half)
+                        aspect=w / h, nearest=self.nearest, half_targets=self.half, half_mask=self.half)
 
     def capture_size(self, capture_res):
         return M.get_resolution(capture_res, *self.canvas)
 
     def capture(self, keywords, transparent, dither, fxcfg, capture_res):
-        """captureScreenshot(): display_model.capture with the handle's storage (rgba8, and the byte bracket
-        lo / hi with BLOOM)."""
+        """captureScreenshot(): display_model.capture with the handle's storage and sampler (rgba8, and the
+        byte bracket lo / hi with BLOOM)."""
         cw, ch = self.canvas
         w, h = self.capture_size(capture_res)
         return M.capture(self.sim.dye, w, h, cw, ch, dither, keywords, transparent, BACK_RGB, cfg=fxcfg,
-                         half_targets=self.half, half_mask=self.half)
+                         nearest=self.nearest, half_targets=self.half, half_mask=self.half)

@@ -7,8 +7,13 @@ their intervals; the launch counters confirm which kernels each size selects.
 Every session also runs on a FLAG_NO_GRAPH twin: after every operation it must hold the graph handle's
 bits and have made as many launches, which tells a step-graph cache fault from a model fault.
 
-On failure the message carries the session's seed, the index of the failing operation and the log of
-operations so far; replay(pkg, half, ops) runs a logged session again."""
+Sessions run in every handle mode of session_model.MODES: fp32 and half storage (HALF_STORAGE |
+HALF_POSTFX), each with the MANUAL advection and LINEAR draws of an ordinary handle, with
+FLUID_FLAG_LINEAR_ADVECTION (linear; desktop, the configuration the reference runs on a desktop browser)
+and with FLUID_FLAG_NEAREST_FILTERING (nearest, nearest_half).
+
+On failure the message carries the session's mode and seed, the index of the failing operation and the
+log of operations so far; replay(pkg, mode, ops) runs a logged session again."""
 import numpy as np
 import pytest
 
@@ -23,8 +28,17 @@ from sim_harness import same_bits
 from webgl_fluid_simulation_b200 import slab
 
 pytestmark = pytest.mark.gpu
-STATS = ("jacobi_launches", "cvd_stream_launches", "gradient_stream_launches", "graph_captures", "jacobi_exact_streams")
+STATS = ("jacobi_launches", "cvd_stream_launches", "gradient_stream_launches", "graph_captures", "jacobi_exact_streams",
+         "advect4_launches")
 FX = {k: S.FXCFG[k] for k in ("BLOOM_RESOLUTION", "SUNRAYS_RESOLUTION")}
+
+
+def mode_flags(pkg, mode):
+    """The flags a handle of session_model mode `mode` is made with."""
+    half, sampler = S.MODES[mode]
+    return ((pkg.FLAG_HALF_STORAGE | pkg.FLAG_HALF_POSTFX if half else 0)
+            | (pkg.FLAG_LINEAR_ADVECTION if sampler == "linear" else 0)
+            | (pkg.FLAG_NEAREST_FILTERING if sampler == "nearest" else 0))
 
 
 @pytest.fixture(scope="module")
@@ -38,15 +52,16 @@ def pkg():
 class Session:
     """A graph handle, its FLAG_NO_GRAPH twin and the model, driven one operation at a time."""
 
-    def __init__(self, pkg, half):
-        self.pkg, self.half = pkg, half
-        self.sched = S.schedule(half)
+    def __init__(self, pkg, mode):
+        self.pkg, self.mode = pkg, mode
+        self.half = S.is_half(mode)
+        self.sched = S.schedule(self.half)
         self.si = 0
         self.dither = DH.golden_dither()
         W, H, Wd, Hd, cw, ch, _ = self.sched[0]
-        flags = pkg.FLAG_HALF_STORAGE | pkg.FLAG_HALF_POSTFX if half else 0
+        flags = mode_flags(pkg, mode)
         self.sims = [self._make(flags), self._make(flags | pkg.FLAG_NO_GRAPH)]
-        self.model = S.SessionModel(W, H, Wd, Hd, (cw, ch), half=half)
+        self.model = S.SessionModel(W, H, Wd, Hd, (cw, ch), mode=mode)
         self.fresh = True                                 # no step since the handle was made or resized
 
     def _make(self, flags):
@@ -112,6 +127,9 @@ class Session:
             streamed = "stream" in self.classes and not self.half
             assert d["cvd_stream_launches"] == int(streamed), (k, d)
             assert d["gradient_stream_launches"] == int(streamed), (k, d)
+            # the 4-cell velocity and dye kernels: fp32 power-of-two grids at least 128 wide, either sampler
+            four = bool({"adv4", "adv4_same"} & self.classes) and not self.half
+            assert d["advect4_launches"] == 2 * four, (k, d)
             if k == 0 and self.fresh:
                 assert d["graph_captures"] == 1, ("the first step after a resize must capture a new graph", d)
             if k == 1:
@@ -238,9 +256,10 @@ class Session:
         assert np.array_equal(got[1], got[0])
 
 
-def replay(pkg, half, ops, seed=None):
-    """Runs a logged session; an AssertionError names the seed, the operation and the log up to it."""
-    s = Session(pkg, half)
+def replay(pkg, mode, ops, seed=None):
+    """Runs a logged session on a handle of `mode`; an AssertionError names the mode, the seed, the
+    operation and the log up to it."""
+    s = Session(pkg, mode)
     try:
         s.check_fields()
         for i, op in enumerate(ops):
@@ -248,8 +267,8 @@ def replay(pkg, half, ops, seed=None):
                 s.run(op)
             except AssertionError as e:
                 log = "\n".join(f"  {k:3d} {o!r}" for k, o in enumerate(ops[:i + 1]))
-                raise AssertionError(f"session seed={seed} half={half}: operation {i} {op!r} failed: {e}\n"
-                                     f"replay(pkg, {half}, ops) with ops =\n{log}") from e
+                raise AssertionError(f"session seed={seed} mode={mode}: operation {i} {op!r} failed: {e}\n"
+                                     f"replay(pkg, {mode!r}, ops) with ops =\n{log}") from e
     finally:
         s.close()
 
@@ -259,51 +278,87 @@ ALL3 = M.SHADING | M.BLOOM | M.SUNRAYS
 SCRIPTS = {
     # fluid_pressure_solve_host flips the pressure parity outside any step: the next replay must read the
     # buffer the solve left its result in (banded at 1024 x 512, one piece at 64 x 64)
-    "host_solve_then_step": (False, [
+    "host_solve_then_step": ("fp32", [
         ("write", "velocity", 1), ("write", "dye", 2), ("step", S.DT_CLAMP), ("host_solve", 20, 3), ("step", S.DT_CLAMP),
         ("resize", 1), ("step", S.DT_CLAMP), ("host_solve", 20, 4), ("step", S.DT_CLAMP), ("step", 0.01),
         ("host_solve", 50, 5), ("host_solve", 13, 6), ("step", S.DT_CLAMP), ("pressure_solve",), ("step", S.DT_CLAMP)]),
     # resize away and back: an earlier graph-cache key returns with new buffers
-    "resize_and_back": (False, [
+    "resize_and_back": ("fp32", [
         ("write", "velocity", 7), ("step", S.DT_CLAMP), ("resize", 1), ("step", S.DT_CLAMP), ("step", S.DT_CLAMP),
         ("resize", 5), ("step", S.DT_CLAMP), ("resize", 9), ("step", S.DT_CLAMP), ("step", S.DT_CLAMP),
         ("resize", 10), ("step", S.DT_CLAMP), ("step", S.DT_CLAMP)]),
-    "half_resize_and_back": (True, [
+    "half_resize_and_back": ("half", [
         ("write", "velocity", 8), ("step", S.DT_CLAMP), ("resize", 1), ("step", S.DT_CLAMP), ("resize", 4),
         ("step", S.DT_CLAMP), ("resize", 8), ("step", S.DT_CLAMP), ("resize", 9), ("step", S.DT_CLAMP)]),
     # SUNRAYS draws its mask into dye.write (and, in half storage, widens dye into the shared scratch)
-    "sunrays_frame_then_splat_and_step": (False, [
+    "sunrays_frame_then_splat_and_step": ("fp32", [
         ("write", "dye", 9), ("render", M.SHADING | M.SUNRAYS, False, False), ("splat", 10), ("step", S.DT_CLAMP),
         ("render", M.BLOOM | M.SUNRAYS, True, False), ("splats", 5, 11), ("step", S.DT_CLAMP),
         ("capture", ALL3, False), ("step", S.DT_CLAMP), ("render", ALL3, True, True), ("step", S.DT_CLAMP)]),
-    "half_sunrays_frame_then_splat_and_step": (True, [
+    "half_sunrays_frame_then_splat_and_step": ("half", [
         ("write", "dye", 12), ("render", M.SHADING | M.SUNRAYS, False, False), ("splat", 13), ("step", S.DT_CLAMP),
         ("render", ALL3, False, False), ("write", "velocity", 14), ("splats", 129, 15), ("step", S.DT_CLAMP),
         ("capture", ALL3, True), ("step", S.DT_CLAMP)]),
     # a host write of tiny divergence rebuilds the tiny map: the next blocked solve must use the exact tail
-    "tiny_divergence_write_then_solve_and_step": (False, [
+    "tiny_divergence_write_then_solve_and_step": ("fp32", [
         ("write", "velocity", 16), ("write_tiny_div", 17), ("pressure_solve",), ("step", S.DT_CLAMP),
         ("write_tiny_div", 18), ("jacobi", 13), ("step", S.DT_CLAMP), ("resize", 1), ("write_tiny_div", 19),
         ("pressure_solve",), ("step", S.DT_CLAMP)]),
     # JACOBI_BLOCK changes the launches of a replayed step but not its bits: the launch counts catch a
     # graph key without it
-    "live_jacobi_block_between_replays": (False, [
+    "live_jacobi_block_between_replays": ("fp32", [
         ("write", "velocity", 20), ("write", "pressure", 21), ("step", S.DT_CLAMP), ("step", S.DT_CLAMP),
         ("jacobi_block", 7), ("step", S.DT_CLAMP), ("step", S.DT_CLAMP), ("jacobi_block", 13), ("step", S.DT_CLAMP),
         ("jacobi_block", 1), ("step", S.DT_CLAMP), ("jacobi_block", 0), ("step", S.DT_CLAMP),
         ("config", "PRESSURE_ITERATIONS", 14), ("step", S.DT_CLAMP), ("config", "PRESSURE_ITERATIONS", 0),
         ("step", S.DT_CLAMP), ("config", "PRESSURE_ITERATIONS", 1), ("step", 0.0), ("jacobi_block", 7),
         ("step", S.DT_CLAMP), ("resize", 1), ("step", S.DT_CLAMP), ("jacobi_block", 13), ("step", S.DT_CLAMP)]),
+    # LINEAR advection across the 4-cell kernels: one-cell -> adv4_same -> adv4 -> ragged -> adv4_same, two
+    # steps at each size, and live dissipations, CURL, PRESSURE_ITERATIONS and JACOBI_BLOCK between replays
+    # (changing a value back replays the graph captured before the change); splats and a host solve before steps
+    "linear_resize_across_adv4_and_back": ("linear", [
+        ("write", "velocity", 31), ("write", "dye", 32), ("step", S.DT_CLAMP), ("step", S.DT_CLAMP),
+        ("resize", 1), ("step", S.DT_CLAMP), ("step", S.DT_CLAMP), ("config", "VELOCITY_DISSIPATION", 4.0),
+        ("step", S.DT_CLAMP), ("config", "VELOCITY_DISSIPATION", 0.2), ("step", S.DT_CLAMP),
+        ("config", "DENSITY_DISSIPATION", 0.0), ("step", S.DT_CLAMP), ("config", "CURL", 55.0), ("step", 0.01),
+        ("host_solve", 20, 33), ("step", S.DT_CLAMP),
+        ("resize", 2), ("step", S.DT_CLAMP), ("step", S.DT_CLAMP), ("splats", 5, 34), ("config", "DENSITY_DISSIPATION", 1.0),
+        ("step", S.DT_CLAMP), ("config", "PRESSURE_ITERATIONS", 13), ("jacobi_block", 7), ("step", S.DT_CLAMP),
+        ("config", "CURL", 30.0), ("step", S.DT_CLAMP), ("config", "CURL", 55.0), ("step", S.DT_CLAMP),
+        ("resize", 4), ("step", S.DT_CLAMP), ("step", S.DT_CLAMP), ("config", "VELOCITY_DISSIPATION", 1.0),
+        ("step", S.DT_CLAMP), ("splat", 35), ("step", S.DT_CLAMP),
+        ("resize", 1), ("step", S.DT_CLAMP), ("step", S.DT_CLAMP), ("config", "DENSITY_DISSIPATION", 4.0),
+        ("jacobi_block", 0), ("step", S.DT_CLAMP), ("config", "DENSITY_DISSIPATION", 1.0), ("step", S.DT_CLAMP)]),
+    # the desktop configuration (HALF_STORAGE | HALF_POSTFX | LINEAR_ADVECTION) through the reference's update():
+    # splats, a step at the clamped dt, a frame with all three keywords; a capture, a host solve, a resize and back
+    "desktop_frame_loop": ("desktop", [
+        ("write", "velocity", 41), ("write", "dye", 42),
+        ("splats", 5, 43), ("step", S.DT_CLAMP), ("render", ALL3, False, False),
+        ("splat", 44), ("step", S.DT_CLAMP), ("render", ALL3, False, False),
+        ("splats", 2, 45), ("step", 0.0123), ("render", ALL3, False, False), ("capture", ALL3, False),
+        ("splats", 3, 46), ("step", S.DT_CLAMP), ("render", ALL3, False, False),
+        ("host_solve", 20, 47), ("step", S.DT_CLAMP), ("render", ALL3, False, False),
+        ("resize", 1), ("splats", 2, 48), ("step", S.DT_CLAMP), ("render", ALL3, False, False),
+        ("resize", 9), ("splat", 49), ("step", S.DT_CLAMP), ("render", ALL3, False, False),
+        ("splats", 5, 50), ("step", S.DT_CLAMP), ("render", ALL3, True, False), ("capture", ALL3, True),
+        ("splats", 129, 51), ("step", S.DT_CLAMP), ("render", ALL3, False, False)]),
+    # NEAREST resize copies in half storage across the whole schedule; after each resize every keyword set is
+    # drawn, a capture taken and one step run
+    "nearest_half_resize_then_draw": ("nearest_half", [("write", "velocity", 61), ("write", "dye", 62)] + [
+        op for si in range(1, len(S.HALF_SCHEDULE)) for op in
+        [("resize", si)] + [("render", kw, bool(kw & 1), kw in (3, 6)) for kw in range(8)]
+        + [("capture", ALL3 if si % 2 else si % 8, bool(si % 3 == 0)), ("step", S.DT_CLAMP)]]),
 }
 
 
 @pytest.mark.parametrize("name", list(SCRIPTS))
 def test_scripted_hand_off(pkg, name):
-    half, ops = SCRIPTS[name]
-    replay(pkg, half, ops, seed=name)
+    mode, ops = SCRIPTS[name]
+    replay(pkg, mode, ops, seed=name)
 
 
 # ---- seeded random sessions ----------------------------------------------------------------------------
-@pytest.mark.parametrize("half,seed", [(h, s) for h in (False, True) for s in S.SEEDS[h]])
-def test_random_session(pkg, half, seed):
-    replay(pkg, half, S.generate(seed, half, S.N_OPS), seed=seed)
+@pytest.mark.parametrize("mode,seed", [(m, s) for m in S.MODES for s in S.SEEDS[m]])
+def test_random_session(pkg, mode, seed):
+    half = S.is_half(mode)
+    replay(pkg, mode, S.generate(seed, half, S.N_OPS), seed=seed)

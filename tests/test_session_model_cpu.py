@@ -3,8 +3,10 @@ goldens, and the operation generator's determinism and reach over the seeds test
 import numpy as np
 import pytest
 
+import display_model as M
 import session_model as S
 from conftest import bits_equal, golden, max_rel
+from linear_advection_model import LinearOracleSim
 
 # what the committed sessions of test_gpu_session.py must reach, per storage mode
 OPS = {"step", "splat", "splats", "write", "pressure_solve", "jacobi", "host_solve", "config", "jacobi_block", "resize",
@@ -22,27 +24,35 @@ REACH = {
 
 
 def test_step_only_sequences_equal_oraclesim(oracle):
-    """Writes, live config and steps through the model == OracleSim driven directly, bit for bit."""
-    for half in (False, True):
-        W, H, Wd, Hd = 36, 20, 54, 30
-        m = S.SessionModel(W, H, Wd, Hd, (72, 40), half=half)
-        ref = oracle.OracleSim(W, H, Wd, Hd, half_storage=half)
-        v = S.field_data("velocity", W, H, Wd, Hd, 1, half)
-        dye = S.field_data("dye", W, H, Wd, Hd, 2, half)
-        m.write("velocity", v); m.write("dye", dye)
-        R = oracle.round_half if half else (lambda a: a.copy())
-        ref.velocity, ref.dye = R(v), R(dye)
-        for k, (key, val, dt) in enumerate([(None, None, S.DT_CLAMP), ("CURL", 12.5, 0.01), ("PRESSURE_ITERATIONS", 13, 0.0),
-                                            ("VELOCITY_DISSIPATION", 4.0, S.TINY_DT), ("PRESSURE", 0.33, S.DT_CLAMP),
-                                            ("PRESSURE_ITERATIONS", 0, S.DT_CLAMP)]):
-            if key:
-                m.config[key] = val
-                setattr(ref, key, val)
-            m.step(dt); ref.step(dt)
-            for n in S.FIELDS:
-                a, b = m.field(n), getattr(ref, n)
-                assert a.shape == b.shape and np.array_equal(np.isnan(a), np.isnan(b)), (half, k, n)
-                assert bits_equal(np.nan_to_num(a), np.nan_to_num(b)), (half, k, n)
+    """Writes, live config and steps through the model of every mode == the mode's simulation driven
+    directly, bit for bit: OracleSim, and LinearOracleSim in the LINEAR modes (linear, desktop), whose
+    steps differ from OracleSim's."""
+    for mode, (half, sampler) in S.MODES.items():
+        sim = LinearOracleSim if sampler == "linear" else oracle.OracleSim
+        for W, H, Wd, Hd in ((36, 20, 54, 30), (128, 64, 256, 128)):
+            m = S.SessionModel(W, H, Wd, Hd, (72, 40), mode=mode)
+            ref = sim(W, H, Wd, Hd, half_storage=half)
+            manual = oracle.OracleSim(W, H, Wd, Hd, half_storage=half)
+            v = S.field_data("velocity", W, H, Wd, Hd, 1, half)
+            dye = S.field_data("dye", W, H, Wd, Hd, 2, half)
+            m.write("velocity", v); m.write("dye", dye)
+            R = oracle.round_half if half else (lambda a: a.copy())
+            ref.velocity, ref.dye = R(v), R(dye)
+            manual.velocity, manual.dye = R(v), R(dye)
+            for k, (key, val, dt) in enumerate([(None, None, S.DT_CLAMP), ("CURL", 12.5, 0.01), ("PRESSURE_ITERATIONS", 13, 0.0),
+                                                ("VELOCITY_DISSIPATION", 4.0, S.TINY_DT), ("PRESSURE", 0.33, S.DT_CLAMP),
+                                                ("PRESSURE_ITERATIONS", 0, S.DT_CLAMP)]):
+                if key:
+                    m.config[key] = val
+                    setattr(ref, key, val)
+                    setattr(manual, key, val)
+                m.step(dt); ref.step(dt); manual.step(dt)
+                for n in S.FIELDS:
+                    a, b = m.field(n), getattr(ref, n)
+                    assert a.shape == b.shape and np.array_equal(np.isnan(a), np.isnan(b)), (mode, k, n)
+                    assert bits_equal(np.nan_to_num(a), np.nan_to_num(b)), (mode, k, n)
+            differs = not bits_equal(np.nan_to_num(m.field("dye")), np.nan_to_num(manual.dye))
+            assert differs == (sampler == "linear"), (mode, W, H)
 
 
 def test_pressure_solves_equal_clear_and_jacobi(oracle):
@@ -59,7 +69,7 @@ def test_pressure_solves_equal_clear_and_jacobi(oracle):
     m.jacobi(5)
     assert bits_equal(m.field("pressure"), oracle.jacobi(oracle.jacobi(oracle.clear(p, 0.8), d, 20), d, 5))
     assert bits_equal(m.pressure_solve_host(d, p, 13), oracle.jacobi(oracle.clear(p, 0.8), d, 13))
-    h = S.SessionModel(W, H, W, H, (48, 32), half=True)
+    h = S.SessionModel(W, H, W, H, (48, 32), mode="half")
     R = oracle.round_half
     want = R(oracle.clear(R(p), 0.8))
     for _ in range(3):
@@ -97,6 +107,39 @@ def test_resize_equals_copy_shader_goldens(oracle):
             assert not m.field(n).any()
 
 
+def test_nearest_resize_equals_display_model_resize(oracle):
+    """The resize of a NEAREST model (nearest, nearest_half): velocity and dye are display_model.resize's
+    NEAREST copy (fp16-rounded in half storage), not the LINEAR copy of the other modes; a field whose size
+    did not change keeps its bits; pressure, divergence and curl start over at zero."""
+    for mode in ("nearest", "nearest_half"):
+        half = S.is_half(mode)
+        W, H, Wd, Hd = 36, 20, 54, 30
+        m = S.SessionModel(W, H, Wd, Hd, (72, 40), mode=mode)
+        lin = S.SessionModel(W, H, Wd, Hd, (72, 40), mode="half" if half else "fp32")
+        for n in ("velocity", "dye"):
+            a = S.field_data(n, W, H, Wd, Hd, 7, half)
+            m.write(n, a); lin.write(n, a)
+        m.write("pressure", np.ones((H, W), np.float32))
+        # up, down, ragged; sim only, dye only; and back
+        for sizes in ((72, 40, 108, 60), (17, 9, 108, 60), (17, 9, 25, 70), (64, 64, 25, 70), (36, 20, 54, 30)):
+            v0, d0 = m.field("velocity").copy(), m.field("dye").copy()
+            m.resize(*sizes, (72, 40)); lin.resize(*sizes, (72, 40))
+            W, H, Wd, Hd = sizes
+            for n, old, (w, h) in (("velocity", v0, (W, H)), ("dye", d0, (Wd, Hd))):
+                got = m.field(n)
+                if old.shape[:2] == (h, w):
+                    assert bits_equal(np.nan_to_num(got), np.nan_to_num(old)), (mode, sizes, n)
+                else:
+                    want = M.resize(old, w, h, half=half)
+                    assert got.shape == want.shape and np.array_equal(np.isnan(got), np.isnan(want)), (mode, sizes, n)
+                    assert bits_equal(np.nan_to_num(got), np.nan_to_num(want)), (mode, sizes, n)
+                    assert not bits_equal(np.nan_to_num(got), np.nan_to_num(lin.field(n))), (mode, sizes, n)
+            for n in ("pressure", "divergence", "curl"):
+                assert m.field(n).shape == (H, W) and not m.field(n).any(), (mode, sizes, n)
+            for n in ("velocity", "dye"):
+                lin.write(n, m.field(n))       # the next resize copies the same fields
+
+
 def test_splat_interval_holds_the_oracle_splat(oracle):
     """The interval the model checks a splat against contains the oracle's own splat (glibc expf)."""
     m = S.SessionModel(48, 32, 96, 64, (150, 100))
@@ -111,12 +154,15 @@ def test_splat_interval_holds_the_oracle_splat(oracle):
     assert S.SM.check_splat(v, lo, hi)[0] == 0
 
 
-@pytest.mark.parametrize("half", [False, True])
-def test_generator_is_deterministic_and_reaches_every_class(half):
-    """Same seed, same session; another seed, another session; and over the committed seeds of
+@pytest.mark.parametrize("mode", list(S.MODES))
+def test_generator_is_deterministic_and_reaches_every_class(mode):
+    """Same seed, same session; another seed, another session; and over the committed seeds of a mode in
     test_gpu_session.py every operation kind, config key, JACOBI_BLOCK value, dt kind, splat count class,
-    resize direction and size class of the schedule is reached, the session ending at its starting size."""
-    seeds = S.SEEDS[half]
+    resize direction and size class of its storage's schedule is reached, the session ending at its
+    starting size."""
+    half = S.is_half(mode)
+    seeds = S.SEEDS[mode]
+    assert len(seeds) >= 3, seeds
     a = S.generate(seeds[0], half, S.N_OPS)
     assert a == S.generate(seeds[0], half, S.N_OPS)
     assert a != S.generate(seeds[0] + 1000, half, S.N_OPS)
