@@ -197,6 +197,8 @@ int fluid_p2p_disable(fluid_t* h);   /* back to NCCL; call on every rank if any 
  *  - fluid_sync, fluid_stat, fluid_launch_count, fluid_mark, fluid_elapsed_ms, fluid_timing_last,
  *    fluid_last_error and fluid_destroy behave as on any handle.
  *  - fluid_render_canvas_batch and fluid_capture_batch draw every member's canvas or capture in one call.
+ *  - Member subsets (below): fluid_read_members and fluid_write_members move, fluid_reset_members resets, and
+ *    fluid_render_canvas_members and fluid_capture_members draw, only the members a list names.
  *  - Every other entry point refuses a batch handle with FLUID_ERR_INVALID and leaves it usable: the fp32
  *    frames (fluid_render, fluid_render_keywords, fluid_render_postfx), fluid_capture, fluid_capture_device
  *    and fluid_render_canvas (use the batch calls), fluid_render_band, fluid_resize, fluid_pass_*,
@@ -223,6 +225,31 @@ int fluid_members(fluid_t* h);
 int fluid_set_param_members(fluid_t* h, int key, const double* values, int n);
 int fluid_get_param_members(fluid_t* h, int key, float* values, int n);
 int fluid_step_members(fluid_t* h, const float* dt, int n);
+
+/* Member subsets of a batch handle: `members` is a host array of n DISTINCT member indices in [0, B), in any
+ * order, and slot (or image) k of the caller's buffer is member members[k].  The list is checked on the host, then
+ * copied, stream-ordered, into a list buffer of B int32 the handle allocates at creation outside the field arena;
+ * the caller may reuse `members` as soon as the call returns.
+ *  - n == 0 does nothing and launches nothing.
+ *  - Refused with FLUID_ERR_INVALID before any work, every field and buffer untouched and the handle usable: an
+ *    index outside [0, B); an index listed twice; n < 0, or members == NULL with n > 0; a buffer whose size does not
+ *    match n; a bad field; an ordinary or slab handle; a device buffer fluid_read_device refuses.
+ *  - No call recaptures a step graph.
+ * fluid_read_members / fluid_write_members: fluid_read / fluid_write of the listed members.  buf is a C-contiguous
+ * (n, H, W[, C]) array, n_floats == n * w * rows * channels.
+ *  - In host memory (on_device == 0): one copy per listed member, straight between its block of the arena and the
+ *    caller's memory, then a stream sync.
+ *  - In device memory (on_device != 0): one launch, stream-ordered and returning without a sync, with the rules of
+ *    fluid_read_device / fluid_write_device.
+ *  - fluid_write_members writes the listed members' .read only; every other member keeps every byte.
+ * fluid_reset_members: the listed members return to the state fluid_create_batch leaves (both slots of velocity,
+ * pressure and dye zero, dye alpha 1, divergence and curl zero), in one launch.  Their per-member values
+ * (fluid_set_param_members) are config, not state, and stay. */
+int fluid_read_members(fluid_t* h, int field, const int32_t* members, int n, float* dst, size_t n_floats,
+                       int dst_on_device);
+int fluid_write_members(fluid_t* h, int field, const int32_t* members, int n, const float* src, size_t n_floats,
+                        int src_on_device);
+int fluid_reset_members(fluid_t* h, const int32_t* members, int n);
 
 void fluid_destroy(fluid_t* h);
 
@@ -499,6 +526,21 @@ int fluid_capture_batch(fluid_t* h, int width, int height, int canvas_w, int can
                         int transparent, const fluid_postfx* fx, const float* dither_rgb, int dw, int dh,
                         float back_r, float back_g, float back_b,
                         uint8_t* dst, size_t n_bytes, int dst_on_device);
+/* fluid_render_canvas_batch and fluid_capture_batch for the n members a list names, with the list rules of the
+ * member-subset calls (fluid_read_members): dst holds n images, n_bytes == n * 4 * width * height, and image k is
+ * byte for byte image members[k] of the whole-batch call.  The same launches as one whole-batch draw, each n
+ * layers of blocks deep, in the same post-FX targets (sized for B), so subset and whole draws alternate without
+ * remaking them.  With SUNRAYS the mask goes into the listed members' dye.write only.  Refused with
+ * FLUID_ERR_INVALID, dst untouched and the handle usable: everything the whole-batch call refuses (n_bytes checked
+ * against n images) and every bad list. */
+int fluid_render_canvas_members(fluid_t* h, int width, int height, uint32_t keywords, int transparent,
+                                const fluid_postfx* fx, const float* dither_rgb, int dw, int dh,
+                                float back_r, float back_g, float back_b,
+                                uint8_t* dst, size_t n_bytes, int dst_on_device, const int32_t* members, int n);
+int fluid_capture_members(fluid_t* h, int width, int height, int canvas_w, int canvas_h, uint32_t keywords,
+                          int transparent, const fluid_postfx* fx, const float* dither_rgb, int dw, int dh,
+                          float back_r, float back_g, float back_b,
+                          uint8_t* dst, size_t n_bytes, int dst_on_device, const int32_t* members, int n);
 
 int fluid_sync(fluid_t* h);
 int fluid_timing_last(fluid_t* h, fluid_timing* out);

@@ -26,7 +26,8 @@ SYMBOLS = [
     "fluid_timing_last", "fluid_host_alloc", "fluid_host_free", "fluid_mark", "fluid_elapsed_ms", "fluid_launch_count", "fluid_device_ptr",
     "fluid_last_error", "fluid_create_batch", "fluid_members", "fluid_splats_batch", "fluid_render_canvas_batch",
     "fluid_capture_batch", "fluid_set_param_members", "fluid_get_param_members", "fluid_step_members",
-    "fluid_splats_device", "fluid_splats_batch_device",
+    "fluid_splats_device", "fluid_splats_batch_device", "fluid_read_members", "fluid_write_members",
+    "fluid_reset_members", "fluid_render_canvas_members", "fluid_capture_members",
 ]
 
 FLUID_OK = 0
@@ -143,6 +144,12 @@ def lib():
     L.fluid_render_canvas.argtypes = [vp, i, i, C.c_uint32, i, C.POINTER(PostFX), vp, i, i, f, f, f, vp, sz, i]
     L.fluid_render_canvas_batch.argtypes = L.fluid_render_canvas.argtypes
     L.fluid_capture_batch.argtypes = L.fluid_capture.argtypes + [i]
+    ip = C.POINTER(C.c_int32)
+    L.fluid_read_members.argtypes = [vp, i, ip, i, vp, sz, i]
+    L.fluid_write_members.argtypes = [vp, i, ip, i, vp, sz, i]
+    L.fluid_reset_members.argtypes = [vp, ip, i]
+    L.fluid_render_canvas_members.argtypes = L.fluid_render_canvas_batch.argtypes + [ip, i]
+    L.fluid_capture_members.argtypes = L.fluid_capture_batch.argtypes + [ip, i]
     L.fluid_sync.argtypes = [vp]
     L.fluid_host_alloc.argtypes = [sz]; L.fluid_host_alloc.restype = vp
     L.fluid_host_free.argtypes = [vp]; L.fluid_host_free.restype = None

@@ -24,6 +24,7 @@
 #include "stream_passes.cuh"
 #include "postfx.cuh"
 #include "half_passes.cuh"
+#include "members.cuh"
 
 namespace {
 
@@ -111,6 +112,7 @@ struct fluid : SlabGeometry {
     float* dt_dev = nullptr;
     std::vector<float> member_host;
     std::vector<double> member_radius_d;
+    int* member_list = nullptr;            // the member-subset calls' list (fluid_read_members ...): B int32, outside the arena
     unsigned char* tiny_map = nullptr;     // where divergence has 0 < |d| < 2^-123 (jacobi.cuh): 1 byte per 128x32 cells, GLOBAL rows
     size_t tiny_map_bytes = 0;
     // 2-D tensor maps the blocked Jacobi kernel stages through: m[k] maps pressure slot k and divergence
@@ -796,7 +798,7 @@ int not_on_slab(fluid_t* h, const char* what) {
 // the batch draw calls
 int not_on_batch(fluid_t* h, const char* what) {
     return fail(h, FLUID_ERR_INVALID, "%s does not take a batch handle; one supports fluid_step / fluid_splats_batch[_device] / "
-                "read / write / set_param / stat / fluid_render_canvas_batch / fluid_capture_batch", what);
+                "read / write / the *_members calls / set_param / stat / fluid_render_canvas_batch / fluid_capture_batch", what);
 }
 
 // Row ownership + ghost-zone heights of rank `rank` of `world` for a sim_h / dye_h grid (DESIGN.md §7).
@@ -897,6 +899,7 @@ int create_common(const fluid_config* cfg, int rank, int world, const void* uid,
         CU(cudaMemsetAsync(h->exact_streams, 0, sizeof(unsigned long long), h->stream));
         if (h->batch) {
             int r = alloc_member_table(h); if (r) return r;
+            CU(cudaMalloc((void**)&h->member_list, (size_t)h->members * sizeof(int32_t)));
         } else {
             CU(cudaMalloc((void**)&h->dt_dev, sizeof(float)));
             CU(cudaMemsetAsync(h->dt_dev, 0, sizeof(float), h->stream));
@@ -1064,6 +1067,7 @@ void fluid_destroy(fluid_t* h) {
     cudaFree(h->halo_flag);
     cudaFree(h->exact_streams);
     cudaFree(h->dt_dev);
+    cudaFree(h->member_list);
     cudaFree(h->scratch);
     cudaFree(h->splat_scratch);
     cudaFree(h->frame);
@@ -1890,6 +1894,111 @@ int fluid_write_device(fluid_t* h, int field, const float* src, size_t n_floats)
     return FLUID_OK;
 }
 
+// ---- member subsets of a batch handle ----------------------------------------------------------------------
+
+// The member list of a member-subset call: n distinct indices in [0, B) on a batch handle, checked on the host
+// before any work.  n == 0 passes; the call then does nothing.
+static int check_member_list(fluid_t* h, const char* what, const int32_t* members, int n) {
+    if (!h->batch) return fail(h, FLUID_ERR_INVALID, "%s needs a batch handle (fluid_create_batch)", what);
+    if (n < 0 || (n > 0 && !members))
+        return fail(h, FLUID_ERR_INVALID, "%s: bad member list (%d members at %p)", what, n, (const void*)members);
+    std::vector<char> seen(h->members, 0);
+    for (int k = 0; k < n; ++k) {
+        const int32_t m = members[k];
+        if (m < 0 || m >= h->members)
+            return fail(h, FLUID_ERR_INVALID, "%s: members[%d] = %d is outside [0, %d)", what, k, m, h->members);
+        if (seen[m]++) return fail(h, FLUID_ERR_INVALID, "%s: member %d is listed twice", what, m);
+    }
+    return FLUID_OK;
+}
+
+// A checked list into the handle's list buffer, which the launches of the call read: stream-ordered, from pageable
+// memory like upload_member_row, so a list buffer still in use by queued work is overwritten only after it.
+static int upload_member_list(fluid_t* h, const int32_t* members, int n) {
+    CU(cudaMemcpyAsync(h->member_list, members, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
+    return FLUID_OK;
+}
+
+// The checks fluid_read_members / fluid_write_members share, all before any work; *p: the field's .read, *per:
+// the floats of one member
+static int members_io_args(fluid_t* h, const char* what, int field, const int32_t* members, int n, const void* buf,
+                           size_t n_floats, int on_device, float** p, size_t* per) {
+    void* q; int w, rows, ch;
+    if (!h) return FLUID_ERR_INVALID;
+    if (field_info(h, field, &q, &w, &rows, &ch)) return fail(h, FLUID_ERR_INVALID, "%s: bad field %d", what, field);
+    if (int rc = check_member_list(h, what, members, n)) return rc;
+    *p = (float*)q;
+    *per = (size_t)w * rows * ch;
+    if (n_floats != *per * n)
+        return fail(h, FLUID_ERR_INVALID, "%s: %d members of field %d have %zu floats, caller passed %zu", what, n, field,
+                    *per * n, n_floats);
+    if (n == 0) return FLUID_OK;
+    if (!buf) return fail(h, FLUID_ERR_INVALID, "%s: NULL buffer", what);
+    return on_device ? check_device_buf(h, what, buf, n_floats * sizeof(float)) : FLUID_OK;
+}
+
+// One launch moving the listed members' blocks of `per` floats between a field and the caller's device buffer,
+// in 16-byte words when the buffer is 16-byte aligned (the member blocks always are)
+static int launch_member_copy(fluid_t* h, bool to_buf, float* field, float* buf, size_t per, int n) {
+    const bool v4 = (uintptr_t)buf % 16 == 0;
+    const size_t units = v4 ? per / 4 : per;
+    const dim3 g((unsigned)std::min<size_t>((units + 255) / 256, 1024), 1, n);
+    if (v4 && to_buf) member_copy_kernel<float4, true><<<g, 256, 0, h->stream>>>((const float4*)field, (float4*)buf, h->member_list, units);
+    else if (v4) member_copy_kernel<float4, false><<<g, 256, 0, h->stream>>>((const float4*)buf, (float4*)field, h->member_list, units);
+    else if (to_buf) member_copy_kernel<float, true><<<g, 256, 0, h->stream>>>(field, buf, h->member_list, units);
+    else member_copy_kernel<float, false><<<g, 256, 0, h->stream>>>(buf, field, h->member_list, units);
+    return check_launch(h, "member_copy_kernel");
+}
+
+// fluid_read for the listed members: slot k of dst is member members[k].  Into host memory one copy per member
+// straight from the arena, then a sync; into device memory one gather launch, stream-ordered.
+int fluid_read_members(fluid_t* h, int field, const int32_t* members, int n, float* dst, size_t n_floats, int dst_on_device) {
+    float* p = nullptr; size_t per = 0;
+    int rc = members_io_args(h, "fluid_read_members", field, members, n, dst, n_floats, dst_on_device, &p, &per);
+    if (rc || n == 0) return rc;
+    if (dst_on_device) {
+        if ((rc = upload_member_list(h, members, n))) return rc;
+        return launch_member_copy(h, true, p, dst, per, n);
+    }
+    for (int k = 0; k < n; ++k)
+        CU(cudaMemcpyAsync(dst + k * per, p + (size_t)members[k] * per, per * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+    CU(cudaStreamSynchronize(h->stream));
+    return check_halo(h);
+}
+
+// fluid_write for the listed members, .read only; every other member keeps every byte.  Written divergence
+// leaves the tiny-divergence map alone: every batch step clears and rebuilds it (cvd_stream_kernel<true>) before
+// the blocked solve reads it, and no other batch call reads it.
+int fluid_write_members(fluid_t* h, int field, const int32_t* members, int n, const float* src, size_t n_floats, int src_on_device) {
+    float* p = nullptr; size_t per = 0;
+    int rc = members_io_args(h, "fluid_write_members", field, members, n, src, n_floats, src_on_device, &p, &per);
+    if (rc || n == 0) return rc;
+    if (src_on_device) {
+        if ((rc = upload_member_list(h, members, n))) return rc;
+        return launch_member_copy(h, false, p, const_cast<float*>(src), per, n);
+    }
+    for (int k = 0; k < n; ++k)
+        CU(cudaMemcpyAsync(p + (size_t)members[k] * per, src + k * per, per * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+    CU(cudaStreamSynchronize(h->stream));
+    return FLUID_OK;
+}
+
+// The listed members back to the state fluid_create_batch leaves, both slots of every pair, in one launch.  Their
+// per-member values are config and stay; no step graph is recaptured (a reset member's slots are alike).
+int fluid_reset_members(fluid_t* h, const int32_t* members, int n) {
+    if (!h) return FLUID_ERR_INVALID;
+    int rc = check_member_list(h, "fluid_reset_members", members, n);
+    if (rc || n == 0) return rc;
+    if ((rc = upload_member_list(h, members, n))) return rc;
+    const size_t sv = sim_cells(h) / 2, ss = sim_cells(h) / 4, sd = dye_cells(h);   // float4 per member
+    const MemberSlots s{{(float4*)h->dye.read, (float4*)h->dye.write, (float4*)h->velocity.read, (float4*)h->velocity.write,
+                         (float4*)h->pressure.read, (float4*)h->pressure.write, (float4*)h->divergence, (float4*)h->curl},
+                        {sd, sd, sv, sv, ss, ss, ss, ss}};
+    const dim3 g((unsigned)std::min<size_t>((sd + 255) / 256, 1024), 1, n);
+    member_reset_kernel<<<g, 256, 0, h->stream>>>(s, h->member_list);
+    return check_launch(h, "member_reset_kernel");
+}
+
 // fluid_pressure_solve_host on one GPU is PCIe-bound (4096^2: 128 MiB up, 64 MiB down per call), so
 // the solve is hidden behind the copies: the grid is cut into row bands, band b is solved as soon as its rows
 // (+ `iters` rows beyond it) have arrived and is copied back while the later bands still upload — the slab
@@ -2147,14 +2256,17 @@ static int post_fx_targets(fluid_t* h, uint32_t keywords, const PostFXOut& o, co
 // The post-FX chains of render() for the keywords that are on, into the targets post_fx_targets made: applyBloom
 // (S:1350-1394) with BLOOM, applySunrays + blur(…, 1) (S:1396-1419; the mask is drawn into dye.write exactly like
 // S:1300) with SUNRAYS.  Sd: the dye's storage policy (the mask is drawn in it), St: the targets', Smp: the sampler
-// of every texture the chains read (postfx.cuh).  BATCH: a batch handle's B members, each target a dense (B, h, w)
-// array and each launch B layers of blocks deep.  Arguments checked by the caller.
+// of every texture the chains read (postfx.cuh).  BATCH: `images` images of a batch handle, each target a dense
+// (B, h, w) array of which image z takes slot z, and each launch `images` layers of blocks deep; image z draws
+// member members[z] (a subset draw's list in device memory), or member z when members is null.  Arguments checked
+// by the caller.
 // A slab rank (fp32, LINEAR) prefilters its band of the bloom FBO's rows and draws the mask on the dye rows it
 // owns; the bands are gathered (halo.cuh gather_bands), so every rank runs the pyramid, the sunrays and the blurs
 // on the inputs one GPU has and ends with its bits.  The dye ghost rows must be fresh (draw_ghost_rows).
 extern "C++" {
 template <class Sd, class St, class Smp, bool BATCH = false>
-static int post_fx_chains(fluid_t* h, uint32_t keywords, const fluid_postfx* fx, const PostFXOut& o) {
+static int post_fx_chains(fluid_t* h, uint32_t keywords, const fluid_postfx* fx, const PostFXOut& o, int images,
+                          const int* members) {
     using D4 = typename Sd::T4;
     using T4 = typename St::T4;
     using T1 = typename St::T1;
@@ -2163,7 +2275,7 @@ static int post_fx_chains(fluid_t* h, uint32_t keywords, const fluid_postfx* fx,
     if (h->slab() && !kSlab) return fail(h, FLUID_ERR_INVALID, "post-FX on a slab handle is fp32 and LINEAR only");
     const bool bloom_on = keywords & FLUID_DISPLAY_BLOOM, sun_on = keywords & FLUID_DISPLAY_SUNRAYS;
     const int bw = o.bw, bh = o.bh, sw = o.sw, sh = o.sh, levels = o.levels;
-    const int Wd = h->cfg.dye_w, Hd = h->cfg.dye_h, B = h->members;
+    const int Wd = h->cfg.dye_w, Hd = h->cfg.dye_h, B = h->members, Z = images;
     T4* bloom = static_cast<T4*>(h->pfx.bloom);
     T1 *sun = static_cast<T1*>(h->pfx.sun), *sun2 = sun ? sun + (size_t)sw * sh * B : nullptr;
     dim3 b(32, 8);
@@ -2181,22 +2293,22 @@ static int post_fx_chains(fluid_t* h, uint32_t keywords, const fluid_postfx* fx,
         const double knee = fx->bloom_threshold * fx->bloom_soft_knee + 0.0001;
         const int j_lo = band_row(bh, h->rank, h->world), j_hi = band_row(bh, h->rank + 1, h->world);
         if (j_hi > j_lo) {
-            bloom_prefilter_kernel<Sd, St, Smp, BATCH><<<grid2d(bw, j_hi - j_lo, b, B), b, 0, h->stream>>>(
+            bloom_prefilter_kernel<Sd, St, Smp, BATCH><<<grid2d(bw, j_hi - j_lo, b, Z), b, 0, h->stream>>>(
                 (const D4*)h->dye.read, Wd, Hd, h->droff, bloom, bw, bh, j_lo, j_hi, (float)(fx->bloom_threshold - knee),
-                (float)(knee * 2), (float)(0.25 / knee), (float)fx->bloom_threshold);
+                (float)(knee * 2), (float)(0.25 / knee), (float)fx->bloom_threshold, members);
             ++nk;
         }
         if ((rc = gather_bands(h, GB_BLOOM))) return rc;
         Lv last{bloom, bw, bh};
         for (auto& d : pyr) {
-            box4_kernel<St, Smp, BATCH><<<grid2d(d.w, d.h, b, B), b, 0, h->stream>>>(last.p, last.w, last.h, d.p, d.w, d.h, 1.0f, 0);
+            box4_kernel<St, Smp, BATCH><<<grid2d(d.w, d.h, b, Z), b, 0, h->stream>>>(last.p, last.w, last.h, d.p, d.w, d.h, 1.0f, 0);
             last = d; ++nk;
         }
         for (int i = (int)pyr.size() - 2; i >= 0; --i) {
-            box4_kernel<St, Smp, BATCH><<<grid2d(pyr[i].w, pyr[i].h, b, B), b, 0, h->stream>>>(last.p, last.w, last.h, pyr[i].p, pyr[i].w, pyr[i].h, 1.0f, 1);
+            box4_kernel<St, Smp, BATCH><<<grid2d(pyr[i].w, pyr[i].h, b, Z), b, 0, h->stream>>>(last.p, last.w, last.h, pyr[i].p, pyr[i].w, pyr[i].h, 1.0f, 1);
             last = pyr[i]; ++nk;
         }
-        box4_kernel<St, Smp, BATCH><<<grid2d(bw, bh, b, B), b, 0, h->stream>>>(last.p, last.w, last.h, bloom, bw, bh, (float)fx->bloom_intensity, 0);
+        box4_kernel<St, Smp, BATCH><<<grid2d(bw, bh, b, Z), b, 0, h->stream>>>(last.p, last.w, last.h, bloom, bw, bh, (float)fx->bloom_intensity, 0);
         ++nk;
     }
     // ---- applySunrays(dye.read, dye.write, sunrays); blur(sunrays, sunraysTemp, 1) -------------------
@@ -2212,11 +2324,11 @@ static int post_fx_chains(fluid_t* h, uint32_t keywords, const fluid_postfx* fx,
             }
         }
         if (!gathered) {
-            sunrays_mask_kernel<Sd, Smp, BATCH><<<grid2d(Wd, Hd, b, B), b, 0, h->stream>>>((const D4*)h->dye.read, (D4*)h->dye.write, Wd, Hd, 0, Hd, 0, nullptr);
-            sunrays_kernel<Sd, St, Smp, BATCH><<<grid2d(sw, sh, b, B), b, 0, h->stream>>>((const D4*)h->dye.write, Wd, Hd, sun, sw, sh, (float)fx->sunrays_weight);
+            sunrays_mask_kernel<Sd, Smp, BATCH><<<grid2d(Wd, Hd, b, Z), b, 0, h->stream>>>((const D4*)h->dye.read, (D4*)h->dye.write, Wd, Hd, 0, Hd, 0, nullptr, members);
+            sunrays_kernel<Sd, St, Smp, BATCH><<<grid2d(sw, sh, b, Z), b, 0, h->stream>>>((const D4*)h->dye.write, Wd, Hd, sun, sw, sh, (float)fx->sunrays_weight, members);
         }
-        blur3_kernel<St, Smp, BATCH><<<grid2d(sw, sh, b, B), b, 0, h->stream>>>(sun, sun2, sw, sh, (float)(1.0 / (double)sw), 0.0f);
-        blur3_kernel<St, Smp, BATCH><<<grid2d(sw, sh, b, B), b, 0, h->stream>>>(sun2, sun, sw, sh, 0.0f, (float)(1.0 / (double)sh));
+        blur3_kernel<St, Smp, BATCH><<<grid2d(sw, sh, b, Z), b, 0, h->stream>>>(sun, sun2, sw, sh, (float)(1.0 / (double)sw), 0.0f);
+        blur3_kernel<St, Smp, BATCH><<<grid2d(sw, sh, b, Z), b, 0, h->stream>>>(sun2, sun, sw, sh, 0.0f, (float)(1.0 / (double)sh));
         nk += 4;
     }
     return check_launch(h, "post-FX kernels", nk);
@@ -2224,7 +2336,7 @@ static int post_fx_chains(fluid_t* h, uint32_t keywords, const fluid_postfx* fx,
 
 // post_fx_chains<Sd, St, Smp> of a handle: the dye's and the targets' storage, and the sampler.  A batch handle
 // is fp32 and LINEAR.
-using Chains = int (*)(fluid_t*, uint32_t, const fluid_postfx*, const PostFXOut&);
+using Chains = int (*)(fluid_t*, uint32_t, const fluid_postfx*, const PostFXOut&, int, const int*);
 template <class Smp>
 static Chains chains_for(const fluid_t* h) {
     return !h->half_fx ? post_fx_chains<StoreF32, StoreF32, Smp>
@@ -2295,6 +2407,8 @@ struct DrawRequest {
     float* host_bloom;                 // the bloom FBO / sunrays texture, read back when given
     float* host_sunrays;
     bool batch;                        // a batch handle's call: one image per member, member by member in dst
+    bool subset;                       // a batch call for the listed members only: image k is member members[k]
+    const int32_t* members; int n_members;
 };
 
 // render(target) of S:1296-1317: the post-FX chains of the keywords that are on, then the background and
@@ -2304,28 +2418,31 @@ struct DrawRequest {
 // call is collective (post_fx_chains gathers), so every argument check comes before the first exchange.
 // Half storage draws from a widened copy of dye; its post-FX needs FLUID_FLAG_HALF_POSTFX, and then the
 // chains read the fp16 dye directly and draw the mask into the fp16 dye.write.  A batch request draws every
-// member of a batch handle through the same launches, each launch B layers of blocks deep; only batch requests
-// take a batch handle.
+// member of a batch handle through the same launches, each launch B layers of blocks deep, or with `subset` the
+// n_members listed members, n_members layers deep; only batch requests take a batch handle.
 static int draw(fluid_t* h, const DrawRequest& r) {
     if (!h) return FLUID_ERR_INVALID;
     if (h->batch && !r.batch) return not_on_batch(h, r.what);
     if (r.batch && !h->batch) return fail(h, FLUID_ERR_INVALID, "%s takes a batch handle (fluid_create_batch)", r.what);
+    if (r.subset) { if (int rc = check_member_list(h, r.what, r.members, r.n_members)) return rc; }
     if (r.keywords & ~(uint32_t)(FLUID_DISPLAY_SHADING | FLUID_DISPLAY_BLOOM | FLUID_DISPLAY_SUNRAYS))
         return fail(h, FLUID_ERR_INVALID, "unknown display keyword bits 0x%x", r.keywords);
     const bool bloom_on = r.keywords & FLUID_DISPLAY_BLOOM, sun_on = r.keywords & FLUID_DISPLAY_SUNRAYS;
     const bool postfx = bloom_on || sun_on, bytes = r.out != OUT_FRAME;
-    if (!r.dst || r.width < 1 || r.height < 1 || r.canvas_w < 1 || r.canvas_h < 1 || (postfx && !r.fx) ||
+    const size_t images = r.subset ? (size_t)r.n_members : (size_t)h->members;
+    if ((!r.dst && images > 0) || r.width < 1 || r.height < 1 || r.canvas_w < 1 || r.canvas_h < 1 || (postfx && !r.fx) ||
         (bloom_on && (!r.dither || r.dw < 1 || r.dh < 1)))
         return fail(h, FLUID_ERR_INVALID, "bad argument");
     int y0 = 0, y1 = r.height;
     if (h->slab()) fluid_render_band(h, r.height, &y0, &y1);
-    const size_t cells = (size_t)r.width * (y1 - y0), images = h->members;
+    const size_t cells = (size_t)r.width * (y1 - y0);
     if (r.batch && r.n != 4 * cells * images)
-        return fail(h, FLUID_ERR_INVALID, "%s: the targets of %d members have %zu bytes, caller passed %zu", r.what,
-                    h->members, 4 * cells * images, r.n);
+        return fail(h, FLUID_ERR_INVALID, "%s: the targets of %zu images have %zu bytes, caller passed %zu", r.what,
+                    images, 4 * cells * images, r.n);
     if (r.n != 4 * cells * images)
         return fail(h, FLUID_ERR_INVALID, "%s: the target%s has %zu %s, caller passed %zu", r.what, h->slab() ? " band" : "",
                     4 * cells, bytes ? "bytes" : "floats", r.n);
+    if (images == 0) return FLUID_OK;
     if (cells == 0 && !h->slab()) return FLUID_OK;      // a slab rank with no rows still takes part in the exchanges
     if (h->half && !h->half_fx && postfx)
         return fail(h, FLUID_ERR_INVALID, "%s with BLOOM or SUNRAYS is not built for FLUID_FLAG_HALF_STORAGE "
@@ -2345,7 +2462,9 @@ static int draw(fluid_t* h, const DrawRequest& r) {
         if (need > h->Gd)
             return fail(h, FLUID_ERR_HALO, "a frame of a %d-row target needs %d dye ghost rows, the slab keeps %d", r.height, need, h->Gd);
     }
-    if (postfx && (rc = chains_of(h)(h, r.keywords, r.fx, o))) return rc;
+    if (r.subset && (rc = upload_member_list(h, r.members, r.n_members))) return rc;
+    const int* list = r.subset ? h->member_list : nullptr;
+    if (postfx && (rc = chains_of(h)(h, r.keywords, r.fx, o, (int)images, list))) return rc;
     const float4* dye_src;
     if ((rc = display_source(h, &dye_src))) return rc;
     // texelSize = 1 / width, 1 / height (S:1337) and getTextureScale (S:1626-1631) are JS doubles, narrowed here
@@ -2355,11 +2474,11 @@ static int draw(fluid_t* h, const DrawRequest& r) {
     const DisplayArgs a{dye_src, h->cfg.dye_w, h->cfg.dye_h, h->droff, bloom_on ? h->pfx.bloom : nullptr, o.bw, o.bh,
                         sun_on ? h->pfx.sun : nullptr, o.sw, o.sh, bloom_on ? h->pfx.dither : nullptr, r.dw, r.dh,
                         r.on_device ? r.dst : h->frame, r.width, r.height, y0, y1, r.back[0], r.back[1], r.back[2], r.bg_mode,
-                        h->cfg.aspect, ts};
+                        h->cfg.aspect, ts, list};
     dim3 b(32, 8);
     const DisplayKernel k = h->batch ? kDisplayBatch[r.out][r.keywords] : kDisplay[h->nearest][r.out][h->half_fx][r.keywords];
     if (cells > 0) {
-        k<<<grid2d(r.width, y1 - y0, b, h->members), b, 0, h->stream>>>(a);
+        k<<<grid2d(r.width, y1 - y0, b, (int)images), b, 0, h->stream>>>(a);
         if ((rc = check_launch(h, "display_kernel"))) return rc;
     }
     if (r.on_device) return FLUID_OK;
@@ -2412,14 +2531,15 @@ int fluid_render_postfx(fluid_t* h, int width, int height, const fluid_postfx* f
 static int capture(fluid_t* h, const char* what, int width, int height, int canvas_w, int canvas_h, uint32_t keywords,
                    int transparent, const fluid_postfx* fx, const float* dither_rgb, int dw, int dh,
                    float back_r, float back_g, float back_b, uint8_t* dst, size_t n_bytes, bool on_device,
-                   bool batch = false) {
+                   bool batch = false, bool subset = false, const int32_t* members = nullptr, int n_members = 0) {
     // drawColor's store of normalizeColor(BACK_COLOR) into the half-float target
     const float b16[3] = {__half2float(__float2half_rn(back_r)), __half2float(__float2half_rn(back_g)),
                           __half2float(__float2half_rn(back_b))};
     return draw(h, {.what = what, .width = width, .height = height, .canvas_w = canvas_w,
                     .canvas_h = canvas_h, .keywords = keywords, .fx = fx, .dither = dither_rgb, .dw = dw, .dh = dh,
                     .back = {b16[0], b16[1], b16[2]}, .bg_mode = transparent ? 2 : 0, .out = OUT_CAPTURE,
-                    .on_device = on_device, .dst = dst, .n = n_bytes, .batch = batch});
+                    .on_device = on_device, .dst = dst, .n = n_bytes, .batch = batch, .subset = subset,
+                    .members = members, .n_members = n_members});
 }
 
 int fluid_capture(fluid_t* h, int width, int height, int canvas_w, int canvas_h, uint32_t keywords,
@@ -2452,11 +2572,13 @@ int fluid_capture_batch(fluid_t* h, int width, int height, int canvas_w, int can
 // frame buffer, or straight into the caller's device memory, stream-ordered.
 static int canvas(fluid_t* h, const char* what, int width, int height, uint32_t keywords, int transparent,
                   const fluid_postfx* fx, const float* dither_rgb, int dw, int dh, float back_r, float back_g,
-                  float back_b, uint8_t* dst, size_t n_bytes, int dst_on_device, bool batch) {
+                  float back_b, uint8_t* dst, size_t n_bytes, int dst_on_device, bool batch, bool subset = false,
+                  const int32_t* members = nullptr, int n_members = 0) {
     return draw(h, {.what = what, .width = width, .height = height, .canvas_w = width,
                     .canvas_h = height, .keywords = keywords, .fx = fx, .dither = dither_rgb, .dw = dw, .dh = dh,
                     .back = {back_r, back_g, back_b}, .bg_mode = transparent ? 1 : 0, .out = OUT_CANVAS,
-                    .on_device = dst_on_device != 0, .dst = dst, .n = n_bytes, .batch = batch});
+                    .on_device = dst_on_device != 0, .dst = dst, .n = n_bytes, .batch = batch, .subset = subset,
+                    .members = members, .n_members = n_members});
 }
 
 int fluid_render_canvas(fluid_t* h, int width, int height, uint32_t keywords, int transparent,
@@ -2474,6 +2596,23 @@ int fluid_render_canvas_batch(fluid_t* h, int width, int height, uint32_t keywor
                               uint8_t* dst, size_t n_bytes, int dst_on_device) {
     return canvas(h, "fluid_render_canvas_batch", width, height, keywords, transparent, fx, dither_rgb, dw, dh,
                   back_r, back_g, back_b, dst, n_bytes, dst_on_device, true);
+}
+
+// fluid_capture_batch and fluid_render_canvas_batch for the listed members: image k is member members[k]'s, through
+// the launches of one whole-batch draw, each n layers of blocks deep, in the same post-FX targets.
+int fluid_capture_members(fluid_t* h, int width, int height, int canvas_w, int canvas_h, uint32_t keywords,
+                          int transparent, const fluid_postfx* fx, const float* dither_rgb, int dw, int dh,
+                          float back_r, float back_g, float back_b, uint8_t* dst, size_t n_bytes, int dst_on_device,
+                          const int32_t* members, int n) {
+    return capture(h, "fluid_capture_members", width, height, canvas_w, canvas_h, keywords, transparent, fx, dither_rgb,
+                   dw, dh, back_r, back_g, back_b, dst, n_bytes, dst_on_device != 0, true, true, members, n);
+}
+int fluid_render_canvas_members(fluid_t* h, int width, int height, uint32_t keywords, int transparent,
+                                const fluid_postfx* fx, const float* dither_rgb, int dw, int dh,
+                                float back_r, float back_g, float back_b,
+                                uint8_t* dst, size_t n_bytes, int dst_on_device, const int32_t* members, int n) {
+    return canvas(h, "fluid_render_canvas_members", width, height, keywords, transparent, fx, dither_rgb, dw, dh,
+                  back_r, back_g, back_b, dst, n_bytes, dst_on_device, true, true, members, n);
 }
 
 void* fluid_host_alloc(size_t bytes) {

@@ -42,13 +42,18 @@ __device__ __forceinline__ float linear_fetch_rgb_r_repeat(const float* __restri
 // the sampler of every texture a chain reads (S:1017, S:1039: the filter of dye, bloom, pyramid and
 // sunrays follows ext.supportLinearFiltering).
 //
-// BATCH: a batch handle's draw, blockIdx.z the member.  Every array a kernel reads or writes holds the B
-// members back to back, as a dense (B, h, w[, C]) array of its own size, so member m of a w x h array starts
+// BATCH: a batch handle's draw, blockIdx.z the image.  Every array a kernel reads or writes holds the members
+// back to back, as a dense (B, h, w[, C]) array of its own size, so member m of a w x h array starts
 // member_offset(w, h) texels in.  The pointers move before any tap, so the sampler's clamp keeps every tap
-// inside the member.
+// inside the member.  Image z draws dye member members[z] when a member list is given (a subset draw), member z
+// otherwise; the post-FX targets stay dense by image.
 
 // texels before member blockIdx.z of a dense (B, h, w) array, in 64 bits
 __device__ __forceinline__ size_t member_offset(int w, int h) { return (size_t)blockIdx.z * w * h; }
+// texels before the dye member image blockIdx.z draws: members[blockIdx.z], or blockIdx.z without a list
+__device__ __forceinline__ size_t dye_member_offset(const int* members, int w, int h) {
+    return (members ? (size_t)__ldg(members + blockIdx.z) : (size_t)blockIdx.z) * w * h;
+}
 // p as T texels, at member blockIdx.z of a w x h array when BATCH
 template <bool BATCH, class T>
 __device__ __forceinline__ const T* member_of(const void* p, int w, int h) {
@@ -64,8 +69,9 @@ template <class Sd, class St, class Smp, bool BATCH = false>
 __global__ void __launch_bounds__(256) bloom_prefilter_kernel(const typename Sd::T4* __restrict__ dye, int Wd, int Hd,
                                                               int dye_row_off, typename St::T4* __restrict__ out, int w,
                                                               int h, int j_lo, int j_hi, float curve0, float curve1,
-                                                              float curve2, float threshold) {
-    if constexpr (BATCH) { dye += member_offset(Wd, Hd); out += member_offset(w, h); }
+                                                              float curve2, float threshold,
+                                                              const int* __restrict__ members = nullptr) {
+    if constexpr (BATCH) { dye += dye_member_offset(members, Wd, Hd); out += member_offset(w, h); }
     const int i = blockIdx.x * blockDim.x + threadIdx.x, j = j_lo + blockIdx.y * blockDim.y + threadIdx.y;
     if (i >= w || j >= j_hi) return;
     const float uvx = ((float)i + 0.5f) / (float)w, uvy = ((float)j + 0.5f) / (float)h;
@@ -102,11 +108,16 @@ __global__ void __launch_bounds__(256) box4_kernel(const typename St::T4* __rest
 // sunraysMaskShader S:676-691 (target = dye.write, like the reference: S:1300, so stored as the dye is), on dye
 // rows [j_lo, j_hi); dye and mask are buffers whose first row is global row row_off.  alpha, when not null, also
 // receives the mask's alpha at global row j of a dense Wd x Hd array: the band a slab rank gathers (fp32 dye only).
+// BATCH: the mask goes into the drawn member's own dye.write.
 template <class Sd, class Smp, bool BATCH = false>
 __global__ void __launch_bounds__(256) sunrays_mask_kernel(const typename Sd::T4* __restrict__ dye,
                                                            typename Sd::T4* __restrict__ mask, int Wd, int Hd,
-                                                           int j_lo, int j_hi, int row_off, float* __restrict__ alpha) {
-    if constexpr (BATCH) { dye += member_offset(Wd, Hd); mask += member_offset(Wd, Hd); }
+                                                           int j_lo, int j_hi, int row_off, float* __restrict__ alpha,
+                                                           const int* __restrict__ members = nullptr) {
+    if constexpr (BATCH) {
+        const size_t mo = dye_member_offset(members, Wd, Hd);
+        dye += mo; mask += mo;
+    }
     const int i = blockIdx.x * blockDim.x + threadIdx.x, j = j_lo + blockIdx.y * blockDim.y + threadIdx.y;
     if (i >= Wd || j >= j_hi) return;
     const float uvx = ((float)i + 0.5f) / (float)Wd, uvy = ((float)j + 0.5f) / (float)Hd;
@@ -123,11 +134,12 @@ __device__ __forceinline__ float mask_alpha(float4 v) { return v.w; }
 __device__ __forceinline__ float mask_alpha(float v) { return v; }
 
 // sunraysShader S:693-724.  M: the mask's texel type, Sd::T4 (the mask in dye.write) or float (a slab's
-// gathered alpha).
+// gathered alpha).  BATCH: the mask of the drawn member, in its dye.write.
 template <class Sd, class St, class Smp, bool BATCH = false, class M = typename Sd::T4>
 __global__ void __launch_bounds__(256) sunrays_kernel(const M* __restrict__ mask, int Wm, int Hm,
-                                                      typename St::T1* __restrict__ out, int w, int h, float weight) {
-    if constexpr (BATCH) { mask += member_offset(Wm, Hm); out += member_offset(w, h); }
+                                                      typename St::T1* __restrict__ out, int w, int h, float weight,
+                                                      const int* __restrict__ members = nullptr) {
+    if constexpr (BATCH) { mask += dye_member_offset(members, Wm, Hm); out += member_offset(w, h); }
     const int i = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y * blockDim.y + threadIdx.y;
     if (i >= w || j >= h) return;
     const float Density = 0.3f, Decay = 0.95f, Exposure = 0.7f;
@@ -218,6 +230,7 @@ struct DisplayArgs {
     int bg_mode;
     float aspect;
     float4 ts;                          // 1/w, 1/h and getTextureScale of the dithering texture (BLOOM)
+    const int* members;                 // BATCH: the dye member of each image (a subset draw), or null: image z
 };
 
 // Output policies of display_kernel: the element type of `out`, the row of `out` that row r of an
@@ -266,13 +279,17 @@ struct StoreCanvas {
 // the background of render() (the output policy's store() blends).  Out: the output policy; Sp: the storage policy
 // of the bloom and sunrays targets (post_fx_chains' St); Smp: the sampler of the dye, bloom and sunrays
 // taps (the dithering tap is LINEAR + REPEAT whatever Smp is).  A slab rank draws the band [y0, y1) of the
-// target from its own dye rows (+ ghost rows); one GPU draws the whole target.  BATCH: member blockIdx.z
-// reads its own dye, bloom FBO and sunrays texture and draws its own image; the dithering texture is shared.
+// target from its own dye rows (+ ghost rows); one GPU draws the whole target.  BATCH: image blockIdx.z reads
+// its member's dye (a.members) and its own bloom FBO and sunrays texture, and draws its own image; the dithering
+// texture is shared.
 template <bool SHADING, bool BLOOM, bool SUNRAYS, class Out, class Sp, class Smp, bool BATCH = false>
 __global__ void __launch_bounds__(256) display_kernel(DisplayArgs a) {
     // the bloom FBO and the sunrays texture are offset where they are read: a member pointer kept across the
-    // shading's IEEE div / sqrt slow paths spills the SHADING | SUNRAYS capture
+    // shading's IEEE div / sqrt slow paths spills the SHADING | SUNRAYS capture.  For the same reason a listed
+    // member's dye is reached by a signed step taken before member z's offset (dye_member_offset, or the step
+    // taken after it, spills that capture)
     if constexpr (BATCH) {
+        if (a.members) a.dye += (ptrdiff_t)(__ldg(a.members + blockIdx.z) - (int)blockIdx.z) * a.Wd * a.Hd;
         a.dye += member_offset(a.Wd, a.Hd);
         a.out = static_cast<typename Out::T*>(a.out) + member_offset(a.w, a.y1 - a.y0);
     }

@@ -696,7 +696,9 @@ class FluidBatch(_Handle):
     applies to every member, except that `member_config[m]` (a dict per member, empty at creation) overrides the
     MEMBER_KEYS for member m: a parameter sweep.  step() takes one dt, or one per member.  flags: FLAG_NO_GRAPH or
     0.  render_canvas() and captureScreenshot() draw every member through one set of launches; render(), resize and
-    the per-pass entry points are FluidSimulation's only."""
+    the per-pass entry points are FluidSimulation's only.  readField(), writeField(), render_canvas() and
+    captureScreenshot() take `members=`, a host list of distinct member indices, to act on those members only, and
+    reset(members) puts members back to their state at creation."""
 
     # the config keys a member can hold a value of its own for (fluid_set_param_members)
     MEMBER_KEYS = ("DENSITY_DISSIPATION", "VELOCITY_DISSIPATION", "PRESSURE", "CURL", "SPLAT_RADIUS")
@@ -794,19 +796,43 @@ class FluidBatch(_Handle):
         self._check(self._L.fluid_splats_batch(self._h, m.ctypes.data_as(C.POINTER(C.c_int32)),
                                                a.ctypes.data_as(C.POINTER(C.c_float)), m.size))
 
-    def _shape(self, name):
+    def _shape(self, name, n=None):
+        """(n, H, W[, C]) of a field: n images, B of them when n is None."""
         w, h, c, _ = self._dims(name)
-        return (self.members, h, w, c) if c > 1 else (self.members, h, w)
+        n = self.members if n is None else n
+        return (n, h, w, c) if c > 1 else (n, h, w)
 
-    def readField(self, name, out=None) -> np.ndarray:
+    @staticmethod
+    def _member_list(members):
+        """`members` (a sequence or numpy array of member indices, or None) as a C-contiguous int32 vector and its
+        ctypes pointer; (None, None) for None.  Member lists live on the host: a CUDA array is a ValueError.  The
+        library checks the indices (distinct, in [0, B))."""
+        if members is None:
+            return None, None
+        if hasattr(members, "__cuda_array_interface__"):
+            raise ValueError("members must be a host sequence or numpy array of member indices, not a CUDA array")
+        a = np.asarray(members)
+        if a.ndim != 1 or (a.size and not np.issubdtype(a.dtype, np.integer)):
+            raise ValueError(f"members must be a 1-D list of integer member indices, got {a.dtype} {a.shape}")
+        m = np.ascontiguousarray(a, np.int32)
+        if not np.array_equal(m, a):
+            raise ValueError("members holds an index outside the int32 range")
+        return m, m.ctypes.data_as(C.POINTER(C.c_int32))
+
+    def readField(self, name, out=None, members=None) -> np.ndarray:
         """(B, H, W[, C]) float32, member by member, row 0 = bottom.  `out` as FluidSimulation.readField: a
         float32 host buffer of that size, or a C-contiguous float32 CUDA array of that many elements, filled on
-        the GPU and returned as passed."""
-        shape = self._shape(name)
+        the GPU and returned as passed.  members: (n, H, W[, C]) of the listed members only, slot k member
+        members[k] (fluid_read_members)."""
+        m, mp = self._member_list(members)
+        shape = self._shape(name, None if m is None else m.size)
         n = int(np.prod(shape))
         dst = _device_array(out, "<f4", n, "readField")
         if dst is not None:
-            self._check(self._L.fluid_read_device(self._h, FIELD[name], dst, n))
+            if m is None:
+                self._check(self._L.fluid_read_device(self._h, FIELD[name], dst, n))
+            else:
+                self._check(self._L.fluid_read_members(self._h, FIELD[name], mp, m.size, dst, n, 1))
             self.sync()
             return out
         if out is None:
@@ -814,46 +840,72 @@ class FluidBatch(_Handle):
         else:
             assert out.dtype == np.float32 and out.flags.c_contiguous and out.size == n
             out = out.reshape(shape)
-        self._check(self._L.fluid_read(self._h, FIELD[name], out.ctypes.data_as(C.c_void_p), out.size))
+        if m is None:
+            self._check(self._L.fluid_read(self._h, FIELD[name], out.ctypes.data_as(C.c_void_p), out.size))
+        else:
+            self._check(self._L.fluid_read_members(self._h, FIELD[name], mp, m.size, out.ctypes.data_as(C.c_void_p),
+                                                   out.size, 0))
         return out
 
-    def writeField(self, name, array):
+    def writeField(self, name, array, members=None):
         """Overwrites a field of every member with `array` ((B, H, W[, C])): anything numpy turns into float32,
-        or a C-contiguous float32 CUDA array of exactly that many elements."""
-        n = int(np.prod(self._shape(name)))
+        or a C-contiguous float32 CUDA array of exactly that many elements.  members: only the listed members,
+        `array` then (n, H, W[, C]) with slot k for member members[k] (fluid_write_members); the others keep
+        every bit."""
+        m, mp = self._member_list(members)
+        n = int(np.prod(self._shape(name, None if m is None else m.size)))
         if hasattr(array, "__cuda_array_interface__"):
             src = _device_array(array, "<f4", n, "writeField")
-            self._check(self._L.fluid_write_device(self._h, FIELD[name], src, n))
+            if m is None:
+                self._check(self._L.fluid_write_device(self._h, FIELD[name], src, n))
+            else:
+                self._check(self._L.fluid_write_members(self._h, FIELD[name], mp, m.size, src, n, 1))
             self.sync()
             return
         a = np.ascontiguousarray(array, np.float32)
-        self._check(self._L.fluid_write(self._h, FIELD[name], a.ctypes.data_as(C.c_void_p), a.size))
+        if m is None:
+            self._check(self._L.fluid_write(self._h, FIELD[name], a.ctypes.data_as(C.c_void_p), a.size))
+        else:
+            self._check(self._L.fluid_write_members(self._h, FIELD[name], mp, m.size, a.ctypes.data_as(C.c_void_p),
+                                                    a.size, 0))
 
-    def render_canvas(self, out=None):
+    def reset(self, members):
+        """The listed members back to their state at creation: every field zero, dye alpha 1, in one launch
+        (fluid_reset_members).  member_config is config and stays."""
+        m, mp = self._member_list(members)
+        if m is None:
+            raise ValueError("reset() takes a list of member indices")
+        self._check(self._L.fluid_reset_members(self._h, mp, m.size))
+
+    def _draw(self, fn_all, fn_members, what, w, h, args, out, members):
+        """A whole-batch draw, or with `members` the draw of the listed members only, image k member members[k]."""
+        m, mp = self._member_list(members)
+        n = self.members if m is None else m.size
+        dst, result, on_device = _u8_destination(out, (n, h, w, 4), what)
+        tail = (dst, 4 * w * h * n, 1 if on_device else 0)
+        self._check(fn_all(self._h, w, h, *args, *tail) if m is None else fn_members(self._h, w, h, *args, *tail, mp, n))
+        if on_device:
+            self.sync()
+        return result
+
+    def render_canvas(self, out=None, members=None):
         """FluidSimulation.render_canvas for every member (fluid_render_canvas_batch): (B, canvas height, canvas
         width, 4) uint8, member by member, member m's image the bytes a FluidSimulation of this config and canvas
         draws from member m's dye.  Config, canvas and `self.dithering` as there.  `out`: a C-contiguous uint8 numpy
         array of that many bytes, or a C-contiguous uint8 CUDA array of them with render_canvas's waits, returned
-        as it was passed."""
+        as it was passed.  members: the listed members' images only, (n, h, w, 4), image k member members[k]
+        (fluid_render_canvas_members)."""
         w, h, args = self._canvas_args()
-        B = self.members
-        dst, result, on_device = _u8_destination(out, (B, h, w, 4), "render_canvas")
-        self._check(self._L.fluid_render_canvas_batch(self._h, w, h, *args, dst, 4 * w * h * B, 1 if on_device else 0))
-        if on_device:
-            self.sync()
-        return result
+        return self._draw(self._L.fluid_render_canvas_batch, self._L.fluid_render_canvas_members, "render_canvas",
+                          w, h, args, out, members)
 
-    def captureScreenshot(self, out=None):
+    def captureScreenshot(self, out=None, members=None):
         """FluidSimulation.captureScreenshot for every member (fluid_capture_batch): (B, h, w, 4) uint8 at
         getResolution(CAPTURE_RESOLUTION) of the canvas, member by member, each top row first.  No PNG is written.
-        `out` as in render_canvas."""
+        `out` and `members` as in render_canvas (fluid_capture_members)."""
         w, h, args = self._capture_args()
-        B = self.members
-        dst, result, on_device = _u8_destination(out, (B, h, w, 4), "captureScreenshot")
-        self._check(self._L.fluid_capture_batch(self._h, w, h, *args, dst, 4 * w * h * B, 1 if on_device else 0))
-        if on_device:
-            self.sync()
-        return result
+        return self._draw(self._L.fluid_capture_batch, self._L.fluid_capture_members, "captureScreenshot",
+                          w, h, args, out, members)
 
 
 def _fx_args(fx, dith):
