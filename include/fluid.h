@@ -196,7 +196,8 @@ int fluid_p2p_disable(fluid_t* h);   /* back to NCCL; call on every rank if any 
  *    the other members following it contiguously.
  *  - fluid_sync, fluid_stat, fluid_launch_count, fluid_mark, fluid_elapsed_ms, fluid_timing_last,
  *    fluid_last_error and fluid_destroy behave as on any handle.
- *  - fluid_render_canvas_batch and fluid_capture_batch draw every member's canvas or capture in one call.
+ *  - fluid_render_canvas_batch and fluid_capture_batch draw every member's canvas or capture in one call;
+ *    fluid_render_canvas_looks and fluid_capture_looks give each image its own post-FX sliders and background.
  *  - Member subsets (below): fluid_read_members and fluid_write_members move, fluid_reset_members resets, and
  *    fluid_render_canvas_members and fluid_capture_members draw, only the members a list names.
  *  - Every other entry point refuses a batch handle with FLUID_ERR_INVALID and leaves it usable: the fp32
@@ -508,7 +509,8 @@ int fluid_render_canvas(fluid_t* h, int width, int height, uint32_t keywords, in
  * the launches one draw of an ordinary handle makes, each launch one layer of blocks per member.
  *  - Member m's image is the bytes fluid_render_canvas, or fluid_capture / fluid_capture_device, give an
  *    ordinary handle of the batch's config whose dye equals member m's.  Keywords, sliders, background and
- *    sizes apply to every member.
+ *    sizes apply to every member (fluid_render_canvas_looks / fluid_capture_looks, below, give each image its
+ *    own sliders and background).
  *  - dst is one C-contiguous (B, height, width, 4) array, member by member, each image top row first;
  *    n_bytes == B * 4 * width * height.
  *  - dst_on_device == 0: host memory, one device-to-host copy, then a stream sync.  dst_on_device != 0:
@@ -541,6 +543,33 @@ int fluid_capture_members(fluid_t* h, int width, int height, int canvas_w, int c
                           int transparent, const fluid_postfx* fx, const float* dither_rgb, int dw, int dh,
                           float back_r, float back_g, float back_b,
                           uint8_t* dst, size_t n_bytes, int dst_on_device, const int32_t* members, int n);
+/* The look of one image of a batch draw: the post-FX sliders of fluid_postfx and the background of the draw calls. */
+typedef struct fluid_look {
+    double bloom_intensity, bloom_threshold, bloom_soft_knee, sunrays_weight;  /* as in fluid_postfx */
+    float back_r, back_g, back_b;                                              /* BACK_COLOR / 255   */
+    int32_t transparent;                                                       /* as the draw calls'  */
+} fluid_look;
+/* Batch draws with a look per image: a contact sheet of one frame under many slider settings, or a dataset that
+ * varies the look per sample, in the launches of one shared-look draw.
+ *  - Which images: with members == NULL, n must be B and image k is member k (fluid_render_canvas_batch /
+ *    fluid_capture_batch); otherwise the list follows the rules of the member-subset calls (fluid_read_members)
+ *    and image k is member members[k] (fluid_render_canvas_members / fluid_capture_members).
+ *  - Image k is byte for byte what fluid_render_canvas, or fluid_capture, give an ordinary handle of the batch's
+ *    config whose dye equals its member's, called with fx's four sliders replaced by looks[k]'s and with
+ *    looks[k]'s back_* and transparent.  fx still supplies BLOOM_ITERATIONS, BLOOM_RESOLUTION and
+ *    SUNRAYS_RESOLUTION; keywords, the dithering texture, the canvas and the target sizes are shared.  As there,
+ *    fx and the sliders are read only with BLOOM or SUNRAYS, and any slider or background value is taken.
+ *  - The launches of the shared-look draw, plus one stream-ordered copy of the n images' looks, derived on the
+ *    host (the prefilter's knee and curve in double, narrowed once), into a table of B looks the handle
+ *    allocates at creation outside the field arena.  The caller may reuse `looks` as soon as the call returns.
+ * Refused with FLUID_ERR_INVALID, dst untouched and the handle usable: everything the _batch / _members calls
+ * refuse; members == NULL with n != B; looks == NULL with n > 0. */
+int fluid_render_canvas_looks(fluid_t* h, int width, int height, uint32_t keywords, const fluid_postfx* fx,
+                              const float* dither_rgb, int dw, int dh, const fluid_look* looks,
+                              uint8_t* dst, size_t n_bytes, int dst_on_device, const int32_t* members, int n);
+int fluid_capture_looks(fluid_t* h, int width, int height, int canvas_w, int canvas_h, uint32_t keywords,
+                        const fluid_postfx* fx, const float* dither_rgb, int dw, int dh, const fluid_look* looks,
+                        uint8_t* dst, size_t n_bytes, int dst_on_device, const int32_t* members, int n);
 
 int fluid_sync(fluid_t* h);
 int fluid_timing_last(fluid_t* h, fluid_timing* out);

@@ -27,7 +27,8 @@ SYMBOLS = [
     "fluid_last_error", "fluid_create_batch", "fluid_members", "fluid_splats_batch", "fluid_render_canvas_batch",
     "fluid_capture_batch", "fluid_set_param_members", "fluid_get_param_members", "fluid_step_members",
     "fluid_splats_device", "fluid_splats_batch_device", "fluid_read_members", "fluid_write_members",
-    "fluid_reset_members", "fluid_render_canvas_members", "fluid_capture_members",
+    "fluid_reset_members", "fluid_render_canvas_members", "fluid_capture_members", "fluid_render_canvas_looks",
+    "fluid_capture_looks",
 ]
 
 FLUID_OK = 0
@@ -66,6 +67,13 @@ class PostFX(C.Structure):
     _fields_ = [("bloom_iterations", C.c_int32), ("bloom_resolution", C.c_int32), ("bloom_intensity", C.c_double),
                 ("bloom_threshold", C.c_double), ("bloom_soft_knee", C.c_double), ("sunrays_resolution", C.c_int32),
                 ("sunrays_weight", C.c_double)]
+
+
+class Look(C.Structure):
+    """fluid_look: one image's post-FX sliders and background in fluid_render_canvas_looks / fluid_capture_looks."""
+    _fields_ = [("bloom_intensity", C.c_double), ("bloom_threshold", C.c_double), ("bloom_soft_knee", C.c_double),
+                ("sunrays_weight", C.c_double), ("back_r", C.c_float), ("back_g", C.c_float), ("back_b", C.c_float),
+                ("transparent", C.c_int32)]
 
 
 class Timing(C.Structure):
@@ -150,6 +158,9 @@ def lib():
     L.fluid_reset_members.argtypes = [vp, ip, i]
     L.fluid_render_canvas_members.argtypes = L.fluid_render_canvas_batch.argtypes + [ip, i]
     L.fluid_capture_members.argtypes = L.fluid_capture_batch.argtypes + [ip, i]
+    lk = C.POINTER(Look)
+    L.fluid_render_canvas_looks.argtypes = [vp, i, i, C.c_uint32, C.POINTER(PostFX), vp, i, i, lk, vp, sz, i, ip, i]
+    L.fluid_capture_looks.argtypes = [vp, i, i, i, i, C.c_uint32, C.POINTER(PostFX), vp, i, i, lk, vp, sz, i, ip, i]
     L.fluid_sync.argtypes = [vp]
     L.fluid_host_alloc.argtypes = [sz]; L.fluid_host_alloc.restype = vp
     L.fluid_host_free.argtypes = [vp]; L.fluid_host_free.restype = None

@@ -113,6 +113,7 @@ struct fluid : SlabGeometry {
     std::vector<float> member_host;
     std::vector<double> member_radius_d;
     int* member_list = nullptr;            // the member-subset calls' list (fluid_read_members ...): B int32, outside the arena
+    fk::ImageLook* look_table = nullptr;   // the looks of fluid_render_canvas_looks / fluid_capture_looks: B entries, outside the arena
     unsigned char* tiny_map = nullptr;     // where divergence has 0 < |d| < 2^-123 (jacobi.cuh): 1 byte per 128x32 cells, GLOBAL rows
     size_t tiny_map_bytes = 0;
     // 2-D tensor maps the blocked Jacobi kernel stages through: m[k] maps pressure slot k and divergence
@@ -900,6 +901,7 @@ int create_common(const fluid_config* cfg, int rank, int world, const void* uid,
         if (h->batch) {
             int r = alloc_member_table(h); if (r) return r;
             CU(cudaMalloc((void**)&h->member_list, (size_t)h->members * sizeof(int32_t)));
+            CU(cudaMalloc((void**)&h->look_table, (size_t)h->members * sizeof(fk::ImageLook)));
         } else {
             CU(cudaMalloc((void**)&h->dt_dev, sizeof(float)));
             CU(cudaMemsetAsync(h->dt_dev, 0, sizeof(float), h->stream));
@@ -1068,6 +1070,7 @@ void fluid_destroy(fluid_t* h) {
     cudaFree(h->exact_streams);
     cudaFree(h->dt_dev);
     cudaFree(h->member_list);
+    cudaFree(h->look_table);
     cudaFree(h->scratch);
     cudaFree(h->splat_scratch);
     cudaFree(h->frame);
@@ -1919,6 +1922,15 @@ static int upload_member_list(fluid_t* h, const int32_t* members, int n) {
     return FLUID_OK;
 }
 
+// The looks of n images (looks.h image_look) into the handle's look table, which the launches of the draw read:
+// one stream-ordered copy from pageable memory, like upload_member_list.
+static int upload_looks(fluid_t* h, const fluid_look* looks, int n) {
+    std::vector<fk::ImageLook> t(n);
+    for (int k = 0; k < n; ++k) t[k] = fk::image_look(looks[k]);
+    CU(cudaMemcpyAsync(h->look_table, t.data(), (size_t)n * sizeof(fk::ImageLook), cudaMemcpyHostToDevice, h->stream));
+    return FLUID_OK;
+}
+
 // The checks fluid_read_members / fluid_write_members share, all before any work; *p: the field's .read, *per:
 // the floats of one member
 static int members_io_args(fluid_t* h, const char* what, int field, const int32_t* members, int n, const void* buf,
@@ -2258,15 +2270,16 @@ static int post_fx_targets(fluid_t* h, uint32_t keywords, const PostFXOut& o, co
 // S:1300) with SUNRAYS.  Sd: the dye's storage policy (the mask is drawn in it), St: the targets', Smp: the sampler
 // of every texture the chains read (postfx.cuh).  BATCH: `images` images of a batch handle, each target a dense
 // (B, h, w) array of which image z takes slot z, and each launch `images` layers of blocks deep; image z draws
-// member members[z] (a subset draw's list in device memory), or member z when members is null.  Arguments checked
-// by the caller.
+// member members[z] (a subset draw's list in device memory), or member z when members is null; with `looks` (a
+// draw with a look per image, in device memory) image z takes its sliders from looks[z] and fx's are not read.
+// Arguments checked by the caller.
 // A slab rank (fp32, LINEAR) prefilters its band of the bloom FBO's rows and draws the mask on the dye rows it
 // owns; the bands are gathered (halo.cuh gather_bands), so every rank runs the pyramid, the sunrays and the blurs
 // on the inputs one GPU has and ends with its bits.  The dye ghost rows must be fresh (draw_ghost_rows).
 extern "C++" {
 template <class Sd, class St, class Smp, bool BATCH = false>
 static int post_fx_chains(fluid_t* h, uint32_t keywords, const fluid_postfx* fx, const PostFXOut& o, int images,
-                          const int* members) {
+                          const int* members, const ImageLook* looks) {
     using D4 = typename Sd::T4;
     using T4 = typename St::T4;
     using T1 = typename St::T1;
@@ -2290,12 +2303,13 @@ static int post_fx_chains(fluid_t* h, uint32_t keywords, const fluid_postfx* fx,
             pyr.push_back({p, pw, ph});
             p += (size_t)pw * ph * B;
         }
-        const double knee = fx->bloom_threshold * fx->bloom_soft_knee + 0.0001;
+        float curve[4];
+        prefilter_curve(fx->bloom_threshold, fx->bloom_soft_knee, curve);
         const int j_lo = band_row(bh, h->rank, h->world), j_hi = band_row(bh, h->rank + 1, h->world);
         if (j_hi > j_lo) {
             bloom_prefilter_kernel<Sd, St, Smp, BATCH><<<grid2d(bw, j_hi - j_lo, b, Z), b, 0, h->stream>>>(
-                (const D4*)h->dye.read, Wd, Hd, h->droff, bloom, bw, bh, j_lo, j_hi, (float)(fx->bloom_threshold - knee),
-                (float)(knee * 2), (float)(0.25 / knee), (float)fx->bloom_threshold, members);
+                (const D4*)h->dye.read, Wd, Hd, h->droff, bloom, bw, bh, j_lo, j_hi, curve[0], curve[1], curve[2], curve[3],
+                members, looks);
             ++nk;
         }
         if ((rc = gather_bands(h, GB_BLOOM))) return rc;
@@ -2308,7 +2322,8 @@ static int post_fx_chains(fluid_t* h, uint32_t keywords, const fluid_postfx* fx,
             box4_kernel<St, Smp, BATCH><<<grid2d(pyr[i].w, pyr[i].h, b, Z), b, 0, h->stream>>>(last.p, last.w, last.h, pyr[i].p, pyr[i].w, pyr[i].h, 1.0f, 1);
             last = pyr[i]; ++nk;
         }
-        box4_kernel<St, Smp, BATCH><<<grid2d(bw, bh, b, Z), b, 0, h->stream>>>(last.p, last.w, last.h, bloom, bw, bh, (float)fx->bloom_intensity, 0);
+        box4_kernel<St, Smp, BATCH><<<grid2d(bw, bh, b, Z), b, 0, h->stream>>>(last.p, last.w, last.h, bloom, bw, bh, (float)fx->bloom_intensity, 0,
+                                                                           looks);
         ++nk;
     }
     // ---- applySunrays(dye.read, dye.write, sunrays); blur(sunrays, sunraysTemp, 1) -------------------
@@ -2325,7 +2340,8 @@ static int post_fx_chains(fluid_t* h, uint32_t keywords, const fluid_postfx* fx,
         }
         if (!gathered) {
             sunrays_mask_kernel<Sd, Smp, BATCH><<<grid2d(Wd, Hd, b, Z), b, 0, h->stream>>>((const D4*)h->dye.read, (D4*)h->dye.write, Wd, Hd, 0, Hd, 0, nullptr, members);
-            sunrays_kernel<Sd, St, Smp, BATCH><<<grid2d(sw, sh, b, Z), b, 0, h->stream>>>((const D4*)h->dye.write, Wd, Hd, sun, sw, sh, (float)fx->sunrays_weight, members);
+            sunrays_kernel<Sd, St, Smp, BATCH><<<grid2d(sw, sh, b, Z), b, 0, h->stream>>>((const D4*)h->dye.write, Wd, Hd, sun, sw, sh, (float)fx->sunrays_weight, members,
+                                                                                    looks);
         }
         blur3_kernel<St, Smp, BATCH><<<grid2d(sw, sh, b, Z), b, 0, h->stream>>>(sun, sun2, sw, sh, (float)(1.0 / (double)sw), 0.0f);
         blur3_kernel<St, Smp, BATCH><<<grid2d(sw, sh, b, Z), b, 0, h->stream>>>(sun2, sun, sw, sh, 0.0f, (float)(1.0 / (double)sh));
@@ -2336,7 +2352,7 @@ static int post_fx_chains(fluid_t* h, uint32_t keywords, const fluid_postfx* fx,
 
 // post_fx_chains<Sd, St, Smp> of a handle: the dye's and the targets' storage, and the sampler.  A batch handle
 // is fp32 and LINEAR.
-using Chains = int (*)(fluid_t*, uint32_t, const fluid_postfx*, const PostFXOut&, int, const int*);
+using Chains = int (*)(fluid_t*, uint32_t, const fluid_postfx*, const PostFXOut&, int, const int*, const ImageLook*);
 template <class Smp>
 static Chains chains_for(const fluid_t* h) {
     return !h->half_fx ? post_fx_chains<StoreF32, StoreF32, Smp>
@@ -2409,6 +2425,8 @@ struct DrawRequest {
     bool batch;                        // a batch handle's call: one image per member, member by member in dst
     bool subset;                       // a batch call for the listed members only: image k is member members[k]
     const int32_t* members; int n_members;
+    bool per_image;                    // a batch call with a look per image: image k's is looks[k], n_members images
+    const fluid_look* looks;
 };
 
 // render(target) of S:1296-1317: the post-FX chains of the keywords that are on, then the background and
@@ -2419,12 +2437,17 @@ struct DrawRequest {
 // Half storage draws from a widened copy of dye; its post-FX needs FLUID_FLAG_HALF_POSTFX, and then the
 // chains read the fp16 dye directly and draw the mask into the fp16 dye.write.  A batch request draws every
 // member of a batch handle through the same launches, each launch B layers of blocks deep, or with `subset` the
-// n_members listed members, n_members layers deep; only batch requests take a batch handle.
+// n_members listed members, n_members layers deep; only batch requests take a batch handle.  With `per_image`
+// each image's sliders and background come from its look, uploaded into the look table before the launches.
 static int draw(fluid_t* h, const DrawRequest& r) {
     if (!h) return FLUID_ERR_INVALID;
     if (h->batch && !r.batch) return not_on_batch(h, r.what);
     if (r.batch && !h->batch) return fail(h, FLUID_ERR_INVALID, "%s takes a batch handle (fluid_create_batch)", r.what);
     if (r.subset) { if (int rc = check_member_list(h, r.what, r.members, r.n_members)) return rc; }
+    if (r.per_image && !r.subset && r.n_members != h->members)
+        return fail(h, FLUID_ERR_INVALID, "%s: n = %d without a member list, the batch has %d members", r.what,
+                    r.n_members, h->members);
+    if (r.per_image && !r.looks && r.n_members > 0) return fail(h, FLUID_ERR_INVALID, "%s: NULL looks", r.what);
     if (r.keywords & ~(uint32_t)(FLUID_DISPLAY_SHADING | FLUID_DISPLAY_BLOOM | FLUID_DISPLAY_SUNRAYS))
         return fail(h, FLUID_ERR_INVALID, "unknown display keyword bits 0x%x", r.keywords);
     const bool bloom_on = r.keywords & FLUID_DISPLAY_BLOOM, sun_on = r.keywords & FLUID_DISPLAY_SUNRAYS;
@@ -2463,8 +2486,10 @@ static int draw(fluid_t* h, const DrawRequest& r) {
             return fail(h, FLUID_ERR_HALO, "a frame of a %d-row target needs %d dye ghost rows, the slab keeps %d", r.height, need, h->Gd);
     }
     if (r.subset && (rc = upload_member_list(h, r.members, r.n_members))) return rc;
+    if (r.per_image && (rc = upload_looks(h, r.looks, r.n_members))) return rc;
     const int* list = r.subset ? h->member_list : nullptr;
-    if (postfx && (rc = chains_of(h)(h, r.keywords, r.fx, o, (int)images, list))) return rc;
+    const ImageLook* looks = r.per_image ? h->look_table : nullptr;
+    if (postfx && (rc = chains_of(h)(h, r.keywords, r.fx, o, (int)images, list, looks))) return rc;
     const float4* dye_src;
     if ((rc = display_source(h, &dye_src))) return rc;
     // texelSize = 1 / width, 1 / height (S:1337) and getTextureScale (S:1626-1631) are JS doubles, narrowed here
@@ -2474,7 +2499,7 @@ static int draw(fluid_t* h, const DrawRequest& r) {
     const DisplayArgs a{dye_src, h->cfg.dye_w, h->cfg.dye_h, h->droff, bloom_on ? h->pfx.bloom : nullptr, o.bw, o.bh,
                         sun_on ? h->pfx.sun : nullptr, o.sw, o.sh, bloom_on ? h->pfx.dither : nullptr, r.dw, r.dh,
                         r.on_device ? r.dst : h->frame, r.width, r.height, y0, y1, r.back[0], r.back[1], r.back[2], r.bg_mode,
-                        h->cfg.aspect, ts, list};
+                        h->cfg.aspect, ts, list, looks};
     dim3 b(32, 8);
     const DisplayKernel k = h->batch ? kDisplayBatch[r.out][r.keywords] : kDisplay[h->nearest][r.out][h->half_fx][r.keywords];
     if (cells > 0) {
@@ -2531,7 +2556,8 @@ int fluid_render_postfx(fluid_t* h, int width, int height, const fluid_postfx* f
 static int capture(fluid_t* h, const char* what, int width, int height, int canvas_w, int canvas_h, uint32_t keywords,
                    int transparent, const fluid_postfx* fx, const float* dither_rgb, int dw, int dh,
                    float back_r, float back_g, float back_b, uint8_t* dst, size_t n_bytes, bool on_device,
-                   bool batch = false, bool subset = false, const int32_t* members = nullptr, int n_members = 0) {
+                   bool batch = false, bool subset = false, const int32_t* members = nullptr, int n_members = 0,
+                   bool per_image = false, const fluid_look* looks = nullptr) {
     // drawColor's store of normalizeColor(BACK_COLOR) into the half-float target
     const float b16[3] = {__half2float(__float2half_rn(back_r)), __half2float(__float2half_rn(back_g)),
                           __half2float(__float2half_rn(back_b))};
@@ -2539,7 +2565,7 @@ static int capture(fluid_t* h, const char* what, int width, int height, int canv
                     .canvas_h = canvas_h, .keywords = keywords, .fx = fx, .dither = dither_rgb, .dw = dw, .dh = dh,
                     .back = {b16[0], b16[1], b16[2]}, .bg_mode = transparent ? 2 : 0, .out = OUT_CAPTURE,
                     .on_device = on_device, .dst = dst, .n = n_bytes, .batch = batch, .subset = subset,
-                    .members = members, .n_members = n_members});
+                    .members = members, .n_members = n_members, .per_image = per_image, .looks = looks});
 }
 
 int fluid_capture(fluid_t* h, int width, int height, int canvas_w, int canvas_h, uint32_t keywords,
@@ -2573,12 +2599,13 @@ int fluid_capture_batch(fluid_t* h, int width, int height, int canvas_w, int can
 static int canvas(fluid_t* h, const char* what, int width, int height, uint32_t keywords, int transparent,
                   const fluid_postfx* fx, const float* dither_rgb, int dw, int dh, float back_r, float back_g,
                   float back_b, uint8_t* dst, size_t n_bytes, int dst_on_device, bool batch, bool subset = false,
-                  const int32_t* members = nullptr, int n_members = 0) {
+                  const int32_t* members = nullptr, int n_members = 0, bool per_image = false,
+                  const fluid_look* looks = nullptr) {
     return draw(h, {.what = what, .width = width, .height = height, .canvas_w = width,
                     .canvas_h = height, .keywords = keywords, .fx = fx, .dither = dither_rgb, .dw = dw, .dh = dh,
                     .back = {back_r, back_g, back_b}, .bg_mode = transparent ? 1 : 0, .out = OUT_CANVAS,
                     .on_device = dst_on_device != 0, .dst = dst, .n = n_bytes, .batch = batch, .subset = subset,
-                    .members = members, .n_members = n_members});
+                    .members = members, .n_members = n_members, .per_image = per_image, .looks = looks});
 }
 
 int fluid_render_canvas(fluid_t* h, int width, int height, uint32_t keywords, int transparent,
@@ -2613,6 +2640,22 @@ int fluid_render_canvas_members(fluid_t* h, int width, int height, uint32_t keyw
                                 uint8_t* dst, size_t n_bytes, int dst_on_device, const int32_t* members, int n) {
     return canvas(h, "fluid_render_canvas_members", width, height, keywords, transparent, fx, dither_rgb, dw, dh,
                   back_r, back_g, back_b, dst, n_bytes, dst_on_device, true, true, members, n);
+}
+
+// The batch draws with a look per image: the whole batch (members == NULL, n == B) or the listed members, image k
+// drawn with looks[k]'s sliders and background through the launches of the shared-look draw.  The call's own
+// background arguments are placeholders the look table replaces.
+int fluid_capture_looks(fluid_t* h, int width, int height, int canvas_w, int canvas_h, uint32_t keywords,
+                        const fluid_postfx* fx, const float* dither_rgb, int dw, int dh, const fluid_look* looks,
+                        uint8_t* dst, size_t n_bytes, int dst_on_device, const int32_t* members, int n) {
+    return capture(h, "fluid_capture_looks", width, height, canvas_w, canvas_h, keywords, 0, fx, dither_rgb, dw, dh,
+                   0.0f, 0.0f, 0.0f, dst, n_bytes, dst_on_device != 0, true, members != nullptr, members, n, true, looks);
+}
+int fluid_render_canvas_looks(fluid_t* h, int width, int height, uint32_t keywords, const fluid_postfx* fx,
+                              const float* dither_rgb, int dw, int dh, const fluid_look* looks,
+                              uint8_t* dst, size_t n_bytes, int dst_on_device, const int32_t* members, int n) {
+    return canvas(h, "fluid_render_canvas_looks", width, height, keywords, 0, fx, dither_rgb, dw, dh, 0.0f, 0.0f, 0.0f,
+                  dst, n_bytes, dst_on_device, true, members != nullptr, members, n, true, looks);
 }
 
 void* fluid_host_alloc(size_t bytes) {

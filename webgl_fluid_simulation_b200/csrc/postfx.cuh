@@ -15,6 +15,7 @@
 #include <cuda_runtime.h>
 
 #include "half_passes.cuh"
+#include "looks.h"
 #include "passes.cuh"
 
 namespace fk {
@@ -46,7 +47,9 @@ __device__ __forceinline__ float linear_fetch_rgb_r_repeat(const float* __restri
 // back to back, as a dense (B, h, w[, C]) array of its own size, so member m of a w x h array starts
 // member_offset(w, h) texels in.  The pointers move before any tap, so the sampler's clamp keeps every tap
 // inside the member.  Image z draws dye member members[z] when a member list is given (a subset draw), member z
-// otherwise; the post-FX targets stay dense by image.
+// otherwise; the post-FX targets stay dense by image.  A draw with a look per image (fluid_render_canvas_looks)
+// also gives the batch forms a table of looks (looks.h ImageLook): image z then reads looks[z] where the other
+// draws read the call's scalars, which only the batch forms take.
 
 // texels before member blockIdx.z of a dense (B, h, w) array, in 64 bits
 __device__ __forceinline__ size_t member_offset(int w, int h) { return (size_t)blockIdx.z * w * h; }
@@ -70,8 +73,15 @@ __global__ void __launch_bounds__(256) bloom_prefilter_kernel(const typename Sd:
                                                               int dye_row_off, typename St::T4* __restrict__ out, int w,
                                                               int h, int j_lo, int j_hi, float curve0, float curve1,
                                                               float curve2, float threshold,
-                                                              const int* __restrict__ members = nullptr) {
-    if constexpr (BATCH) { dye += dye_member_offset(members, Wd, Hd); out += member_offset(w, h); }
+                                                              const int* __restrict__ members = nullptr,
+                                                              const ImageLook* __restrict__ looks = nullptr) {
+    if constexpr (BATCH) {
+        dye += dye_member_offset(members, Wd, Hd); out += member_offset(w, h);
+        if (looks) {
+            const float* c = looks[blockIdx.z].curve;
+            curve0 = __ldg(c); curve1 = __ldg(c + 1); curve2 = __ldg(c + 2); threshold = __ldg(c + 3);
+        }
+    }
     const int i = blockIdx.x * blockDim.x + threadIdx.x, j = j_lo + blockIdx.y * blockDim.y + threadIdx.y;
     if (i >= w || j >= j_hi) return;
     const float uvx = ((float)i + 0.5f) / (float)w, uvy = ((float)j + 0.5f) / (float)h;
@@ -84,11 +94,16 @@ __global__ void __launch_bounds__(256) bloom_prefilter_kernel(const typename Sd:
 }
 
 // bloomBlurShader S:633-651 / bloomFinalShader S:653-674; add = blendFunc(ONE, ONE) (S:1374-1375): the
-// fragment plus the widened destination texel, rounded once by the store
+// fragment plus the widened destination texel, rounded once by the store.  BATCH: the final pass of a draw with
+// a look per image takes image z's intensity as its scale.
 template <class St, class Smp, bool BATCH = false>
 __global__ void __launch_bounds__(256) box4_kernel(const typename St::T4* __restrict__ src, int ws, int hs,
-                                                   typename St::T4* __restrict__ dst, int w, int h, float scale, int add) {
-    if constexpr (BATCH) { src += member_offset(ws, hs); dst += member_offset(w, h); }
+                                                   typename St::T4* __restrict__ dst, int w, int h, float scale, int add,
+                                                   const ImageLook* __restrict__ looks = nullptr) {
+    if constexpr (BATCH) {
+        src += member_offset(ws, hs); dst += member_offset(w, h);
+        if (looks) scale = __ldg(&looks[blockIdx.z].intensity);
+    }
     const int i = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y * blockDim.y + threadIdx.y;
     if (i >= w || j >= h) return;
     const float tsx = (float)(1.0 / (double)ws), tsy = (float)(1.0 / (double)hs);
@@ -134,12 +149,16 @@ __device__ __forceinline__ float mask_alpha(float4 v) { return v.w; }
 __device__ __forceinline__ float mask_alpha(float v) { return v; }
 
 // sunraysShader S:693-724.  M: the mask's texel type, Sd::T4 (the mask in dye.write) or float (a slab's
-// gathered alpha).  BATCH: the mask of the drawn member, in its dye.write.
+// gathered alpha).  BATCH: the mask of the drawn member, in its dye.write, and image z's weight with looks.
 template <class Sd, class St, class Smp, bool BATCH = false, class M = typename Sd::T4>
 __global__ void __launch_bounds__(256) sunrays_kernel(const M* __restrict__ mask, int Wm, int Hm,
                                                       typename St::T1* __restrict__ out, int w, int h, float weight,
-                                                      const int* __restrict__ members = nullptr) {
-    if constexpr (BATCH) { mask += dye_member_offset(members, Wm, Hm); out += member_offset(w, h); }
+                                                      const int* __restrict__ members = nullptr,
+                                                      const ImageLook* __restrict__ looks = nullptr) {
+    if constexpr (BATCH) {
+        mask += dye_member_offset(members, Wm, Hm); out += member_offset(w, h);
+        if (looks) weight = __ldg(&looks[blockIdx.z].weight);
+    }
     const int i = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y * blockDim.y + threadIdx.y;
     if (i >= w || j >= h) return;
     const float Density = 0.3f, Decay = 0.95f, Exposure = 0.7f;
@@ -231,25 +250,36 @@ struct DisplayArgs {
     float aspect;
     float4 ts;                          // 1/w, 1/h and getTextureScale of the dithering texture (BLOOM)
     const int* members;                 // BATCH: the dye member of each image (a subset draw), or null: image z
+    const ImageLook* looks;             // BATCH: each image's background (a draw with a look per image), or null
 };
 
 // Output policies of display_kernel: the element type of `out`, the row of `out` that row r of an
-// n-row band goes to, and what is stored for the display fragment (c, alpha) at uv, blend included.
+// n-row band goes to, and what is stored for the display fragment (c, alpha) at uv, blend included.  `look`:
+// the image's entry of a batch draw with a look per image, whose background replaces the call's; null otherwise.
 // StoreFrame: the fp32 RGBA frame of render(), row 0 = bottom.
 struct StoreFrame {
     using T = float4;
     static __device__ __forceinline__ int row(int r, int) { return r; }
-    static __device__ __forceinline__ float4 store(const float (&c)[3], float alpha, const DisplayArgs& a, float uvx, float uvy) {
+    static __device__ __forceinline__ float4 store(const float (&c)[3], float alpha, const DisplayArgs& a, float uvx, float uvy,
+                                                   const ImageLook*) {
         return blend_over_background(c[0], c[1], c[2], alpha, a.bg_mode, a.br, a.bg, a.bb, a.aspect, uvx, uvy);
     }
 };
 // StoreCapture: captureScreenshot (S:287-327) up to the bytes toDataURL encodes: the blend of render(),
-// the fp16 store, then normalizeTexture's 8-bit truncation and its flip (top row first).
+// the fp16 store, then normalizeTexture's 8-bit truncation and its flip (top row first).  A look's background is
+// its fp16 BACK_COLOR, or none (bg_mode 2) when transparent.
 struct StoreCapture {
     using T = uchar4;
     static __device__ __forceinline__ int row(int r, int n) { return n - 1 - r; }
-    static __device__ __forceinline__ uchar4 store(const float (&c)[3], float alpha, const DisplayArgs& a, float uvx, float uvy) {
-        const float4 v = blend_over_background(c[0], c[1], c[2], alpha, a.bg_mode, a.br, a.bg, a.bb, a.aspect, uvx, uvy);
+    static __device__ __forceinline__ uchar4 store(const float (&c)[3], float alpha, const DisplayArgs& a, float uvx, float uvy,
+                                                   const ImageLook* look) {
+        float br = a.br, bg = a.bg, bb = a.bb;
+        int bg_mode = a.bg_mode;
+        if (look) {
+            br = __ldg(&look->back16[0]); bg = __ldg(&look->back16[1]); bb = __ldg(&look->back16[2]);
+            bg_mode = __ldg(&look->transparent) ? 2 : 0;
+        }
+        const float4 v = blend_over_background(c[0], c[1], c[2], alpha, bg_mode, br, bg, bb, a.aspect, uvx, uvy);
         return make_uchar4(capture_byte(v.x), capture_byte(v.y), capture_byte(v.z), capture_byte(v.w));
     }
 };
@@ -257,14 +287,22 @@ struct StoreCapture {
 // S:118-119), top row first like ImageData.  The destination holds bytes: u8(BACK_COLOR) (bg_mode 0) or
 // u8(checkerboard) (bg_mode 1), alpha byte 255.  A fixed-point buffer clamps the source and the blend
 // factors before blending (GLES 3.0 §4.1.7), so ONE, ONE_MINUS_SRC_ALPHA is clamp01(c) + d * (1 -
-// clamp01(a)) on d = d8 / 255, rounded once more to a byte.  Every operation is rounded on its own.
+// clamp01(a)) on d = d8 / 255, rounded once more to a byte.  Every operation is rounded on its own.  A look's
+// destination is its u8(BACK_COLOR), or the checkerboard when transparent.
 struct StoreCanvas {
     using T = uchar4;
     static __device__ __forceinline__ int row(int r, int n) { return n - 1 - r; }
-    static __device__ __forceinline__ uchar4 store(const float (&c)[3], float alpha, const DisplayArgs& a, float uvx, float uvy) {
+    static __device__ __forceinline__ uchar4 store(const float (&c)[3], float alpha, const DisplayArgs& a, float uvx, float uvy,
+                                                   const ImageLook* look) {
+        // the empty asm, which takes alpha, keeps the look's loads below the shading's IEEE div / sqrt slow paths:
+        // hoisted above them, their values spill (the SHADING | SUNRAYS canvas)
+        if (look) asm volatile("" : "+l"(look) : "f"(alpha));
         float d[3];
-        if (a.bg_mode == 1) {
+        if (look ? __ldg(&look->transparent) != 0 : a.bg_mode == 1) {
             d[0] = d[1] = d[2] = unorm8_value(unorm8(checkerboard(a.aspect, uvx, uvy)));
+        } else if (look) {
+            d[0] = unorm8_value(__ldg(&look->back8[0])); d[1] = unorm8_value(__ldg(&look->back8[1]));
+            d[2] = unorm8_value(__ldg(&look->back8[2]));
         } else {
             d[0] = unorm8_value(unorm8(a.br)); d[1] = unorm8_value(unorm8(a.bg)); d[2] = unorm8_value(unorm8(a.bb));
         }
@@ -280,8 +318,8 @@ struct StoreCanvas {
 // of the bloom and sunrays targets (post_fx_chains' St); Smp: the sampler of the dye, bloom and sunrays
 // taps (the dithering tap is LINEAR + REPEAT whatever Smp is).  A slab rank draws the band [y0, y1) of the
 // target from its own dye rows (+ ghost rows); one GPU draws the whole target.  BATCH: image blockIdx.z reads
-// its member's dye (a.members) and its own bloom FBO and sunrays texture, and draws its own image; the dithering
-// texture is shared.
+// its member's dye (a.members) and its own bloom FBO and sunrays texture, and draws its own image over its own
+// background when the draw has a look per image (a.looks); the dithering texture is shared.
 template <bool SHADING, bool BLOOM, bool SUNRAYS, class Out, class Sp, class Smp, bool BATCH = false>
 __global__ void __launch_bounds__(256) display_kernel(DisplayArgs a) {
     // the bloom FBO and the sunrays texture are offset where they are read: a member pointer kept across the
@@ -340,7 +378,9 @@ __global__ void __launch_bounds__(256) display_kernel(DisplayArgs a) {
         }
     }
     const float alpha = fmaxf(cc[0], fmaxf(cc[1], cc[2]));
-    *o = Out::store(cc, alpha, a, uvx, uvy);
+    const ImageLook* look = nullptr;
+    if constexpr (BATCH) { if (a.looks) look = a.looks + blockIdx.z; }
+    *o = Out::store(cc, alpha, a, uvx, uvy, look);
 }
 
 }  // namespace fk

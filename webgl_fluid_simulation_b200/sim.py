@@ -698,10 +698,16 @@ class FluidBatch(_Handle):
     0.  render_canvas() and captureScreenshot() draw every member through one set of launches; render(), resize and
     the per-pass entry points are FluidSimulation's only.  readField(), writeField(), render_canvas() and
     captureScreenshot() take `members=`, a host list of distinct member indices, to act on those members only, and
-    reset(members) puts members back to their state at creation."""
+    reset(members) puts members back to their state at creation.  `member_config[m]` may also override the
+    DISPLAY_MEMBER_KEYS: render_canvas() and captureScreenshot() then draw member m with its own post-FX sliders and
+    background, still through one set of launches."""
 
     # the config keys a member can hold a value of its own for (fluid_set_param_members)
     MEMBER_KEYS = ("DENSITY_DISSIPATION", "VELOCITY_DISSIPATION", "PRESSURE", "CURL", "SPLAT_RADIUS")
+    # the config keys of a member's look in render_canvas() and captureScreenshot() (fluid_render_canvas_looks,
+    # fluid_capture_looks): the post-FX sliders and the background
+    DISPLAY_MEMBER_KEYS = ("BLOOM_INTENSITY", "BLOOM_THRESHOLD", "BLOOM_SOFT_KNEE", "SUNRAYS_WEIGHT", "BACK_COLOR",
+                           "TRANSPARENT")
 
     def __init__(self, members: int, config: dict | None = None, canvas_width: int = 1024, canvas_height: int = 1024,
                  sizes: tuple | None = None, flags: int = 0, jacobi_block: int = 0, device: int = -1):
@@ -725,15 +731,21 @@ class FluidBatch(_Handle):
     def members(self) -> int:
         return int(self._L.fluid_members(self._h))
 
-    def _live_values(self):
-        """A MEMBER_KEYS value is the float64 vector of every member's value, `member_config` over `config`."""
+    def _check_member_config(self):
+        """ValueError unless member_config holds one dict per member, each overriding MEMBER_KEYS and
+        DISPLAY_MEMBER_KEYS only."""
         B = self.members
         if len(self.member_config) != B:
             raise ValueError(f"member_config holds {len(self.member_config)} dicts for {B} members")
+        keys = self.MEMBER_KEYS + self.DISPLAY_MEMBER_KEYS
         for m, over in enumerate(self.member_config):
-            bad = sorted(set(over) - set(self.MEMBER_KEYS))
+            bad = sorted(set(over) - set(keys))
             if bad:
-                raise ValueError(f"member_config[{m}] sets {bad}: only {list(self.MEMBER_KEYS)} can differ between members")
+                raise ValueError(f"member_config[{m}] sets {bad}: only {list(keys)} can differ between members")
+
+    def _live_values(self):
+        """A MEMBER_KEYS value is the float64 vector of every member's value, `member_config` over `config`."""
+        self._check_member_config()
         vals = super()._live_values()
         for k in self.MEMBER_KEYS:
             vec = np.array([float(over.get(k, self.config[k])) for over in self.member_config], np.float64)
@@ -877,13 +889,36 @@ class FluidBatch(_Handle):
             raise ValueError("reset() takes a list of member indices")
         self._check(self._L.fluid_reset_members(self._h, mp, m.size))
 
-    def _draw(self, fn_all, fn_members, what, w, h, args, out, members):
-        """A whole-batch draw, or with `members` the draw of the listed members only, image k member members[k]."""
+    def _looks(self, m):
+        """None when no member overrides a DISPLAY_MEMBER_KEYS key: the draw takes one look from `config`.  Otherwise
+        the fluid_look of each image, `member_config` over `config`: member k's for image k, or member m[k]'s for a
+        member list m (an index outside [0, B) gets `config`'s look; the library refuses the list)."""
+        self._check_member_config()
+        if not any(k in over for over in self.member_config for k in self.DISPLAY_MEMBER_KEYS):
+            return None
+        B = self.members
+        idx = range(B) if m is None else m.tolist()
+        looks = (_lib.Look * len(idx))()
+        for k, i in enumerate(idx):
+            c = {**self.config, **(self.member_config[i] if 0 <= i < B else {})}
+            looks[k] = _lib.Look(float(c["BLOOM_INTENSITY"]), float(c["BLOOM_THRESHOLD"]), float(c["BLOOM_SOFT_KNEE"]),
+                                 float(c["SUNRAYS_WEIGHT"]), *_back_rgb(c), 1 if c.get("TRANSPARENT") else 0)
+        return looks
+
+    def _draw(self, fn_all, fn_members, fn_looks, what, w, h, args, look_args, out, members):
+        """A whole-batch draw, or with `members` the draw of the listed members only, image k member members[k].
+        When a member overrides a DISPLAY_MEMBER_KEYS key, fn_looks draws every image with its member's look; its
+        arguments `look_args` are `args` without transparent and back_*."""
         m, mp = self._member_list(members)
         n = self.members if m is None else m.size
+        looks = self._looks(m)
         dst, result, on_device = _u8_destination(out, (n, h, w, 4), what)
         tail = (dst, 4 * w * h * n, 1 if on_device else 0)
-        self._check(fn_all(self._h, w, h, *args, *tail) if m is None else fn_members(self._h, w, h, *args, *tail, mp, n))
+        if looks is not None:
+            self._check(fn_looks(self._h, w, h, *look_args, looks, *tail, mp, n))
+        else:
+            self._check(fn_all(self._h, w, h, *args, *tail) if m is None else
+                        fn_members(self._h, w, h, *args, *tail, mp, n))
         if on_device:
             self.sync()
         return result
@@ -894,18 +929,22 @@ class FluidBatch(_Handle):
         draws from member m's dye.  Config, canvas and `self.dithering` as there.  `out`: a C-contiguous uint8 numpy
         array of that many bytes, or a C-contiguous uint8 CUDA array of them with render_canvas's waits, returned
         as it was passed.  members: the listed members' images only, (n, h, w, 4), image k member members[k]
-        (fluid_render_canvas_members)."""
+        (fluid_render_canvas_members).  A member's DISPLAY_MEMBER_KEYS overrides give its image that member's
+        sliders and background (fluid_render_canvas_looks)."""
         w, h, args = self._canvas_args()
-        return self._draw(self._L.fluid_render_canvas_batch, self._L.fluid_render_canvas_members, "render_canvas",
-                          w, h, args, out, members)
+        look_args = (args[0], *args[2:6])                    # keywords, fx, dither_rgb, dw, dh
+        return self._draw(self._L.fluid_render_canvas_batch, self._L.fluid_render_canvas_members,
+                          self._L.fluid_render_canvas_looks, "render_canvas", w, h, args, look_args, out, members)
 
     def captureScreenshot(self, out=None, members=None):
         """FluidSimulation.captureScreenshot for every member (fluid_capture_batch): (B, h, w, 4) uint8 at
         getResolution(CAPTURE_RESOLUTION) of the canvas, member by member, each top row first.  No PNG is written.
-        `out` and `members` as in render_canvas (fluid_capture_members)."""
+        `out`, `members` and the DISPLAY_MEMBER_KEYS overrides as in render_canvas (fluid_capture_members,
+        fluid_capture_looks)."""
         w, h, args = self._capture_args()
-        return self._draw(self._L.fluid_capture_batch, self._L.fluid_capture_members, "captureScreenshot",
-                          w, h, args, out, members)
+        look_args = (*args[:3], *args[4:8])                  # canvas_w, canvas_h, keywords, fx, dither_rgb, dw, dh
+        return self._draw(self._L.fluid_capture_batch, self._L.fluid_capture_members, self._L.fluid_capture_looks,
+                          "captureScreenshot", w, h, args, look_args, out, members)
 
 
 def _fx_args(fx, dith):
